@@ -2,6 +2,7 @@
 
     python bench.py --gpus N --steps K --warmup W [--impl vcl|reference|library]
                     [--config 2|3|4|5] [--clips B] [--model 7b|13b] [--frames 32,64,100]
+                    [--dump-outputs DIR]
 
 Configurations (numbering of SURVEY.md 8d; BASELINE.json `configs` is 0-based, so config k = configs[k-1]):
   2  (default, the configuration the metric is quoted on) 1 clip per GPU: 100 synthetic 224x224
@@ -34,6 +35,10 @@ Printed JSON (rank 0, one line):
                        cost on the box (SURVEY.md 2.3); 1 warm-up + 1 timed clip
 `--impl reference` times the CPU path as the arm of its own (rank 0 only; one bounded sample whatever
 --steps says); `--impl library` prints the library baseline alone.
+`--dump-outputs DIR` (product arm, rank 0): after the timed steps, writes what the last device-resident step
+computed -- the pooled clip features and the greedy token ids (config 5: the pooled features at every T) -- as
+DIR/<name>.npy in float32 / float64. Weights, frames and prompts are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 import argparse
 import json
@@ -66,8 +71,8 @@ def peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         d = json.load(open(path))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 6650.0, 1400.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+    return 3350.0, 989.0, "H100 SXM data sheet (dense bf16, 700 W card; not reached on a power-limited one)"
 
 
 # ---------------------------------------------------------------------------------------------
@@ -98,13 +103,13 @@ def workload_config(cfg_id, model, B, world):
                 "parallelism": f"dp{world} (clips sharded, one all_gather of per-clip checksums)",
                 "weights": "random-init bf16 (seed 0)",
                 "l2": "no flush: every clip streams its own frames and activations (0.7 GB per 100-frame clip) through "
-                      "the 126 MB L2"}
+                      "the 50 MB L2"}
     return {"workload": f"{CONFIGS[cfg_id]['label']}; per clip: {T_FRAMES} frames 224x224 -> CLIP ViT-L/14 (23 layers) -> pool -> "
                         f"projector -> Vicuna-{model.upper()} prefill S={S_PROMPT} -> {N_NEW} greedy tokens",
             "clips_per_gpu": B, "parallelism": f"dp{world} (clips sharded, one all_gather of token ids)",
             "weights": "random-init bf16 (seed 0)",
             "l2": "no flush: every step streams inputs+weights far larger than L2 "
-                  f"({w['weights_step'] / 1e9:.1f} GB of weights per decode step vs 126 MB)"}
+                  f"({w['weights_step'] / 1e9:.1f} GB of weights per decode step vs 50 MB)"}
 
 
 def metric_name(cfg_id, model):
@@ -391,24 +396,6 @@ def library_sample(model, dev, clip_sd, llm_sd):
 
 
 # ---------------------------------------------------------------------------------------------
-# measured DRAM traffic of the decode loop, from the committed ncu capture
-# ---------------------------------------------------------------------------------------------
-def decode_traffic_from_ncu(model, B):
-    """Measured DRAM bytes of the decode loop: profiles/r02_decode_step_traffic.json (tools/decode_traffic.py:
-    dram__bytes_read + dram__bytes_write of every kernel of one decode step in an `ncu --set full` capture,
-    per-layer part scaled to the model depth) x the steps of the loop. None when there is no capture for
-    this configuration (7B, 1 clip)."""
-    path = os.path.join(ROOT, "profiles", "r02_decode_step_traffic.json")
-    if model != "7b" or B != 1 or not os.path.exists(path):
-        return None, None
-    try:
-        d = json.load(open(path))
-        return d["step_dram_bytes"] * (N_NEW - 1), os.path.relpath(path, ROOT) + " <- " + d["source"]
-    except Exception:
-        return None, None
-
-
-# ---------------------------------------------------------------------------------------------
 # product arm
 # ---------------------------------------------------------------------------------------------
 def init_dist(world, dev):
@@ -453,7 +440,9 @@ def run_vcl(args, rank, world, local_rank):
     m = MODELS[args.model]
     B = args.clips
     model, tower, eng, (clip_sd, llm_sd) = build_model(args.model, B, dev)
-    want_library = rank == 0 and world == 1 and not args.no_library
+    # the 13B engine (weights + the decode-order copy, 52 GB) leaves no room on an 80 GB GPU for the library
+    # baseline's own bf16 copy of the weights
+    want_library = rank == 0 and world == 1 and not args.no_library and args.model == "7b"
     if not want_library:
         del clip_sd, llm_sd
         clip_sd = llm_sd = None
@@ -511,6 +500,8 @@ def run_vcl(args, rank, world, local_rank):
         clocks.start()
         ms_dev, evs = timed(args.steps, 4, False)
         launches = vn.launch_count() - l0
+        # the first 32 clips' features at most (47 MB of float32), every clip's tokens
+        dumped = {"clip_features": feats[:32].float().cpu().numpy(), "tokens": toks.double().cpu().numpy()}
         ms_e2e, _ = timed(args.steps, 0, True)
         clk = clocks.stop()
         stream.synchronize()
@@ -522,7 +513,6 @@ def run_vcl(args, rank, world, local_rank):
     hbm, tf, src = peaks()
     dec_bytes = (N_NEW - 1) * w["weights_step"] + B * w["kv_per_tok"] * sum(S_PROMPT + i for i in range(1, N_NEW))
     dec_gbs = dec_bytes / (stage[2] * 1e-3) / 1e9
-    traffic, traffic_src = decode_traffic_from_ncu(args.model, B)
     total_clips = world * B * args.steps
     out = {
         "metric": metric_name(args.config, args.model),
@@ -537,10 +527,8 @@ def run_vcl(args, rank, world, local_rank):
                 "tokens_equal_device_resident_run": agree},
         "gpu_launches": int(launches),
         "roofline": {"bound": "hbm", "achieved": dec_gbs, "peak": hbm, "unit": "GB/s", "frac": dec_gbs / hbm,
-                     "traffic": traffic,
-                     "traffic_note": ("dram__bytes_read+write summed over the kernels of one decode step in the committed "
-                                      f"ncu --set full capture ({traffic_src}) x {N_NEW - 1} steps; algorithmic bytes "
-                                      f"{dec_bytes / 1e9:.1f} GB") if traffic else "no committed ncu capture for this configuration",
+                     "traffic": None,
+                     "traffic_note": f"measured DRAM traffic: not measured; algorithmic bytes {dec_bytes / 1e9:.1f} GB",
                      "peak_source": src,
                      "kernel": f"decode loop: {N_NEW - 1} steps x (4 weight-streaming launches + attention per layer x "
                                f"{m['layers']} layers + head), one CUDA graph; bytes = weights streamed + KV read"},
@@ -552,6 +540,8 @@ def run_vcl(args, rank, world, local_rank):
         "clocks": clk,
     }
     if rank == 0:
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, dumped)
         out["tokens_rank0_clip0"] = toks[0].tolist()
         if want_library:
             lib = library_sample(args.model, dev, clip_sd, llm_sd)
@@ -622,6 +612,7 @@ def run_clip_sweep(args, rank, world, local_rank):
         clocks.start()
         ms_dev, evs = timed(args.steps, len(Ts) + 1, False)
         launches = vn.launch_count() - l0
+        dumped = {f"clip_features_T{t}": outs[t].float().cpu().numpy() for t in Ts}
         ms_e2e, _ = timed(args.steps, 0, True)
         clk = clocks.stop()
     per_t = np.array([[ev[i].elapsed_time(ev[i + 1]) for i in range(len(Ts))] for ev in evs]).mean(0)   # ms per clip at each T
@@ -644,16 +635,32 @@ def run_clip_sweep(args, rank, world, local_rank):
                 "api": "vision_tower(frames).hidden_states[-2][:, 1:] -> get_spatio_temporal_features_torch, pinned host frames"},
         "gpu_launches": int(launches),
         "roofline": {"bound": "tensor", "achieved": ach, "peak": tf, "unit": "TFLOP/s", "frac": ach / tf, "traffic": None,
-                     "peak_source": src, "kernel": "the ViT's tcgen05 GEMMs + attention over one clip (algorithmic flops of SURVEY.md 8d / clip time)"},
+                     "peak_source": src, "kernel": "the ViT's wgmma GEMMs + attention over one clip (algorithmic flops of SURVEY.md 8d / clip time)"},
         "sweep": sweep,
         "job": {"clips_per_T": SWEEP_CLIPS, "seconds_for_the_whole_sweep": sum(v["job_seconds_1000_clips"] for v in sweep.values())},
         "clocks": clk,
     }
     if rank == 0:
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, dumped)
         emit(out)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(directory, arrays):
+    """DIR/<name>.npy for every output array (float32 / float64), at most 64 MB in all."""
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise SystemExit(f"--dump-outputs: {total} bytes of outputs exceed the {DUMP_LIMIT_BYTES}-byte limit")
+    os.makedirs(directory, exist_ok=True)
+    for name, a in arrays.items():
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        np.save(os.path.join(directory, name + ".npy"), a)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -722,7 +729,11 @@ def main():
     ap.add_argument("--frames", default="32,64,100", help="config 5: frames per clip, comma separated")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-library", action="store_true", help="skip the library_baseline leg")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs as DIR/<name>.npy (product arm, rank 0)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.model is None:
         args.model = CONFIGS[args.config]["model"]
     if args.clips is None:

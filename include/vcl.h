@@ -1,4 +1,4 @@
-/* vcl.h -- C ABI of libvcl.so, the B200-native replacement for the device side of
+/* vcl.h -- C ABI of libvcl.so, the H100-native (sm_90a) replacement for the device side of
  * PG-Video-LLaVA's video-conversation inference path.
  *
  * The reference (mbzuai-oryx/Video-LLaVA) has no FFI or operator registry: its boundary is a set
@@ -15,7 +15,7 @@
  *     except vcl_load_* which return after the repack has completed;
  *   - return value 0 = ok, negative = error; vcl_last_error() gives the message of the last
  *     failure on the calling thread's process (one handle per process/GPU, not thread-safe);
- *   - there is no CPU fallback: on a machine without an sm_100 device every compute entry point
+ *   - there is no CPU fallback: on a machine without an sm_90 (H100) device every compute entry point
  *     fails with an error.
  */
 #ifndef VCL_H_
@@ -184,8 +184,9 @@ int vcl_op_gemm(const void* A, int64_t lda, const void* W, int64_t ldw, void* C,
                 const void* bias, const void* residual, int64_t ldr, int M, int N, int K, int act,
                 int block_n, void* stream);
 /* same with an explicit thread-block-cluster size along M (1, 2 or 4): the CTAs of a cluster share
- * each weight tile through TMA multicast; cluster = -2: CTA pairs (tcgen05 cta_group::2, one M = 256 MMA
- * per pair, each CTA stages half of the weight tile; block_n 256 or 128) */
+ * each weight tile through TMA multicast (block_n 128 or 256; narrower tiles run without a cluster);
+ * cluster = -2: a CTA pair on one 256-row tile, each CTA fetching half of the weight tile (on sm_90 the same
+ * launch as cluster = 2, since a wgmma reads only its own CTA's shared memory) */
 int vcl_op_gemm_ex(const void* A, int64_t lda, const void* W, int64_t ldw, void* C, int64_t ldc,
                    const void* bias, const void* residual, int64_t ldr, int M, int N, int K, int act,
                    int block_n, int cluster, void* stream);
@@ -196,7 +197,7 @@ int vcl_op_rmsnorm(const void* x, void* y, const void* w, int rows, int D, float
 int vcl_op_attention(const void* q, const void* k, const void* v, void* o, int B, int S, int H,
                      int head_dim, float scale, int causal, void* stream);
 /* ViT attention on the fused projection output: qkv [n_frames*S, 3*H*64] (q|k|v) -> out
- * [n_frames*S, H*64]; tcgen05 kernel, 129 <= S <= 257, non-causal, scale 64^-1/2 */
+ * [n_frames*S, H*64]; non-causal, scale 64^-1/2; wgmma kernel for 129 <= S <= 257 */
 int vcl_op_attention_vit(const void* qkv, void* out, int n_frames, int S, int H, void* stream);
 /* out[b,n] = x[b,:].W[n,:] (+res) with optional RMSNorm of x: B <= 4 the ring kernel of the single-clip
  * decode path (fused norm), 5 <= B <= 16 the wide ring kernel (norm + window-major re-layout by a launch of

@@ -1,7 +1,7 @@
 """pytest configuration: registers the `gpu` marker and puts the package dir on sys.path.
 
 `-m "not gpu"` runs on the CPU-only build container (oracle vs golden vectors, host logic, C-ABI
-symbol export); `-m gpu` runs the parity tests proper on a B200 through the C ABI.
+symbol export); `-m gpu` runs the parity tests proper on an H100 through the C ABI.
 """
 import os
 import sys
@@ -16,7 +16,7 @@ for p in (ROOT, PKG):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -123,7 +123,7 @@ def test_layernorm_rmsnorm(rows, D):
 @pytest.mark.parametrize("B,S,H,hd,causal", [(3, 257, 16, 64, False), (2, 448, 4, 128, True),
                                              (1, 64, 2, 128, True), (5, 577, 2, 64, False),
                                              (1, 100, 3, 128, True),
-                                             # causal hd 128 up to 512 keys: the tcgen05 prefill kernel (1..4 key blocks,
+                                             # causal hd 128 up to 512 keys: the wgmma prefill kernel (1..4 key blocks,
                                              # ragged last tile, a single head / clip); 640 keys: the mma.sync kernel
                                              (1, 512, 2, 128, True), (2, 129, 3, 128, True), (1, 300, 1, 128, True),
                                              (3, 448, 32, 128, True), (1, 640, 2, 128, True)])
@@ -146,9 +146,10 @@ def test_attention(B, S, H, hd, causal):
 
 @pytest.mark.parametrize("B,S,H", [(1, 448, 32), (2, 77, 5), (3, 129, 3), (1, 511, 1), (2, 512, 4), (1, 16, 2)])
 def test_attention_prefill_tcgen05_vs_mma_sync(B, S, H):
-    """The tcgen05 prefill kernel against the flash-style mma.sync kernel it replaces, same inputs, one process
+    """The wgmma prefill kernel against the flash-style mma.sync kernel, same inputs, one process
     (VCL_PREFILL_ATTN_FLASH is read per call): they differ only in where P is rounded (relative to the final row
-    maximum vs the running one), so they agree far inside the tolerance either has against the eager reference."""
+    maximum vs the running one) and in summation order, so they agree far inside the tolerance either has against
+    the eager reference."""
     import os
     torch.manual_seed(B * 1000 + S + H)
     dev = _dev()
@@ -199,11 +200,15 @@ def test_gemv(B, N, K, norm, res):
     xf = x.float()
     if norm:
         xf = (nw.float() * (xf * torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + 1e-5)).bfloat16().float()).bfloat16().float()
-    ref = xf @ w.float().t()
+    ref = (xf.double() @ w.double().t()).float()     # exact products: the reference does not depend on the GPU's BLAS
+    mag = ref.abs()
     if res:
         ref = ref.bfloat16().float() + r.float()
     assert _rel(out, ref) < 3e-3, _rel(out, ref)
-    assert ((out.float() - ref).abs() <= 2.5 * ref.abs().clamp_min(1e-2) * 2 ** -7).all()
+    # element-wise: as in test_gemm_tcgen05, a couple of bf16 ulps of the largest intermediate (the projection is
+    # rounded to bf16 before the residual add; a sum on a rounding boundary may round either way)
+    mag = torch.maximum(mag, ref.abs())
+    assert ((out.float() - ref).abs() <= 2.5 * mag.clamp_min(1e-2) * 2 ** -7).all()
 
 
 @pytest.mark.parametrize("T,P,C,dt_in,dt_out", [(100, 256, 1024, torch.bfloat16, torch.float16),
@@ -262,8 +267,8 @@ def test_gemm_cluster_multicast(M, N, K, bn, cl, act):
     (25700, 1024, 4096, 256, True, True, vn.ACT_NONE),
 ])
 def test_gemm_cta_pair(M, N, K, bn, has_bias, has_res, act):
-    """cta_group::2: two CTAs drive one M = 256 MMA (each stages half of the weight tile). Same tiles and
-    the same accumulation order as the single-CTA kernel -> bit-identical results."""
+    """cluster = -2, CTA pairs: two CTAs of a cluster share one 256-row tile, each fetching half of the weight
+    tile. Same tiles and the same accumulation order as the single-CTA kernel -> bit-identical results."""
     torch.manual_seed(M + N + K + bn)
     dev = _dev()
     a = torch.randn(M, K, device=dev).bfloat16()

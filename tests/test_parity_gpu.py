@@ -158,7 +158,7 @@ def test_llm_7b_width_two_layers():
 @torch.no_grad()
 @pytest.mark.parametrize("NB", [3, 9, 17])
 def test_decode_batch_paths_agree(NB):
-    """Batched decode (2..16: mma.sync weight streaming, one or two 8-row blocks; > 16: tcgen05 GEMM
+    """Batched decode (2..16: mma.sync weight streaming, one or two 8-row blocks; > 16: wgmma GEMM
     with a narrow N tile) must reproduce, per clip, what the clip gets when decoded alone through
     the single-clip GEMV path (clips are independent)."""
     cfg = O.LlmCfg(hidden=512, inter=1024, heads=4, layers=2)
@@ -277,7 +277,7 @@ def test_decode_small_batch_ring_kernel(NB):
     """2..4 clips (width 2560) go through the multi-column gemv_tc kernel (activation vectors of all
     clips in shared memory, one MMA column per clip): per clip it must reproduce the single-clip
     decode (same weights, same summation order; the caches come from differently tiled prefills)."""
-    cfg = O.LlmCfg(hidden=2560, inter=6912, heads=20, layers=2)   # every projection >= 148 row groups: ring kernel
+    cfg = O.LlmCfg(hidden=2560, inter=6912, heads=20, layers=2)   # every projection >= 132 row groups (one per SM): ring kernel
     sd = O.random_llm_state(cfg, seed=8)
     ids = O.make_prompt_ids(cfg, 356, seed=6, batch=NB).to(DEV)
     vf = (torch.randn(NB, 356, 1024, generator=torch.Generator().manual_seed(13)) * 0.5).half().float().to(DEV)

@@ -1,5 +1,5 @@
 """Parity at the REAL benchmark configurations (BASELINE.json configs[1..3], SURVEY.md 8d), through the
-C ABI, against the pinned oracle run on the same B200 in bf16 ("the reference's own PyTorch path on
+C ABI, against the pinned oracle run on the same GPU in bf16 ("the reference's own PyTorch path on
 identical inputs", reference: video_chatgpt/model/video_chatgpt.py:193-251 over HF LLaMA / CLIP) and in
 fp32 (gold):
 

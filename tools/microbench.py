@@ -1,5 +1,5 @@
-"""Kernel micro-benchmarks on one B200 (CUDA events, L2 flushed between timed launches).
-Prints achieved TFLOP/s for the tcgen05 GEMM on the hot-path shapes and GB/s for the HBM-bound
+"""Kernel micro-benchmarks on one GPU (CUDA events, L2 flushed between timed launches).
+Prints achieved TFLOP/s for the wgmma GEMM on the hot-path shapes and GB/s for the HBM-bound
 kernels. Development tool, not the contract bench (bench.py)."""
 import math
 import os
@@ -91,10 +91,21 @@ if __name__ == "__main__":
 
 
 def attn_case(n, S, H):
+    """The ViT attention: the wgmma kernel and the mma.sync flash kernel (VCL_VIT_ATTN_FLASH, read per call)."""
     qkv = torch.randn(n * S, 3 * H * 64, device=dev).bfloat16()
-    ms = timeit(lambda: vn.op_attention_vit(qkv, n, S, H))
     fl = n * H * 4.0 * S * S * 64
-    print(f"attn_vit_tc n={n} S={S} H={H}: {ms*1e3:.1f} us {fl/ms/1e9:.0f} TFLOP/s", flush=True)
+    outs = {}
+    for name, flash in (("wgmma", False), ("flash mma.sync", True)):
+        if flash:
+            os.environ["VCL_VIT_ATTN_FLASH"] = "1"
+        try:
+            ms = timeit(lambda: vn.op_attention_vit(qkv, n, S, H))
+            outs[name] = vn.op_attention_vit(qkv, n, S, H).float()
+        finally:
+            os.environ.pop("VCL_VIT_ATTN_FLASH", None)
+        print(f"attn_vit {name} n={n} S={S} H={H}: {ms*1e3:.1f} us {fl/ms/1e9:.0f} TFLOP/s", flush=True)
+    a, b = outs.values()
+    print(f"attn_vit wgmma vs flash: rel {((a - b).norm() / b.norm()).item():.2e}", flush=True)
 
 
 if __name__ == "__main__" and (len(sys.argv) < 2 or sys.argv[1] in ("all", "attn")):

@@ -1,10 +1,10 @@
-"""Build libvcl.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libvcl.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
     python video-llava_b200/build.py [--force] [--verbose]
 
 Objects and the shared library land next to the sources (video-llava_b200/csrc/*.o,
-video-llava_b200/libvcl.so); both are git-ignored but travel to the GPU box with the snapshot.
-nvcc cross-compiles without a GPU, so this also serves as the CPU-side "does it build" check.
+video-llava_b200/libvcl.so); both are git-ignored. nvcc cross-compiles without a GPU, so this
+also serves as the CPU-side "does it build" check.
 """
 from __future__ import annotations
 
@@ -20,7 +20,7 @@ LIB = os.path.join(HERE, "libvcl.so")
 SOURCES = ["vcl_api.cu", "gemm_tc.cu", "gemv.cu", "gemv_tc.cu", "gemv_tcw.cu", "gemv_mma.cu", "attention.cu", "attention_tc.cu", "attention_prefill_tc.cu", "decode_attention.cu", "elementwise.cu", "st_pool.cu"]
 HEADERS = ["common.cuh", "kernels.h", os.path.join("..", "..", "include", "vcl.h")]
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
           "--expt-relaxed-constexpr"]
 

@@ -9,9 +9,10 @@
 //     multiplied by `scaling` (a second bf16 rounding), softmax runs in fp32 and is cast back to
 //     bf16 before the PV matmul. The score roundings are reproduced; the probabilities are rounded
 //     to bf16 un-normalised (flash form), the one place this kernel differs from eager by design.
-//     The hot path no longer comes here: the ViT's S = 257 runs in attention_tc.cu, the causal hd-128 prefill
-//     up to 512 keys in attention_prefill_tc.cu (both tcgen05). This kernel serves the other shapes: the
-//     336-px tower (S = 577), longer prompts, continued prefills beyond 512 keys.
+//     It serves the 336-px ViT tower (S = 577, read straight out of the fused q|k|v activation,
+//     launch_attention_vit), longer prompts and continued prefills beyond 512 keys; the ViT's S = 257 runs in
+//     attention_tc.cu, the causal hd-128 prefill up to 512 keys in attention_prefill_tc.cu (both wgmma, exact
+//     full-row softmax).
 //
 // (2) the single-query decode attention lives in decode_attention.cu (cluster of 4 CTAs per head).
 #include "common.cuh"
@@ -253,6 +254,7 @@ int init_attention_kernels() {
   VCL_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 64 * 64 * 2));
   VCL_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 64 * 128 * 2));
   VCL_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 64 * 128 * 2));
+  if (init_attention_tc_kernels() != 0) return -2;
   return init_attention_prefill_tc_kernels();
 }
 
@@ -268,6 +270,19 @@ int launch_attention(const AttnArgs& a, cudaStream_t stream) {
     return a.causal ? launch_attn_t<64, true>(a, stream) : launch_attn_t<64, false>(a, stream);
   }
   return a.causal ? launch_attn_t<128, true>(a, stream) : launch_attn_t<128, false>(a, stream);
+}
+
+// qkv: [n_frames * S, 3*C] (q | k | v, heads of 64 contiguous), out: [n_frames * S, C]
+int launch_attention_vit(const bf16* qkv, bf16* out, int n_frames, int S, int H, int C, cudaStream_t stream) {
+  VCL_REQUIRE(C == H * 64, "attention_vit: head_dim must be 64");
+  if (attention_vit_tc_supported(S)) return launch_attention_vit_tc(qkv, out, n_frames, S, H, C, stream);
+  AttnArgs a;
+  a.q = qkv;         a.q_sb = (long long)S * 3 * C; a.q_sh = 64; a.q_ss = 3 * C;
+  a.k = qkv + C;     a.k_sb = a.q_sb; a.k_sh = 64; a.k_ss = 3 * C;
+  a.v = qkv + 2 * C; a.v_sb = a.q_sb; a.v_sh = 64; a.v_ss = 3 * C;
+  a.o = out;         a.o_sb = (long long)S * C; a.o_sh = 64; a.o_ss = C;
+  a.B = n_frames; a.H = H; a.S = S; a.head_dim = 64; a.scale = 0.125f; a.causal = 0;
+  return launch_attention(a, stream);
 }
 
 }  // namespace vcl

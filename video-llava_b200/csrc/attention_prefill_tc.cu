@@ -1,338 +1,186 @@
-// Causal self-attention of the LLaMA prefill on the 5th-generation tensor cores (head_dim 128, up to 512 keys).
+// Causal self-attention of the LLaMA prefill on the Hopper warpgroup tensor cores (head_dim 128, up to 512 keys).
 //
-// Replaces the flash-style mma.sync kernel (attention.cu) for the prompt lengths of the hot path (S_p = 448):
-// that kernel walks the key tiles of a 64-query tile one after the other (7 serial steps of ~3 us for the last
-// rows: 23.5 us per layer at S = 448). Here the whole score row of 128 queries fits in TMEM (4 x 128 fp32
-// columns), so the softmax is the EXACT full-row softmax of the eager reference -- no online rescaling -- and
-// the chain of a CTA is: loads -> 8 MMAs per key block -> softmax -> 16 MMAs per key block -> epilogue.
+// One CTA = one warpgroup per (clip, head, 64-query tile); causal: the tile needs the key blocks of 128 keys up to
+// its last query only. Every operand is a K-major 128-byte-swizzled tile in shared memory (the layout TMA writes
+// with CU_TENSOR_MAP_SWIZZLE_128B, built here by the threads themselves: [rows x 64 bf16] tiles, 16-byte chunk c of
+// row r stored at chunk c ^ (r % 8)), so both products run on wgmma.mma_async from shared-memory descriptors:
+//   S_j = Q . K_j^T   M64 x N128 x K128 (8 k-steps)      Q [64 x 128 d], K_j [128 keys x 128 d]
+//   O  += P_j . V_j   M64 x N128 x K128 (8 k-steps)      P_j [64 x 128 keys], V_j^T [128 d x 128 keys]
+// V is transposed on its way into shared memory, so no MN-major operand is needed.
 //
-// One CTA per (clip, head, 128-query tile); causal: tile t needs the key blocks 0 .. t only.
-//   warp 16 (1 thread)  TMA: Q tile and the K blocks it needs (each [128 rows x 128 d] as two 128-B-swizzled
-//                       [128 x 64] tiles), V blocks through a two-slot ring; issues all tcgen05.mma:
-//                         S_j = Q . K_j^T   M128 x N128 x K128  -> TMEM columns [128 j, 128 j + 128)
-//                         O  += P_j . V_j   M128 x N64 (x2: d halves) x K128 -> TMEM columns [0, 128)
-//                       (V is an MN-major B operand; O re-uses the columns of S_0 once the scores are consumed)
-//   warps 0-15          softmax: thread (row, column quarter) owns 32 columns of every key block. Pass 1 reads
-//                       them from TMEM for the row maximum (block j as soon as its MMAs retired, the load of
-//                       block j + 1 in flight meanwhile; maxima exchanged through shared memory), pass 2 reads
-//                       them again, exponentiates, writes P as bf16 into the K-major swizzled tiles the second
-//                       MMA consumes (over the dead K blocks) and keeps the row sum; then 32 O columns each
-//   warp 17             TMEM allocator (512 columns)
-// Shared memory: Q 32 KB | K / P 4 x 32 KB | V ring 2 x 32 KB = 224 KB: one CTA per SM; B x H x ceil(S / 128)
-// CTAs (128 for one clip of Vicuna-7B).
+// The softmax is the EXACT full-row softmax of the eager reference: pass 1 computes the scores of every key block
+// for the row maximum, pass 2 computes them again, exponentiates against the final maximum, writes P as bf16 and
+// accumulates O and the row sum. (The flash kernel of attention.cu rescales against a running maximum instead.)
 //
 // Arithmetic follows transformers/models/llama/modeling_llama.py:199-222 (eager): the scores are a bf16 tensor,
 // multiplied by `scaling` into another bf16 tensor, masked, softmax in fp32, probabilities cast to bf16 for the
 // P.V product. As in the other attention kernels of this library P is rounded before the normalisation.
-// Rows of K / V beyond the key count and rows of Q beyond S are zero-filled by the TMA (tensor-map bounds), so
-// stale cache rows never reach the MMAs.
 #include "common.cuh"
 #include "kernels.h"
 
-#include <cudaTypedefs.h>
 #include <stdlib.h>
 
 namespace vcl {
 
 namespace {
 
-constexpr int PA_SM_WARPS = 16;
-constexpr int PA_SM_THREADS = PA_SM_WARPS * 32;          // 512
-constexpr int PA_THREADS = PA_SM_THREADS + 64;
-constexpr int PA_HALF = 128 * 128;                       // one [128 rows x 64 bf16] swizzled tile (16 KB)
-constexpr int PA_BLK = 2 * PA_HALF;                      // one [128 x 128] block = two tiles
-constexpr int PA_MAX_KB = 4;                             // key blocks: 512 TMEM columns of scores
-constexpr int PA_OFF_Q = 0;                              // after the S MMAs: row maxima / sums
-constexpr int PA_OFF_KP = PA_BLK;
-constexpr int PA_OFF_V = PA_OFF_KP + PA_MAX_KB * PA_BLK;
-constexpr int PA_OFF_BAR = PA_OFF_V + 2 * PA_BLK;
-constexpr int PA_SMEM = PA_OFF_BAR + 256 + 1024;         // + barriers + manual 1024-B alignment
+constexpr int PA_THREADS = 128;                          // one warpgroup
+constexpr int PA_MAX_KB = 4;                             // key blocks of 128: 512 keys
+constexpr int PA_OFF_Q = 0;                              // Q: 2 tiles [64 x 64]      16 KB
+constexpr int PA_OFF_K = PA_OFF_Q + 2 * 64 * 128;        // K: 2 tiles [128 x 64]     32 KB
+constexpr int PA_OFF_VT = PA_OFF_K + 2 * 128 * 128;      // V^T: 2 tiles [128 x 64]   32 KB
+constexpr int PA_OFF_P = PA_OFF_VT + 2 * 128 * 128;      // P: 2 tiles [64 x 64]      16 KB
+constexpr int PA_SMEM = PA_OFF_P + 2 * 64 * 128 + 1024;  // + manual 1024-B alignment
 
 __device__ __forceinline__ uint32_t pa_sw128(int row, int chunk) {   // byte offset inside a SW128 tile
   return (uint32_t)row * 128u + (uint32_t)((chunk ^ (row & 7)) << 4);
 }
-// MN-major SW128 operand (V: rows = keys = K index, 64 contiguous d = N): 8-row groups 1024 B apart
-__device__ __forceinline__ uint64_t pa_desc_mn_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3ffffu) >> 4);
-  d |= (uint64_t)(1024u >> 4) << 16;
-  d |= (uint64_t)(1024u >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__device__ __forceinline__ float pa_ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ void pa_bar_sync(int id, int n) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
-}
-// 4-D tiled load (d, position, head, clip) -> shared memory
-__device__ __forceinline__ void tma_load_4d(uint32_t dst_smem, const void* tmap, uint32_t bar, int32_t c0,
-                                            int32_t c1, int32_t c2, int32_t c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(dst_smem),
-      "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
+
+__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// rows [row0, row0 + R) x 128 d of a strided matrix -> two swizzled [R x 64] tiles; rows >= n_rows are zero
+template <int R>
+__device__ __forceinline__ void pa_load_rows(uint8_t* dst, const bf16* g, long long ss, int row0, int n_rows) {
+#pragma unroll 4
+  for (int idx = threadIdx.x; idx < R * 16; idx += PA_THREADS) {
+    const int r = idx >> 4, c = idx & 15;
+    uint4 v = make_uint4(0u, 0u, 0u, 0u);
+    if (row0 + r < n_rows) v = *reinterpret_cast<const uint4*>(g + (long long)(row0 + r) * ss + c * 8);
+    *reinterpret_cast<uint4*>(dst + (c >> 3) * (R * 128) + pa_sw128(r, c & 7)) = v;
+  }
 }
 
-__global__ void __launch_bounds__(PA_THREADS, 1)
-attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                       const __grid_constant__ CUtensorMap tmap_v, bf16* __restrict__ out, long long o_sb,
-                       long long o_sh, long long o_ss, int S, int S_kv, int q_off, float scale, int q_hf, int k_hf,
-                       int v_hf) {
+// V rows [key0, key0 + 128) -> V^T as two swizzled [128 d x 64 keys] tiles; keys >= n_keys are zero
+__device__ __forceinline__ void pa_load_vt(uint8_t* dst, const bf16* g, long long ss, int key0, int n_keys) {
+#pragma unroll 4
+  for (int idx = threadIdx.x; idx < 128 * 16; idx += PA_THREADS) {
+    const int key = idx & 127, c = idx >> 7;              // consecutive threads: consecutive keys, same 8 d
+    uint4 v = make_uint4(0u, 0u, 0u, 0u);
+    if (key0 + key < n_keys) v = *reinterpret_cast<const uint4*>(g + (long long)(key0 + key) * ss + c * 8);
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    uint8_t* tile = dst + (key >> 6) * (128 * 128);
+    const int kc = (key & 63) >> 3, ke = key & 7;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int d = c * 8 + e;
+      const uint16_t h = (uint16_t)(e & 1 ? w[e >> 1] >> 16 : w[e >> 1] & 0xffffu);
+      *reinterpret_cast<uint16_t*>(tile + pa_sw128(d, kc) + ke * 2) = h;
+    }
+  }
+}
+
+// acc = A[64 x 128] . B[128 x 128]^T over K = 128 (two swizzle spans of both operands)
+__device__ __forceinline__ void pa_mma(float (&acc)[64], uint32_t a_base, int a_tile_bytes, uint32_t b_base,
+                                       int b_tile_bytes, bool accumulate) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const uint64_t ad = wgmma_desc_k_sw128(a_base + (k >> 2) * a_tile_bytes) + 2u * (k & 3);
+    const uint64_t bd = wgmma_desc_k_sw128(b_base + (k >> 2) * b_tile_bytes) + 2u * (k & 3);
+    wgmma_bf16<128>(acc, ad, bd, (accumulate || k > 0) ? 1u : 0u);
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc);
+}
+
+__global__ void __launch_bounds__(PA_THREADS)
+attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t pad = ((raw + 1023u) & ~1023u) - raw;
+  const uint32_t raw_addr = smem_u32(smem_raw);
+  const uint32_t pad = ((raw_addr + 1023u) & ~1023u) - raw_addr;
   uint8_t* smem = smem_raw + pad;
-  const uint32_t sbase = raw + pad;
-  const uint32_t bar0 = sbase + PA_OFF_BAR;
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
-  enum { B_Q = 0, B_K = 1 /* .. 4 */, B_VF = 5 /* 5, 6 */, B_VE = 7 /* 7, 8 */, B_S = 9 /* .. 12 */, B_P = 13, B_O = 14, N_BAR = 15 };
-  volatile uint32_t* tmem_ptr = reinterpret_cast<volatile uint32_t*>(smem + PA_OFF_BAR + 8 * N_BAR);
-  float* smax = reinterpret_cast<float*>(smem + PA_OFF_Q);            // [4][128], valid once the S MMAs retired
-  float* ssum = smax + 4 * 128;
+  const uint32_t sbase = raw_addr + pad;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int t = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-  // keys this query tile can see: positions <= q_off + (last row of the tile), and < S_kv
-  const int kv_end = min(S_kv, q_off + (t + 1) * 128);
-  const int nkb = (kv_end + 127) >> 7;                                // 1 .. PA_MAX_KB
+  const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int lane = threadIdx.x & 31, wq = threadIdx.x >> 5;
+  const int q0 = qt * 64;
+  const bf16* qg = a.q + (long long)b * a.q_sb + (long long)h * a.q_sh;
+  const bf16* kg = a.k + (long long)b * a.k_sb + (long long)h * a.k_sh;
+  const bf16* vg = a.v + (long long)b * a.v_sb + (long long)h * a.v_sh;
+  // key blocks this tile touches: keys up to the absolute position of its last query
+  const int last_key = min(S_kv - 1, a.q_off + min(q0 + 63, a.S - 1));
+  const int n_kb = last_key / 128 + 1;
 
-  if (warp == PA_SM_WARPS && lane == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
-    for (int i = 0; i < N_BAR; ++i) mbar_init(BAR(i), i == B_P ? PA_SM_THREADS : 1);
-    mbar_fence_init();
+  pa_load_rows<64>(smem + PA_OFF_Q, qg, a.q_ss, q0, a.S);
+
+  const int r0 = 16 * wq + (lane >> 2), c2 = 2 * (lane & 3);
+  int qpos[2];                                           // absolute positions of this thread's two rows
+  qpos[0] = a.q_off + q0 + r0;
+  qpos[1] = qpos[0] + 8;
+  const float scale = a.scale;
+  float acc[64] = {};
+  // scaled, rounded, masked score of accumulator element i of key block kb (reference rounding points)
+  auto score = [&](int kb, int i) {
+    const int key = kb * 128 + 8 * (i >> 2) + c2 + (i & 1);
+    const float x = bf16r(bf16r(acc[i]) * scale);
+    return (key >= S_kv || key > qpos[(i >> 1) & 1]) ? -INFINITY : x;
+  };
+
+  // ---- pass 1: row maxima over every key block ----
+  float m[2] = {-INFINITY, -INFINITY};
+  for (int kb = 0; kb < n_kb; ++kb) {
+    __syncthreads();                                     // previous readers of K are done
+    pa_load_rows<128>(smem + PA_OFF_K, kg, a.k_ss, kb * 128, S_kv);
+    fence_async_smem();
+    __syncthreads();
+    pa_mma(acc, sbase + PA_OFF_Q, 64 * 128, sbase + PA_OFF_K, 128 * 128, false);
+#pragma unroll
+    for (int i = 0; i < 64; ++i) m[(i >> 1) & 1] = fmaxf(m[(i >> 1) & 1], score(kb, i));
   }
-  if (warp == PA_SM_WARPS + 1) tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_ptr)), 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_ptr;
-
-  if (warp == PA_SM_WARPS) {
-    // ================================ TMA + MMA issuer ================================
-    if (lane == 0) {
-      // hf: the tensor map has the head dimension in front of the position dimension (make_tmap_attn)
-      auto load_blk = [&](uint32_t dst, const CUtensorMap* tm, int hf, uint32_t bar, int row0) {
-        mbar_arrive_expect_tx(bar, PA_BLK);
-        tma_load_4d(dst, tm, bar, 0, hf ? h : row0, hf ? row0 : h, b);
-        tma_load_4d(dst + PA_HALF, tm, bar, 64, hf ? h : row0, hf ? row0 : h, b);
-      };
-      load_blk(sbase + PA_OFF_Q, &tmap_q, q_hf, BAR(B_Q), t * 128);
-      for (int j = 0; j < nkb; ++j) load_blk(sbase + PA_OFF_KP + j * PA_BLK, &tmap_k, k_hf, BAR(B_K + j), j * 128);
-      for (int j = 0; j < nkb && j < 2; ++j) load_blk(sbase + PA_OFF_V + j * PA_BLK, &tmap_v, v_hf, BAR(B_VF + j), j * 128);
-
-      constexpr uint32_t idesc_s = umma_idesc_bf16(128, 128);
-      constexpr uint32_t idesc_o = umma_idesc_bf16(128, 64) | (1u << 16);     // B operand MN-major
-      mbar_wait_safe(BAR(B_Q), 0);
-      for (int j = 0; j < nkb; ++j) {
-        mbar_wait_safe(BAR(B_K + j), 0);
-        tc_fence_after();
 #pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {                    // 16 d per step: tile half kk / 4, 32 B inside the span
-          const uint64_t qd = umma_desc_k_sw128(sbase + PA_OFF_Q + (kk >> 2) * PA_HALF) + 2u * (kk & 3);
-          const uint64_t kd = umma_desc_k_sw128(sbase + PA_OFF_KP + j * PA_BLK + (kk >> 2) * PA_HALF) + 2u * (kk & 3);
-          tc_mma_bf16(tmem + 128 * j, qd, kd, idesc_s, kk != 0 ? 1u : 0u);
-        }
-        tc_commit(BAR(B_S + j));                            // the softmax warps start on block j while K_j+1 lands
-      }
+  for (int r = 0; r < 2; ++r) {
+    m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], 1));
+    m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], 2));
+    if (m[r] == -INFINITY) m[r] = 0.f;                   // rows beyond S (all keys masked): P = 0
+  }
 
-      mbar_wait_safe(BAR(B_P), 0);                          // P written (over the K blocks), scores consumed
-      tc_fence_after();
-      auto pv_block = [&](int j) {
-        const int slot = j & 1;
-        mbar_wait_safe(BAR(B_VF + slot), (uint32_t)(j >> 1));
-        tc_fence_after();
+  // ---- pass 2: P against the final maximum, O += P . V ----
+  float o[64] = {};
+  float l[2] = {0.f, 0.f};
+  for (int kb = 0; kb < n_kb; ++kb) {
+    __syncthreads();                                     // previous readers of K / V^T / P are done
+    pa_load_rows<128>(smem + PA_OFF_K, kg, a.k_ss, kb * 128, S_kv);
+    pa_load_vt(smem + PA_OFF_VT, vg, a.v_ss, kb * 128, S_kv);
+    fence_async_smem();
+    __syncthreads();
+    pa_mma(acc, sbase + PA_OFF_Q, 64 * 128, sbase + PA_OFF_K, 128 * 128, false);
 #pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {                    // 16 keys per step
-          const uint64_t pd = umma_desc_k_sw128(sbase + PA_OFF_KP + j * PA_BLK + (kk >> 2) * PA_HALF) + 2u * (kk & 3);
+    for (int j = 0; j < 16; ++j) {
 #pragma unroll
-          for (int dh = 0; dh < 2; ++dh) {
-            const uint64_t vd = pa_desc_mn_sw128(sbase + PA_OFF_V + slot * PA_BLK + dh * PA_HALF) + (uint64_t)((kk * 2048) >> 4);
-            tc_mma_bf16(tmem + dh * 64, pd, vd, idesc_o, (j | kk) != 0 ? 1u : 0u);
-          }
-        }
-        tc_commit(BAR(B_VE + slot));                        // the slot is free once these MMAs retired
-      };
-      pv_block(0);
-      if (nkb > 1) pv_block(1);
-      for (int j = 2; j < nkb; ++j) {                       // blocks 2, 3 re-use the slots of blocks 0, 1
-        mbar_wait_safe(BAR(B_VE + (j & 1)), 0);
-        load_blk(sbase + PA_OFF_V + (j & 1) * PA_BLK, &tmap_v, v_hf, BAR(B_VF + (j & 1)), j * 128);
-      }
-      for (int j = 2; j < nkb; ++j) pv_block(j);
-      tc_commit(BAR(B_O));
-    }
-  } else if (warp < PA_SM_WARPS) {
-    // ================================ softmax warps ================================
-    const int q4 = warp & 3, cq = warp >> 2;                // TMEM lane quarter, column quarter of every key block
-    const int r = q4 * 32 + lane;
-    const int qr = t * 128 + r;                             // query row inside the clip
-    const int qpos = q_off + qr;                            // its absolute position
-    const uint32_t tlane = tmem + ((uint32_t)(q4 * 32) << 16);
-    constexpr float LOG2E = 1.4426950408889634f;
-
-    // Scores as the reference holds them: bf16(q.k), times `scaling` (fp32) into bf16 again, masked. Two raw
-    // scores -> one packed bf16 pair. Only the blocks that touch the diagonal or the end of the keys need the
-    // mask; a block is clear when its last key is visible to the first row of the tile.
-    auto scaled_pair = [&](uint32_t r0, uint32_t r1) {
-      const uint32_t s2 = pack_bf16x2(__uint_as_float(r0), __uint_as_float(r1));
-      return pack_bf16x2(bf16lo(s2) * scale, bf16hi(s2) * scale);
-    };
-    auto masked_pair = [&](uint32_t x2, int kidx) {        // keys kidx, kidx + 1
-      const uint32_t lo = (kidx > qpos || kidx >= S_kv) ? 0xff80u : (x2 & 0xffffu);            // bf16 -inf
-      const uint32_t hi = (kidx + 1 > qpos || kidx + 1 >= S_kv) ? 0xff800000u : (x2 & 0xffff0000u);
-      return lo | hi;
-    };
-    const int clear_until = min(q_off + t * 128, S_kv - 1);   // keys <= this are visible to every row of the tile
-    // the TMEM load of block j + 1 is in flight while block j is worked on (two register buffers)
-    auto issue_ld = [&](uint32_t (&v)[32], int j, bool wait_s) {
-      if (wait_s) { mbar_wait_safe(BAR(B_S + j), 0); tc_fence_after(); }
-      __syncwarp();
-      tmem_ld_32x32(tlane + 128 * j + 32 * cq, v);
-    };
-
-    // ---- pass 1: row maximum ----
-    __nv_bfloat162 mx2 = __float2bfloat162_rn(-INFINITY);
-    auto pass1 = [&](const uint32_t (&v)[32], int j) {
-      const int k0 = 128 * j + 32 * cq;
-      const bool clear = k0 + 31 <= clear_until;
-#pragma unroll
-      for (int c = 0; c < 16; ++c) {
-        uint32_t x2 = scaled_pair(v[2 * c], v[2 * c + 1]);
-        if (!clear) x2 = masked_pair(x2, k0 + 2 * c);
-        mx2 = __hmax2(mx2, *reinterpret_cast<const __nv_bfloat162*>(&x2));
-      }
-    };
-    uint32_t va[32], vb[32];
-    issue_ld(va, 0, true);
-    for (int j = 0; j < nkb; j += 2) {
-      tc_wait_ld();
-      if (j + 1 < nkb) issue_ld(vb, j + 1, true);
-      pass1(va, j);
-      if (j + 1 < nkb) {
-        tc_wait_ld();
-        if (j + 2 < nkb) issue_ld(va, j + 2, true);
-        pass1(vb, j + 1);
+      for (int hh = 0; hh < 2; ++hh) {
+        const int i = 4 * j + 2 * hh;
+        const float p0 = exp2f((score(kb, i) - m[hh]) * 1.4426950408889634f);
+        const float p1 = exp2f((score(kb, i + 1) - m[hh]) * 1.4426950408889634f);
+        l[hh] += p0 + p1;
+        const int row = r0 + 8 * hh, col = 8 * j + c2;   // col = key inside the block
+        *reinterpret_cast<uint32_t*>(smem + PA_OFF_P + (col >> 6) * (64 * 128) + pa_sw128(row, (col & 63) >> 3) +
+                                     (col & 7) * 2) = pack_bf16x2(p0, p1);
       }
     }
-    issue_ld(va, 0, false);                                 // pass 2's first block, in flight across the exchange
-    smax[cq * 128 + r] = fmaxf(__low2float(mx2), __high2float(mx2));   // all S MMAs have retired: Q is dead
-    pa_bar_sync(1, PA_SM_THREADS);
-    const float m = fmaxf(fmaxf(smax[r], smax[128 + r]), fmaxf(smax[256 + r], smax[384 + r]));   // key 0 is never masked
-    const float mb = m * LOG2E;
+    fence_async_smem();
+    __syncthreads();
+    pa_mma(o, sbase + PA_OFF_P, 64 * 128, sbase + PA_OFF_VT, 128 * 128, kb > 0);
+  }
 
-    // ---- pass 2: exponentials, P -> shared memory, row sum ----
-    float sum = 0.f;
-    auto pass2 = [&](const uint32_t (&v)[32], int j) {
-      const int k0 = 128 * j + 32 * cq;
-      const bool clear = k0 + 31 <= clear_until;
-      uint32_t pk[16];
+  // ---- O / l -> bf16 ----
 #pragma unroll
-      for (int c = 0; c < 16; ++c) {
-        uint32_t x2 = scaled_pair(v[2 * c], v[2 * c + 1]);
-        if (!clear) x2 = masked_pair(x2, k0 + 2 * c);
-        const float p0 = pa_ex2(fmaf(bf16lo(x2), LOG2E, -mb));
-        const float p1 = pa_ex2(fmaf(bf16hi(x2), LOG2E, -mb));
-        sum += p0 + p1;
-        pk[c] = pack_bf16x2(p0, p1);
-      }
-      // keys [32 cq, 32 cq + 32) of block j: tile half cq / 2, 16-byte chunks 4 (cq & 1) .. + 3 of row r
-      uint8_t* tile = smem + PA_OFF_KP + j * PA_BLK + (cq >> 1) * PA_HALF;
+  for (int r = 0; r < 2; ++r) {
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
+  }
+  bf16* og = a.o + (long long)b * a.o_sb + (long long)h * a.o_sh;
 #pragma unroll
-      for (int q = 0; q < 4; ++q)
-        *reinterpret_cast<uint4*>(tile + pa_sw128(r, (cq & 1) * 4 + q)) =
-            make_uint4(pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-    };
-    for (int j = 0; j < nkb; j += 2) {
-      tc_wait_ld();
-      if (j + 1 < nkb) issue_ld(vb, j + 1, false);
-      pass2(va, j);
-      if (j + 1 < nkb) {
-        tc_wait_ld();
-        if (j + 2 < nkb) issue_ld(va, j + 2, false);
-        pass2(vb, j + 1);
-      }
-    }
-    ssum[cq * 128 + r] = sum;
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc_fence_before();
-    mbar_arrive(BAR(B_P));
-
-    mbar_wait_safe(BAR(B_O), 0);
-    tc_fence_after();
-    uint32_t o[32];
-    __syncwarp();
-    tmem_ld_32x32(tlane + 32 * cq, o);
-    tc_wait_ld();
-    if (qr < S) {
-      const float inv = 1.0f / (ssum[r] + ssum[128 + r] + ssum[256 + r] + ssum[384 + r]);
-      bf16* dst = out + (long long)b * o_sb + (long long)h * o_sh + (long long)qr * o_ss + cq * 32;
+  for (int hh = 0; hh < 2; ++hh) {
+    const int qrow = q0 + r0 + 8 * hh;
+    if (qrow < a.S) {
+      const float inv = 1.0f / l[hh];
+      bf16* dst = og + (long long)qrow * a.o_ss + c2;
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        uint32_t w[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e)
-          w[e] = pack_bf16x2(__uint_as_float(o[8 * q + 2 * e]) * inv, __uint_as_float(o[8 * q + 2 * e + 1]) * inv);
-        *reinterpret_cast<uint4*>(dst + q * 8) = make_uint4(w[0], w[1], w[2], w[3]);
-      }
+      for (int j = 0; j < 16; ++j)
+        *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_bf16x2(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == PA_SM_WARPS + 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 512);
-  }
-}
-
-// 4-D bf16 tensor map over (d, position, head, clip) given element strides; box = [64 d x 128 positions], 128-B
-// swizzle. Positions >= n_pos are out of bounds and read as zero. The driver documents the strides as growing
-// from dimension to dimension, so the head dimension goes in front of the position dimension when its stride is
-// the smaller one ([clip, position, head, d] activations) and behind it otherwise ([clip, head, position, d]
-// cache); *head_first tells the kernel which coordinate order to use.
-int make_tmap_attn(CUtensorMap* out, int* head_first, const bf16* ptr, int n_pos, int H, int B, long long s_pos,
-                   long long s_head, long long s_clip) {
-  static PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
-  if (encode == nullptr) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres);
-    if (e != cudaSuccess || fn == nullptr || qres != cudaDriverEntryPointSuccess) {
-      set_last_error("cuTensorMapEncodeTiled is not available from the driver (%s)", cudaGetErrorString(e));
-      return -2;
-    }
-    encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
-  }
-  const bool hf = H > 1 && s_head < s_pos;
-  *head_first = hf ? 1 : 0;
-  cuuint64_t gdim[4] = {128u, (cuuint64_t)(hf ? H : n_pos), (cuuint64_t)(hf ? n_pos : H), (cuuint64_t)B};
-  long long st[3] = {hf ? s_head : s_pos, hf ? s_pos : s_head, s_clip};
-  cuuint64_t gstride[3];
-  cuuint64_t prev = 128 * 2;                               // bytes spanned by the previous dimension
-  for (int i = 0; i < 3; ++i) {
-    // a dimension of extent 1 is never stepped over: give it the packed stride
-    gstride[i] = gdim[i + 1] > 1 ? (cuuint64_t)st[i] * 2 : prev;
-    prev = gstride[i] * gdim[i + 1];
-  }
-  cuuint32_t box[4] = {64u, hf ? 1u : 128u, hf ? 128u : 1u, 1u};
-  cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
-  CUresult r = encode(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<bf16*>(ptr), gdim, gstride, box, estr,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error("attention_prefill_tc: cuTensorMapEncodeTiled failed (%d) n_pos=%d H=%d B=%d strides %lld %lld %lld",
-                   (int)r, n_pos, H, B, s_pos, s_head, s_clip);
-    return -2;
-  }
-  return 0;
 }
 
 }  // namespace
@@ -349,20 +197,16 @@ bool attention_prefill_tc_supported(const AttnArgs& a) {
   const int S_kv = a.S_kv > 0 ? a.S_kv : a.S;
   if (off || !a.causal || a.head_dim != 128 || S_kv > 128 * PA_MAX_KB || a.S <= 0) return false;
   if (a.q_off + a.S > S_kv) return false;                                 // every query sees its own key
-  if (a.o_ss % 8 != 0 || a.o_sh % 8 != 0 || a.o_sb % 8 != 0 || ((uintptr_t)a.o % 16) != 0) return false;
+  if (a.o_ss % 2 != 0 || a.o_sh % 2 != 0 || a.o_sb % 2 != 0 || ((uintptr_t)a.o % 4) != 0) return false;
+  if (a.q_ss % 8 != 0 || a.q_sh % 8 != 0 || a.q_sb % 8 != 0 || a.k_ss % 8 != 0 || a.k_sh % 8 != 0 ||
+      a.k_sb % 8 != 0 || a.v_ss % 8 != 0 || a.v_sh % 8 != 0 || a.v_sb % 8 != 0) return false;   // 16-byte row loads
   return ((uintptr_t)a.q % 16) == 0 && ((uintptr_t)a.k % 16) == 0 && ((uintptr_t)a.v % 16) == 0;
 }
 
 int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t stream) {
   const int S_kv = a.S_kv > 0 ? a.S_kv : a.S;
-  CUtensorMap tq, tk, tv;
-  int q_hf, k_hf, v_hf;
-  if (make_tmap_attn(&tq, &q_hf, a.q, a.S, a.H, a.B, a.q_ss, a.q_sh, a.q_sb) != 0) return -2;
-  if (make_tmap_attn(&tk, &k_hf, a.k, S_kv, a.H, a.B, a.k_ss, a.k_sh, a.k_sb) != 0) return -2;
-  if (make_tmap_attn(&tv, &v_hf, a.v, S_kv, a.H, a.B, a.v_ss, a.v_sh, a.v_sb) != 0) return -2;
-  dim3 grid((a.S + 127) / 128, a.H, a.B);
-  attn_prefill_tc_kernel<<<grid, PA_THREADS, PA_SMEM, stream>>>(tq, tk, tv, a.o, a.o_sb, a.o_sh, a.o_ss, a.S, S_kv,
-                                                                a.q_off, a.scale, q_hf, k_hf, v_hf);
+  dim3 grid((a.S + 63) / 64, a.H, a.B);
+  attn_prefill_tc_kernel<<<grid, PA_THREADS, PA_SMEM, stream>>>(a, S_kv);
   VCL_CUDA_OK(cudaGetLastError());
   count_launches(1);
   return 0;

@@ -1,696 +1,220 @@
-// CLIP ViT self-attention on the 5th-generation tensor cores (non-causal, head_dim 64, S = P+1).
+// Attention of the CLIP ViT on the Hopper warpgroup tensor cores (head_dim 64, non-causal, 129 <= S <= 257).
 //
-// A work item is one 128-query tile of one (frame, head); two CTAs per SM. The S x S problem is tiny
-// (257 x 257 for ViT-L/14 @224), so the whole K and V of the head live in shared memory and the scores of
-// 128 queries x 256 keys live in TMEM:
+// One CTA per (frame, head), two warpgroups; warpgroup w takes the 64-query tiles w, w + 2, ... of the frame (three
+// warpgroups fit in shared memory, but not in registers without spilling: measured slower).
+// K (all keys of the head, up to 320 rows) and Q tiles arrive by TMA straight out of the fused q|k|v activation
+// (2-D tensor map, 128-byte swizzle: one 64-wide head is exactly one swizzle span, so the tiles land in the K-major
+// layout wgmma reads); V is transposed by the threads into K-major [64 d x 64 keys] tiles, keys >= S zero.
+//   S = Q . K^T    wgmma M64 x N256 x K64 over keys [0, 256), plus M64 x N32 over keys [256, 288) when S > 256
+//   O = P . V      wgmma M64 x N64, K = keys (16 k-steps, plus one for key 256), P from shared memory
+// The whole score row of a query lives in registers, so the softmax is the EXACT full-row softmax of the eager
+// reference (one pass, P against the final row maximum). Keys >= S (rows of the next frame, or TMA zero fill at the
+// end of the tensor) are masked; queries >= S are computed and not stored.
 //
-//   warp 8 (1 thread)  TMA: Q tile [128 x 64], K, V tiles [256 rows x 64] of this (frame, head) straight
-//                      out of the fused qkv activation (128-B swizzle); then issues all tcgen05.mma:
-//                        S = Q . K^T      M128 x N256 x K64   -> TMEM columns [0, 256)
-//                        O = P . V        M128 x N64  x K256  -> TMEM columns [0, 64)
-//                      (V is used as an MN-major B operand, so no transpose is ever materialised)
-//   warps 0-7          softmax: thread (row, column half) reads its 128 score columns from TMEM ONCE,
-//                      keeps them as packed bf16 in registers (row max on the packed pairs), then exp2,
-//                      writes P as bf16 into a K-major swizzled smem tile that the second MMA consumes,
-//                      and finally normalises and stores 32 O columns
-//   warp 9             TMEM allocator; softmax + PV of query row 256 (the 257th token)
-//
-// Two kernels share this tile pipeline:
-//   attn_vit_tc1p_kernel  (default) persistent: 2 x #SMs CTAs walk the tile list; set-up once per CTA, the
-//                         next tile's Q | K are fetched while the current tile's epilogue runs
-//   attn_vit_tc1_kernel   one CTA per tile (VCL_ATTN_ONE_SHOT=1): 95 us per layer against 87-93 us
-// Per-tile timeline of the persistent kernel (tools/attn_trace.py, two CTAs sharing the SM): 0.8 us wait
-// for Q | K, 1.3 us row-256 dot products + wait for S, 0.4 us pass 1, 2.7 us exp2 pass, 1.1 us wait for
-// P.V, 1.2 us epilogue = 7.5 us per tile and CTA. Measured alternatives (tools/experiments/): one CTA per
-// (frame, head) with both tiles in 512 TMEM columns (round 1: 119 us per layer); a persistent CTA per SM
-// that runs both tiles of an item in lock-step (round 2: parity-green, 108 us -- two independent CTAs per
-// SM overlap each other's phases better).
-//
-// S = 257 = 2*128 + 1: the 257th KEY is folded in analytically (one extra 64-long dot product per
-// query row, added to the max / sum / output), and the 257th QUERY row is a 33k-MAC problem whose
-// scores are computed by the softmax threads (one dot product each) and finished by warp 17 --
-// this keeps the tensor-core problem at exactly two M128 x N256 tiles and TMEM at 512 columns.
-//
-// The kernel is bound by CUDA-core work (exp2 on the MUFU pipe and the instructions around it),
-// not by the MMAs (6.6 % tensor-pipe active in the first version), so the softmax is spread over 16
-// warps and its inner loop is kept to ~5 instructions per score.
-//
-// Arithmetic follows transformers/models/clip/modeling_clip.py:261-279 (eager): the score tensor
-// is rounded to bf16 before the (exact, 2^-3) scaling, softmax statistics are fp32, P is rounded to
-// bf16 before the PV product. Like the flash-style kernel it replaces, P is rounded before the
-// normalisation rather than after (the one deliberate difference, inside the parity tolerance).
+// Arithmetic follows transformers/models/clip/modeling_clip.py:261-279 (eager): the scores are a bf16 tensor,
+// multiplied by `scale` into another bf16 tensor, softmax in fp32, probabilities cast to bf16 for P.V. As in the
+// other attention kernels of this library P is rounded before the normalisation.
 #include "common.cuh"
 #include "kernels.h"
 
-#include <cudaTypedefs.h>
-#include <stddef.h>
 #include <stdlib.h>
 
 namespace vcl {
 
 namespace {
 
-constexpr int TILE_BYTES = 256 * 128;            // 256 rows x 64 bf16
-unsigned long long* g_attn_trace = nullptr;      // debug: set by vcl_debug_set_attn_trace (tools/attn_trace.py)
+constexpr int VA_WG = 2;                                 // warpgroups per CTA
+constexpr int VA_THREADS = VA_WG * 128;
+constexpr int VA_TILE = 64 * 128;                        // one [64 rows x 64 bf16] swizzled tile (8 KB)
+constexpr int VA_KEY_TILES = 5;                          // keys [0, 320)
+constexpr int VA_OFF_K = 0;                              // K: [320 keys x 64 d]
+constexpr int VA_OFF_VT = VA_OFF_K + VA_KEY_TILES * VA_TILE;    // V^T: 5 tiles [64 d x 64 keys]
+constexpr int VA_OFF_Q = VA_OFF_VT + VA_KEY_TILES * VA_TILE;    // Q: one tile per warpgroup
+constexpr int VA_OFF_P = VA_OFF_Q + VA_WG * VA_TILE;            // P: 5 tiles [64 q x 64 keys] per warpgroup
+constexpr int VA_OFF_BAR = VA_OFF_P + VA_WG * VA_KEY_TILES * VA_TILE;
+constexpr int VA_SMEM = VA_OFF_BAR + 64 + 1024;          // + barriers + manual 1024-B alignment
+static_assert(VA_SMEM <= 227 * 1024, "shared memory");
 
-__device__ __forceinline__ uint32_t sw128(int row, int chunk) {   // byte offset inside a SW128 tile
+__device__ __forceinline__ uint32_t va_sw128(int row, int chunk) {
   return (uint32_t)row * 128u + (uint32_t)((chunk ^ (row & 7)) << 4);
 }
 
-// MN-major SW128 operand (V: rows = keys = K index, 64 contiguous d = N): 8-row groups 1024 B apart.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3ffffu) >> 4);
-  d |= (uint64_t)(1024u >> 4) << 16;   // leading byte offset (next 64-wide MN atom; single atom here)
-  d |= (uint64_t)(1024u >> 4) << 32;   // stride byte offset: next group of 8 K rows
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
+__device__ __forceinline__ void named_bar_sync_wg(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
-__device__ __forceinline__ void named_bar_sync(int id, int n) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
-}
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-// 32 lanes x 16 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, "
-      "%12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-// 64-long dot product of an fp32 vector in smem with one row of a swizzled bf16 tile
-__device__ __forceinline__ float dot64(const uint8_t* tile, int row, const float* vec) {
-  float d = 0.f;
-#pragma unroll
-  for (int c = 0; c < 8; ++c) {
-    const uint4 u = *reinterpret_cast<const uint4*>(tile + sw128(row, c));
-    const float4 a = *reinterpret_cast<const float4*>(vec + c * 8);
-    const float4 b = *reinterpret_cast<const float4*>(vec + c * 8 + 4);
-    d += a.x * bf16lo(u.x) + a.y * bf16hi(u.x) + a.z * bf16lo(u.y) + a.w * bf16hi(u.y) +
-         b.x * bf16lo(u.z) + b.y * bf16hi(u.z) + b.z * bf16lo(u.w) + b.w * bf16hi(u.w);
-  }
-  return d;
-}
-
-// ---------------------------------------------------------------------------------------------
-// Single-tile variant: one CTA per (frame, head, 128-query tile), TWO CTAs per SM (256 TMEM columns
-// and ~104 KB of shared memory each), so that one CTA's TMA / MMA / barrier latencies overlap the
-// other's softmax. Same arithmetic as above. P (64 KB) re-uses the Q|K region (48 KB) plus one
-// extra 16 KB block once S has been computed and the Q / K rows have been read.
-// ---------------------------------------------------------------------------------------------
-constexpr int T1_SM_WARPS = 8;
-constexpr int T1_SM_THREADS = T1_SM_WARPS * 32;              // 256
-constexpr int T1_THREADS = T1_SM_THREADS + 64;
-constexpr int T1_OFF_Q = 0, T1_OFF_K = 128 * 128, T1_OFF_V = T1_OFF_K + TILE_BYTES;
-constexpr int T1_OFF_P3 = T1_OFF_V + TILE_BYTES;             // 4th P block (blocks 0-2 alias Q|K)
-constexpr int T1_OFF_SMALL = T1_OFF_P3 + 16384;
-constexpr int T1_SMEM = T1_OFF_SMALL + 8192 + 1024;
-
-struct Small1 {
-  unsigned long long bar[8];
-  uint32_t tmem_base, pad_[3];
-  float q256[64], k256[64], v256[64];
-  float p256[128];
-  float s256[128];
-  float tsc[260];
-  float smax[2][128];
-  float ssum[2][128];
-};
-static_assert(sizeof(Small1) <= 8192, "Small1");
-
-template <bool FULL>
-__global__ void __launch_bounds__(T1_THREADS, 2)
-attn_vit_tc1_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
-                    const bf16* __restrict__ qkv, bf16* __restrict__ out, int S, int H, int C,
-                    unsigned long long* __restrict__ trace) {
-  // optional per-CTA phase timestamps (tools/attn_trace.py); null in production
-  auto stamp = [&](int ev) {
-    if (trace != nullptr) {
-      unsigned long long t_;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_));
-      trace[(size_t)blockIdx.x * 8 + ev] = t_;
-    }
-  };
-  if (threadIdx.x == 0) stamp(0);
+__global__ void __launch_bounds__(VA_THREADS, 1)
+attn_vit_tc_kernel(const __grid_constant__ CUtensorMap tmap, const bf16* __restrict__ qkv, bf16* __restrict__ out,
+                   int S, int H, int C) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t pad = ((raw + 1023u) & ~1023u) - raw;
+  const uint32_t raw_addr = smem_u32(smem_raw);
+  const uint32_t pad = ((raw_addr + 1023u) & ~1023u) - raw_addr;
   uint8_t* smem = smem_raw + pad;
-  const uint32_t sbase = raw + pad;
-  Small1* sm = reinterpret_cast<Small1*>(smem + T1_OFF_SMALL);
-  const uint32_t bar0 = sbase + T1_OFF_SMALL + (uint32_t)offsetof(Small1, bar);
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
-  enum { B_LOAD = 0, B_S = 1, B_P = 2, B_O = 3, B_TAIL = 4 };
+  const uint32_t sbase = raw_addr + pad;
+  const uint32_t kbar = sbase + VA_OFF_BAR;
+  auto qbar = [&](int w) { return sbase + VA_OFF_BAR + 8u * (1 + w); };
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int t = blockIdx.x & 1;                              // query tile of this CTA
-  const int h = (blockIdx.x >> 1) % H, n = (blockIdx.x >> 1) / H;
-  const long long row0 = (long long)n * S;
-  const int ld = 3 * C;
-  const bool key256 = S > 256;
-  const bool do_tail = key256 && t == 1;                     // query row 256 rides with tile 1
+  const int frame = blockIdx.x / H, h = blockIdx.x - frame * H;
+  const int row0 = frame * S;                            // first row of this frame in the activation
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127, lane = threadIdx.x & 31, wq = t >> 5;
+  const int n_qt = (S + 63) / 64;
+  const int n_kt = (S + 63) / 64;                        // K tiles that hold keys
 
-  if (warp == T1_SM_WARPS && lane == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_kv);
-    mbar_init(BAR(B_LOAD), 1);
-    mbar_init(BAR(B_S), 1);
-    mbar_init(BAR(B_P), T1_SM_THREADS);
-    mbar_init(BAR(B_O), 1);
-    mbar_init(BAR(B_TAIL), T1_SM_THREADS);
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap);
+    mbar_init(kbar, 1);
+    for (int w = 0; w < VA_WG; ++w) mbar_init(qbar(w), 1);
     mbar_fence_init();
   }
-  if (warp == T1_SM_WARPS + 1) {
-    tmem_alloc(sbase + T1_OFF_SMALL + (uint32_t)offsetof(Small1, tmem_base), 256);
-    const bf16* r = qkv + (row0 + 256) * ld + h * 64;
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      const int d = lane * 2 + j;
-      sm->q256[d] = key256 ? __bfloat162float(r[d]) : 0.f;
-      sm->k256[d] = key256 ? __bfloat162float(r[C + d]) : 0.f;
-      sm->v256[d] = key256 ? __bfloat162float(r[2 * C + d]) : 0.f;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(kbar, n_kt * VA_TILE);
+    for (int i = 0; i < n_kt; ++i) tma_load_2d(sbase + VA_OFF_K + i * VA_TILE, &tmap, kbar, C + h * 64, row0 + 64 * i);
+    for (int w = 0; w < VA_WG && w < n_qt; ++w) {
+      mbar_arrive_expect_tx(qbar(w), VA_TILE);
+      tma_load_2d(sbase + VA_OFF_Q + w * VA_TILE, &tmap, qbar(w), h * 64, row0 + 64 * w);
     }
   }
-  tc_fence_before();
+  // V^T: element (d, key) in tile key / 64, row d; keys >= S (and the unused rows of K's last tile) read as zero
+  const bf16* vg = qkv + (long long)row0 * 3 * C + 2 * C + h * 64;
+  for (int idx = threadIdx.x; idx < VA_KEY_TILES * 64 * 8; idx += VA_THREADS) {
+    const int key = idx % (VA_KEY_TILES * 64), c = idx / (VA_KEY_TILES * 64);
+    uint4 v = make_uint4(0u, 0u, 0u, 0u);
+    if (key < S) v = *reinterpret_cast<const uint4*>(vg + (long long)key * 3 * C + c * 8);
+    const uint32_t w4[4] = {v.x, v.y, v.z, v.w};
+    uint8_t* tile = smem + VA_OFF_VT + (key >> 6) * VA_TILE;
+    const int kc = (key & 63) >> 3, ke = key & 7;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const uint16_t hv = (uint16_t)(e & 1 ? w4[e >> 1] >> 16 : w4[e >> 1] & 0xffffu);
+      *reinterpret_cast<uint16_t*>(tile + va_sw128(c * 8 + e, kc) + ke * 2) = hv;
+    }
+  }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   __syncthreads();
-  tc_fence_after();
-  if (threadIdx.x == 0) stamp(1);
-  const uint32_t tmem = sm->tmem_base;
-  constexpr float SCALE = 0.125f;
-  constexpr float LOG2E = 1.4426950408889634f;
-  // P block kb lives at: blocks 0..2 -> the Q|K region, block 3 -> its own 16 KB
-  auto p_off = [&](int kb) { return kb < 3 ? (uint32_t)(kb * 16384) : (uint32_t)T1_OFF_P3; };
+  mbar_wait(kbar, 0);
 
-  if (warp == T1_SM_WARPS) {
-    if (lane == 0) {
-      mbar_arrive_expect_tx(BAR(B_LOAD), 128 * 128 + 2 * TILE_BYTES);
-      tma_load_2d(sbase + T1_OFF_Q, &tmap_q, BAR(B_LOAD), h * 64, (int)row0 + t * 128);
-      tma_load_2d(sbase + T1_OFF_K, &tmap_kv, BAR(B_LOAD), C + h * 64, (int)row0);
-      tma_load_2d(sbase + T1_OFF_V, &tmap_kv, BAR(B_LOAD), 2 * C + h * 64, (int)row0);
-      mbar_wait(BAR(B_LOAD), 0);
-      tc_fence_after();
-      constexpr uint32_t idesc_s = umma_idesc_bf16(128, 256);
-      constexpr uint32_t idesc_o = umma_idesc_bf16(128, 64) | (1u << 16);
-      const uint64_t kdesc = umma_desc_k_sw128(sbase + T1_OFF_K);
-      const uint64_t qdesc = umma_desc_k_sw128(sbase + T1_OFF_Q);
+  const int r0 = 16 * wq + (lane >> 2), c2 = 2 * (lane & 3);
+  const bool tail = S > 256;                             // keys [256, S): one more N32 block
+  uint8_t* P = smem + VA_OFF_P + wg * VA_KEY_TILES * VA_TILE;
+  const uint32_t p_addr = sbase + VA_OFF_P + wg * VA_KEY_TILES * VA_TILE;
+  const uint32_t q_addr = sbase + VA_OFF_Q + wg * VA_TILE;
+  uint32_t qphase = 0;
+  float s[128], s2[16], o[32];
+  for (int qt = wg; qt < n_qt; qt += VA_WG) {
+    mbar_wait(qbar(wg), qphase);
+    qphase ^= 1u;
+    // ---- S = Q . K^T ----  (the accumulators are defined here, so they are not live across iterations)
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-        tc_mma_bf16(tmem, qdesc + 2u * k, kdesc + 2u * k, idesc_s, k != 0 ? 1u : 0u);
-      tc_commit(BAR(B_S));
-      mbar_wait(BAR(B_P), 0);
-      tc_fence_after();
-      const uint64_t vdesc = umma_desc_mn_sw128(sbase + T1_OFF_V);
+    for (int i = 0; i < 128; ++i) s[i] = 0.f;
 #pragma unroll
-      for (int kk = 0; kk < 16; ++kk) {
-        const uint64_t pdesc = umma_desc_k_sw128(sbase + p_off(kk >> 2)) + 2u * (kk & 3);
-        tc_mma_bf16(tmem, pdesc, vdesc + (uint64_t)((kk * 2048) >> 4), idesc_o, kk != 0 ? 1u : 0u);
-      }
-      tc_commit(BAR(B_O));
+    for (int i = 0; i < 16; ++i) s2[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint64_t ad = wgmma_desc_k_sw128(q_addr) + 2u * k;
+      wgmma_bf16<256>(s, ad, wgmma_desc_k_sw128(sbase + VA_OFF_K) + 2u * k, k > 0 ? 1u : 0u);
+      if (tail) wgmma_bf16<32>(s2, ad, wgmma_desc_k_sw128(sbase + VA_OFF_K + 256 * 128) + 2u * k, k > 0 ? 1u : 0u);
     }
-  } else if (warp == T1_SM_WARPS + 1) {
-    if (do_tail) {
-      mbar_wait(BAR(B_TAIL), 0);
-      if (lane == 0) {
-        float d = 0.f;
-#pragma unroll
-        for (int c = 0; c < 64; ++c) d += sm->q256[c] * sm->k256[c];
-        sm->tsc[256] = bf16r(d) * SCALE;
-      }
-      __syncwarp();
-      float sc[9];
-      float mx = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < 9; ++i) {
-        const int j = lane + 32 * i;
-        sc[i] = (j <= 256) ? sm->tsc[j] : -INFINITY;
-        mx = fmaxf(mx, sc[i]);
-      }
-      mx = warp_max(mx);
-      float sum = 0.f;
-      __syncwarp();
-#pragma unroll
-      for (int i = 0; i < 9; ++i) {
-        const int j = lane + 32 * i;
-        const float p = (j <= 256) ? ex2_approx((sc[i] - mx) * LOG2E) : 0.f;
-        sum += p;
-        if (j <= 256) sm->tsc[j] = bf16r(p);
-      }
-      sum = warp_sum(sum);
-      __syncwarp();
-      float o0 = 0.f, o1 = 0.f;
-      const int ch = lane >> 2, wi = (lane & 3) * 4;
-#pragma unroll 8
-      for (int j = 0; j < 256; ++j) {
-        const uint32_t v = *reinterpret_cast<const uint32_t*>(smem + T1_OFF_V + sw128(j, ch) + wi);
-        const float p = sm->tsc[j];
-        o0 += p * bf16lo(v);
-        o1 += p * bf16hi(v);
-      }
-      o0 += sm->tsc[256] * sm->v256[2 * lane];
-      o1 += sm->tsc[256] * sm->v256[2 * lane + 1];
-      const float inv = 1.0f / sum;
-      *reinterpret_cast<uint32_t*>(out + (row0 + 256) * C + h * 64 + 2 * lane) = pack_bf16x2(o0 * inv, o1 * inv);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    wgmma_fence_regs(s2);
+    named_bar_sync_wg(1 + wg);                           // every thread's wgmma has read Q and the previous P
+    if (t == 0 && qt + VA_WG < n_qt) {                   // next query tile of this warpgroup
+      mbar_arrive_expect_tx(qbar(wg), VA_TILE);
+      tma_load_2d(q_addr, &tmap, qbar(wg), h * 64, row0 + 64 * (qt + VA_WG));
     }
-  } else {
-    const int q4 = warp & 3, hf = warp >> 2;                  // TMEM lane quarter, column half
-    const int r = q4 * 32 + lane;
-    mbar_wait(BAR(B_LOAD), 0);
-    if (threadIdx.x == 0) stamp(2);
-    if (key256) {
-      const int tix = threadIdx.x;                            // 0..255
-      if (tix < 128) sm->s256[tix] = bf16r(dot64(smem + T1_OFF_Q, tix, sm->k256)) * SCALE;
-      if (do_tail) sm->tsc[tix] = bf16r(dot64(smem + T1_OFF_K, tix, sm->q256)) * SCALE;
-    } else if (threadIdx.x < 128) {
-      sm->s256[threadIdx.x] = -INFINITY;
+    // ---- exact softmax over the full row ----  (the scaled scores are bf16 values: kept packed in pairs)
+    auto sc = [&](float x, int key) { return key < S ? bf16r(bf16r(x) * 0.125f) : -INFINITY; };
+    float m[2] = {-INFINITY, -INFINITY};
+    uint32_t sp[64], sp2[8];
+    auto pack_sc = [&](const float* a, int i, int key0) {     // pair i of a block whose first key is key0
+      const int hh = i & 1, col = key0 + 8 * (i >> 1) + c2;
+      const float x0 = sc(a[2 * i], col), x1 = sc(a[2 * i + 1], col + 1);
+      m[hh] = fmaxf(m[hh], fmaxf(x0, x1));
+      return pack_bf16x2(x0, x1);
+    };
+    if (tail) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) sp2[i] = pack_sc(s2, i, 256);
     }
-    mbar_arrive(BAR(B_TAIL));
-    const uint32_t taddr = tmem + ((uint32_t)(q4 * 32) << 16) + hf * 128;
-    const int n_valid = FULL ? 128 : max(0, min(128, S - hf * 128));
-    mbar_wait(BAR(B_S), 0);
-    tc_fence_after();
-    if (threadIdx.x == 0) stamp(3);
-    // The 128 scores of this thread are read from TMEM ONCE (TMEM reads run at 64 B/clk per SM and
-    // were the largest single cost of the kernel when every score was read twice): they are rounded to
-    // bf16 right away -- the reference rounds the score tensor to bf16 before the scaling -- and kept
-    // packed in 64 registers; the row maximum is taken on the packed pairs (max commutes with rounding).
-    uint32_t st[64];
-    __nv_bfloat162 mx2 = __float2bfloat162_rn(-INFINITY);
 #pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      uint32_t v[16];
-      __syncwarp();
-      tmem_ld_32x16(taddr + c * 16, v);
-      tc_wait_ld();
+    for (int i = 0; i < 64; ++i) sp[i] = pack_sc(s, i, 0);
+    float l[2] = {0.f, 0.f};
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float a = __uint_as_float(v[2 * j]), b = __uint_as_float(v[2 * j + 1]);
-        if (!FULL) {
-          if (c * 16 + 2 * j >= n_valid) a = -INFINITY;
-          if (c * 16 + 2 * j + 1 >= n_valid) b = -INFINITY;
-        }
-        const uint32_t s2 = pack_bf16x2(a, b);
-        st[c * 8 + j] = s2;
-        mx2 = __hmax2(mx2, *reinterpret_cast<const __nv_bfloat162*>(&s2));
-      }
+    for (int r = 0; r < 2; ++r) {
+      m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], 1));
+      m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], 2));
     }
-    const float mx = fmaxf(__low2float(mx2), __high2float(mx2));
-    sm->smax[hf][r] = mx * SCALE;
-    named_bar_sync(1, T1_SM_THREADS);                         // also: all Q / K row reads are done
-    if (threadIdx.x == 0) stamp(4);
-    const float m = fmaxf(fmaxf(sm->smax[0][r], sm->smax[1][r]), sm->s256[r]);
-    const float mb = m * LOG2E;
-    if (hf == 0) sm->p256[r] = key256 ? ex2_approx(sm->s256[r] * LOG2E - mb) : 0.f;
-    float sum = 0.f;
+    auto put_p = [&](uint32_t x2, int i, int key0) {        // P pair (row, col), (row, col + 1) as bf16
+      const int hh = i & 1, row = r0 + 8 * hh, col = key0 + 8 * (i >> 1) + c2;
+      const float p0 = exp2f((bf16lo(x2) - m[hh]) * 1.4426950408889634f);
+      const float p1 = exp2f((bf16hi(x2) - m[hh]) * 1.4426950408889634f);
+      l[hh] += p0 + p1;
+      *reinterpret_cast<uint32_t*>(P + (col >> 6) * VA_TILE + va_sw128(row, (col & 63) >> 3) + (col & 7) * 2) =
+          pack_bf16x2(p0, p1);
+    };
 #pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      uint32_t pk[16];
+    for (int i = 0; i < 64; ++i) put_p(sp[i], i, 0);
+    if (tail) {
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const uint32_t s2 = st[c * 16 + j];
-        // masked columns hold -inf: exp2(-inf) = 0, no select needed
-        const float p0 = ex2_approx(fmaf(bf16lo(s2), SCALE * LOG2E, -mb));
-        const float p1 = ex2_approx(fmaf(bf16hi(s2), SCALE * LOG2E, -mb));
-        sum += p0 + p1;
-        pk[j] = pack_bf16x2(p0, p1);
-      }
-      const int key0 = hf * 128 + c * 32;
-      const uint32_t pb = p_off(key0 >> 6);
-      const int ch0 = (key0 & 63) >> 3;
-#pragma unroll
-      for (int q = 0; q < 4; ++q)
-        *reinterpret_cast<uint4*>(smem + pb + sw128(r, ch0 + q)) =
-            make_uint4(pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
+      for (int i = 0; i < 8; ++i) put_p(sp2[i], i, 256);
     }
-    sm->ssum[hf][r] = sum;
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc_fence_before();
-    mbar_arrive(BAR(B_P));
-    if (threadIdx.x == 0) stamp(5);
-    // epilogue: 32 of the 64 output columns per thread
-    mbar_wait(BAR(B_O), 0);
-    tc_fence_after();
-    if (threadIdx.x == 0) stamp(6);
-    uint32_t v[32];
-    __syncwarp();
-    tmem_ld_32x32(tmem + ((uint32_t)(q4 * 32) << 16) + hf * 32, v);
-    tc_wait_ld();
-    const int qr = t * 128 + r;
-    if (qr < S && qr < 256) {
-      const float p256 = sm->p256[r];
-      const float total = sm->ssum[0][r] + sm->ssum[1][r] + p256;
-      const float inv = 1.0f / total;
-      const float pb = bf16r(p256);
-      uint32_t o[16];
+    named_bar_sync_wg(1 + wg);
+    // ---- O = P . V ----
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const float a = __uint_as_float(v[2 * j]) + pb * sm->v256[hf * 32 + 2 * j];
-        const float b = __uint_as_float(v[2 * j + 1]) + pb * sm->v256[hf * 32 + 2 * j + 1];
-        o[j] = pack_bf16x2(a * inv, b * inv);
-      }
-      bf16* dst = out + (row0 + qr) * C + h * 64 + hf * 32;
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    wgmma_fence();
 #pragma unroll
-      for (int q = 0; q < 4; ++q)
-        *reinterpret_cast<uint4*>(dst + q * 8) = make_uint4(o[4 * q], o[4 * q + 1], o[4 * q + 2], o[4 * q + 3]);
+    for (int kk = 0; kk < 16; ++kk)
+      wgmma_bf16<64>(o, wgmma_desc_k_sw128(p_addr + (kk >> 2) * VA_TILE) + 2u * (kk & 3),
+                     wgmma_desc_k_sw128(sbase + VA_OFF_VT + (kk >> 2) * VA_TILE) + 2u * (kk & 3), kk > 0 ? 1u : 0u);
+    if (tail)
+      wgmma_bf16<64>(o, wgmma_desc_k_sw128(p_addr + 4 * VA_TILE), wgmma_desc_k_sw128(sbase + VA_OFF_VT + 4 * VA_TILE), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    // ---- O / l -> bf16 ----
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+      l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x == 0) stamp(7);
-  if (warp == T1_SM_WARPS + 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 256);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// The same tile pipeline as attn_vit_tc1_kernel with the CTA kept alive: 2 CTAs per SM walk over the
-// (frame, head, tile) work items. The per-CTA timeline of the one-shot kernel (tools/attn_trace.py) has
-// 1.2 us of set-up (TMEM allocation, barrier initialisation, descriptor prefetch), ~1.4 us of CTA relaunch
-// gap per slot and 2.1 us of TMA wait in front of 4.1 us of work; here the set-up is paid once per CTA
-// and the next tile's Q / K load is issued as soon as the P.V MMAs of the current tile have retired
-// (everything in shared memory is dead then except V, which the row-256 warp may still read: V follows
-// when the tile is finished), so it overlaps the epilogue. All barriers flip once per tile.
-// ---------------------------------------------------------------------------------------------
-template <bool FULL>
-__global__ void __launch_bounds__(T1_THREADS, 2)
-attn_vit_tc1p_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
-                     const bf16* __restrict__ qkv, bf16* __restrict__ out, int S, int H, int C, int n_tiles,
-                     unsigned long long* __restrict__ trace) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t pad = ((raw + 1023u) & ~1023u) - raw;
-  uint8_t* smem = smem_raw + pad;
-  const uint32_t sbase = raw + pad;
-  Small1* sm = reinterpret_cast<Small1*>(smem + T1_OFF_SMALL);
-  const uint32_t bar0 = sbase + T1_OFF_SMALL + (uint32_t)offsetof(Small1, bar);
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
-  // B_QK: Q and K of the tile have landed; B_V: V landed; B_S: scores in TMEM; B_ROW: row 256's q/k/v vectors
-  // are in smem; B_TAIL: s256 / tsc written; B_P: P in smem; B_O: O in TMEM; B_EPI: tile finished
-  enum { B_QK = 0, B_V = 1, B_S = 2, B_ROW = 3, B_TAIL = 4, B_P = 5, B_O = 6, B_EPI = 7 };
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int ld = 3 * C;
-  const bool key256 = S > 256;
-  if (warp == T1_SM_WARPS && lane == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_kv);
-    mbar_init(BAR(B_QK), 1); mbar_init(BAR(B_V), 1); mbar_init(BAR(B_S), 1);
-    mbar_init(BAR(B_ROW), 32);
-    mbar_init(BAR(B_TAIL), T1_SM_THREADS);
-    mbar_init(BAR(B_P), T1_SM_THREADS);
-    mbar_init(BAR(B_O), 1);
-    mbar_init(BAR(B_EPI), T1_SM_THREADS + 32);
-    mbar_fence_init();
-  }
-  if (warp == T1_SM_WARPS + 1) tmem_alloc(sbase + T1_OFF_SMALL + (uint32_t)offsetof(Small1, tmem_base), 256);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = sm->tmem_base;
-  constexpr float SCALE = 0.125f;
-  constexpr float LOG2E = 1.4426950408889634f;
-  auto p_off = [&](int kb) { return kb < 3 ? (uint32_t)(kb * 16384) : (uint32_t)T1_OFF_P3; };
-
-  if (warp == T1_SM_WARPS) {
-    // ================================ TMA + MMA issuer ================================
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16(128, 256);
-      constexpr uint32_t idesc_o = umma_idesc_bf16(128, 64) | (1u << 16);
-      auto load_qk = [&](int tile) {
-        const int t = tile & 1, h = (tile >> 1) % H, n = (tile >> 1) / H;
-        const int row0 = n * S;
-        mbar_arrive_expect_tx(BAR(B_QK), 128 * 128 + TILE_BYTES);
-        tma_load_2d(sbase + T1_OFF_Q, &tmap_q, BAR(B_QK), h * 64, row0 + t * 128);
-        tma_load_2d(sbase + T1_OFF_K, &tmap_kv, BAR(B_QK), C + h * 64, row0);
-      };
-      auto load_v = [&](int tile) {
-        const int h = (tile >> 1) % H, n = (tile >> 1) / H;
-        mbar_arrive_expect_tx(BAR(B_V), TILE_BYTES);
-        tma_load_2d(sbase + T1_OFF_V, &tmap_kv, BAR(B_V), 2 * C + h * 64, n * S);
-      };
-      int tile = blockIdx.x;
-      if (tile < n_tiles) { load_qk(tile); load_v(tile); }
-      for (int i = 0; tile < n_tiles; ++i, tile += gridDim.x) {
-        const uint32_t ph = (uint32_t)(i & 1);
-        mbar_wait_safe(BAR(B_QK), ph);
-        tc_fence_after();
-        const uint64_t kdesc = umma_desc_k_sw128(sbase + T1_OFF_K);
-        const uint64_t qdesc = umma_desc_k_sw128(sbase + T1_OFF_Q);
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          tc_mma_bf16(tmem, qdesc + 2u * k, kdesc + 2u * k, idesc_s, k != 0 ? 1u : 0u);
-        tc_commit(BAR(B_S));
-        mbar_wait_safe(BAR(B_P), ph);
-        mbar_wait_safe(BAR(B_V), ph);
-        tc_fence_after();
-        const uint64_t vdesc = umma_desc_mn_sw128(sbase + T1_OFF_V);
+    for (int hh = 0; hh < 2; ++hh) {
+      const int q = qt * 64 + r0 + 8 * hh;
+      if (q < S) {
+        const float inv = 1.0f / l[hh];
+        bf16* dst = out + (long long)(row0 + q) * C + h * 64 + c2;
 #pragma unroll
-        for (int kk = 0; kk < 16; ++kk) {
-          const uint64_t pdesc = umma_desc_k_sw128(sbase + p_off(kk >> 2)) + 2u * (kk & 3);
-          tc_mma_bf16(tmem, pdesc, vdesc + (uint64_t)((kk * 2048) >> 4), idesc_o, kk != 0 ? 1u : 0u);
-        }
-        tc_commit(BAR(B_O));
-        const int next = tile + gridDim.x;
-        mbar_wait_safe(BAR(B_O), ph);                         // P (over Q|K) and V have been read by the MMAs
-        if (next < n_tiles) load_qk(next);                    // overlaps the epilogue of this tile
-        mbar_wait_safe(BAR(B_EPI), ph);                       // TMEM read out; the row-256 warp is done with V
-        if (next < n_tiles) load_v(next);
+        for (int j = 0; j < 8; ++j)
+          *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_bf16x2(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
       }
     }
-  } else if (warp == T1_SM_WARPS + 1) {
-    // ================================ row 256 of the tiles with t == 1 ================================
-    int tile = blockIdx.x;
-    for (int i = 0; tile < n_tiles; ++i, tile += gridDim.x) {
-      const uint32_t ph = (uint32_t)(i & 1);
-      const int t = tile & 1, h = (tile >> 1) % H, n = (tile >> 1) / H;
-      const long long row0 = (long long)n * S;
-      const bool do_tail = key256 && t == 1;
-      const bf16* r = qkv + (row0 + 256) * ld + h * 64;
-      // the loads are in flight while the previous tile's readers of these vectors finish
-      uint32_t rq = 0, rk = 0, rv = 0;
-      if (key256) {
-        rq = *reinterpret_cast<const uint32_t*>(r + 2 * lane);
-        rk = *reinterpret_cast<const uint32_t*>(r + C + 2 * lane);
-        rv = *reinterpret_cast<const uint32_t*>(r + 2 * C + 2 * lane);
-      }
-      if (i > 0) mbar_wait_safe(BAR(B_EPI), ph ^ 1u);
-      sm->q256[2 * lane] = bf16lo(rq); sm->q256[2 * lane + 1] = bf16hi(rq);
-      sm->k256[2 * lane] = bf16lo(rk); sm->k256[2 * lane + 1] = bf16hi(rk);
-      sm->v256[2 * lane] = bf16lo(rv); sm->v256[2 * lane + 1] = bf16hi(rv);
-      mbar_arrive(BAR(B_ROW));
-      if (do_tail) {
-        mbar_wait_safe(BAR(B_TAIL), ph);
-        if (lane == 0) {
-          float d = 0.f;
-#pragma unroll
-          for (int c = 0; c < 64; ++c) d += sm->q256[c] * sm->k256[c];
-          sm->tsc[256] = bf16r(d) * SCALE;
-        }
-        __syncwarp();
-        float sc[9];
-        float mx = -INFINITY;
-#pragma unroll
-        for (int k = 0; k < 9; ++k) {
-          const int j = lane + 32 * k;
-          sc[k] = (j <= 256) ? sm->tsc[j] : -INFINITY;
-          mx = fmaxf(mx, sc[k]);
-        }
-        mx = warp_max(mx);
-        float sum = 0.f;
-        __syncwarp();
-#pragma unroll
-        for (int k = 0; k < 9; ++k) {
-          const int j = lane + 32 * k;
-          const float p = (j <= 256) ? ex2_approx((sc[k] - mx) * LOG2E) : 0.f;
-          sum += p;
-          if (j <= 256) sm->tsc[j] = bf16r(p);
-        }
-        sum = warp_sum(sum);
-        __syncwarp();
-        mbar_wait_safe(BAR(B_V), ph);
-        float o0 = 0.f, o1 = 0.f;
-        const int ch = lane >> 2, wi = (lane & 3) * 4;
-#pragma unroll 8
-        for (int j = 0; j < 256; ++j) {
-          const uint32_t v = *reinterpret_cast<const uint32_t*>(smem + T1_OFF_V + sw128(j, ch) + wi);
-          const float p = sm->tsc[j];
-          o0 += p * bf16lo(v);
-          o1 += p * bf16hi(v);
-        }
-        o0 += sm->tsc[256] * sm->v256[2 * lane];
-        o1 += sm->tsc[256] * sm->v256[2 * lane + 1];
-        const float inv = 1.0f / sum;
-        *reinterpret_cast<uint32_t*>(out + (row0 + 256) * C + h * 64 + 2 * lane) = pack_bf16x2(o0 * inv, o1 * inv);
-      }
-      mbar_arrive(BAR(B_EPI));
-    }
-  } else {
-    // ================================ softmax warps ================================
-    const int q4 = warp & 3, hf = warp >> 2;                  // TMEM lane quarter, column half
-    const int r = q4 * 32 + lane;
-    const int tix = threadIdx.x;                              // 0..255
-    int tile = blockIdx.x;
-    for (int i = 0; tile < n_tiles; ++i, tile += gridDim.x) {
-      const uint32_t ph = (uint32_t)(i & 1);
-      const int t = tile & 1, h = (tile >> 1) % H, n = (tile >> 1) / H;
-      const long long row0 = (long long)n * S;
-      const bool do_tail = key256 && t == 1;
-      // optional phase stamps of the first 12 tiles of every CTA (tools/attn_trace.py); null in production
-      auto stamp = [&](int ev) {
-        if (trace != nullptr && tix == 0 && i < 12) {
-          unsigned long long t_;
-          asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_));
-          trace[((size_t)blockIdx.x * 12 + i) * 8 + ev] = t_;
-        }
-      };
-      stamp(0);
-      mbar_wait_safe(BAR(B_QK), ph);
-      mbar_wait_safe(BAR(B_ROW), ph);
-      stamp(1);
-      if (key256) {
-        if (tix < 128) sm->s256[tix] = bf16r(dot64(smem + T1_OFF_Q, tix, sm->k256)) * SCALE;
-        if (do_tail) sm->tsc[tix] = bf16r(dot64(smem + T1_OFF_K, tix, sm->q256)) * SCALE;
-      } else if (tix < 128) {
-        sm->s256[tix] = -INFINITY;
-      }
-      mbar_arrive(BAR(B_TAIL));
-      const uint32_t taddr = tmem + ((uint32_t)(q4 * 32) << 16) + hf * 128;
-      const int n_valid = FULL ? 128 : max(0, min(128, S - hf * 128));
-      mbar_wait_safe(BAR(B_S), ph);
-      tc_fence_after();
-      stamp(2);
-      uint32_t st[64];
-      __nv_bfloat162 mx2 = __float2bfloat162_rn(-INFINITY);
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        uint32_t v[16];
-        __syncwarp();
-        tmem_ld_32x16(taddr + c * 16, v);
-        tc_wait_ld();
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float a = __uint_as_float(v[2 * j]), b = __uint_as_float(v[2 * j + 1]);
-          if (!FULL) {
-            if (c * 16 + 2 * j >= n_valid) a = -INFINITY;
-            if (c * 16 + 2 * j + 1 >= n_valid) b = -INFINITY;
-          }
-          const uint32_t s2 = pack_bf16x2(a, b);
-          st[c * 8 + j] = s2;
-          mx2 = __hmax2(mx2, *reinterpret_cast<const __nv_bfloat162*>(&s2));
-        }
-      }
-      sm->smax[hf][r] = fmaxf(__low2float(mx2), __high2float(mx2)) * SCALE;
-      named_bar_sync(1, T1_SM_THREADS);                       // also: all Q / K row reads are done
-      stamp(3);
-      const float m = fmaxf(fmaxf(sm->smax[0][r], sm->smax[1][r]), sm->s256[r]);
-      const float mb = m * LOG2E;
-      const float p256 = key256 ? ex2_approx(sm->s256[r] * LOG2E - mb) : 0.f;
-      float sum = 0.f;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t pk[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const uint32_t s2 = st[c * 16 + j];
-          const float p0 = ex2_approx(fmaf(bf16lo(s2), SCALE * LOG2E, -mb));
-          const float p1 = ex2_approx(fmaf(bf16hi(s2), SCALE * LOG2E, -mb));
-          sum += p0 + p1;
-          pk[j] = pack_bf16x2(p0, p1);
-        }
-        const int key0 = hf * 128 + c * 32;
-        const uint32_t pb = p_off(key0 >> 6);
-        const int ch0 = (key0 & 63) >> 3;
-#pragma unroll
-        for (int q = 0; q < 4; ++q)
-          *reinterpret_cast<uint4*>(smem + pb + sw128(r, ch0 + q)) =
-              make_uint4(pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-      }
-      sm->ssum[hf][r] = sum;
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      tc_fence_before();
-      mbar_arrive(BAR(B_P));
-      stamp(4);
-      mbar_wait_safe(BAR(B_O), ph);
-      tc_fence_after();
-      stamp(5);
-      uint32_t v[32];
-      __syncwarp();
-      tmem_ld_32x32(tmem + ((uint32_t)(q4 * 32) << 16) + hf * 32, v);
-      tc_wait_ld();
-      const int qr = t * 128 + r;
-      if (qr < S && qr < 256) {
-        const float total = sm->ssum[0][r] + sm->ssum[1][r] + p256;
-        const float inv = 1.0f / total;
-        const float pb = bf16r(p256);
-        uint32_t o[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float a = __uint_as_float(v[2 * j]) + pb * sm->v256[hf * 32 + 2 * j];
-          const float b = __uint_as_float(v[2 * j + 1]) + pb * sm->v256[hf * 32 + 2 * j + 1];
-          o[j] = pack_bf16x2(a * inv, b * inv);
-        }
-        bf16* dst = out + (row0 + qr) * C + h * 64 + hf * 32;
-#pragma unroll
-        for (int q = 0; q < 4; ++q)
-          *reinterpret_cast<uint4*>(dst + q * 8) = make_uint4(o[4 * q], o[4 * q + 1], o[4 * q + 2], o[4 * q + 3]);
-      }
-      tc_fence_before();
-      mbar_arrive(BAR(B_EPI));
-      stamp(6);
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == T1_SM_WARPS + 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 256);
   }
 }
 
 }  // namespace
 
-extern "C" void vcl_debug_set_attn_trace(void* dev_buffer) {
-  g_attn_trace = reinterpret_cast<unsigned long long*>(dev_buffer);
-}
-
 int init_attention_tc_kernels() {
-  VCL_CUDA_OK(cudaFuncSetAttribute(attn_vit_tc1_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T1_SMEM));
-  VCL_CUDA_OK(cudaFuncSetAttribute(attn_vit_tc1_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T1_SMEM));
-  VCL_CUDA_OK(cudaFuncSetAttribute(attn_vit_tc1p_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T1_SMEM));
-  VCL_CUDA_OK(cudaFuncSetAttribute(attn_vit_tc1p_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T1_SMEM));
+  VCL_CUDA_OK(cudaFuncSetAttribute(attn_vit_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, VA_SMEM));
   return 0;
 }
 
+bool attention_vit_tc_supported(int S) {
+  const bool off = getenv("VCL_VIT_ATTN_FLASH") != nullptr;   // A/B: the mma.sync kernel (read per call, so that
+                                                              // a test can compare the two in one process)
+  return !off && S >= 129 && S <= 257;
+}
+
 // qkv: [n_frames * S, 3*C] (q | k | v, heads of 64 contiguous), out: [n_frames * S, C]
-int launch_attention_vit_tc(const bf16* qkv, bf16* out, int n_frames, int S, int H, int C,
-                            cudaStream_t stream) {
-  VCL_REQUIRE(C == H * 64, "attention_tc: head_dim must be 64");
-  VCL_REQUIRE(S >= 129 && S <= 257, "attention_tc: S=%d outside 129..257 (other sizes use the mma.sync kernel)", S);
-  CUtensorMap tm, tq;
-  if (make_tmap_2d(&tm, qkv, (long long)n_frames * S, 3LL * C, 3LL * C, 256) != 0) return -2;
-  if (make_tmap_2d(&tq, qkv, (long long)n_frames * S, 3LL * C, 3LL * C, 128) != 0) return -2;
-  static const bool one_shot = getenv("VCL_ATTN_ONE_SHOT") != nullptr;   // A/B: one CTA per tile instead of persistent CTAs
-  const int n_tiles = n_frames * H * 2;
-  const int grid = n_tiles < 2 * device_num_sms() ? n_tiles : 2 * device_num_sms();
-  if (one_shot) {
-    if (S >= 256) attn_vit_tc1_kernel<true><<<n_tiles, T1_THREADS, T1_SMEM, stream>>>(tq, tm, qkv, out, S, H, C, g_attn_trace);
-    else attn_vit_tc1_kernel<false><<<n_tiles, T1_THREADS, T1_SMEM, stream>>>(tq, tm, qkv, out, S, H, C, g_attn_trace);
-  } else if (S >= 256) {
-    attn_vit_tc1p_kernel<true><<<grid, T1_THREADS, T1_SMEM, stream>>>(tq, tm, qkv, out, S, H, C, n_tiles, g_attn_trace);
-  } else {
-    attn_vit_tc1p_kernel<false><<<grid, T1_THREADS, T1_SMEM, stream>>>(tq, tm, qkv, out, S, H, C, n_tiles, g_attn_trace);
-  }
+int launch_attention_vit_tc(const bf16* qkv, bf16* out, int n_frames, int S, int H, int C, cudaStream_t stream) {
+  VCL_REQUIRE(C == H * 64, "attention_vit_tc: head_dim must be 64");
+  VCL_REQUIRE(S >= 129 && S <= 257, "attention_vit_tc: S=%d outside 129..257", S);
+  VCL_REQUIRE(((uintptr_t)qkv % 16) == 0 && ((uintptr_t)out % 16) == 0, "attention_vit_tc: pointers must be 16-byte aligned");
+  CUtensorMap tm;
+  if (make_tmap_2d(&tm, qkv, (long long)n_frames * S, 3LL * C, 3LL * C, 64) != 0) return -2;
+  attn_vit_tc_kernel<<<n_frames * H, VA_THREADS, VA_SMEM, stream>>>(tm, qkv, out, S, H, C);
   VCL_CUDA_OK(cudaGetLastError());
   count_launches(1);
   return 0;

@@ -2,7 +2,7 @@
 //
 // One query row per (clip, head) against kv_len cached keys: 2 * kv_len * 256 B of K/V per head
 // (7.5 MB per layer for 32 heads at kv_len ~ 460) and almost no math -- HBM/L2-latency bound. A
-// single CTA per head leaves 116 of 148 SMs idle and serialises three dependent phases, so each
+// single CTA per head leaves 100 of 132 SMs idle and serialises three dependent phases, so each
 // head is given a CLUSTER of 4 CTAs: every CTA owns a quarter of the keys, and the softmax
 // statistics and the partial outputs are exchanged through distributed shared memory:
 //
@@ -191,7 +191,6 @@ int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, c
   // CTAs per head: enough CTAs to cover the SMs a few times over, no more
   static const int forced = getenv("VCL_DA_SPLIT") ? atoi(getenv("VCL_DA_SPLIT")) : 0;      // A/B switch: 1, 2 or 4
   const int heads = B * H;
-  // measured at 16 clips x 32 heads (config 3, decode loop of 31 steps): 4 CTAs per head 143 ms, 2: 133 ms, 1: 130 ms
   int split = heads <= 2 * device_num_sms() ? 4 : (heads <= 3 * device_num_sms() ? 2 : 1);
   if (forced == 1 || forced == 2 || forced == 4) split = forced;
   const int per = ((kv_cap + split - 1) / split + 15) / 16 * 16;   // keys per CTA, multiple of 16

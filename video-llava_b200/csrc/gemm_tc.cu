@@ -1,20 +1,20 @@
-// Dense bf16 GEMM on the 5th-generation tensor cores:  C[M,N] = epilogue(A[M,K] . W[N,K]^T)
+// Dense bf16 GEMM on the Hopper warpgroup tensor cores:  C[M,N] = epilogue(A[M,K] . W[N,K]^T)
 //
 // This one kernel serves every dense contraction on the hot path (SURVEY.md section 2.3 rows
 // V1, V3, V5-V7, J1, L1, L4-L6): both operands are K-major exactly as nn.Linear stores them
 // (activations [rows, K], weights [out, in]), so no transposes are ever materialised.
 //
-//   warp 0      TMA producer : cp.async.bulk.tensor 2-D tiles (128B swizzle) -> smem ring
-//   warp 1      MMA issuer   : one thread issues tcgen05.mma (M=128, N=BLOCK_N, K=16) x4 per stage
-//   warp 2      TMEM allocator (2 accumulator buffers of BLOCK_N fp32 columns)
-//   warps 4-11  epilogue     : tcgen05.ld 32 lanes x 32 columns -> bias / activation / residual
-//                              -> bf16 -> a 2 KB per-warp staging block in shared memory (a thread owns
-//                              64 contiguous bytes of ONE row; the block is read back transposed so that
-//                              a store instruction writes 8 rows x 64 contiguous bytes) -> global; two
-//                              warps per TMEM lane quarter, software-pipelined over the column chunks
+//   warpgroup 0     TMA producer : one thread issues cp.async.bulk.tensor 2-D tiles (128B swizzle) into a
+//                                  smem ring; the warpgroup hands most of its registers to the consumers
+//   warpgroups 1-2  consumers    : 64 rows each of the 128 x BLOCK_N tile, wgmma.mma_async m64nBLOCK_Nk16
+//                                  with fp32 accumulators in registers; the stage is released once the
+//                                  wgmma that read it has retired (one group kept in flight)
+//   epilogue (consumers)         : accumulators -> bias / activation / RoPE -> bf16 into a padded staging
+//                                  block in shared memory, then read back as 16-byte row chunks (+ residual)
+//                                  and stored with whole contiguous row segments per instruction
 //
-// Persistent: grid = min(#tiles, #SMs); the accumulator is double-buffered in TMEM so the
-// epilogue of tile i overlaps the mainloop of tile i+1.
+// Persistent: grid = the number of CTAs (clusters) that fit at once, capped by the tile count; the producer
+// runs ahead into the next tile while the consumers drain the current one.
 //
 // Rounding points reproduce the reference's eager bf16 path (each nn.Linear output is rounded to
 // bf16 before the following elementwise op):
@@ -36,310 +36,156 @@ template <int BLOCK_N>
 struct GemmCfg {
   static constexpr int BLOCK_M = 128;
   static constexpr int BLOCK_K = 64;  // 64 bf16 = one 128-byte swizzle span
-  static constexpr int STAGES = (BLOCK_N == 256) ? 4 : (BLOCK_N == 128 ? 6 : 8);
   static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
   static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int OUT_PITCH = BLOCK_N * 2 + 16;     // bytes per staged output row (+16: no bank conflicts)
+  static constexpr int OUT_BYTES = BLOCK_M * OUT_PITCH;
   static constexpr int BAR_BYTES = 256;
-  static constexpr int OUT_STAGE_BYTES = 8 * 2048;   // per epilogue warp: a 32 x 32 bf16 block on its way to global memory
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + OUT_STAGE_BYTES + 1024;  // +1024: manual align
-  static constexpr int TMEM_COLS = 2 * BLOCK_N;
-  static_assert(TMEM_COLS >= 32 && TMEM_COLS <= 512 && (TMEM_COLS & (TMEM_COLS - 1)) == 0, "tmem");
-  static_assert((2 * STAGES + 4) * 8 + 8 <= BAR_BYTES, "barrier area");
+  // as many ring stages as fit next to the staging block in the 227 KB a CTA may use
+  static constexpr int STAGES = (BLOCK_N == 256) ? 3 : (BLOCK_N == 128 ? 5 : 8);
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + OUT_BYTES + 1024;  // +1024: manual align
+  static_assert(2 * STAGES * 8 <= BAR_BYTES, "barrier area");
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory");
 };
 
-__device__ __forceinline__ float act_quick_gelu(float x) {
-  // three bf16 tensors are materialised by the reference: 1.702*x, sigmoid(.), x*sigmoid(.)
-  x = bf16r(x);
-  float t = bf16r(1.702f * x);
-  float s = bf16r(1.0f / (1.0f + __expf(-t)));
-  return x * s;
-}
 __device__ __forceinline__ float act_gelu_erf(float x) {
   x = bf16r(x);
   return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f));
 }
-__device__ __forceinline__ float act_silu(float g) {
-  g = bf16r(g);
-  return bf16r(g / (1.0f + __expf(-g)));
+
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
-// ACT_ROPE epilogue (kernels.h: RopeEpilogue). A 128-column block of the q|k|v output is one head; the RoPE
-// partner of column d is d + 64, which sits 64 TMEM columns further in the same lane, so a thread reads BOTH
-// 32-column chunks of its pairs and the rotation is thread-local: with 128-wide tiles the two warps of a lane
-// quarter split the head's 64 pairs (d in [32 hf, 32 hf + 32)), with 256-wide tiles each takes one head.
-// Arithmetic = rope_kv_prefill_kernel (elementwise.cu): x rounded to bf16, every product rounded, fp32 sum, one
-// final rounding (transformers/models/llama/modeling_llama.py:124-168).
-template <int BLOCK_N, class WaitFn, class ArriveFn>
-__device__ __forceinline__ void gemm_epilogue_rope(uint32_t tmem_acc, int q4, int hf, int lane, int m_blk, int n_blk,
-                                                   bf16* C, long long ldc, int M, const RopeEpilogue& rp,
-                                                   uint8_t* stg, WaitFn wait_full, ArriveFn arrive_empty) {
-  if constexpr (BLOCK_N == 128 || BLOCK_N == 256) {
-    constexpr int UNITS = BLOCK_N / 128;
-    const int row = m_blk * 128 + q4 * 32 + lane;
-    const bool row_ok = row < M;
-    const int b = row / rp.S, s = row - b * rp.S;
-    const int pos = rp.start_pos + s;
-    wait_full();
-    const uint32_t tl = tmem_acc + ((uint32_t)(q4 * 32) << 16);
+// Epilogue, phase 1: this warpgroup's 64 x BLOCK_N accumulators -> bf16 outputs in the staging block
+// (stg = its first row). Each thread holds column pairs (2c, 2c+1) of two rows (accumulator layout in common.cuh).
+//   ACT_SWIGLU: weight rows are interleaved (2j = gate_j, 2j+1 = up_j), so a pair is one output column j.
+//   ACT_ROPE  : a 128-column block is one head of q | k | v; the RoPE partner of column d is d + 64, which the
+//               same thread holds 8 accumulator groups further on, so the rotation is thread-local. Arithmetic =
+//               rope_kv_prefill_kernel (elementwise.cu): x rounded to bf16, every product rounded, fp32 sum, one
+//               final rounding (transformers/models/llama/modeling_llama.py:124-168).
+template <int BLOCK_N, int ACT>
+__device__ __forceinline__ void gemm_epilogue_stage(const float (&acc)[BLOCK_N / 2], uint8_t* stg, int lane, int wq,
+                                                    int row_base, int n_blk, const bf16* __restrict__ bias, int M,
+                                                    int N, const RopeEpilogue& rp) {
+  using Cfg = GemmCfg<BLOCK_N>;
+  const int r0 = 16 * wq + (lane >> 2);
+  const int c2 = 2 * (lane & 3);
+  if constexpr (ACT == ACT_ROPE) {
+    static_assert(BLOCK_N % 128 == 0, "one head (128 columns) per tile at least");
 #pragma unroll
-    for (int u = 0; u < UNITS; ++u) {
-      const int hh = BLOCK_N == 128 ? 0 : hf;                 // head inside the tile
-      const int d0 = 32 * (BLOCK_N == 128 ? hf : u);          // first pair of this unit
-      uint32_t lo[32], hi[32];
-      __syncwarp();
-      tmem_ld_32x32(tl + hh * 128 + d0, lo);
-      tmem_ld_32x32(tl + hh * 128 + 64 + d0, hi);
-      tc_wait_ld();
-      if (u == UNITS - 1) arrive_empty();                     // every TMEM read of this accumulator has completed
-      const int gh = n_blk * UNITS + hh;                      // head index over q | k | v (the same for the warp)
-      const int which = gh / rp.H, head = gh - which * rp.H;
-      uint32_t olo[16], ohi[16];
-      if (row_ok && which == 2) {
+    for (int hh = 0; hh < BLOCK_N / 128; ++hh) {
+      const int gh = n_blk * (BLOCK_N / 128) + hh;               // head index over q | k | v
+      const int which = gh / rp.H;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          olo[j] = pack_bf16x2(__uint_as_float(lo[2 * j]), __uint_as_float(lo[2 * j + 1]));
-          ohi[j] = pack_bf16x2(__uint_as_float(hi[2 * j]), __uint_as_float(hi[2 * j + 1]));
-        }
-      } else if (row_ok) {
-        const bf16* ct = rp.cos_t + (long long)pos * 64 + d0;
-        const bf16* st = rp.sin_t + (long long)pos * 64 + d0;
+      for (int h = 0; h < 2; ++h) {
+        const int r = r0 + 8 * h;
+        const int grow = row_base + r;
+        const int pos = rp.start_pos + (grow < M ? grow % rp.S : 0);
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const uint4 c4 = __ldg(reinterpret_cast<const uint4*>(ct + q * 8));
-          const uint4 s4 = __ldg(reinterpret_cast<const uint4*>(st + q * 8));
-          const uint32_t cw[4] = {c4.x, c4.y, c4.z, c4.w}, sw[4] = {s4.x, s4.y, s4.z, s4.w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int j = q * 4 + e;                        // pair of columns 2j, 2j + 1
-            const uint32_t l2 = pack_bf16x2(__uint_as_float(lo[2 * j]), __uint_as_float(lo[2 * j + 1]));
-            const uint32_t h2 = pack_bf16x2(__uint_as_float(hi[2 * j]), __uint_as_float(hi[2 * j + 1]));
+        for (int jj = 0; jj < 8; ++jj) {
+          const int j = hh * 16 + jj, d = 8 * jj + c2;
+          const uint32_t l2 = pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+          const uint32_t h2 = pack_bf16x2(acc[4 * (j + 8) + 2 * h], acc[4 * (j + 8) + 2 * h + 1]);
+          uint32_t olo = l2, ohi = h2;
+          if (which != 2 && grow < M) {
+            const uint32_t cw = __ldg(reinterpret_cast<const uint32_t*>(rp.cos_t + (long long)pos * 64 + d));
+            const uint32_t sw = __ldg(reinterpret_cast<const uint32_t*>(rp.sin_t + (long long)pos * 64 + d));
             const float l0 = bf16lo(l2), l1 = bf16hi(l2), h0 = bf16lo(h2), h1 = bf16hi(h2);
-            const float c0 = bf16lo(cw[e]), c1 = bf16hi(cw[e]), s0 = bf16lo(sw[e]), s1 = bf16hi(sw[e]);
-            olo[j] = pack_bf16x2(bf16r(l0 * c0) + bf16r(-h0 * s0), bf16r(l1 * c1) + bf16r(-h1 * s1));
-            ohi[j] = pack_bf16x2(bf16r(h0 * c0) + bf16r(l0 * s0), bf16r(h1 * c1) + bf16r(l1 * s1));
+            const float c0 = bf16lo(cw), c1 = bf16hi(cw), s0 = bf16lo(sw), s1 = bf16hi(sw);
+            olo = pack_bf16x2(bf16r(l0 * c0) + bf16r(-h0 * s0), bf16r(l1 * c1) + bf16r(-h1 * s1));
+            ohi = pack_bf16x2(bf16r(h0 * c0) + bf16r(l0 * s0), bf16r(h1 * c1) + bf16r(l1 * s1));
           }
+          *reinterpret_cast<uint32_t*>(stg + r * Cfg::OUT_PITCH + (hh * 128 + d) * 2) = olo;
+          *reinterpret_cast<uint32_t*>(stg + r * Cfg::OUT_PITCH + (hh * 128 + 64 + d) * 2) = ohi;
         }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) { olo[j] = 0u; ohi[j] = 0u; }
-      }
-      // both 64-byte halves of the row leave through the warp's staging block (gemm_epilogue_tile): 8 rows x 64
-      // contiguous bytes per store instruction; the destination row is recomputed for the row a lane stores
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        const int swz = (lane >> 1) & 3;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const uint32_t* src = half == 0 ? olo : ohi;
-          *reinterpret_cast<uint4*>(stg + lane * 64 + ((q ^ swz) << 4)) =
-              make_uint4(src[4 * q], src[4 * q + 1], src[4 * q + 2], src[4 * q + 3]);
-        }
-        __syncwarp();
-        const int r0 = lane >> 2, cc = lane & 3;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int r = 8 * k + r0;
-          const uint4 val = *reinterpret_cast<const uint4*>(stg + r * 64 + ((cc ^ ((r >> 1) & 3)) << 4));
-          const int grow = m_blk * 128 + q4 * 32 + r;
-          if (grow < M) {
-            const int gb = grow / rp.S, gs = grow - gb * rp.S;
-            bf16* dst = which == 0
-                ? C + (long long)grow * ldc + gh * 128 + d0
-                : (which == 1 ? rp.kcache : rp.vcache) + (((long long)gb * rp.H + head) * rp.s_max + rp.start_pos + gs) * 128 + d0;
-            *reinterpret_cast<uint4*>(dst + half * 64 + cc * 8) = val;
-          }
-        }
-        __syncwarp();
       }
     }
   } else {
-    wait_full();               // narrower tiles are never launched with ACT_ROPE (launch_gemm_bf16_tn)
-    arrive_empty();
-  }
-}
-
-// One output tile of the epilogue, for the 32 rows x (BLOCK_N / 2) columns this warp owns: TMEM -> bias /
-// activation / residual -> bf16 -> global. warp w reads TMEM lanes 32*(w%4).. (hardware restriction) and
-// owns one half (hf) of the tile's 32-column chunks; the tcgen05.ld and the residual loads of chunk i+1
-// are issued before the math of chunk i so their latency hides behind it. wait_full() blocks until the
-// accumulator is complete, arrive_empty() hands it back to the MMA issuer once it has been read out.
-template <int BLOCK_N, int ACT, class WaitFn, class ArriveFn>
-__device__ __forceinline__ void gemm_epilogue_tile(uint32_t tmem_acc, int q4, int hf, int lane, int m_blk, int n_blk,
-                                                   bf16* C, long long ldc, const bf16* __restrict__ bias,
-                                                   const bf16* residual, long long ldr, int M, int N,
-                                                   const RopeEpilogue& rope, uint8_t* stg, WaitFn wait_full,
-                                                   ArriveFn arrive_empty) {
-  if constexpr (ACT == ACT_ROPE) {
-    gemm_epilogue_rope<BLOCK_N>(tmem_acc, q4, hf, lane, m_blk, n_blk, C, ldc, M, rope, stg, wait_full, arrive_empty);
-    return;
-  }
-  constexpr int CH = BLOCK_N / 32;
-  constexpr int PER = (CH + 1) / 2;
-  const int c_begin = hf * PER;
-  const int n_mine = (c_begin + PER <= CH) ? PER : (CH > c_begin ? CH - c_begin : 0);
-  const int row = m_blk * 128 + q4 * 32 + lane;
-  const bool row_ok = row < M;
-  const int colbase = n_blk * BLOCK_N + c_begin * 32;
-  const bf16* rrow = residual + (long long)row * ldr + colbase;
-  const bool has_res = (residual != nullptr) && row_ok;
-  uint32_t v[2][32];
-  uint4 rr[2][4];
-  if (has_res && n_mine > 0 && colbase < N) {
 #pragma unroll
-    for (int q = 0; q < 4; ++q) rr[0][q] = *reinterpret_cast<const uint4*>(rrow + q * 8);
-  }
-  wait_full();
-  const uint32_t taddr = tmem_acc + ((uint32_t)(q4 * 32) << 16) + c_begin * 32;
-  __syncwarp();
-  if (n_mine > 0) {
-    tmem_ld_32x32(taddr, v[0]);
-    tc_wait_ld();
-  }
-  if (n_mine <= 1) {
-    arrive_empty();
-  }
-#pragma unroll
-  for (int i = 0; i < PER; ++i) {
-    if (i < n_mine) {
-      const int cur = i & 1, nxt = cur ^ 1;
-      const int col0 = colbase + i * 32;
-      if (i + 1 < n_mine) {
-        if (has_res && col0 + 32 < N) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q)
-            rr[nxt][q] = *reinterpret_cast<const uint4*>(rrow + (i + 1) * 32 + q * 8);
-        }
-        __syncwarp();
-        tmem_ld_32x32(taddr + (i + 1) * 32, v[nxt]);
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+      const int col = 8 * j + c2;
+      const int gcol = n_blk * BLOCK_N + col;
+      float b0 = 0.f, b1 = 0.f;
+      if (bias != nullptr && gcol < N) {
+        const uint32_t bw = __ldg(reinterpret_cast<const uint32_t*>(bias + gcol));
+        b0 = bf16lo(bw); b1 = bf16hi(bw);
       }
-      auto load_f = [&](float (&f)[32]) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[cur][j]);
-        if (bias != nullptr) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const uint4 b = *reinterpret_cast<const uint4*>(bias + col0 + q * 8);
-            f[q * 8 + 0] += bf16lo(b.x); f[q * 8 + 1] += bf16hi(b.x);
-            f[q * 8 + 2] += bf16lo(b.y); f[q * 8 + 3] += bf16hi(b.y);
-            f[q * 8 + 4] += bf16lo(b.z); f[q * 8 + 5] += bf16hi(b.z);
-            f[q * 8 + 6] += bf16lo(b.w); f[q * 8 + 7] += bf16hi(b.w);
-          }
-        }
-      };
-      if constexpr (ACT == ACT_SWIGLU) {
-        if (col0 < N) {                            // warp-uniform
-          // weight rows are interleaved (2j = gate_j, 2j+1 = up_j): 32 columns -> 16 outputs (32 bytes per row)
-          uint32_t o[8];
-          if (row_ok) {
-            float f[32];
-            load_f(f);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const uint32_t g2 = pack_bf16x2(f[4 * j + 0], f[4 * j + 2]);   // gate pair (bf16)
-              const uint32_t u2 = pack_bf16x2(f[4 * j + 1], f[4 * j + 3]);   // up pair (bf16)
-              const float g0 = bf16lo(g2), g1 = bf16hi(g2);
-              const uint32_t s2 = pack_bf16x2(__fdividef(g0, 1.0f + __expf(-g0)),
-                                              __fdividef(g1, 1.0f + __expf(-g1)));   // silu (bf16)
-              o[j] = bf16x2_mul(s2, u2);
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) o[j] = 0u;
-          }
-          // staged like the plain path below: 16 rows x 32 contiguous bytes (one sector each) per instruction
-          const int sw = (lane >> 2) & 1;
-          *reinterpret_cast<uint4*>(stg + lane * 32 + ((0 ^ sw) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
-          *reinterpret_cast<uint4*>(stg + lane * 32 + ((1 ^ sw) << 4)) = make_uint4(o[4], o[5], o[6], o[7]);
-          __syncwarp();
-          const int r0 = lane >> 1, cc = lane & 1;
-#pragma unroll
-          for (int k = 0; k < 2; ++k) {
-            const int r = 16 * k + r0;
-            const uint4 val = *reinterpret_cast<const uint4*>(stg + r * 32 + ((cc ^ ((r >> 2) & 1)) << 4));
-            const int grow = m_blk * 128 + q4 * 32 + r;
-            if (grow < M) *reinterpret_cast<uint4*>(C + (long long)grow * ldc + (col0 >> 1) + cc * 8) = val;
-          }
-          __syncwarp();
-        }
-      } else if (col0 < N) {                       // warp-uniform: every lane takes part in the staged store
-        uint32_t o[16];
-        if (row_ok) {
-          float f[32];
-          load_f(f);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if constexpr (ACT == ACT_QGELU) {
-              // x*sigmoid(1.702x): the three bf16 tensors of the reference are materialised
-              const uint32_t x2 = pack_bf16x2(f[2 * j], f[2 * j + 1]);
-              const uint32_t t2 = pack_bf16x2(1.702f * bf16lo(x2), 1.702f * bf16hi(x2));
-              const uint32_t s2 = pack_bf16x2(__fdividef(1.0f, 1.0f + __expf(-bf16lo(t2))),
-                                              __fdividef(1.0f, 1.0f + __expf(-bf16hi(t2))));
-              o[j] = bf16x2_mul(x2, s2);
-            } else if constexpr (ACT == ACT_GELU) {
-              o[j] = pack_bf16x2(act_gelu_erf(f[2 * j]), act_gelu_erf(f[2 * j + 1]));
-            } else {
-              o[j] = pack_bf16x2(f[2 * j], f[2 * j + 1]);
-            }
-          }
-          if (has_res) {
-            // bf16(linear output) + residual, one more bf16 rounding (packed bf16x2 add)
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              o[q * 4 + 0] = bf16x2_add(o[q * 4 + 0], rr[cur][q].x);
-              o[q * 4 + 1] = bf16x2_add(o[q * 4 + 1], rr[cur][q].y);
-              o[q * 4 + 2] = bf16x2_add(o[q * 4 + 2], rr[cur][q].z);
-              o[q * 4 + 3] = bf16x2_add(o[q * 4 + 3], rr[cur][q].w);
-            }
-          }
+      for (int h = 0; h < 2; ++h) {
+        const int r = r0 + 8 * h;
+        const float x0 = acc[4 * j + 2 * h] + b0, x1 = acc[4 * j + 2 * h + 1] + b1;
+        if constexpr (ACT == ACT_SWIGLU) {
+          const float g = bf16r(x0);
+          const bf16 s = __float2bfloat16_rn(__fdividef(g, 1.0f + __expf(-g)));       // silu (bf16)
+          const bf16 o = __hmul(s, __float2bfloat16_rn(x1));                           // * up (bf16)
+          *reinterpret_cast<bf16*>(stg + r * Cfg::OUT_PITCH + col) = o;                // output column col / 2
         } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) o[j] = 0u;
-        }
-        // A thread holds 64 contiguous bytes of ONE row: storing them directly makes every store instruction
-        // touch 32 rows with 16 bytes each (half sectors; the stores of a 128 x 256 tile cost ~20 % of the ViT
-        // GEMMs: 130 -> 102 us without them). The 32 x 32 block goes through this warp's 2 KB of shared memory
-        // (XOR-swizzled, conflict-free both ways) and leaves as 8 rows x 64 contiguous bytes per instruction.
-        {
-          const int sw = (lane >> 1) & 3;
-#pragma unroll
-          for (int q = 0; q < 4; ++q)
-            *reinterpret_cast<uint4*>(stg + lane * 64 + ((q ^ sw) << 4)) =
-                make_uint4(o[q * 4 + 0], o[q * 4 + 1], o[q * 4 + 2], o[q * 4 + 3]);
-          __syncwarp();
-          const int r0 = lane >> 2, cc = lane & 3;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int r = 8 * k + r0;
-            const uint4 val = *reinterpret_cast<const uint4*>(stg + r * 64 + ((cc ^ ((r >> 1) & 3)) << 4));
-            const int grow = m_blk * 128 + q4 * 32 + r;
-            if (grow < M) *reinterpret_cast<uint4*>(C + (long long)grow * ldc + col0 + cc * 8) = val;
+          uint32_t o;
+          if constexpr (ACT == ACT_QGELU) {
+            // x*sigmoid(1.702x): the three bf16 tensors of the reference are materialised
+            const uint32_t x2 = pack_bf16x2(x0, x1);
+            const uint32_t t2 = pack_bf16x2(1.702f * bf16lo(x2), 1.702f * bf16hi(x2));
+            const uint32_t s2 = pack_bf16x2(__fdividef(1.0f, 1.0f + __expf(-bf16lo(t2))),
+                                            __fdividef(1.0f, 1.0f + __expf(-bf16hi(t2))));
+            o = bf16x2_mul(x2, s2);
+          } else if constexpr (ACT == ACT_GELU) {
+            o = pack_bf16x2(act_gelu_erf(x0), act_gelu_erf(x1));
+          } else {
+            o = pack_bf16x2(x0, x1);
           }
-          __syncwarp();
-        }
-      }
-      if (i + 1 < n_mine) {
-        __syncwarp();
-        tc_wait_ld();
-        if (i + 2 >= n_mine) {
-          // every TMEM read of this accumulator has completed: hand it back to the MMA warp
-          arrive_empty();
+          *reinterpret_cast<uint32_t*>(stg + r * Cfg::OUT_PITCH + col * 2) = o;
         }
       }
     }
+  }
+}
+
+// Epilogue, phase 2: the staged 64-row block leaves as 16-byte chunks, consecutive threads on consecutive chunks
+// of a row (whole contiguous row segments per store instruction); the residual is added here, one more bf16
+// rounding (packed bf16x2 add). ACT_ROPE: q goes to C, k and v straight into the KV cache.
+template <int BLOCK_N, int ACT>
+__device__ __forceinline__ void gemm_epilogue_store(const uint8_t* stg, int t, int row_base, int n_blk, bf16* C,
+                                                    long long ldc, const bf16* residual, long long ldr, int M, int N,
+                                                    const RopeEpilogue& rp) {
+  using Cfg = GemmCfg<BLOCK_N>;
+  constexpr int OUT_W = ACT == ACT_SWIGLU ? BLOCK_N / 2 : BLOCK_N;
+  constexpr int CPR = OUT_W / 8;                      // 16-byte chunks per row
+  const int n_out = ACT == ACT_SWIGLU ? N / 2 : N;
+#pragma unroll 4
+  for (int idx = t; idx < 64 * CPR; idx += 128) {
+    const int r = idx / CPR, c = idx - r * CPR;
+    const int grow = row_base + r, col = n_blk * OUT_W + c * 8;
+    if (grow >= M || col >= n_out) continue;
+    uint4 val = *reinterpret_cast<const uint4*>(stg + r * Cfg::OUT_PITCH + c * 16);
+    bf16* dst = C + (long long)grow * ldc + col;
+    if constexpr (ACT == ACT_ROPE) {
+      const int gh = col >> 7, d = col & 127;
+      const int which = gh / rp.H, head = gh - which * rp.H;
+      if (which != 0) {
+        const int gb = grow / rp.S, gs = grow - gb * rp.S;
+        dst = (which == 1 ? rp.kcache : rp.vcache) + (((long long)gb * rp.H + head) * rp.s_max + rp.start_pos + gs) * 128 + d;
+      }
+    } else if (residual != nullptr) {
+      const uint4 rr = *reinterpret_cast<const uint4*>(residual + (long long)grow * ldr + col);
+      val.x = bf16x2_add(val.x, rr.x); val.y = bf16x2_add(val.y, rr.y);
+      val.z = bf16x2_add(val.z, rr.z); val.w = bf16x2_add(val.w, rr.w);
+    }
+    *reinterpret_cast<uint4*>(dst) = val;
   }
 }
 
 // CL = thread-block-cluster size along M (1, 2 or 4). The CL CTAs of a cluster work on CL
 // consecutive M tiles of the SAME N tile: every CTA fetches 1/CL of the weight tile and TMA-multicasts
 // it into all CL shared memories, so a weight byte crosses L2->SM once per cluster instead of once
-// per CTA (the 128x256 tile is L2-bandwidth-limited otherwise, above all for the short-M prefill).
+// per CTA. A ring slot is refilled only once the consumers of EVERY CTA of the cluster have released it.
 template <int BLOCK_N, int ACT, int CL>
 __global__ void __launch_bounds__(384, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
                     const __grid_constant__ CUtensorMap tmap_b, bf16* C, long long ldc,
                     const bf16* __restrict__ bias, const bf16* residual, long long ldr, int M,
-                    int N, int K, int pf_ahead, const RopeEpilogue rope) {
+                    int N, int K, const RopeEpilogue rope) {
   using Cfg = GemmCfg<BLOCK_N>;
   constexpr int STAGES = Cfg::STAGES;
 
@@ -352,37 +198,21 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
   const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };
-  volatile uint32_t* tmem_ptr_smem =
-      reinterpret_cast<volatile uint32_t*>(smem + STAGES * Cfg::STAGE_BYTES + 8 * (2 * STAGES + 4));
+  uint8_t* stage_out = smem + STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), CL);      // one tcgen05.commit arrival from every CTA of the cluster
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), 256);
+      mbar_init(empty_bar(s), 2 * CL);   // one arrival per consumer warpgroup of every CTA of the cluster
     }
     mbar_fence_init();
   }
-  if (warp == 2) {
-    tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_ptr_smem)), Cfg::TMEM_COLS);
-  }
-  tc_fence_before();
   __syncthreads();
   if (CL > 1) cluster_sync_all();      // peers' barriers are initialised before anyone signals them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   const int num_m = (M + Cfg::BLOCK_M - 1) / Cfg::BLOCK_M;
   const int num_n = (N + BLOCK_N - 1) / BLOCK_N;
@@ -394,34 +224,21 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
   constexpr uint16_t MC_MASK = (uint16_t)((1u << CL) - 1u);
   constexpr int B_SLICE_ROWS = BLOCK_N / CL;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ------------------------------ TMA producer ------------------------------
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      // L2 look-ahead for the weight operand: with few row tiles (prefill, M = 448) the weights come from
-      // HBM and the ring alone holds few of this CTA's own weight bytes in flight (4 stages x an 8 KB multicast
-      // slice). A prefetch cursor runs pf_ahead k-blocks in front of the loads, across tile boundaries; the
-      // launcher turns it on only where it measured faster (weight_prefetch_depth).
-      int pf_tile = cluster_id, pf_kb = 0;
-      auto prefetch_next = [&]() {
-        if (pf_tile < num_tiles) {
-          tma_prefetch_2d(&tmap_b, pf_kb * Cfg::BLOCK_K, (pf_tile % num_n) * BLOCK_N + cta_rank * B_SLICE_ROWS);
-          if (++pf_kb == num_k) { pf_kb = 0; pf_tile += n_clusters; }
-        }
-      };
-      for (int i = 0; i < pf_ahead; ++i) prefetch_next();
       for (int tile = cluster_id; tile < num_tiles; tile += n_clusters) {
         const int m_blk = (tile / num_n) * CL + cta_rank, n_blk = tile % num_n;
         for (int kb = 0; kb < num_k; ++kb) {
-          if (pf_ahead > 0) prefetch_next();
           mbar_wait(empty_bar(stage), phase ^ 1u);    // slot free in EVERY CTA of the cluster
           mbar_arrive_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
           const uint32_t a_dst = smem_base + stage * Cfg::STAGE_BYTES;
           tma_load_2d(a_dst, &tmap_a, full_bar(stage), kb * Cfg::BLOCK_K, m_blk * Cfg::BLOCK_M);
           if (CL == 1) {
-            tma_load_2d(a_dst + Cfg::A_BYTES, &tmap_b, full_bar(stage), kb * Cfg::BLOCK_K,
-                        n_blk * BLOCK_N);
+            tma_load_2d(a_dst + Cfg::A_BYTES, &tmap_b, full_bar(stage), kb * Cfg::BLOCK_K, n_blk * BLOCK_N);
           } else {
             // my slice of the weight tile, delivered to the same offset in all CL shared memories
             tma_load_2d_mc(a_dst + Cfg::A_BYTES + cta_rank * B_SLICE_ROWS * 128, &tmap_b,
@@ -432,250 +249,64 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer ------------------------------
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(Cfg::BLOCK_M, BLOCK_N);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += n_clusters) {
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);   // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(full_bar(stage), phase);          // TMA bytes have landed
-          tc_fence_after();
-          const uint32_t a_addr = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint64_t a_desc = umma_desc_k_sw128(a_addr);
-          const uint64_t b_desc = umma_desc_k_sw128(a_addr + Cfg::A_BYTES);
+  } else {
+    // ------------------------------ consumers: 64 rows each ------------------------------
+    setmaxnreg_inc<232>();
+    const int cw = wg - 1;
+    const int t = threadIdx.x & 127, lane = threadIdx.x & 31, wq = t >> 5;
+    uint8_t* stg = stage_out + cw * 64 * Cfg::OUT_PITCH;
+    auto release = [&](int s) {
+      if (t == 0) {
+        if (CL == 1) {
+          mbar_arrive(empty_bar(s));
+        } else {
 #pragma unroll
-          for (int k = 0; k < Cfg::BLOCK_K / 16; ++k) {
-            // advance 16 bf16 = 32 B along K inside the swizzle span: +2 in the (addr >> 4) field
-            tc_mma_bf16(d_tmem, a_desc + 2u * k, b_desc + 2u * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          // smem slot free once these MMAs retire; with a cluster, tell every CTA that multicasts here
-          if (CL == 1) tc_commit(empty_bar(stage));
-          else tc_commit_mc(empty_bar(stage), MC_MASK);
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+          for (int r = 0; r < CL; ++r) mbar_arrive_cluster(mapa_cluster(empty_bar(s), (uint32_t)r));
         }
-        tc_commit(tfull_bar(acc));                    // accumulator complete -> epilogue
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1u;
       }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------ epilogue (8 warps) ------------------------------
-    // warp w reads TMEM lanes 32*(w%4).. (hardware restriction) and owns one half of the tile's
-    // 32-column chunks; the tcgen05.ld and the residual loads of chunk i+1 are issued before the
-    // math of chunk i so their latency hides behind it.
-    const int q4 = warp & 3;
-    const int hf = (warp - 4) >> 2;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    };
+    float acc[BLOCK_N / 2];
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = cluster_id; tile < num_tiles; tile += n_clusters) {
       const int m_blk = (tile / num_n) * CL + cta_rank, n_blk = tile % num_n;
-      gemm_epilogue_tile<BLOCK_N, ACT>(
-          tmem_base + acc * BLOCK_N, q4, hf, lane, m_blk, n_blk, C, ldc, bias, residual, ldr, M, N, rope,
-          smem + STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES + (warp - 4) * 2048,
-          [&]() { mbar_wait(tfull_bar(acc), acc_phase); tc_fence_after(); },
-          [&]() { tc_fence_before(); mbar_arrive(tempty_bar(acc)); });
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1u;
+      int prev = -1;
+      for (int kb = 0; kb < num_k; ++kb) {
+        mbar_wait(full_bar(stage), phase);            // TMA bytes have landed
+        const uint32_t a_addr = smem_base + stage * Cfg::STAGE_BYTES;
+        const uint64_t a_desc = wgmma_desc_k_sw128(a_addr + cw * 64 * 128);
+        const uint64_t b_desc = wgmma_desc_k_sw128(a_addr + Cfg::A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < Cfg::BLOCK_K / 16; ++k) {
+          // advance 16 bf16 = 32 B along K inside the swizzle span: +2 in the (addr >> 4) field
+          wgmma_bf16<BLOCK_N>(acc, a_desc + 2u * k, b_desc + 2u * k, (kb | k) != 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                              // the previous k-block's wgmma has retired: its slot is free
+        if (prev >= 0) release(prev);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+      release(prev);
+      wgmma_fence_regs(acc);
+      const int row_base = m_blk * Cfg::BLOCK_M + cw * 64;
+      named_bar_sync(1 + cw, 128);                    // the previous tile's staged block has been stored
+      gemm_epilogue_stage<BLOCK_N, ACT>(acc, stg, lane, wq, row_base, n_blk, bias, M, N, rope);
+      named_bar_sync(1 + cw, 128);
+      gemm_epilogue_store<BLOCK_N, ACT>(stg, t, row_base, n_blk, C, ldc, residual, ldr, M, N, rope);
     }
   }
 
-  tc_fence_before();
   __syncthreads();
   if (CL > 1) cluster_sync_all();      // nobody exits while a peer may still multicast / signal into it
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// CTA-pair variant (tcgen05 cta_group::2): the two CTAs of a cluster work on ONE 256 x BLOCK_N tile. Each
-// CTA stages its own 128 rows of A and only HALF of the weight tile (BLOCK_N / 2 rows); the leader CTA
-// issues M = 256 MMAs that read both shared memories, and each CTA finds its 128 accumulator rows in its
-// own TMEM. Against the multicast clusters above (same L2 traffic) this halves the shared-memory footprint
-// and the shared-memory reads of the weight operand per CTA: 32 KB stages, six of them.
-//   full barrier   lives in the leader, which expects the TMA bytes of BOTH CTAs; the peer's loads complete on
-//                  it too but the peer does not arrive (a remote mbarrier.arrive.release.cluster per stage
-//                  cost the peer's producer ~0.5 us and paced the whole kernel at 0.75 us per k-block).
-//                  The peer cannot run a ring turn ahead: its slot is released by the MMAs of the previous
-//                  turn, which waited for that turn's phase of this barrier
-//   empty barrier  in both CTAs, released by the leader's tcgen05.commit (multicast to the pair)
-//   tmem full      in both CTAs (multicast commit); tmem empty in the leader, 2 x 256 epilogue arrivals
-// ---------------------------------------------------------------------------------------------
-template <int BLOCK_N>
-struct Gemm2Cfg {
-  static constexpr int STAGES = 6;
-  static constexpr int A_BYTES = 128 * 64 * 2;
-  static constexpr int B_BYTES = (BLOCK_N / 2) * 64 * 2;     // this CTA's half of the weight tile
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BAR_BYTES = 256;
-  static constexpr int OUT_STAGE_BYTES = 8 * 2048;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + OUT_STAGE_BYTES + 1024;
-  static constexpr int TMEM_COLS = 2 * BLOCK_N;
-  static_assert(BLOCK_N == 256 || BLOCK_N == 128, "pair tiles are 256 x 256 or 256 x 128");
-};
-
-template <int BLOCK_N, int ACT>
-__global__ void __launch_bounds__(384, 1)
-gemm2_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, bf16* C,
-                     long long ldc, const bf16* __restrict__ bias, const bf16* residual, long long ldr, int M, int N,
-                     int K, int pf_ahead, unsigned long long* __restrict__ trace, const RopeEpilogue rope) {
-  // debug timeline (tools/gemm_pair_trace.py): [cta < 2][k-block < 128, counted over the tiles][4] globaltimer stamps; null in production
-  auto stamp = [&](int kbi, int ev) {
-    if (trace != nullptr && blockIdx.x < 2 && kbi < 128) {
-      unsigned long long t_;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_));
-      trace[((size_t)blockIdx.x * 128 + kbi) * 4 + ev] = t_;
-    }
-  };
-  using Cfg = Gemm2Cfg<BLOCK_N>;
-  constexpr int STAGES = Cfg::STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  const uint32_t pad = ((raw_addr + 1023u) & ~1023u) - raw_addr;
-  uint8_t* smem = smem_raw + pad;
-  const uint32_t smem_base = raw_addr + pad;
-  const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };
-  volatile uint32_t* tmem_ptr_smem =
-      reinterpret_cast<volatile uint32_t*>(smem + STAGES * Cfg::STAGE_BYTES + 8 * (2 * STAGES + 4));
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();                  // 0 = leader: issues the MMAs, owns the full barriers
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 1);            // the leader's arrive.expect_tx (bytes of both CTAs)
-      mbar_init(empty_bar(s), 1);           // one multicast commit
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), 512);        // the epilogue threads of both CTAs
-    }
-    mbar_fence_init();
-  }
-  if (warp == 2) tmem_alloc2(smem_u32(const_cast<uint32_t*>(tmem_ptr_smem)), Cfg::TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  const int num_pairs = (M + 255) / 256;
-  const int num_n = (N + BLOCK_N - 1) / BLOCK_N;
-  const int num_k = (K + 63) / 64;
-  const int cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
-  const int num_tiles = num_pairs * num_n;
-
-  if (warp == 0) {
-    // ------------------------------ TMA producer (both CTAs) ------------------------------
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int pf_tile = cluster_id, pf_kb = 0;                   // L2 look-ahead for this CTA's half of the weight tiles
-      auto prefetch_next = [&]() {
-        if (pf_tile < num_tiles) {
-          tma_prefetch_2d(&tmap_b, pf_kb * 64, (pf_tile % num_n) * BLOCK_N + (int)rank * (BLOCK_N / 2));
-          if (++pf_kb == num_k) { pf_kb = 0; pf_tile += n_clusters; }
-        }
-      };
-      for (int i = 0; i < pf_ahead; ++i) prefetch_next();
-      int gkb = 0;                                           // k-blocks issued by this CTA so far (trace index)
-      for (int tile = cluster_id; tile < num_tiles; tile += n_clusters) {
-        const int m_blk = (tile / num_n) * 2 + (int)rank, n_blk = tile % num_n;
-        for (int kb = 0; kb < num_k; ++kb, ++gkb) {
-          if (pf_ahead > 0) prefetch_next();
-          stamp(gkb, 0);
-          mbar_wait_safe(empty_bar(stage), phase ^ 1u);
-          stamp(gkb, 1);
-          const uint32_t lead_full = mapa_cluster(full_bar(stage), 0);
-          if (rank == 0) mbar_arrive_expect_tx(full_bar(stage), 2 * Cfg::STAGE_BYTES);   // the bytes of BOTH CTAs
-          const uint32_t a_dst = smem_base + stage * Cfg::STAGE_BYTES;
-          tma_load_2d_2cta(a_dst, &tmap_a, lead_full, kb * 64, m_blk * 128);
-          tma_load_2d_2cta(a_dst + Cfg::A_BYTES, &tmap_b, lead_full, kb * 64, n_blk * BLOCK_N + (int)rank * (BLOCK_N / 2));
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer (leader only) ------------------------------
-    if (lane == 0 && rank == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(256, BLOCK_N);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      int gkb = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += n_clusters) {
-        mbar_wait_safe(tempty_bar(acc), acc_phase ^ 1u);     // both epilogues have drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int kb = 0; kb < num_k; ++kb, ++gkb) {
-          stamp(gkb, 2);
-          mbar_wait_safe(full_bar(stage), phase);
-          tc_fence_after();
-          stamp(gkb, 3);
-          const uint32_t a_addr = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint64_t a_desc = umma_desc_k_sw128(a_addr);
-          const uint64_t b_desc = umma_desc_k_sw128(a_addr + Cfg::A_BYTES);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            tc_mma_bf16_2cta(d_tmem, a_desc + 2u * k, b_desc + 2u * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          tc_commit_2cta(empty_bar(stage), 3);               // the slot is free in both CTAs
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        tc_commit_2cta(tfull_bar(acc), 3);                   // accumulator complete -> both epilogues
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1u;
-      }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------ epilogue (8 warps per CTA, own 128 rows) ------------------------------
-    const int q4 = warp & 3;
-    const int hf = (warp - 4) >> 2;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = cluster_id; tile < num_tiles; tile += n_clusters) {
-      const int m_blk = (tile / num_n) * 2 + (int)rank, n_blk = tile % num_n;
-      const uint32_t lead_tempty = mapa_cluster(tempty_bar(acc), 0);
-      gemm_epilogue_tile<BLOCK_N, ACT>(
-          tmem_base + acc * BLOCK_N, q4, hf, lane, m_blk, n_blk, C, ldc, bias, residual, ldr, M, N, rope,
-          smem + STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES + (warp - 4) * 2048,
-          [&]() { mbar_wait_safe(tfull_bar(acc), acc_phase); tc_fence_after(); },
-          [&]() { tc_fence_before(); mbar_arrive_cluster(lead_tempty); });
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1u;
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                  // nobody exits (or frees TMEM) while the peer may still read / signal it
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, Cfg::TMEM_COLS);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
 static PFN_cuTensorMapEncodeTiled_v12000 g_encode = nullptr;
-static unsigned long long* g_gemm_trace = nullptr;     // debug: vcl_debug_set_gemm_trace
-
 static int resolve_encode() {
   if (g_encode) return 0;
   void* fn = nullptr;
@@ -716,66 +347,9 @@ int device_num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
+    if (g_num_sms <= 0) g_num_sms = 132;
   }
   return g_num_sms;
-}
-
-// k-blocks of L2 look-ahead for the weight operand (see the producer), measured on the prefill shapes
-// (M = 448, tools/sweep_gemm.py with VCL_GEMM_PF = 0 / 8 / 16 / 32): it pays only where one CTA of a 4-cluster
-// streams its quarter of a 256-wide weight tile -- gate|up 95 -> 88 us at depth 8, q|k|v 71 -> 65 us (level with
-// the 128-wide tiles it then uses anyway) -- is neutral for the CTA pairs and costs 5-10 % where every row tile
-// prefetches the same weights for itself (no cluster). VCL_GEMM_PF=<k-blocks> overrides (0 = off) for A/B runs.
-// The ACTIVATION operand of the ViT GEMMs was tried too: the per-k-block timeline (tools/gemm_pair_trace.py,
-// PAIR_SHAPE=25700,3072,1024) shows a ~2.9 us bubble at every tile start (the first loads of rows nobody has touched
-// take 2.6-4.4 us against 0.33 us per k-block), yet pulling the next tile's rows into L2 ahead of time made every
-// shape SLOWER, through the TMA (q|k|v 132 -> 144 us, fc2 153 -> 188) as well as with plain prefetch.global.L2
-// issued by the idle warp (128 -> 143, 153 -> 172). Not kept.
-static int weight_prefetch_depth(const GemmArgs& g, int block_n, int cl) {
-  static const int forced = getenv("VCL_GEMM_PF") ? atoi(getenv("VCL_GEMM_PF")) : -1;
-  if (forced >= 0) return forced;
-  return (cl == 4 && block_n == 256 && (g.M + 127) / 128 <= 16) ? 8 : 0;
-}
-
-template <int BLOCK_N, int ACT>
-static int launch_pair(const GemmArgs& g, cudaStream_t stream) {
-  using Cfg = Gemm2Cfg<BLOCK_N>;
-  auto kern = gemm2_bf16_tn_kernel<BLOCK_N, ACT>;
-  CUtensorMap ta, tb;
-  if (make_tmap_2d(&ta, g.A, g.M, g.K, g.lda, 128) != 0) return -2;
-  if (make_tmap_2d(&tb, g.W, g.N, g.K, g.ldw, BLOCK_N / 2) != 0) return -2;
-  const int num_tiles = ((g.M + 255) / 256) * ((g.N + BLOCK_N - 1) / BLOCK_N);
-  int clusters = device_num_sms() / 2;
-  if (clusters > num_tiles) clusters = num_tiles;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(clusters * 2);
-  cfg.blockDim = dim3(384);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, ta, tb, g.C, (long long)g.ldc, g.bias, g.residual, (long long)g.ldr, g.M,
-                                 g.N, g.K, weight_prefetch_depth(g, BLOCK_N, -2), g_gemm_trace, g.rope));
-  count_launches(1);
-  return 0;
-}
-
-template <int BLOCK_N>
-static int launch_pair_act(const GemmArgs& g, cudaStream_t stream) {
-  switch (g.act) {
-    case ACT_NONE: return launch_pair<BLOCK_N, ACT_NONE>(g, stream);
-    case ACT_QGELU: return launch_pair<BLOCK_N, ACT_QGELU>(g, stream);
-    case ACT_GELU: return launch_pair<BLOCK_N, ACT_GELU>(g, stream);
-    case ACT_SWIGLU: return launch_pair<BLOCK_N, ACT_SWIGLU>(g, stream);
-    case ACT_ROPE: return launch_pair<BLOCK_N, ACT_ROPE>(g, stream);
-  }
-  set_last_error("gemm: unknown activation %d", g.act);
-  return -1;
 }
 
 template <int BLOCK_N, int ACT, int CL>
@@ -787,12 +361,7 @@ static int launch_one(const GemmArgs& g, cudaStream_t stream) {
   if (make_tmap_2d(&tb, g.W, g.N, g.K, g.ldw, BLOCK_N / CL) != 0) return -2;
   const int num_m = (g.M + 127) / 128;
   const int num_tiles = ((num_m + CL - 1) / CL) * ((g.N + BLOCK_N - 1) / BLOCK_N);   // cluster-tiles
-  int clusters = device_num_sms() / CL;
-  if (CL == 4) clusters -= 4;            // GPC boundaries strand ~16 SMs for 4-CTA clusters
-  if (clusters > num_tiles) clusters = num_tiles;
-  if (g.max_ctas > 0 && clusters * CL > g.max_ctas) clusters = g.max_ctas / CL > 0 ? g.max_ctas / CL : 1;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(clusters * CL);
   cfg.blockDim = dim3(384);
   cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
   cfg.stream = stream;
@@ -803,8 +372,21 @@ static int launch_one(const GemmArgs& g, cudaStream_t stream) {
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = CL > 1 ? 1 : 0;
+  // persistent CTAs: as many clusters as are resident at once (GPC boundaries strand some SMs for clusters)
+  static int resident = 0;
+  if (resident == 0) {
+    if (CL > 1) {
+      cfg.gridDim = dim3(CL);
+      VCL_CUDA_OK(cudaOccupancyMaxActiveClusters(&resident, kern, &cfg));
+    }
+    if (resident <= 0) resident = device_num_sms() / CL;
+  }
+  int clusters = resident;
+  if (clusters > num_tiles) clusters = num_tiles;
+  if (g.max_ctas > 0 && clusters * CL > g.max_ctas) clusters = g.max_ctas / CL > 0 ? g.max_ctas / CL : 1;
+  cfg.gridDim = dim3(clusters * CL);
   VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, ta, tb, g.C, (long long)g.ldc, g.bias, g.residual,
-                                 (long long)g.ldr, g.M, g.N, g.K, weight_prefetch_depth(g, BLOCK_N, CL), g.rope));
+                                 (long long)g.ldr, g.M, g.N, g.K, g.rope));
   count_launches(1);
   return 0;
 }
@@ -857,26 +439,10 @@ static int init_bn() {
   }
   return 0;
 }
-// Opt every instantiation into its dynamic shared memory size (done once, outside any capture).
-template <int BLOCK_N>
-static int init_pair() {
-  VCL_CUDA_OK(cudaFuncSetAttribute(gemm2_bf16_tn_kernel<BLOCK_N, ACT_NONE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Gemm2Cfg<BLOCK_N>::SMEM_BYTES));
-  VCL_CUDA_OK(cudaFuncSetAttribute(gemm2_bf16_tn_kernel<BLOCK_N, ACT_QGELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, Gemm2Cfg<BLOCK_N>::SMEM_BYTES));
-  VCL_CUDA_OK(cudaFuncSetAttribute(gemm2_bf16_tn_kernel<BLOCK_N, ACT_GELU>, cudaFuncAttributeMaxDynamicSharedMemorySize, Gemm2Cfg<BLOCK_N>::SMEM_BYTES));
-  VCL_CUDA_OK(cudaFuncSetAttribute(gemm2_bf16_tn_kernel<BLOCK_N, ACT_SWIGLU>, cudaFuncAttributeMaxDynamicSharedMemorySize, Gemm2Cfg<BLOCK_N>::SMEM_BYTES));
-  VCL_CUDA_OK(cudaFuncSetAttribute(gemm2_bf16_tn_kernel<BLOCK_N, ACT_ROPE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Gemm2Cfg<BLOCK_N>::SMEM_BYTES));
-  return 0;
-}
-
 int init_gemm_kernels() {
   if (resolve_encode() != 0) return -2;
-  if (init_pair<256>() || init_pair<128>()) return -2;
   if (init_bn<256>() || init_bn<128>() || init_bn<64>() || init_bn<32>()) return -2;
   return 0;
-}
-
-extern "C" void vcl_debug_set_gemm_trace(void* dev_buffer) {
-  g_gemm_trace = reinterpret_cast<unsigned long long*>(dev_buffer);
 }
 
 int launch_gemm_bf16_tn(const GemmArgs& g, cudaStream_t stream) {
@@ -901,7 +467,7 @@ int launch_gemm_bf16_tn(const GemmArgs& g, cudaStream_t stream) {
   int bn = g.block_n;
   int cl = g.cluster;
   if (bn == 0) {
-    // Tile / cluster choice, from the block_n x cluster sweep on B200 (profiles/r01_gemm_sweep.txt):
+    // Tile / cluster choice (heuristic, not tuned by a sweep on this GPU):
     //  * many M tiles (ViT, batched prefill): 128x256 tiles, pairs of CTAs sharing each weight tile;
     //  * few M tiles (single-clip prefill, M = 448): the weight stream dominates L2->SM traffic, so
     //    all M tiles of an N tile form one cluster (multicast x4) when there are enough tiles to fill
@@ -911,10 +477,7 @@ int launch_gemm_bf16_tn(const GemmArgs& g, cudaStream_t stream) {
     const long long mt = (g.M + 127) / 128;
     int auto_cl = 1;
     if (mt >= 16 && g.N % 256 == 0) {
-      // long-K tiles (ViT fc2, K = 4096): CTA pairs (cta_group::2, 256 x 256 per pair) are 2-3 % ahead of the
-      // multicast pairs; with K = 1024 the pair's longer fill / drain per tile costs more than it saves
-      // (profiles/r02_gemm_sweep.txt: q|k|v 154 vs 129 us, fc1 188 vs 166, out 57 vs 53, fc2 156 vs 160)
-      bn = 256; auto_cl = g.K >= 4096 ? -2 : 2;
+      bn = 256; auto_cl = 2;
     } else if (mt >= 2) {
       const int mcl = mt >= 4 ? 4 : 2;
       if (g.N % 256 == 0 && mt * (g.N / 256) >= 2 * sms) { bn = 256; auto_cl = mcl; }
@@ -931,13 +494,12 @@ int launch_gemm_bf16_tn(const GemmArgs& g, cudaStream_t stream) {
     if (forced_cl == 1 && mt >= 2 && mt < 16 && bn == 128 && g.N % 256 == 0 && mt * (g.N / 256) >= sms) bn = 256;
   }
   if (cl == 0) cl = 1;
+  // cluster = -2: a CTA pair on one 256 x BLOCK_N tile, each CTA fetching half of the weight tile. sm_90 has no
+  // pair MMA (each CTA's wgmma reads only its own shared memory), so the pair is the 2-CTA multicast cluster:
+  // both halves land in both CTAs. Pairs take 128- or 256-wide tiles; anything else runs without a cluster.
+  if (cl == -2) cl = (bn == 256 || bn == 128) && g.N % bn == 0 ? 2 : 1;
   if (g.act == ACT_ROPE && g.block_n == 0 && bn < 128) bn = 128;      // one head (128 columns) per tile at least
   VCL_REQUIRE(g.act != ACT_ROPE || bn == 128 || bn == 256, "gemm: ACT_ROPE needs 128- or 256-wide tiles (one head = 128 columns), got %d", bn);
-  // cluster = -2 (or VCL_GEMM_PAIR=1 for every launch with at least two row tiles): CTA pairs, cta_group::2
-  static const bool pair_all = getenv("VCL_GEMM_PAIR") != nullptr;
-  if ((cl == -2 || (pair_all && g.M > 128)) && (bn == 256 || bn == 128) && g.N % bn == 0)
-    return bn == 256 ? launch_pair_act<256>(g, stream) : launch_pair_act<128>(g, stream);
-  if (cl == -2) cl = 1;
   VCL_REQUIRE(cl == 1 || cl == 2 || cl == 4, "gemm: cluster must be 1, 2 or 4 (got %d)", cl);
   switch (bn) {
     case 256: return launch_act<256>(g, cl, stream);

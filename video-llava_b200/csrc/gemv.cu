@@ -6,7 +6,7 @@
 //
 // With one token per clip every weight byte is used once per step (13.2 GB per step for the 7B
 // model, SURVEY.md section 8d), so these kernels are pure HBM streaming; 5 <= B <= 16 uses
-// gemv_mma.cu, larger batches the tcgen05 GEMM with a narrow N tile.
+// gemv_mma.cu, larger batches the wgmma GEMM with a narrow N tile.
 //
 // Work decomposition (one CTA = 16 warps = 512 threads):
 //   * the N weight rows are cut into equal contiguous blocks, one per CTA (grid ~ #SMs, so every
@@ -319,7 +319,7 @@ int launch_nb(const GemvParams& p, cudaStream_t stream) {
 
 template <int MODE>
 int launch_mode(int B, const GemvParams& p, cudaStream_t stream) {
-  VCL_REQUIRE(B >= 1 && B <= 4, "gemv: batch %d outside 1..4 (larger batches use the tcgen05 GEMM)", B);
+  VCL_REQUIRE(B >= 1 && B <= 4, "gemv: batch %d outside 1..4 (larger batches use the wgmma GEMM)", B);
   VCL_REQUIRE(p.K % 8 == 0 && p.ldx % 8 == 0, "gemv: K and pitch must be multiples of 8");
   VCL_REQUIRE(((uintptr_t)p.x % 16) == 0 && ((uintptr_t)p.W % 16) == 0, "gemv: 16-byte alignment required");
   switch (B) {

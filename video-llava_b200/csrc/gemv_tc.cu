@@ -1,19 +1,15 @@
 // Single-clip decode projections (B = 1): out[n] = x . W[n, :], one kernel per weight matrix.
 //
-// What bounds these kernels is how much of the time HBM is kept streaming. Measured on this part
-// (profiles/r01_hbm_read_probe.txt, r01_hbm_chain_probe.txt, r01_tc_trace.txt):
-//   * one B200 reads at 7.2-7.3 TB/s; a chain of 129 pure-read kernels over the step's 13.2 GB
-//     reaches 6.9-7.0 TB/s with programmatic dependent launch (the next kernel's first loads are
-//     in flight while the current one drains), 6.1-6.2 TB/s when every kernel starts cold;
-//   * cp.async.bulk rings stream as fast as the best register pipelines, cost no registers and no
-//     issue slots in the consumer warps, but the copy engine retires only ~23 copies/us per SM
-//     whatever their size: one copy per 1 KB row segment gives 3.4 TB/s, 2 KB 6.8 TB/s, so the
-//     slots have to be contiguous in memory and fetched with ONE copy each;
-//   * the CUDA-core GEMV (gemv.cu) spends ~50 instructions per KB of weights (unpack, FMA, warp
-//     shuffle reduction) and loses 10 % when a few more are added; mma.sync does the K reduction
-//     in the tensor pipe at ~6 instructions per KB;
+// What bounds these kernels is how much of the time HBM is kept streaming:
+//   * a chain of per-matrix kernels keeps HBM busier with programmatic dependent launch (the next
+//     kernel's first loads are in flight while the current one drains) than when every kernel starts cold;
+//   * cp.async.bulk rings cost no registers and no issue slots in the consumer warps, but the copy engine
+//     retires a limited number of copies per SM whatever their size, so the slots have to be contiguous
+//     in memory and fetched with ONE copy each;
+//   * the CUDA-core GEMV (gemv.cu) spends tens of instructions per KB of weights (unpack, FMA, warp
+//     shuffle reduction); mma.sync does the K reduction in the tensor pipe at a few instructions per KB;
 //   * the serial latency after griddepcontrol.wait (activation fetch + norm) is dead time for HBM
-//     once the ring is full: it is one L2 round trip here (1.0-1.4 us, was 2.9 us).
+//     once the ring is full, so it is kept to one L2 round trip.
 //
 // Structure (one CTA per SM, 9 warps, 8 x 16 KB ring):
 //   warp 8      producer: walks this CTA's 16-row groups, K chunk by K chunk (512 k), and fills
@@ -29,13 +25,7 @@
 //               vector. fp32 accumulators live across the K chunks of a row group; the 8 per-warp
 //               partials meet in shared memory after every group and the fused epilogues (RoPE +
 //               KV append, SwiGLU, residual, logits) run once at the end.
-// Ring depth: 6 slots -> 79 ms per 31 decode steps (7B), 8 -> 74 ms, 9 -> 79 ms, 13 -> 81 ms; two
-// half-SM CTAs of consecutive kernels (6 slots each) -> 77-82 ms. 8 it is.
-// Deeper rings only for the kernels that are not followed by the attention kernel (round 2: 12 slots for
-// gate|up, 11 for down, 12 for the head) do not help either: 77.1 / 74.6 / 75.8 (all three) against 74.7-75.3 ms.
-// An L2 look-ahead (round 2: the producer issuing cp.async.bulk.prefetch.L2 for the 4 / 8 / 16 / 32 slots of
-// its share in front of the ring, to keep HBM streaming while the ring is full during a hand-off) made the
-// decode loop slower the further it ran ahead: 76.5 / 78.2 / 83.2 / 91.4 ms against 75.8 ms without.
+// Ring depth: 8 slots by default (VCL_GEMV_TC_SLOTS overrides it for A/B runs); not re-tuned on the H100.
 //
 // Arithmetic and rounding points are those of gemv.cu (reference: transformers/models/llama/
 // modeling_llama.py:53-67 RMSNorm, :124-168 RoPE, :171-184 MLP, :325,331 residuals).
@@ -57,7 +47,7 @@ constexpr int TC_THREADS = TC_CONSUMERS + 32;
 constexpr int TC_KC = 512;                          // k elements per slot
 constexpr int TC_SLOT_BYTES = 16 * TC_KC * 2;       // 16 KB, one bulk copy
 constexpr int TC_MAX_SLOTS = 14;                    // barrier array size
-constexpr int TC_DEFAULT_SLOTS = 8;                 // measured optimum (7 B shapes): 6 -> 79 ms, 8 -> 74 ms, 9 -> 79 ms per 31 steps
+constexpr int TC_DEFAULT_SLOTS = 8;
 constexpr int TC_SMEM_BUDGET = 160 * 1024;          // one CTA per SM; the rest of the SM stays free for the
                                                     // attention kernel's CTAs, which launch early (PDL)
 
@@ -140,11 +130,7 @@ __global__ void __launch_bounds__(TC_THREADS, 2) gemv_tc_kernel(const TcParams p
   uint32_t par = 0;
   auto advance = [&]() { if (++slot == n_slots) { slot = 0; par ^= 1u; } };
   // contiguous blocks of 16-row groups per CTA, sizes differing by at most one group, the larger shares
-  // spread evenly over the grid. (Round 2: giving the larger shares to the lowest block indices -- the
-  // blocks that are dispatched first, to the SMs whose previous CTA had the smaller share -- measured the
-  // same, 77.3 vs 77.5 ms per decode loop; the reverse order 79.0 ms.) (Cutting the
-  // matrix into equal SLOT shares with partial sums exchanged between neighbours - stream-K - was
-  // measured: every CTA then streams the same bytes, but the kernels got 9 % slower.)
+  // spread evenly over the grid.
   auto my_groups = [&](int N, int& grp_begin) {
     const int n_groups = (N + 15) >> 4;
     grp_begin = (int)(((long long)blockIdx.x * n_groups) / gridDim.x);
@@ -594,8 +580,8 @@ int plan(const TcPhase* ph, int n, int nb, int grid, size_t* smem_bytes, int* x_
   static const int env_slots = getenv("VCL_GEMV_TC_SLOTS") ? atoi(getenv("VCL_GEMV_TC_SLOTS")) : 0;
   static const size_t budget = getenv("VCL_GEMV_TC_SMEM_KB") ? (size_t)atoi(getenv("VCL_GEMV_TC_SMEM_KB")) * 1024 : (size_t)TC_SMEM_BUDGET;
   if (fixed + 4 * (size_t)TC_SLOT_BYTES > (nb > 1 ? (size_t)212 * 1024 : budget)) return 0;
-  // a launch may ask for a deeper ring (the projection after the attention kernel sits resident for
-  // ~7 us with nothing to do but prefetch); the hard limit leaves room for the attention CTAs
+  // a launch may ask for a deeper ring (the projection after the attention kernel sits resident with
+  // nothing to do but prefetch); the hard limit leaves room for the attention CTAs
   const size_t limit = (want > TC_DEFAULT_SLOTS || nb > 1) ? (size_t)212 * 1024 : budget;   // several clips: x takes the room
   int slots = (int)((limit - fixed) / TC_SLOT_BYTES);
   if (want > TC_MAX_SLOTS) want = TC_MAX_SLOTS;

@@ -23,10 +23,8 @@
 //     at the end, in the (then idle) ring memory.
 //   * clip b is column b of the m16n8k16 B operand: two column blocks cover 16 clips.
 //
-// Measured on the way (tools/microbench.py gemv16, 16 clips, 7B shapes, cold): a warp per row group (no
-// reduction at all) streamed at 3-4 TB/s whatever the number of warps per group -- with a slot held for
-// ~1000 cycles by its one consumer only three of the eight ring slots were in flight -- and 1.6-2.2 TB/s
-// on o_proj / down_proj because of the per-row window copies.
+// A warp per row group (no reduction at all) keeps a slot held for ~1000 cycles by its one consumer, so only
+// a few of the ring slots are in flight; per-row window copies make the copy engine the limit.
 //
 // Epilogues (RoPE + KV append, SwiGLU, residual, logits) and every rounding point are those of
 // gemv_tc.cu / gemv.cu (reference: transformers/models/llama/modeling_llama.py:124-168 RoPE, :171-184
@@ -234,7 +232,7 @@ __global__ void __launch_bounds__(TW_THREADS, 1) gemv_tcw_kernel(const TwParams 
   // All 256 consumer threads share the items of every group: thread = (row or row pair, clip) with the ROW
   // index fastest, so that a warp's accesses to the residual / output rows are contiguous runs (a warp per
   // group walking (row, clip) items with the clip fastest touched 32 sectors per instruction, one dependent
-  // round trip per 32 items: ~10 us at the end of every launch). The 8 partial tiles are summed on the fly,
+  // round trip per 32 items at the end of every launch). The 8 partial tiles are summed on the fly,
   // in a fixed order.
   const int mode = p.mode;
   const bool pairs = (mode == TW_SWIGLU || mode == TW_QKV);

@@ -26,7 +26,7 @@ void count_launches(long long n);
 long long launch_count();
 int device_num_sms();
 
-// ---- gemm_tc.cu : C[M,N] = epi(A[M,K] . W[N,K]^T), tcgen05 + TMA -------------------------------
+// ---- gemm_tc.cu : C[M,N] = epi(A[M,K] . W[N,K]^T), wgmma + TMA ----------------------------------
 struct GemmArgs {
   const bf16* A = nullptr;  long long lda = 0;   // activations, row pitch in elements
   const bf16* W = nullptr;  long long ldw = 0;   // weights [N,K] (nn.Linear layout)
@@ -100,15 +100,18 @@ struct AttnArgs {
   int S_kv = 0;      // number of keys (0: = S); > S when the queries continue a cached sequence
   int q_off = 0;     // absolute position of query 0 for the causal mask (S_kv - S for a continuation)
 };
-int launch_attention(const AttnArgs& a, cudaStream_t stream);     // dispatches to the tcgen05 prefill kernel when it applies
+int launch_attention(const AttnArgs& a, cudaStream_t stream);     // dispatches to the wgmma prefill kernel when it applies
 int init_attention_kernels();
-// ---- attention_prefill_tc.cu : tcgen05 causal attention (hd 128, <= 512 keys) -----------------------
+// ---- attention_prefill_tc.cu : wgmma causal attention (hd 128, <= 512 keys, exact full-row softmax) ----
 bool attention_prefill_tc_supported(const AttnArgs& a);
 int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t stream);
 int init_attention_prefill_tc_kernels();
-// ---- attention_tc.cu : tcgen05 attention for the ViT (hd 64, 129 <= S <= 257, non-causal) ----------
-int launch_attention_vit_tc(const bf16* qkv, bf16* out, int n_frames, int S, int H, int C,
-                            cudaStream_t stream);
+// the ViT's attention (hd 64, non-causal) straight out of the fused q|k|v activation [n_frames * S, 3*C]:
+// the wgmma kernel below for 129 <= S <= 257, the mma.sync kernel otherwise (336-px tower, S = 577)
+int launch_attention_vit(const bf16* qkv, bf16* out, int n_frames, int S, int H, int C, cudaStream_t stream);
+// ---- attention_tc.cu : wgmma ViT attention (hd 64, non-causal, 129 <= S <= 257, exact full-row softmax) ----
+bool attention_vit_tc_supported(int S);
+int launch_attention_vit_tc(const bf16* qkv, bf16* out, int n_frames, int S, int H, int C, cudaStream_t stream);
 int init_attention_tc_kernels();
 // single-query attention against the cache: q [B, H*hd] -> o [B, H*hd]; kv_len keys per clip
 int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, const bf16* vcache,

@@ -16,8 +16,7 @@
 // channels (one coalesced 128-bit load per input row, 1 KB contiguous per group), the 4 groups deal the
 // input rows round-robin with 8 loads in flight per lane, and a fixed-order shared-memory combine of the
 // 4 partial sums finishes the mean (deterministic). 2 x 356 = 712 CTAs of 256 threads: ALL resident at
-// once (one wave, ~5 per SM, ~150 KB of loads in flight per SM). Round 1 ran 356 CTAs of 1024 threads
-// (2 per SM, 20.4 us = 0.40 of the HBM rate); 1424 CTAs of 256 threads ran in 1.2 waves (17 us).
+// once (one wave, ~5 per SM, ~150 KB of loads in flight per SM).
 // Both roles stream the same tensor concurrently, so the second touch of a line is an L2 hit rather
 // than a second HBM read.
 #include "common.cuh"

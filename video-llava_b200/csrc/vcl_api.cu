@@ -99,7 +99,6 @@ struct vcl_handle {
   unsigned long long graph_clock = 0;
   int* d_pos = nullptr;                        // prompt length of the running decode loop (device scalar)
   ArgmaxPart* amax = nullptr;                  // [#SMs][max_batch] per-CTA partial arg-max of the logits kernel
-  bool force_legacy_attention = false;
 
   size_t cache_layer_elems() const {
     return (size_t)cfg.max_batch * cfg.llm_heads * cfg.max_seq * 128;
@@ -164,8 +163,7 @@ int check_device() {
   }
   int major = 0;
   VCL_CUDA_OK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  VCL_REQUIRE(major == 10, "device compute capability %d.x is not sm_100 (B200); libvcl is sm_100a only",
-              major);
+  VCL_REQUIRE(major == 9, "device compute capability %d.x is not sm_90 (H100); libvcl is sm_90a only", major);
   return 0;
 }
 
@@ -205,8 +203,6 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   int rc = 0;
   rc |= init_gemm_kernels();
   rc |= init_attention_kernels();
-  rc |= init_attention_tc_kernels();
-  h->force_legacy_attention = getenv("VCL_LEGACY_ATTENTION") != nullptr;
   rc |= init_gemv_kernels();
   rc |= init_gemv_tc_kernels();
   rc |= init_gemv_mma_kernels();
@@ -425,22 +421,11 @@ int clip_forward(vcl_handle* h, const void* pixels, int fmt, int n_frames, int n
                h->KP, ACT_NONE, st));
   VCL_TRY(launch_clip_embed_ln(patch_out, h->cls, h->pos, h->pre_w, h->pre_b, h->v_h, n_frames, P, C,
                                c.clip_ln_eps, st));
-  const float scale = 0.125f;  // head_dim 64 ^ -1/2
   for (int l = 0; l < n_layers; ++l) {
     const ClipLayerW& w = h->cl[l];
     VCL_TRY(launch_layernorm(h->v_h, C, h->v_x, C, w.ln1_w, w.ln1_b, M, C, c.clip_ln_eps, st));
     VCL_TRY(gemm(h->v_x, C, w.wqkv, C, h->v_qkv, 3 * C, w.bqkv, nullptr, 0, M, 3 * C, C, ACT_NONE, st));
-    AttnArgs a;
-    a.q = h->v_qkv;         a.q_sb = (long long)S * 3 * C; a.q_sh = 64; a.q_ss = 3 * C;
-    a.k = h->v_qkv + C;     a.k_sb = a.q_sb; a.k_sh = 64; a.k_ss = 3 * C;
-    a.v = h->v_qkv + 2 * C; a.v_sb = a.q_sb; a.v_sh = 64; a.v_ss = 3 * C;
-    a.o = h->v_attn;        a.o_sb = (long long)S * C; a.o_sh = 64; a.o_ss = C;
-    a.B = n_frames; a.H = c.clip_heads; a.S = S; a.head_dim = 64; a.scale = scale; a.causal = 0;
-    if (S >= 129 && S <= 257 && !h->force_legacy_attention) {
-      VCL_TRY(launch_attention_vit_tc(h->v_qkv, h->v_attn, n_frames, S, c.clip_heads, C, st));
-    } else {
-      VCL_TRY(launch_attention(a, st));   // 336-px tower (S = 577): flash-style mma.sync kernel
-    }
+    VCL_TRY(launch_attention_vit(h->v_qkv, h->v_attn, n_frames, S, c.clip_heads, C, st));
     VCL_TRY(gemm(h->v_attn, C, w.wo, C, h->v_h, C, w.bo, h->v_h, C, M, C, C, ACT_NONE, st));
     VCL_TRY(launch_layernorm(h->v_h, C, h->v_x, C, w.ln2_w, w.ln2_b, M, C, c.clip_ln_eps, st));
     VCL_TRY(gemm(h->v_x, C, w.w1, C, h->v_act, F, w.b1, nullptr, 0, M, F, C, ACT_QGELU, st));
@@ -913,11 +898,10 @@ int vcl_op_attention_vit(const void* qkv, void* out, int n_frames, int S, int H,
   if (check_device() != 0) return -2;
   static bool inited = false;
   if (!inited) {
-    VCL_TRY(init_gemm_kernels());
-    VCL_TRY(init_attention_tc_kernels());
+    VCL_TRY(init_attention_kernels());
     inited = true;
   }
-  return launch_attention_vit_tc(reinterpret_cast<const bf16*>(qkv), reinterpret_cast<bf16*>(out), n_frames, S, H,
+  return launch_attention_vit(reinterpret_cast<const bf16*>(qkv), reinterpret_cast<bf16*>(out), n_frames, S, H,
                                  H * 64, as_stream(stream));
 }
 

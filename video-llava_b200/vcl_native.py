@@ -1,7 +1,7 @@
 """ctypes binding of libvcl.so (include/vcl.h). PyTorch is used only as the owner of device
 memory and streams: every call passes raw device pointers and the current CUDA stream.
 
-There is no fallback: if the shared library is missing or the device is not an sm_100 GPU the
+There is no fallback: if the shared library is missing or the device is not an sm_90 (H100) GPU the
 calls raise.
 """
 from __future__ import annotations
@@ -168,7 +168,7 @@ def op_attention(q, k, v, scale, causal):
 
 
 def op_attention_vit(qkv, n_frames, S, H):
-    """qkv: [n_frames*S, 3*H*64] bf16 -> [n_frames*S, H*64] (tcgen05 ViT attention)."""
+    """qkv: [n_frames*S, 3*H*64] bf16 -> [n_frames*S, H*64] (ViT attention)."""
     out = torch.empty(n_frames * S, H * 64, dtype=torch.bfloat16, device=qkv.device)
     check(lib().vcl_op_attention_vit(ptr(qkv), ptr(out), n_frames, S, H, cur_stream()))
     return out

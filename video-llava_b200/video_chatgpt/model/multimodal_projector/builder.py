@@ -1,6 +1,6 @@
 """mm_projector factory (reference: video_chatgpt/model/multimodal_projector/builder.py:33-51).
 
-In this build the projector is not an nn.Module: its GEMM(s) run inside libvcl.so (tcgen05 GEMM with
+In this build the projector is not an nn.Module: its GEMM(s) run inside libvcl.so (wgmma GEMM with
 bias / erf-GELU epilogues, written straight into the rows that get spliced into the prompt). The
 factory therefore returns a ProjectorSpec that names the state_dict keys and the C-ABI proj_type.
 """
