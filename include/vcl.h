@@ -54,7 +54,8 @@ typedef struct vcl_config {
   /* language model: LLaMA/Vicuna ($TF/models/llama/modeling_llama.py:355-425) */
   int32_t llm_layers;    /* 32 (7B) / 40 (13B) */
   int32_t llm_hidden;    /* 4096 / 5120 (head_dim must be 128) */
-  int32_t llm_inter;     /* 11008 / 13824 */
+  int32_t llm_inter;     /* 11008 / 13824; at most 14336 (the 1..4-clip decode kernel stages the
+                            down_proj input in shared memory): vcl_create rejects larger values */
   int32_t llm_heads;     /* 32 / 40 (kv heads == heads) */
   int32_t vocab;         /* 32003 after the three video tokens are added (eval/model_utils.py:114-119) */
   float rms_eps;         /* 1e-5 */
@@ -88,8 +89,7 @@ void vcl_destroy(vcl_handle* h);
  * (fused q|k|v, interleaved gate/up, K-padded patch-embed matrix). Unknown names are ignored
  * (e.g. vision_model.post_layernorm.*, unused by the path); a missing required name is an error.
  * vcl_load_llm_weights additionally builds a decode-only copy of the streamed matrices in the slot
- * order of the single-clip decode kernel (+1x the LLM weight bytes; VCL_NO_TILED_WEIGHTS=1 in the
- * environment skips it and decode falls back to the row-major kernels). */
+ * order of the decode kernels (+1x the LLM weight bytes). */
 int vcl_load_clip_weights(vcl_handle* h, const vcl_tensor* tensors, int n);
 int vcl_load_llm_weights(vcl_handle* h, const vcl_tensor* tensors, int n);
 

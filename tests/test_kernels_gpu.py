@@ -188,7 +188,8 @@ def test_attention_vit_tcgen05(n, S, H):
 
 @pytest.mark.parametrize("B,N,K,norm,res", [(1, 4096, 4096, False, True), (1, 12288, 4096, True, False),
                                             (4, 4096, 11008, False, True), (3, 1000, 5120, True, True),
-                                            (2, 32003, 4096, True, False)])
+                                            (2, 32003, 4096, True, False), (16, 32003, 4096, False, False),
+                                            (8, 1000, 5120, True, True)])
 def test_gemv(B, N, K, norm, res):
     torch.manual_seed(N + K + B)
     dev = _dev()

@@ -39,7 +39,7 @@ lib.vcl_debug_tc_trace_dump.argtypes = [ctypes.c_char_p]
 print("dump rc", lib.vcl_debug_tc_trace_dump(path.encode()))
 raw = np.fromfile(path, dtype=np.uint64)
 n_rec, G = int(raw[0]), int(raw[1])
-t = raw[2:].reshape(-1, G, 1, 8).astype(np.int64)[:, :, 0, :]     # [launch][CTA][8 stamps]
+t = raw[2:].reshape(-1, G, 8).astype(np.int64)     # [launch][CTA][8 stamps]
 per_step = 4 * L + 1
 recs = t[n_rec - per_step:n_rec]
 names = {2: "qkv", 0: "res", 1: "swiglu", 3: "logits"}

@@ -27,7 +27,7 @@
 // a few of the ring slots are in flight; per-row window copies make the copy engine the limit.
 //
 // Epilogues (RoPE + KV append, SwiGLU, residual, logits) and every rounding point are those of
-// gemv_tc.cu / gemv.cu (reference: transformers/models/llama/modeling_llama.py:124-168 RoPE, :171-184
+// gemv_tc.cu (reference: transformers/models/llama/modeling_llama.py:124-168 RoPE, :171-184
 // MLP, :325,331 residuals).
 #include "common.cuh"
 #include "kernels.h"
@@ -50,6 +50,7 @@ constexpr int TW_XWIN = 4;                             // activation windows in 
                                                        // an L2 round trip for a window every second chunk
 constexpr int TW_SMEM = TW_SLOTS * TW_SLOT_BYTES + TW_XWIN * TW_XBUF + 256;
 constexpr int TW_TILE = 16 * 17;                       // floats of one partial tile (16 rows x 16 clips, padded rows)
+constexpr int TW_NG_MAX = 14;                          // row groups per CTA of the largest instance (18 would spill)
 
 enum { TW_RES = 0, TW_SWIGLU = 1, TW_QKV = 2, TW_LOGITS = 3 };
 
@@ -305,23 +306,41 @@ TwParams tw_base(const GemvArgs& g, int mode) {
   return p;
 }
 
+// RES / LOGITS over more than 14 row groups per SM (the lm_head): consecutive launches over near-equal
+// row slices
 int tw_launch(const TwParams& p, cudaStream_t stream) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(device_num_sms());
-  cfg.blockDim = dim3(TW_THREADS);
-  cfg.dynamicSmemBytes = TW_SMEM;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  const int ng_max = ((p.N + 15) / 16 + (int)cfg.gridDim.x - 1) / (int)cfg.gridDim.x;     // groups of the busiest CTA
-  if (ng_max <= 2) VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tcw_kernel<2>, p));
-  else if (ng_max <= 6) VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tcw_kernel<6>, p));
-  else if (ng_max <= 10) VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tcw_kernel<10>, p));
-  else VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tcw_kernel<14>, p));
-  count_launches(1);
+  VCL_REQUIRE(gemv_tcw_fits(p.B, p.N, p.K, p.mode == TW_SWIGLU || p.mode == TW_QKV),
+              "gemv_tcw: B=%d N=%d K=%d is outside the kernel's range", p.B, p.N, p.K);
+  VCL_REQUIRE(p.W_tiled != nullptr && (uintptr_t)p.x % 16 == 0 && (uintptr_t)p.W_tiled % 16 == 0,
+              "gemv_tcw: operands must be 16-byte aligned");
+  const int groups = (p.N + 15) / 16, sms = device_num_sms();
+  const int n_slices = (groups + TW_NG_MAX * sms - 1) / (TW_NG_MAX * sms);
+  for (int s = 0; s < n_slices; ++s) {
+    const int g0 = (int)((long long)groups * s / n_slices), g1 = (int)((long long)groups * (s + 1) / n_slices);
+    const long long r0 = (long long)g0 * 16;
+    TwParams q = p;
+    q.W_tiled = p.W_tiled + r0 * p.K;
+    q.N = (p.N < g1 * 16 ? p.N : g1 * 16) - (int)r0;
+    if (q.out != nullptr) q.out += r0;
+    if (q.res != nullptr) q.res += r0;
+    if (q.logits != nullptr) q.logits += r0;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(g1 - g0 < sms ? g1 - g0 : sms);                  // no CTA without a row group
+    cfg.blockDim = dim3(TW_THREADS);
+    cfg.dynamicSmemBytes = TW_SMEM;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    const int ng_max = (g1 - g0 + (int)cfg.gridDim.x - 1) / (int)cfg.gridDim.x;     // groups of the busiest CTA
+    if (ng_max <= 2) VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tcw_kernel<2>, q));
+    else if (ng_max <= 6) VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tcw_kernel<6>, q));
+    else if (ng_max <= 10) VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tcw_kernel<10>, q));
+    else VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tcw_kernel<TW_NG_MAX>, q));
+    count_launches(1);
+  }
   return 0;
 }
 
@@ -331,29 +350,23 @@ int init_gemv_tcw_kernels() {
   VCL_CUDA_OK(cudaFuncSetAttribute(gemv_tcw_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
   VCL_CUDA_OK(cudaFuncSetAttribute(gemv_tcw_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
   VCL_CUDA_OK(cudaFuncSetAttribute(gemv_tcw_kernel<10>, cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
-  VCL_CUDA_OK(cudaFuncSetAttribute(gemv_tcw_kernel<14>, cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
+  VCL_CUDA_OK(cudaFuncSetAttribute(gemv_tcw_kernel<TW_NG_MAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
   return 0;
 }
 
-// 5..16 clips, a slot-ordered weight copy, between 1 and 14 row groups per CTA; g.x is in xwin layout
-bool gemv_tcw_supported(const GemvArgs& g) {
-  static const bool off = getenv("VCL_GEMV_TCW_OFF") != nullptr;   // A/B switch: fall back to gemv_mma
-  if (off || g.W_tiled == nullptr || g.norm_w != nullptr || g.B < 5 || g.B > 16) return false;
-  if (g.K % 32 != 0 || ((uintptr_t)g.x % 16) != 0 || ((uintptr_t)g.W_tiled % 16) != 0) return false;
-  const int n_groups = (g.N + 15) / 16, grid = device_num_sms();
-  return n_groups >= grid && n_groups <= 14 * grid;
+bool gemv_tcw_fits(int B, int N, int K, bool pairs) {
+  return B >= 5 && B <= 16 && N >= 1 && K % 32 == 0 && (!pairs || (N + 15) / 16 <= TW_NG_MAX * device_num_sms());
 }
 
 int launch_gemv_tcw_residual(const GemvArgs& g, bf16* out, long long ldo, const bf16* res, long long ldr,
                              cudaStream_t stream) {
-  VCL_REQUIRE(gemv_tcw_supported(g), "gemv_tcw: unsupported problem B=%d N=%d K=%d", g.B, g.N, g.K);
   TwParams p = tw_base(g, TW_RES);
   p.out = out; p.ldo = ldo; p.res = res; p.ldr = ldr;
   return tw_launch(p, stream);
 }
 
 int launch_gemv_tcw_swiglu(const GemvArgs& g, bf16* out, long long ldo, bool out_xwin, cudaStream_t stream) {
-  VCL_REQUIRE(gemv_tcw_supported(g) && g.N % 2 == 0, "gemv_tcw swiglu: unsupported problem B=%d N=%d K=%d", g.B, g.N, g.K);
+  VCL_REQUIRE(g.N % 2 == 0, "gemv_tcw swiglu: N must be even (interleaved gate/up rows)");
   TwParams p = tw_base(g, TW_SWIGLU);
   p.out = out; p.ldo = ldo; p.out_xwin = out_xwin ? 1 : 0;
   return tw_launch(p, stream);
@@ -362,7 +375,7 @@ int launch_gemv_tcw_swiglu(const GemvArgs& g, bf16* out, long long ldo, bool out
 int launch_gemv_tcw_qkv_rope(const GemvArgs& g, bf16* q_out, long long ldq, bf16* kcache, bf16* vcache,
                              const bf16* cos_t, const bf16* sin_t, int H, int s_max, int pos, cudaStream_t stream,
                              const int* pos_dev) {
-  VCL_REQUIRE(gemv_tcw_supported(g) && g.N == 3 * H * 128, "gemv_tcw qkv: unsupported problem B=%d N=%d K=%d", g.B, g.N, g.K);
+  VCL_REQUIRE(g.N == 3 * H * 128, "gemv_tcw qkv: N=%d != 3*H*128", g.N);
   TwParams p = tw_base(g, TW_QKV);
   p.q_out = q_out; p.ldq = ldq; p.kcache = kcache; p.vcache = vcache;
   p.cos_t = cos_t; p.sin_t = sin_t; p.H = H; p.s_max = s_max; p.pos = pos; p.pos_dev = pos_dev;
@@ -370,7 +383,6 @@ int launch_gemv_tcw_qkv_rope(const GemvArgs& g, bf16* q_out, long long ldq, bf16
 }
 
 int launch_gemv_tcw_logits(const GemvArgs& g, float* logits, long long ldl, cudaStream_t stream) {
-  VCL_REQUIRE(gemv_tcw_supported(g), "gemv_tcw logits: unsupported problem B=%d N=%d K=%d", g.B, g.N, g.K);
   TwParams p = tw_base(g, TW_LOGITS);
   p.logits = logits; p.ldl = ldl;
   return tw_launch(p, stream);

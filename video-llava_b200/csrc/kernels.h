@@ -119,22 +119,22 @@ int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, c
                             int kv_len, float scale, cudaStream_t stream, const int* pos_dev = nullptr,
                             bool o_xwin = false);   // o_xwin: the output [B][H*hd] is written in xwin layout
 
-// ---- gemv.cu : decode-time weight streaming (M = B <= 8 rows) ------------------------------------
+// ---- decode-time weight streaming (1..16 new tokens): gemv_tc.cu (1..4 clips), gemv_tcw.cu (5..16) ----
+// Both kernels read a decode-only copy of each matrix in slot order (launch_gemv_tc_repack below).
 // per-CTA partial arg-max of the logits kernel: the next step's q|k|v kernel reduces the grid's
 // partials itself (lowest index wins ties), so no arg-max kernel runs between two decode steps
 struct ArgmaxPart { float v; int idx; };
 
 struct GemvArgs {
-  const bf16* x = nullptr; long long ldx = 0;   // [B, K]
-  const bf16* W = nullptr;                      // [N, K]
-  const bf16* W_tiled = nullptr;                // optional decode-only tiled copy (gemv_tc.cu), B = 1
+  const bf16* x = nullptr; long long ldx = 0;   // [B][ldx] (gemv_tcw: xwin layout, see below)
+  const bf16* W_tiled = nullptr;                // slot-ordered copy of the [N, K] matrix
   int ring_slots = 0;                           // gemv_tc: deeper shared-memory ring than the default (0 = default)
   int B = 0, N = 0, K = 0;
-  const bf16* norm_w = nullptr; float eps = 0;  // optional fused RMSNorm prologue
+  const bf16* norm_w = nullptr; float eps = 0;  // gemv_tc: optional fused RMSNorm prologue
   // gemv_tc only. q|k|v with a fused token-embedding gather: x is row `token` of `embed` [vocab, K],
   // the token read from tok_in[b * tok_stride] or reduced from the previous step's arg-max partials
   // (amax_in [amax_n][B]); CTA 0 then stores the token (tok_out) and the raw row (h_out [B][K], the
-  // residual stream). Logits: amax_out [grid][B] receives the per-CTA partial arg-max.
+  // residual stream). Logits: amax_out [gemv_tc_grid(N)][B] receives the per-CTA partial arg-max.
   const bf16* embed = nullptr; int vocab = 0;
   const int* tok_in = nullptr; long long tok_stride = 0;
   const ArgmaxPart* amax_in = nullptr; int amax_n = 0;
@@ -142,62 +142,26 @@ struct GemvArgs {
   bf16* h_out = nullptr;
   ArgmaxPart* amax_out = nullptr;
 };
-// out[b, n] = bf16(bf16(x.W[n]) + res[b, n])      (res may alias out; res == null -> plain)
-int launch_gemv_residual(const GemvArgs& g, bf16* out, long long ldo, const bf16* res,
-                         long long ldr, cudaStream_t stream);
-// W rows interleaved (2j gate, 2j+1 up): out[b, j] = silu(gate)*up,  N = 2*F
-int launch_gemv_swiglu(const GemvArgs& g, bf16* out, long long ldo, cudaStream_t stream);
-// fused q/k/v projection + RoPE + cache write for one new token per clip at position pos
-int launch_gemv_qkv_rope(const GemvArgs& g, bf16* q_out, long long ldq, bf16* kcache, bf16* vcache,
-                         const bf16* cos_t, const bf16* sin_t, int H, int head_dim, int s_max,
-                         int pos, cudaStream_t stream, const int* pos_dev = nullptr);
-int init_gemv_kernels();
 
-// ---- gemv_tc.cu : 1..4 clips (bulk-copy ring over a slot-ordered weight copy + mma.sync) ---------
-// The launch_gemv_* entry points above route to these when gemv_tc_supported(g).
+// ---- gemv_tc.cu : 1..4 clips (bulk-copy ring over the slot-ordered copy + mma.sync), K <= 14336 ----
 int init_gemv_tc_kernels();
-enum { TC_MODE_RES = 0, TC_MODE_SWIGLU = 1, TC_MODE_QKV = 2, TC_MODE_LOGITS = 3 };
-struct TcPhase {
-  int mode = TC_MODE_RES;
-  const bf16* W_tiled = nullptr; int N = 0, K = 0;   // slot-ordered copy of the [N, K] matrix
-  const bf16* x = nullptr; long long ldx = 0;        // [B][ldx] input (written by the previous phase / kernel)
-  int B = 1;                                         // clips (1..4; chains of several phases: 1)
-  const bf16* norm_w = nullptr;                      // optional fused RMSNorm of x
-  int ring_slots = 0;                                // 0 = default ring depth
-  bf16* out = nullptr; long long ldo = 0;            // RES: out[B][N] (+res); SWIGLU: out[B][N/2]
-  const bf16* res = nullptr; long long ldr = 0;
-  bf16* q_out = nullptr; long long ldq = 0;          // QKV: q [B][ldq], cache base of the layer [B][H][S][128]
-  bf16* kcache = nullptr; bf16* vcache = nullptr;
-  float* logits = nullptr; long long ldl = 0;        // LOGITS: [B][ldl] bf16-rounded fp32 (null: not stored)
-  ArgmaxPart* amax_out = nullptr;                    // LOGITS: [grid][B] per-CTA partial arg-max
-  // QKV with a fused embedding gather (see GemvArgs)
-  const bf16* embed = nullptr; int vocab = 0;
-  const int* tok_in = nullptr; long long tok_stride = 0;
-  const ArgmaxPart* amax_in = nullptr; int amax_n = 0;
-  int* tok_out = nullptr; long long tok_out_stride = 0;
-  bf16* h_out = nullptr;
-};
-struct TcChainCommon {
-  float eps = 0.f;
-  const bf16* cos_t = nullptr; const bf16* sin_t = nullptr;
-  int H = 0, s_max = 0, pos = 0;
-  const int* pos_dev = nullptr;                      // position = pos + *pos_dev
-};
-bool gemv_tc_chain_supported(const TcPhase* ph, int n);
-int launch_gemv_tc_chain(const TcPhase* ph, int n, const TcChainCommon& c, cudaStream_t stream);
-bool gemv_tc_supported(const GemvArgs& g);
+// whether a [N, K] projection of B clips (norm: with the fused RMSNorm) fits the kernel's shared-memory plan
+bool gemv_tc_fits(int B, int N, int K, bool norm);
+int gemv_tc_grid(int N);                      // CTAs of a launch over N rows
 size_t gemv_tc_tiled_elems(int N, int K);     // elements of the tiled copy of an [N, K] matrix
 // qkv_pairs: rows are taken in the order of the fused q/k/v kernel (RoPE pairs adjacent)
 int launch_gemv_tc_repack(const bf16* W, bf16* dst, int N, int K, bool qkv_pairs, cudaStream_t stream);
+// out[b, n] = bf16(bf16(x.W[n]) + res[b, n])      (res may alias out; res == null -> plain)
 int launch_gemv_tc_residual(const GemvArgs& g, bf16* out, long long ldo, const bf16* res, long long ldr,
                             cudaStream_t stream);
+// W rows interleaved (2j gate, 2j+1 up): out[b, j] = silu(gate)*up,  N = 2*F
 int launch_gemv_tc_swiglu(const GemvArgs& g, bf16* out, long long ldo, cudaStream_t stream);
+// fused q/k/v projection + RoPE + cache write for one new token per clip at position pos
 int launch_gemv_tc_qkv_rope(const GemvArgs& g, bf16* q_out, long long ldq, bf16* kcache, bf16* vcache,
                             const bf16* cos_t, const bf16* sin_t, int H, int s_max, int pos, cudaStream_t stream,
                             const int* pos_dev = nullptr);
+// logits (bf16-rounded, stored fp32) [B, N]; logits == null: only the arg-max partials (g.amax_out)
 int launch_gemv_tc_logits(const GemvArgs& g, float* logits, long long ldl, cudaStream_t stream);
-// logits (bf16-rounded, stored fp32) [B, N]
-int launch_gemv_logits(const GemvArgs& g, float* logits, long long ldl, cudaStream_t stream);
 
 // ---- gemv_tcw.cu : 5..16 clips over the slot-ordered weight copy (chunk-major K walk); the activations
 // g.x are already normalised (norm_w must be null) and stored window-major ("xwin"): element (b, k) of a
@@ -210,7 +174,8 @@ inline size_t xwin_elems(int B, int K) { return (size_t)((K + XWIN_KC - 1) / XWI
 // y (xwin layout) = x [B][ldx] rows, RMS-normalised when w != null (LlamaRMSNorm rounding order)
 int launch_xwin_norm(const bf16* x, long long ldx, bf16* y, const bf16* w, int B, int K, float eps, cudaStream_t stream);
 int init_gemv_tcw_kernels();
-bool gemv_tcw_supported(const GemvArgs& g);
+// 5..16 clips, K a multiple of 32; pairs (q|k|v, gate|up): at most 14 row groups of 16 per SM
+bool gemv_tcw_fits(int B, int N, int K, bool pairs);
 int launch_gemv_tcw_residual(const GemvArgs& g, bf16* out, long long ldo, const bf16* res, long long ldr,
                              cudaStream_t stream);
 int launch_gemv_tcw_swiglu(const GemvArgs& g, bf16* out, long long ldo, bool out_xwin, cudaStream_t stream);
@@ -218,16 +183,5 @@ int launch_gemv_tcw_qkv_rope(const GemvArgs& g, bf16* q_out, long long ldq, bf16
                              const bf16* cos_t, const bf16* sin_t, int H, int s_max, int pos, cudaStream_t stream,
                              const int* pos_dev = nullptr);
 int launch_gemv_tcw_logits(const GemvArgs& g, float* logits, long long ldl, cudaStream_t stream);
-
-// ---- gemv_mma.cu : small-batch (2..16) decode projections on mma.sync, input already normalised ----
-int init_gemv_mma_kernels();
-int launch_gemv_mma_residual(const GemvArgs& g, bf16* out, long long ldo, const bf16* res, long long ldr,
-                             cudaStream_t stream);
-int launch_gemv_mma_swiglu(const GemvArgs& g, bf16* out, long long ldo, cudaStream_t stream);
-int launch_gemv_mma_qkv_rope(const GemvArgs& g, bf16* q_out, long long ldq, bf16* kcache, bf16* vcache,
-                             const bf16* cos_t, const bf16* sin_t, int H, int head_dim, int s_max, int pos,
-                             cudaStream_t stream, const int* pos_dev = nullptr);
-int launch_gemv_mma_logits(const GemvArgs& g, float* logits, long long ldl, cudaStream_t stream);
-
 
 }  // namespace vcl

@@ -46,7 +46,7 @@ struct ClipLayerW {
 };
 struct LlmLayerW {
   bf16 *ln1, *wqkv, *wo, *ln2, *wgu, *wd;
-  bf16 *wqkv_t = nullptr, *wo_t = nullptr, *wgu_t = nullptr, *wd_t = nullptr;   // tiled copies for B = 1 decode
+  bf16 *wqkv_t = nullptr, *wo_t = nullptr, *wgu_t = nullptr, *wd_t = nullptr;   // slot-ordered copies for decode
 };
 struct GraphEntry {
   int B, S, n_new;     // S = -1: the prompt length is read on the device (h->d_pos), any S replays it
@@ -98,7 +98,7 @@ struct vcl_handle {
   std::vector<GraphEntry> graphs;
   unsigned long long graph_clock = 0;
   int* d_pos = nullptr;                        // prompt length of the running decode loop (device scalar)
-  ArgmaxPart* amax = nullptr;                  // [#SMs][max_batch] per-CTA partial arg-max of the logits kernel
+  ArgmaxPart* amax = nullptr;                  // [gemv_tc_grid(vocab)][max_batch] per-CTA partial arg-max of the logits kernel
 
   size_t cache_layer_elems() const {
     return (size_t)cfg.max_batch * cfg.llm_heads * cfg.max_seq * 128;
@@ -192,6 +192,19 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   VCL_REQUIRE(c->clip_layers >= 0 && c->llm_layers >= 0 && c->vocab > 0, "vcl_create: bad layer/vocab counts");
   VCL_REQUIRE(c->max_frames > 0 && c->max_batch > 0 && c->max_seq > 0, "vcl_create: capacities must be > 0");
   VCL_REQUIRE(c->proj_type == VCL_PROJ_LINEAR || c->proj_type == VCL_PROJ_MLP2X_GELU, "vcl_create: proj_type");
+  {
+    // every decode projection must have a kernel for every clip count up to 16 (beyond: the GEMM)
+    const int D = c->llm_hidden, F = c->llm_inter;
+    const struct { const char* name; int N, K; bool norm, pairs; } mats[5] = {
+        {"q|k|v", 3 * D, D, true, true}, {"o_proj", D, D, false, false}, {"gate|up", 2 * F, D, true, true},
+        {"down_proj", D, F, false, false}, {"lm_head", c->vocab, D, true, false}};
+    for (int B = 1; B <= c->max_batch && B <= 16; ++B)
+      for (const auto& m : mats)
+        VCL_REQUIRE(B <= 4 ? gemv_tc_fits(B, m.N, m.K, m.norm) : gemv_tcw_fits(B, m.N, m.K, m.pairs),
+                    "vcl_create: the %s projection [%d x %d] has no decode kernel for %d clips (1..4 clips: K <= 14336 "
+                    "and the shared-memory plan; 5..16 clips: q|k|v and gate|up at most 14 row groups of 16 per SM)",
+                    m.name, m.N, m.K, B);
+  }
 
   vcl_handle* h = new vcl_handle();
   h->cfg = *c;
@@ -203,9 +216,7 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   int rc = 0;
   rc |= init_gemm_kernels();
   rc |= init_attention_kernels();
-  rc |= init_gemv_kernels();
   rc |= init_gemv_tc_kernels();
-  rc |= init_gemv_mma_kernels();
   rc |= init_gemv_tcw_kernels();
 
   const size_t C = c->clip_hidden, F = c->clip_inter;
@@ -362,20 +373,18 @@ int vcl_load_llm_weights(vcl_handle* h, const vcl_tensor* tensors, int n) {
                              cudaMemcpyDeviceToDevice));
     if (load_copy(h, m, lp + "mlp.down_proj.weight", &w.wd, 2, D, F)) return -1;
   }
-  // Decode-only second copy of every streamed matrix in the tile order of gemv_tc.cu (one bulk
-  // copy per 16 KB slot). 13.2 GB more for the 7B model, 25.7 GB for 13B - HBM is 180 GB.
-  if (getenv("VCL_NO_TILED_WEIGHTS") == nullptr && D % 32 == 0 && F % 32 == 0) {
-    auto tiled = [&](const bf16* src, bf16** dst, int N, int K, bool qkv) -> int {
-      if (dalloc(h, dst, gemv_tc_tiled_elems(N, K))) return -2;
-      return launch_gemv_tc_repack(src, *dst, N, K, qkv, nullptr);
-    };
-    for (int l = 0; l < c.llm_layers; ++l) {
-      LlmLayerW& w = h->ll[l];
-      if (tiled(w.wqkv, &w.wqkv_t, 3 * D, D, true) || tiled(w.wo, &w.wo_t, D, D, false) ||
-          tiled(w.wgu, &w.wgu_t, 2 * F, D, false) || tiled(w.wd, &w.wd_t, D, F, false)) return -2;
-    }
-    if (tiled(h->lm_head, &h->lm_head_t, V, D, false)) return -2;
+  // Decode-only second copy of every streamed matrix in the slot order of the decode kernels (one bulk
+  // copy per 16 KB slot, gemv_tc.cu). 13.2 GB more for the 7B model, 25.7 GB for 13B.
+  auto tiled = [&](const bf16* src, bf16** dst, int N, int K, bool qkv) -> int {
+    if (dalloc(h, dst, gemv_tc_tiled_elems(N, K))) return -2;
+    return launch_gemv_tc_repack(src, *dst, N, K, qkv, nullptr);
+  };
+  for (int l = 0; l < c.llm_layers; ++l) {
+    LlmLayerW& w = h->ll[l];
+    if (tiled(w.wqkv, &w.wqkv_t, 3 * D, D, true) || tiled(w.wo, &w.wo_t, D, D, false) ||
+        tiled(w.wgu, &w.wgu_t, 2 * F, D, false) || tiled(w.wd, &w.wd_t, D, F, false)) return -2;
   }
+  if (tiled(h->lm_head, &h->lm_head_t, V, D, false)) return -2;
   VCL_CUDA_OK(cudaDeviceSynchronize());
   h->llm_loaded = true;
   return 0;
@@ -437,54 +446,30 @@ int clip_forward(vcl_handle* h, const void* pixels, int fmt, int n_frames, int n
 bf16* kc_layer(vcl_handle* h, int l) { return h->kcache + (size_t)l * h->cache_layer_elems(); }
 bf16* vc_layer(vcl_handle* h, int l) { return h->vcache + (size_t)l * h->cache_layer_elems(); }
 
-// 1..4 clips take the ring-kernel family (gemv_tc, activation vectors of all clips in shared memory)
-// when every projection of the model fits its shared-memory plan; 5..16 clips use gemv_mma
-static bool tc_batch(vcl_handle* h, int B) {
-  if (B < 1 || B > 4 || h->lm_head_t == nullptr || h->ll.empty()) return false;
-  const vcl_config& c = h->cfg;
-  const int D = c.llm_hidden, F = c.llm_inter;
-  const int shapes[5][2] = {{3 * D, D}, {D, D}, {2 * F, D}, {D, F}, {c.vocab, D}};
-  for (const auto& nk : shapes) {
-    GemvArgs g;
-    g.x = h->d_h; g.ldx = nk[1]; g.W = h->lm_head; g.W_tiled = h->lm_head_t; g.B = B; g.N = nk[0]; g.K = nk[1];
-    if (!gemv_tc_supported(g)) return false;
-  }
-  return true;
-}
-
 // final RMSNorm + lm_head on rows x[b*ldx .. ] (b < B), arg-max
 // partials_out: the arg-max is left as per-CTA partials in h->amax for the next step's q|k|v kernel
 int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* logits_out,
                    int32_t* tok_out, long long tok_stride, cudaStream_t st, bool partials_out = false) {
   const vcl_config& c = h->cfg;
-  if (partials_out) {
-    GemvArgs g;
-    g.x = x; g.ldx = ldx; g.W = h->lm_head; g.W_tiled = h->lm_head_t; g.B = B; g.N = c.vocab;
-    g.K = c.llm_hidden; g.norm_w = h->norm_w; g.eps = c.rms_eps; g.amax_out = h->amax;
-    return launch_gemv_tc_logits(g, nullptr, c.vocab, st);
-  }
-  if (B >= 2 && !tc_batch(h, B)) {
-    // small batches: normalise the B rows once, then the mma.sync weight-streaming kernel
-    for (int b0 = 0; b0 < B; b0 += 16) {
-      const int nb = B - b0 < 16 ? B - b0 : 16;
-      GemvArgs g;
-      g.x = h->d_x; g.ldx = c.llm_hidden; g.W = h->lm_head; g.W_tiled = h->lm_head_t; g.B = nb; g.N = c.vocab; g.K = c.llm_hidden;
-      if (gemv_tcw_supported(g)) {
-        VCL_TRY(launch_xwin_norm(x + (long long)b0 * ldx, ldx, h->d_x, h->norm_w, nb, c.llm_hidden, c.rms_eps, st));
-        VCL_TRY(launch_gemv_tcw_logits(g, h->logits + (size_t)b0 * c.vocab, c.vocab, st));
-      } else {
-        VCL_TRY(launch_rmsnorm(x + (long long)b0 * ldx, ldx, h->d_x, c.llm_hidden, h->norm_w, nb, c.llm_hidden,
-                               c.rms_eps, st));
-        VCL_TRY(launch_gemv_mma_logits(g, h->logits + (size_t)b0 * c.vocab, c.vocab, st));
-      }
+  GemvArgs g;
+  g.W_tiled = h->lm_head_t; g.N = c.vocab; g.K = c.llm_hidden;
+  if (B <= 4) {
+    g.x = x; g.ldx = ldx; g.B = B; g.norm_w = h->norm_w; g.eps = c.rms_eps;
+    if (partials_out) {
+      g.amax_out = h->amax;
+      return launch_gemv_tc_logits(g, nullptr, c.vocab, st);
     }
-  } else
-  for (int b0 = 0; b0 < B; b0 += 4) {
-    const int nb = B - b0 < 4 ? B - b0 : 4;
-    GemvArgs g;
-    g.x = x + (long long)b0 * ldx; g.ldx = ldx; g.W = h->lm_head; g.W_tiled = h->lm_head_t; g.B = nb; g.N = c.vocab;
-    g.K = c.llm_hidden; g.norm_w = h->norm_w; g.eps = c.rms_eps;
-    VCL_TRY(launch_gemv_logits(g, h->logits + (size_t)b0 * c.vocab, c.vocab, st));
+    VCL_TRY(launch_gemv_tc_logits(g, h->logits, c.vocab, st));
+  } else {
+    // 5..16 clips per launch, the rows normalised into the window-major layout first; more clips are split
+    // into ceil(B / 16) near-equal chunks (at least 8 clips each)
+    const int n_chunks = (B + 15) / 16;
+    for (int i = 0; i < n_chunks; ++i) {
+      const int b0 = B * i / n_chunks, nb = B * (i + 1) / n_chunks - b0;
+      g.x = h->d_x; g.ldx = c.llm_hidden; g.B = nb;
+      VCL_TRY(launch_xwin_norm(x + (long long)b0 * ldx, ldx, h->d_x, h->norm_w, nb, c.llm_hidden, c.rms_eps, st));
+      VCL_TRY(launch_gemv_tcw_logits(g, h->logits + (size_t)b0 * c.vocab, c.vocab, st));
+    }
   }
   if (logits_out != nullptr && logits_out != h->logits)
     VCL_CUDA_OK(cudaMemcpyAsync(logits_out, h->logits, (size_t)B * c.vocab * sizeof(float),
@@ -581,72 +566,57 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
   const float scale = 0.08838834764831845f;
   const int* pd = io.pos_dev;
   VCL_REQUIRE(pos >= 0 && pos < c.max_seq, "decode position %d outside the cache (max_seq %d)", pos, c.max_seq);
-  const bool tc = tc_batch(h, B);
-  // On the ring-kernel path the embedding lookup is part of layer 0's q|k|v kernel (and with it the
-  // arg-max of the previous step); every other path gathers the rows with a kernel of its own.
-  const bool fused_embed = tc && c.llm_layers > 0;
-  VCL_REQUIRE(fused_embed || (!io.tok_from_partials && !io.partials_out), "partial arg-max hand-off needs the ring-kernel path");
+  // 1..4 clips: the embedding lookup is part of layer 0's q|k|v kernel (and with it the arg-max of the
+  // previous step); every other path gathers the rows with a kernel of its own.
+  const bool fused_embed = B <= 4 && c.llm_layers > 0;
+  VCL_REQUIRE(fused_embed || (!io.tok_from_partials && !io.partials_out), "partial arg-max hand-off needs 1..4 clips");
   if (!fused_embed) VCL_TRY(launch_embed_tokens(io.tok_in, io.in_stride, h->embed, h->d_h, B, D, c.vocab, st));
   for (int l = 0; l < c.llm_layers; ++l) {
     const LlmLayerW& w = h->ll[l];
-    if (B >= 2 && B <= 16 && !tc) {
-      GemvArgs g, go, gg, gd;
-      g.x = h->d_x; g.ldx = D; g.W = w.wqkv; g.W_tiled = w.wqkv_t; g.B = B; g.N = 3 * D; g.K = D;
-      go.x = h->d_attn; go.ldx = D; go.W = w.wo; go.W_tiled = w.wo_t; go.B = B; go.N = D; go.K = D;
-      gg.x = h->d_x; gg.ldx = D; gg.W = w.wgu; gg.W_tiled = w.wgu_t; gg.B = B; gg.N = 2 * F; gg.K = D;
-      gd.x = h->d_act; gd.ldx = F; gd.W = w.wd; gd.W_tiled = w.wd_t; gd.B = B; gd.N = D; gd.K = F;
-      if (gemv_tcw_supported(g) && gemv_tcw_supported(go) && gemv_tcw_supported(gg) && gemv_tcw_supported(gd)) {
-        // 5..16 clips: the ring kernel over the slot-ordered copy (gemv_tcw). Its inputs travel in the
-        // window-major layout (kernels.h: xwin), written by the norm, the attention kernel and its own
-        // SwiGLU epilogue; the residual stream d_h stays row-major.
-        VCL_TRY(launch_xwin_norm(h->d_h, D, h->d_x, w.ln1, B, D, c.rms_eps, st));
-        VCL_TRY(launch_gemv_tcw_qkv_rope(g, h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->rope_cos, h->rope_sin, H,
-                                         c.max_seq, pos, st, pd));
-        VCL_TRY(launch_decode_attention(h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->d_attn, D, B, H, 128,
-                                        c.max_seq, pos + 1, scale, st, pd, /*o_xwin=*/true));
-        VCL_TRY(launch_gemv_tcw_residual(go, h->d_h, D, h->d_h, D, st));
-        VCL_TRY(launch_xwin_norm(h->d_h, D, h->d_x, w.ln2, B, D, c.rms_eps, st));
-        VCL_TRY(launch_gemv_tcw_swiglu(gg, h->d_act, F, /*out_xwin=*/true, st));
-        VCL_TRY(launch_gemv_tcw_residual(gd, h->d_h, D, h->d_h, D, st));
-      } else {
-        // 2..4 clips without a slot-ordered copy, and shapes the ring kernels do not take: weights straight
-        // from global memory into MMA fragments (gemv_mma)
-        VCL_TRY(launch_rmsnorm(h->d_h, D, h->d_x, D, w.ln1, B, D, c.rms_eps, st));
-        VCL_TRY(launch_gemv_mma_qkv_rope(g, h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->rope_cos, h->rope_sin,
-                                         H, 128, c.max_seq, pos, st, pd));
-        VCL_TRY(launch_decode_attention(h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->d_attn, D, B, H, 128,
-                                        c.max_seq, pos + 1, scale, st, pd));
-        VCL_TRY(launch_gemv_mma_residual(go, h->d_h, D, h->d_h, D, st));
-        VCL_TRY(launch_rmsnorm(h->d_h, D, h->d_x, D, w.ln2, B, D, c.rms_eps, st));
-        VCL_TRY(launch_gemv_mma_swiglu(gg, h->d_act, F, st));
-        VCL_TRY(launch_gemv_mma_residual(gd, h->d_h, D, h->d_h, D, st));
-      }
-    } else if (B <= 4) {
+    if (B <= 4) {
       GemvArgs g;
-      g.x = h->d_h; g.ldx = D; g.W = w.wqkv; g.W_tiled = w.wqkv_t; g.B = B; g.N = 3 * D; g.K = D; g.norm_w = w.ln1; g.eps = c.rms_eps;
-      if (fused_embed && l == 0) {
+      g.x = h->d_h; g.ldx = D; g.W_tiled = w.wqkv_t; g.B = B; g.N = 3 * D; g.K = D; g.norm_w = w.ln1; g.eps = c.rms_eps;
+      if (l == 0) {
         g.x = nullptr; g.embed = h->embed; g.vocab = c.vocab; g.h_out = h->d_h;
         if (io.tok_from_partials) {
-          g.amax_in = h->amax; g.amax_n = device_num_sms(); g.tok_out = io.tok_store; g.tok_out_stride = io.store_stride;
+          g.amax_in = h->amax; g.amax_n = gemv_tc_grid(c.vocab); g.tok_out = io.tok_store; g.tok_out_stride = io.store_stride;
         } else {
           g.tok_in = io.tok_in; g.tok_stride = io.in_stride;
         }
       }
-      VCL_TRY(launch_gemv_qkv_rope(g, h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->rope_cos, h->rope_sin,
-                                   H, 128, c.max_seq, pos, st, pd));
+      VCL_TRY(launch_gemv_tc_qkv_rope(g, h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->rope_cos, h->rope_sin,
+                                      H, c.max_seq, pos, st, pd));
       VCL_TRY(launch_decode_attention(h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->d_attn, D, B, H, 128,
                                       c.max_seq, pos + 1, scale, st, pd));
       GemvArgs go;
-      go.x = h->d_attn; go.ldx = D; go.W = w.wo; go.W_tiled = w.wo_t; go.B = B; go.N = D; go.K = D;
+      go.x = h->d_attn; go.ldx = D; go.W_tiled = w.wo_t; go.B = B; go.N = D; go.K = D;
       static const int o_slots = getenv("VCL_OPROJ_SLOTS") ? atoi(getenv("VCL_OPROJ_SLOTS")) : 0;   // A/B switch
       go.ring_slots = o_slots;
-      VCL_TRY(launch_gemv_residual(go, h->d_h, D, h->d_h, D, st));
+      VCL_TRY(launch_gemv_tc_residual(go, h->d_h, D, h->d_h, D, st));
       GemvArgs gg;
-      gg.x = h->d_h; gg.ldx = D; gg.W = w.wgu; gg.W_tiled = w.wgu_t; gg.B = B; gg.N = 2 * F; gg.K = D; gg.norm_w = w.ln2; gg.eps = c.rms_eps;
-      VCL_TRY(launch_gemv_swiglu(gg, h->d_act, F, st));
+      gg.x = h->d_h; gg.ldx = D; gg.W_tiled = w.wgu_t; gg.B = B; gg.N = 2 * F; gg.K = D; gg.norm_w = w.ln2; gg.eps = c.rms_eps;
+      VCL_TRY(launch_gemv_tc_swiglu(gg, h->d_act, F, st));
       GemvArgs gd;
-      gd.x = h->d_act; gd.ldx = F; gd.W = w.wd; gd.W_tiled = w.wd_t; gd.B = B; gd.N = D; gd.K = F;
-      VCL_TRY(launch_gemv_residual(gd, h->d_h, D, h->d_h, D, st));
+      gd.x = h->d_act; gd.ldx = F; gd.W_tiled = w.wd_t; gd.B = B; gd.N = D; gd.K = F;
+      VCL_TRY(launch_gemv_tc_residual(gd, h->d_h, D, h->d_h, D, st));
+    } else if (B <= 16) {
+      // 5..16 clips: the wide ring kernel (gemv_tcw). Its inputs travel in the window-major layout
+      // (kernels.h: xwin), written by the norm, the attention kernel and its own SwiGLU epilogue; the
+      // residual stream d_h stays row-major.
+      GemvArgs g, go, gg, gd;
+      g.x = h->d_x; g.W_tiled = w.wqkv_t; g.B = B; g.N = 3 * D; g.K = D;
+      go.x = h->d_attn; go.W_tiled = w.wo_t; go.B = B; go.N = D; go.K = D;
+      gg.x = h->d_x; gg.W_tiled = w.wgu_t; gg.B = B; gg.N = 2 * F; gg.K = D;
+      gd.x = h->d_act; gd.W_tiled = w.wd_t; gd.B = B; gd.N = D; gd.K = F;
+      VCL_TRY(launch_xwin_norm(h->d_h, D, h->d_x, w.ln1, B, D, c.rms_eps, st));
+      VCL_TRY(launch_gemv_tcw_qkv_rope(g, h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->rope_cos, h->rope_sin, H,
+                                       c.max_seq, pos, st, pd));
+      VCL_TRY(launch_decode_attention(h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->d_attn, D, B, H, 128,
+                                      c.max_seq, pos + 1, scale, st, pd, /*o_xwin=*/true));
+      VCL_TRY(launch_gemv_tcw_residual(go, h->d_h, D, h->d_h, D, st));
+      VCL_TRY(launch_xwin_norm(h->d_h, D, h->d_x, w.ln2, B, D, c.rms_eps, st));
+      VCL_TRY(launch_gemv_tcw_swiglu(gg, h->d_act, F, /*out_xwin=*/true, st));
+      VCL_TRY(launch_gemv_tcw_residual(gd, h->d_h, D, h->d_h, D, st));
     } else {
       // B > 16: tensor-core path, the B new rows ride in one (mostly empty) 128-row tile and the
       // N tile is narrowed so that every SM streams a slice of the weights
@@ -667,11 +637,11 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
 }
 
 // Steps 1 .. n_new-1 of a greedy loop over the token scratch tk [B][n_new] (tk[:, 0] is given).
-// On the ring-kernel path no arg-max / embedding kernel runs between two steps: the logits kernel
-// leaves per-CTA partials, the next step's first q|k|v kernel reduces them, records the token and
-// gathers its embedding row.
+// For 1..4 clips no arg-max / embedding kernel runs between two steps: the logits kernel leaves
+// per-CTA partials, the next step's first q|k|v kernel reduces them, records the token and gathers
+// its embedding row.
 int decode_steps(vcl_handle* h, int32_t* tk, int B, int S, int n_new, const int* pos_dev, cudaStream_t st) {
-  const bool hand_off = tc_batch(h, B) && h->cfg.llm_layers > 0;
+  const bool hand_off = B <= 4 && h->cfg.llm_layers > 0;
   for (int i = 1; i < n_new; ++i) {
     StepIo io;
     io.pos_dev = pos_dev;
@@ -908,33 +878,33 @@ int vcl_op_attention_vit(const void* qkv, void* out, int n_frames, int S, int H,
 int vcl_op_gemv(const void* x, const void* W, void* out, const void* res, const void* norm_w,
                 float eps, int B, int N, int K, void* stream) {
   if (check_device() != 0) return -2;
+  VCL_REQUIRE(B >= 1 && B <= 16, "vcl_op_gemv: B=%d outside 1..16 (more rows take the GEMM)", B);
+  VCL_REQUIRE(B <= 4 ? gemv_tc_fits(B, N, K, norm_w != nullptr) : gemv_tcw_fits(B, N, K, false),
+              "vcl_op_gemv: B=%d N=%d K=%d is outside the decode kernels' range", B, N, K);
   static bool inited = false;
   if (!inited) {
-    VCL_TRY(init_gemv_kernels());
     VCL_TRY(init_gemv_tc_kernels());
     VCL_TRY(init_gemv_tcw_kernels());
     inited = true;
   }
   GemvArgs g;
-  g.x = reinterpret_cast<const bf16*>(x); g.ldx = K; g.W = reinterpret_cast<const bf16*>(W);
+  g.x = reinterpret_cast<const bf16*>(x); g.ldx = K;
   g.B = B; g.N = N; g.K = K; g.norm_w = reinterpret_cast<const bf16*>(norm_w); g.eps = eps;
-  // exercise the slot-ordered-copy kernels the decode loop uses. The copy is built here and kept for the
-  // next call with the same matrix (this entry point is a test / micro-benchmark hook, not a hot path).
+  // the decode kernels read the slot-ordered copy of the matrix. It is built here and kept for the next call
+  // with the same matrix (this entry point is a test / micro-benchmark hook, not a hot path); the copy is only
+  // REUSED when VCL_OP_GEMV_CACHE is set (tools/microbench.py), because a caller may hand in a different
+  // matrix at a recycled address
   static const void* c_W = nullptr; static int c_N = 0, c_K = 0; static bf16* c_tiled = nullptr;
-  if (B <= 16 && K % 32 == 0 && N >= 16 && getenv("VCL_GEMV_LEGACY") == nullptr) {
-    // (the copy is only REUSED when VCL_OP_GEMV_CACHE is set -- tools/microbench.py -- because a caller may
-    // hand in a different matrix at a recycled address)
-    if (c_W != W || c_N != N || c_K != K || getenv("VCL_OP_GEMV_CACHE") == nullptr) {
-      cudaStreamSynchronize(as_stream(stream));
-      if (c_tiled != nullptr) cudaFree(c_tiled);
-      c_tiled = nullptr; c_W = nullptr;
-      VCL_CUDA_OK(cudaMalloc(&c_tiled, gemv_tc_tiled_elems(N, K) * sizeof(bf16)));
-      const int rc0 = launch_gemv_tc_repack(g.W, c_tiled, N, K, false, as_stream(stream));
-      if (rc0 != 0) { cudaFree(c_tiled); c_tiled = nullptr; return rc0; }
-      c_W = W; c_N = N; c_K = K;
-    }
-    g.W_tiled = c_tiled;
+  if (c_W != W || c_N != N || c_K != K || getenv("VCL_OP_GEMV_CACHE") == nullptr) {
+    cudaStreamSynchronize(as_stream(stream));
+    if (c_tiled != nullptr) cudaFree(c_tiled);
+    c_tiled = nullptr; c_W = nullptr;
+    VCL_CUDA_OK(cudaMalloc(&c_tiled, gemv_tc_tiled_elems(N, K) * sizeof(bf16)));
+    const int rc0 = launch_gemv_tc_repack(reinterpret_cast<const bf16*>(W), c_tiled, N, K, false, as_stream(stream));
+    if (rc0 != 0) { cudaFree(c_tiled); c_tiled = nullptr; return rc0; }
+    c_W = W; c_N = N; c_K = K;
   }
+  g.W_tiled = c_tiled;
   if (B >= 5) {
     // 5..16 rows: the wide ring kernel; its input is normalised and re-laid out (xwin) by a launch of its own,
     // as on the decode path
@@ -947,10 +917,9 @@ int vcl_op_gemv(const void* x, const void* W, void* out, const void* res, const 
     }
     VCL_TRY(launch_xwin_norm(g.x, K, xn, g.norm_w, B, K, eps, as_stream(stream)));
     g.x = xn; g.norm_w = nullptr;
-    VCL_REQUIRE(gemv_tcw_supported(g), "vcl_op_gemv: B=%d N=%d K=%d is outside the wide ring kernel's range", B, N, K);
     return launch_gemv_tcw_residual(g, reinterpret_cast<bf16*>(out), N, reinterpret_cast<const bf16*>(res), N, as_stream(stream));
   }
-  return launch_gemv_residual(g, reinterpret_cast<bf16*>(out), N, reinterpret_cast<const bf16*>(res), N, as_stream(stream));
+  return launch_gemv_tc_residual(g, reinterpret_cast<bf16*>(out), N, reinterpret_cast<const bf16*>(res), N, as_stream(stream));
 }
 
 }  // extern "C"
