@@ -1,4 +1,4 @@
-"""Timeline of the per-matrix decode kernels (gemv_tc.cu) over one eager decode step (VCL_TC_TRACE)."""
+"""Timeline of the per-matrix decode kernels (gemv_tc_kernel, decode_gemv.cu) over one eager decode step (VCL_TC_TRACE)."""
 import ctypes
 import os
 import sys

@@ -20,8 +20,6 @@
 #include "common.cuh"
 #include "kernels.h"
 
-#include <stdlib.h>
-
 namespace vcl {
 
 namespace {
@@ -189,10 +187,8 @@ int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, c
   // shared memory is sized for the longest sequence when the length is only known on the device
   const int kv_cap = pos_dev != nullptr ? s_max : kv_len;
   // CTAs per head: enough CTAs to cover the SMs a few times over, no more
-  static const int forced = getenv("VCL_DA_SPLIT") ? atoi(getenv("VCL_DA_SPLIT")) : 0;      // A/B switch: 1, 2 or 4
   const int heads = B * H;
-  int split = heads <= 2 * device_num_sms() ? 4 : (heads <= 3 * device_num_sms() ? 2 : 1);
-  if (forced == 1 || forced == 2 || forced == 4) split = forced;
+  const int split = heads <= 2 * device_num_sms() ? 4 : (heads <= 3 * device_num_sms() ? 2 : 1);
   const int per = ((kv_cap + split - 1) / split + 15) / 16 * 16;   // keys per CTA, multiple of 16
   const size_t smem = (size_t)(per + 16 * 128 + 128 + 2 + 8) * sizeof(float);
   VCL_REQUIRE(smem <= 48 * 1024, "decode attention: kv_len %d too long for the smem budget", kv_len);

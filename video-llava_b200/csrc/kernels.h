@@ -119,22 +119,24 @@ int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, c
                             int kv_len, float scale, cudaStream_t stream, const int* pos_dev = nullptr,
                             bool o_xwin = false);   // o_xwin: the output [B][H*hd] is written in xwin layout
 
-// ---- decode-time weight streaming (1..16 new tokens): gemv_tc.cu (1..4 clips), gemv_tcw.cu (5..16) ----
-// Both kernels read a decode-only copy of each matrix in slot order (launch_gemv_tc_repack below).
+// ---- decode_gemv.cu : decode-time weight streaming (1..16 new tokens) -------------------------------
+// Two ring kernels (bulk-copy ring over a slot-ordered copy of the matrix + mma.sync) behind one launcher:
+// 1..4 clips stage the activation vectors in shared memory (K <= 14336, optional fused RMSNorm and, for
+// q|k|v, a fused token-embedding gather); 5..16 clips read activations that are already normalised and
+// stored window-major ("xwin", below). Both read the copy that launch_gemv_repack builds.
 // per-CTA partial arg-max of the logits kernel: the next step's q|k|v kernel reduces the grid's
 // partials itself (lowest index wins ties), so no arg-max kernel runs between two decode steps
 struct ArgmaxPart { float v; int idx; };
 
 struct GemvArgs {
-  const bf16* x = nullptr; long long ldx = 0;   // [B][ldx] (gemv_tcw: xwin layout, see below)
+  const bf16* x = nullptr; long long ldx = 0;   // [B][ldx] (5..16 clips: xwin layout, see below)
   const bf16* W_tiled = nullptr;                // slot-ordered copy of the [N, K] matrix
-  int ring_slots = 0;                           // gemv_tc: deeper shared-memory ring than the default (0 = default)
   int B = 0, N = 0, K = 0;
-  const bf16* norm_w = nullptr; float eps = 0;  // gemv_tc: optional fused RMSNorm prologue
-  // gemv_tc only. q|k|v with a fused token-embedding gather: x is row `token` of `embed` [vocab, K],
+  const bf16* norm_w = nullptr; float eps = 0;  // 1..4 clips: optional fused RMSNorm prologue
+  // 1..4 clips only. q|k|v with a fused token-embedding gather: x is row `token` of `embed` [vocab, K],
   // the token read from tok_in[b * tok_stride] or reduced from the previous step's arg-max partials
   // (amax_in [amax_n][B]); CTA 0 then stores the token (tok_out) and the raw row (h_out [B][K], the
-  // residual stream). Logits: amax_out [gemv_tc_grid(N)][B] receives the per-CTA partial arg-max.
+  // residual stream). Logits: amax_out [gemv_grid(N)][B] receives the per-CTA partial arg-max.
   const bf16* embed = nullptr; int vocab = 0;
   const int* tok_in = nullptr; long long tok_stride = 0;
   const ArgmaxPart* amax_in = nullptr; int amax_n = 0;
@@ -143,29 +145,28 @@ struct GemvArgs {
   ArgmaxPart* amax_out = nullptr;
 };
 
-// ---- gemv_tc.cu : 1..4 clips (bulk-copy ring over the slot-ordered copy + mma.sync), K <= 14336 ----
-int init_gemv_tc_kernels();
-// whether a [N, K] projection of B clips (norm: with the fused RMSNorm) fits the kernel's shared-memory plan
-bool gemv_tc_fits(int B, int N, int K, bool norm);
-int gemv_tc_grid(int N);                      // CTAs of a launch over N rows
-size_t gemv_tc_tiled_elems(int N, int K);     // elements of the tiled copy of an [N, K] matrix
-// qkv_pairs: rows are taken in the order of the fused q/k/v kernel (RoPE pairs adjacent)
-int launch_gemv_tc_repack(const bf16* W, bf16* dst, int N, int K, bool qkv_pairs, cudaStream_t stream);
-// out[b, n] = bf16(bf16(x.W[n]) + res[b, n])      (res may alias out; res == null -> plain)
-int launch_gemv_tc_residual(const GemvArgs& g, bf16* out, long long ldo, const bf16* res, long long ldr,
-                            cudaStream_t stream);
-// W rows interleaved (2j gate, 2j+1 up): out[b, j] = silu(gate)*up,  N = 2*F
-int launch_gemv_tc_swiglu(const GemvArgs& g, bf16* out, long long ldo, cudaStream_t stream);
-// fused q/k/v projection + RoPE + cache write for one new token per clip at position pos
-int launch_gemv_tc_qkv_rope(const GemvArgs& g, bf16* q_out, long long ldq, bf16* kcache, bf16* vcache,
-                            const bf16* cos_t, const bf16* sin_t, int H, int s_max, int pos, cudaStream_t stream,
-                            const int* pos_dev = nullptr);
-// logits (bf16-rounded, stored fp32) [B, N]; logits == null: only the arg-max partials (g.amax_out)
-int launch_gemv_tc_logits(const GemvArgs& g, float* logits, long long ldl, cudaStream_t stream);
+// what the projection's fused epilogue does with out[b][n] (the values are recorded by VCL_TC_TRACE)
+enum GemvMode {
+  GEMV_RES = 0,      // out[b, n] = bf16(bf16(x.W[n]) + res[b, n])   (res may alias out; res == null -> plain)
+  GEMV_SWIGLU = 1,   // W rows interleaved (2j gate, 2j+1 up): out[b, j] = silu(gate)*up,  N = 2*F
+  GEMV_QKV = 2,      // q|k|v projection + RoPE + cache write for one new token per clip, N = 3*H*128
+  GEMV_LOGITS = 3    // logits (bf16-rounded, stored fp32) [B, N]; logits == null: only the arg-max partials
+};
+struct GemvEpilogue {
+  int mode = GEMV_RES;
+  bf16* out = nullptr; long long ldo = 0;       // RES: out[B][ldo]; SWIGLU: out[B][ldo] ...
+  bool out_xwin = false;                        // ... or, 5..16 clips, in xwin layout (feeds down_proj)
+  const bf16* res = nullptr; long long ldr = 0; // RES
+  bf16* q_out = nullptr; long long ldq = 0;     // QKV: q [B][ldq], cache base of the layer [B][H][s_max][128]
+  bf16* kcache = nullptr; bf16* vcache = nullptr;
+  const bf16* cos_t = nullptr; const bf16* sin_t = nullptr;
+  int H = 0, s_max = 0, pos = 0;
+  const int* pos_dev = nullptr;                 // position = pos + *pos_dev
+  float* logits = nullptr; long long ldl = 0;   // LOGITS
+};
 
-// ---- gemv_tcw.cu : 5..16 clips over the slot-ordered weight copy (chunk-major K walk); the activations
-// g.x are already normalised (norm_w must be null) and stored window-major ("xwin"): element (b, k) of a
-// [B][K] activation lives at xwin_offset(b, k, B); a buffer holds xwin_elems(B, K) elements ----
+// xwin: element (b, k) of a [B][K] activation lives at xwin_offset(b, k, B); a buffer holds xwin_elems(B, K)
+// elements
 constexpr int XWIN_KC = 512, XWIN_PITCH = 544;        // 512 k per window row + 32 elements (64 B) of padding
 __host__ __device__ inline size_t xwin_offset(int b, int k, int B) {
   return ((size_t)(k / XWIN_KC) * B + b) * XWIN_PITCH + (k % XWIN_KC);
@@ -173,15 +174,17 @@ __host__ __device__ inline size_t xwin_offset(int b, int k, int B) {
 inline size_t xwin_elems(int B, int K) { return (size_t)((K + XWIN_KC - 1) / XWIN_KC) * B * XWIN_PITCH; }
 // y (xwin layout) = x [B][ldx] rows, RMS-normalised when w != null (LlamaRMSNorm rounding order)
 int launch_xwin_norm(const bf16* x, long long ldx, bf16* y, const bf16* w, int B, int K, float eps, cudaStream_t stream);
-int init_gemv_tcw_kernels();
-// 5..16 clips, K a multiple of 32; pairs (q|k|v, gate|up): at most 14 row groups of 16 per SM
-bool gemv_tcw_fits(int B, int N, int K, bool pairs);
-int launch_gemv_tcw_residual(const GemvArgs& g, bf16* out, long long ldo, const bf16* res, long long ldr,
-                             cudaStream_t stream);
-int launch_gemv_tcw_swiglu(const GemvArgs& g, bf16* out, long long ldo, bool out_xwin, cudaStream_t stream);
-int launch_gemv_tcw_qkv_rope(const GemvArgs& g, bf16* q_out, long long ldq, bf16* kcache, bf16* vcache,
-                             const bf16* cos_t, const bf16* sin_t, int H, int s_max, int pos, cudaStream_t stream,
-                             const int* pos_dev = nullptr);
-int launch_gemv_tcw_logits(const GemvArgs& g, float* logits, long long ldl, cudaStream_t stream);
+
+int init_gemv_kernels();
+// whether a [N, K] projection of B clips has a decode kernel. norm: with the fused RMSNorm (1..4 clips);
+// pairs: a SWIGLU or QKV epilogue (5..16 clips: such a matrix has at most 14 row groups of 16 per SM)
+bool gemv_fits(int B, int N, int K, bool norm, bool pairs);
+int gemv_grid(int N);                         // CTAs of a 1..4-clip launch over N rows
+size_t gemv_tiled_elems(int N, int K);        // elements of the slot-ordered copy of an [N, K] matrix
+// qkv_pairs: rows are taken in the order of the fused q/k/v epilogue (RoPE pairs adjacent)
+int launch_gemv_repack(const bf16* W, bf16* dst, int N, int K, bool qkv_pairs, cudaStream_t stream);
+// 1..4 clips: gemv_tc_kernel; 5..16 clips: gemv_tcw_kernel (several launches over row slices when a RES /
+// LOGITS matrix has more than 14 row groups per SM)
+int launch_gemv(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream);
 
 }  // namespace vcl

@@ -98,7 +98,7 @@ struct vcl_handle {
   std::vector<GraphEntry> graphs;
   unsigned long long graph_clock = 0;
   int* d_pos = nullptr;                        // prompt length of the running decode loop (device scalar)
-  ArgmaxPart* amax = nullptr;                  // [gemv_tc_grid(vocab)][max_batch] per-CTA partial arg-max of the logits kernel
+  ArgmaxPart* amax = nullptr;                  // [gemv_grid(vocab)][max_batch] per-CTA partial arg-max of the logits kernel
 
   size_t cache_layer_elems() const {
     return (size_t)cfg.max_batch * cfg.llm_heads * cfg.max_seq * 128;
@@ -200,7 +200,7 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
         {"down_proj", D, F, false, false}, {"lm_head", c->vocab, D, true, false}};
     for (int B = 1; B <= c->max_batch && B <= 16; ++B)
       for (const auto& m : mats)
-        VCL_REQUIRE(B <= 4 ? gemv_tc_fits(B, m.N, m.K, m.norm) : gemv_tcw_fits(B, m.N, m.K, m.pairs),
+        VCL_REQUIRE(gemv_fits(B, m.N, m.K, m.norm, m.pairs),
                     "vcl_create: the %s projection [%d x %d] has no decode kernel for %d clips (1..4 clips: K <= 14336 "
                     "and the shared-memory plan; 5..16 clips: q|k|v and gate|up at most 14 row groups of 16 per SM)",
                     m.name, m.N, m.K, B);
@@ -216,8 +216,7 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   int rc = 0;
   rc |= init_gemm_kernels();
   rc |= init_attention_kernels();
-  rc |= init_gemv_tc_kernels();
-  rc |= init_gemv_tcw_kernels();
+  rc |= init_gemv_kernels();
 
   const size_t C = c->clip_hidden, F = c->clip_inter;
   const size_t Mv = (size_t)c->max_frames * (h->P + 1);
@@ -374,10 +373,10 @@ int vcl_load_llm_weights(vcl_handle* h, const vcl_tensor* tensors, int n) {
     if (load_copy(h, m, lp + "mlp.down_proj.weight", &w.wd, 2, D, F)) return -1;
   }
   // Decode-only second copy of every streamed matrix in the slot order of the decode kernels (one bulk
-  // copy per 16 KB slot, gemv_tc.cu). 13.2 GB more for the 7B model, 25.7 GB for 13B.
+  // copy per 16 KB slot, decode_gemv.cu). 13.2 GB more for the 7B model, 25.7 GB for 13B.
   auto tiled = [&](const bf16* src, bf16** dst, int N, int K, bool qkv) -> int {
-    if (dalloc(h, dst, gemv_tc_tiled_elems(N, K))) return -2;
-    return launch_gemv_tc_repack(src, *dst, N, K, qkv, nullptr);
+    if (dalloc(h, dst, gemv_tiled_elems(N, K))) return -2;
+    return launch_gemv_repack(src, *dst, N, K, qkv, nullptr);
   };
   for (int l = 0; l < c.llm_layers; ++l) {
     LlmLayerW& w = h->ll[l];
@@ -453,13 +452,16 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
   const vcl_config& c = h->cfg;
   GemvArgs g;
   g.W_tiled = h->lm_head_t; g.N = c.vocab; g.K = c.llm_hidden;
+  GemvEpilogue e;
+  e.mode = GEMV_LOGITS; e.ldl = c.vocab;
   if (B <= 4) {
     g.x = x; g.ldx = ldx; g.B = B; g.norm_w = h->norm_w; g.eps = c.rms_eps;
     if (partials_out) {
       g.amax_out = h->amax;
-      return launch_gemv_tc_logits(g, nullptr, c.vocab, st);
+      return launch_gemv(g, e, st);
     }
-    VCL_TRY(launch_gemv_tc_logits(g, h->logits, c.vocab, st));
+    e.logits = h->logits;
+    VCL_TRY(launch_gemv(g, e, st));
   } else {
     // 5..16 clips per launch, the rows normalised into the window-major layout first; more clips are split
     // into ceil(B / 16) near-equal chunks (at least 8 clips each)
@@ -468,7 +470,8 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
       const int b0 = B * i / n_chunks, nb = B * (i + 1) / n_chunks - b0;
       g.x = h->d_x; g.ldx = c.llm_hidden; g.B = nb;
       VCL_TRY(launch_xwin_norm(x + (long long)b0 * ldx, ldx, h->d_x, h->norm_w, nb, c.llm_hidden, c.rms_eps, st));
-      VCL_TRY(launch_gemv_tcw_logits(g, h->logits + (size_t)b0 * c.vocab, c.vocab, st));
+      e.logits = h->logits + (size_t)b0 * c.vocab;
+      VCL_TRY(launch_gemv(g, e, st));
     }
   }
   if (logits_out != nullptr && logits_out != h->logits)
@@ -573,50 +576,52 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
   if (!fused_embed) VCL_TRY(launch_embed_tokens(io.tok_in, io.in_stride, h->embed, h->d_h, B, D, c.vocab, st));
   for (int l = 0; l < c.llm_layers; ++l) {
     const LlmLayerW& w = h->ll[l];
-    if (B <= 4) {
+    if (B <= 16) {
+      // the ring kernels. 1..4 clips fuse the RMSNorm into the projection (and, in layer 0, the embedding
+      // gather); 5..16 clips take their inputs window-major (kernels.h: xwin), written by launch_xwin_norm,
+      // the attention kernel and the SwiGLU epilogue. The residual stream d_h stays row-major.
+      const bool wide = B > 4;
+      auto normed = [&](GemvArgs& g, const bf16* ln) -> int {
+        g.ldx = D;
+        if (wide) {
+          g.x = h->d_x;
+          return launch_xwin_norm(h->d_h, D, h->d_x, ln, B, D, c.rms_eps, st);
+        }
+        g.x = h->d_h; g.norm_w = ln; g.eps = c.rms_eps;
+        return 0;
+      };
+      GemvEpilogue residual;
+      residual.mode = GEMV_RES; residual.out = h->d_h; residual.ldo = D; residual.res = h->d_h; residual.ldr = D;
+
       GemvArgs g;
-      g.x = h->d_h; g.ldx = D; g.W_tiled = w.wqkv_t; g.B = B; g.N = 3 * D; g.K = D; g.norm_w = w.ln1; g.eps = c.rms_eps;
-      if (l == 0) {
+      g.W_tiled = w.wqkv_t; g.B = B; g.N = 3 * D; g.K = D;
+      VCL_TRY(normed(g, w.ln1));
+      if (fused_embed && l == 0) {
         g.x = nullptr; g.embed = h->embed; g.vocab = c.vocab; g.h_out = h->d_h;
         if (io.tok_from_partials) {
-          g.amax_in = h->amax; g.amax_n = gemv_tc_grid(c.vocab); g.tok_out = io.tok_store; g.tok_out_stride = io.store_stride;
+          g.amax_in = h->amax; g.amax_n = gemv_grid(c.vocab); g.tok_out = io.tok_store; g.tok_out_stride = io.store_stride;
         } else {
           g.tok_in = io.tok_in; g.tok_stride = io.in_stride;
         }
       }
-      VCL_TRY(launch_gemv_tc_qkv_rope(g, h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->rope_cos, h->rope_sin,
-                                      H, c.max_seq, pos, st, pd));
+      GemvEpilogue qkv;
+      qkv.mode = GEMV_QKV; qkv.q_out = h->d_q; qkv.ldq = D; qkv.kcache = kc_layer(h, l); qkv.vcache = vc_layer(h, l);
+      qkv.cos_t = h->rope_cos; qkv.sin_t = h->rope_sin; qkv.H = H; qkv.s_max = c.max_seq; qkv.pos = pos; qkv.pos_dev = pd;
+      VCL_TRY(launch_gemv(g, qkv, st));
       VCL_TRY(launch_decode_attention(h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->d_attn, D, B, H, 128,
-                                      c.max_seq, pos + 1, scale, st, pd));
+                                      c.max_seq, pos + 1, scale, st, pd, /*o_xwin=*/wide));
       GemvArgs go;
       go.x = h->d_attn; go.ldx = D; go.W_tiled = w.wo_t; go.B = B; go.N = D; go.K = D;
-      static const int o_slots = getenv("VCL_OPROJ_SLOTS") ? atoi(getenv("VCL_OPROJ_SLOTS")) : 0;   // A/B switch
-      go.ring_slots = o_slots;
-      VCL_TRY(launch_gemv_tc_residual(go, h->d_h, D, h->d_h, D, st));
+      VCL_TRY(launch_gemv(go, residual, st));
       GemvArgs gg;
-      gg.x = h->d_h; gg.ldx = D; gg.W_tiled = w.wgu_t; gg.B = B; gg.N = 2 * F; gg.K = D; gg.norm_w = w.ln2; gg.eps = c.rms_eps;
-      VCL_TRY(launch_gemv_tc_swiglu(gg, h->d_act, F, st));
+      gg.W_tiled = w.wgu_t; gg.B = B; gg.N = 2 * F; gg.K = D;
+      VCL_TRY(normed(gg, w.ln2));
+      GemvEpilogue swiglu;
+      swiglu.mode = GEMV_SWIGLU; swiglu.out = h->d_act; swiglu.ldo = F; swiglu.out_xwin = wide;
+      VCL_TRY(launch_gemv(gg, swiglu, st));
       GemvArgs gd;
       gd.x = h->d_act; gd.ldx = F; gd.W_tiled = w.wd_t; gd.B = B; gd.N = D; gd.K = F;
-      VCL_TRY(launch_gemv_tc_residual(gd, h->d_h, D, h->d_h, D, st));
-    } else if (B <= 16) {
-      // 5..16 clips: the wide ring kernel (gemv_tcw). Its inputs travel in the window-major layout
-      // (kernels.h: xwin), written by the norm, the attention kernel and its own SwiGLU epilogue; the
-      // residual stream d_h stays row-major.
-      GemvArgs g, go, gg, gd;
-      g.x = h->d_x; g.W_tiled = w.wqkv_t; g.B = B; g.N = 3 * D; g.K = D;
-      go.x = h->d_attn; go.W_tiled = w.wo_t; go.B = B; go.N = D; go.K = D;
-      gg.x = h->d_x; gg.W_tiled = w.wgu_t; gg.B = B; gg.N = 2 * F; gg.K = D;
-      gd.x = h->d_act; gd.W_tiled = w.wd_t; gd.B = B; gd.N = D; gd.K = F;
-      VCL_TRY(launch_xwin_norm(h->d_h, D, h->d_x, w.ln1, B, D, c.rms_eps, st));
-      VCL_TRY(launch_gemv_tcw_qkv_rope(g, h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->rope_cos, h->rope_sin, H,
-                                       c.max_seq, pos, st, pd));
-      VCL_TRY(launch_decode_attention(h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->d_attn, D, B, H, 128,
-                                      c.max_seq, pos + 1, scale, st, pd, /*o_xwin=*/true));
-      VCL_TRY(launch_gemv_tcw_residual(go, h->d_h, D, h->d_h, D, st));
-      VCL_TRY(launch_xwin_norm(h->d_h, D, h->d_x, w.ln2, B, D, c.rms_eps, st));
-      VCL_TRY(launch_gemv_tcw_swiglu(gg, h->d_act, F, /*out_xwin=*/true, st));
-      VCL_TRY(launch_gemv_tcw_residual(gd, h->d_h, D, h->d_h, D, st));
+      VCL_TRY(launch_gemv(gd, residual, st));
     } else {
       // B > 16: tensor-core path, the B new rows ride in one (mostly empty) 128-row tile and the
       // N tile is narrowed so that every SM streams a slice of the weights
@@ -879,12 +884,11 @@ int vcl_op_gemv(const void* x, const void* W, void* out, const void* res, const 
                 float eps, int B, int N, int K, void* stream) {
   if (check_device() != 0) return -2;
   VCL_REQUIRE(B >= 1 && B <= 16, "vcl_op_gemv: B=%d outside 1..16 (more rows take the GEMM)", B);
-  VCL_REQUIRE(B <= 4 ? gemv_tc_fits(B, N, K, norm_w != nullptr) : gemv_tcw_fits(B, N, K, false),
+  VCL_REQUIRE(gemv_fits(B, N, K, norm_w != nullptr, false),
               "vcl_op_gemv: B=%d N=%d K=%d is outside the decode kernels' range", B, N, K);
   static bool inited = false;
   if (!inited) {
-    VCL_TRY(init_gemv_tc_kernels());
-    VCL_TRY(init_gemv_tcw_kernels());
+    VCL_TRY(init_gemv_kernels());
     inited = true;
   }
   GemvArgs g;
@@ -899,12 +903,14 @@ int vcl_op_gemv(const void* x, const void* W, void* out, const void* res, const 
     cudaStreamSynchronize(as_stream(stream));
     if (c_tiled != nullptr) cudaFree(c_tiled);
     c_tiled = nullptr; c_W = nullptr;
-    VCL_CUDA_OK(cudaMalloc(&c_tiled, gemv_tc_tiled_elems(N, K) * sizeof(bf16)));
-    const int rc0 = launch_gemv_tc_repack(reinterpret_cast<const bf16*>(W), c_tiled, N, K, false, as_stream(stream));
+    VCL_CUDA_OK(cudaMalloc(&c_tiled, gemv_tiled_elems(N, K) * sizeof(bf16)));
+    const int rc0 = launch_gemv_repack(reinterpret_cast<const bf16*>(W), c_tiled, N, K, false, as_stream(stream));
     if (rc0 != 0) { cudaFree(c_tiled); c_tiled = nullptr; return rc0; }
     c_W = W; c_N = N; c_K = K;
   }
   g.W_tiled = c_tiled;
+  GemvEpilogue e;
+  e.mode = GEMV_RES; e.out = reinterpret_cast<bf16*>(out); e.ldo = N; e.res = reinterpret_cast<const bf16*>(res); e.ldr = N;
   if (B >= 5) {
     // 5..16 rows: the wide ring kernel; its input is normalised and re-laid out (xwin) by a launch of its own,
     // as on the decode path
@@ -917,9 +923,8 @@ int vcl_op_gemv(const void* x, const void* W, void* out, const void* res, const 
     }
     VCL_TRY(launch_xwin_norm(g.x, K, xn, g.norm_w, B, K, eps, as_stream(stream)));
     g.x = xn; g.norm_w = nullptr;
-    return launch_gemv_tcw_residual(g, reinterpret_cast<bf16*>(out), N, reinterpret_cast<const bf16*>(res), N, as_stream(stream));
   }
-  return launch_gemv_tc_residual(g, reinterpret_cast<bf16*>(out), N, reinterpret_cast<const bf16*>(res), N, as_stream(stream));
+  return launch_gemv(g, e, as_stream(stream));
 }
 
 }  // extern "C"
