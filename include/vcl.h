@@ -130,6 +130,24 @@ int vcl_llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats,
                     float* logits_out, int32_t* next_tok, void* stream);
 #define VCL_NO_VIDEO (-2147483647 - 1)
 
+/* vcl_llm_prefill for a batch of prompts of different lengths, left-padded to one length S (HF's
+ * tokenizer with padding_side="left" and its attention_mask). n_pad_host [B] int32 in HOST memory: row b
+ * starts with n_pad_host[b] pad ids (0 <= n_pad_host[b] < S, checked), its real tokens fill columns
+ * n_pad_host[b] .. S-1. Every clip is computed as if it ran alone: cache column c holds the token at RoPE
+ * position c - n_pad_host[b], and a real query attends keys n_pad_host[b] .. its own column only. The outputs
+ * of pad rows (hidden_out) are finite but unspecified; logits / next token come from column S-1 as in
+ * vcl_llm_prefill. vid_start[b] stays a column of the padded row, and the video span must lie inside the real
+ * tokens. The pad ids are looked up like any other id, so they must be valid (< vocab).
+ *
+ * Padding state. The pad counts describe the KV cache, and the handle keeps them (in a device array of
+ * max_batch entries): vcl_llm_prefill_padded / vcl_llm_generate_padded set them, vcl_llm_prefill,
+ * vcl_llm_prefill_states and vcl_llm_generate clear them, and vcl_llm_prefill_append, vcl_llm_decode_step and
+ * vcl_llm_decode_loop continue whatever padding the cache has. All-zero pad counts are no padding: the call is
+ * then exactly vcl_llm_prefill. */
+int vcl_llm_prefill_padded(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
+                           const int32_t* n_pad_host, int B, int S, int n_layers, void* hidden_out,
+                           float* logits_out, int32_t* next_tok, void* stream);
+
 /* forward(..., output_hidden_states=True) (video_chatgpt/model/video_chatgpt.py:205-218): the same
  * full-depth prefill, keeping every hidden state: states_out is [llm_layers + 1][B][S][D] bf16, entry i
  * = the raw output of decoder layer i (entry 0: the spliced input embeddings). HF returns the LAST
@@ -144,13 +162,16 @@ int vcl_llm_prefill_states(vcl_handle* h, const int64_t* ids, const void* video_
  * whole prompt on every turn (video_chatgpt/chat.py:137-154, inference.py:86-112); with the cache of
  * the previous turn only the new question is prefilled. Outputs as in vcl_llm_prefill (hidden_out
  * [B,S,D] of the new positions; logits / next token at the last new position). start_pos must be the
- * number of positions the cache of every clip already holds (> 0). */
+ * number of positions the cache of every clip already holds (> 0). A left-padded cache
+ * (vcl_llm_prefill_padded) stays padded: the new tokens continue each clip's RoPE positions and do not attend
+ * to its pad columns; start_pos must lie past the padding. */
 int vcl_llm_prefill_append(vcl_handle* h, const int64_t* ids, int B, int S, int start_pos, void* hidden_out,
                            float* logits_out, int32_t* next_tok, void* stream);
 
 /* One cached decoding step (the `input_ids.shape[1] == 1` branch, model/video_chatgpt.py:103,
  * 253-257): tok_in [B] int32 are fed at position `pos` (= tokens already in the cache).
- * logits_out / tok_out as above. Used for teacher-forced parity checks. */
+ * logits_out / tok_out as above. Used for teacher-forced parity checks. After a padded prefill the step
+ * continues the padding (RoPE position pos - n_pad[b], pad keys not read); pos must lie past the padding. */
 int vcl_llm_decode_step(vcl_handle* h, const int32_t* tok_in, int B, int pos, float* logits_out,
                         int32_t* tok_out, void* stream);
 
@@ -169,9 +190,16 @@ int vcl_llm_generate(vcl_handle* h, const int64_t* ids, const void* video_feats,
 
 /* The decode half of vcl_llm_generate on its own (so a caller can time prefill and decode
  * separately): first_tok [B] int32 is the token produced by the prefill; runs n_new-1 cached steps
- * at positions S, S+1, ... and writes [B, n_new] (first_tok included) to out_tokens. */
+ * at positions S, S+1, ... and writes [B, n_new] (first_tok included) to out_tokens. It continues the
+ * cache's left padding, if any; the graph cache is keyed by (B, n_new, padded or not), and one padded graph
+ * serves every set of pad counts (they are read from device memory). */
 int vcl_llm_decode_loop(vcl_handle* h, const int32_t* first_tok, int B, int S, int n_new,
                         int32_t* out_tokens, void* stream);
+
+/* vcl_llm_generate for a left-padded batch: vcl_llm_prefill_padded + vcl_llm_decode_loop (padding as
+ * described at vcl_llm_prefill_padded; out_tokens [B, n_new] int32, new tokens only). */
+int vcl_llm_generate_padded(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
+                            const int32_t* n_pad_host, int B, int S, int n_new, int32_t* out_tokens, void* stream);
 
 /* Number of kernels of this library launched so far in the process (CUDA-graph replays count the
  * kernel nodes they contain). Evidence for bench.py's "gpu_launches". */

@@ -74,7 +74,10 @@ __device__ __forceinline__ void load_tile(uint32_t sbase, const bf16* g, long lo
   }
 }
 
-template <int HD, bool CAUSAL>
+// PAD (causal only): left-padded clips (a.n_pad): a real query (cache column >= n_pad[b]) attends keys n_pad[b] ..
+// its own column, and a tile of real queries starts at the first key tile that holds a real key; a pad query
+// attends causally
+template <int HD, bool CAUSAL, bool PAD = false>
 __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
   extern __shared__ __align__(128) uint8_t smem[];
   constexpr int TILE_BYTES = 64 * HD * 2;
@@ -94,10 +97,12 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
 
   const int n_tiles_all = (S_kv + 63) / 64;
   const int n_tiles = CAUSAL ? min(n_tiles_all, (q_off + q0 + 63) / 64 + 1) : n_tiles_all;
+  const int k_pad = PAD ? __ldg(a.n_pad + b) : 0;                    // first real key of the clip
+  const int jt0 = (PAD && q_off + q0 >= k_pad) ? k_pad / 64 : 0;     // key tiles below hold pad keys only
 
   load_tile<HD>(sQ, qg, a.q_ss, q0, S);
-  load_tile<HD>(sK, kg, a.k_ss, 0, S_kv);
-  load_tile<HD>(sV, vg, a.v_ss, 0, S_kv);
+  load_tile<HD>(sK, kg, a.k_ss, jt0 * 64, S_kv);
+  load_tile<HD>(sV, vg, a.v_ss, jt0 * 64, S_kv);
   cp_async_commit();
 
   uint32_t qf[HD / 16][4];
@@ -108,9 +113,14 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
   float l_run[2] = {0.f, 0.f};
   const float scale = a.scale;
   const int qrow0 = q0 + warp * 16 + (lane >> 2);  // rows qrow0 and qrow0 + 8
+  int kmin[2] = {0, 0};                             // key floor of the two rows
+  if constexpr (PAD) {
+    kmin[0] = qrow0 + q_off >= k_pad ? k_pad : 0;
+    kmin[1] = qrow0 + 8 + q_off >= k_pad ? k_pad : 0;
+  }
 
-  for (int jt = 0; jt < n_tiles; ++jt) {
-    const int buf = jt & 1;
+  for (int jt = jt0; jt < n_tiles; ++jt) {
+    const int buf = (jt - jt0) & 1;
     if (jt + 1 < n_tiles) {
       load_tile<HD>(sK + (buf ^ 1) * TILE_BYTES, kg, a.k_ss, (jt + 1) * 64, S_kv);
       load_tile<HD>(sV + (buf ^ 1) * TILE_BYTES, vg, a.v_ss, (jt + 1) * 64, S_kv);
@@ -121,7 +131,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
     }
     __syncthreads();
 
-    if (jt == 0) {
+    if (jt == jt0) {
 #pragma unroll
       for (int kk = 0; kk < HD / 16; ++kk) {
         const int r = warp * 16 + (lane & 15);
@@ -160,6 +170,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
         const int qrow = qrow0 + (e >> 1) * 8;
         float x = bf16r(bf16r(s[nb][e]) * scale);
         if (kidx >= S_kv || (CAUSAL && kidx > qrow + q_off)) x = -INFINITY;
+        if (PAD && kidx < kmin[e >> 1]) x = -INFINITY;
         s[nb][e] = x;
         mx[e >> 1] = fmaxf(mx[e >> 1], x);
       }
@@ -236,10 +247,10 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
   }
 }
 
-template <int HD, bool CAUSAL>
+template <int HD, bool CAUSAL, bool PAD = false>
 int launch_attn_t(const AttnArgs& a, cudaStream_t stream) {
   constexpr int SMEM = 5 * 64 * HD * 2;
-  auto kern = attn_fwd_kernel<HD, CAUSAL>;
+  auto kern = attn_fwd_kernel<HD, CAUSAL, PAD>;
   dim3 grid((a.S + 63) / 64, a.H, a.B);
   kern<<<grid, 128, SMEM, stream>>>(a);
   VCL_CUDA_OK(cudaGetLastError());
@@ -254,6 +265,7 @@ int init_attention_kernels() {
   VCL_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 64 * 64 * 2));
   VCL_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 64 * 128 * 2));
   VCL_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 64 * 128 * 2));
+  VCL_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<128, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 64 * 128 * 2));
   if (init_attention_tc_kernels() != 0) return -2;
   return init_attention_prefill_tc_kernels();
 }
@@ -264,8 +276,10 @@ int launch_attention(const AttnArgs& a, cudaStream_t stream) {
                   a.k_sh % 8 == 0 && a.v_sh % 8 == 0 && a.q_sb % 8 == 0 && a.k_sb % 8 == 0 &&
                   a.v_sb % 8 == 0 && a.o_ss % 2 == 0 && a.o_sh % 2 == 0 && a.o_sb % 2 == 0,
               "attention: strides must keep 16-byte row alignment");
+  VCL_REQUIRE(a.n_pad == nullptr || (a.causal && a.head_dim == 128), "attention: left padding needs causal hd-128 attention");
   if (a.B <= 0 || a.H <= 0 || a.S <= 0) return 0;
   if (attention_prefill_tc_supported(a)) return launch_attention_prefill_tc(a, stream);   // LLaMA prefill up to 512 keys
+  if (a.n_pad != nullptr) return launch_attn_t<128, true, true>(a, stream);
   if (a.head_dim == 64) {
     return a.causal ? launch_attn_t<64, true>(a, stream) : launch_attn_t<64, false>(a, stream);
   }

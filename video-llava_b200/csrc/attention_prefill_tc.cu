@@ -84,6 +84,9 @@ __device__ __forceinline__ void pa_mma(float (&acc)[64], uint32_t a_base, int a_
   wgmma_fence_regs(acc);
 }
 
+// PAD: left-padded clips (a.n_pad): a real query (cache column >= n_pad[b]) attends keys n_pad[b] .. its own column,
+// and a tile of real queries starts at the first key block that holds a real key; a pad query attends causally
+template <bool PAD>
 __global__ void __launch_bounds__(PA_THREADS)
 attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
   extern __shared__ uint8_t smem_raw[];
@@ -101,6 +104,8 @@ attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
   // key blocks this tile touches: keys up to the absolute position of its last query
   const int last_key = min(S_kv - 1, a.q_off + min(q0 + 63, a.S - 1));
   const int n_kb = last_key / 128 + 1;
+  const int k_pad = PAD ? __ldg(a.n_pad + b) : 0;                  // first real key of the clip
+  const int kb0 = (PAD && a.q_off + q0 >= k_pad) ? k_pad / 128 : 0;   // key blocks below hold pad keys only
 
   pa_load_rows<64>(smem + PA_OFF_Q, qg, a.q_ss, q0, a.S);
 
@@ -108,18 +113,24 @@ attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
   int qpos[2];                                           // absolute positions of this thread's two rows
   qpos[0] = a.q_off + q0 + r0;
   qpos[1] = qpos[0] + 8;
+  int kmin[2] = {0, 0};                                  // key floor of the two rows
+  if constexpr (PAD) {
+    kmin[0] = qpos[0] >= k_pad ? k_pad : 0;
+    kmin[1] = qpos[1] >= k_pad ? k_pad : 0;
+  }
   const float scale = a.scale;
   float acc[64] = {};
   // scaled, rounded, masked score of accumulator element i of key block kb (reference rounding points)
   auto score = [&](int kb, int i) {
     const int key = kb * 128 + 8 * (i >> 2) + c2 + (i & 1);
     const float x = bf16r(bf16r(acc[i]) * scale);
+    if (PAD && key < kmin[(i >> 1) & 1]) return -INFINITY;
     return (key >= S_kv || key > qpos[(i >> 1) & 1]) ? -INFINITY : x;
   };
 
   // ---- pass 1: row maxima over every key block ----
   float m[2] = {-INFINITY, -INFINITY};
-  for (int kb = 0; kb < n_kb; ++kb) {
+  for (int kb = kb0; kb < n_kb; ++kb) {
     __syncthreads();                                     // previous readers of K are done
     pa_load_rows<128>(smem + PA_OFF_K, kg, a.k_ss, kb * 128, S_kv);
     fence_async_smem();
@@ -138,7 +149,7 @@ attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
   // ---- pass 2: P against the final maximum, O += P . V ----
   float o[64] = {};
   float l[2] = {0.f, 0.f};
-  for (int kb = 0; kb < n_kb; ++kb) {
+  for (int kb = kb0; kb < n_kb; ++kb) {
     __syncthreads();                                     // previous readers of K / V^T / P are done
     pa_load_rows<128>(smem + PA_OFF_K, kg, a.k_ss, kb * 128, S_kv);
     pa_load_vt(smem + PA_OFF_VT, vg, a.v_ss, kb * 128, S_kv);
@@ -160,7 +171,7 @@ attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
     }
     fence_async_smem();
     __syncthreads();
-    pa_mma(o, sbase + PA_OFF_P, 64 * 128, sbase + PA_OFF_VT, 128 * 128, kb > 0);
+    pa_mma(o, sbase + PA_OFF_P, 64 * 128, sbase + PA_OFF_VT, 128 * 128, kb > kb0);
   }
 
   // ---- O / l -> bf16 ----
@@ -186,7 +197,8 @@ attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
 }  // namespace
 
 int init_attention_prefill_tc_kernels() {
-  VCL_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PA_SMEM));
+  VCL_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PA_SMEM));
+  VCL_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, PA_SMEM));
   return 0;
 }
 
@@ -206,7 +218,8 @@ bool attention_prefill_tc_supported(const AttnArgs& a) {
 int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t stream) {
   const int S_kv = a.S_kv > 0 ? a.S_kv : a.S;
   dim3 grid((a.S + 63) / 64, a.H, a.B);
-  attn_prefill_tc_kernel<<<grid, PA_THREADS, PA_SMEM, stream>>>(a, S_kv);
+  if (a.n_pad != nullptr) attn_prefill_tc_kernel<true><<<grid, PA_THREADS, PA_SMEM, stream>>>(a, S_kv);
+  else attn_prefill_tc_kernel<false><<<grid, PA_THREADS, PA_SMEM, stream>>>(a, S_kv);
   VCL_CUDA_OK(cudaGetLastError());
   count_launches(1);
   return 0;

@@ -48,26 +48,29 @@ __device__ __forceinline__ float block_reduce(float v, bool is_max, float* scrat
 }
 
 // DA_SPLIT = CTAs per (clip, head): 4 for few clips (latency: more CTAs than SMs are needed to fill the
-// machine at all), 2 or 1 when clips x heads alone oversubscribe it (throughput: fewer barriers per byte)
-template <int DA_SPLIT>
+// machine at all), 2 or 1 when clips x heads alone oversubscribe it (throughput: fewer barriers per byte).
+// PAD: left-padded clips (n_pad): the keys of clip b are n_pad[b] .. kv_len-1, split over the CTAs as above
+template <int DA_SPLIT, bool PAD>
 __global__ void __launch_bounds__(DA_THREADS)
 decode_attn_cluster_kernel(const bf16* __restrict__ q, long long q_ld, const bf16* __restrict__ kcache,
                            const bf16* __restrict__ vcache, bf16* __restrict__ o, long long o_ld, int H,
                            int s_max, int kv_len, int per_cap, float scale, const int* __restrict__ pos_dev,
-                           int o_xwin) {
+                           int o_xwin, const int* __restrict__ n_pad) {
   extern __shared__ float sm[];
   float* sc = sm;                       // [per_cap] scores -> probabilities of my keys
   float* red = sm + per_cap;            // [16][128] partial outputs over the 16 key groups
+  const int h = blockIdx.y, b = blockIdx.z;
   // the number of cached keys may live on the device (one captured graph for every prompt length);
-  // it is constant while the graph runs, so it can be read before the dependency wait
+  // it is constant while the graph runs, so it can be read before the dependency wait. So is the left
+  // padding of the clip: its first k0 cache columns hold pad keys, which are neither read nor split
   if (pos_dev != nullptr) kv_len += __ldg(pos_dev);
-  const int per = ((kv_len + DA_SPLIT - 1) / DA_SPLIT + 15) / 16 * 16;   // keys per CTA, multiple of 16
+  const int k0 = PAD ? __ldg(n_pad + b) : 0;
+  const int per = ((kv_len - k0 + DA_SPLIT - 1) / DA_SPLIT + 15) / 16 * 16;   // keys per CTA, multiple of 16
   float* outp = red + 16 * 128;         // [128] this CTA's partial output
   float* stat = outp + 128;             // [0] local max, [1] local sum
   float* scratch = stat + 2;            // [8]
   const uint32_t rank = cluster_ctarank();
-  const int h = blockIdx.y, b = blockIdx.z;
-  const int lo = (int)rank * per;
+  const int lo = k0 + (int)rank * per;
   const int n_loc = max(0, min(kv_len - lo, per));
   const long long coff = (((long long)b * H + h) * s_max + lo) * 128;
   const bf16* kc = kcache + coff;
@@ -181,7 +184,8 @@ decode_attn_cluster_kernel(const bf16* __restrict__ q, long long q_ld, const bf1
 
 int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, const bf16* vcache,
                             bf16* o, long long o_ld, int B, int H, int head_dim, int s_max,
-                            int kv_len, float scale, cudaStream_t stream, const int* pos_dev, bool o_xwin) {
+                            int kv_len, float scale, cudaStream_t stream, const int* pos_dev, bool o_xwin,
+                            const int* n_pad) {
   VCL_REQUIRE(head_dim == 128, "decode attention: head_dim must be 128");
   VCL_REQUIRE(kv_len > 0 && kv_len <= s_max, "decode attention: kv_len %d out of range", kv_len);
   // shared memory is sized for the longest sequence when the length is only known on the device
@@ -206,15 +210,11 @@ int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, c
   attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 2;
-  if (split == 4)
-    VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, decode_attn_cluster_kernel<4>, q, q_ld, kcache, vcache, o, o_ld, H, s_max, kv_len,
-                                   per, scale, pos_dev, o_xwin ? 1 : 0));
-  else if (split == 2)
-    VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, decode_attn_cluster_kernel<2>, q, q_ld, kcache, vcache, o, o_ld, H, s_max, kv_len,
-                                   per, scale, pos_dev, o_xwin ? 1 : 0));
-  else
-    VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, decode_attn_cluster_kernel<1>, q, q_ld, kcache, vcache, o, o_ld, H, s_max, kv_len,
-                                   per, scale, pos_dev, o_xwin ? 1 : 0));
+  auto kern = n_pad ? decode_attn_cluster_kernel<4, true> : decode_attn_cluster_kernel<4, false>;
+  if (split == 2) kern = n_pad ? decode_attn_cluster_kernel<2, true> : decode_attn_cluster_kernel<2, false>;
+  if (split == 1) kern = n_pad ? decode_attn_cluster_kernel<1, true> : decode_attn_cluster_kernel<1, false>;
+  VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, q, q_ld, kcache, vcache, o, o_ld, H, s_max, kv_len, per, scale, pos_dev,
+                                 o_xwin ? 1 : 0, n_pad));
   count_launches(1);
   return 0;
 }

@@ -176,7 +176,10 @@ __device__ __forceinline__ void epi_swiglu(const GemvEpilogue& e, int b, int row
   e.out[o] = __float2bfloat16_rn(sg * bf16r(up));
 }
 // QKV: row = (which*H + head)*128 + 2*d holds dims (d, d + 64) of q, k or v (RoPE pairs adjacent); q and k are
-// rotated, q goes to q_out, k and v to the cache at position pos
+// rotated, q goes to q_out, k and v to the cache at column pos. With left padding (e.n_pad) the rotation angle is
+// that of position pos - n_pad[b]; the cache column stays pos. PAD: the kernel instance of a padded cache (the
+// unpadded instances keep the code they had before padding existed).
+template <bool PAD>
 __device__ __forceinline__ void epi_qkv_rope(const GemvEpilogue& e, int b, int row, int pos, float v0, float v1) {
   const int hr = row >> 7;
   const int which = hr / e.H, head = hr - which * e.H;
@@ -187,8 +190,9 @@ __device__ __forceinline__ void epi_qkv_rope(const GemvEpilogue& e, int b, int r
     e.vcache[coff + d] = __float2bfloat16_rn(lo);
     e.vcache[coff + d + 64] = __float2bfloat16_rn(hi);
   } else {
-    const float cs = __bfloat162float(e.cos_t[(long long)pos * 64 + d]);
-    const float sn = __bfloat162float(e.sin_t[(long long)pos * 64 + d]);
+    const int rpos = PAD ? max(pos - __ldg(e.n_pad + b), 0) : pos;
+    const float cs = __bfloat162float(e.cos_t[(long long)rpos * 64 + d]);
+    const float sn = __bfloat162float(e.sin_t[(long long)rpos * 64 + d]);
     const float olo = bf16r(lo * cs) + bf16r(-hi * sn);
     const float ohi = bf16r(hi * cs) + bf16r(lo * sn);
     if (which == 0) {
@@ -209,6 +213,7 @@ __device__ __forceinline__ long long qkv_row(int v) {
 // ---------------------------------------------------------------------------------------------
 // 1..4 clips
 // ---------------------------------------------------------------------------------------------
+template <bool PAD>
 __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   // layout: ring[n_slots] | x[nb][K] bf16 (+ norm weights [K]) | pbuf[2][CWARPS][16][4] | result[r_cap][4] fp32
@@ -538,7 +543,7 @@ __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
       if (mode == GEMV_RES) epi_residual(e, b, vrow, v0);
       else if (mode == GEMV_LOGITS) epi_logit(e, b, vrow, v0);
       else if (mode == GEMV_SWIGLU) epi_swiglu(e, b, vrow, NB, v0, v1);
-      else epi_qkv_rope(e, b, vrow, decode_pos(e), v0, v1);
+      else epi_qkv_rope<PAD>(e, b, vrow, decode_pos(e), v0, v1);
     }
   }
   if (mode == GEMV_LOGITS && a.amax_out != nullptr) {
@@ -575,7 +580,7 @@ __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
 // 5..16 clips. NG = upper bound of the row groups a CTA owns (the accumulator arrays are sized and
 // unrolled by it); a.x holds the activations in the xwin layout
 // ---------------------------------------------------------------------------------------------
-template <int NG>
+template <int NG, bool PAD>
 __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, const GemvEpilogue e) {
   extern __shared__ __align__(128) uint8_t smem[];
   // layout: ring[8] (after the main loop: partial tiles [warp][group]) | x windows [4][16][1088 B] | barriers
@@ -751,7 +756,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
       if (b >= NB || vrow >= N) continue;
       const float v0 = tile_sum(lg, rr * 17 + b), v1 = tile_sum(lg, (rr + 1) * 17 + b);
       if (mode == GEMV_SWIGLU) epi_swiglu(e, b, vrow, NB, v0, v1);
-      else epi_qkv_rope(e, b, vrow, pos, v0, v1);
+      else epi_qkv_rope<PAD>(e, b, vrow, pos, v0, v1);
     }
   }
 }
@@ -836,7 +841,7 @@ int launch_tc(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
   }
   cudaLaunchAttribute attr[1];
   cudaLaunchConfig_t cfg = pdl_config(grid, smem, stream, attr);
-  VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tc_kernel, p));
+  VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, e.n_pad != nullptr ? gemv_tc_kernel<true> : gemv_tc_kernel<false>, p));
   count_launches(1);
   return 0;
 }
@@ -865,10 +870,12 @@ int launch_tcw(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
     cudaLaunchAttribute attr[1];
     cudaLaunchConfig_t cfg = pdl_config(grid, TW_SMEM, stream, attr);
     const int ng_max = (g1 - g0 + grid - 1) / grid;                  // groups of the busiest CTA
-    if (ng_max <= 2) VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tcw_kernel<2>, sa, se));
-    else if (ng_max <= 6) VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tcw_kernel<6>, sa, se));
-    else if (ng_max <= 10) VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tcw_kernel<10>, sa, se));
-    else VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tcw_kernel<TW_NG_MAX>, sa, se));
+    const bool pad = e.n_pad != nullptr;
+    auto kern = pad ? gemv_tcw_kernel<TW_NG_MAX, true> : gemv_tcw_kernel<TW_NG_MAX, false>;
+    if (ng_max <= 2) kern = pad ? gemv_tcw_kernel<2, true> : gemv_tcw_kernel<2, false>;
+    else if (ng_max <= 6) kern = pad ? gemv_tcw_kernel<6, true> : gemv_tcw_kernel<6, false>;
+    else if (ng_max <= 10) kern = pad ? gemv_tcw_kernel<10, true> : gemv_tcw_kernel<10, false>;
+    VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, sa, se));
     count_launches(1);
   }
   return 0;
@@ -891,11 +898,12 @@ extern "C" int vcl_debug_tc_trace_dump(const char* path) {
 }
 
 int init_gemv_kernels() {
-  VCL_CUDA_OK(cudaFuncSetAttribute(gemv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-  VCL_CUDA_OK(cudaFuncSetAttribute(gemv_tcw_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
-  VCL_CUDA_OK(cudaFuncSetAttribute(gemv_tcw_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
-  VCL_CUDA_OK(cudaFuncSetAttribute(gemv_tcw_kernel<10>, cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
-  VCL_CUDA_OK(cudaFuncSetAttribute(gemv_tcw_kernel<TW_NG_MAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
+  for (auto k : {gemv_tc_kernel<false>, gemv_tc_kernel<true>})
+    VCL_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+  for (auto k : {gemv_tcw_kernel<2, false>, gemv_tcw_kernel<6, false>, gemv_tcw_kernel<10, false>,
+                 gemv_tcw_kernel<TW_NG_MAX, false>, gemv_tcw_kernel<2, true>, gemv_tcw_kernel<6, true>,
+                 gemv_tcw_kernel<10, true>, gemv_tcw_kernel<TW_NG_MAX, true>})
+    VCL_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
   return 0;
 }
 
@@ -931,6 +939,7 @@ int launch_gemv(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
               "row groups of 16 per SM)", a.B, a.N, a.K);
   VCL_REQUIRE(e.mode != GEMV_SWIGLU || a.N % 2 == 0, "gemv swiglu: N must be even (interleaved gate/up rows)");
   VCL_REQUIRE(e.mode != GEMV_QKV || a.N == 3 * e.H * 128, "gemv qkv: N=%d != 3*H*128", a.N);
+  VCL_REQUIRE(e.n_pad == nullptr || e.mode == GEMV_QKV, "gemv: left padding applies to the q|k|v epilogue only");
   VCL_REQUIRE(a.embed == nullptr || (a.vocab > 0 && (a.tok_in != nullptr || (a.amax_in != nullptr && a.amax_n > 0))),
               "gemv: the fused embedding gather needs a token source");
   return a.B <= 4 ? launch_tc(a, e, stream) : launch_tcw(a, e, stream);

@@ -302,7 +302,8 @@ __global__ void rope_table_kernel(bf16* cos_t, bf16* sin_t, int max_pos, int hea
 __global__ void __launch_bounds__(256)
 rope_kv_prefill_kernel(bf16* qkv, bf16* __restrict__ kcache, bf16* __restrict__ vcache,
                        const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t, int B, int S,
-                       int H, int s_max, int pos0, const int* __restrict__ pos_dev) {
+                       int H, int s_max, int pos0, const int* __restrict__ pos_dev,
+                       const int* __restrict__ n_pad) {
   const long long wid = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (wid >= (long long)B * S * H) return;
@@ -313,6 +314,8 @@ rope_kv_prefill_kernel(bf16* qkv, bf16* __restrict__ kcache, bf16* __restrict__ 
   bf16* row = qkv + tok * 3LL * D;
   const int pos = pos0 + s + (pos_dev != nullptr ? __ldg(pos_dev) : 0);
   const long long cache_off = (((long long)b * H + head) * s_max + pos) * 128;
+  // RoPE position of this cache column: left padding shifts it (pad columns clamp at 0)
+  const int rpos = n_pad != nullptr ? max(pos - __ldg(n_pad + b), 0) : pos;
   if (lane < 16) {
     const int which = lane >> 3;              // 0 = q, 1 = k
     const int d0 = (lane & 7) * 8;            // 0..56, partner at +64
@@ -320,8 +323,8 @@ rope_kv_prefill_kernel(bf16* qkv, bf16* __restrict__ kcache, bf16* __restrict__ 
     float lo[8], hi[8], c[8], sn[8], olo[8], ohi[8];
     unpack8(*reinterpret_cast<const uint4*>(base + d0), lo);
     unpack8(*reinterpret_cast<const uint4*>(base + d0 + 64), hi);
-    unpack8(*reinterpret_cast<const uint4*>(cos_t + (long long)pos * 64 + d0), c);
-    unpack8(*reinterpret_cast<const uint4*>(sin_t + (long long)pos * 64 + d0), sn);
+    unpack8(*reinterpret_cast<const uint4*>(cos_t + (long long)rpos * 64 + d0), c);
+    unpack8(*reinterpret_cast<const uint4*>(sin_t + (long long)rpos * 64 + d0), sn);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       // q*cos + rotate_half(q)*sin with every product and the sum rounded to bf16
@@ -467,13 +470,13 @@ int launch_rope_table(bf16* cos_t, bf16* sin_t, int max_pos, int head_dim, float
 
 int launch_rope_kv_prefill(bf16* qkv, bf16* kcache, bf16* vcache, const bf16* cos_t,
                            const bf16* sin_t, int B, int S, int H, int head_dim, int s_max, int pos0,
-                           cudaStream_t stream, const int* pos_dev) {
+                           cudaStream_t stream, const int* pos_dev, const int* n_pad) {
   VCL_REQUIRE(head_dim == 128, "rope: head_dim must be 128 (got %d)", head_dim);
   VCL_REQUIRE(pos0 + S <= s_max, "rope: positions %d..%d exceed the cache (%d)", pos0, pos0 + S, s_max);
   const long long warps = (long long)B * S * H;
   if (warps <= 0) return 0;
   rope_kv_prefill_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, stream>>>(qkv, kcache, vcache, cos_t,
-                                                                        sin_t, B, S, H, s_max, pos0, pos_dev);
+                                                                        sin_t, B, S, H, s_max, pos0, pos_dev, n_pad);
   VCL_CUDA_OK(cudaGetLastError());
   count_launches(1);
   return 0;

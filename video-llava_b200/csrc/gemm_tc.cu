@@ -64,7 +64,8 @@ __device__ __forceinline__ void named_bar_sync(int id, int threads) {
 //   ACT_ROPE  : a 128-column block is one head of q | k | v; the RoPE partner of column d is d + 64, which the
 //               same thread holds 8 accumulator groups further on, so the rotation is thread-local. Arithmetic =
 //               rope_kv_prefill_kernel (elementwise.cu): x rounded to bf16, every product rounded, fp32 sum, one
-//               final rounding (transformers/models/llama/modeling_llama.py:124-168).
+//               final rounding (transformers/models/llama/modeling_llama.py:124-168). With left padding
+//               (rp.n_pad) the angle is that of cache column - n_pad[clip], clamped at 0; the columns do not move.
 template <int BLOCK_N, int ACT>
 __device__ __forceinline__ void gemm_epilogue_stage(const float (&acc)[BLOCK_N / 2], uint8_t* stg, int lane, int wq,
                                                     int row_base, int n_blk, const bf16* __restrict__ bias, int M,
@@ -82,7 +83,8 @@ __device__ __forceinline__ void gemm_epilogue_stage(const float (&acc)[BLOCK_N /
       for (int h = 0; h < 2; ++h) {
         const int r = r0 + 8 * h;
         const int grow = row_base + r;
-        const int pos = rp.start_pos + (grow < M ? grow % rp.S : 0);
+        int pos = rp.start_pos + (grow < M ? grow % rp.S : 0);
+        if (rp.n_pad != nullptr && grow < M) pos = max(pos - __ldg(rp.n_pad + grow / rp.S), 0);   // left padding
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
           const int j = hh * 16 + jj, d = 8 * jj + c2;

@@ -19,7 +19,13 @@ struct RopeEpilogue {
   const bf16* cos_t = nullptr; const bf16* sin_t = nullptr;    // [s_max][64]
   bf16* kcache = nullptr; bf16* vcache = nullptr;              // [clip][head][s_max][128] of this layer
   int S = 0, start_pos = 0, H = 0, s_max = 0;                  // rows per clip, position of row 0, heads
+  const int* n_pad = nullptr;                                  // [clip] left padding (see below) or null
 };
+
+// Left padding (a batch of prompts of different lengths): clip b's first n_pad[b] cache columns hold pad
+// tokens. Cache column c holds RoPE position max(c - n_pad[b], 0); a query at column c >= n_pad[b] attends keys
+// n_pad[b] .. c, a pad query attends causally from key 0 (its output is unused but finite). Every `n_pad`
+// argument below is a device array [clip]; null means no padding and leaves the kernels' arithmetic unchanged.
 
 void set_last_error(const char* fmt, ...);
 void count_launches(long long n);
@@ -72,7 +78,7 @@ int launch_rope_table(bf16* cos_t, bf16* sin_t, int max_pos, int head_dim, float
 // serves every prompt length; the same convention holds for every `pos_dev` below)
 int launch_rope_kv_prefill(bf16* qkv, bf16* kcache, bf16* vcache, const bf16* cos_t,
                            const bf16* sin_t, int B, int S, int H, int head_dim, int s_max, int pos0,
-                           cudaStream_t stream, const int* pos_dev = nullptr);
+                           cudaStream_t stream, const int* pos_dev = nullptr, const int* n_pad = nullptr);
 // h[b,:] = table[tok[b*tok_stride]]  (decode-time embedding lookup, tokens live on the device)
 int launch_embed_tokens(const int* tok, long long tok_stride, const bf16* table, bf16* h, int B,
                         int D, int vocab, cudaStream_t stream);
@@ -99,6 +105,7 @@ struct AttnArgs {
   int causal;
   int S_kv = 0;      // number of keys (0: = S); > S when the queries continue a cached sequence
   int q_off = 0;     // absolute position of query 0 for the causal mask (S_kv - S for a continuation)
+  const int* n_pad = nullptr;   // causal only: [B] left padding, the key floor of real queries (or null)
 };
 int launch_attention(const AttnArgs& a, cudaStream_t stream);     // dispatches to the wgmma prefill kernel when it applies
 int init_attention_kernels();
@@ -117,7 +124,8 @@ int init_attention_tc_kernels();
 int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, const bf16* vcache,
                             bf16* o, long long o_ld, int B, int H, int head_dim, int s_max,
                             int kv_len, float scale, cudaStream_t stream, const int* pos_dev = nullptr,
-                            bool o_xwin = false);   // o_xwin: the output [B][H*hd] is written in xwin layout
+                            bool o_xwin = false,    // o_xwin: the output [B][H*hd] is written in xwin layout
+                            const int* n_pad = nullptr);   // keys n_pad[b] .. kv_len-1 only
 
 // ---- decode_gemv.cu : decode-time weight streaming (1..16 new tokens) -------------------------------
 // Two ring kernels (bulk-copy ring over a slot-ordered copy of the matrix + mma.sync) behind one launcher:
@@ -162,6 +170,7 @@ struct GemvEpilogue {
   const bf16* cos_t = nullptr; const bf16* sin_t = nullptr;
   int H = 0, s_max = 0, pos = 0;
   const int* pos_dev = nullptr;                 // position = pos + *pos_dev
+  const int* n_pad = nullptr;                   // QKV: [B] left padding, RoPE angle at position - n_pad[b]
   float* logits = nullptr; long long ldl = 0;   // LOGITS
 };
 

@@ -50,6 +50,7 @@ struct LlmLayerW {
 };
 struct GraphEntry {
   int B, S, n_new;     // S = -1: the prompt length is read on the device (h->d_pos), any S replays it
+  bool padded;         // captured with the left-padding array (h->d_npad): replays only for a padded cache
   cudaGraphExec_t exec;
   long long kernels;   // kernel nodes in the graph (for vcl_launch_count)
   unsigned long long last_use;
@@ -98,6 +99,12 @@ struct vcl_handle {
   std::vector<GraphEntry> graphs;
   unsigned long long graph_clock = 0;
   int* d_pos = nullptr;                        // prompt length of the running decode loop (device scalar)
+  // Left padding of the cache (vcl_llm_prefill_padded): the first d_npad[b] cache columns of clip b hold pad
+  // tokens. Set by a padded prefill, cleared by an unpadded one; appends and decode steps continue it. The
+  // array lives at a fixed address, so a captured decode graph serves every set of pad counts.
+  int* d_npad = nullptr;                       // [max_batch]
+  bool padded = false;
+  int npad_max = 0;                            // largest pad count of the padded batch (host copy)
   ArgmaxPart* amax = nullptr;                  // [gemv_grid(vocab)][max_batch] per-CTA partial arg-max of the logits kernel
 
   size_t cache_layer_elems() const {
@@ -251,6 +258,7 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   rc |= dalloc(h, &h->d_attn, xwin_elems((int)Bm, (int)D) > Bm * D ? xwin_elems((int)Bm, (int)D) : Bm * D);
   rc |= dalloc(h, &h->d_act, xwin_elems((int)Bm, (int)LF) > Bm * LF ? xwin_elems((int)Bm, (int)LF) : Bm * LF);
   rc |= dalloc(h, &h->d_pos, 4);
+  rc |= dalloc(h, &h->d_npad, Bm);
   rc |= dalloc(h, &h->amax, (size_t)device_num_sms() * Bm);
   if (rc == 0) rc = launch_rope_table(h->rope_cos, h->rope_sin, c->max_seq, 128, c->rope_theta, 0);
   if (rc == 0) {
@@ -485,9 +493,12 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
 // and attend to the whole cache (multi-turn reuse; no video span in a continuation).
 // states_out (optional): [n_layers + 1][B][S][D], entry i = HF's hidden_states[i] (the raw output of
 // layer i; entry 0 the spliced input embeddings), copied out as the stack advances.
+// A new sequence (start_pos == 0) sets the cache's left padding: n_pad_host [B] (host memory), or none when it is
+// null or all zero. A continuation keeps the padding of the cache.
 int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
                 int B, int S, int n_layers, void* hidden_out, float* logits_out, int32_t* next_tok,
-                long long tok_stride, cudaStream_t st, int start_pos = 0, void* states_out = nullptr) {
+                long long tok_stride, cudaStream_t st, int start_pos = 0, void* states_out = nullptr,
+                const int32_t* n_pad_host = nullptr) {
   const vcl_config& c = h->cfg;
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
   VCL_REQUIRE(B > 0 && B <= c.max_batch, "B=%d outside 1..%d", B, c.max_batch);
@@ -498,6 +509,24 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
   VCL_REQUIRE(start_pos == 0 || video_feats == nullptr, "a continuation cannot carry a video span");
   VCL_REQUIRE((logits_out == nullptr && next_tok == nullptr) || n_layers == c.llm_layers,
               "logits / next token need the full stack (n_layers == %d)", c.llm_layers);
+  if (start_pos == 0) {
+    int npad_max = 0;
+    if (n_pad_host != nullptr) {
+      for (int b = 0; b < B; ++b) {
+        VCL_REQUIRE(n_pad_host[b] >= 0 && n_pad_host[b] < S,
+                    "n_pad[%d] = %d outside 0..%d (a row needs at least one real token)", b, n_pad_host[b], S - 1);
+        npad_max = n_pad_host[b] > npad_max ? n_pad_host[b] : npad_max;
+      }
+    }
+    h->padded = npad_max > 0;
+    h->npad_max = npad_max;
+    if (h->padded)
+      VCL_CUDA_OK(cudaMemcpyAsync(h->d_npad, n_pad_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  } else {
+    VCL_REQUIRE(start_pos > h->npad_max, "start_pos %d lies inside the left padding (%d columns)", start_pos,
+                h->npad_max);
+  }
+  const int* np = h->padded ? h->d_npad : nullptr;
   const int D = c.llm_hidden, F = c.llm_inter, H = c.llm_heads, NV = h->NV;
   const int M = B * S;
   if (video_feats != nullptr) {
@@ -533,12 +562,12 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
       g.A = h->l_x; g.lda = D; g.W = w.wqkv; g.ldw = D; g.C = h->l_qkv; g.ldc = 3 * D; g.M = M; g.N = 3 * D; g.K = D;
       g.act = ACT_ROPE;
       g.rope.cos_t = h->rope_cos; g.rope.sin_t = h->rope_sin; g.rope.kcache = kc_layer(h, l); g.rope.vcache = vc_layer(h, l);
-      g.rope.S = S; g.rope.start_pos = start_pos; g.rope.H = H; g.rope.s_max = c.max_seq;
+      g.rope.S = S; g.rope.start_pos = start_pos; g.rope.H = H; g.rope.s_max = c.max_seq; g.rope.n_pad = np;
       VCL_TRY(launch_gemm_bf16_tn(g, st));
     } else {
       VCL_TRY(gemm(h->l_x, D, w.wqkv, D, h->l_qkv, 3 * D, nullptr, nullptr, 0, M, 3 * D, D, ACT_NONE, st));
       VCL_TRY(launch_rope_kv_prefill(h->l_qkv, kc_layer(h, l), vc_layer(h, l), h->rope_cos, h->rope_sin, B,
-                                     S, H, 128, c.max_seq, start_pos, st));
+                                     S, H, 128, c.max_seq, start_pos, st, nullptr, np));
     }
     AttnArgs a;
     a.q = h->l_qkv; a.q_sb = (long long)S * 3 * D; a.q_sh = 128; a.q_ss = 3 * D;
@@ -546,7 +575,7 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
     a.v = vc_layer(h, l); a.v_sb = a.k_sb; a.v_sh = a.k_sh; a.v_ss = 128;
     a.o = h->l_attn; a.o_sb = (long long)S * D; a.o_sh = 128; a.o_ss = D;
     a.B = B; a.H = H; a.S = S; a.head_dim = 128; a.scale = scale; a.causal = 1;
-    a.S_kv = start_pos + S; a.q_off = start_pos;
+    a.S_kv = start_pos + S; a.q_off = start_pos; a.n_pad = np;
     VCL_TRY(launch_attention(a, st));
     VCL_TRY(gemm(h->l_attn, D, w.wo, D, h->l_h, D, nullptr, h->l_h, D, M, D, D, ACT_NONE, st));
     VCL_TRY(launch_rmsnorm(h->l_h, D, h->l_x, D, w.ln2, M, D, c.rms_eps, st));
@@ -568,7 +597,10 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
   const int D = c.llm_hidden, F = c.llm_inter, H = c.llm_heads;
   const float scale = 0.08838834764831845f;
   const int* pd = io.pos_dev;
+  const int* np = h->padded ? h->d_npad : nullptr;   // a padded cache stays padded
   VCL_REQUIRE(pos >= 0 && pos < c.max_seq, "decode position %d outside the cache (max_seq %d)", pos, c.max_seq);
+  VCL_REQUIRE(pd != nullptr || pos >= h->npad_max, "decode position %d lies inside the left padding (%d columns)",
+              pos, h->npad_max);
   // 1..4 clips: the embedding lookup is part of layer 0's q|k|v kernel (and with it the arg-max of the
   // previous step); every other path gathers the rows with a kernel of its own.
   const bool fused_embed = B <= 4 && c.llm_layers > 0;
@@ -607,9 +639,10 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
       GemvEpilogue qkv;
       qkv.mode = GEMV_QKV; qkv.q_out = h->d_q; qkv.ldq = D; qkv.kcache = kc_layer(h, l); qkv.vcache = vc_layer(h, l);
       qkv.cos_t = h->rope_cos; qkv.sin_t = h->rope_sin; qkv.H = H; qkv.s_max = c.max_seq; qkv.pos = pos; qkv.pos_dev = pd;
+      qkv.n_pad = np;
       VCL_TRY(launch_gemv(g, qkv, st));
       VCL_TRY(launch_decode_attention(h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->d_attn, D, B, H, 128,
-                                      c.max_seq, pos + 1, scale, st, pd, /*o_xwin=*/wide));
+                                      c.max_seq, pos + 1, scale, st, pd, /*o_xwin=*/wide, np));
       GemvArgs go;
       go.x = h->d_attn; go.ldx = D; go.W_tiled = w.wo_t; go.B = B; go.N = D; go.K = D;
       VCL_TRY(launch_gemv(go, residual, st));
@@ -628,9 +661,9 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
       VCL_TRY(launch_rmsnorm(h->d_h, D, h->d_x, D, w.ln1, B, D, c.rms_eps, st));
       VCL_TRY(gemm(h->d_x, D, w.wqkv, D, h->d_qkv, 3 * D, nullptr, nullptr, 0, B, 3 * D, D, ACT_NONE, st));
       VCL_TRY(launch_rope_kv_prefill(h->d_qkv, kc_layer(h, l), vc_layer(h, l), h->rope_cos, h->rope_sin, B,
-                                     1, H, 128, c.max_seq, pos, st, pd));
+                                     1, H, 128, c.max_seq, pos, st, pd, np));
       VCL_TRY(launch_decode_attention(h->d_qkv, 3 * D, kc_layer(h, l), vc_layer(h, l), h->d_attn, D, B, H,
-                                      128, c.max_seq, pos + 1, scale, st, pd));
+                                      128, c.max_seq, pos + 1, scale, st, pd, false, np));
       VCL_TRY(gemm(h->d_attn, D, w.wo, D, h->d_h, D, nullptr, h->d_h, D, B, D, D, ACT_NONE, st));
       VCL_TRY(launch_rmsnorm(h->d_h, D, h->d_x, D, w.ln2, B, D, c.rms_eps, st));
       VCL_TRY(gemm(h->d_x, D, w.wgu, D, h->d_act, F, nullptr, nullptr, 0, B, 2 * F, D, ACT_SWIGLU, st));
@@ -744,17 +777,19 @@ int vcl_llm_decode_loop(vcl_handle* h, const int32_t* first_tok, int B, int S, i
   VCL_REQUIRE(B > 0 && B <= h->cfg.max_batch, "B=%d outside 1..%d", B, h->cfg.max_batch);
   VCL_REQUIRE(n_new >= 1 && S + n_new <= h->cfg.max_seq + 1, "S + n_new = %d exceeds max_seq %d", S + n_new,
               h->cfg.max_seq);
+  VCL_REQUIRE(S >= h->npad_max, "S = %d lies inside the left padding (%d columns)", S, h->npad_max);
   cudaStream_t st = as_stream(stream);
   int32_t* tk = h->tokens;  // [B, n_new] row-major scratch
   if (first_tok != tk)
     VCL_CUDA_OK(cudaMemcpy2DAsync(tk, (size_t)n_new * sizeof(int32_t), first_tok, sizeof(int32_t),
                                   sizeof(int32_t), B, cudaMemcpyDeviceToDevice, st));
   if (n_new > 1) {
-    // One graph per (B, n_new): the prompt length S reaches the kernels through h->d_pos, so a new
-    // prompt length replays the same graph. Bounded LRU cache (an entry holds thousands of nodes).
+    // One graph per (B, n_new, padded): the prompt length S reaches the kernels through h->d_pos and the pad
+    // counts through h->d_npad, so a new prompt length or padding replays the same graph. Bounded LRU cache (an
+    // entry holds thousands of nodes).
     GraphEntry* ge = nullptr;
     for (auto& g : h->graphs)
-      if (g.B == B && g.n_new == n_new && g.S == -1) ge = &g;
+      if (g.B == B && g.n_new == n_new && g.S == -1 && g.padded == h->padded) ge = &g;
     const bool can_capture = (st != nullptr) && (st != cudaStreamLegacy);
     if (ge == nullptr && can_capture) {
       if (h->graphs.size() >= MAX_DECODE_GRAPHS) {
@@ -786,7 +821,7 @@ int vcl_llm_decode_loop(vcl_handle* h, const int32_t* first_tok, int B, int S, i
         set_last_error("decode graph instantiate failed: %s", cudaGetErrorString(e));
         return -2;
       }
-      h->graphs.push_back({B, -1, n_new, exec, nodes, 0});
+      h->graphs.push_back({B, -1, n_new, h->padded, exec, nodes, 0});
       ge = &h->graphs.back();
     }
     if (ge != nullptr) {
@@ -811,6 +846,25 @@ int vcl_llm_generate(vcl_handle* h, const int64_t* ids, const void* video_feats,
   cudaStream_t st = as_stream(stream);
   VCL_TRY(llm_prefill(h, ids, video_feats, vid_start, B, S, h->cfg.llm_layers, nullptr, nullptr, h->tokens,
                       n_new, st));
+  return vcl_llm_decode_loop(h, h->tokens, B, S, n_new, out_tokens, stream);
+}
+
+int vcl_llm_prefill_padded(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
+                           const int32_t* n_pad_host, int B, int S, int n_layers, void* hidden_out,
+                           float* logits_out, int32_t* next_tok, void* stream) {
+  VCL_REQUIRE(h != nullptr && n_pad_host != nullptr, "vcl_llm_prefill_padded: null argument");
+  return llm_prefill(h, ids, video_feats, vid_start, B, S, n_layers, hidden_out, logits_out, next_tok, 1,
+                     as_stream(stream), 0, nullptr, n_pad_host);
+}
+
+int vcl_llm_generate_padded(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
+                            const int32_t* n_pad_host, int B, int S, int n_new, int32_t* out_tokens, void* stream) {
+  VCL_REQUIRE(h && out_tokens && n_pad_host, "vcl_llm_generate_padded: null argument");
+  VCL_REQUIRE(n_new >= 1 && S + n_new <= h->cfg.max_seq + 1, "S + n_new = %d exceeds max_seq %d", S + n_new,
+              h->cfg.max_seq);
+  cudaStream_t st = as_stream(stream);
+  VCL_TRY(llm_prefill(h, ids, video_feats, vid_start, B, S, h->cfg.llm_layers, nullptr, nullptr, h->tokens,
+                      n_new, st, 0, nullptr, n_pad_host));
   return vcl_llm_decode_loop(h, h->tokens, B, S, n_new, out_tokens, stream);
 }
 

@@ -62,6 +62,10 @@ _SIGNATURES = {
     "vcl_llm_generate": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
                                  c_void_p]),
     "vcl_llm_decode_loop": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "vcl_llm_prefill_padded": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_int,
+                                       c_void_p, c_void_p, c_void_p, c_void_p]),
+    "vcl_llm_generate_padded": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_int,
+                                        c_void_p, c_void_p]),
     "vcl_launch_count": (ctypes.c_longlong, []),
     "vcl_op_gemm": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
                             c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -201,6 +205,14 @@ def _tensor_array(state: dict, keep: list):
     return arr
 
 
+def _host_pads(n_pad, B: int):
+    """n_pad (sequence / tensor of B ints, any device) -> ctypes int32[B] in host memory."""
+    vals = n_pad.tolist() if isinstance(n_pad, torch.Tensor) else list(n_pad)
+    if len(vals) != B:
+        raise VclError(f"n_pad has {len(vals)} entries for {B} rows")
+    return (c_int32 * B)(*[int(v) for v in vals])
+
+
 def launch_count() -> int:
     return int(lib().vcl_launch_count())
 
@@ -277,7 +289,9 @@ class Engine:
 
     # ---- language model ----
     def prefill(self, ids, video_feats, vid_start, n_layers=None, want_hidden=False, want_logits=False,
-                want_token=True, tok_out=None):
+                want_token=True, tok_out=None, n_pad=None):
+        """n_pad: None (vcl_llm_prefill), or B left-padding counts (vcl_llm_prefill_padded; the cache stays
+        padded for the appends and decode steps that follow)."""
         B, S = ids.shape
         nl = self.cfg.llm_layers if n_layers is None else n_layers
         dev = ids.device
@@ -289,8 +303,13 @@ class Engine:
         if video_feats is not None:
             vf = video_feats.to(torch.bfloat16).contiguous()
             assert vf.shape == (B, self.NV, self.cfg.clip_hidden), vf.shape
-        check(lib().vcl_llm_prefill(self._h, ptr(ids.contiguous()), ptr(vf), ptr(vid_start.contiguous()), B, S,
-                                    nl, ptr(hidden), ptr(logits), ptr(tok), cur_stream()))
+        if n_pad is None:
+            check(lib().vcl_llm_prefill(self._h, ptr(ids.contiguous()), ptr(vf), ptr(vid_start.contiguous()), B, S,
+                                        nl, ptr(hidden), ptr(logits), ptr(tok), cur_stream()))
+        else:
+            check(lib().vcl_llm_prefill_padded(self._h, ptr(ids.contiguous()), ptr(vf), ptr(vid_start.contiguous()),
+                                               _host_pads(n_pad, B), B, S, nl, ptr(hidden), ptr(logits), ptr(tok),
+                                               cur_stream()))
         return hidden, logits, tok
 
     def prefill_states(self, ids, video_feats, vid_start, want_logits=False):
@@ -335,12 +354,17 @@ class Engine:
         check(lib().vcl_llm_decode_loop(self._h, ptr(first_tok.contiguous()), B, S, n_new, ptr(out), cur_stream()))
         return out
 
-    def generate(self, ids, video_feats, vid_start, n_new):
+    def generate(self, ids, video_feats, vid_start, n_new, n_pad=None):
+        """n_pad: None (vcl_llm_generate), or B left-padding counts (vcl_llm_generate_padded)."""
         B, S = ids.shape
         out = torch.empty(B, n_new, dtype=torch.int32, device=ids.device)
         vf = None
         if video_feats is not None:
             vf = video_feats.to(torch.bfloat16).contiguous()
-        check(lib().vcl_llm_generate(self._h, ptr(ids.contiguous()), ptr(vf), ptr(vid_start.contiguous()), B, S,
-                                     n_new, ptr(out), cur_stream()))
+        if n_pad is None:
+            check(lib().vcl_llm_generate(self._h, ptr(ids.contiguous()), ptr(vf), ptr(vid_start.contiguous()), B, S,
+                                         n_new, ptr(out), cur_stream()))
+        else:
+            check(lib().vcl_llm_generate_padded(self._h, ptr(ids.contiguous()), ptr(vf), ptr(vid_start.contiguous()),
+                                                _host_pads(n_pad, B), B, S, n_new, ptr(out), cur_stream()))
         return out

@@ -16,7 +16,12 @@ conventions. Differences from the reference, all documented where they occur:
     [B,S,V] and every caller on this path reads [:, -1]);
   * the vision tower's `hidden_states` are lazy: an entry is computed when indexed (the path reads [-2]);
     the language model's `hidden_states` are the L+1 tensors HF returns (the last one after the final
-    RMSNorm), produced by ONE prefill pass.
+    RMSNorm), produced by ONE prefill pass;
+  * a batch of prompts of different lengths is LEFT-padded (tokenizer.padding_side = "left") and passed
+    with its `attention_mask`, as for HF's LLaMA: every row is computed as if it ran alone (its real tokens
+    take positions 0..len-1 and never attend to a pad token). The reference reads the mask but drops the
+    positions HF derives from it, and its callers run one video at a time. Right padding and masks with
+    holes are rejected (left_padding below).
 """
 from __future__ import annotations
 
@@ -100,6 +105,34 @@ class VideoChatGPTConfig:
         j = json.load(open(os.path.join(path, "config.json")))
         j.update(kw)
         return cls(**j)
+
+
+def left_padding(attention_mask, shape) -> list | None:
+    """Pad count per row of a left-padded batch from its HF attention_mask ([B, S], bool or integer 0/1):
+    each row must be zeros followed by ones, with at least one 1. Returns None when nothing is padded
+    (an all-ones mask: the unpadded path), else the list of B pad counts. Raises ValueError otherwise;
+    it runs on the host, before any device work."""
+    if attention_mask is None:
+        return None
+    m = torch.as_tensor(attention_mask).detach().cpu()
+    B, S = int(shape[0]), int(shape[1])
+    if tuple(m.shape) != (B, S):
+        raise ValueError(f"attention_mask has shape {tuple(m.shape)}, input_ids {(B, S)}")
+    if m.dtype != torch.bool:
+        if m.is_floating_point() or m.is_complex() or not bool(((m == 0) | (m == 1)).all()):
+            raise ValueError("attention_mask must be bool or integer 0/1")
+        m = m != 0
+    pads = []
+    for b in range(B):
+        row = m[b]
+        n_pad = S - int(row.sum())
+        if n_pad == S:
+            raise ValueError(f"attention_mask row {b} has no real token")
+        if not bool(row[n_pad:].all()):
+            raise ValueError(f"attention_mask row {b} is not left padding (zeros, then ones): right padding and "
+                             "holes are not supported; tokenize with padding_side='left'")
+        pads.append(n_pad)
+    return pads if any(pads) else None
 
 
 class _LazyStates:
@@ -321,12 +354,13 @@ class VideoChatGPTLlamaForCausalLM:
         return self._engine
 
     # ---- validation (same errors as video_chatgpt.py:119-128,150-157) ---------------------
-    def _video_spans(self, input_ids: torch.Tensor, n_vid: int) -> list:
-        """Index of the row after which the projected video rows are spliced, per sample (-1: none)."""
+    def _video_spans(self, input_ids: torch.Tensor, n_vid: int, n_pad: list | None = None) -> list:
+        """Index of the row after which the projected video rows are spliced, per sample (-1: none).
+        n_pad: left padding per row; a video span must lie inside the real tokens."""
         vc = self.get_model().vision_config
         ids = input_ids.cpu()
         starts = []
-        for row in ids:
+        for b, row in enumerate(ids):
             if (row == vc.vid_patch_token).sum() == 0:
                 starts.append(vn.NO_VIDEO)             # text-only sample
                 continue
@@ -348,10 +382,14 @@ class VideoChatGPTLlamaForCausalLM:
                 if (idx != torch.arange(s0, s0 + n_vid)).any():
                     raise ValueError("The video patch tokens should be consecutive.")
                 starts.append(s0 - 1)                  # rows s0 .. s0+n_vid-1 are replaced (-1: from row 0)
+            first = starts[-1] + (0 if vc.use_vid_start_end else 1)      # first column of the span
+            if n_pad is not None and first < n_pad[b]:
+                raise ValueError(f"sample {b}: the video span starts at column {first}, inside the left padding "
+                                 f"({n_pad[b]} columns)")
         return starts
 
-    def _spans_dev(self, ids, feats, n_vid):
-        starts = self._video_spans(ids, n_vid) if feats is not None else [vn.NO_VIDEO] * ids.shape[0]
+    def _spans_dev(self, ids, feats, n_vid, n_pad=None):
+        starts = self._video_spans(ids, n_vid, n_pad) if feats is not None else [vn.NO_VIDEO] * ids.shape[0]
         return torch.tensor(starts, dtype=torch.int32, device="cuda")
 
     # ---- forward / generate ----------------------------------------------------------------
@@ -361,17 +399,22 @@ class VideoChatGPTLlamaForCausalLM:
                 video_spatio_temporal_features=None, return_dict=None):
         if inputs_embeds is not None or labels is not None or output_attentions:
             raise NotImplementedError("inference path only: input_ids in, logits out")
+        B, S = input_ids.shape
+        cached_step = S == 1 and past_key_values is not None
+        # a cached step ignores the mask: the KV cache carries the padding of its prefill
+        pads = None if cached_step else left_padding(attention_mask, (B, S))
+        if pads is not None and output_hidden_states:
+            raise NotImplementedError("output_hidden_states is not supported with a padded attention_mask")
         eng = self._ensure_engine(need_llm=True)
         ids = input_ids.cuda().to(torch.int64)
-        B, S = ids.shape
-        if S == 1 and past_key_values is not None:
+        if cached_step:
             # cached single-token step: the video features are ignored, as in the reference (:103)
             logits, _ = eng.decode_step(ids[:, 0].to(torch.int32).contiguous(), self._pos, want_logits=True)
             self._pos += 1
             hs = None
         else:
             feats = video_spatio_temporal_features
-            vs = self._spans_dev(ids, feats, eng.NV)
+            vs = self._spans_dev(ids, feats, eng.NV, pads)
             if feats is not None:
                 feats = feats.cuda()
             hs = None
@@ -384,7 +427,7 @@ class VideoChatGPTLlamaForCausalLM:
                 last = vn.op_rmsnorm(states[L].reshape(B * S, D), norm_w, self.config.rms_norm_eps).view(B, S, D)
                 hs = tuple(states[i] for i in range(L)) + (last,)
             else:
-                _, logits, _ = eng.prefill(ids, feats, vs, want_logits=True, want_token=False)
+                _, logits, _ = eng.prefill(ids, feats, vs, want_logits=True, want_token=False, n_pad=pads)
             self._pos = S
         return SimpleNamespace(loss=None, logits=logits.to(torch.bfloat16)[:, None, :], past_key_values=self._pos,
                                hidden_states=hs, attentions=None)
@@ -421,7 +464,7 @@ class VideoChatGPTLlamaForCausalLM:
     @torch.no_grad()
     def generate(self, input_ids, video_spatio_temporal_features=None, do_sample=False, temperature=1.0,
                  max_new_tokens=32, stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50,
-                 **kw):
+                 attention_mask=None, **kw):
         """Returns [B, S+n] int64 INCLUDING the prompt, like HF generate (inference.py:105-120), and
         like HF it stops at EOS (config.eos_token_id unless eos_token_id is given; None disables it):
         finished rows are padded, the call returns when every row has finished.
@@ -429,12 +472,15 @@ class VideoChatGPTLlamaForCausalLM:
         loops of 32 tokens with one host-side EOS check per loop (a single loop of exactly
         max_new_tokens when EOS is disabled). Sampling (temperature, top-k 50 as HF defaults) or
         stopping criteria take one C-ABI step per token with the host-side check the reference also
-        performs every step."""
+        performs every step.
+        attention_mask [B, S]: a left-padded batch of prompts of different lengths (module docstring); every
+        path continues the padding through its decode steps. An all-ones mask is the same as none."""
+        pads = left_padding(attention_mask, input_ids.shape)
         eng = self._ensure_engine(need_llm=True)
         ids = input_ids.cuda().to(torch.int64)
         B, S = ids.shape
         feats = video_spatio_temporal_features
-        vs = self._spans_dev(ids, feats, eng.NV)
+        vs = self._spans_dev(ids, feats, eng.NV, pads)
         if feats is not None:
             feats = feats.cuda()
         n = min(max_new_tokens, self._max_seq - S)
@@ -442,26 +488,26 @@ class VideoChatGPTLlamaForCausalLM:
             raise ValueError(f"prompt length {S} leaves no room in max_seq {self._max_seq}")
         eos, pad = self._eos_pad(eos_token_id, pad_token_id)
         if do_sample or stopping_criteria:
-            _, logits, _ = eng.prefill(ids, feats, vs, want_logits=True, want_token=False)
+            _, logits, _ = eng.prefill(ids, feats, vs, want_logits=True, want_token=False, n_pad=pads)
             self._pos = S
             self._last_out = self._stepwise(eng, ids, logits, n, do_sample, temperature, stopping_criteria, eos, pad,
                                             top_k)
             return self._last_out
         if eos is None:
-            new = eng.generate(ids, feats, vs, n).to(torch.int64)
+            new = eng.generate(ids, feats, vs, n, n_pad=pads).to(torch.int64)
             self._pos = S + n - 1
             self._last_out = torch.cat([ids, new], dim=1)
             return self._last_out
         # greedy with EOS: device loops of _GREEDY_CHUNK tokens, EOS looked for between them
         c = min(n, self._GREEDY_CHUNK)
-        new = eng.generate(ids, feats, vs, c).to(torch.int64)
+        new = eng.generate(ids, feats, vs, c, n_pad=pads).to(torch.int64)
         while True:
             new, done = self._mask_finished(new, eos, pad)
             k = new.shape[1]
             if done or k >= n:
                 break
             m = min(self._GREEDY_CHUNK, n - k)
-            more = eng.decode_loop(new[:, -1].to(torch.int32).contiguous(), S + k - 1, m + 1)
+            more = eng.decode_loop(new[:, -1].to(torch.int32).contiguous(), S + k - 1, m + 1)   # padding continues
             new = torch.cat([new, more[:, 1:].to(torch.int64)], dim=1)
         self._pos = S + new.shape[1] - 1
         self._last_out = torch.cat([ids, new], dim=1)
@@ -484,7 +530,9 @@ class VideoChatGPTLlamaForCausalLM:
         """Next turn about the SAME video(s): `new_input_ids` [B, S_new] follow everything generated
         so far. Only the tokens the KV cache does not hold yet (the last generated token and the new
         text) are prefilled (vcl_llm_prefill_append); the reference re-runs the tower and the whole
-        prompt every turn (chat.py:137-154). Returns the full sequence [B, S_total + n] like generate."""
+        prompt every turn (chat.py:137-154). Returns the full sequence [B, S_total + n] like generate.
+        After a left-padded generate the cache stays padded, so every row continues its own positions; the
+        new text of every row has the same length S_new (no padding inside a turn)."""
         if getattr(self, "_last_out", None) is None:
             raise ValueError("generate_continue: no previous generate() to continue")
         eng = self._ensure_engine(need_llm=True)
