@@ -4,17 +4,22 @@
 // V1, V3, V5-V7, J1, L1, L4-L6): both operands are K-major exactly as nn.Linear stores them
 // (activations [rows, K], weights [out, in]), so no transposes are ever materialised.
 //
-//   warpgroup 0     TMA producer : one thread issues cp.async.bulk.tensor 2-D tiles (128B swizzle) into a
-//                                  smem ring; the warpgroup hands most of its registers to the consumers
-//   warpgroups 1-2  consumers    : 64 rows each of the 128 x BLOCK_N tile, wgmma.mma_async m64nBLOCK_Nk16
-//                                  with fp32 accumulators in registers; the stage is released once the
-//                                  wgmma that read it has retired (one group kept in flight)
-//   epilogue (consumers)         : accumulators -> bias / activation / RoPE -> bf16 into a padded staging
-//                                  block in shared memory, then read back as 16-byte row chunks (+ residual)
-//                                  and stored with whole contiguous row segments per instruction
+//   warpgroup 0, warp 0, lane 0  TMA producer : issues cp.async.bulk.tensor 2-D tiles (128B swizzle) into a
+//                                               smem ring; the warpgroup hands most of its registers to the
+//                                               consumers
+//   warpgroup 0, warps 1-3       store warps  : read each staged 64-row block back as 16-byte row chunks
+//                                               (+ residual) and store whole contiguous row segments per
+//                                               instruction, while the consumers run the next tile
+//   warpgroups 1-2               consumers    : 64 rows each of the 128 x BLOCK_N tile, wgmma.mma_async
+//                                               m64nBLOCK_Nk16 with fp32 accumulators in registers; the stage is
+//                                               released once the wgmma that read it has retired (one group kept
+//                                               in flight); then accumulators -> bias / activation / RoPE -> bf16
+//                                               into their padded staging block in shared memory
 //
 // Persistent: grid = the number of CTAs (clusters) that fit at once, capped by the tile count; the producer
-// runs ahead into the next tile while the consumers drain the current one.
+// runs ahead into the next tile while the consumers stage the current one, and the store warps drain a staged
+// block while the consumers' tensor cores work on the next tile (one staging block per consumer warpgroup,
+// handed over through the staged / drained mbarriers).
 //
 // Rounding points reproduce the reference's eager bf16 path (each nn.Linear output is rounded to
 // bf16 before the following elementwise op):
@@ -28,7 +33,6 @@
 #include "kernels.h"
 
 #include <cudaTypedefs.h>
-#include <stdlib.h>
 
 namespace vcl {
 
@@ -45,17 +49,13 @@ struct GemmCfg {
   // as many ring stages as fit next to the staging block in the 227 KB a CTA may use
   static constexpr int STAGES = (BLOCK_N == 256) ? 3 : (BLOCK_N == 128 ? 5 : 8);
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + OUT_BYTES + 1024;  // +1024: manual align
-  static_assert(2 * STAGES * 8 <= BAR_BYTES, "barrier area");
+  static_assert((2 * STAGES + 4) * 8 <= BAR_BYTES, "barrier area");
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory");
 };
 
 __device__ __forceinline__ float act_gelu_erf(float x) {
   x = bf16r(x);
   return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f));
-}
-
-__device__ __forceinline__ void named_bar_sync(int id, int threads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
 // Epilogue, phase 1: this warpgroup's 64 x BLOCK_N accumulators -> bf16 outputs in the staging block
@@ -144,9 +144,14 @@ __device__ __forceinline__ void gemm_epilogue_stage(const float (&acc)[BLOCK_N /
   }
 }
 
-// Epilogue, phase 2: the staged 64-row block leaves as 16-byte chunks, consecutive threads on consecutive chunks
-// of a row (whole contiguous row segments per store instruction); the residual is added here, one more bf16
-// rounding (packed bf16x2 add). ACT_ROPE: q goes to C, k and v straight into the KV cache.
+// Epilogue, phase 2 (the store warps): the staged 64-row block leaves as 16-byte chunks, consecutive threads on
+// consecutive chunks of a row (whole contiguous row segments per store instruction); the residual is added here,
+// one more bf16 rounding (packed bf16x2 add). ACT_ROPE: q goes to C, k and v straight into the KV cache.
+// The store warps have a whole mainloop to drain a block; the residual GEMMs need 64 KB in per 128 x 256 tile,
+// so each thread first issues RES_INFLIGHT residual loads and only then adds and stores them. 96 is a multiple of
+// every chunk count per row (4 ... 32), so a store thread keeps one column chunk and walks down the rows.
+constexpr int STORE_THREADS = 96;     // warps 1-3 of warpgroup 0
+constexpr int RES_INFLIGHT = 4;       // 16-byte residual loads in flight per store thread
 template <int BLOCK_N, int ACT>
 __device__ __forceinline__ void gemm_epilogue_store(const uint8_t* stg, int t, int row_base, int n_blk, bf16* C,
                                                     long long ldc, const bf16* residual, long long ldr, int M, int N,
@@ -154,27 +159,42 @@ __device__ __forceinline__ void gemm_epilogue_store(const uint8_t* stg, int t, i
   using Cfg = GemmCfg<BLOCK_N>;
   constexpr int OUT_W = ACT == ACT_SWIGLU ? BLOCK_N / 2 : BLOCK_N;
   constexpr int CPR = OUT_W / 8;                      // 16-byte chunks per row
+  constexpr int RSTEP = STORE_THREADS / CPR;          // rows between a thread's consecutive chunks
+  static_assert(STORE_THREADS % CPR == 0, "one column chunk per store thread");
+  constexpr bool RES = ACT != ACT_ROPE && ACT != ACT_SWIGLU;
   const int n_out = ACT == ACT_SWIGLU ? N / 2 : N;
-#pragma unroll 4
-  for (int idx = t; idx < 64 * CPR; idx += 128) {
-    const int r = idx / CPR, c = idx - r * CPR;
-    const int grow = row_base + r, col = n_blk * OUT_W + c * 8;
-    if (grow >= M || col >= n_out) continue;
-    uint4 val = *reinterpret_cast<const uint4*>(stg + r * Cfg::OUT_PITCH + c * 16);
-    bf16* dst = C + (long long)grow * ldc + col;
-    if constexpr (ACT == ACT_ROPE) {
-      const int gh = col >> 7, d = col & 127;
-      const int which = gh / rp.H, head = gh - which * rp.H;
-      if (which != 0) {
-        const int gb = grow / rp.S, gs = grow - gb * rp.S;
-        dst = (which == 1 ? rp.kcache : rp.vcache) + (((long long)gb * rp.H + head) * rp.s_max + rp.start_pos + gs) * 128 + d;
+  const int c = t % CPR, col = n_blk * OUT_W + c * 8;
+  if (col >= n_out) return;
+  const int rows = min(64, M - row_base);
+  for (int r0 = t / CPR; r0 < rows; r0 += RSTEP * RES_INFLIGHT) {
+    uint4 rr[RES_INFLIGHT];
+    if (RES && residual != nullptr) {
+#pragma unroll
+      for (int u = 0; u < RES_INFLIGHT; ++u) {
+        const int r = r0 + u * RSTEP;
+        if (r < rows) rr[u] = *reinterpret_cast<const uint4*>(residual + (long long)(row_base + r) * ldr + col);
       }
-    } else if (residual != nullptr) {
-      const uint4 rr = *reinterpret_cast<const uint4*>(residual + (long long)grow * ldr + col);
-      val.x = bf16x2_add(val.x, rr.x); val.y = bf16x2_add(val.y, rr.y);
-      val.z = bf16x2_add(val.z, rr.z); val.w = bf16x2_add(val.w, rr.w);
     }
-    *reinterpret_cast<uint4*>(dst) = val;
+#pragma unroll
+    for (int u = 0; u < RES_INFLIGHT; ++u) {
+      const int r = r0 + u * RSTEP;
+      if (r >= rows) break;
+      const int grow = row_base + r;
+      uint4 val = *reinterpret_cast<const uint4*>(stg + r * Cfg::OUT_PITCH + c * 16);
+      bf16* dst = C + (long long)grow * ldc + col;
+      if constexpr (ACT == ACT_ROPE) {
+        const int gh = col >> 7, d = col & 127;
+        const int which = gh / rp.H, head = gh - which * rp.H;
+        if (which != 0) {
+          const int gb = grow / rp.S, gs = grow - gb * rp.S;
+          dst = (which == 1 ? rp.kcache : rp.vcache) + (((long long)gb * rp.H + head) * rp.s_max + rp.start_pos + gs) * 128 + d;
+        }
+      } else if (RES && residual != nullptr) {
+        val.x = bf16x2_add(val.x, rr[u].x); val.y = bf16x2_add(val.y, rr[u].y);
+        val.z = bf16x2_add(val.z, rr[u].z); val.w = bf16x2_add(val.w, rr[u].w);
+      }
+      *reinterpret_cast<uint4*>(dst) = val;
+    }
   }
 }
 
@@ -197,9 +217,18 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
   uint8_t* smem = smem_raw + pad;                 // 1024-byte aligned (SWIZZLE_128B atoms)
   const uint32_t smem_base = raw_addr + pad;
 
+  // mbarriers (BAR_BYTES): full[STAGES] | empty[STAGES] | staged[2] | drained[2].
+  //   full / empty : the operand ring; a consumer waits on full with the ring phase, the producer on empty with its
+  //                  inverse.
+  //   staged[cw]   : consumer warpgroup cw has written tile i's outputs to its staging block (128 arrivals); the
+  //                  store warps wait with phase i & 1.
+  //   drained[cw]  : the store warps have read that block out (96 arrivals); consumer warpgroup cw waits with
+  //                  phase (i - 1) & 1 before it stages tile i > 0 into the same block.
   const uint32_t bar_base = smem_base + STAGES * Cfg::STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  auto staged_bar = [&](int cw) { return bar_base + 8u * (2 * STAGES + cw); };
+  auto drained_bar = [&](int cw) { return bar_base + 8u * (2 * STAGES + 2 + cw); };
   uint8_t* stage_out = smem + STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES;
 
   const int wg = threadIdx.x >> 7;
@@ -210,6 +239,10 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 2 * CL);   // one arrival per consumer warpgroup of every CTA of the cluster
+    }
+    for (int cw = 0; cw < 2; ++cw) {
+      mbar_init(staged_bar(cw), 128);
+      mbar_init(drained_bar(cw), STORE_THREADS);
     }
     mbar_fence_init();
   }
@@ -228,7 +261,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
 
   if (wg == 0) {
     // ------------------------------ TMA producer ------------------------------
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<56>();    // the store warps keep RES_INFLIGHT residual chunks in registers
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -250,10 +283,25 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
           if (++stage == STAGES) { stage = 0; phase ^= 1u; }
         }
       }
+    } else if (threadIdx.x >= 32) {
+      // ------------------------------ store warps ------------------------------
+      const int t = threadIdx.x - 32;
+      uint32_t phase = 0;
+      for (int tile = cluster_id; tile < num_tiles; tile += n_clusters) {
+        const int m_blk = (tile / num_n) * CL + cta_rank, n_blk = tile % num_n;
+#pragma unroll 1
+        for (int cw = 0; cw < 2; ++cw) {
+          mbar_wait(staged_bar(cw), phase);
+          gemm_epilogue_store<BLOCK_N, ACT>(stage_out + cw * 64 * Cfg::OUT_PITCH, t, m_blk * Cfg::BLOCK_M + cw * 64,
+                                            n_blk, C, ldc, residual, ldr, M, N, rope);
+          mbar_arrive(drained_bar(cw));
+        }
+        phase ^= 1u;
+      }
     }
   } else {
     // ------------------------------ consumers: 64 rows each ------------------------------
-    setmaxnreg_inc<232>();
+    setmaxnreg_inc<224>();   // 56 * 128 + 224 * 256 = the 168 * 384 registers the CTA was launched with
     const int cw = wg - 1;
     const int t = threadIdx.x & 127, lane = threadIdx.x & 31, wq = t >> 5;
     uint8_t* stg = stage_out + cw * 64 * Cfg::OUT_PITCH;
@@ -269,7 +317,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
     };
     float acc[BLOCK_N / 2];
     int stage = 0;
-    uint32_t phase = 0;
+    uint32_t phase = 0, out_phase = 0;
     for (int tile = cluster_id; tile < num_tiles; tile += n_clusters) {
       const int m_blk = (tile / num_n) * CL + cta_rank, n_blk = tile % num_n;
       int prev = -1;
@@ -293,15 +341,16 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a,
       wgmma_wait<0>();
       release(prev);
       wgmma_fence_regs(acc);
-      const int row_base = m_blk * Cfg::BLOCK_M + cw * 64;
-      named_bar_sync(1 + cw, 128);                    // the previous tile's staged block has been stored
-      gemm_epilogue_stage<BLOCK_N, ACT>(acc, stg, lane, wq, row_base, n_blk, bias, M, N, rope);
-      named_bar_sync(1 + cw, 128);
-      gemm_epilogue_store<BLOCK_N, ACT>(stg, t, row_base, n_blk, C, ldc, residual, ldr, M, N, rope);
+      if (tile != cluster_id) {                       // the previous tile's staged block has been read out
+        mbar_wait(drained_bar(cw), out_phase);
+        out_phase ^= 1u;
+      }
+      gemm_epilogue_stage<BLOCK_N, ACT>(acc, stg, lane, wq, m_blk * Cfg::BLOCK_M + cw * 64, n_blk, bias, M, N, rope);
+      mbar_arrive(staged_bar(cw));                    // hand the block to the store warps, start the next tile
     }
   }
 
-  __syncthreads();
+  __syncthreads();                     // after the store warps' last store
   if (CL > 1) cluster_sync_all();      // nobody exits while a peer may still multicast / signal into it
 }
 
@@ -469,31 +518,24 @@ int launch_gemm_bf16_tn(const GemmArgs& g, cudaStream_t stream) {
   int bn = g.block_n;
   int cl = g.cluster;
   if (bn == 0) {
-    // Tile / cluster choice (heuristic, not tuned by a sweep on this GPU):
-    //  * many M tiles (ViT, batched prefill): 128x256 tiles, pairs of CTAs sharing each weight tile;
-    //  * few M tiles (single-clip prefill, M = 448): the weight stream dominates L2->SM traffic, so
-    //    all M tiles of an N tile form one cluster (multicast x4) when there are enough tiles to fill
-    //    the machine twice, else narrower tiles without a cluster to get more CTAs in flight;
-    //  * one M tile (decode with B > 4): the narrowest tile that still gives every SM work.
+    // Tile choice, from tools/sweep_gemm.py on an H100 80GB HBM3 at 400 W (DESIGN.md section 6). No cluster: the
+    // multicast clusters (CL 2 / 4) were 1.5-3x slower than CL 1 at every shape the model runs.
     const int sms = device_num_sms();
     const long long mt = (g.M + 127) / 128;
-    int auto_cl = 1;
-    if (mt >= 16 && g.N % 256 == 0) {
-      bn = 256; auto_cl = 2;
-    } else if (mt >= 2) {
-      const int mcl = mt >= 4 ? 4 : 2;
-      if (g.N % 256 == 0 && mt * (g.N / 256) >= 2 * sms) { bn = 256; auto_cl = mcl; }
-      else if (g.N % 128 == 0 && mt * (g.N / 128) >= 2 * sms) { bn = 128; auto_cl = mcl; }
-      else if (g.N % 128 == 0) { bn = 128; }
-      else { bn = (g.N % 64 == 0) ? 64 : 32; }
-    } else {
+    if (mt == 1) {
+      // one M tile (decode beyond 16 clips): the narrowest tile that still gives every SM work
       bn = 256;
-      while (bn > 32 && (g.N % bn != 0 || mt * (g.N / bn) < sms)) bn >>= 1;
+      while (bn > 32 && (g.N % bn != 0 || g.N / bn < sms)) bn >>= 1;
       if (g.N % bn != 0) bn = 32;
+    } else if (g.N % 256 == 0 && mt * (g.N / 256) >= sms && !(g.N <= 1024 && g.K <= 1024)) {
+      // enough 128 x 256 tiles for every SM: ViT qkv 305 vs 326 us (bn 128), fc1 463 vs 496, fc2 453 vs 461;
+      // prefill M = 448 q|k|v 136 vs 139, gate|up 233 vs 292; M = 7168 o 463 vs 577, down 1173 vs 1656
+      bn = 256;
+    } else {
+      // fewer 256-wide tiles than SMs (M = 448 o 46 vs 62 us, down 109 vs 140; projector 19 vs 27), or N = 1024 at
+      // K <= 1024, where 4 N tiles of 256 leave a last wave 9 % full (ViT out 136 vs 146, patch-embed 65 vs 73)
+      bn = (g.N % 128 == 0) ? 128 : (g.N % 64 == 0) ? 64 : 32;
     }
-    static const int forced_cl = getenv("VCL_GEMM_CLUSTER") ? atoi(getenv("VCL_GEMM_CLUSTER")) : 0;   // A/B switch
-    if (cl == 0) cl = forced_cl ? forced_cl : auto_cl;
-    if (forced_cl == 1 && mt >= 2 && mt < 16 && bn == 128 && g.N % 256 == 0 && mt * (g.N / 256) >= sms) bn = 256;
   }
   if (cl == 0) cl = 1;
   // cluster = -2: a CTA pair on one 256 x BLOCK_N tile, each CTA fetching half of the weight tile. sm_90 has no
