@@ -201,6 +201,25 @@ int vcl_llm_decode_loop(vcl_handle* h, const int32_t* first_tok, int B, int S, i
 int vcl_llm_generate_padded(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
                             const int32_t* n_pad_host, int B, int S, int n_new, int32_t* out_tokens, void* stream);
 
+/* forward(input_ids, labels=..., ...) (video_chatgpt/model/video_chatgpt.py:225-239): lm_head at EVERY
+ * position and, with labels, the shifted cross-entropy of CrossEntropyLoss (ignore_index -100): column s of
+ * clip b is scored against labels[b, s+1]; column S-1 has no target. The prefill is vcl_llm_prefill's
+ * (n_pad_host NULL) or vcl_llm_prefill_padded's (n_pad_host as there), and leaves the KV cache, and its
+ * padding state, exactly as that call does, so cached steps can follow.
+ *   labels      optional [B,S] int64; -100 is not scored. A label outside 0 .. vocab-1 gives a NaN row (and a
+ *               NaN loss); it is never used as an index
+ *   logits_out  optional [B,S,vocab] bf16: every position's logits, as the reference's logits tensor
+ *   nll_out     optional [B,S-1] fp32 (needs labels): -log_softmax(logits[b,s])[labels[b,s+1]], the
+ *               log-softmax computed in fp32 and rounded to bf16 as torch does on bf16 logits; 0 where the
+ *               label is -100
+ *   loss_out    optional [1] fp32 (needs labels): the mean of nll over the scored positions (NaN when
+ *               there is none, as in torch); fixed summation order, identical from run to run
+ * Work space is the handle's activation buffers: the lm_head GEMM runs over chunks of rows that fit the
+ * q|k|v activation (max_batch * max_seq * 3 * llm_hidden elements). */
+int vcl_llm_score(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
+                  const int32_t* n_pad_host, int B, int S, const int64_t* labels, void* logits_out, float* nll_out,
+                  float* loss_out, void* stream);
+
 /* Number of kernels of this library launched so far in the process (CUDA-graph replays count the
  * kernel nodes they contain). Evidence for bench.py's "gpu_launches". */
 long long vcl_launch_count(void);
@@ -218,6 +237,11 @@ int vcl_op_gemm(const void* A, int64_t lda, const void* W, int64_t ldw, void* C,
 int vcl_op_gemm_ex(const void* A, int64_t lda, const void* W, int64_t ldw, void* C, int64_t ldc,
                    const void* bias, const void* residual, int64_t ldr, int M, int N, int K, int act,
                    int block_n, int cluster, void* stream);
+/* The cross-entropy kernel of vcl_llm_score without the shift: logits [rows, ld] bf16 (first V columns
+ * used; 16-byte aligned, ld a multiple of 8), labels [rows] int64 (-100 ignored) -> nll_out [rows] fp32
+ * (required) and, optionally, loss_out [1] fp32, the mean over the rows whose label is not -100. */
+int vcl_op_cross_entropy(const void* logits, int64_t ld, const int64_t* labels, int rows, int V,
+                         float* nll_out, float* loss_out, void* stream);
 int vcl_op_layernorm(const void* x, void* y, const void* w, const void* b, int rows, int D, float eps,
                      void* stream);
 int vcl_op_rmsnorm(const void* x, void* y, const void* w, int rows, int D, float eps, void* stream);

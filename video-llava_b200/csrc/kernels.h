@@ -92,6 +92,19 @@ int launch_st_pool(const void* feats, int in_dtype, long long frame_stride, long
                    int T, int P, int C, int n_temporal, void* out, int out_dtype,
                    cudaStream_t stream);
 
+// ---- cross_entropy.cu ---------------------------------------------------------------------------
+// Rows row0 .. row0+rows-1 of a labelled batch whose logits [rows, ld] (first V columns) are at `logits`:
+// nll[i] = -bf16(log_softmax(row i)[label]) (0 for label -100 or no target, NaN for a label outside 0..V-1),
+// and logits_out [rows, V] (optional) the compact copy. Labels: labels[row] (seg == 0), or HF's shift over
+// clips of seg columns: row = clip * seg + column, scored against labels[row + 1]; the last column of a clip
+// has no target. nll may be null (labels may then be null too).
+int launch_cross_entropy(const bf16* logits, long long ld, int V, const long long* labels, long long row0, int rows,
+                         int seg, float* nll, bf16* logits_out, cudaStream_t stream);
+// loss_out[0] = mean of nll[0 .. rows) over the rows with a target (NaN when there is none), fixed order;
+// nll_out (optional): a copy of nll, [rows] (seg == 0) or [clip][seg - 1] (the last column of each clip dropped)
+int launch_nll_mean(const float* nll, const long long* labels, long long rows, int seg, float* nll_out,
+                    float* loss_out, cudaStream_t stream);
+
 // ---- attention.cu -------------------------------------------------------------------------------
 // softmax(Q K^T * scale [+ causal]) V for S_q == S_kv, bf16, fp32 softmax; element (b,h,s,d) of
 // each operand lives at base + b*sb + h*sh + s*ss + d.

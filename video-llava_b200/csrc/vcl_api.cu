@@ -110,6 +110,8 @@ struct vcl_handle {
   size_t cache_layer_elems() const {
     return (size_t)cfg.max_batch * cfg.llm_heads * cfg.max_seq * 128;
   }
+  // rows of the row-major lm_head: vocab rounded up to the 256-wide GEMM tile, the extra rows zero
+  int vocab_padded() const { return (cfg.vocab + 255) / 256 * 256; }
 };
 
 namespace {
@@ -345,7 +347,15 @@ int vcl_load_llm_weights(vcl_handle* h, const vcl_tensor* tensors, int n) {
   const long long D = c.llm_hidden, F = c.llm_inter, V = c.vocab, CV = c.clip_hidden;
   if (load_copy(h, m, "model.embed_tokens.weight", &h->embed, 2, V, D)) return -1;
   if (load_copy(h, m, "model.norm.weight", &h->norm_w, 1, D)) return -1;
-  if (load_copy(h, m, "lm_head.weight", &h->lm_head, 2, V, D)) return -1;
+  {
+    // row-major lm_head padded with zero rows to vocab_padded() (the scoring GEMM's N), decode reads the first V
+    const vcl_tensor* t = find_tensor(m, "lm_head.weight", 2, V, D);
+    if (!t) return -1;
+    const size_t Vp = h->vocab_padded();
+    if (dalloc(h, &h->lm_head, Vp * D) != 0) return -2;
+    VCL_CUDA_OK(cudaMemset(h->lm_head + (size_t)V * D, 0, (Vp - V) * D * sizeof(bf16)));
+    VCL_CUDA_OK(cudaMemcpy(h->lm_head, t->data, (size_t)V * D * sizeof(bf16), cudaMemcpyDeviceToDevice));
+  }
   if (c.proj_type == VCL_PROJ_LINEAR) {
     if (load_copy(h, m, "model.mm_projector.weight", &h->proj_w0, 2, D, CV)) return -1;
     if (load_copy(h, m, "model.mm_projector.bias", &h->proj_b0, 1, D)) return -1;
@@ -588,6 +598,37 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
   if (logits_out != nullptr || next_tok != nullptr)
     VCL_TRY(lm_head_argmax(h, h->l_h + (size_t)(S - 1) * D, (long long)S * D, B, logits_out, next_tok,
                            tok_stride, st));
+  return 0;
+}
+
+// Rows per lm_head GEMM of the scoring tail: as many [., vocab_padded] bf16 rows as the q|k|v activation
+// (max_batch * max_seq * 3D elements) holds, in whole 128-row tiles when there is room for one.
+int score_chunk_rows(const vcl_handle* h) {
+  const long long cap = (long long)h->cfg.max_batch * h->cfg.max_seq * 3 * h->cfg.llm_hidden / h->vocab_padded();
+  return (int)(cap >= 128 ? cap / 128 * 128 : cap);
+}
+
+// Scoring tail after a full-depth prefill (h->l_h: the last layer's output, B*S rows): the final RMSNorm over
+// every row into l_x, then per chunk of rows the lm_head GEMM into l_qkv (dead after the last layer) and the
+// cross-entropy kernel over it. The per-row NLL waits in l_attn (also dead) for the mean over all rows. The KV
+// cache is not touched. labels [B,S] (HF's shift: column s is scored against labels[b, s+1]) or null.
+int score_tail(vcl_handle* h, int B, int S, const int64_t* labels, bf16* logits_out, float* nll_out,
+               float* loss_out, cudaStream_t st) {
+  const vcl_config& c = h->cfg;
+  const int D = c.llm_hidden, V = c.vocab, Vp = h->vocab_padded();
+  const long long M = (long long)B * S;
+  const int chunk = score_chunk_rows(h);
+  VCL_REQUIRE(chunk > 0, "scoring needs max_batch * max_seq * 3 * llm_hidden >= %d (one padded vocabulary row)", Vp);
+  const long long* lab = reinterpret_cast<const long long*>(labels);
+  float* nll = labels != nullptr ? reinterpret_cast<float*>(h->l_attn) : nullptr;
+  VCL_TRY(launch_rmsnorm(h->l_h, D, h->l_x, D, h->norm_w, (int)M, D, c.rms_eps, st));
+  for (long long r0 = 0; r0 < M; r0 += chunk) {
+    const int m = (int)(M - r0 < chunk ? M - r0 : chunk);
+    VCL_TRY(gemm(h->l_x + r0 * D, D, h->lm_head, D, h->l_qkv, Vp, nullptr, nullptr, 0, m, Vp, D, ACT_NONE, st));
+    VCL_TRY(launch_cross_entropy(h->l_qkv, Vp, V, lab, r0, m, S, nll != nullptr ? nll + r0 : nullptr,
+                                 logits_out != nullptr ? logits_out + r0 * V : nullptr, st));
+  }
+  if (labels != nullptr) VCL_TRY(launch_nll_mean(nll, lab, M, S, nll_out, loss_out, st));
   return 0;
 }
 
@@ -868,6 +909,19 @@ int vcl_llm_generate_padded(vcl_handle* h, const int64_t* ids, const void* video
   return vcl_llm_decode_loop(h, h->tokens, B, S, n_new, out_tokens, stream);
 }
 
+int vcl_llm_score(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
+                  const int32_t* n_pad_host, int B, int S, const int64_t* labels, void* logits_out, float* nll_out,
+                  float* loss_out, void* stream) {
+  VCL_REQUIRE(h != nullptr, "vcl_llm_score: null handle");
+  VCL_REQUIRE(labels != nullptr || (nll_out == nullptr && loss_out == nullptr),
+              "vcl_llm_score: nll_out / loss_out need labels");
+  cudaStream_t st = as_stream(stream);
+  VCL_TRY(llm_prefill(h, ids, video_feats, vid_start, B, S, h->cfg.llm_layers, nullptr, nullptr, nullptr, 1, st, 0,
+                      nullptr, n_pad_host));
+  if (logits_out == nullptr && labels == nullptr) return 0;
+  return score_tail(h, B, S, labels, reinterpret_cast<bf16*>(logits_out), nll_out, loss_out, st);
+}
+
 long long vcl_launch_count(void) { return launch_count(); }
 
 // ---- single-operator entry points ----
@@ -889,6 +943,17 @@ int vcl_op_gemm_ex(const void* A, int64_t lda, const void* W, int64_t ldw, void*
   return gemm(reinterpret_cast<const bf16*>(A), lda, reinterpret_cast<const bf16*>(W), ldw,
               reinterpret_cast<bf16*>(C), ldc, reinterpret_cast<const bf16*>(bias),
               reinterpret_cast<const bf16*>(residual), ldr, M, N, K, act, as_stream(stream), block_n, cluster);
+}
+
+int vcl_op_cross_entropy(const void* logits, int64_t ld, const int64_t* labels, int rows, int V, float* nll_out,
+                         float* loss_out, void* stream) {
+  if (check_device() != 0) return -2;
+  VCL_REQUIRE(logits != nullptr && labels != nullptr && nll_out != nullptr,
+              "vcl_op_cross_entropy: logits, labels and nll_out are required");
+  const long long* lab = reinterpret_cast<const long long*>(labels);
+  VCL_TRY(launch_cross_entropy(reinterpret_cast<const bf16*>(logits), ld, V, lab, 0, rows, 0, nll_out, nullptr,
+                               as_stream(stream)));
+  return loss_out != nullptr ? launch_nll_mean(nll_out, lab, rows, 0, nullptr, loss_out, as_stream(stream)) : 0;
 }
 
 int vcl_op_layernorm(const void* x, void* y, const void* w, const void* b, int rows, int D, float eps,

@@ -66,7 +66,10 @@ _SIGNATURES = {
                                        c_void_p, c_void_p, c_void_p, c_void_p]),
     "vcl_llm_generate_padded": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_int,
                                         c_void_p, c_void_p]),
+    "vcl_llm_score": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_void_p,
+                              c_void_p, c_void_p, c_void_p, c_void_p]),
     "vcl_launch_count": (ctypes.c_longlong, []),
+    "vcl_op_cross_entropy": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_op_gemm": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
                             c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "vcl_op_gemm_ex": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
@@ -176,6 +179,19 @@ def op_attention_vit(qkv, n_frames, S, H):
     out = torch.empty(n_frames * S, H * 64, dtype=torch.bfloat16, device=qkv.device)
     check(lib().vcl_op_attention_vit(ptr(qkv), ptr(out), n_frames, S, H, cur_stream()))
     return out
+
+
+def op_cross_entropy(logits, labels, V=None, want_loss=True):
+    """logits [rows, ld] bf16 (the first V columns, default all; row pitch a multiple of 8), labels [rows] int64
+    (-100 ignored) -> (nll [rows] fp32, loss 0-d fp32 | None); see vcl_op_cross_entropy."""
+    rows, ld = logits.shape
+    assert logits.dtype == torch.bfloat16 and logits.stride(1) == 1
+    lab = labels.to(device=logits.device, dtype=torch.int64).contiguous()
+    nll = torch.empty(rows, dtype=torch.float32, device=logits.device)
+    loss = torch.empty((), dtype=torch.float32, device=logits.device) if want_loss else None
+    check(lib().vcl_op_cross_entropy(c_void_p(logits.data_ptr()), logits.stride(0), ptr(lab), rows,
+                                     ld if V is None else V, ptr(nll), ptr(loss), cur_stream()))
+    return nll, loss
 
 
 def op_gemv(x, w, res=None, norm_w=None, eps=0.0):
@@ -311,6 +327,28 @@ class Engine:
                                                _host_pads(n_pad, B), B, S, nl, ptr(hidden), ptr(logits), ptr(tok),
                                                cur_stream()))
         return hidden, logits, tok
+
+    def score(self, ids, video_feats, vid_start, labels=None, n_pad=None, want_logits=False):
+        """Full-depth prefill with lm_head at every position (vcl_llm_score). labels [B, S] (-100 ignored; HF's
+        shift: column s is scored against labels[:, s+1]). Returns (logits [B,S,vocab] bf16 | None,
+        nll [B,S-1] fp32 | None, loss 0-d fp32 | None); nll and loss need labels. n_pad as in prefill."""
+        B, S = ids.shape
+        dev = ids.device
+        logits = torch.empty(B, S, self.cfg.vocab, dtype=torch.bfloat16, device=dev) if want_logits else None
+        nll = loss = lab = None
+        if labels is not None:
+            lab = labels.to(device=dev, dtype=torch.int64).contiguous()
+            assert lab.shape == (B, S), lab.shape
+            nll = torch.empty(B, S - 1, dtype=torch.float32, device=dev)
+            loss = torch.empty((), dtype=torch.float32, device=dev)
+        vf = None
+        if video_feats is not None:
+            vf = video_feats.to(torch.bfloat16).contiguous()
+            assert vf.shape == (B, self.NV, self.cfg.clip_hidden), vf.shape
+        pads = None if n_pad is None else _host_pads(n_pad, B)
+        check(lib().vcl_llm_score(self._h, ptr(ids.contiguous()), ptr(vf), ptr(vid_start.contiguous()), pads, B, S,
+                                  ptr(lab), ptr(logits), ptr(nll), ptr(loss), cur_stream()))
+        return logits, nll, loss
 
     def prefill_states(self, ids, video_feats, vid_start, want_logits=False):
         """Full-depth prefill keeping every hidden state: ([L+1, B, S, D] bf16 raw layer outputs,

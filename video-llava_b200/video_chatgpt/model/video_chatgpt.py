@@ -13,7 +13,9 @@ the reference does (same ValueError texts for malformed video spans) and transla
 conventions. Differences from the reference, all documented where they occur:
   * compute dtype is bf16 (BASELINE.json); `.half()` is accepted and ignored;
   * `forward` returns logits for the LAST position only, shape [B,1,V] (the reference materialises
-    [B,S,V] and every caller on this path reads [:, -1]);
+    [B,S,V] and every caller on this path reads [:, -1]), unless it is given `labels` (then, as the
+    reference, the loss and [B,S,V]) or `logits_to_keep=0` ([B,S,V]). With labels, a right-padded mask
+    (train.py's collator) is accepted as well as a left-padded one (score_padding below);
   * the vision tower's `hidden_states` are lazy: an entry is computed when indexed (the path reads [-2]);
     the language model's `hidden_states` are the L+1 tensors HF returns (the last one after the final
     RMSNorm), produced by ONE prefill pass;
@@ -107,13 +109,8 @@ class VideoChatGPTConfig:
         return cls(**j)
 
 
-def left_padding(attention_mask, shape) -> list | None:
-    """Pad count per row of a left-padded batch from its HF attention_mask ([B, S], bool or integer 0/1):
-    each row must be zeros followed by ones, with at least one 1. Returns None when nothing is padded
-    (an all-ones mask: the unpadded path), else the list of B pad counts. Raises ValueError otherwise;
-    it runs on the host, before any device work."""
-    if attention_mask is None:
-        return None
+def _mask_bool(attention_mask, shape) -> torch.Tensor:
+    """HF attention_mask ([B, S], bool or integer 0/1) -> a bool tensor on the host; ValueError otherwise"""
     m = torch.as_tensor(attention_mask).detach().cpu()
     B, S = int(shape[0]), int(shape[1])
     if tuple(m.shape) != (B, S):
@@ -122,6 +119,65 @@ def left_padding(attention_mask, shape) -> list | None:
         if m.is_floating_point() or m.is_complex() or not bool(((m == 0) | (m == 1)).all()):
             raise ValueError("attention_mask must be bool or integer 0/1")
         m = m != 0
+    return m
+
+
+def score_padding(attention_mask, labels, shape, vocab: int) -> list | None:
+    """Host-side checks of forward(labels=...), before any device work. labels [B, S] must hold ids in
+    [0, vocab) or -100 (IGNORE_INDEX). The mask may be left padding (-> the B pad counts, the padded prefill) or
+    right padding, the layout of train.py's collator (pad_sequence with labels padded by -100) -> None: the batch
+    runs unpadded, which under causal attention gives every real column exactly what its row alone gives.
+    Every pad column must be labelled -100; with left padding so must the first real token, since no real position
+    predicts it. Raises ValueError otherwise."""
+    B, S = int(shape[0]), int(shape[1])
+    lab = torch.as_tensor(labels).detach().cpu()
+    if tuple(lab.shape) != (B, S):
+        raise ValueError(f"labels have shape {tuple(lab.shape)}, input_ids {(B, S)}")
+    if lab.is_floating_point() or lab.is_complex() or lab.dtype == torch.bool:
+        raise ValueError(f"labels must be integer ids, got {lab.dtype}")
+    lab = lab.to(torch.int64)
+    bad = ~(((lab >= 0) & (lab < vocab)) | (lab == -100))
+    if bool(bad.any()):
+        b, s = (int(i) for i in bad.nonzero()[0])
+        raise ValueError(f"labels[{b}, {s}] = {int(lab[b, s])} is neither a token id in [0, {vocab}) nor -100")
+    if attention_mask is None:
+        return None
+    m = _mask_bool(attention_mask, shape)
+    pads, right = [], False
+    for b in range(B):
+        row = m[b]
+        n_real = int(row.sum())
+        if n_real == 0:
+            raise ValueError(f"attention_mask row {b} has no real token")
+        if bool(row[S - n_real:].all()):
+            pads.append(S - n_real)                     # left padding (or none)
+        elif bool(row[:n_real].all()):
+            pads.append(0)                              # right padding
+            right = True
+        else:
+            raise ValueError(f"attention_mask row {b} has holes: only left or right padding is supported")
+    if right and any(pads):
+        raise ValueError("attention_mask mixes left- and right-padded rows")
+    need_ignore = ~m
+    for b, n in enumerate(pads):
+        if n > 0:
+            need_ignore[b, n] = True
+    if bool((lab[need_ignore] != -100).any()):
+        b, s = (int(i) for i in (need_ignore & (lab != -100)).nonzero()[0])
+        raise ValueError(f"labels[{b}, {s}] = {int(lab[b, s])} lies on a pad column (or, with left padding, on the "
+                         "first real token, which no real position predicts): it must be -100")
+    return pads if any(pads) else None
+
+
+def left_padding(attention_mask, shape) -> list | None:
+    """Pad count per row of a left-padded batch from its HF attention_mask ([B, S], bool or integer 0/1):
+    each row must be zeros followed by ones, with at least one 1. Returns None when nothing is padded
+    (an all-ones mask: the unpadded path), else the list of B pad counts. Raises ValueError otherwise;
+    it runs on the host, before any device work."""
+    if attention_mask is None:
+        return None
+    m = _mask_bool(attention_mask, shape)
+    B, S = int(shape[0]), int(shape[1])
     pads = []
     for b in range(B):
         row = m[b]
@@ -396,11 +452,19 @@ class VideoChatGPTLlamaForCausalLM:
     @torch.no_grad()
     def forward(self, input_ids=None, attention_mask=None, past_key_values=None, inputs_embeds=None, labels=None,
                 use_cache=None, output_attentions=None, output_hidden_states=None,
-                video_spatio_temporal_features=None, return_dict=None):
-        if inputs_embeds is not None or labels is not None or output_attentions:
+                video_spatio_temporal_features=None, return_dict=None, logits_to_keep=1):
+        """logits_to_keep (transformers 5.x's name): 1, the default, returns the last position's logits [B,1,V];
+        0 returns every position's [B,S,V]. labels [B,S] (train.py's IGNORE_INDEX -100 on prompt and padding)
+        returns the reference's loss, a 0-d bf16 tensor, with the logits of every position (vcl_llm_score)."""
+        if inputs_embeds is not None or output_attentions:
             raise NotImplementedError("inference path only: input_ids in, logits out")
+        if logits_to_keep not in (0, 1):
+            raise NotImplementedError(f"logits_to_keep={logits_to_keep}: only 1 (last position) and 0 (all positions)")
         B, S = input_ids.shape
         cached_step = S == 1 and past_key_values is not None
+        if labels is not None or (logits_to_keep == 0 and not cached_step):
+            return self._score(input_ids, attention_mask, labels, cached_step, output_hidden_states,
+                               video_spatio_temporal_features)
         # a cached step ignores the mask: the KV cache carries the padding of its prefill
         pads = None if cached_step else left_padding(attention_mask, (B, S))
         if pads is not None and output_hidden_states:
@@ -433,6 +497,28 @@ class VideoChatGPTLlamaForCausalLM:
                                hidden_states=hs, attentions=None)
 
     __call__ = forward
+
+    def _score(self, input_ids, attention_mask, labels, cached_step, output_hidden_states, feats):
+        """forward with labels and / or every position's logits: one vcl_llm_score call"""
+        if cached_step:
+            raise NotImplementedError("labels on a cached single-token step are not supported")
+        if output_hidden_states:
+            raise NotImplementedError("output_hidden_states together with labels or logits_to_keep=0 is not supported")
+        B, S = input_ids.shape
+        if labels is not None:
+            pads = score_padding(attention_mask, labels, (B, S), self.config.vocab_size)
+        else:
+            pads = left_padding(attention_mask, (B, S))
+        eng = self._ensure_engine(need_llm=True)
+        ids = input_ids.cuda().to(torch.int64)
+        vs = self._spans_dev(ids, feats, eng.NV, pads)
+        if feats is not None:
+            feats = feats.cuda()
+        lab = None if labels is None else torch.as_tensor(labels).cuda().to(torch.int64)
+        logits, _, loss = eng.score(ids, feats, vs, labels=lab, n_pad=pads, want_logits=True)
+        self._pos = S
+        return SimpleNamespace(loss=None if loss is None else loss.to(torch.bfloat16), logits=logits,
+                               past_key_values=self._pos, hidden_states=None, attentions=None)
 
     def prepare_inputs_for_generation(self, input_ids, past_key_values=None, attention_mask=None,
                                       inputs_embeds=None, **kwargs):
