@@ -201,6 +201,30 @@ int vcl_llm_decode_loop(vcl_handle* h, const int32_t* first_tok, int B, int S, i
 int vcl_llm_generate_padded(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
                             const int32_t* n_pad_host, int B, int S, int n_new, int32_t* out_tokens, void* stream);
 
+/* In-flight (continuous) batching: every clip of the KV cache is a SLOT that holds its own sequence at its own
+ * length, so a finished request's slot takes the next queued request while the other slots keep decoding.
+ * There are min(max_batch, 16) slots (the decode ring kernels take up to 16 clips per launch). Slots are
+ * unpadded.
+ *
+ * vcl_llm_slot_prefill: vcl_llm_prefill of ONE prompt (ids [1,S], video_feats [1, n_temporal+P, 1024] or NULL,
+ * vid_start [1]) into cache slot `slot` (0 <= slot < min(max_batch, 16)). The slot then holds positions
+ * 0 .. S-1; no other slot's cache columns are read or written. next_tok [1] int32: the arg-max at the last
+ * position. Like vcl_llm_prefill it clears the cache's left padding (vcl_llm_prefill_padded): the other slots
+ * must be (re)started with vcl_llm_slot_prefill before they are decoded. */
+int vcl_llm_slot_prefill(vcl_handle* h, int slot, const int64_t* ids, const void* video_feats,
+                         const int32_t* vid_start, int S, int32_t* next_tok, void* stream);
+
+/* vcl_llm_decode_loop with a position per slot: slot b (0 <= b < n_slots) is fed first_tok[b] at position
+ * pos_host[b] (HOST memory: the number of tokens its cache holds), then runs n_new-1 greedy steps;
+ * out_tokens is [n_slots, n_new] int32, first_tok included. Every pos_host[b] + n_new - 1 must be <= max_seq
+ * (checked before any device work). A slot without a request is computed like any other; its tokens are
+ * meaningless and it writes only its own cache columns (park it at position 0). The positions are copied to
+ * a device array of the handle at a fixed address, so one CUDA graph per (n_slots, n_new) serves every set of
+ * positions (the same graph cache as vcl_llm_decode_loop). 1 <= n_slots <= min(max_batch, 16); a left-padded
+ * cache is rejected. */
+int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* pos_host, int n_slots, int n_new,
+                        int32_t* out_tokens, void* stream);
+
 /* forward(input_ids, labels=..., ...) (video_chatgpt/model/video_chatgpt.py:225-239): lm_head at EVERY
  * position and, with labels, the shifted cross-entropy of CrossEntropyLoss (ignore_index -100): column s of
  * clip b is scored against labels[b, s+1]; column S-1 has no target. The prefill is vcl_llm_prefill's

@@ -148,8 +148,11 @@ __device__ __forceinline__ void warp_argmax(float& v, int& i) {
 }
 
 // ---- epilogue items: the fp32 dot product(s) of one row (pair) and clip b -> outputs ----
-// position of the new token: pos + *pos_dev (one captured graph for every prompt length)
-__device__ __forceinline__ int decode_pos(const GemvEpilogue& e) {
+// position of clip b's new token: pos + *pos_dev (one captured graph for every prompt length), or with SLOT
+// (every cache slot at its own position) pos + pos_dev[b]
+template <bool SLOT>
+__device__ __forceinline__ int decode_pos(const GemvEpilogue& e, int b) {
+  if (SLOT) return e.pos + __ldg(e.pos_dev + b);
   return e.pos + (e.pos_dev != nullptr ? __ldg(e.pos_dev) : 0);
 }
 // RES: out[b][row] = bf16(bf16(v) + res[b][row])
@@ -178,7 +181,7 @@ __device__ __forceinline__ void epi_swiglu(const GemvEpilogue& e, int b, int row
 // QKV: row = (which*H + head)*128 + 2*d holds dims (d, d + 64) of q, k or v (RoPE pairs adjacent); q and k are
 // rotated, q goes to q_out, k and v to the cache at column pos. With left padding (e.n_pad) the rotation angle is
 // that of position pos - n_pad[b]; the cache column stays pos. PAD: the kernel instance of a padded cache (the
-// unpadded instances keep the code they had before padding existed).
+// unpadded instances keep the code they had before padding existed). The caller passes clip b's position.
 template <bool PAD>
 __device__ __forceinline__ void epi_qkv_rope(const GemvEpilogue& e, int b, int row, int pos, float v0, float v1) {
   const int hr = row >> 7;
@@ -211,9 +214,9 @@ __device__ __forceinline__ long long qkv_row(int v) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// 1..4 clips
+// 1..4 clips. PAD / SLOT: the q|k|v instances of a padded cache / of per-slot positions (never both)
 // ---------------------------------------------------------------------------------------------
-template <bool PAD>
+template <bool PAD, bool SLOT>
 __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   // layout: ring[n_slots] | x[nb][K] bf16 (+ norm weights [K]) | pbuf[2][CWARPS][16][4] | result[r_cap][4] fp32
@@ -543,7 +546,7 @@ __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
       if (mode == GEMV_RES) epi_residual(e, b, vrow, v0);
       else if (mode == GEMV_LOGITS) epi_logit(e, b, vrow, v0);
       else if (mode == GEMV_SWIGLU) epi_swiglu(e, b, vrow, NB, v0, v1);
-      else epi_qkv_rope<PAD>(e, b, vrow, decode_pos(e), v0, v1);
+      else epi_qkv_rope<PAD>(e, b, vrow, decode_pos<SLOT>(e, b), v0, v1);
     }
   }
   if (mode == GEMV_LOGITS && a.amax_out != nullptr) {
@@ -578,9 +581,9 @@ __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
 
 // ---------------------------------------------------------------------------------------------
 // 5..16 clips. NG = upper bound of the row groups a CTA owns (the accumulator arrays are sized and
-// unrolled by it); a.x holds the activations in the xwin layout
+// unrolled by it); a.x holds the activations in the xwin layout. PAD / SLOT as for gemv_tc_kernel
 // ---------------------------------------------------------------------------------------------
-template <int NG, bool PAD>
+template <int NG, bool PAD, bool SLOT>
 __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, const GemvEpilogue e) {
   extern __shared__ __align__(128) uint8_t smem[];
   // layout: ring[8] (after the main loop: partial tiles [warp][group]) | x windows [4][16][1088 B] | barriers
@@ -730,7 +733,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
   // in a fixed order.
   const int mode = e.mode;
   const bool pairs = (mode == GEMV_SWIGLU || mode == GEMV_QKV);
-  const int pos = decode_pos(e);
+  const int pos = decode_pos<false>(e, 0);
   auto tile_sum = [&](int lg, int el) {
     float v = tiles[(size_t)lg * TW_TILE + el];
 #pragma unroll
@@ -756,7 +759,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
       if (b >= NB || vrow >= N) continue;
       const float v0 = tile_sum(lg, rr * 17 + b), v1 = tile_sum(lg, (rr + 1) * 17 + b);
       if (mode == GEMV_SWIGLU) epi_swiglu(e, b, vrow, NB, v0, v1);
-      else epi_qkv_rope<PAD>(e, b, vrow, pos, v0, v1);
+      else epi_qkv_rope<PAD>(e, b, vrow, SLOT ? decode_pos<true>(e, b) : pos, v0, v1);
     }
   }
 }
@@ -841,9 +844,18 @@ int launch_tc(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
   }
   cudaLaunchAttribute attr[1];
   cudaLaunchConfig_t cfg = pdl_config(grid, smem, stream, attr);
-  VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, e.n_pad != nullptr ? gemv_tc_kernel<true> : gemv_tc_kernel<false>, p));
+  auto kern = e.n_pad != nullptr ? gemv_tc_kernel<true, false>
+                                 : (e.pos_per_clip ? gemv_tc_kernel<false, true> : gemv_tc_kernel<false, false>);
+  VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p));
   count_launches(1);
   return 0;
+}
+
+// the gemv_tcw instance of NG row groups for the epilogue's position mode
+template <int NG>
+auto tcw_kernel(const GemvEpilogue& e) {
+  return e.n_pad != nullptr ? gemv_tcw_kernel<NG, true, false>
+                            : (e.pos_per_clip ? gemv_tcw_kernel<NG, false, true> : gemv_tcw_kernel<NG, false, false>);
 }
 
 // RES / LOGITS over more than 14 row groups per SM (the lm_head): consecutive launches over near-equal
@@ -870,11 +882,10 @@ int launch_tcw(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
     cudaLaunchAttribute attr[1];
     cudaLaunchConfig_t cfg = pdl_config(grid, TW_SMEM, stream, attr);
     const int ng_max = (g1 - g0 + grid - 1) / grid;                  // groups of the busiest CTA
-    const bool pad = e.n_pad != nullptr;
-    auto kern = pad ? gemv_tcw_kernel<TW_NG_MAX, true> : gemv_tcw_kernel<TW_NG_MAX, false>;
-    if (ng_max <= 2) kern = pad ? gemv_tcw_kernel<2, true> : gemv_tcw_kernel<2, false>;
-    else if (ng_max <= 6) kern = pad ? gemv_tcw_kernel<6, true> : gemv_tcw_kernel<6, false>;
-    else if (ng_max <= 10) kern = pad ? gemv_tcw_kernel<10, true> : gemv_tcw_kernel<10, false>;
+    auto kern = tcw_kernel<TW_NG_MAX>(e);
+    if (ng_max <= 2) kern = tcw_kernel<2>(e);
+    else if (ng_max <= 6) kern = tcw_kernel<6>(e);
+    else if (ng_max <= 10) kern = tcw_kernel<10>(e);
     VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, sa, se));
     count_launches(1);
   }
@@ -898,11 +909,14 @@ extern "C" int vcl_debug_tc_trace_dump(const char* path) {
 }
 
 int init_gemv_kernels() {
-  for (auto k : {gemv_tc_kernel<false>, gemv_tc_kernel<true>})
+  for (auto k : {gemv_tc_kernel<false, false>, gemv_tc_kernel<true, false>, gemv_tc_kernel<false, true>})
     VCL_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-  for (auto k : {gemv_tcw_kernel<2, false>, gemv_tcw_kernel<6, false>, gemv_tcw_kernel<10, false>,
-                 gemv_tcw_kernel<TW_NG_MAX, false>, gemv_tcw_kernel<2, true>, gemv_tcw_kernel<6, true>,
-                 gemv_tcw_kernel<10, true>, gemv_tcw_kernel<TW_NG_MAX, true>})
+  for (auto k : {gemv_tcw_kernel<2, false, false>, gemv_tcw_kernel<6, false, false>, gemv_tcw_kernel<10, false, false>,
+                 gemv_tcw_kernel<TW_NG_MAX, false, false>, gemv_tcw_kernel<2, true, false>,
+                 gemv_tcw_kernel<6, true, false>, gemv_tcw_kernel<10, true, false>,
+                 gemv_tcw_kernel<TW_NG_MAX, true, false>, gemv_tcw_kernel<2, false, true>,
+                 gemv_tcw_kernel<6, false, true>, gemv_tcw_kernel<10, false, true>,
+                 gemv_tcw_kernel<TW_NG_MAX, false, true>})
     VCL_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
   return 0;
 }
@@ -940,6 +954,8 @@ int launch_gemv(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
   VCL_REQUIRE(e.mode != GEMV_SWIGLU || a.N % 2 == 0, "gemv swiglu: N must be even (interleaved gate/up rows)");
   VCL_REQUIRE(e.mode != GEMV_QKV || a.N == 3 * e.H * 128, "gemv qkv: N=%d != 3*H*128", a.N);
   VCL_REQUIRE(e.n_pad == nullptr || e.mode == GEMV_QKV, "gemv: left padding applies to the q|k|v epilogue only");
+  VCL_REQUIRE(!e.pos_per_clip || (e.mode == GEMV_QKV && e.pos_dev != nullptr && e.n_pad == nullptr),
+              "gemv: per-slot positions apply to the unpadded q|k|v epilogue and need pos_dev");
   VCL_REQUIRE(a.embed == nullptr || (a.vocab > 0 && (a.tok_in != nullptr || (a.amax_in != nullptr && a.amax_n > 0))),
               "gemv: the fused embedding gather needs a token source");
   return a.B <= 4 ? launch_tc(a, e, stream) : launch_tcw(a, e, stream);

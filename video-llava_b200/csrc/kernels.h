@@ -138,7 +138,8 @@ int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, c
                             bf16* o, long long o_ld, int B, int H, int head_dim, int s_max,
                             int kv_len, float scale, cudaStream_t stream, const int* pos_dev = nullptr,
                             bool o_xwin = false,    // o_xwin: the output [B][H*hd] is written in xwin layout
-                            const int* n_pad = nullptr);   // keys n_pad[b] .. kv_len-1 only
+                            const int* n_pad = nullptr,    // keys n_pad[b] .. kv_len-1 only
+                            bool pos_per_clip = false);    // kv_len + pos_dev[b] keys per clip (unpadded)
 
 // ---- decode_gemv.cu : decode-time weight streaming (1..16 new tokens) -------------------------------
 // Two ring kernels (bulk-copy ring over a slot-ordered copy of the matrix + mma.sync) behind one launcher:
@@ -182,7 +183,8 @@ struct GemvEpilogue {
   bf16* kcache = nullptr; bf16* vcache = nullptr;
   const bf16* cos_t = nullptr; const bf16* sin_t = nullptr;
   int H = 0, s_max = 0, pos = 0;
-  const int* pos_dev = nullptr;                 // position = pos + *pos_dev
+  const int* pos_dev = nullptr;                 // position = pos + *pos_dev ...
+  bool pos_per_clip = false;                    // ... or, QKV unpadded, clip b at pos + pos_dev[b] (cache slots)
   const int* n_pad = nullptr;                   // QKV: [B] left padding, RoPE angle at position - n_pad[b]
   float* logits = nullptr; long long ldl = 0;   // LOGITS
 };

@@ -51,6 +51,7 @@ struct LlmLayerW {
 struct GraphEntry {
   int B, S, n_new;     // S = -1: the prompt length is read on the device (h->d_pos), any S replays it
   bool padded;         // captured with the left-padding array (h->d_npad): replays only for a padded cache
+  bool slots;          // captured with per-slot positions (h->d_slot_pos): replays only for vcl_llm_slot_decode
   cudaGraphExec_t exec;
   long long kernels;   // kernel nodes in the graph (for vcl_launch_count)
   unsigned long long last_use;
@@ -65,7 +66,8 @@ struct StepIo {
   bool partials_out = false;      // leave this step's arg-max as per-CTA partials for the next step (no arg-max kernel)
   float* logits_out = nullptr;
   int32_t* tok_out = nullptr; long long out_stride = 1;
-  const int* pos_dev = nullptr;   // position = pos + *pos_dev
+  const int* pos_dev = nullptr;   // position = pos + *pos_dev ...
+  bool pos_per_clip = false;      // ... or clip b at pos + pos_dev[b] (cache slots, 1..16 clips, unpadded)
 };
 
 }  // namespace
@@ -105,6 +107,9 @@ struct vcl_handle {
   int* d_npad = nullptr;                       // [max_batch]
   bool padded = false;
   int npad_max = 0;                            // largest pad count of the padded batch (host copy)
+  // Cache slots (vcl_llm_slot_prefill / vcl_llm_slot_decode): clip b of the cache is a slot of its own, fed at
+  // position d_slot_pos[b]. Fixed address, so a captured slot graph serves every set of positions.
+  int* d_slot_pos = nullptr;                   // [max_batch]
   ArgmaxPart* amax = nullptr;                  // [gemv_grid(vocab)][max_batch] per-CTA partial arg-max of the logits kernel
 
   size_t cache_layer_elems() const {
@@ -112,6 +117,8 @@ struct vcl_handle {
   }
   // rows of the row-major lm_head: vocab rounded up to the 256-wide GEMM tile, the extra rows zero
   int vocab_padded() const { return (cfg.vocab + 255) / 256 * 256; }
+  // cache slots: as many as clips the decode ring kernels take in one launch
+  int n_slots_max() const { return cfg.max_batch < 16 ? cfg.max_batch : 16; }
 };
 
 namespace {
@@ -261,6 +268,7 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   rc |= dalloc(h, &h->d_act, xwin_elems((int)Bm, (int)LF) > Bm * LF ? xwin_elems((int)Bm, (int)LF) : Bm * LF);
   rc |= dalloc(h, &h->d_pos, 4);
   rc |= dalloc(h, &h->d_npad, Bm);
+  rc |= dalloc(h, &h->d_slot_pos, Bm);
   rc |= dalloc(h, &h->amax, (size_t)device_num_sms() * Bm);
   if (rc == 0) rc = launch_rope_table(h->rope_cos, h->rope_sin, c->max_seq, 128, c->rope_theta, 0);
   if (rc == 0) {
@@ -505,13 +513,17 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
 // layer i; entry 0 the spliced input embeddings), copied out as the stack advances.
 // A new sequence (start_pos == 0) sets the cache's left padding: n_pad_host [B] (host memory), or none when it is
 // null or all zero. A continuation keeps the padding of the cache.
+// slot > 0 (B = 1): the sequence goes to clip `slot` of the cache; every layer's cache base moves by that many
+// clips, and no other clip's columns are read or written.
 int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
                 int B, int S, int n_layers, void* hidden_out, float* logits_out, int32_t* next_tok,
                 long long tok_stride, cudaStream_t st, int start_pos = 0, void* states_out = nullptr,
-                const int32_t* n_pad_host = nullptr) {
+                const int32_t* n_pad_host = nullptr, int slot = 0) {
   const vcl_config& c = h->cfg;
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
   VCL_REQUIRE(B > 0 && B <= c.max_batch, "B=%d outside 1..%d", B, c.max_batch);
+  VCL_REQUIRE(slot == 0 || (B == 1 && slot > 0 && slot < c.max_batch), "slot %d needs B = 1 and a clip of the cache",
+              slot);
   VCL_REQUIRE(S > 0 && start_pos >= 0 && start_pos + S <= c.max_seq, "positions %d..%d outside the cache (max_seq %d)",
               start_pos, start_pos + S - 1, c.max_seq);
   VCL_REQUIRE(n_layers >= 0 && n_layers <= c.llm_layers, "n_layers=%d outside 0..%d", n_layers, c.llm_layers);
@@ -539,6 +551,9 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
   const int* np = h->padded ? h->d_npad : nullptr;
   const int D = c.llm_hidden, F = c.llm_inter, H = c.llm_heads, NV = h->NV;
   const int M = B * S;
+  const size_t slot_off = (size_t)slot * H * c.max_seq * 128;
+  auto kc = [&](int l) { return kc_layer(h, l) + slot_off; };
+  auto vc = [&](int l) { return vc_layer(h, l) + slot_off; };
   if (video_feats != nullptr) {
     const bf16* vf = reinterpret_cast<const bf16*>(video_feats);
     if (c.proj_type == VCL_PROJ_LINEAR) {
@@ -571,18 +586,18 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
       GemmArgs g;
       g.A = h->l_x; g.lda = D; g.W = w.wqkv; g.ldw = D; g.C = h->l_qkv; g.ldc = 3 * D; g.M = M; g.N = 3 * D; g.K = D;
       g.act = ACT_ROPE;
-      g.rope.cos_t = h->rope_cos; g.rope.sin_t = h->rope_sin; g.rope.kcache = kc_layer(h, l); g.rope.vcache = vc_layer(h, l);
+      g.rope.cos_t = h->rope_cos; g.rope.sin_t = h->rope_sin; g.rope.kcache = kc(l); g.rope.vcache = vc(l);
       g.rope.S = S; g.rope.start_pos = start_pos; g.rope.H = H; g.rope.s_max = c.max_seq; g.rope.n_pad = np;
       VCL_TRY(launch_gemm_bf16_tn(g, st));
     } else {
       VCL_TRY(gemm(h->l_x, D, w.wqkv, D, h->l_qkv, 3 * D, nullptr, nullptr, 0, M, 3 * D, D, ACT_NONE, st));
-      VCL_TRY(launch_rope_kv_prefill(h->l_qkv, kc_layer(h, l), vc_layer(h, l), h->rope_cos, h->rope_sin, B,
+      VCL_TRY(launch_rope_kv_prefill(h->l_qkv, kc(l), vc(l), h->rope_cos, h->rope_sin, B,
                                      S, H, 128, c.max_seq, start_pos, st, nullptr, np));
     }
     AttnArgs a;
     a.q = h->l_qkv; a.q_sb = (long long)S * 3 * D; a.q_sh = 128; a.q_ss = 3 * D;
-    a.k = kc_layer(h, l); a.k_sb = (long long)H * c.max_seq * 128; a.k_sh = (long long)c.max_seq * 128; a.k_ss = 128;
-    a.v = vc_layer(h, l); a.v_sb = a.k_sb; a.v_sh = a.k_sh; a.v_ss = 128;
+    a.k = kc(l); a.k_sb = (long long)H * c.max_seq * 128; a.k_sh = (long long)c.max_seq * 128; a.k_ss = 128;
+    a.v = vc(l); a.v_sb = a.k_sb; a.v_sh = a.k_sh; a.v_ss = 128;
     a.o = h->l_attn; a.o_sb = (long long)S * D; a.o_sh = 128; a.o_ss = D;
     a.B = B; a.H = H; a.S = S; a.head_dim = 128; a.scale = scale; a.causal = 1;
     a.S_kv = start_pos + S; a.q_off = start_pos; a.n_pad = np;
@@ -632,7 +647,7 @@ int score_tail(vcl_handle* h, int B, int S, const int64_t* labels, bf16* logits_
   return 0;
 }
 
-// One decode step: the token of io is fed at position pos (+ *io.pos_dev).
+// One decode step: the token of io is fed at position pos (+ *io.pos_dev, or + io.pos_dev[b] per clip).
 int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_t st) {
   const vcl_config& c = h->cfg;
   const int D = c.llm_hidden, F = c.llm_inter, H = c.llm_heads;
@@ -640,6 +655,8 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
   const int* pd = io.pos_dev;
   const int* np = h->padded ? h->d_npad : nullptr;   // a padded cache stays padded
   VCL_REQUIRE(pos >= 0 && pos < c.max_seq, "decode position %d outside the cache (max_seq %d)", pos, c.max_seq);
+  VCL_REQUIRE(!io.pos_per_clip || (pd != nullptr && np == nullptr && B <= 16),
+              "per-slot positions need 1..16 unpadded clips");
   VCL_REQUIRE(pd != nullptr || pos >= h->npad_max, "decode position %d lies inside the left padding (%d columns)",
               pos, h->npad_max);
   // 1..4 clips: the embedding lookup is part of layer 0's q|k|v kernel (and with it the arg-max of the
@@ -680,10 +697,10 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
       GemvEpilogue qkv;
       qkv.mode = GEMV_QKV; qkv.q_out = h->d_q; qkv.ldq = D; qkv.kcache = kc_layer(h, l); qkv.vcache = vc_layer(h, l);
       qkv.cos_t = h->rope_cos; qkv.sin_t = h->rope_sin; qkv.H = H; qkv.s_max = c.max_seq; qkv.pos = pos; qkv.pos_dev = pd;
-      qkv.n_pad = np;
+      qkv.pos_per_clip = io.pos_per_clip; qkv.n_pad = np;
       VCL_TRY(launch_gemv(g, qkv, st));
       VCL_TRY(launch_decode_attention(h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->d_attn, D, B, H, 128,
-                                      c.max_seq, pos + 1, scale, st, pd, /*o_xwin=*/wide, np));
+                                      c.max_seq, pos + 1, scale, st, pd, /*o_xwin=*/wide, np, io.pos_per_clip));
       GemvArgs go;
       go.x = h->d_attn; go.ldx = D; go.W_tiled = w.wo_t; go.B = B; go.N = D; go.K = D;
       VCL_TRY(launch_gemv(go, residual, st));
@@ -719,11 +736,13 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
 // For 1..4 clips no arg-max / embedding kernel runs between two steps: the logits kernel leaves
 // per-CTA partials, the next step's first q|k|v kernel reduces them, records the token and gathers
 // its embedding row.
-int decode_steps(vcl_handle* h, int32_t* tk, int B, int S, int n_new, const int* pos_dev, cudaStream_t st) {
+// pos_dev: the positions on the device (per_clip: one per clip), S the shared position otherwise.
+int decode_steps(vcl_handle* h, int32_t* tk, int B, int S, int n_new, const int* pos_dev, bool per_clip,
+                 cudaStream_t st) {
   const bool hand_off = B <= 4 && h->cfg.llm_layers > 0;
   for (int i = 1; i < n_new; ++i) {
     StepIo io;
-    io.pos_dev = pos_dev;
+    io.pos_dev = pos_dev; io.pos_per_clip = per_clip;
     if (hand_off && i > 1) {
       io.tok_from_partials = true; io.tok_store = tk + (i - 1); io.store_stride = n_new;
     } else {
@@ -733,6 +752,57 @@ int decode_steps(vcl_handle* h, int32_t* tk, int B, int S, int n_new, const int*
     else { io.tok_out = tk + i; io.out_stride = n_new; }
     VCL_TRY(llm_decode_step(h, io, B, (pos_dev ? 0 : S) + i - 1, st));
   }
+  return 0;
+}
+
+// decode_steps from one captured graph per (B, n_new, padded, slots). The shared prompt length S reaches the
+// kernels through h->d_pos, the pad counts through h->d_npad and, with `slots`, the per-slot positions through
+// h->d_slot_pos (written by the caller), so new positions or padding replay the same graph. Bounded LRU cache
+// (an entry holds thousands of nodes). A stream that cannot be captured runs the steps eagerly.
+int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int S, int n_new, bool slots, cudaStream_t st) {
+  const int* pos_dev = slots ? h->d_slot_pos : h->d_pos;
+  GraphEntry* ge = nullptr;
+  for (auto& g : h->graphs)
+    if (g.B == B && g.n_new == n_new && g.S == -1 && g.padded == h->padded && g.slots == slots) ge = &g;
+  const bool can_capture = (st != nullptr) && (st != cudaStreamLegacy);
+  if (ge == nullptr && can_capture) {
+    if (h->graphs.size() >= MAX_DECODE_GRAPHS) {
+      size_t victim = 0;
+      for (size_t i = 1; i < h->graphs.size(); ++i)
+        if (h->graphs[i].last_use < h->graphs[victim].last_use) victim = i;
+      cudaGraphExecDestroy(h->graphs[victim].exec);
+      h->graphs.erase(h->graphs.begin() + victim);
+    }
+    const long long before = launch_count();
+    VCL_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    const int rc = decode_steps(h, tk, B, S, n_new, pos_dev, slots, st);
+    cudaGraph_t graph = nullptr;
+    cudaError_t e = cudaStreamEndCapture(st, &graph);
+    const long long nodes = launch_count() - before;
+    count_launches(-nodes);  // captured, not executed
+    if (rc != 0) {
+      if (graph) cudaGraphDestroy(graph);
+      return rc;
+    }
+    if (e != cudaSuccess) {
+      set_last_error("decode graph capture failed: %s", cudaGetErrorString(e));
+      return -2;
+    }
+    cudaGraphExec_t exec = nullptr;
+    e = cudaGraphInstantiate(&exec, graph, 0);
+    cudaGraphDestroy(graph);
+    if (e != cudaSuccess) {
+      set_last_error("decode graph instantiate failed: %s", cudaGetErrorString(e));
+      return -2;
+    }
+    h->graphs.push_back({B, -1, n_new, h->padded, slots, exec, nodes, 0});
+    ge = &h->graphs.back();
+  }
+  if (ge == nullptr) return decode_steps(h, tk, B, S, n_new, slots ? pos_dev : nullptr, slots, st);
+  ge->last_use = ++h->graph_clock;
+  if (!slots) VCL_TRY(launch_set_int(h->d_pos, S, st));
+  VCL_CUDA_OK(cudaGraphLaunch(ge->exec, st));
+  count_launches(ge->kernels);
   return 0;
 }
 
@@ -824,57 +894,46 @@ int vcl_llm_decode_loop(vcl_handle* h, const int32_t* first_tok, int B, int S, i
   if (first_tok != tk)
     VCL_CUDA_OK(cudaMemcpy2DAsync(tk, (size_t)n_new * sizeof(int32_t), first_tok, sizeof(int32_t),
                                   sizeof(int32_t), B, cudaMemcpyDeviceToDevice, st));
-  if (n_new > 1) {
-    // One graph per (B, n_new, padded): the prompt length S reaches the kernels through h->d_pos and the pad
-    // counts through h->d_npad, so a new prompt length or padding replays the same graph. Bounded LRU cache (an
-    // entry holds thousands of nodes).
-    GraphEntry* ge = nullptr;
-    for (auto& g : h->graphs)
-      if (g.B == B && g.n_new == n_new && g.S == -1 && g.padded == h->padded) ge = &g;
-    const bool can_capture = (st != nullptr) && (st != cudaStreamLegacy);
-    if (ge == nullptr && can_capture) {
-      if (h->graphs.size() >= MAX_DECODE_GRAPHS) {
-        size_t victim = 0;
-        for (size_t i = 1; i < h->graphs.size(); ++i)
-          if (h->graphs[i].last_use < h->graphs[victim].last_use) victim = i;
-        cudaGraphExecDestroy(h->graphs[victim].exec);
-        h->graphs.erase(h->graphs.begin() + victim);
-      }
-      const long long before = launch_count();
-      VCL_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      const int rc = decode_steps(h, tk, B, S, n_new, h->d_pos, st);
-      cudaGraph_t graph = nullptr;
-      cudaError_t e = cudaStreamEndCapture(st, &graph);
-      const long long nodes = launch_count() - before;
-      count_launches(-nodes);  // captured, not executed
-      if (rc != 0) {
-        if (graph) cudaGraphDestroy(graph);
-        return rc;
-      }
-      if (e != cudaSuccess) {
-        set_last_error("decode graph capture failed: %s", cudaGetErrorString(e));
-        return -2;
-      }
-      cudaGraphExec_t exec = nullptr;
-      e = cudaGraphInstantiate(&exec, graph, 0);
-      cudaGraphDestroy(graph);
-      if (e != cudaSuccess) {
-        set_last_error("decode graph instantiate failed: %s", cudaGetErrorString(e));
-        return -2;
-      }
-      h->graphs.push_back({B, -1, n_new, h->padded, exec, nodes, 0});
-      ge = &h->graphs.back();
-    }
-    if (ge != nullptr) {
-      ge->last_use = ++h->graph_clock;
-      VCL_TRY(launch_set_int(h->d_pos, S, st));
-      VCL_CUDA_OK(cudaGraphLaunch(ge->exec, st));
-      count_launches(ge->kernels);
-    } else {
-      VCL_TRY(decode_steps(h, tk, B, S, n_new, nullptr, st));
-    }
-  }
+  if (n_new > 1) VCL_TRY(run_decode_steps(h, tk, B, S, n_new, /*slots=*/false, st));
   VCL_CUDA_OK(cudaMemcpyAsync(out_tokens, tk, (size_t)B * n_new * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
+int vcl_llm_slot_prefill(vcl_handle* h, int slot, const int64_t* ids, const void* video_feats,
+                         const int32_t* vid_start, int S, int32_t* next_tok, void* stream) {
+  VCL_REQUIRE(h && ids && vid_start && next_tok, "vcl_llm_slot_prefill: null argument");
+  VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
+  VCL_REQUIRE(slot >= 0 && slot < h->n_slots_max(), "vcl_llm_slot_prefill: slot %d outside 0..%d (max_batch %d, at "
+              "most 16 slots)", slot, h->n_slots_max() - 1, h->cfg.max_batch);
+  return llm_prefill(h, ids, video_feats, vid_start, 1, S, h->cfg.llm_layers, nullptr, nullptr, next_tok, 1,
+                     as_stream(stream), 0, nullptr, nullptr, slot);
+}
+
+int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* pos_host, int n_slots, int n_new,
+                        int32_t* out_tokens, void* stream) {
+  VCL_REQUIRE(h && first_tok && pos_host && out_tokens, "vcl_llm_slot_decode: null argument");
+  VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
+  VCL_REQUIRE(n_slots >= 1 && n_slots <= h->n_slots_max(), "vcl_llm_slot_decode: n_slots=%d outside 1..%d (max_batch "
+              "%d, at most 16 slots)", n_slots, h->n_slots_max(), h->cfg.max_batch);
+  VCL_REQUIRE(!h->padded, "vcl_llm_slot_decode: the cache is left-padded; slots are unpadded (start each one with "
+              "vcl_llm_slot_prefill)");
+  VCL_REQUIRE(n_new >= 1 && n_new <= h->cfg.max_seq, "vcl_llm_slot_decode: n_new=%d outside 1..max_seq %d", n_new,
+              h->cfg.max_seq);
+  for (int b = 0; b < n_slots; ++b)
+    VCL_REQUIRE(pos_host[b] >= 0 && pos_host[b] + n_new - 1 <= h->cfg.max_seq,
+                "vcl_llm_slot_decode: slot %d: pos %d + n_new - 1 = %d exceeds max_seq %d", b, pos_host[b],
+                pos_host[b] + n_new - 1, h->cfg.max_seq);
+  cudaStream_t st = as_stream(stream);
+  int32_t* tk = h->tokens;  // [n_slots, n_new] row-major scratch
+  VCL_CUDA_OK(cudaMemcpy2DAsync(tk, (size_t)n_new * sizeof(int32_t), first_tok, sizeof(int32_t), sizeof(int32_t),
+                                n_slots, cudaMemcpyDeviceToDevice, st));
+  if (n_new > 1) {
+    VCL_CUDA_OK(cudaMemcpyAsync(h->d_slot_pos, pos_host, (size_t)n_slots * sizeof(int32_t), cudaMemcpyHostToDevice,
+                                st));
+    VCL_TRY(run_decode_steps(h, tk, n_slots, 0, n_new, /*slots=*/true, st));
+  }
+  VCL_CUDA_OK(cudaMemcpyAsync(out_tokens, tk, (size_t)n_slots * n_new * sizeof(int32_t), cudaMemcpyDeviceToDevice,
+                              st));
   return 0;
 }
 

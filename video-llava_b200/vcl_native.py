@@ -68,6 +68,8 @@ _SIGNATURES = {
                                         c_void_p, c_void_p]),
     "vcl_llm_score": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_void_p,
                               c_void_p, c_void_p, c_void_p, c_void_p]),
+    "vcl_llm_slot_prefill": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "vcl_llm_slot_decode": (c_int, [c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_void_p, c_void_p]),
     "vcl_launch_count": (ctypes.c_longlong, []),
     "vcl_op_cross_entropy": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_op_gemm": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
@@ -405,4 +407,33 @@ class Engine:
         else:
             check(lib().vcl_llm_generate_padded(self._h, ptr(ids.contiguous()), ptr(vf), ptr(vid_start.contiguous()),
                                                 _host_pads(n_pad, B), B, S, n_new, ptr(out), cur_stream()))
+        return out
+
+    # ---- cache slots (in-flight batching) ----
+    def slot_prefill(self, slot, ids, video_feats, vid_start, tok_out=None):
+        """One prompt ids [1, S] (or [S]) into cache slot `slot` (vcl_llm_slot_prefill); video_feats [NV, C] /
+        [1, NV, C] or None, vid_start [1] int32. Returns its first token, [1] int32 on the device (tok_out if
+        given)."""
+        ids = ids.reshape(1, -1).contiguous()
+        tok = tok_out if tok_out is not None else torch.empty(1, dtype=torch.int32, device=ids.device)
+        vf = None
+        if video_feats is not None:
+            vf = video_feats.to(torch.bfloat16).reshape(1, *video_feats.shape[-2:]).contiguous()
+            assert vf.shape == (1, self.NV, self.cfg.clip_hidden), vf.shape
+        check(lib().vcl_llm_slot_prefill(self._h, int(slot), ptr(ids), ptr(vf), ptr(vid_start.contiguous()),
+                                         ids.shape[1], ptr(tok), cur_stream()))
+        return tok
+
+    def slot_decode(self, first_tok, positions, n_new, out=None):
+        """Slot b is fed first_tok[b] (device int32 [n_slots]) at positions[b] (host ints: the tokens its cache
+        holds) and runs n_new-1 greedy steps (vcl_llm_slot_decode); returns [n_slots, n_new] int32, first token
+        included."""
+        n = first_tok.shape[0]
+        pos = list(positions)
+        if len(pos) != n:
+            raise VclError(f"{len(pos)} positions for {n} slots")
+        if out is None:
+            out = torch.empty(n, n_new, dtype=torch.int32, device=first_tok.device)
+        check(lib().vcl_llm_slot_decode(self._h, ptr(first_tok.contiguous()), (c_int32 * n)(*[int(p) for p in pos]), n,
+                                        n_new, ptr(out), cur_stream()))
         return out

@@ -27,6 +27,7 @@ conventions. Differences from the reference, all documented where they occur:
 """
 from __future__ import annotations
 
+import collections
 import json
 import os
 import sys
@@ -610,6 +611,114 @@ class VideoChatGPTLlamaForCausalLM:
             first = is_eos.to(torch.int32).argmax(dim=1)
             return new[:, : int(first.max()) + 1], True
         return new, False
+
+    # decode steps per slot_decode call of generate_requests between two host-side checks. 8 measured best with
+    # tools/bench_inflight.py (64 requests, 16..384 tokens, 7B shapes, H100 at 400 W): 7.89 / 8.13 / 8.35 s for 8 /
+    # 16 / 32 at 16 slots, 19.5 / 19.9 / 20.7 s at 4 -- a retired slot idles for the rest of its chunk
+    _SLOT_CHUNK = 8
+
+    @torch.no_grad()
+    def generate_requests(self, requests, max_new_tokens=32, eos_token_id="config", stopping_criteria=None,
+                          slots=None, do_sample=False):
+        """Greedy generation for many independent requests by in-flight (continuous) batching: every request
+        owns a slot of the KV cache while it runs, and a finished request's slot takes the next queued one at
+        once while the other slots keep decoding (a static batch decodes until its longest row finishes).
+
+        requests: each a dict with "input_ids" [S_i] or [1, S_i], optionally "video_spatio_temporal_features"
+        (the pooled [100+P, 1024] features of its video), "max_new_tokens" and "stopping_criteria" (a list, e.g.
+        the reference's KeywordsStoppingCriteria built for this prompt); a bare tensor is a prompt alone. The
+        keyword arguments are the defaults of requests that do not set their own; a shared stopping criterion is
+        called with every request's own sequence, so it must not keep per-prompt state.
+        Returns a list in request order: request i's [1, S_i + n_i] int64, prompt included, as generate returns
+        it for that request alone. A request ends at its first EOS, at its max_new_tokens, or at the first token
+        where one of its stopping criteria fires (called token by token with the [1, S_i + k] prefix on the host,
+        as a stepwise generate would call it).
+        slots: cache slots in flight, default and at most min(max_batch, 16). Requests are admitted one prefill
+        at a time; all slots then decode _SLOT_CHUNK steps per device call. Everything is validated before any
+        device work. Afterwards there is no turn for generate_continue to continue."""
+        if do_sample:
+            raise NotImplementedError("generate_requests decodes greedily; sampling runs on generate")
+        cap = min(self._max_batch, 16)
+        n_slots = cap if slots is None else int(slots)
+        if not 1 <= n_slots <= cap:
+            raise ValueError(f"slots={slots} outside 1..{cap} (at most 16 and at most max_batch {self._max_batch})")
+        eng = self._ensure_engine(need_llm=True)
+        reqs = [self._request(i, r, max_new_tokens, stopping_criteria, eng.NV) for i, r in enumerate(requests)]
+        eos, _ = self._eos_pad(eos_token_id, None)
+        self._last_out, self._pos = None, 0
+        dev = self.device
+        n_slots = min(n_slots, len(reqs))
+        results = [None] * len(reqs)
+        queue = collections.deque(range(len(reqs)))
+        owner = [None] * n_slots            # request of each slot
+        pos = [0] * n_slots                 # tokens in each slot's cache; a slot without a request is parked at 0
+        unseen = [False] * n_slots          # the slot's first token (from its prefill) has not reached the host yet
+        gen = {}                            # request -> its new tokens so far
+        first = torch.zeros(n_slots, dtype=torch.int32, device=dev)     # the token each slot is fed next
+        while True:
+            for s in range(n_slots):
+                if owner[s] is None and queue:
+                    i = queue.popleft()
+                    r = reqs[i]
+                    feats = None if r.feats is None else r.feats.to(dev)
+                    vs = torch.tensor([r.vid_start], dtype=torch.int32, device=dev)
+                    eng.slot_prefill(s, r.ids.to(dev), feats, vs, tok_out=first[s:s + 1])
+                    owner[s], pos[s], unseen[s], gen[i] = i, r.S, True, []
+            active = [s for s in range(n_slots) if owner[s] is not None]
+            if not active:
+                return results
+            # shorter than a chunk only when a slot nears max_seq
+            m = min([self._SLOT_CHUNK] + [self._max_seq - pos[s] for s in active])
+            out = eng.slot_decode(first, pos, m + 1)
+            first = out[:, m].contiguous()
+            host = out.tolist()
+            for s in active:
+                i = owner[s]
+                r = reqs[i]
+                pos[s] += m
+                for t in (host[s] if unseen[s] else host[s][1:]):
+                    gen[i].append(t)
+                    if self._request_done(r, gen[i], eos):
+                        results[i] = torch.cat([r.ids, torch.tensor(gen[i], dtype=torch.int64)])[None].to(dev)
+                        owner[s], pos[s] = None, 0
+                        break
+                unseen[s] = False
+
+    def _request(self, i, r, max_new_tokens, stopping_criteria, n_vid):
+        """One request of generate_requests, checked on the host -> (ids [S] int64 on the host, S, n, feats,
+        vid_start, criteria)"""
+        if isinstance(r, torch.Tensor):
+            r = {"input_ids": r}
+        ids = torch.as_tensor(r["input_ids"]).detach().cpu().to(torch.int64)
+        if ids.dim() == 2 and ids.shape[0] == 1:
+            ids = ids[0]
+        if ids.dim() != 1 or ids.numel() == 0:
+            raise ValueError(f"request {i}: input_ids must be [S] or [1, S], got shape {tuple(ids.shape)}")
+        S, n = ids.numel(), int(r.get("max_new_tokens", max_new_tokens))
+        if n < 1 or S + n > self._max_seq:
+            raise ValueError(f"request {i}: prompt length {S} + max_new_tokens {n} does not fit max_seq {self._max_seq}")
+        feats, vs = r.get("video_spatio_temporal_features"), vn.NO_VIDEO
+        if feats is not None:
+            if feats.dim() == 3 and feats.shape[0] == 1:
+                feats = feats[0]
+            if feats.dim() != 2 or feats.shape[0] != n_vid:
+                raise ValueError(f"request {i}: video_spatio_temporal_features must be [{n_vid}, C], got "
+                                 f"{tuple(feats.shape)}")
+            vs = self._video_spans(ids[None], n_vid)[0]
+        crit = r.get("stopping_criteria", stopping_criteria)
+        return SimpleNamespace(ids=ids, S=S, n=n, feats=feats, vid_start=vs, criteria=list(crit or []))
+
+    @staticmethod
+    def _request_done(r, gen, eos):
+        """Whether the request ends with its newest token gen[-1]: EOS, then the stopping criteria, then the
+        length limit, in the order of _stepwise"""
+        if eos is not None and gen[-1] == eos:
+            return True
+        if r.criteria:
+            seq = torch.cat([r.ids, torch.tensor(gen, dtype=torch.int64)])[None]
+            if any(c(seq, None) for c in r.criteria):
+                return True
+        return len(gen) >= r.n
 
     def generate_continue(self, new_input_ids, do_sample=False, temperature=1.0, max_new_tokens=32,
                           stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50):
