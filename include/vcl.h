@@ -191,8 +191,8 @@ int vcl_llm_generate(vcl_handle* h, const int64_t* ids, const void* video_feats,
 /* The decode half of vcl_llm_generate on its own (so a caller can time prefill and decode
  * separately): first_tok [B] int32 is the token produced by the prefill; runs n_new-1 cached steps
  * at positions S, S+1, ... and writes [B, n_new] (first_tok included) to out_tokens. It continues the
- * cache's left padding, if any; the graph cache is keyed by (B, n_new, padded or not), and one padded graph
- * serves every set of pad counts (they are read from device memory). */
+ * cache's left padding, if any; the graph cache is keyed by (B, n_new) alone, because the positions and the
+ * pad counts are read from device memory: one graph serves every S and every padding. */
 int vcl_llm_decode_loop(vcl_handle* h, const int32_t* first_tok, int B, int S, int n_new,
                         int32_t* out_tokens, void* stream);
 
@@ -220,8 +220,8 @@ int vcl_llm_slot_prefill(vcl_handle* h, int slot, const int64_t* ids, const void
  * (checked before any device work). A slot without a request is computed like any other; its tokens are
  * meaningless and it writes only its own cache columns (park it at position 0). The positions are copied to
  * a device array of the handle at a fixed address, so one CUDA graph per (n_slots, n_new) serves every set of
- * positions (the same graph cache as vcl_llm_decode_loop). 1 <= n_slots <= min(max_batch, 16); a left-padded
- * cache is rejected. */
+ * positions; it is the graph vcl_llm_decode_loop uses for (B = n_slots, n_new). 1 <= n_slots <= min(max_batch,
+ * 16); a left-padded cache is rejected. */
 int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* pos_host, int n_slots, int n_new,
                         int32_t* out_tokens, void* stream);
 

@@ -286,33 +286,39 @@ def test_errors_before_any_device_work(small_state):
 
 @torch.no_grad()
 def test_graph_is_reused_for_other_positions(small_state):
-    """A second slot_decode with other positions replays the captured graph: the launch count grows by the same
-    node count, the call is a replay (no capture or instantiation on the host), and its tokens are those of a fresh
-    engine at those positions."""
+    """A second slot_decode with other positions, and then a decode_loop with the same (B, n_new), replay the graph
+    the first call captured: the launch count grows by the same node count, each call is a replay (no capture or
+    instantiation on the host), and its tokens are those of a fresh engine doing the same call."""
     NB, k = 3, 8
     eng = make_engine(llm=SMALL, max_batch=NB, max_seq=480)
     eng.load_llm(small_state)
     fresh = make_engine(llm=SMALL, max_batch=NB, max_seq=480)
     fresh.load_llm(small_state)
     rows = [text_prompt(400 + b, 30 + 11 * b) for b in range(NB)]
+    S = len(rows[0]) - 9        # the shared position: every slot's columns below it hold its prompt in both engines
     st = torch.cuda.Stream()
-    deltas, host_ms = [], []
+    deltas, host_ms, outs = [], [], []
     with torch.cuda.stream(st):
         first = torch.cat([admit(eng, b, r, None) for b, r in enumerate(rows)])
         first_f = torch.cat([admit(fresh, b, r, None) for b, r in enumerate(rows)])
         st.synchronize()
-        for posv in ([len(r) for r in rows], [len(r) - 9 for r in rows]):
+        for call in (lambda: eng.slot_decode(first, [len(r) for r in rows], k),
+                     lambda: eng.slot_decode(first, [len(r) - 9 for r in rows], k),
+                     lambda: eng.decode_loop(first, S, k)):
             n0 = vn.launch_count()
             ev = torch.cuda.Event()
             t0 = time.perf_counter()
-            out = eng.slot_decode(first, posv, k)
+            outs.append(call())
             host_ms.append((time.perf_counter() - t0) * 1e3)
             ev.record(st)
             ev.synchronize()
             deltas.append(vn.launch_count() - n0)
         # the second call fed each slot at len - 9: a fresh engine whose slots hold the same prompts does the same
         ref = fresh.slot_decode(first_f, [len(r) - 9 for r in rows], k)
+        ref_loop = fresh.decode_loop(first_f, S, k)
     st.synchronize()
-    assert deltas[0] == deltas[1] > (k - 1) * SMALL.layers, deltas
-    assert host_ms[1] < 0.5 * host_ms[0], host_ms
-    assert torch.equal(out, ref)
+    # decode_loop launches one kernel of its own before the graph: the fill of the shared position
+    assert deltas[0] == deltas[1] == deltas[2] - 1 > (k - 1) * SMALL.layers, deltas
+    assert host_ms[1] < 0.5 * host_ms[0] and host_ms[2] < 0.5 * host_ms[0], host_ms
+    assert torch.equal(outs[1], ref)
+    assert torch.equal(outs[2], ref_loop)

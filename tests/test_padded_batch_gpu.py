@@ -189,8 +189,9 @@ def test_padded_prefill_flash_variant_at_short_prompts(monkeypatch):
 
 @torch.no_grad()
 def test_padding_state_does_not_leak_into_plain_runs():
-    """A padded generate, then a plain generate with the same (B, n_new) on the same engine: the plain run must
-    not replay the padded decode graph (nor the reverse) -- its tokens equal a fresh engine's."""
+    """A padded generate, then a plain generate with the same (B, n_new) on the same engine: both replay one decode
+    graph, which reads the pad counts from the device, so the plain run must find them cleared (and the padded run
+    after it set again) -- its tokens equal a fresh engine's."""
     sd = to_dev(O.random_llm_state(SMALL, seed=21))
     ids_p, pads, _ = padded_batch(SMALL, [63, 35, 50], seed=90)
     ids_u = O.make_prompt_ids(SMALL, 356, seed=91, batch=3).to(DEV)

@@ -49,9 +49,8 @@ __device__ __forceinline__ float block_reduce(float v, bool is_max, float* scrat
 
 // DA_SPLIT = CTAs per (clip, head): 4 for few clips (latency: more CTAs than SMs are needed to fill the
 // machine at all), 2 or 1 when clips x heads alone oversubscribe it (throughput: fewer barriers per byte).
-// PAD: left-padded clips (n_pad): the keys of clip b are n_pad[b] .. kv_len-1, split over the CTAs as above.
-// SLOT: every clip (cache slot) at its own position, kv_len + pos_dev[b] keys (unpadded; never with PAD)
-template <int DA_SPLIT, bool PAD, bool SLOT>
+// The keys of clip b, n_pad[b] .. kv_len + pos_dev[b] - 1 (kernels.h: decode positions), are split over the CTAs.
+template <int DA_SPLIT>
 __global__ void __launch_bounds__(DA_THREADS)
 decode_attn_cluster_kernel(const bf16* __restrict__ q, long long q_ld, const bf16* __restrict__ kcache,
                            const bf16* __restrict__ vcache, bf16* __restrict__ o, long long o_ld, int H,
@@ -61,11 +60,11 @@ decode_attn_cluster_kernel(const bf16* __restrict__ q, long long q_ld, const bf1
   float* sc = sm;                       // [per_cap] scores -> probabilities of my keys
   float* red = sm + per_cap;            // [16][128] partial outputs over the 16 key groups
   const int h = blockIdx.y, b = blockIdx.z;
-  // the number of cached keys may live on the device (one captured graph for every prompt length);
-  // it is constant while the graph runs, so it can be read before the dependency wait. So is the left
-  // padding of the clip: its first k0 cache columns hold pad keys, which are neither read nor split
-  if (pos_dev != nullptr) kv_len += __ldg(pos_dev + (SLOT ? b : 0));
-  const int k0 = PAD ? __ldg(n_pad + b) : 0;
+  // the clip's position and key floor live on the device (one captured graph for every position and padding);
+  // they are constant while the graph runs, so they can be read before the dependency wait. The first k0
+  // cache columns hold pad keys, which are neither read nor split
+  if (pos_dev != nullptr) kv_len += __ldg(pos_dev + b);
+  const int k0 = __ldg(n_pad + b);
   const int per = ((kv_len - k0 + DA_SPLIT - 1) / DA_SPLIT + 15) / 16 * 16;   // keys per CTA, multiple of 16
   float* outp = red + 16 * 128;         // [128] this CTA's partial output
   float* stat = outp + 128;             // [0] local max, [1] local sum
@@ -183,22 +182,14 @@ decode_attn_cluster_kernel(const bf16* __restrict__ q, long long q_ld, const bf1
   cluster_sync_all();   // keep every CTA's shared memory alive until rank 0 has read it
 }
 
-// the instance of DA_SPLIT CTAs per head for the position mode
-template <int DA_SPLIT>
-auto decode_attn_kernel(bool pad, bool slot) {
-  return pad ? decode_attn_cluster_kernel<DA_SPLIT, true, false>
-             : (slot ? decode_attn_cluster_kernel<DA_SPLIT, false, true> : decode_attn_cluster_kernel<DA_SPLIT, false, false>);
-}
-
 }  // namespace
 
 int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, const bf16* vcache,
                             bf16* o, long long o_ld, int B, int H, int head_dim, int s_max,
                             int kv_len, float scale, cudaStream_t stream, const int* pos_dev, bool o_xwin,
-                            const int* n_pad, bool pos_per_clip) {
+                            const int* n_pad) {
   VCL_REQUIRE(head_dim == 128, "decode attention: head_dim must be 128");
-  VCL_REQUIRE(!pos_per_clip || (pos_dev != nullptr && n_pad == nullptr),
-              "decode attention: per-slot positions need pos_dev and an unpadded cache");
+  VCL_REQUIRE(n_pad != nullptr, "decode attention: needs the key floors n_pad");
   VCL_REQUIRE(kv_len > 0 && kv_len <= s_max, "decode attention: kv_len %d out of range", kv_len);
   // shared memory is sized for the longest sequence when the length is only known on the device
   const int kv_cap = pos_dev != nullptr ? s_max : kv_len;
@@ -222,10 +213,9 @@ int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, c
   attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 2;
-  const bool pad = n_pad != nullptr;
-  auto kern = decode_attn_kernel<4>(pad, pos_per_clip);
-  if (split == 2) kern = decode_attn_kernel<2>(pad, pos_per_clip);
-  if (split == 1) kern = decode_attn_kernel<1>(pad, pos_per_clip);
+  auto kern = decode_attn_cluster_kernel<4>;
+  if (split == 2) kern = decode_attn_cluster_kernel<2>;
+  if (split == 1) kern = decode_attn_cluster_kernel<1>;
   VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, q, q_ld, kcache, vcache, o, o_ld, H, s_max, kv_len, per, scale, pos_dev,
                                  o_xwin ? 1 : 0, n_pad));
   count_launches(1);

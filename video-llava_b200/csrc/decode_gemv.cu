@@ -148,13 +148,6 @@ __device__ __forceinline__ void warp_argmax(float& v, int& i) {
 }
 
 // ---- epilogue items: the fp32 dot product(s) of one row (pair) and clip b -> outputs ----
-// position of clip b's new token: pos + *pos_dev (one captured graph for every prompt length), or with SLOT
-// (every cache slot at its own position) pos + pos_dev[b]
-template <bool SLOT>
-__device__ __forceinline__ int decode_pos(const GemvEpilogue& e, int b) {
-  if (SLOT) return e.pos + __ldg(e.pos_dev + b);
-  return e.pos + (e.pos_dev != nullptr ? __ldg(e.pos_dev) : 0);
-}
 // RES: out[b][row] = bf16(bf16(v) + res[b][row])
 __device__ __forceinline__ void epi_residual(const GemvEpilogue& e, int b, int row, float v) {
   float y = bf16r(v);
@@ -179,21 +172,24 @@ __device__ __forceinline__ void epi_swiglu(const GemvEpilogue& e, int b, int row
   e.out[o] = __float2bfloat16_rn(sg * bf16r(up));
 }
 // QKV: row = (which*H + head)*128 + 2*d holds dims (d, d + 64) of q, k or v (RoPE pairs adjacent); q and k are
-// rotated, q goes to q_out, k and v to the cache at column pos. With left padding (e.n_pad) the rotation angle is
-// that of position pos - n_pad[b]; the cache column stays pos. PAD: the kernel instance of a padded cache (the
-// unpadded instances keep the code they had before padding existed). The caller passes clip b's position.
-template <bool PAD>
-__device__ __forceinline__ void epi_qkv_rope(const GemvEpilogue& e, int b, int row, int pos, float v0, float v1) {
+// rotated by the angle of max(col - floor, 0), q goes to q_out, k and v to the cache at column col. The caller
+// passes clip b's column (decode_col) and key floor n_pad[b], so that both loads are issued before the epilogue's
+// dependent chain (kernels.h: decode positions).
+__device__ __forceinline__ int decode_col(const GemvEpilogue& e, int b) {
+  return e.pos + (e.pos_dev != nullptr ? __ldg(e.pos_dev + b) : 0);
+}
+__device__ __forceinline__ void epi_qkv_rope(const GemvEpilogue& e, int b, int row, int col, int floor, float v0,
+                                             float v1) {
   const int hr = row >> 7;
   const int which = hr / e.H, head = hr - which * e.H;
   const int d = (row & 127) >> 1;
   const float lo = bf16r(v0), hi = bf16r(v1);
-  const long long coff = (((long long)b * e.H + head) * e.s_max + pos) * 128;
+  const long long coff = (((long long)b * e.H + head) * e.s_max + col) * 128;
   if (which == 2) {
     e.vcache[coff + d] = __float2bfloat16_rn(lo);
     e.vcache[coff + d + 64] = __float2bfloat16_rn(hi);
   } else {
-    const int rpos = PAD ? max(pos - __ldg(e.n_pad + b), 0) : pos;
+    const int rpos = max(col - floor, 0);
     const float cs = __bfloat162float(e.cos_t[(long long)rpos * 64 + d]);
     const float sn = __bfloat162float(e.sin_t[(long long)rpos * 64 + d]);
     const float olo = bf16r(lo * cs) + bf16r(-hi * sn);
@@ -214,9 +210,8 @@ __device__ __forceinline__ long long qkv_row(int v) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// 1..4 clips. PAD / SLOT: the q|k|v instances of a padded cache / of per-slot positions (never both)
+// 1..4 clips
 // ---------------------------------------------------------------------------------------------
-template <bool PAD, bool SLOT>
 __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   // layout: ring[n_slots] | x[nb][K] bf16 (+ norm weights [K]) | pbuf[2][CWARPS][16][4] | result[r_cap][4] fp32
@@ -546,7 +541,7 @@ __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
       if (mode == GEMV_RES) epi_residual(e, b, vrow, v0);
       else if (mode == GEMV_LOGITS) epi_logit(e, b, vrow, v0);
       else if (mode == GEMV_SWIGLU) epi_swiglu(e, b, vrow, NB, v0, v1);
-      else epi_qkv_rope<PAD>(e, b, vrow, decode_pos<SLOT>(e, b), v0, v1);
+      else epi_qkv_rope(e, b, vrow, decode_col(e, b), __ldg(e.n_pad + b), v0, v1);
     }
   }
   if (mode == GEMV_LOGITS && a.amax_out != nullptr) {
@@ -581,9 +576,9 @@ __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
 
 // ---------------------------------------------------------------------------------------------
 // 5..16 clips. NG = upper bound of the row groups a CTA owns (the accumulator arrays are sized and
-// unrolled by it); a.x holds the activations in the xwin layout. PAD / SLOT as for gemv_tc_kernel
+// unrolled by it); a.x holds the activations in the xwin layout
 // ---------------------------------------------------------------------------------------------
-template <int NG, bool PAD, bool SLOT>
+template <int NG>
 __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, const GemvEpilogue e) {
   extern __shared__ __align__(128) uint8_t smem[];
   // layout: ring[8] (after the main loop: partial tiles [warp][group]) | x windows [4][16][1088 B] | barriers
@@ -733,7 +728,6 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
   // in a fixed order.
   const int mode = e.mode;
   const bool pairs = (mode == GEMV_SWIGLU || mode == GEMV_QKV);
-  const int pos = decode_pos<false>(e, 0);
   auto tile_sum = [&](int lg, int el) {
     float v = tiles[(size_t)lg * TW_TILE + el];
 #pragma unroll
@@ -753,13 +747,15 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
     }
   } else {
     const int pr = tid & 7, b = (tid >> 3) & 15;         // 8 row pairs x 16 clips of TWO groups per pass
+    int col = 0, floor = 0;                              // q|k|v: clip b's column and key floor, loaded once
+    if (mode == GEMV_QKV && b < NB) { col = decode_col(e, b); floor = __ldg(e.n_pad + b); }
     for (int lg = tid >> 7; lg < ng; lg += 2) {
       const int rr = 2 * pr;
       const int vrow = (grp_begin + lg) * 16 + rr;
       if (b >= NB || vrow >= N) continue;
       const float v0 = tile_sum(lg, rr * 17 + b), v1 = tile_sum(lg, (rr + 1) * 17 + b);
       if (mode == GEMV_SWIGLU) epi_swiglu(e, b, vrow, NB, v0, v1);
-      else epi_qkv_rope<PAD>(e, b, vrow, SLOT ? decode_pos<true>(e, b) : pos, v0, v1);
+      else epi_qkv_rope(e, b, vrow, col, floor, v0, v1);
     }
   }
 }
@@ -844,18 +840,9 @@ int launch_tc(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
   }
   cudaLaunchAttribute attr[1];
   cudaLaunchConfig_t cfg = pdl_config(grid, smem, stream, attr);
-  auto kern = e.n_pad != nullptr ? gemv_tc_kernel<true, false>
-                                 : (e.pos_per_clip ? gemv_tc_kernel<false, true> : gemv_tc_kernel<false, false>);
-  VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p));
+  VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tc_kernel, p));
   count_launches(1);
   return 0;
-}
-
-// the gemv_tcw instance of NG row groups for the epilogue's position mode
-template <int NG>
-auto tcw_kernel(const GemvEpilogue& e) {
-  return e.n_pad != nullptr ? gemv_tcw_kernel<NG, true, false>
-                            : (e.pos_per_clip ? gemv_tcw_kernel<NG, false, true> : gemv_tcw_kernel<NG, false, false>);
 }
 
 // RES / LOGITS over more than 14 row groups per SM (the lm_head): consecutive launches over near-equal
@@ -882,10 +869,10 @@ int launch_tcw(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
     cudaLaunchAttribute attr[1];
     cudaLaunchConfig_t cfg = pdl_config(grid, TW_SMEM, stream, attr);
     const int ng_max = (g1 - g0 + grid - 1) / grid;                  // groups of the busiest CTA
-    auto kern = tcw_kernel<TW_NG_MAX>(e);
-    if (ng_max <= 2) kern = tcw_kernel<2>(e);
-    else if (ng_max <= 6) kern = tcw_kernel<6>(e);
-    else if (ng_max <= 10) kern = tcw_kernel<10>(e);
+    auto kern = gemv_tcw_kernel<TW_NG_MAX>;
+    if (ng_max <= 2) kern = gemv_tcw_kernel<2>;
+    else if (ng_max <= 6) kern = gemv_tcw_kernel<6>;
+    else if (ng_max <= 10) kern = gemv_tcw_kernel<10>;
     VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, sa, se));
     count_launches(1);
   }
@@ -909,14 +896,8 @@ extern "C" int vcl_debug_tc_trace_dump(const char* path) {
 }
 
 int init_gemv_kernels() {
-  for (auto k : {gemv_tc_kernel<false, false>, gemv_tc_kernel<true, false>, gemv_tc_kernel<false, true>})
-    VCL_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-  for (auto k : {gemv_tcw_kernel<2, false, false>, gemv_tcw_kernel<6, false, false>, gemv_tcw_kernel<10, false, false>,
-                 gemv_tcw_kernel<TW_NG_MAX, false, false>, gemv_tcw_kernel<2, true, false>,
-                 gemv_tcw_kernel<6, true, false>, gemv_tcw_kernel<10, true, false>,
-                 gemv_tcw_kernel<TW_NG_MAX, true, false>, gemv_tcw_kernel<2, false, true>,
-                 gemv_tcw_kernel<6, false, true>, gemv_tcw_kernel<10, false, true>,
-                 gemv_tcw_kernel<TW_NG_MAX, false, true>})
+  VCL_CUDA_OK(cudaFuncSetAttribute(gemv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+  for (auto k : {gemv_tcw_kernel<2>, gemv_tcw_kernel<6>, gemv_tcw_kernel<10>, gemv_tcw_kernel<TW_NG_MAX>})
     VCL_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
   return 0;
 }
@@ -953,9 +934,8 @@ int launch_gemv(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
               "row groups of 16 per SM)", a.B, a.N, a.K);
   VCL_REQUIRE(e.mode != GEMV_SWIGLU || a.N % 2 == 0, "gemv swiglu: N must be even (interleaved gate/up rows)");
   VCL_REQUIRE(e.mode != GEMV_QKV || a.N == 3 * e.H * 128, "gemv qkv: N=%d != 3*H*128", a.N);
-  VCL_REQUIRE(e.n_pad == nullptr || e.mode == GEMV_QKV, "gemv: left padding applies to the q|k|v epilogue only");
-  VCL_REQUIRE(!e.pos_per_clip || (e.mode == GEMV_QKV && e.pos_dev != nullptr && e.n_pad == nullptr),
-              "gemv: per-slot positions apply to the unpadded q|k|v epilogue and need pos_dev");
+  VCL_REQUIRE((e.n_pad != nullptr) == (e.mode == GEMV_QKV),
+              "gemv: the q|k|v epilogue needs the key floors n_pad, and no other epilogue takes them");
   VCL_REQUIRE(a.embed == nullptr || (a.vocab > 0 && (a.tok_in != nullptr || (a.amax_in != nullptr && a.amax_n > 0))),
               "gemv: the fused embedding gather needs a token source");
   return a.B <= 4 ? launch_tc(a, e, stream) : launch_tcw(a, e, stream);

@@ -312,7 +312,7 @@ rope_kv_prefill_kernel(bf16* qkv, bf16* __restrict__ kcache, bf16* __restrict__ 
   const int b = (int)(tok / S), s = (int)(tok % S);
   const int D = H * 128;
   bf16* row = qkv + tok * 3LL * D;
-  const int pos = pos0 + s + (pos_dev != nullptr ? __ldg(pos_dev) : 0);
+  const int pos = pos0 + s + (pos_dev != nullptr ? __ldg(pos_dev + b) : 0);
   const long long cache_off = (((long long)b * H + head) * s_max + pos) * 128;
   // RoPE position of this cache column: left padding shifts it (pad columns clamp at 0)
   const int rpos = n_pad != nullptr ? max(pos - __ldg(n_pad + b), 0) : pos;
@@ -482,7 +482,9 @@ int launch_rope_kv_prefill(bf16* qkv, bf16* kcache, bf16* vcache, const bf16* co
   return 0;
 }
 
-__global__ void set_int_kernel(int* dst, int value) { *dst = value; }
+__global__ void fill_int_kernel(int* dst, int value, int n) {
+  for (int i = threadIdx.x; i < n; i += blockDim.x) dst[i] = value;
+}
 
 // Decode-path RMSNorm for 5..16 clips: one CTA per clip, output in the window-major layout the wide GEMV
 // streams (kernels.h: xwin). w == null: plain re-layout.
@@ -532,8 +534,8 @@ int launch_xwin_norm(const bf16* x, long long ldx, bf16* y, const bf16* w, int B
   return 0;
 }
 
-int launch_set_int(int* dst, int value, cudaStream_t stream) {
-  set_int_kernel<<<1, 1, 0, stream>>>(dst, value);
+int launch_fill_int(int* dst, int value, int n, cudaStream_t stream) {
+  fill_int_kernel<<<1, 128, 0, stream>>>(dst, value, n);
   VCL_CUDA_OK(cudaGetLastError());
   count_launches(1);
   return 0;

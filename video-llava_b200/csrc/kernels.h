@@ -22,10 +22,14 @@ struct RopeEpilogue {
   const int* n_pad = nullptr;                                  // [clip] left padding (see below) or null
 };
 
-// Left padding (a batch of prompts of different lengths): clip b's first n_pad[b] cache columns hold pad
-// tokens. Cache column c holds RoPE position max(c - n_pad[b], 0); a query at column c >= n_pad[b] attends keys
-// n_pad[b] .. c, a pad query attends causally from key 0 (its output is unused but finite). Every `n_pad`
-// argument below is a device array [clip]; null means no padding and leaves the kernels' arithmetic unchanged.
+// Positions in the KV cache. Left padding (a batch of prompts of different lengths): clip b's first n_pad[b]
+// cache columns hold pad tokens, column c holds RoPE position max(c - n_pad[b], 0), a query at column
+// c >= n_pad[b] attends keys n_pad[b] .. c, and a pad query attends causally from key 0 (its output is unused but
+// finite). Every `n_pad` below is a device array [clip]; the prefill kernels take null for no padding, the decode
+// kernels always take one (all zeros for an unpadded cache). A decode token of clip b goes to column
+// c_b = pos + (pos_dev ? pos_dev[b] : 0) (pos a host int, pos_dev a device array [clip]): it is rotated by the
+// angle of max(c_b - n_pad[b], 0), appended at column c_b and attends keys n_pad[b] .. c_b. Both arrays are read
+// on the device, so one captured decode graph serves every prompt length, padding and set of per-clip positions.
 
 void set_last_error(const char* fmt, ...);
 void count_launches(long long n);
@@ -73,9 +77,8 @@ int launch_embed_splice(const long long* ids, const bf16* table, const bf16* vid
 // cos/sin tables [max_pos, head_dim/2] rounded to bf16 (stored as bf16)
 int launch_rope_table(bf16* cos_t, bf16* sin_t, int max_pos, int head_dim, float theta,
                       cudaStream_t stream);
-// prefill: rotate q (in place inside qkv) and k, write k/v into the cache at [pos0, pos0+S)
-// (pos_dev != null: the position is pos0 + *pos_dev, read on the device -- a captured decode graph then
-// serves every prompt length; the same convention holds for every `pos_dev` below)
+// prefill: rotate q (in place inside qkv) and k, write k/v into the cache at [pos0, pos0+S) (decode beyond 16
+// clips: S = 1 at the decode positions above)
 int launch_rope_kv_prefill(bf16* qkv, bf16* kcache, bf16* vcache, const bf16* cos_t,
                            const bf16* sin_t, int B, int S, int H, int head_dim, int s_max, int pos0,
                            cudaStream_t stream, const int* pos_dev = nullptr, const int* n_pad = nullptr);
@@ -84,7 +87,7 @@ int launch_embed_tokens(const int* tok, long long tok_stride, const bf16* table,
                         int D, int vocab, cudaStream_t stream);
 int launch_argmax(const float* logits, int* out, long long out_stride, int B, int V,
                   cudaStream_t stream);
-int launch_set_int(int* dst, int value, cudaStream_t stream);
+int launch_fill_int(int* dst, int value, int n, cudaStream_t stream);   // dst[0 .. n) = value
 
 // ---- st_pool.cu ---------------------------------------------------------------------------------
 // dtype codes: 0 = fp16, 1 = bf16
@@ -133,13 +136,12 @@ int launch_attention_vit(const bf16* qkv, bf16* out, int n_frames, int S, int H,
 bool attention_vit_tc_supported(int S);
 int launch_attention_vit_tc(const bf16* qkv, bf16* out, int n_frames, int S, int H, int C, cudaStream_t stream);
 int init_attention_tc_kernels();
-// single-query attention against the cache: q [B, H*hd] -> o [B, H*hd]; kv_len keys per clip
+// single-query attention against the cache at the decode positions above (kv_len = pos + 1):
+// q [B, H*hd] -> o [B, H*hd], written in xwin layout with o_xwin
 int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, const bf16* vcache,
                             bf16* o, long long o_ld, int B, int H, int head_dim, int s_max,
-                            int kv_len, float scale, cudaStream_t stream, const int* pos_dev = nullptr,
-                            bool o_xwin = false,    // o_xwin: the output [B][H*hd] is written in xwin layout
-                            const int* n_pad = nullptr,    // keys n_pad[b] .. kv_len-1 only
-                            bool pos_per_clip = false);    // kv_len + pos_dev[b] keys per clip (unpadded)
+                            int kv_len, float scale, cudaStream_t stream, const int* pos_dev, bool o_xwin,
+                            const int* n_pad);
 
 // ---- decode_gemv.cu : decode-time weight streaming (1..16 new tokens) -------------------------------
 // Two ring kernels (bulk-copy ring over a slot-ordered copy of the matrix + mma.sync) behind one launcher:
@@ -183,9 +185,8 @@ struct GemvEpilogue {
   bf16* kcache = nullptr; bf16* vcache = nullptr;
   const bf16* cos_t = nullptr; const bf16* sin_t = nullptr;
   int H = 0, s_max = 0, pos = 0;
-  const int* pos_dev = nullptr;                 // position = pos + *pos_dev ...
-  bool pos_per_clip = false;                    // ... or, QKV unpadded, clip b at pos + pos_dev[b] (cache slots)
-  const int* n_pad = nullptr;                   // QKV: [B] left padding, RoPE angle at position - n_pad[b]
+  const int* pos_dev = nullptr;                 // QKV: the decode positions above (pos_dev may be null) ...
+  const int* n_pad = nullptr;                   // ... and the key floors [B] (required)
   float* logits = nullptr; long long ldl = 0;   // LOGITS
 };
 

@@ -49,9 +49,7 @@ struct LlmLayerW {
   bf16 *wqkv_t = nullptr, *wo_t = nullptr, *wgu_t = nullptr, *wd_t = nullptr;   // slot-ordered copies for decode
 };
 struct GraphEntry {
-  int B, S, n_new;     // S = -1: the prompt length is read on the device (h->d_pos), any S replays it
-  bool padded;         // captured with the left-padding array (h->d_npad): replays only for a padded cache
-  bool slots;          // captured with per-slot positions (h->d_slot_pos): replays only for vcl_llm_slot_decode
+  int B, n_new;        // the positions and pad counts are read on the device (h->d_pos, h->d_npad)
   cudaGraphExec_t exec;
   long long kernels;   // kernel nodes in the graph (for vcl_launch_count)
   unsigned long long last_use;
@@ -66,8 +64,7 @@ struct StepIo {
   bool partials_out = false;      // leave this step's arg-max as per-CTA partials for the next step (no arg-max kernel)
   float* logits_out = nullptr;
   int32_t* tok_out = nullptr; long long out_stride = 1;
-  const int* pos_dev = nullptr;   // position = pos + *pos_dev ...
-  bool pos_per_clip = false;      // ... or clip b at pos + pos_dev[b] (cache slots, 1..16 clips, unpadded)
+  const int* pos_dev = nullptr;   // clip b at position pos + pos_dev[b] (null: pos)
 };
 
 }  // namespace
@@ -100,16 +97,16 @@ struct vcl_handle {
        *d_act = nullptr;
   std::vector<GraphEntry> graphs;
   unsigned long long graph_clock = 0;
-  int* d_pos = nullptr;                        // prompt length of the running decode loop (device scalar)
-  // Left padding of the cache (vcl_llm_prefill_padded): the first d_npad[b] cache columns of clip b hold pad
-  // tokens. Set by a padded prefill, cleared by an unpadded one; appends and decode steps continue it. The
-  // array lives at a fixed address, so a captured decode graph serves every set of pad counts.
+  // The decode positions of kernels.h: a decode loop feeds clip b at d_pos[b] + step, with key floor d_npad[b].
+  // Both arrays live at fixed addresses, so one captured decode graph per (B, n_new) serves every prompt
+  // length, padding and set of slot positions. d_pos is written by each decode loop before it runs (the shared
+  // prompt length, or one position per cache slot). d_npad holds the left padding of the cache
+  // (vcl_llm_prefill_padded): the first d_npad[b] cache columns of clip b hold pad tokens. It is set by a padded
+  // prefill, continued by appends and decode steps, and all zeros whenever the cache is not padded.
+  int* d_pos = nullptr;                        // [max_batch]
   int* d_npad = nullptr;                       // [max_batch]
-  bool padded = false;
-  int npad_max = 0;                            // largest pad count of the padded batch (host copy)
-  // Cache slots (vcl_llm_slot_prefill / vcl_llm_slot_decode): clip b of the cache is a slot of its own, fed at
-  // position d_slot_pos[b]. Fixed address, so a captured slot graph serves every set of positions.
-  int* d_slot_pos = nullptr;                   // [max_batch]
+  bool padded = false;                         // host copies for the checks: d_npad is not all zeros ...
+  int npad_max = 0;                            // ... and its largest entry
   ArgmaxPart* amax = nullptr;                  // [gemv_grid(vocab)][max_batch] per-CTA partial arg-max of the logits kernel
 
   size_t cache_layer_elems() const {
@@ -266,13 +263,13 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   rc |= dalloc(h, &h->d_qkv, Bm * 3 * D);
   rc |= dalloc(h, &h->d_attn, xwin_elems((int)Bm, (int)D) > Bm * D ? xwin_elems((int)Bm, (int)D) : Bm * D);
   rc |= dalloc(h, &h->d_act, xwin_elems((int)Bm, (int)LF) > Bm * LF ? xwin_elems((int)Bm, (int)LF) : Bm * LF);
-  rc |= dalloc(h, &h->d_pos, 4);
+  rc |= dalloc(h, &h->d_pos, Bm);
   rc |= dalloc(h, &h->d_npad, Bm);
-  rc |= dalloc(h, &h->d_slot_pos, Bm);
   rc |= dalloc(h, &h->amax, (size_t)device_num_sms() * Bm);
   if (rc == 0) rc = launch_rope_table(h->rope_cos, h->rope_sin, c->max_seq, 128, c->rope_theta, 0);
   if (rc == 0) {
-    cudaError_t e = cudaDeviceSynchronize();
+    cudaError_t e = cudaMemset(h->d_npad, 0, Bm * sizeof(int));   // the cache starts unpadded
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
     if (e != cudaSuccess) {
       set_last_error("vcl_create: %s", cudaGetErrorString(e));
       rc = -2;
@@ -540,10 +537,12 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
         npad_max = n_pad_host[b] > npad_max ? n_pad_host[b] : npad_max;
       }
     }
+    if (npad_max > 0)
+      VCL_CUDA_OK(cudaMemcpyAsync(h->d_npad, n_pad_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    else if (h->padded)
+      VCL_CUDA_OK(cudaMemsetAsync(h->d_npad, 0, (size_t)c.max_batch * sizeof(int32_t), st));
     h->padded = npad_max > 0;
     h->npad_max = npad_max;
-    if (h->padded)
-      VCL_CUDA_OK(cudaMemcpyAsync(h->d_npad, n_pad_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   } else {
     VCL_REQUIRE(start_pos > h->npad_max, "start_pos %d lies inside the left padding (%d columns)", start_pos,
                 h->npad_max);
@@ -647,16 +646,14 @@ int score_tail(vcl_handle* h, int B, int S, const int64_t* labels, bf16* logits_
   return 0;
 }
 
-// One decode step: the token of io is fed at position pos (+ *io.pos_dev, or + io.pos_dev[b] per clip).
+// One decode step: the token of io is fed to clip b at position pos (+ io.pos_dev[b]), key floor h->d_npad[b].
 int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_t st) {
   const vcl_config& c = h->cfg;
   const int D = c.llm_hidden, F = c.llm_inter, H = c.llm_heads;
   const float scale = 0.08838834764831845f;
   const int* pd = io.pos_dev;
-  const int* np = h->padded ? h->d_npad : nullptr;   // a padded cache stays padded
+  const int* np = h->d_npad;
   VCL_REQUIRE(pos >= 0 && pos < c.max_seq, "decode position %d outside the cache (max_seq %d)", pos, c.max_seq);
-  VCL_REQUIRE(!io.pos_per_clip || (pd != nullptr && np == nullptr && B <= 16),
-              "per-slot positions need 1..16 unpadded clips");
   VCL_REQUIRE(pd != nullptr || pos >= h->npad_max, "decode position %d lies inside the left padding (%d columns)",
               pos, h->npad_max);
   // 1..4 clips: the embedding lookup is part of layer 0's q|k|v kernel (and with it the arg-max of the
@@ -697,10 +694,10 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
       GemvEpilogue qkv;
       qkv.mode = GEMV_QKV; qkv.q_out = h->d_q; qkv.ldq = D; qkv.kcache = kc_layer(h, l); qkv.vcache = vc_layer(h, l);
       qkv.cos_t = h->rope_cos; qkv.sin_t = h->rope_sin; qkv.H = H; qkv.s_max = c.max_seq; qkv.pos = pos; qkv.pos_dev = pd;
-      qkv.pos_per_clip = io.pos_per_clip; qkv.n_pad = np;
+      qkv.n_pad = np;
       VCL_TRY(launch_gemv(g, qkv, st));
       VCL_TRY(launch_decode_attention(h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->d_attn, D, B, H, 128,
-                                      c.max_seq, pos + 1, scale, st, pd, /*o_xwin=*/wide, np, io.pos_per_clip));
+                                      c.max_seq, pos + 1, scale, st, pd, /*o_xwin=*/wide, np));
       GemvArgs go;
       go.x = h->d_attn; go.ldx = D; go.W_tiled = w.wo_t; go.B = B; go.N = D; go.K = D;
       VCL_TRY(launch_gemv(go, residual, st));
@@ -735,14 +732,12 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
 // Steps 1 .. n_new-1 of a greedy loop over the token scratch tk [B][n_new] (tk[:, 0] is given).
 // For 1..4 clips no arg-max / embedding kernel runs between two steps: the logits kernel leaves
 // per-CTA partials, the next step's first q|k|v kernel reduces them, records the token and gathers
-// its embedding row.
-// pos_dev: the positions on the device (per_clip: one per clip), S the shared position otherwise.
-int decode_steps(vcl_handle* h, int32_t* tk, int B, int S, int n_new, const int* pos_dev, bool per_clip,
-                 cudaStream_t st) {
+// its embedding row. Step i feeds clip b at position h->d_pos[b] + i - 1.
+int decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st) {
   const bool hand_off = B <= 4 && h->cfg.llm_layers > 0;
   for (int i = 1; i < n_new; ++i) {
     StepIo io;
-    io.pos_dev = pos_dev; io.pos_per_clip = per_clip;
+    io.pos_dev = h->d_pos;
     if (hand_off && i > 1) {
       io.tok_from_partials = true; io.tok_store = tk + (i - 1); io.store_stride = n_new;
     } else {
@@ -750,20 +745,18 @@ int decode_steps(vcl_handle* h, int32_t* tk, int B, int S, int n_new, const int*
     }
     if (hand_off && i + 1 < n_new) io.partials_out = true;
     else { io.tok_out = tk + i; io.out_stride = n_new; }
-    VCL_TRY(llm_decode_step(h, io, B, (pos_dev ? 0 : S) + i - 1, st));
+    VCL_TRY(llm_decode_step(h, io, B, i - 1, st));
   }
   return 0;
 }
 
-// decode_steps from one captured graph per (B, n_new, padded, slots). The shared prompt length S reaches the
-// kernels through h->d_pos, the pad counts through h->d_npad and, with `slots`, the per-slot positions through
-// h->d_slot_pos (written by the caller), so new positions or padding replay the same graph. Bounded LRU cache
-// (an entry holds thousands of nodes). A stream that cannot be captured runs the steps eagerly.
-int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int S, int n_new, bool slots, cudaStream_t st) {
-  const int* pos_dev = slots ? h->d_slot_pos : h->d_pos;
+// decode_steps from one captured graph per (B, n_new). The positions (h->d_pos, written by the caller) and the
+// pad counts (h->d_npad) are read on the device, so new positions or padding replay the same graph. Bounded LRU
+// cache (an entry holds thousands of nodes). A stream that cannot be captured runs the steps eagerly.
+int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st) {
   GraphEntry* ge = nullptr;
   for (auto& g : h->graphs)
-    if (g.B == B && g.n_new == n_new && g.S == -1 && g.padded == h->padded && g.slots == slots) ge = &g;
+    if (g.B == B && g.n_new == n_new) ge = &g;
   const bool can_capture = (st != nullptr) && (st != cudaStreamLegacy);
   if (ge == nullptr && can_capture) {
     if (h->graphs.size() >= MAX_DECODE_GRAPHS) {
@@ -775,7 +768,7 @@ int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int S, int n_new, bool s
     }
     const long long before = launch_count();
     VCL_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    const int rc = decode_steps(h, tk, B, S, n_new, pos_dev, slots, st);
+    const int rc = decode_steps(h, tk, B, n_new, st);
     cudaGraph_t graph = nullptr;
     cudaError_t e = cudaStreamEndCapture(st, &graph);
     const long long nodes = launch_count() - before;
@@ -795,14 +788,25 @@ int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int S, int n_new, bool s
       set_last_error("decode graph instantiate failed: %s", cudaGetErrorString(e));
       return -2;
     }
-    h->graphs.push_back({B, -1, n_new, h->padded, slots, exec, nodes, 0});
+    h->graphs.push_back({B, n_new, exec, nodes, 0});
     ge = &h->graphs.back();
   }
-  if (ge == nullptr) return decode_steps(h, tk, B, S, n_new, slots ? pos_dev : nullptr, slots, st);
+  if (ge == nullptr) return decode_steps(h, tk, B, n_new, st);
   ge->last_use = ++h->graph_clock;
-  if (!slots) VCL_TRY(launch_set_int(h->d_pos, S, st));
   VCL_CUDA_OK(cudaGraphLaunch(ge->exec, st));
   count_launches(ge->kernels);
+  return 0;
+}
+
+// The greedy loop of vcl_llm_decode_loop and vcl_llm_slot_decode, with h->d_pos written by the caller: first_tok
+// [B] is fed, n_new - 1 steps follow, and [B, n_new] tokens (first_tok included) go to out_tokens.
+int decode_loop(vcl_handle* h, const int32_t* first_tok, int B, int n_new, int32_t* out_tokens, cudaStream_t st) {
+  int32_t* tk = h->tokens;  // [B, n_new] row-major scratch
+  if (first_tok != tk)
+    VCL_CUDA_OK(cudaMemcpy2DAsync(tk, (size_t)n_new * sizeof(int32_t), first_tok, sizeof(int32_t),
+                                  sizeof(int32_t), B, cudaMemcpyDeviceToDevice, st));
+  if (n_new > 1) VCL_TRY(run_decode_steps(h, tk, B, n_new, st));
+  VCL_CUDA_OK(cudaMemcpyAsync(out_tokens, tk, (size_t)B * n_new * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
@@ -890,13 +894,8 @@ int vcl_llm_decode_loop(vcl_handle* h, const int32_t* first_tok, int B, int S, i
               h->cfg.max_seq);
   VCL_REQUIRE(S >= h->npad_max, "S = %d lies inside the left padding (%d columns)", S, h->npad_max);
   cudaStream_t st = as_stream(stream);
-  int32_t* tk = h->tokens;  // [B, n_new] row-major scratch
-  if (first_tok != tk)
-    VCL_CUDA_OK(cudaMemcpy2DAsync(tk, (size_t)n_new * sizeof(int32_t), first_tok, sizeof(int32_t),
-                                  sizeof(int32_t), B, cudaMemcpyDeviceToDevice, st));
-  if (n_new > 1) VCL_TRY(run_decode_steps(h, tk, B, S, n_new, /*slots=*/false, st));
-  VCL_CUDA_OK(cudaMemcpyAsync(out_tokens, tk, (size_t)B * n_new * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-  return 0;
+  if (n_new > 1) VCL_TRY(launch_fill_int(h->d_pos, S, B, st));
+  return decode_loop(h, first_tok, B, n_new, out_tokens, st);
 }
 
 int vcl_llm_slot_prefill(vcl_handle* h, int slot, const int64_t* ids, const void* video_feats,
@@ -924,17 +923,9 @@ int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* 
                 "vcl_llm_slot_decode: slot %d: pos %d + n_new - 1 = %d exceeds max_seq %d", b, pos_host[b],
                 pos_host[b] + n_new - 1, h->cfg.max_seq);
   cudaStream_t st = as_stream(stream);
-  int32_t* tk = h->tokens;  // [n_slots, n_new] row-major scratch
-  VCL_CUDA_OK(cudaMemcpy2DAsync(tk, (size_t)n_new * sizeof(int32_t), first_tok, sizeof(int32_t), sizeof(int32_t),
-                                n_slots, cudaMemcpyDeviceToDevice, st));
-  if (n_new > 1) {
-    VCL_CUDA_OK(cudaMemcpyAsync(h->d_slot_pos, pos_host, (size_t)n_slots * sizeof(int32_t), cudaMemcpyHostToDevice,
-                                st));
-    VCL_TRY(run_decode_steps(h, tk, n_slots, 0, n_new, /*slots=*/true, st));
-  }
-  VCL_CUDA_OK(cudaMemcpyAsync(out_tokens, tk, (size_t)n_slots * n_new * sizeof(int32_t), cudaMemcpyDeviceToDevice,
-                              st));
-  return 0;
+  if (n_new > 1)
+    VCL_CUDA_OK(cudaMemcpyAsync(h->d_pos, pos_host, (size_t)n_slots * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  return decode_loop(h, first_tok, n_slots, n_new, out_tokens, st);
 }
 
 int vcl_llm_generate(vcl_handle* h, const int64_t* ids, const void* video_feats,
