@@ -275,6 +275,19 @@ int vcl_op_attention(const void* q, const void* k, const void* v, void* o, int B
 /* ViT attention on the fused projection output: qkv [n_frames*S, 3*H*64] (q|k|v) -> out
  * [n_frames*S, H*64]; non-causal, scale 64^-1/2; wgmma kernel for 129 <= S <= 257 */
 int vcl_op_attention_vit(const void* qkv, void* out, int n_frames, int S, int H, void* stream);
+/* Copy decoder layer `layer`'s whole K and V cache, each [max_batch][llm_heads][max_seq][128] bf16, out of the
+ * handle into k / v (write = 0) or from k / v into the handle (write = 1): one cudaMemcpyAsync per tensor on
+ * `stream`. Lets a test read back exactly what the RoPE / cache writers stored, or fill the cache with a sentinel
+ * first to see which columns a call touches. */
+int vcl_kv_cache_copy(vcl_handle* h, int layer, int write, void* k, void* v, void* stream);
+/* The decode attention kernel on its own: q [B][q_ld] (head h at columns h*128 ..), k / v caches
+ * [B][H][s_max][128], clip b's query at column c_b = kv_len - 1 + (pos_dev ? pos_dev[b] : 0) attending keys
+ * n_pad[b] .. c_b (pos_dev, n_pad: device int32 [B]; pos_dev may be NULL). o [B][H*128] row-major, or with
+ * o_xwin the window-major layout of the 5..16-clip decode kernels (kernels.h: xwin_offset, a buffer of
+ * ceil(H*128 / 512) * B * 544 elements). With pos_dev, shared memory is sized for s_max keys. */
+int vcl_op_decode_attention(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int B, int H,
+                            int s_max, int kv_len, const int32_t* pos_dev, const int32_t* n_pad, float scale,
+                            int o_xwin, void* stream);
 /* out[b,n] = x[b,:].W[n,:] (+res) with optional RMSNorm of x: B <= 4 the ring kernel of the single-clip
  * decode path (fused norm), 5 <= B <= 16 the wide ring kernel (norm + window-major re-layout by a launch of
  * its own, as on the decode path) */

@@ -351,8 +351,10 @@ argmax_kernel(const float* __restrict__ logits, int* __restrict__ out, long long
   __shared__ float sv[32];
   __shared__ int si[32];
   const float* l = logits + (long long)blockIdx.x * V;
+  // start at index 0, as torch.argmax does: a row with no logit above -inf (all -inf or NaN) gives token 0, a
+  // valid row of the embedding table, instead of an index past the vocabulary
   float best = -INFINITY;
-  int bi = 0x7fffffff;
+  int bi = 0;
   constexpr int U = 8;
   for (int i0 = threadIdx.x; i0 < V; i0 += 1024 * U) {
     float x[U];

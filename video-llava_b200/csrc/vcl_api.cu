@@ -974,6 +974,22 @@ int vcl_llm_score(vcl_handle* h, const int64_t* ids, const void* video_feats, co
 
 long long vcl_launch_count(void) { return launch_count(); }
 
+int vcl_kv_cache_copy(vcl_handle* h, int layer, int write, void* k, void* v, void* stream) {
+  VCL_REQUIRE(h && k && v, "vcl_kv_cache_copy: null argument");
+  VCL_REQUIRE(layer >= 0 && layer < h->cfg.llm_layers, "vcl_kv_cache_copy: layer %d outside 0..%d", layer,
+              h->cfg.llm_layers - 1);
+  const size_t bytes = h->cache_layer_elems() * sizeof(bf16);
+  cudaStream_t st = as_stream(stream);
+  if (write) {
+    VCL_CUDA_OK(cudaMemcpyAsync(kc_layer(h, layer), k, bytes, cudaMemcpyDeviceToDevice, st));
+    VCL_CUDA_OK(cudaMemcpyAsync(vc_layer(h, layer), v, bytes, cudaMemcpyDeviceToDevice, st));
+  } else {
+    VCL_CUDA_OK(cudaMemcpyAsync(k, kc_layer(h, layer), bytes, cudaMemcpyDeviceToDevice, st));
+    VCL_CUDA_OK(cudaMemcpyAsync(v, vc_layer(h, layer), bytes, cudaMemcpyDeviceToDevice, st));
+  }
+  return 0;
+}
+
 // ---- single-operator entry points ----
 int vcl_op_gemm(const void* A, int64_t lda, const void* W, int64_t ldw, void* C, int64_t ldc,
                 const void* bias, const void* residual, int64_t ldr, int M, int N, int K, int act,
@@ -1094,6 +1110,18 @@ int vcl_op_gemv(const void* x, const void* W, void* out, const void* res, const 
     g.x = xn; g.norm_w = nullptr;
   }
   return launch_gemv(g, e, as_stream(stream));
+}
+
+int vcl_op_decode_attention(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int B, int H,
+                            int s_max, int kv_len, const int32_t* pos_dev, const int32_t* n_pad, float scale,
+                            int o_xwin, void* stream) {
+  if (check_device() != 0) return -2;
+  VCL_REQUIRE(q && k && v && o && n_pad, "vcl_op_decode_attention: q, k, v, o and n_pad are required");
+  VCL_REQUIRE(B > 0 && H > 0 && q_ld >= (int64_t)H * 128 && q_ld % 8 == 0,
+              "vcl_op_decode_attention: B=%d H=%d q_ld=%lld", B, H, (long long)q_ld);
+  return launch_decode_attention(reinterpret_cast<const bf16*>(q), q_ld, reinterpret_cast<const bf16*>(k),
+                                 reinterpret_cast<const bf16*>(v), reinterpret_cast<bf16*>(o), (long long)H * 128, B,
+                                 H, 128, s_max, kv_len, scale, as_stream(stream), pos_dev, o_xwin != 0, n_pad);
 }
 
 }  // extern "C"

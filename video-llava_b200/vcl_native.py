@@ -71,6 +71,9 @@ _SIGNATURES = {
     "vcl_llm_slot_prefill": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "vcl_llm_slot_decode": (c_int, [c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_void_p, c_void_p]),
     "vcl_launch_count": (ctypes.c_longlong, []),
+    "vcl_kv_cache_copy": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "vcl_op_decode_attention": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                        c_void_p, c_void_p, c_float, c_int, c_void_p]),
     "vcl_op_cross_entropy": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_op_gemm": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
                             c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -202,6 +205,29 @@ def op_gemv(x, w, res=None, norm_w=None, eps=0.0):
     out = torch.empty(B, N, dtype=torch.bfloat16, device=x.device)
     check(lib().vcl_op_gemv(ptr(x), ptr(w), ptr(out), ptr(res), ptr(norm_w), eps, B, N, K, cur_stream()))
     return out
+
+
+XWIN_KC, XWIN_PITCH = 512, 544     # kernels.h: the window-major activation layout of the 5..16-clip decode kernels
+
+
+def xwin_offset(b, k, B):
+    """element (b, k) of a [B][K] activation in the xwin layout (kernels.h)"""
+    return ((k // XWIN_KC) * B + b) * XWIN_PITCH + k % XWIN_KC
+
+
+def op_decode_attention(q, k, v, kv_len, n_pad, pos_dev=None, scale=128 ** -0.5, o_xwin=False):
+    """The decode attention kernel alone (vcl_op_decode_attention). q [B, q_ld] bf16 (head h at columns
+    h*128 ..; q_ld >= H*128), k / v [B, H, s_max, 128] bf16 caches, n_pad / pos_dev int32 [B] on the device
+    (pos_dev optional). Returns o [B, H*128], or with o_xwin the flat xwin buffer (see xwin_offset)."""
+    B, H, s_max, hd = k.shape
+    assert hd == 128 and q.shape[0] == B and q.stride(1) == 1 and v.shape == k.shape
+    if o_xwin:
+        o = torch.empty((H * 128 + XWIN_KC - 1) // XWIN_KC * B * XWIN_PITCH, dtype=torch.bfloat16, device=q.device)
+    else:
+        o = torch.empty(B, H * 128, dtype=torch.bfloat16, device=q.device)
+    check(lib().vcl_op_decode_attention(ptr(q), q.stride(0), ptr(k), ptr(v), ptr(o), B, H, s_max, int(kv_len),
+                                        ptr(pos_dev), ptr(n_pad), scale, int(o_xwin), cur_stream()))
+    return o
 
 
 # ---------------------------------------------------------------------------------------------
@@ -408,6 +434,24 @@ class Engine:
             check(lib().vcl_llm_generate_padded(self._h, ptr(ids.contiguous()), ptr(vf), ptr(vid_start.contiguous()),
                                                 _host_pads(n_pad, B), B, S, n_new, ptr(out), cur_stream()))
         return out
+
+    # ---- KV cache read-back (tests) ----
+    def _cache_shape(self):
+        c = self.cfg
+        return (c.max_batch, c.llm_heads, c.max_seq, 128)
+
+    def kv_cache(self, layer):
+        """(k, v) copies of decoder layer `layer`'s cache, each [max_batch, heads, max_seq, 128] bf16."""
+        k = torch.empty(self._cache_shape(), dtype=torch.bfloat16, device="cuda")
+        v = torch.empty_like(k)
+        check(lib().vcl_kv_cache_copy(self._h, int(layer), 0, ptr(k), ptr(v), cur_stream()))
+        return k, v
+
+    def set_kv_cache(self, layer, k, v):
+        """Overwrite decoder layer `layer`'s whole cache with k / v ([max_batch, heads, max_seq, 128] bf16)."""
+        shape = self._cache_shape()
+        assert tuple(k.shape) == shape and tuple(v.shape) == shape and k.dtype == v.dtype == torch.bfloat16
+        check(lib().vcl_kv_cache_copy(self._h, int(layer), 1, ptr(k), ptr(v), cur_stream()))
 
     # ---- cache slots (in-flight batching) ----
     def slot_prefill(self, slot, ids, video_feats, vid_start, tok_out=None):
