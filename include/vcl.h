@@ -214,6 +214,24 @@ int vcl_llm_generate_padded(vcl_handle* h, const int64_t* ids, const void* video
 int vcl_llm_slot_prefill(vcl_handle* h, int slot, const int64_t* ids, const void* video_feats,
                          const int32_t* vid_start, int S, int32_t* next_tok, void* stream);
 
+/* Batched admission: n prompts into n cache slots in ONE pass of the layer stack. Prompt i has seq_len_host[i]
+ * tokens and goes to slot slots_host[i] (both HOST memory, [n] int32). ids is the packed [sum S_i] int64: the
+ * prompts concatenated without padding. video_feats is [n, n_temporal+P, 1024] or NULL; vid_start [n] int32 and
+ * next_tok [n] int32 are device arrays, vid_start[i] counted from prompt i's first token (VCL_NO_VIDEO: prompt i
+ * is text only and its feature rows are ignored). Every prompt comes out exactly as vcl_llm_slot_prefill of that
+ * prompt alone leaves it: the same cache bits in its slot (columns 0 .. S_i-1) and the same first token
+ * next_tok[i]. No other cache column is read or written. Like vcl_llm_slot_prefill it clears the cache's left
+ * padding. Rejected before any device work, the handle and cache untouched: n outside 1 .. min(max_batch, 16),
+ * a slot outside 0 .. min(max_batch, 16)-1 or given twice, S_i outside 1 .. min(512, max_seq) (512: the key limit
+ * of the prefill attention kernel). So sum S_i never exceeds the activations (max_batch * max_seq rows). The call always
+ * runs the q|k|v GEMM's fused RoPE / cache-write epilogue and the wgmma prefill attention, whatever
+ * VCL_PREFILL_ROPE_SEPARATE and VCL_PREFILL_ATTN_FLASH say (those switch the other prefill entry points only).
+ * Its launches do not depend on n beyond the choice of decode kernel for the lm_head (1..4 or 5..16 rows); the
+ * row layout reaches the kernels through one host-to-device copy into a device map of the handle. */
+int vcl_llm_slots_prefill(vcl_handle* h, int n, const int32_t* slots_host, const int32_t* seq_len_host,
+                          const int64_t* ids, const void* video_feats, const int32_t* vid_start,
+                          int32_t* next_tok, void* stream);
+
 /* vcl_llm_decode_loop with a position per slot: slot b (0 <= b < n_slots) is fed first_tok[b] at position
  * pos_host[b] (HOST memory: the number of tokens its cache holds), then runs n_new-1 greedy steps;
  * out_tokens is [n_slots, n_new] int32, first_tok included. Every pos_host[b] + n_new - 1 must be <= max_seq

@@ -1,7 +1,8 @@
 """In-flight (continuous) batching against static batches and one request at a time.
 
     python tools/bench_inflight.py [--requests 64] [--min-new 16] [--max-new 384] [--slots 4,8,16]
-                                   [--chunks 16] [--repeats 2] [--out DIR]
+                                   [--chunks 16] [--repeats 2] [--no-static] [--no-alone] [--out DIR]
+    python tools/bench_inflight.py --prefill-cost [--ks 1,2,4,8,16] [--iters 10] [--out DIR]
 
 Vicuna-7B shapes with random-init bf16 weights (bench.device_weights, seed 0), random pooled video features, and
 prompts of 400..448 tokens (bench.synthetic_prompt_ids with a shorter text before the video). Random weights never
@@ -11,11 +12,16 @@ one, and every arm produces the same tokens per request. Arms, per slot count:
                 to the group's longest request; the outputs are cut to each request's length
   (b) inflight  generate_requests with the same slots (and each chunk length of --chunks, set on the class
                 constant _SLOT_CHUNK)
+  (p) packed    (b) with packed_admission=True: every admission point fills all free slots with one packed
+                prefill (vcl_llm_slots_prefill)
   (c) alone     one generate per request; run once, after the others (it is the longest and does not depend on
                 the slot count)
-After one warm-up round of (a) and (b) over the first `slots` requests, (a) and (b) alternate --repeats times.
-Each arm is timed with a host clock around its calls, ended by a stream synchronise. The admission share of (b) is
-the device time of its slot prefills (CUDA events around each one) over its wall time.
+After one warm-up round of (a), (b) and (p) over the first `slots` requests, they alternate --repeats times.
+Each arm is timed with a host clock around its calls, ended by a stream synchronise. The admission share of (b) and
+(p) is the device time of their prefills (CUDA events around each call) over the wall time.
+--prefill-cost instead times admission alone: one slots_prefill of k requests (400..448 tokens with video) against
+k slot_prefill calls of the same requests, for each k of --ks, the two arms alternated, CUDA events around each
+arm, median and spread over --iters rounds after one warm-up.
 Prints one JSON line: per arm requests/s, generated tokens/s, median and p90 request latency (from the start of
 the arm to the synchronise after the call that completed the request: for (a) its group, for (b) the whole run,
 since generate_requests returns once), the card name and power limit, and whether every request's tokens agree
@@ -96,9 +102,9 @@ def static(model, reqs, slots):
     return toks, done
 
 
-def inflight(model, reqs, slots):
+def inflight(model, reqs, slots, packed=False):
     t0 = time.perf_counter()
-    outs = model.generate_requests(reqs, eos_token_id=None, slots=slots)
+    outs = model.generate_requests(reqs, eos_token_id=None, slots=slots, packed_admission=packed)
     torch.cuda.current_stream().synchronize()
     t = time.perf_counter() - t0
     return [o[0, r["input_ids"].numel():].tolist() for o, r in zip(outs, reqs)], [t] * len(reqs)
@@ -136,6 +142,44 @@ def agree_to_tie(model, eng, r, a, b):
     return bool(((top[0] - top[1]) / ulp) < 3)
 
 
+def prefill_cost(model, eng, reqs, ks, iters):
+    """-> {k: {"packed_ms": median, "single_ms": median, "..._range": [min, max]}} over iters alternated rounds"""
+    res = {}
+    for k in ks:
+        grp = reqs[:k]
+        ids = [r["input_ids"].cuda() for r in grp]
+        feats = [r["video_spatio_temporal_features"] for r in grp]
+        vstarts = [int(model._video_spans(r["input_ids"][None], eng.NV)[0]) for r in grp]
+        tok = torch.empty(k, dtype=torch.int32, device="cuda")
+
+        def single():
+            for s in range(k):
+                vs = torch.tensor([vstarts[s]], dtype=torch.int32, device="cuda")
+                eng.slot_prefill(s, ids[s][None], feats[s], vs, tok_out=tok[s:s + 1])
+
+        def packed():
+            eng.slots_prefill(list(range(k)), ids, feats, vstarts, tok_out=tok)
+
+        times = {"single": [], "packed": []}
+        for it in range(iters + 1):
+            for name, fn in (("single", single), ("packed", packed)) if it % 2 == 0 else (("packed", packed),
+                                                                                           ("single", single)):
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                fn()
+                e1.record()
+                e1.synchronize()
+                if it > 0:
+                    times[name].append(e0.elapsed_time(e1))
+        res[k] = {}
+        for name, t in times.items():
+            res[k][f"{name}_ms"] = round(statistics.median(t), 2)
+            res[k][f"{name}_range_ms"] = [round(min(t), 2), round(max(t), 2)]
+        res[k]["speedup"] = round(res[k]["single_ms"] / res[k]["packed_ms"], 3)
+        log(f"prefill k={k}: {res[k]}")
+    return res
+
+
 def log(*a):
     print(*a, file=sys.stderr, flush=True)
 
@@ -149,6 +193,10 @@ def main():
     ap.add_argument("--chunks", default=None, help="chunk lengths of the in-flight arm (default: the class constant)")
     ap.add_argument("--repeats", type=int, default=2)
     ap.add_argument("--no-alone", action="store_true", help="skip arm (c)")
+    ap.add_argument("--no-static", action="store_true", help="skip arm (a)")
+    ap.add_argument("--prefill-cost", action="store_true", help="time admission alone (see above)")
+    ap.add_argument("--ks", default="1,2,4,8,16")
+    ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--out", default=None, help="also write the JSON line to DIR/bench_inflight.json")
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -157,6 +205,24 @@ def main():
     slot_counts = [int(s) for s in a.slots.split(",")]
     default_chunk = VideoChatGPTLlamaForCausalLM._SLOT_CHUNK
     chunks = [int(c) for c in a.chunks.split(",")] if a.chunks else [default_chunk]
+    if a.prefill_cost:
+        ks = [int(k) for k in a.ks.split(",")]
+        model, eng = make_model(max(ks), S_MAX + a.max_new)
+        reqs = make_requests(max(ks), a.min_new, a.max_new)
+        st = torch.cuda.Stream()
+        with torch.cuda.stream(st):
+            res = {"what": "one slots_prefill of k requests against k slot_prefill calls, prompts 400..448 tokens "
+                           "with video, Vicuna-7B shapes, CUDA events, median of alternated rounds",
+                   "card": name, "power_limit": power, "iters": a.iters,
+                   "prefill": prefill_cost(model, eng, reqs, ks, a.iters)}
+        st.synchronize()
+        line = json.dumps(res)
+        print(line)
+        if a.out:
+            os.makedirs(a.out, exist_ok=True)
+            with open(os.path.join(a.out, "bench_prefill_cost.json"), "w") as f:
+                f.write(line + "\n")
+        return
     model, eng = make_model(max(slot_counts), S_MAX + a.max_new)
     reqs = make_requests(a.requests, a.min_new, a.max_new)
     n_tokens = sum(r["max_new_tokens"] for r in reqs)
@@ -173,6 +239,17 @@ def main():
         return out
 
     eng.slot_prefill = timed_prefill
+    slots_prefill = eng.slots_prefill
+
+    def timed_slots_prefill(*args, **kw):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        out = slots_prefill(*args, **kw)
+        e1.record()
+        prefill_ms.append((e0, e1))
+        return out
+
+    eng.slots_prefill = timed_slots_prefill
     st = torch.cuda.Stream()          # decode loops are captured into CUDA graphs on a non-default stream
     res = {"what": f"{a.requests} requests, prompts 400..{S_MAX} tokens with video, max_new_tokens uniform "
                    f"{a.min_new}..{a.max_new} ({n_tokens} tokens), Vicuna-7B shapes, random bf16 weights",
@@ -181,34 +258,39 @@ def main():
     with torch.cuda.stream(st):
         for slots in slot_counts:
             warm = reqs[:slots]
-            static(model, warm, slots)
+            if not a.no_static:
+                static(model, warm, slots)
             for c in chunks:
                 VideoChatGPTLlamaForCausalLM._SLOT_CHUNK = c
                 inflight(model, warm, slots)
+                inflight(model, warm, slots, packed=True)
             runs = {}
-            for _ in range(a.repeats):
-                t0 = time.perf_counter()
-                tok, done = static(model, reqs, slots)
-                runs.setdefault("static", []).append((time.perf_counter() - t0, done))
-                log(f"slots {slots} static {runs['static'][-1][0]:.2f} s")
-                tokens[f"static_{slots}"] = tok
+            for rep in range(a.repeats):
+                if not a.no_static:
+                    t0 = time.perf_counter()
+                    tok, done = static(model, reqs, slots)
+                    runs.setdefault("static", []).append((time.perf_counter() - t0, done))
+                    log(f"slots {slots} static {runs['static'][-1][0]:.2f} s")
+                    tokens[f"static_{slots}"] = tok
                 for c in chunks:
                     VideoChatGPTLlamaForCausalLM._SLOT_CHUNK = c
-                    prefill_ms.clear()
-                    t0 = time.perf_counter()
-                    tok, done = inflight(model, reqs, slots)
-                    wall = time.perf_counter() - t0
-                    adm = sum(e0.elapsed_time(e1) for e0, e1 in prefill_ms) / 1e3
-                    runs.setdefault(f"inflight_chunk{c}", []).append((wall, done, adm))
-                    log(f"slots {slots} inflight chunk {c} {wall:.2f} s, admissions {adm:.2f} s")
-                    tokens[f"inflight_{slots}_chunk{c}"] = tok
+                    for packed in ((False, True) if rep % 2 == 0 else (True, False)):
+                        arm = f"{'packed' if packed else 'inflight'}_chunk{c}"
+                        prefill_ms.clear()
+                        t0 = time.perf_counter()
+                        tok, done = inflight(model, reqs, slots, packed=packed)
+                        wall = time.perf_counter() - t0
+                        adm = sum(e0.elapsed_time(e1) for e0, e1 in prefill_ms) / 1e3
+                        runs.setdefault(arm, []).append((wall, done, adm, len(prefill_ms)))
+                        log(f"slots {slots} {arm} {wall:.2f} s, admissions {adm:.2f} s in {len(prefill_ms)} calls")
+                        tokens[f"{arm}_{slots}"] = tok
             for arm, rs in runs.items():
                 best = min(rs, key=lambda x: x[0])
                 s = summary(best[0], best[1], n_tokens)
                 s["wall_s_all"] = [round(x[0], 3) for x in rs]
-                if arm.startswith("inflight"):
+                if arm.startswith(("inflight", "packed")):
                     s["admission_share"] = round(best[2] / best[0], 3)
-                    s["admissions"] = a.requests
+                    s["admission_calls"] = best[3]
                 res["arms"][f"{arm}_slots{slots}"] = s
         VideoChatGPTLlamaForCausalLM._SLOT_CHUNK = default_chunk
         if not a.no_alone:
@@ -227,6 +309,12 @@ def main():
             to_tie += same or all(agree_to_tie(model, eng, r, ref[i], tokens[k][i]) for k in names)
     st.synchronize()
     res["tokens_identical_across_arms"] = f"{identical}/{len(reqs)}"
+    # packed admission against one at a time with the same slots and chunk: bit-identical by construction
+    for slots in slot_counts:
+        for c in chunks:
+            a_tok, p_tok = tokens[f"inflight_chunk{c}_{slots}"], tokens[f"packed_chunk{c}_{slots}"]
+            res[f"packed_identical_to_inflight_slots{slots}_chunk{c}"] = \
+                f"{sum(x == y for x, y in zip(a_tok, p_tok))}/{len(reqs)}"
     res["tokens_match_margin_rule"] = f"{to_tie}/{len(reqs)}"
     line = json.dumps(res)
     print(line)

@@ -277,7 +277,10 @@ int launch_attention(const AttnArgs& a, cudaStream_t stream) {
                   a.v_sb % 8 == 0 && a.o_ss % 2 == 0 && a.o_sh % 2 == 0 && a.o_sb % 2 == 0,
               "attention: strides must keep 16-byte row alignment");
   VCL_REQUIRE(a.n_pad == nullptr || (a.causal && a.head_dim == 128), "attention: left padding needs causal hd-128 attention");
+  VCL_REQUIRE(a.pack == nullptr || (a.causal && a.head_dim == 128 && a.n_pad == nullptr && a.S <= 512),
+              "attention: packed sequences need causal hd-128 attention over at most 512 keys, unpadded");
   if (a.B <= 0 || a.H <= 0 || a.S <= 0) return 0;
+  if (a.pack != nullptr) return launch_attention_prefill_tc(a, stream);   // the only kernel with packed sequences
   if (attention_prefill_tc_supported(a)) return launch_attention_prefill_tc(a, stream);   // LLaMA prefill up to 512 keys
   if (a.n_pad != nullptr) return launch_attn_t<128, true, true>(a, stream);
   if (a.head_dim == 64) {

@@ -85,8 +85,11 @@ __device__ __forceinline__ void pa_mma(float (&acc)[64], uint32_t a_base, int a_
 }
 
 // PAD: left-padded clips (a.n_pad): a real query (cache column >= n_pad[b]) attends keys n_pad[b] .. its own column,
-// and a tile of real queries starts at the first key block that holds a real key; a pad query attends causally
-template <bool PAD>
+// and a tile of real queries starts at the first key block that holds a real key; a pad query attends causally.
+// PACK: packed sequences (a.pack): blockIdx.z is sequence i, whose S_i queries start at its row offset and whose keys
+// are clip slot_i of the cache (S = S_kv = S_i, q_off = 0); the grid covers the longest sequence, so a CTA whose
+// query tile starts past S_i has nothing to do.
+template <bool PAD, bool PACK>
 __global__ void __launch_bounds__(PA_THREADS)
 attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
   extern __shared__ uint8_t smem_raw[];
@@ -98,20 +101,29 @@ attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
   const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int lane = threadIdx.x & 31, wq = threadIdx.x >> 5;
   const int q0 = qt * 64;
-  const bf16* qg = a.q + (long long)b * a.q_sb + (long long)h * a.q_sh;
-  const bf16* kg = a.k + (long long)b * a.k_sb + (long long)h * a.k_sh;
-  const bf16* vg = a.v + (long long)b * a.v_sb + (long long)h * a.v_sh;
+  int S = a.S, q_off = a.q_off;
+  long long q_base = (long long)b * a.q_sb, o_base = (long long)b * a.o_sb, kv_clip = b;
+  if constexpr (PACK) {
+    S = __ldg(pack_len(a.pack) + b);
+    if (q0 >= S) return;                                 // before the first barrier: the whole CTA leaves
+    const long long off = __ldg(pack_off(a.pack) + b);
+    S_kv = S; q_off = 0;
+    q_base = off * a.q_ss; o_base = off * a.o_ss; kv_clip = __ldg(pack_slot(a.pack) + b);
+  }
+  const bf16* qg = a.q + q_base + (long long)h * a.q_sh;
+  const bf16* kg = a.k + kv_clip * a.k_sb + (long long)h * a.k_sh;
+  const bf16* vg = a.v + kv_clip * a.v_sb + (long long)h * a.v_sh;
   // key blocks this tile touches: keys up to the absolute position of its last query
-  const int last_key = min(S_kv - 1, a.q_off + min(q0 + 63, a.S - 1));
+  const int last_key = min(S_kv - 1, q_off + min(q0 + 63, S - 1));
   const int n_kb = last_key / 128 + 1;
   const int k_pad = PAD ? __ldg(a.n_pad + b) : 0;                  // first real key of the clip
-  const int kb0 = (PAD && a.q_off + q0 >= k_pad) ? k_pad / 128 : 0;   // key blocks below hold pad keys only
+  const int kb0 = (PAD && q_off + q0 >= k_pad) ? k_pad / 128 : 0;     // key blocks below hold pad keys only
 
-  pa_load_rows<64>(smem + PA_OFF_Q, qg, a.q_ss, q0, a.S);
+  pa_load_rows<64>(smem + PA_OFF_Q, qg, a.q_ss, q0, S);
 
   const int r0 = 16 * wq + (lane >> 2), c2 = 2 * (lane & 3);
   int qpos[2];                                           // absolute positions of this thread's two rows
-  qpos[0] = a.q_off + q0 + r0;
+  qpos[0] = q_off + q0 + r0;
   qpos[1] = qpos[0] + 8;
   int kmin[2] = {0, 0};                                  // key floor of the two rows
   if constexpr (PAD) {
@@ -180,11 +192,11 @@ attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
     l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
     l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
   }
-  bf16* og = a.o + (long long)b * a.o_sb + (long long)h * a.o_sh;
+  bf16* og = a.o + o_base + (long long)h * a.o_sh;
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     const int qrow = q0 + r0 + 8 * hh;
-    if (qrow < a.S) {
+    if (qrow < S) {
       const float inv = 1.0f / l[hh];
       bf16* dst = og + (long long)qrow * a.o_ss + c2;
 #pragma unroll
@@ -197,8 +209,9 @@ attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
 }  // namespace
 
 int init_attention_prefill_tc_kernels() {
-  VCL_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PA_SMEM));
-  VCL_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, PA_SMEM));
+  VCL_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PA_SMEM));
+  VCL_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PA_SMEM));
+  VCL_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, PA_SMEM));
   return 0;
 }
 
@@ -218,8 +231,9 @@ bool attention_prefill_tc_supported(const AttnArgs& a) {
 int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t stream) {
   const int S_kv = a.S_kv > 0 ? a.S_kv : a.S;
   dim3 grid((a.S + 63) / 64, a.H, a.B);
-  if (a.n_pad != nullptr) attn_prefill_tc_kernel<true><<<grid, PA_THREADS, PA_SMEM, stream>>>(a, S_kv);
-  else attn_prefill_tc_kernel<false><<<grid, PA_THREADS, PA_SMEM, stream>>>(a, S_kv);
+  if (a.pack != nullptr) attn_prefill_tc_kernel<false, true><<<grid, PA_THREADS, PA_SMEM, stream>>>(a, S_kv);
+  else if (a.n_pad != nullptr) attn_prefill_tc_kernel<true, false><<<grid, PA_THREADS, PA_SMEM, stream>>>(a, S_kv);
+  else attn_prefill_tc_kernel<false, false><<<grid, PA_THREADS, PA_SMEM, stream>>>(a, S_kv);
   VCL_CUDA_OK(cudaGetLastError());
   count_launches(1);
   return 0;

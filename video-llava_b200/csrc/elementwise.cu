@@ -254,9 +254,14 @@ im2col_kernel(const void* __restrict__ pixels, int mode, bf16* __restrict__ out,
 __global__ void __launch_bounds__(128)
 embed_splice_kernel(const long long* __restrict__ ids, const bf16* __restrict__ table,
                     const bf16* __restrict__ vid, const int* __restrict__ vid_start,
-                    bf16* __restrict__ h, int S, int D, int n_vid, int vocab) {
+                    bf16* __restrict__ h, int S, int D, int n_vid, int vocab, const int* __restrict__ pack) {
   const long long row = blockIdx.x;
-  const int b = (int)(row / S), s = (int)(row % S);
+  int b, s;
+  if (pack != nullptr) {
+    b = __ldg(pack_row(pack, row)); s = __ldg(pack_row(pack, row) + 1);
+  } else {
+    b = (int)(row / S); s = (int)(row % S);
+  }
   // vid_start[b] = index of the row AFTER which the video rows go (-1: the video rows start at row 0);
   // anything below -1 (VCL_NO_VIDEO), or a null array, marks a text-only row
   const int vs = vid_start != nullptr ? vid_start[b] : -2;
@@ -442,10 +447,11 @@ int launch_clip_embed_ln(const bf16* patch_out, const bf16* cls, const bf16* pos
 
 int launch_embed_splice(const long long* ids, const bf16* table, const bf16* vid,
                         const int* vid_start, bf16* h, int B, int S, int D, int n_vid, int vocab,
-                        cudaStream_t stream) {
+                        cudaStream_t stream, const int* pack, int M) {
   VCL_REQUIRE(D % 8 == 0, "embed_splice: D must be x8");
-  if (B * S <= 0) return 0;
-  embed_splice_kernel<<<B * S, 128, 0, stream>>>(ids, table, vid, vid_start, h, S, D, n_vid, vocab);
+  const int rows = pack != nullptr ? M : B * S;
+  if (rows <= 0) return 0;
+  embed_splice_kernel<<<rows, 128, 0, stream>>>(ids, table, vid, vid_start, h, S, D, n_vid, vocab, pack);
   VCL_CUDA_OK(cudaGetLastError());
   count_launches(1);
   return 0;

@@ -66,6 +66,7 @@ __device__ __forceinline__ float act_gelu_erf(float x) {
 //               rope_kv_prefill_kernel (elementwise.cu): x rounded to bf16, every product rounded, fp32 sum, one
 //               final rounding (transformers/models/llama/modeling_llama.py:124-168). With left padding
 //               (rp.n_pad) the angle is that of cache column - n_pad[clip], clamped at 0; the columns do not move.
+//               Packed rows (rp.pack): the angle is the row's position in its sequence.
 template <int BLOCK_N, int ACT>
 __device__ __forceinline__ void gemm_epilogue_stage(const float (&acc)[BLOCK_N / 2], uint8_t* stg, int lane, int wq,
                                                     int row_base, int n_blk, const bf16* __restrict__ bias, int M,
@@ -83,8 +84,13 @@ __device__ __forceinline__ void gemm_epilogue_stage(const float (&acc)[BLOCK_N /
       for (int h = 0; h < 2; ++h) {
         const int r = r0 + 8 * h;
         const int grow = row_base + r;
-        int pos = rp.start_pos + (grow < M ? grow % rp.S : 0);
-        if (rp.n_pad != nullptr && grow < M) pos = max(pos - __ldg(rp.n_pad + grow / rp.S), 0);   // left padding
+        int pos;
+        if (rp.pack != nullptr) {
+          pos = grow < M ? __ldg(pack_row(rp.pack, grow) + 1) : 0;                                  // packed rows
+        } else {
+          pos = rp.start_pos + (grow < M ? grow % rp.S : 0);
+          if (rp.n_pad != nullptr && grow < M) pos = max(pos - __ldg(rp.n_pad + grow / rp.S), 0);   // left padding
+        }
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
           const int j = hh * 16 + jj, d = 8 * jj + c2;
@@ -175,7 +181,9 @@ __device__ __forceinline__ void gemm_epilogue_store(const uint8_t* stg, int t, i
         if (r < rows) rr[u] = *reinterpret_cast<const uint4*>(residual + (long long)(row_base + r) * ldr + col);
       }
     }
-#pragma unroll
+    // ACT_ROPE: not unrolled, the cache address of a row (a map lookup for packed rows) fits the store warps'
+    // registers one row at a time
+#pragma unroll (ACT == ACT_ROPE ? 1 : RES_INFLIGHT)
     for (int u = 0; u < RES_INFLIGHT; ++u) {
       const int r = r0 + u * RSTEP;
       if (r >= rows) break;
@@ -186,8 +194,14 @@ __device__ __forceinline__ void gemm_epilogue_store(const uint8_t* stg, int t, i
         const int gh = col >> 7, d = col & 127;
         const int which = gh / rp.H, head = gh - which * rp.H;
         if (which != 0) {
-          const int gb = grow / rp.S, gs = grow - gb * rp.S;
-          dst = (which == 1 ? rp.kcache : rp.vcache) + (((long long)gb * rp.H + head) * rp.s_max + rp.start_pos + gs) * 128 + d;
+          int gb, col_c;   // cache clip and column of the row
+          if (rp.pack != nullptr) {
+            const int2 sp = __ldg(reinterpret_cast<const int2*>(pack_row(rp.pack, grow)));
+            gb = __ldg(pack_slot(rp.pack) + sp.x); col_c = sp.y;
+          } else {
+            gb = grow / rp.S; col_c = rp.start_pos + grow - gb * rp.S;
+          }
+          dst = (which == 1 ? rp.kcache : rp.vcache) + (((long long)gb * rp.H + head) * rp.s_max + col_c) * 128 + d;
         }
       } else if (RES && residual != nullptr) {
         val.x = bf16x2_add(val.x, rr[u].x); val.y = bf16x2_add(val.y, rr[u].y);
@@ -510,7 +524,8 @@ int launch_gemm_bf16_tn(const GemmArgs& g, cudaStream_t stream) {
   if (g.act == ACT_ROPE) {
     const RopeEpilogue& r = g.rope;
     VCL_REQUIRE(r.cos_t && r.sin_t && r.kcache && r.vcache && r.S > 0 && r.H > 0, "gemm: ACT_ROPE needs the RoPE tables and the cache");
-    VCL_REQUIRE(g.N == 3 * r.H * 128 && g.M % r.S == 0 && r.start_pos + r.S <= r.s_max && g.bias == nullptr && g.residual == nullptr,
+    VCL_REQUIRE(g.N == 3 * r.H * 128 && (r.pack != nullptr || g.M % r.S == 0) && r.start_pos + r.S <= r.s_max &&
+                    g.bias == nullptr && g.residual == nullptr,
                 "gemm: ACT_ROPE shape (N=%d, H=%d, M=%d, S=%d, start %d, cache %d)", g.N, r.H, g.M, r.S, r.start_pos, r.s_max);
     VCL_REQUIRE(((uintptr_t)r.kcache % 16) == 0 && ((uintptr_t)r.vcache % 16) == 0 && ((uintptr_t)r.cos_t % 16) == 0 &&
                     ((uintptr_t)r.sin_t % 16) == 0, "gemm: ACT_ROPE pointers must be 16-byte aligned");

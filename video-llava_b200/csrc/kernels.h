@@ -11,15 +11,33 @@ namespace vcl {
 
 typedef __nv_bfloat16 bf16;
 
+// Packed prefill (vcl_llm_slots_prefill): n <= PACK_SEQ_MAX sequences of lengths S_0 .. S_{n-1} concatenated
+// without padding into M = sum S_i rows, sequence i going to cache slot slot_i. One device int array describes the
+// layout, and every kernel of a packed prefill reads it through the accessors below:
+//   [0, 16)   row offset of sequence i      [16, 32)  its length S_i
+//   [32, 48)  its cache slot                [48, 64)  its last row (offset + S_i - 1), whose logits give its token
+//   [64 + 2r] sequence of row r             [64 + 2r + 1] position of row r inside its sequence
+constexpr int PACK_SEQ_MAX = 16;
+constexpr int PACK_HEAD = 4 * PACK_SEQ_MAX;
+inline size_t pack_elems(long long rows) { return PACK_HEAD + 2 * (size_t)rows; }
+template <class T> __host__ __device__ inline T* pack_off(T* p) { return p; }
+template <class T> __host__ __device__ inline T* pack_len(T* p) { return p + PACK_SEQ_MAX; }
+template <class T> __host__ __device__ inline T* pack_slot(T* p) { return p + 2 * PACK_SEQ_MAX; }
+template <class T> __host__ __device__ inline T* pack_last(T* p) { return p + 3 * PACK_SEQ_MAX; }
+template <class T> __host__ __device__ inline T* pack_row(T* p, long long r) { return p + PACK_HEAD + 2 * r; }   // [seq, pos]
+
 enum Act { ACT_NONE = 0, ACT_QGELU = 1, ACT_GELU = 2, ACT_SWIGLU = 3, ACT_ROPE = 4 };
-// ACT_ROPE: the GEMM is the LLaMA q|k|v projection of a prefill (N = 3 * H * 128, rows = [clip][position]).
-// The epilogue rotates q and k (RoPE, every product and the sum rounded to bf16 like the reference), writes q to
-// C (columns [0, H * 128)), k and v straight into the KV cache; the k | v columns of C are not written.
+// ACT_ROPE: the GEMM is the LLaMA q|k|v projection of a prefill (N = 3 * H * 128, rows = [clip][position], or the
+// packed rows of `pack`). The epilogue rotates q and k (RoPE, every product and the sum rounded to bf16 like the
+// reference), writes q to C (columns [0, H * 128)), k and v straight into the KV cache; the k | v columns of C are
+// not written.
 struct RopeEpilogue {
   const bf16* cos_t = nullptr; const bf16* sin_t = nullptr;    // [s_max][64]
   bf16* kcache = nullptr; bf16* vcache = nullptr;              // [clip][head][s_max][128] of this layer
   int S = 0, start_pos = 0, H = 0, s_max = 0;                  // rows per clip, position of row 0, heads
   const int* n_pad = nullptr;                                  // [clip] left padding (see below) or null
+  const int* pack = nullptr;   // packed rows (above) or null: row r is rotated by its position p and lands at
+                               // column p of its sequence's slot (S, start_pos and n_pad are then unused)
 };
 
 // Positions in the KV cache. Left padding (a batch of prompts of different lengths): clip b's first n_pad[b]
@@ -71,9 +89,11 @@ int launch_im2col(const void* pixels, int mode, bf16* out, int n_frames, int ima
 int launch_clip_embed_ln(const bf16* patch_out, const bf16* cls, const bf16* pos, const bf16* ln_w,
                          const bf16* ln_b, bf16* h, int n_frames, int P, int D, float eps,
                          cudaStream_t stream);
-// token-embedding gather with the projected video rows spliced in after <vid_start>
+// token-embedding gather with the projected video rows spliced in after <vid_start>. pack (packed rows, M = B * S
+// when null): row r is position p of sequence i, takes vid_start[i] and video row block i
 int launch_embed_splice(const long long* ids, const bf16* table, const bf16* vid, const int* vid_start,
-                        bf16* h, int B, int S, int D, int n_vid, int vocab, cudaStream_t stream);
+                        bf16* h, int B, int S, int D, int n_vid, int vocab, cudaStream_t stream,
+                        const int* pack = nullptr, int M = 0);
 // cos/sin tables [max_pos, head_dim/2] rounded to bf16 (stored as bf16)
 int launch_rope_table(bf16* cos_t, bf16* sin_t, int max_pos, int head_dim, float theta,
                       cudaStream_t stream);
@@ -122,6 +142,10 @@ struct AttnArgs {
   int S_kv = 0;      // number of keys (0: = S); > S when the queries continue a cached sequence
   int q_off = 0;     // absolute position of query 0 for the causal mask (S_kv - S for a continuation)
   const int* n_pad = nullptr;   // causal only: [B] left padding, the key floor of real queries (or null)
+  // packed rows (kernels.h, above) or null. Sequence i (i < B) has S = S_kv = S_i, q_off 0: its queries / outputs
+  // are rows offset_i .. of q / o (q_sb, o_sb unused), its keys / values clip slot_i of k / v. a.S is max S_i.
+  // Always the wgmma kernel (S_i <= 512), whatever VCL_PREFILL_ATTN_FLASH says.
+  const int* pack = nullptr;
 };
 int launch_attention(const AttnArgs& a, cudaStream_t stream);     // dispatches to the wgmma prefill kernel when it applies
 int init_attention_kernels();

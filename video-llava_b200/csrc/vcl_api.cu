@@ -108,6 +108,8 @@ struct vcl_handle {
   bool padded = false;                         // host copies for the checks: d_npad is not all zeros ...
   int npad_max = 0;                            // ... and its largest entry
   ArgmaxPart* amax = nullptr;                  // [gemv_grid(vocab)][max_batch] per-CTA partial arg-max of the logits kernel
+  int* d_pack = nullptr;                       // pack_elems(max_batch * max_seq): the packed-row map of kernels.h,
+                                               // written by each vcl_llm_slots_prefill with one host-to-device copy
 
   size_t cache_layer_elems() const {
     return (size_t)cfg.max_batch * cfg.llm_heads * cfg.max_seq * 128;
@@ -266,6 +268,7 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   rc |= dalloc(h, &h->d_pos, Bm);
   rc |= dalloc(h, &h->d_npad, Bm);
   rc |= dalloc(h, &h->amax, (size_t)device_num_sms() * Bm);
+  rc |= dalloc(h, &h->d_pack, pack_elems((long long)Ml));
   if (rc == 0) rc = launch_rope_table(h->rope_cos, h->rope_sin, c->max_seq, 128, c->rope_theta, 0);
   if (rc == 0) {
     cudaError_t e = cudaMemset(h->d_npad, 0, Bm * sizeof(int));   // the cache starts unpadded
@@ -512,15 +515,22 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
 // null or all zero. A continuation keeps the padding of the cache.
 // slot > 0 (B = 1): the sequence goes to clip `slot` of the cache; every layer's cache base moves by that many
 // clips, and no other clip's columns are read or written.
+// packed_rows > 0: B new sequences packed without padding into packed_rows rows, each into its own cache slot, as
+// the map in h->d_pack (kernels.h) describes them; S is the longest. Every row is computed as it would be in a
+// prefill of its sequence alone; next_tok [B] receives each sequence's first token.
 int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
                 int B, int S, int n_layers, void* hidden_out, float* logits_out, int32_t* next_tok,
                 long long tok_stride, cudaStream_t st, int start_pos = 0, void* states_out = nullptr,
-                const int32_t* n_pad_host = nullptr, int slot = 0) {
+                const int32_t* n_pad_host = nullptr, int slot = 0, int packed_rows = 0) {
   const vcl_config& c = h->cfg;
+  const bool packed = packed_rows > 0;
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
   VCL_REQUIRE(B > 0 && B <= c.max_batch, "B=%d outside 1..%d", B, c.max_batch);
   VCL_REQUIRE(slot == 0 || (B == 1 && slot > 0 && slot < c.max_batch), "slot %d needs B = 1 and a clip of the cache",
               slot);
+  VCL_REQUIRE(!packed || (start_pos == 0 && n_pad_host == nullptr && states_out == nullptr && hidden_out == nullptr &&
+                          logits_out == nullptr && slot == 0),
+              "packed sequences start unpadded and return their next tokens only");
   VCL_REQUIRE(S > 0 && start_pos >= 0 && start_pos + S <= c.max_seq, "positions %d..%d outside the cache (max_seq %d)",
               start_pos, start_pos + S - 1, c.max_seq);
   VCL_REQUIRE(n_layers >= 0 && n_layers <= c.llm_layers, "n_layers=%d outside 0..%d", n_layers, c.llm_layers);
@@ -548,8 +558,9 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
                 h->npad_max);
   }
   const int* np = h->padded ? h->d_npad : nullptr;
+  const int* pk = packed ? h->d_pack : nullptr;
   const int D = c.llm_hidden, F = c.llm_inter, H = c.llm_heads, NV = h->NV;
-  const int M = B * S;
+  const int M = packed ? packed_rows : B * S;
   const size_t slot_off = (size_t)slot * H * c.max_seq * 128;
   auto kc = [&](int l) { return kc_layer(h, l) + slot_off; };
   auto vc = [&](int l) { return vc_layer(h, l) + slot_off; };
@@ -566,7 +577,7 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
     }
   }
   VCL_TRY(launch_embed_splice(reinterpret_cast<const long long*>(ids), h->embed, h->l_vid, vid_start,
-                              h->l_h, B, S, D, video_feats ? NV : 0, c.vocab, st));
+                              h->l_h, B, S, D, video_feats ? NV : 0, c.vocab, st, pk, M));
   const float scale = 0.08838834764831845f;  // 128 ^ -1/2
   auto keep_state = [&](int i) -> int {
     if (states_out == nullptr) return 0;
@@ -579,14 +590,16 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
     const LlmLayerW& w = h->ll[l];
     VCL_TRY(launch_rmsnorm(h->l_h, D, h->l_x, D, w.ln1, M, D, c.rms_eps, st));
     // q|k|v projection with RoPE and the KV-cache write in its epilogue: q lands (rotated) in l_qkv, k and v in
-    // the cache. VCL_PREFILL_ROPE_SEPARATE=1: plain GEMM + rope_kv_prefill_kernel (A/B)
+    // the cache. VCL_PREFILL_ROPE_SEPARATE=1: plain GEMM + rope_kv_prefill_kernel (A/B; packed sequences always
+    // take the epilogue)
     static const bool rope_separate = getenv("VCL_PREFILL_ROPE_SEPARATE") != nullptr;
-    if (!rope_separate) {
+    if (!rope_separate || packed) {
       GemmArgs g;
       g.A = h->l_x; g.lda = D; g.W = w.wqkv; g.ldw = D; g.C = h->l_qkv; g.ldc = 3 * D; g.M = M; g.N = 3 * D; g.K = D;
       g.act = ACT_ROPE;
       g.rope.cos_t = h->rope_cos; g.rope.sin_t = h->rope_sin; g.rope.kcache = kc(l); g.rope.vcache = vc(l);
       g.rope.S = S; g.rope.start_pos = start_pos; g.rope.H = H; g.rope.s_max = c.max_seq; g.rope.n_pad = np;
+      g.rope.pack = pk;
       VCL_TRY(launch_gemm_bf16_tn(g, st));
     } else {
       VCL_TRY(gemm(h->l_x, D, w.wqkv, D, h->l_qkv, 3 * D, nullptr, nullptr, 0, M, 3 * D, D, ACT_NONE, st));
@@ -599,7 +612,7 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
     a.v = vc(l); a.v_sb = a.k_sb; a.v_sh = a.k_sh; a.v_ss = 128;
     a.o = h->l_attn; a.o_sb = (long long)S * D; a.o_sh = 128; a.o_ss = D;
     a.B = B; a.H = H; a.S = S; a.head_dim = 128; a.scale = scale; a.causal = 1;
-    a.S_kv = start_pos + S; a.q_off = start_pos; a.n_pad = np;
+    a.S_kv = start_pos + S; a.q_off = start_pos; a.n_pad = np; a.pack = pk;
     VCL_TRY(launch_attention(a, st));
     VCL_TRY(gemm(h->l_attn, D, w.wo, D, h->l_h, D, nullptr, h->l_h, D, M, D, D, ACT_NONE, st));
     VCL_TRY(launch_rmsnorm(h->l_h, D, h->l_x, D, w.ln2, M, D, c.rms_eps, st));
@@ -609,6 +622,11 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
   }
   if (hidden_out != nullptr)
     VCL_CUDA_OK(cudaMemcpyAsync(hidden_out, h->l_h, (size_t)M * D * 2, cudaMemcpyDeviceToDevice, st));
+  if (packed && next_tok != nullptr) {
+    // each sequence's last row, gathered into B contiguous rows of l_x (dead after the last layer)
+    VCL_TRY(launch_embed_tokens(pack_last(pk), 1, h->l_h, h->l_x, B, D, M, st));
+    return lm_head_argmax(h, h->l_x, D, B, nullptr, next_tok, tok_stride, st);
+  }
   if (logits_out != nullptr || next_tok != nullptr)
     VCL_TRY(lm_head_argmax(h, h->l_h + (size_t)(S - 1) * D, (long long)S * D, B, logits_out, next_tok,
                            tok_stride, st));
@@ -906,6 +924,44 @@ int vcl_llm_slot_prefill(vcl_handle* h, int slot, const int64_t* ids, const void
               "most 16 slots)", slot, h->n_slots_max() - 1, h->cfg.max_batch);
   return llm_prefill(h, ids, video_feats, vid_start, 1, S, h->cfg.llm_layers, nullptr, nullptr, next_tok, 1,
                      as_stream(stream), 0, nullptr, nullptr, slot);
+}
+
+int vcl_llm_slots_prefill(vcl_handle* h, int n, const int32_t* slots_host, const int32_t* seq_len_host,
+                          const int64_t* ids, const void* video_feats, const int32_t* vid_start, int32_t* next_tok,
+                          void* stream) {
+  VCL_REQUIRE(h != nullptr, "vcl_llm_slots_prefill: null handle");
+  const vcl_config& c = h->cfg;
+  VCL_REQUIRE(n >= 1 && n <= h->n_slots_max(), "vcl_llm_slots_prefill: n=%d outside 1..%d (max_batch %d, at most 16 "
+              "slots)", n, h->n_slots_max(), c.max_batch);
+  VCL_REQUIRE(slots_host && seq_len_host && ids && vid_start && next_tok, "vcl_llm_slots_prefill: null argument");
+  VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
+  const int s_lim = c.max_seq < 512 ? c.max_seq : 512;   // 512: the key limit of the wgmma prefill attention
+  long long M = 0;
+  int S_max = 0;
+  for (int i = 0; i < n; ++i) {
+    const int s = slots_host[i], len = seq_len_host[i];
+    VCL_REQUIRE(s >= 0 && s < h->n_slots_max(), "vcl_llm_slots_prefill: slot %d outside 0..%d", s, h->n_slots_max() - 1);
+    for (int j = 0; j < i; ++j)
+      VCL_REQUIRE(slots_host[j] != s, "vcl_llm_slots_prefill: slot %d is given twice", s);
+    VCL_REQUIRE(len >= 1 && len <= s_lim, "vcl_llm_slots_prefill: sequence %d has %d tokens, outside 1..%d", i, len,
+                s_lim);
+    M += len;
+    S_max = len > S_max ? len : S_max;
+  }
+  // n <= max_batch sequences of at most max_seq tokens: M fits the activations (max_batch * max_seq rows)
+  std::vector<int> map(pack_elems(M), 0);
+  int* p = map.data();
+  for (int i = 0, r = 0; i < n; ++i) {
+    pack_off(p)[i] = r; pack_len(p)[i] = seq_len_host[i]; pack_slot(p)[i] = slots_host[i];
+    pack_last(p)[i] = r + seq_len_host[i] - 1;
+    for (int j = 0; j < seq_len_host[i]; ++j, ++r) {
+      pack_row(p, r)[0] = i; pack_row(p, r)[1] = j;
+    }
+  }
+  cudaStream_t st = as_stream(stream);
+  VCL_CUDA_OK(cudaMemcpyAsync(h->d_pack, p, map.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  return llm_prefill(h, ids, video_feats, vid_start, n, S_max, c.llm_layers, nullptr, nullptr, next_tok, 1, st, 0,
+                     nullptr, nullptr, 0, (int)M);
 }
 
 int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* pos_host, int n_slots, int n_new,

@@ -69,6 +69,8 @@ _SIGNATURES = {
     "vcl_llm_score": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_void_p,
                               c_void_p, c_void_p, c_void_p, c_void_p]),
     "vcl_llm_slot_prefill": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "vcl_llm_slots_prefill": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), c_void_p, c_void_p,
+                                      c_void_p, c_void_p, c_void_p]),
     "vcl_llm_slot_decode": (c_int, [c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_void_p, c_void_p]),
     "vcl_launch_count": (ctypes.c_longlong, []),
     "vcl_kv_cache_copy": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
@@ -466,6 +468,31 @@ class Engine:
             assert vf.shape == (1, self.NV, self.cfg.clip_hidden), vf.shape
         check(lib().vcl_llm_slot_prefill(self._h, int(slot), ptr(ids), ptr(vf), ptr(vid_start.contiguous()),
                                          ids.shape[1], ptr(tok), cur_stream()))
+        return tok
+
+    def slots_prefill(self, slots, ids_list, feats_list, vid_starts, tok_out=None):
+        """Prompt i (ids_list[i], [S_i] or [1, S_i]) into cache slot slots[i], all in one packed prefill
+        (vcl_llm_slots_prefill). feats_list[i]: its video features [NV, C] / [1, NV, C] or None (text only; its
+        vid_starts entry is then ignored), vid_starts: ints. Returns the first tokens, [n] int32 on the device
+        (tok_out if given); each equals slot_prefill of that prompt alone, and so does the slot's cache."""
+        n = len(slots)
+        if not (len(ids_list) == len(feats_list) == len(vid_starts) == n):
+            raise VclError(f"{n} slots, {len(ids_list)} prompts, {len(feats_list)} features, {len(vid_starts)} vid_starts")
+        dev = "cuda"
+        ids = [torch.as_tensor(t).reshape(-1) for t in ids_list]
+        lens = [t.numel() for t in ids]
+        packed = torch.cat([t.to(dev, torch.int64) for t in ids]) if n else torch.empty(0, dtype=torch.int64, device=dev)
+        vf = None
+        if any(f is not None for f in feats_list):
+            vf = torch.zeros(n, self.NV, self.cfg.clip_hidden, dtype=torch.bfloat16, device=dev)
+            for i, f in enumerate(feats_list):
+                if f is not None:
+                    vf[i] = f.reshape(self.NV, self.cfg.clip_hidden)
+        vs = torch.tensor([int(v) if f is not None else NO_VIDEO for v, f in zip(vid_starts, feats_list)],
+                          dtype=torch.int32, device=dev)
+        tok = tok_out if tok_out is not None else torch.empty(n, dtype=torch.int32, device=dev)
+        check(lib().vcl_llm_slots_prefill(self._h, n, (c_int32 * n)(*[int(s) for s in slots]), (c_int32 * n)(*lens),
+                                          ptr(packed), ptr(vf), ptr(vs), ptr(tok), cur_stream()))
         return tok
 
     def slot_decode(self, first_tok, positions, n_new, out=None):

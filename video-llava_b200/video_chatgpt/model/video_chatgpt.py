@@ -616,10 +616,12 @@ class VideoChatGPTLlamaForCausalLM:
     # tools/bench_inflight.py (64 requests, 16..384 tokens, 7B shapes, H100 at 400 W): 7.89 / 8.13 / 8.35 s for 8 /
     # 16 / 32 at 16 slots, 19.5 / 19.9 / 20.7 s at 4 -- a retired slot idles for the rest of its chunk
     _SLOT_CHUNK = 8
+    # the longest prompt a packed admission (vcl_llm_slots_prefill) takes: the key limit of its attention kernel
+    _PACKED_MAX_S = 512
 
     @torch.no_grad()
     def generate_requests(self, requests, max_new_tokens=32, eos_token_id="config", stopping_criteria=None,
-                          slots=None, do_sample=False):
+                          slots=None, do_sample=False, packed_admission=False):
         """Greedy generation for many independent requests by in-flight (continuous) batching: every request
         owns a slot of the KV cache while it runs, and a finished request's slot takes the next queued one at
         once while the other slots keep decoding (a static batch decodes until its longest row finishes).
@@ -635,7 +637,10 @@ class VideoChatGPTLlamaForCausalLM:
         as a stepwise generate would call it).
         slots: cache slots in flight, default and at most min(max_batch, 16). Requests are admitted one prefill
         at a time; all slots then decode _SLOT_CHUNK steps per device call. Everything is validated before any
-        device work. Afterwards there is no turn for generate_continue to continue."""
+        device work. Afterwards there is no turn for generate_continue to continue.
+        packed_admission: at every admission point all free slots are filled from the queue (in queue order) by
+        one packed prefill (Engine.slots_prefill) instead of one prefill each; a prompt longer than
+        _PACKED_MAX_S is admitted alone. The results are the same either way."""
         if do_sample:
             raise NotImplementedError("generate_requests decodes greedily; sampling runs on generate")
         cap = min(self._max_batch, 16)
@@ -656,14 +661,19 @@ class VideoChatGPTLlamaForCausalLM:
         gen = {}                            # request -> its new tokens so far
         first = torch.zeros(n_slots, dtype=torch.int32, device=dev)     # the token each slot is fed next
         while True:
+            admitted = []
             for s in range(n_slots):
                 if owner[s] is None and queue:
                     i = queue.popleft()
                     r = reqs[i]
-                    feats = None if r.feats is None else r.feats.to(dev)
-                    vs = torch.tensor([r.vid_start], dtype=torch.int32, device=dev)
-                    eng.slot_prefill(s, r.ids.to(dev), feats, vs, tok_out=first[s:s + 1])
+                    if not packed_admission:
+                        feats = None if r.feats is None else r.feats.to(dev)
+                        vs = torch.tensor([r.vid_start], dtype=torch.int32, device=dev)
+                        eng.slot_prefill(s, r.ids.to(dev), feats, vs, tok_out=first[s:s + 1])
+                    admitted.append((s, i))
                     owner[s], pos[s], unseen[s], gen[i] = i, r.S, True, []
+            if admitted and packed_admission:
+                self._admit_packed(eng, [(s, reqs[i]) for s, i in admitted], first)
             active = [s for s in range(n_slots) if owner[s] is not None]
             if not active:
                 return results
@@ -683,6 +693,27 @@ class VideoChatGPTLlamaForCausalLM:
                         owner[s], pos[s] = None, 0
                         break
                 unseen[s] = False
+
+    def _admit_packed(self, eng, group, first):
+        """Prefill the (slot, request) pairs of one admission point: prompts longer than _PACKED_MAX_S one at a time
+        (slot_prefill), all others in one slots_prefill. Each slot's first token goes to first[slot]. The packed
+        prompts always fit the activations (max_batch * max_seq tokens): there are at most max_batch of them, each
+        shorter than max_seq (_request)."""
+        dev = first.device
+        packed = []
+        for s, r in group:
+            if r.S > self._PACKED_MAX_S:
+                feats = None if r.feats is None else r.feats.to(dev)
+                vs = torch.tensor([r.vid_start], dtype=torch.int32, device=dev)
+                eng.slot_prefill(s, r.ids.to(dev), feats, vs, tok_out=first[s:s + 1])
+            else:
+                packed.append((s, r))
+        if packed:
+            slots = [s for s, _ in packed]
+            tok = eng.slots_prefill(slots, [r.ids for _, r in packed],
+                                    [None if r.feats is None else r.feats.to(dev) for _, r in packed],
+                                    [r.vid_start for _, r in packed])
+            first[torch.tensor(slots, device=dev)] = tok
 
     def _request(self, i, r, max_new_tokens, stopping_criteria, n_vid):
         """One request of generate_requests, checked on the host -> (ids [S] int64 on the host, S, n, feats,
