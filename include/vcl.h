@@ -243,6 +243,26 @@ int vcl_llm_slots_prefill(vcl_handle* h, int n, const int32_t* slots_host, const
 int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* pos_host, int n_slots, int n_new,
                         int32_t* out_tokens, void* stream);
 
+/* Sampling (model.generate(do_sample=True, temperature=T, top_k=k), video_chatgpt/inference.py:105-107, i.e.
+ * transformers' TemperatureLogitsWarper then TopKLogitsWarper then a multinomial draw). The handle holds one
+ * sampling table of max_batch entries at fixed device addresses; entry b belongs to clip b, or to cache slot b.
+ * Every call that produces a token (vcl_llm_prefill(_padded), _prefill_append, _decode_step, _generate(_padded),
+ * _decode_loop, _slot_prefill, _slots_prefill -- prompt i with entry slots_host[i] -- and _slot_decode) picks
+ * clip b's token by entry b: temperature 0 is greedy (the arg-max), otherwise the token is drawn from
+ * softmax(logits / T) over the top-k logits (ties at the k-th value kept; k = 0 or k >= vocab keeps all) with
+ * u from Philox4x32-10, key = the entry's seed, counter = the RoPE position the new token takes. So a sequence's
+ * tokens depend on (seed, positions) only, not on its clip or slot, its neighbours, padding or chunking. A row
+ * whose scaled maximum logit is not finite falls back to the arg-max. The exact rules are in DESIGN.md section 3.
+ * When every entry a call uses is greedy, the call launches the same kernels as before any sampling was set; a
+ * sampled decode loop has a CUDA graph of its own per (B, n_new), replayed for any settings.
+ *
+ * vcl_llm_set_sampling writes n entries: clip clips_host[i] gets temperature_host[i], top_k_host[i] and
+ * seed_host[i] (all HOST memory, [n]); one host-to-device copy on `stream`. All entries are greedy after
+ * vcl_create. Rejected before any device work: n outside 1 .. max_batch, a clip outside 0 .. max_batch-1 or
+ * given twice, a temperature below 0 or not finite, a negative top_k. */
+int vcl_llm_set_sampling(vcl_handle* h, int n, const int32_t* clips_host, const float* temperature_host,
+                         const int32_t* top_k_host, const uint64_t* seed_host, void* stream);
+
 /* forward(input_ids, labels=..., ...) (video_chatgpt/model/video_chatgpt.py:225-239): lm_head at EVERY
  * position and, with labels, the shifted cross-entropy of CrossEntropyLoss (ignore_index -100): column s of
  * clip b is scored against labels[b, s+1]; column S-1 has no target. The prefill is vcl_llm_prefill's
@@ -284,6 +304,12 @@ int vcl_op_gemm_ex(const void* A, int64_t lda, const void* W, int64_t ldw, void*
  * (required) and, optionally, loss_out [1] fp32, the mean over the rows whose label is not -100. */
 int vcl_op_cross_entropy(const void* logits, int64_t ld, const int64_t* labels, int rows, int V,
                          float* nll_out, float* loss_out, void* stream);
+/* The sampling kernel on its own: row b of logits [B, ld] fp32 (first V columns; bf16-representable values, as
+ * the lm_head writes them) is sampled with temperature_host[b] (0: greedy), top_k_host[b], seed_host[b] and the
+ * Philox counter counter_host[b] (all HOST memory, [B]); tok_out [B] int32 on the device. V <= 81920. */
+int vcl_op_sample(const float* logits, int64_t ld, int B, int V, const float* temperature_host,
+                  const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host, int32_t* tok_out,
+                  void* stream);
 int vcl_op_layernorm(const void* x, void* y, const void* w, const void* b, int rows, int D, float eps,
                      void* stream);
 int vcl_op_rmsnorm(const void* x, void* y, const void* w, int rows, int D, float eps, void* stream);

@@ -17,7 +17,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libvcl.so")
-SOURCES = ["vcl_api.cu", "gemm_tc.cu", "decode_gemv.cu", "attention.cu", "attention_tc.cu", "attention_prefill_tc.cu", "decode_attention.cu", "elementwise.cu", "st_pool.cu", "cross_entropy.cu"]
+SOURCES = ["vcl_api.cu", "gemm_tc.cu", "decode_gemv.cu", "attention.cu", "attention_tc.cu", "attention_prefill_tc.cu", "decode_attention.cu", "elementwise.cu", "st_pool.cu", "cross_entropy.cu", "sampling.cu"]
 HEADERS = ["common.cuh", "kernels.h", os.path.join("..", "..", "include", "vcl.h")]
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

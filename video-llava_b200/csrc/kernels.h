@@ -128,6 +128,20 @@ int launch_cross_entropy(const bf16* logits, long long ld, int V, const long lon
 int launch_nll_mean(const float* nll, const long long* labels, long long rows, int seg, float* nll_out,
                     float* loss_out, cudaStream_t stream);
 
+// ---- sampling.cu --------------------------------------------------------------------------------
+// Next token of each logits row [B][ld] (first V columns; bf16 values in fp32 storage) by the rules at the top of
+// sampling.cu. Row r uses entry t = entry0 + (rowmap ? rowmap[r] : r) of the sampling table (temperature, top_k,
+// seed: device arrays; temperature 0 is greedy) and draws at counter p = col + (col_dev ? col_dev[r] : 0) -
+// (n_pad ? n_pad[t] : 0), the RoPE position its token takes. out[r * out_stride] receives the token.
+struct SampleArgs {
+  const float* logits = nullptr; long long ld = 0; int V = 0, B = 0;
+  const float* temperature = nullptr; const int* top_k = nullptr; const unsigned long long* seed = nullptr;
+  int entry0 = 0; const int* rowmap = nullptr;
+  int col = 0; const int* col_dev = nullptr; const int* n_pad = nullptr;
+  int* out = nullptr; long long out_stride = 1;
+};
+int launch_sample(const SampleArgs& a, cudaStream_t stream);
+
 // ---- attention.cu -------------------------------------------------------------------------------
 // softmax(Q K^T * scale [+ causal]) V for S_q == S_kv, bf16, fp32 softmax; element (b,h,s,d) of
 // each operand lives at base + b*sb + h*sh + s*ss + d.

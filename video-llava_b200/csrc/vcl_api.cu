@@ -49,7 +49,8 @@ struct LlmLayerW {
   bf16 *wqkv_t = nullptr, *wo_t = nullptr, *wgu_t = nullptr, *wd_t = nullptr;   // slot-ordered copies for decode
 };
 struct GraphEntry {
-  int B, n_new;        // the positions and pad counts are read on the device (h->d_pos, h->d_npad)
+  int B, n_new;        // the positions and pad counts are read on the device (h->d_pos, h->d_npad) ...
+  bool sampled;        // ... and so is the sampling table: a sampled graph serves every temperature / top_k / seed
   cudaGraphExec_t exec;
   long long kernels;   // kernel nodes in the graph (for vcl_launch_count)
   unsigned long long last_use;
@@ -65,6 +66,15 @@ struct StepIo {
   float* logits_out = nullptr;
   int32_t* tok_out = nullptr; long long out_stride = 1;
   const int* pos_dev = nullptr;   // clip b at position pos + pos_dev[b] (null: pos)
+  bool sampled = false;           // the sampler picks tok_out (entry b of the sampling table for clip b)
+};
+
+// which sampling-table entries the rows of an lm_head call use, and the cache column their tokens take
+// (SampleArgs in kernels.h; the counter subtracts the clip's left padding)
+struct SampleAt {
+  bool on = false;                              // some entry samples: the sampler replaces the arg-max kernel
+  int entry0 = 0; const int* rowmap = nullptr;  // row r: entry entry0 + (rowmap ? rowmap[r] : r)
+  int col = 0; const int* col_dev = nullptr;    // row r: column col + (col_dev ? col_dev[r] : 0)
 };
 
 }  // namespace
@@ -110,6 +120,22 @@ struct vcl_handle {
   ArgmaxPart* amax = nullptr;                  // [gemv_grid(vocab)][max_batch] per-CTA partial arg-max of the logits kernel
   int* d_pack = nullptr;                       // pack_elems(max_batch * max_seq): the packed-row map of kernels.h,
                                                // written by each vcl_llm_slots_prefill with one host-to-device copy
+  // The sampling table (vcl_llm_set_sampling): entry b belongs to clip b / cache slot b. One device block at a
+  // fixed address, [max_batch] seeds (u64), temperatures (f32), top_k (i32), so one sampled decode graph serves
+  // every setting; samp_host is its host copy, written whole by one host-to-device copy per call. All zeros
+  // (greedy) at vcl_create.
+  unsigned char* samp = nullptr;
+  std::vector<unsigned char> samp_host;
+  unsigned long long* samp_seed(unsigned char* base) const { return reinterpret_cast<unsigned long long*>(base); }
+  float* samp_temp(unsigned char* base) const { return reinterpret_cast<float*>(base + 8 * cfg.max_batch); }
+  int* samp_topk(unsigned char* base) const { return reinterpret_cast<int*>(base + 12 * cfg.max_batch); }
+  // whether entry first .. first + n - 1 samples (a temperature above 0)
+  bool sampling(int first, int n) {
+    const float* t = samp_temp(samp_host.data());
+    for (int b = first; b < first + n; ++b)
+      if (t[b] > 0.f) return true;
+    return false;
+  }
 
   size_t cache_layer_elems() const {
     return (size_t)cfg.max_batch * cfg.llm_heads * cfg.max_seq * 128;
@@ -269,9 +295,12 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   rc |= dalloc(h, &h->d_npad, Bm);
   rc |= dalloc(h, &h->amax, (size_t)device_num_sms() * Bm);
   rc |= dalloc(h, &h->d_pack, pack_elems((long long)Ml));
+  rc |= dalloc(h, &h->samp, Bm * 16);
+  h->samp_host.assign(Bm * 16, 0);
   if (rc == 0) rc = launch_rope_table(h->rope_cos, h->rope_sin, c->max_seq, 128, c->rope_theta, 0);
   if (rc == 0) {
     cudaError_t e = cudaMemset(h->d_npad, 0, Bm * sizeof(int));   // the cache starts unpadded
+    if (e == cudaSuccess) e = cudaMemset(h->samp, 0, Bm * 16);        // and every entry greedy
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
     if (e != cudaSuccess) {
       set_last_error("vcl_create: %s", cudaGetErrorString(e));
@@ -473,9 +502,12 @@ bf16* vc_layer(vcl_handle* h, int l) { return h->vcache + (size_t)l * h->cache_l
 
 // final RMSNorm + lm_head on rows x[b*ldx .. ] (b < B), arg-max
 // partials_out: the arg-max is left as per-CTA partials in h->amax for the next step's q|k|v kernel
+// smp.on: the sampler picks the tokens instead of the arg-max kernel (the logits are then always written)
 int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* logits_out,
-                   int32_t* tok_out, long long tok_stride, cudaStream_t st, bool partials_out = false) {
+                   int32_t* tok_out, long long tok_stride, cudaStream_t st, bool partials_out = false,
+                   const SampleAt& smp = SampleAt()) {
   const vcl_config& c = h->cfg;
+  VCL_REQUIRE(!(partials_out && smp.on), "sampled rows need the logits, not the partial arg-max");
   GemvArgs g;
   g.W_tiled = h->lm_head_t; g.N = c.vocab; g.K = c.llm_hidden;
   GemvEpilogue e;
@@ -503,6 +535,14 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
   if (logits_out != nullptr && logits_out != h->logits)
     VCL_CUDA_OK(cudaMemcpyAsync(logits_out, h->logits, (size_t)B * c.vocab * sizeof(float),
                                 cudaMemcpyDeviceToDevice, st));
+  if (tok_out != nullptr && smp.on) {
+    SampleArgs sa;
+    sa.logits = h->logits; sa.ld = c.vocab; sa.V = c.vocab; sa.B = B;
+    sa.temperature = h->samp_temp(h->samp); sa.top_k = h->samp_topk(h->samp); sa.seed = h->samp_seed(h->samp);
+    sa.entry0 = smp.entry0; sa.rowmap = smp.rowmap; sa.col = smp.col; sa.col_dev = smp.col_dev; sa.n_pad = h->d_npad;
+    sa.out = tok_out; sa.out_stride = tok_stride;
+    return launch_sample(sa, st);
+  }
   if (tok_out != nullptr) VCL_TRY(launch_argmax(h->logits, tok_out, tok_stride, B, c.vocab, st));
   return 0;
 }
@@ -521,7 +561,7 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
 int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
                 int B, int S, int n_layers, void* hidden_out, float* logits_out, int32_t* next_tok,
                 long long tok_stride, cudaStream_t st, int start_pos = 0, void* states_out = nullptr,
-                const int32_t* n_pad_host = nullptr, int slot = 0, int packed_rows = 0) {
+                const int32_t* n_pad_host = nullptr, int slot = 0, int packed_rows = 0, bool pack_sampled = false) {
   const vcl_config& c = h->cfg;
   const bool packed = packed_rows > 0;
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
@@ -625,11 +665,17 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
   if (packed && next_tok != nullptr) {
     // each sequence's last row, gathered into B contiguous rows of l_x (dead after the last layer)
     VCL_TRY(launch_embed_tokens(pack_last(pk), 1, h->l_h, h->l_x, B, D, M, st));
-    return lm_head_argmax(h, h->l_x, D, B, nullptr, next_tok, tok_stride, st);
+    // sequence i samples with its slot's entry; its token takes column S_i
+    SampleAt smp;
+    smp.on = pack_sampled; smp.rowmap = pack_slot(pk); smp.col_dev = pack_len(pk);
+    return lm_head_argmax(h, h->l_x, D, B, nullptr, next_tok, tok_stride, st, false, smp);
   }
-  if (logits_out != nullptr || next_tok != nullptr)
+  if (logits_out != nullptr || next_tok != nullptr) {
+    SampleAt smp;   // clip b (slot `slot` for B = 1) samples with its entry; its token takes column start_pos + S
+    smp.on = next_tok != nullptr && h->sampling(slot, B); smp.entry0 = slot; smp.col = start_pos + S;
     VCL_TRY(lm_head_argmax(h, h->l_h + (size_t)(S - 1) * D, (long long)S * D, B, logits_out, next_tok,
-                           tok_stride, st));
+                           tok_stride, st, false, smp));
+  }
   return 0;
 }
 
@@ -743,7 +789,9 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
       VCL_TRY(gemm(h->d_act, F, w.wd, F, h->d_h, D, nullptr, h->d_h, D, B, D, F, ACT_NONE, st));
     }
   }
-  VCL_TRY(lm_head_argmax(h, h->d_h, D, B, io.logits_out, io.tok_out, io.out_stride, st, io.partials_out));
+  SampleAt smp;   // the token fed at column c_b is followed by one at column c_b + 1
+  smp.on = io.sampled; smp.col = pos + 1; smp.col_dev = pd;
+  VCL_TRY(lm_head_argmax(h, h->d_h, D, B, io.logits_out, io.tok_out, io.out_stride, st, io.partials_out, smp));
   return 0;
 }
 
@@ -751,11 +799,14 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
 // For 1..4 clips no arg-max / embedding kernel runs between two steps: the logits kernel leaves
 // per-CTA partials, the next step's first q|k|v kernel reduces them, records the token and gathers
 // its embedding row. Step i feeds clip b at position h->d_pos[b] + i - 1.
-int decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st) {
-  const bool hand_off = B <= 4 && h->cfg.llm_layers > 0;
+// sampled: the sampler writes tk[:, i] from the full logits, and the next step gathers from tk (fused into
+// layer 0 for 1..4 clips, the embedding kernel otherwise).
+int decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, bool sampled) {
+  const bool hand_off = B <= 4 && h->cfg.llm_layers > 0 && !sampled;
   for (int i = 1; i < n_new; ++i) {
     StepIo io;
     io.pos_dev = h->d_pos;
+    io.sampled = sampled;
     if (hand_off && i > 1) {
       io.tok_from_partials = true; io.tok_store = tk + (i - 1); io.store_stride = n_new;
     } else {
@@ -768,13 +819,14 @@ int decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st) 
   return 0;
 }
 
-// decode_steps from one captured graph per (B, n_new). The positions (h->d_pos, written by the caller) and the
-// pad counts (h->d_npad) are read on the device, so new positions or padding replay the same graph. Bounded LRU
-// cache (an entry holds thousands of nodes). A stream that cannot be captured runs the steps eagerly.
-int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st) {
+// decode_steps from one captured graph per (B, n_new, sampled). The positions (h->d_pos, written by the caller),
+// the pad counts (h->d_npad) and the sampling table are read on the device, so new positions, padding or sampling
+// settings replay the same graph. Bounded LRU cache (an entry holds thousands of nodes). A stream that cannot be
+// captured runs the steps eagerly.
+int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, bool sampled) {
   GraphEntry* ge = nullptr;
   for (auto& g : h->graphs)
-    if (g.B == B && g.n_new == n_new) ge = &g;
+    if (g.B == B && g.n_new == n_new && g.sampled == sampled) ge = &g;
   const bool can_capture = (st != nullptr) && (st != cudaStreamLegacy);
   if (ge == nullptr && can_capture) {
     if (h->graphs.size() >= MAX_DECODE_GRAPHS) {
@@ -786,7 +838,7 @@ int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t 
     }
     const long long before = launch_count();
     VCL_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    const int rc = decode_steps(h, tk, B, n_new, st);
+    const int rc = decode_steps(h, tk, B, n_new, st, sampled);
     cudaGraph_t graph = nullptr;
     cudaError_t e = cudaStreamEndCapture(st, &graph);
     const long long nodes = launch_count() - before;
@@ -806,24 +858,25 @@ int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t 
       set_last_error("decode graph instantiate failed: %s", cudaGetErrorString(e));
       return -2;
     }
-    h->graphs.push_back({B, n_new, exec, nodes, 0});
+    h->graphs.push_back({B, n_new, sampled, exec, nodes, 0});
     ge = &h->graphs.back();
   }
-  if (ge == nullptr) return decode_steps(h, tk, B, n_new, st);
+  if (ge == nullptr) return decode_steps(h, tk, B, n_new, st, sampled);
   ge->last_use = ++h->graph_clock;
   VCL_CUDA_OK(cudaGraphLaunch(ge->exec, st));
   count_launches(ge->kernels);
   return 0;
 }
 
-// The greedy loop of vcl_llm_decode_loop and vcl_llm_slot_decode, with h->d_pos written by the caller: first_tok
-// [B] is fed, n_new - 1 steps follow, and [B, n_new] tokens (first_tok included) go to out_tokens.
+// The loop of vcl_llm_decode_loop and vcl_llm_slot_decode, with h->d_pos written by the caller: first_tok
+// [B] is fed, n_new - 1 steps follow, and [B, n_new] tokens (first_tok included) go to out_tokens. Greedy unless
+// one of the entries 0 .. B-1 of the sampling table samples.
 int decode_loop(vcl_handle* h, const int32_t* first_tok, int B, int n_new, int32_t* out_tokens, cudaStream_t st) {
   int32_t* tk = h->tokens;  // [B, n_new] row-major scratch
   if (first_tok != tk)
     VCL_CUDA_OK(cudaMemcpy2DAsync(tk, (size_t)n_new * sizeof(int32_t), first_tok, sizeof(int32_t),
                                   sizeof(int32_t), B, cudaMemcpyDeviceToDevice, st));
-  if (n_new > 1) VCL_TRY(run_decode_steps(h, tk, B, n_new, st));
+  if (n_new > 1) VCL_TRY(run_decode_steps(h, tk, B, n_new, st, h->sampling(0, B)));
   VCL_CUDA_OK(cudaMemcpyAsync(out_tokens, tk, (size_t)B * n_new * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
@@ -899,7 +952,7 @@ int vcl_llm_decode_step(vcl_handle* h, const int32_t* tok_in, int B, int pos, fl
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
   VCL_REQUIRE(B > 0 && B <= h->cfg.max_batch, "B=%d outside 1..%d", B, h->cfg.max_batch);
   StepIo io;
-  io.tok_in = tok_in; io.logits_out = logits_out; io.tok_out = tok_out;
+  io.tok_in = tok_in; io.logits_out = logits_out; io.tok_out = tok_out; io.sampled = h->sampling(0, B);
   return llm_decode_step(h, io, B, pos, as_stream(stream));
 }
 
@@ -960,8 +1013,10 @@ int vcl_llm_slots_prefill(vcl_handle* h, int n, const int32_t* slots_host, const
   }
   cudaStream_t st = as_stream(stream);
   VCL_CUDA_OK(cudaMemcpyAsync(h->d_pack, p, map.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  bool sampled = false;
+  for (int i = 0; i < n; ++i) sampled = sampled || h->sampling(slots_host[i], 1);
   return llm_prefill(h, ids, video_feats, vid_start, n, S_max, c.llm_layers, nullptr, nullptr, next_tok, 1, st, 0,
-                     nullptr, nullptr, 0, (int)M);
+                     nullptr, nullptr, 0, (int)M, sampled);
 }
 
 int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* pos_host, int n_slots, int n_new,
@@ -982,6 +1037,33 @@ int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* 
   if (n_new > 1)
     VCL_CUDA_OK(cudaMemcpyAsync(h->d_pos, pos_host, (size_t)n_slots * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   return decode_loop(h, first_tok, n_slots, n_new, out_tokens, st);
+}
+
+int vcl_llm_set_sampling(vcl_handle* h, int n, const int32_t* clips_host, const float* temperature_host,
+                         const int32_t* top_k_host, const uint64_t* seed_host, void* stream) {
+  VCL_REQUIRE(h != nullptr, "vcl_llm_set_sampling: null handle");
+  const int mb = h->cfg.max_batch;
+  VCL_REQUIRE(n >= 1 && n <= mb, "vcl_llm_set_sampling: n=%d outside 1..%d", n, mb);
+  VCL_REQUIRE(clips_host && temperature_host && top_k_host && seed_host, "vcl_llm_set_sampling: null argument");
+  for (int i = 0; i < n; ++i) {
+    const int b = clips_host[i];
+    const float T = temperature_host[i];
+    VCL_REQUIRE(b >= 0 && b < mb, "vcl_llm_set_sampling: clip %d outside 0..%d", b, mb - 1);
+    for (int j = 0; j < i; ++j)
+      VCL_REQUIRE(clips_host[j] != b, "vcl_llm_set_sampling: clip %d is given twice", b);
+    VCL_REQUIRE(isfinite(T) && T >= 0.f, "vcl_llm_set_sampling: temperature %g of clip %d is not a finite value >= 0",
+                (double)T, b);
+    VCL_REQUIRE(top_k_host[i] >= 0, "vcl_llm_set_sampling: top_k %d of clip %d is negative", top_k_host[i], b);
+  }
+  unsigned char* hb = h->samp_host.data();
+  for (int i = 0; i < n; ++i) {
+    const int b = clips_host[i];
+    h->samp_seed(hb)[b] = seed_host[i];
+    h->samp_temp(hb)[b] = temperature_host[i];
+    h->samp_topk(hb)[b] = top_k_host[i];
+  }
+  VCL_CUDA_OK(cudaMemcpyAsync(h->samp, hb, h->samp_host.size(), cudaMemcpyHostToDevice, as_stream(stream)));
+  return 0;
 }
 
 int vcl_llm_generate(vcl_handle* h, const int64_t* ids, const void* video_feats,
@@ -1076,6 +1158,39 @@ int vcl_op_cross_entropy(const void* logits, int64_t ld, const int64_t* labels, 
   VCL_TRY(launch_cross_entropy(reinterpret_cast<const bf16*>(logits), ld, V, lab, 0, rows, 0, nll_out, nullptr,
                                as_stream(stream)));
   return loss_out != nullptr ? launch_nll_mean(nll_out, lab, rows, 0, nullptr, loss_out, as_stream(stream)) : 0;
+}
+
+int vcl_op_sample(const float* logits, int64_t ld, int B, int V, const float* temperature_host,
+                  const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host, int32_t* tok_out,
+                  void* stream) {
+  if (check_device() != 0) return -2;
+  VCL_REQUIRE(logits && temperature_host && top_k_host && seed_host && counter_host && tok_out,
+              "vcl_op_sample: null argument");
+  VCL_REQUIRE(B >= 1, "vcl_op_sample: B=%d", B);
+  for (int b = 0; b < B; ++b)
+    VCL_REQUIRE(isfinite(temperature_host[b]) && temperature_host[b] >= 0.f && top_k_host[b] >= 0 &&
+                counter_host[b] >= 0, "vcl_op_sample: row %d: temperature %g, top_k %d, counter %d", b,
+                (double)temperature_host[b], top_k_host[b], counter_host[b]);
+  // the per-row settings in one stream-ordered block: [B] seeds, temperatures, top_k, counters
+  std::vector<unsigned char> hb((size_t)B * 20);
+  memcpy(hb.data(), seed_host, (size_t)B * 8);
+  memcpy(hb.data() + (size_t)B * 8, temperature_host, (size_t)B * 4);
+  memcpy(hb.data() + (size_t)B * 12, top_k_host, (size_t)B * 4);
+  memcpy(hb.data() + (size_t)B * 16, counter_host, (size_t)B * 4);
+  cudaStream_t st = as_stream(stream);
+  unsigned char* d = nullptr;
+  VCL_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&d), hb.size(), st));
+  VCL_CUDA_OK(cudaMemcpyAsync(d, hb.data(), hb.size(), cudaMemcpyHostToDevice, st));
+  SampleArgs sa;
+  sa.logits = logits; sa.ld = ld; sa.V = V; sa.B = B;
+  sa.seed = reinterpret_cast<const unsigned long long*>(d);
+  sa.temperature = reinterpret_cast<const float*>(d + (size_t)B * 8);
+  sa.top_k = reinterpret_cast<const int*>(d + (size_t)B * 12);
+  sa.col_dev = reinterpret_cast<const int*>(d + (size_t)B * 16);
+  sa.out = tok_out;
+  const int rc = launch_sample(sa, st);
+  VCL_CUDA_OK(cudaFreeAsync(d, st));
+  return rc;
 }
 
 int vcl_op_layernorm(const void* x, void* y, const void* w, const void* b, int rows, int D, float eps,

@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int64, c_void_p
+from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int64, c_uint64, c_void_p
 
 import torch
 
@@ -72,6 +72,8 @@ _SIGNATURES = {
     "vcl_llm_slots_prefill": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), c_void_p, c_void_p,
                                       c_void_p, c_void_p, c_void_p]),
     "vcl_llm_slot_decode": (c_int, [c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_void_p, c_void_p]),
+    "vcl_llm_set_sampling": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_float), POINTER(c_int32),
+                                     POINTER(c_uint64), c_void_p]),
     "vcl_launch_count": (ctypes.c_longlong, []),
     "vcl_kv_cache_copy": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_op_decode_attention": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
@@ -81,6 +83,8 @@ _SIGNATURES = {
                             c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "vcl_op_gemm_ex": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
                                c_int64, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "vcl_op_sample": (c_int, [c_void_p, c_int64, c_int, c_int, POINTER(c_float), POINTER(c_int32), POINTER(c_uint64),
+                              POINTER(c_int32), c_void_p, c_void_p]),
     "vcl_op_layernorm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "vcl_op_rmsnorm": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "vcl_op_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
@@ -199,6 +203,29 @@ def op_cross_entropy(logits, labels, V=None, want_loss=True):
     check(lib().vcl_op_cross_entropy(c_void_p(logits.data_ptr()), logits.stride(0), ptr(lab), rows,
                                      ld if V is None else V, ptr(nll), ptr(loss), cur_stream()))
     return nll, loss
+
+
+def _seeds(seeds, n):
+    """n 64-bit seeds (ints, taken mod 2**64) -> ctypes uint64[n]"""
+    vals = [int(v) % 2 ** 64 for v in seeds]
+    if len(vals) != n:
+        raise VclError(f"{len(vals)} seeds for {n} rows")
+    return (c_uint64 * n)(*vals)
+
+
+def op_sample(logits, temperature, top_k, seed, counter):
+    """The sampling kernel alone (vcl_op_sample). logits [B, ld] fp32 on the device (bf16-representable values);
+    temperature / top_k / seed / counter: B host values per row (temperature 0: greedy). Returns [B] int32."""
+    B, ld = logits.shape
+    assert logits.dtype == torch.float32 and logits.stride(1) == 1
+    out = torch.empty(B, dtype=torch.int32, device=logits.device)
+    vals = [list(v) for v in (temperature, top_k, counter)]
+    if not all(len(v) == B for v in vals):
+        raise VclError(f"temperature / top_k / counter need {B} entries each")
+    check(lib().vcl_op_sample(c_void_p(logits.data_ptr()), logits.stride(0), B, ld,
+                              (c_float * B)(*[float(t) for t in vals[0]]), (c_int32 * B)(*[int(k) for k in vals[1]]),
+                              _seeds(seed, B), (c_int32 * B)(*[int(c) for c in vals[2]]), ptr(out), cur_stream()))
+    return out
 
 
 def op_gemv(x, w, res=None, norm_w=None, eps=0.0):
@@ -436,6 +463,17 @@ class Engine:
             check(lib().vcl_llm_generate_padded(self._h, ptr(ids.contiguous()), ptr(vf), ptr(vid_start.contiguous()),
                                                 _host_pads(n_pad, B), B, S, n_new, ptr(out), cur_stream()))
         return out
+
+    # ---- sampling ----
+    def set_sampling(self, clips, temperature, top_k, seed):
+        """Entries `clips` of the sampling table (vcl_llm_set_sampling): clip / slot clips[i] samples with
+        temperature[i] (0: greedy), top_k[i] (0: all tokens) and the 64-bit seed[i]. Host lists of equal length."""
+        n = len(clips)
+        if not (len(temperature) == len(top_k) == n):
+            raise VclError(f"{n} clips, {len(temperature)} temperatures, {len(top_k)} top_k")
+        check(lib().vcl_llm_set_sampling(self._h, n, (c_int32 * n)(*[int(b) for b in clips]),
+                                         (c_float * n)(*[float(t) for t in temperature]),
+                                         (c_int32 * n)(*[int(k) for k in top_k]), _seeds(seed, n), cur_stream()))
 
     # ---- KV cache read-back (tests) ----
     def _cache_shape(self):

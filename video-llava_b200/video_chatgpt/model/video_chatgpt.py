@@ -28,7 +28,9 @@ conventions. Differences from the reference, all documented where they occur:
 from __future__ import annotations
 
 import collections
+import contextlib
 import json
+import math
 import os
 import sys
 from types import SimpleNamespace
@@ -548,10 +550,33 @@ class VideoChatGPTLlamaForCausalLM:
             pad_token_id = eos_token_id
         return eos_token_id, pad_token_id
 
+    @staticmethod
+    def _sampling_args(temperature, top_k, seed, what="generate"):
+        """Checks the settings of the device sampler on the host -> (temperature, top_k, seed mod 2**64)"""
+        t = float(temperature)
+        if not math.isfinite(t) or t < 0:
+            raise ValueError(f"{what}: temperature {temperature} must be a finite value >= 0")
+        k = 0 if top_k is None else top_k
+        if isinstance(k, bool) or not isinstance(k, int) or k < 0:
+            raise ValueError(f"{what}: top_k {top_k} must be an int >= 0 (0 or None: every token)")
+        if seed is not None and (isinstance(seed, bool) or not isinstance(seed, int)):
+            raise ValueError(f"{what}: seed {seed!r} must be an int")
+        return t, k, None if seed is None else seed % 2 ** 64
+
+    @contextlib.contextmanager
+    def _sampling(self, eng, clips, temperature, top_k, seeds):
+        """Entries `clips` of the engine's sampling table sample for the duration of the block and are greedy
+        again afterwards, also when the block raises."""
+        eng.set_sampling(clips, temperature, top_k, seeds)
+        try:
+            yield
+        finally:
+            eng.set_sampling(clips, [0.0] * len(clips), [0] * len(clips), [0] * len(clips))
+
     @torch.no_grad()
     def generate(self, input_ids, video_spatio_temporal_features=None, do_sample=False, temperature=1.0,
                  max_new_tokens=32, stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50,
-                 attention_mask=None, **kw):
+                 attention_mask=None, seed=None, **kw):
         """Returns [B, S+n] int64 INCLUDING the prompt, like HF generate (inference.py:105-120), and
         like HF it stops at EOS (config.eos_token_id unless eos_token_id is given; None disables it):
         finished rows are padded, the call returns when every row has finished.
@@ -561,7 +586,15 @@ class VideoChatGPTLlamaForCausalLM:
         stopping criteria take one C-ABI step per token with the host-side check the reference also
         performs every step.
         attention_mask [B, S]: a left-padded batch of prompts of different lengths (module docstring); every
-        path continues the padding through its decode steps. An all-ones mask is the same as none."""
+        path continues the padding through its decode steps. An all-ones mask is the same as none.
+        seed (an int): do_sample=True samples ON THE DEVICE (vcl_llm_set_sampling) with the same temperature /
+        top-k rules, row b with seed + b (mod 2**64), through the prefill and the CUDA-graph loops; EOS, padding
+        and stopping criteria are applied on the host between loops of _GREEDY_CHUNK tokens, token by token as
+        the stepwise path does. Each row's tokens depend on its seed and positions only. Without a seed,
+        do_sample=True keeps the stepwise path and torch's RNG (torch.manual_seed)."""
+        seeded = do_sample and seed is not None
+        if seeded:
+            temperature, top_k, seed = self._sampling_args(temperature, top_k, seed)
         pads = left_padding(attention_mask, input_ids.shape)
         eng = self._ensure_engine(need_llm=True)
         ids = input_ids.cuda().to(torch.int64)
@@ -574,6 +607,17 @@ class VideoChatGPTLlamaForCausalLM:
         if n <= 0:
             raise ValueError(f"prompt length {S} leaves no room in max_seq {self._max_seq}")
         eos, pad = self._eos_pad(eos_token_id, pad_token_id)
+        if seeded:
+            clips = list(range(B))
+            with self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips]):
+                if eos is None and not stopping_criteria:
+                    new = eng.generate(ids, feats, vs, n, n_pad=pads)
+                    self._pos = S + n - 1
+                    self._last_out = torch.cat([ids, new.to(torch.int64)], dim=1)
+                else:
+                    first = eng.generate(ids, feats, vs, min(n, self._GREEDY_CHUNK), n_pad=pads)
+                    self._last_out = self._host_stops(eng, ids, first, n, stopping_criteria, eos, pad)
+            return self._last_out
         if do_sample or stopping_criteria:
             _, logits, _ = eng.prefill(ids, feats, vs, want_logits=True, want_token=False, n_pad=pads)
             self._pos = S
@@ -600,6 +644,48 @@ class VideoChatGPTLlamaForCausalLM:
         self._last_out = torch.cat([ids, new], dim=1)
         return self._last_out
 
+    def _host_stops(self, eng, out, new, n, stopping_criteria, eos, pad):
+        """The device-sampled loop of generate / generate_continue: `new` [B, c] int32 holds the first c tokens
+        after the context `out` [B, L] (the first at column L). _stepwise's EOS / padding / stopping-criteria
+        logic runs token by token over each chunk on the host; the device decodes the next _GREEDY_CHUNK tokens
+        from the last kept (padded) token until a rule stops or n tokens are out. Returns [B, L + k]; self._pos
+        ends at L + k - 1, where _stepwise leaves it (columns decoded past the stop are overwritten by a
+        continuation). The sequence lives in one [B, L + n] buffer on out's device, filled by one copy per chunk;
+        a stopping criterion is called with a view of its first L + j columns, so a call costs no copy."""
+        dev, (B, L) = out.device, out.shape
+        full = torch.empty(B, L + n, dtype=torch.int64, device=dev)
+        full[:, :L] = out
+        unfinished = [True] * B
+        k = 0                                   # tokens kept so far
+        while True:
+            chunk, done, eos_stop = [], False, False
+            for col in zip(*new.tolist()):
+                if eos is not None:
+                    col = [t if u else pad for t, u in zip(col, unfinished)]
+                    unfinished = [u and t != eos for t, u in zip(col, unfinished)]
+                chunk.append(col)
+                if eos is not None and not any(unfinished):
+                    done = eos_stop = True
+                    break
+                if k + len(chunk) == n:
+                    done = True
+                    break
+            full[:, L + k:L + k + len(chunk)] = torch.tensor(chunk, dtype=torch.int64).T.to(dev)
+            if stopping_criteria:
+                # as in _stepwise: the criteria are not asked about the step at which every row has reached EOS
+                for j in range(len(chunk) - (1 if eos_stop else 0)):
+                    if any(c(full[:, :L + k + j + 1], None) for c in stopping_criteria):
+                        chunk, done = chunk[:j + 1], True
+                        break
+            k += len(chunk)
+            if done:
+                break
+            m = min(self._GREEDY_CHUNK, n - k)
+            last = full[:, L + k - 1].to(torch.int32).contiguous()
+            new = eng.decode_loop(last, L + k - 1, m + 1)[:, 1:]
+        self._pos = L + k - 1
+        return full[:, :L + k].clone()
+
     @staticmethod
     def _mask_finished(new, eos, pad):
         """Pad every row after its first EOS; when all rows have one, cut at the longest row."""
@@ -621,7 +707,7 @@ class VideoChatGPTLlamaForCausalLM:
 
     @torch.no_grad()
     def generate_requests(self, requests, max_new_tokens=32, eos_token_id="config", stopping_criteria=None,
-                          slots=None, do_sample=False, packed_admission=False):
+                          slots=None, do_sample=False, packed_admission=False, temperature=1.0, top_k=50, seed=None):
         """Greedy generation for many independent requests by in-flight (continuous) batching: every request
         owns a slot of the KV cache while it runs, and a finished request's slot takes the next queued one at
         once while the other slots keep decoding (a static batch decodes until its longest row finishes).
@@ -640,19 +726,39 @@ class VideoChatGPTLlamaForCausalLM:
         device work. Afterwards there is no turn for generate_continue to continue.
         packed_admission: at every admission point all free slots are filled from the queue (in queue order) by
         one packed prefill (Engine.slots_prefill) instead of one prefill each; a prompt longer than
-        _PACKED_MAX_S is admitted alone. The results are the same either way."""
-        if do_sample:
-            raise NotImplementedError("generate_requests decodes greedily; sampling runs on generate")
+        _PACKED_MAX_S is admitted alone. The results are the same either way.
+        do_sample / temperature / top_k / seed: sampling on the device, as generate(seed=...) samples. A request dict
+        may set its own "do_sample", "temperature", "top_k" and "seed"; a sampled request without its own seed
+        gets seed + its index (mod 2**64). Greedy and sampled requests share the batch; each admission writes the
+        admitted slots' entries of the engine's sampling table with one set_sampling call, and every slot is
+        greedy again when the call returns. A request's tokens depend on its seed and positions only: not on its
+        slot, its neighbours, the queue order or the admission mode. Sampling without any seed is not supported
+        in flight (only the stepwise generate draws from torch's RNG)."""
+        for i, r in enumerate(requests):
+            r = r if isinstance(r, dict) else {}
+            if r.get("do_sample", do_sample) and r.get("seed", seed) is None:
+                raise NotImplementedError(f"request {i}: generate_requests decodes greedily unless given a seed; "
+                                          "sampling in flight needs seed= (the call's or the request's own)")
         cap = min(self._max_batch, 16)
         n_slots = cap if slots is None else int(slots)
         if not 1 <= n_slots <= cap:
             raise ValueError(f"slots={slots} outside 1..{cap} (at most 16 and at most max_batch {self._max_batch})")
         eng = self._ensure_engine(need_llm=True)
-        reqs = [self._request(i, r, max_new_tokens, stopping_criteria, eng.NV) for i, r in enumerate(requests)]
+        samp = dict(do_sample=do_sample, temperature=temperature, top_k=top_k, seed=seed)
+        reqs = [self._request(i, r, max_new_tokens, stopping_criteria, eng.NV, samp) for i, r in enumerate(requests)]
+        sampling = any(r.temperature > 0 for r in reqs)
         eos, _ = self._eos_pad(eos_token_id, None)
         self._last_out, self._pos = None, 0
-        dev = self.device
         n_slots = min(n_slots, len(reqs))
+        try:
+            return self._schedule(eng, reqs, n_slots, packed_admission, sampling, eos)
+        finally:
+            if sampling:
+                eng.set_sampling(list(range(n_slots)), [0.0] * n_slots, [0] * n_slots, [0] * n_slots)
+
+    def _schedule(self, eng, reqs, n_slots, packed_admission, sampling, eos):
+        """The admission / decode loop of generate_requests"""
+        dev = self.device
         results = [None] * len(reqs)
         queue = collections.deque(range(len(reqs)))
         owner = [None] * n_slots            # request of each slot
@@ -665,15 +771,20 @@ class VideoChatGPTLlamaForCausalLM:
             for s in range(n_slots):
                 if owner[s] is None and queue:
                     i = queue.popleft()
-                    r = reqs[i]
-                    if not packed_admission:
-                        feats = None if r.feats is None else r.feats.to(dev)
-                        vs = torch.tensor([r.vid_start], dtype=torch.int32, device=dev)
-                        eng.slot_prefill(s, r.ids.to(dev), feats, vs, tok_out=first[s:s + 1])
                     admitted.append((s, i))
-                    owner[s], pos[s], unseen[s], gen[i] = i, r.S, True, []
+                    owner[s], pos[s], unseen[s], gen[i] = i, reqs[i].S, True, []
+            if admitted and sampling:
+                rs = [reqs[i] for _, i in admitted]
+                eng.set_sampling([s for s, _ in admitted], [r.temperature for r in rs], [r.top_k for r in rs],
+                                 [r.seed for r in rs])
             if admitted and packed_admission:
                 self._admit_packed(eng, [(s, reqs[i]) for s, i in admitted], first)
+            elif admitted:
+                for s, i in admitted:
+                    r = reqs[i]
+                    feats = None if r.feats is None else r.feats.to(dev)
+                    vs = torch.tensor([r.vid_start], dtype=torch.int32, device=dev)
+                    eng.slot_prefill(s, r.ids.to(dev), feats, vs, tok_out=first[s:s + 1])
             active = [s for s in range(n_slots) if owner[s] is not None]
             if not active:
                 return results
@@ -715,9 +826,9 @@ class VideoChatGPTLlamaForCausalLM:
                                     [r.vid_start for _, r in packed])
             first[torch.tensor(slots, device=dev)] = tok
 
-    def _request(self, i, r, max_new_tokens, stopping_criteria, n_vid):
+    def _request(self, i, r, max_new_tokens, stopping_criteria, n_vid, samp=None):
         """One request of generate_requests, checked on the host -> (ids [S] int64 on the host, S, n, feats,
-        vid_start, criteria)"""
+        vid_start, criteria, and its sampling-table entry: temperature (0: greedy), top_k, seed)"""
         if isinstance(r, torch.Tensor):
             r = {"input_ids": r}
         ids = torch.as_tensor(r["input_ids"]).detach().cpu().to(torch.int64)
@@ -737,7 +848,17 @@ class VideoChatGPTLlamaForCausalLM:
                                  f"{tuple(feats.shape)}")
             vs = self._video_spans(ids[None], n_vid)[0]
         crit = r.get("stopping_criteria", stopping_criteria)
-        return SimpleNamespace(ids=ids, S=S, n=n, feats=feats, vid_start=vs, criteria=list(crit or []))
+        samp = samp or dict(do_sample=False, temperature=1.0, top_k=50, seed=None)
+        T, k, seed = 0.0, 0, 0
+        if r.get("do_sample", samp["do_sample"]):
+            own = r.get("seed") is not None       # a seed is there (generate_requests checks it first)
+            T, k, seed = self._sampling_args(r.get("temperature", samp["temperature"]), r.get("top_k", samp["top_k"]),
+                                             r["seed"] if own else samp["seed"], f"request {i}")
+            seed = seed if own else (seed + i) % 2 ** 64
+            if T == 0:
+                k, seed = 0, 0
+        return SimpleNamespace(ids=ids, S=S, n=n, feats=feats, vid_start=vs, criteria=list(crit or []),
+                               temperature=T, top_k=k, seed=seed)
 
     @staticmethod
     def _request_done(r, gen, eos):
@@ -752,15 +873,19 @@ class VideoChatGPTLlamaForCausalLM:
         return len(gen) >= r.n
 
     def generate_continue(self, new_input_ids, do_sample=False, temperature=1.0, max_new_tokens=32,
-                          stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50):
+                          stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50, seed=None):
         """Next turn about the SAME video(s): `new_input_ids` [B, S_new] follow everything generated
         so far. Only the tokens the KV cache does not hold yet (the last generated token and the new
         text) are prefilled (vcl_llm_prefill_append); the reference re-runs the tower and the whole
         prompt every turn (chat.py:137-154). Returns the full sequence [B, S_total + n] like generate.
         After a left-padded generate the cache stays padded, so every row continues its own positions; the
-        new text of every row has the same length S_new (no padding inside a turn)."""
+        new text of every row has the same length S_new (no padding inside a turn).
+        seed: do_sample=True samples on the device as generate(seed=...) does."""
         if getattr(self, "_last_out", None) is None:
             raise ValueError("generate_continue: no previous generate() to continue")
+        seeded = do_sample and seed is not None
+        if seeded:
+            temperature, top_k, seed = self._sampling_args(temperature, top_k, seed, "generate_continue")
         eng = self._ensure_engine(need_llm=True)
         prev = self._last_out
         tail = torch.cat([prev[:, self._pos:], new_input_ids.cuda().to(torch.int64)], dim=1)
@@ -770,6 +895,14 @@ class VideoChatGPTLlamaForCausalLM:
         if n <= 0:
             raise ValueError(f"context length {ctx.shape[1]} leaves no room in max_seq {self._max_seq}")
         eos, pad = self._eos_pad(eos_token_id, pad_token_id)
+        if seeded:
+            B = ctx.shape[0]
+            clips = list(range(B))
+            with self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips]):
+                _, _, tok = eng.prefill_append(tail, start)
+                first = eng.decode_loop(tok, ctx.shape[1], min(n, self._GREEDY_CHUNK))
+                self._last_out = self._host_stops(eng, ctx, first, n, stopping_criteria, eos, pad)
+            return self._last_out
         _, logits, _ = eng.prefill_append(tail, start, want_logits=True, want_token=False)
         self._pos = ctx.shape[1]
         self._last_out = self._stepwise(eng, ctx, logits, n, do_sample, temperature, stopping_criteria, eos, pad, top_k)
