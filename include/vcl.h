@@ -36,6 +36,10 @@ extern "C" {
 #define VCL_PIXELS_BF16_NCHW 0 /* [N,3,H,W] bf16, already CLIP-normalised (inference.py:86-89)   */
 #define VCL_PIXELS_U8_NHWC 1   /* [N,H,W,3] uint8 raw frames; (x/255-mean)/std applied on device */
 
+#define VCL_WEIGHTS_BF16 0     /* the checkpoint's bf16 weights, as loaded (the default)                      */
+#define VCL_WEIGHTS_FP8_E4M3 1 /* the language model's streamed matrices as E4M3 codes with power-of-two row
+                                  scales (vcl_load_llm_weights_ex)                                            */
+
 #define VCL_PROJ_LINEAR 0     /* nn.Linear(1024, D)            video_chatgpt/model/video_chatgpt.py:51-53 */
 #define VCL_PROJ_MLP2X_GELU 1 /* Linear-GELU-Linear            model/multimodal_projector/builder.py:39-46 */
 
@@ -89,9 +93,25 @@ void vcl_destroy(vcl_handle* h);
  * (fused q|k|v, interleaved gate/up, K-padded patch-embed matrix). Unknown names are ignored
  * (e.g. vision_model.post_layernorm.*, unused by the path); a missing required name is an error.
  * vcl_load_llm_weights additionally builds a decode-only copy of the streamed matrices in the slot
- * order of the decode kernels (+1x the LLM weight bytes). */
+ * order of the decode kernels (+1x the LLM weight bytes; +0.5x with vcl_load_llm_weights_ex's fp8 format). */
 int vcl_load_clip_weights(vcl_handle* h, const vcl_tensor* tensors, int n);
 int vcl_load_llm_weights(vcl_handle* h, const vcl_tensor* tensors, int n);
+
+/* vcl_load_llm_weights with a weight format for the five streamed matrices of the language model (fused
+ * q|k|v, o_proj, interleaved gate|up, down_proj, lm_head; the embedding table, the norms, the projector and the
+ * CLIP tower stay bf16). VCL_WEIGHTS_BF16 is vcl_load_llm_weights. VCL_WEIGHTS_FP8_E4M3, per row r of each
+ * matrix W (after the fusion / interleave above):
+ *   a_r = max_k |W[r,k]|; e_r = the smallest integer with a_r <= 448 * 2^e_r (0 for an all-zero row);
+ *   q[r,k] = E4M3(W[r,k] * 2^-e_r), round to nearest even, subnormals included (torch's .to(float8_e4m3fn));
+ *   W~[r,k] = q[r,k] * 2^e_r, which is exactly a bf16 number.
+ * The load writes W~ over the row-major matrix, so prefill, decode beyond 16 clips and vcl_llm_score compute
+ * with W~, and keeps the codes (slot order of the decode kernels, one byte each) and 2^e_r per row instead of
+ * the bf16 decode copy: the decode kernels read half the bytes, and the engine holds about half the LLM weight
+ * bytes less. Every output is then bit for bit that of a VCL_WEIGHTS_BF16 engine loaded with W~. Rejected: an
+ * unknown format (before any allocation), a non-finite weight, and a row whose 2^e_r is not a normal fp32
+ * number or whose W~ is not exactly a finite bf16 (a row maximum below ~1e-36); the message names the
+ * state-dict tensor and row. */
+int vcl_load_llm_weights_ex(vcl_handle* h, const vcl_tensor* tensors, int n, int weight_format);
 
 /* vision_tower(pixel_values, output_hidden_states=True).hidden_states[k]
  * (video_chatgpt/inference.py:93-94, scripts/save_spatio_temporal_clip_features.py:116-120).
@@ -337,6 +357,15 @@ int vcl_op_decode_attention(const void* q, int64_t q_ld, const void* k, const vo
  * its own, as on the decode path) */
 int vcl_op_gemv(const void* x, const void* W, void* out, const void* res, const void* norm_w,
                 float eps, int B, int N, int K, void* stream);
+/* The load-time quantizer of VCL_WEIGHTS_FP8_E4M3 on its own, rows in order: W [N,K] bf16 (K a multiple of 32)
+ * -> w_deq [N,K] bf16 = W~ (may be W), scales [N] fp32 = 2^e_r, codes = ceil(N/16)*16*K bytes in the slot order of
+ * the decode kernels: row r, column k at (r/16)*16*K + (k/512)*8192 + (k%512/32)*512 + (r%16/8)*256 +
+ * ((r%8)*4 + k%32/8)*8 + k%8 (rows past N zero). Nothing is checked: a non-finite row gives unspecified codes. */
+int vcl_op_quantize_fp8(const void* W, int N, int K, void* w_deq, void* codes, float* scales, void* stream);
+/* vcl_op_gemv with fp8 weights: W is quantized by the quantizer above (into scratch; W is not changed) and the
+ * fp8 instances of the ring kernels run; equals vcl_op_gemv on W~ bit for bit. */
+int vcl_op_gemv_fp8(const void* x, const void* W, void* out, const void* res, const void* norm_w,
+                    float eps, int B, int N, int K, void* stream);
 
 #ifdef __cplusplus
 }

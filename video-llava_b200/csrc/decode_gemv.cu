@@ -50,6 +50,16 @@
 //   * a warp per row group (no reduction at all) keeps a slot held for ~1000 cycles by its one consumer, so
 //     only a few of the ring slots are in flight; per-row window copies make the copy engine the limit.
 //
+// Weight formats (GemvArgs): both kernels are templates over the format of the slot-ordered copy.
+//   W_BF16  the bf16 copy above.
+//   W_FP8   E4M3 codes q in the SAME order, one byte per weight (a 512-k slot is 8 KB; the ring keeps its 128 KB
+//           and holds twice as many slots), plus a power-of-two scale 2^e per row (w_scale). The consumers turn
+//           the codes into exactly the bf16 A fragments of q (e4m3x2_bf16x2), issue the same MMAs in the same k
+//           order and warp split, and multiply each row's fp32 dot product, after the cross-warp sum, by 2^e.
+//           A power-of-two factor commutes with every fp32 rounding of those sums (no under- or overflow), so the
+//           result equals the bf16 kernel's on W~ = q * 2^e bit for bit (DESIGN.md section 3). The load-time
+//           quantizer (gemv_quantize_fp8_kernel) writes W~ over the row-major matrix for every other path.
+//
 // Rounding points (reference: transformers/models/llama/modeling_llama.py:53-67 RMSNorm, :124-168 RoPE,
 // :171-184 MLP, :325,331 residuals): the normalised activation w * bf16(x * rstd) is rounded to bf16, every
 // projection is rounded to bf16 before its epilogue, and so are the RoPE products, silu(gate) and the
@@ -57,6 +67,8 @@
 // where these roundings are written down for both kernels.
 #include "common.cuh"
 #include "kernels.h"
+
+#include <cuda_fp8.h>
 
 #include <stdio.h>
 #include <stdlib.h>
@@ -89,6 +101,16 @@ constexpr int TW_SMEM = SLOTS * SLOT_BYTES + TW_XWIN * TW_XBUF + 256;
 constexpr int TW_TILE = 16 * 17;                    // floats of one partial tile (16 rows x 16 clips, padded rows)
 constexpr int TW_NG_MAX = 14;                       // row groups per CTA of the largest instance (18 would spill)
 
+// the ring of each weight format: bytes per weight, per slot, and slots in the same 128 KB
+constexpr int W_BF16 = 0, W_FP8 = 1;
+template <int FMT> struct Ring {
+  static constexpr int EB = FMT == W_FP8 ? 1 : 2;
+  static constexpr int SLOT = 16 * KC * EB;
+  static constexpr int NSLOT = SLOTS * 2 / EB;
+};
+constexpr int TW_SMEM_FP8 = SLOTS * SLOT_BYTES + TW_XWIN * TW_XBUF + 512;   // 16 + 16 + 8 barriers
+template <int FMT> constexpr int tw_smem() { return FMT == W_FP8 ? TW_SMEM_FP8 : TW_SMEM; }
+
 struct TcParams {
   GemvArgs a;                       // a.B clips (1..4) are the columns of the MMA B operand
   GemvEpilogue e;
@@ -113,6 +135,44 @@ __device__ __forceinline__ void mma_bf16(float (&c)[4], uint32_t a0, uint32_t a1
       "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
       : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
       : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+// Two E4M3 codes (bytes 0, 1 of w with SEL 0x9180, bytes 2, 3 with 0xB3A2) -> the bf16 pair of equal value, the
+// lower byte in the lower half. prmt lays out [code, sign x 8] per half; shifted by 4 and masked, the half holds
+// the code's sign, its 4-bit exponent field in the low bits of bf16's 8-bit one and its 3 mantissa bits on top
+// of bf16's 7, i.e. the bf16 number code * 2^-120 (a normal code stays normal, a subnormal one stays subnormal,
+// +-0 stays +-0). The multiplication by 2^120 is exact for every finite code (NaN codes never occur).
+template <uint32_t SEL>
+__device__ __forceinline__ uint32_t e4m3x2_bf16x2(uint32_t w) {
+  uint32_t t, r;
+  asm("prmt.b32 %0, %1, 0, %2;" : "=r"(t) : "r"(w), "n"(SEL));
+  t = (t << 4) & 0x87f087f0u;
+  asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(r) : "r"(t), "r"(0x7b807b80u));   // 0x7b80 = bf16(2^120)
+  return r;
+}
+// The A fragments of one 32-wide K block of a slot, rows g (wa) and g + 8 (wb): 8 consecutive k per lane and row
+// half, k order (0,1) (2,3) (4,5) (6,7) in .x .y .z .w
+template <int FMT>
+__device__ __forceinline__ void load_a(const uint8_t* base, int kb, int lane, uint4& wa, uint4& wb) {
+  if constexpr (FMT == W_FP8) {
+    const uint2 ca = *reinterpret_cast<const uint2*>(base + kb * 512 + lane * 8);
+    const uint2 cb = *reinterpret_cast<const uint2*>(base + kb * 512 + 256 + lane * 8);
+    wa = make_uint4(e4m3x2_bf16x2<0x9180>(ca.x), e4m3x2_bf16x2<0xB3A2>(ca.x), e4m3x2_bf16x2<0x9180>(ca.y),
+                    e4m3x2_bf16x2<0xB3A2>(ca.y));
+    wb = make_uint4(e4m3x2_bf16x2<0x9180>(cb.x), e4m3x2_bf16x2<0xB3A2>(cb.x), e4m3x2_bf16x2<0x9180>(cb.y),
+                    e4m3x2_bf16x2<0xB3A2>(cb.y));
+  } else {
+    wa = *reinterpret_cast<const uint4*>(base + kb * 1024 + lane * 16);          // row g
+    wb = *reinterpret_cast<const uint4*>(base + kb * 1024 + 512 + lane * 16);    // row g + 8
+  }
+}
+// the weight bytes of a launch and the fp32 row scale (1 for bf16 weights)
+template <int FMT> __device__ __forceinline__ const uint8_t* weight_bytes(const GemvArgs& a) {
+  if constexpr (FMT == W_FP8) return a.W_fp8;
+  else return reinterpret_cast<const uint8_t*>(a.W_tiled);
+}
+template <int FMT> __device__ __forceinline__ float row_scaled(const GemvArgs& a, int row, float v) {
+  if constexpr (FMT == W_FP8) return v * __ldg(a.w_scale + row);
+  else return v;
 }
 __device__ __forceinline__ void cbar() {            // barrier among the consumer warps only
   asm volatile("bar.sync 1, %0;" ::"r"(CONSUMERS) : "memory");
@@ -212,12 +272,14 @@ __device__ __forceinline__ long long qkv_row(int v) {
 // ---------------------------------------------------------------------------------------------
 // 1..4 clips
 // ---------------------------------------------------------------------------------------------
+template <int FMT>
 __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
+  using RG = Ring<FMT>;
   extern __shared__ __align__(128) uint8_t smem[];
   // layout: ring[n_slots] | x[nb][K] bf16 (+ norm weights [K]) | pbuf[2][CWARPS][16][4] | result[r_cap][4] fp32
   //         | red | barriers
   const int n_slots = p.n_slots;
-  bf16* xs = reinterpret_cast<bf16*>(smem + (size_t)n_slots * SLOT_BYTES);
+  bf16* xs = reinterpret_cast<bf16*>(smem + (size_t)n_slots * RG::SLOT);
   float* pbuf = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(xs) + (size_t)p.x_elems * 2);
   float* result = pbuf + 2 * CWARPS * 16 * 4;
   float* red = result + p.r_cap * 4;
@@ -225,7 +287,7 @@ __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
   const uint32_t ring0 = smem_u32(smem);
   const uint32_t bar0 = smem_u32(bars);
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
-  auto empty_bar = [&](int s) { return bar0 + 8u * (SLOTS + s); };
+  auto empty_bar = [&](int s) { return bar0 + 8u * (RG::NSLOT + s); };
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   auto trace = [&](int ev) {
@@ -254,12 +316,12 @@ __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
       const int ng = cta_row_groups(a.N, grp_begin);
       trace(5);
       for (int g = 0; g < ng; ++g) {
-        const bf16* src = a.W_tiled + (size_t)(grp_begin + g) * 16 * K;
+        const uint8_t* src = weight_bytes<FMT>(a) + (size_t)(grp_begin + g) * 16 * K * RG::EB;
         for (int kc = 0; kc < nkc; ++kc) {
-          const uint32_t bytes = (uint32_t)min(KC, K - kc * KC) * 32u;    // 16 rows x 2 B
+          const uint32_t bytes = (uint32_t)min(KC, K - kc * KC) * (16u * RG::EB);    // 16 rows
           mbar_wait(empty_bar(slot), par ^ 1u);
           mbar_arrive_expect_tx(full_bar(slot), bytes);
-          bulk_g2s(ring0 + slot * SLOT_BYTES, src + (size_t)kc * KC * 16, bytes, full_bar(slot));
+          bulk_g2s(ring0 + slot * RG::SLOT, src + (size_t)kc * KC * 16 * RG::EB, bytes, full_bar(slot));
           advance();
         }
       }
@@ -490,13 +552,13 @@ __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
     for (int kc = 0; kc < nkc; ++kc) {
       const int kb_n = min(KC, K - kc * KC) >> 5;        // 32-wide K blocks in this slot
       mbar_wait(full_bar(slot), par);
-      const uint8_t* base = smem + slot * SLOT_BYTES;
+      const uint8_t* base = smem + slot * RG::SLOT;
 #pragma unroll
       for (int t = 0; t < KC / 32 / CWARPS; ++t) {
         const int kb = warp + CWARPS * t;
         if (kb < kb_n) {
-          const uint4 wa = *reinterpret_cast<const uint4*>(base + kb * 1024 + lane * 16);        // row g
-          const uint4 wb = *reinterpret_cast<const uint4*>(base + kb * 1024 + 512 + lane * 16);  // row g+8
+          uint4 wa, wb;                                                                            // rows g, g+8
+          load_a<FMT>(base, kb, lane, wa, wb);
           uint4 xq = make_uint4(0, 0, 0, 0);
           if (g < NB) xq = *reinterpret_cast<const uint4*>(xs + (size_t)g * K + kc * KC + kb * 32 + q * 8);   // column g = clip g
           mma_bf16(c, wa.x, wb.x, wa.y, wb.y, xq.x, xq.y);
@@ -519,6 +581,10 @@ __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
       float v = 0.f;
 #pragma unroll
       for (int w = 0; w < CWARPS; ++w) v += pb[w * 64 + tid];
+      if constexpr (FMT == W_FP8) {
+        const int row = row0 + grp * 16 + (tid >> 2);
+        if (row < N) v = row_scaled<FMT>(a, row, v);
+      }
       result[grp * 64 + tid] = v;
     }
   }
@@ -578,17 +644,19 @@ __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
 // 5..16 clips. NG = upper bound of the row groups a CTA owns (the accumulator arrays are sized and
 // unrolled by it); a.x holds the activations in the xwin layout
 // ---------------------------------------------------------------------------------------------
-template <int NG>
+template <int NG, int FMT>
 __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, const GemvEpilogue e) {
+  using RG = Ring<FMT>;
   extern __shared__ __align__(128) uint8_t smem[];
-  // layout: ring[8] (after the main loop: partial tiles [warp][group]) | x windows [4][16][1088 B] | barriers
+  // layout: ring[RG::NSLOT] (128 KB; after the main loop: partial tiles [warp][group]) | x windows [4][16][1088 B]
+  //         | barriers
   uint8_t* xs = smem + SLOTS * SLOT_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(xs + TW_XWIN * TW_XBUF);
   const uint32_t ring0 = smem_u32(smem), xs0 = smem_u32(xs), bar0 = smem_u32(bars);
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
-  auto empty_bar = [&](int s) { return bar0 + 8u * (SLOTS + s); };
-  auto xfull_bar = [&](int s) { return bar0 + 8u * (2 * SLOTS + s); };
-  auto xempty_bar = [&](int s) { return bar0 + 8u * (2 * SLOTS + TW_XWIN + s); };
+  auto empty_bar = [&](int s) { return bar0 + 8u * (RG::NSLOT + s); };
+  auto xfull_bar = [&](int s) { return bar0 + 8u * (2 * RG::NSLOT + s); };
+  auto xempty_bar = [&](int s) { return bar0 + 8u * (2 * RG::NSLOT + TW_XWIN + s); };
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int K = a.K, N = a.N, NB = a.B;
@@ -597,7 +665,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
   const int ng = cta_row_groups(N, grp_begin);        // 1..NG
 
   if (tid == 0) {
-    for (int s = 0; s < SLOTS; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CWARPS); }
+    for (int s = 0; s < RG::NSLOT; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CWARPS); }
     for (int s = 0; s < TW_XWIN; ++s) { mbar_init(xfull_bar(s), 1); mbar_init(xempty_bar(s), CWARPS); }
     mbar_fence_init();
   }
@@ -613,15 +681,16 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
     // single-lane region and the uniform-datapath code around the bulk copies then faults)
     if (lane == 0) {
       const int total = ng * nkc;
-      const int pre = total < SLOTS ? total : SLOTS;
+      const int pre = total < RG::NSLOT ? total : RG::NSLOT;
+      const uint8_t* W = weight_bytes<FMT>(a);
       // the weights never depend on the previous kernel: fill the ring before the dependency wait
       {
         int kc = 0, lg = 0;
         for (int idx = 0; idx < pre; ++idx) {
-          const uint32_t bytes = (uint32_t)min(KC, K - kc * KC) * 32u;
-          const bf16* src = a.W_tiled + (size_t)(grp_begin + lg) * 16 * K + (size_t)kc * KC * 16;
+          const uint32_t bytes = (uint32_t)min(KC, K - kc * KC) * (16u * RG::EB);
+          const uint8_t* src = W + ((size_t)(grp_begin + lg) * 16 * K + (size_t)kc * KC * 16) * RG::EB;
           mbar_arrive_expect_tx(full_bar(idx), bytes);
-          bulk_g2s(ring0 + idx * SLOT_BYTES, src, bytes, full_bar(idx));
+          bulk_g2s(ring0 + idx * RG::SLOT, src, bytes, full_bar(idx));
           if (++lg == ng) { lg = 0; ++kc; }
         }
       }
@@ -635,14 +704,14 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
         bulk_g2s(xs0 + xb * TW_XBUF, a.x + (size_t)kc * NB * XWIN_PITCH, win_bytes, xfull_bar(xb));
         for (int lg = 0; lg < ng; ++lg) {
           if (idx >= pre) {
-            const uint32_t bytes = (uint32_t)min(KC, K - kc * KC) * 32u;
-            const bf16* src = a.W_tiled + (size_t)(grp_begin + lg) * 16 * K + (size_t)kc * KC * 16;
+            const uint32_t bytes = (uint32_t)min(KC, K - kc * KC) * (16u * RG::EB);
+            const uint8_t* src = W + ((size_t)(grp_begin + lg) * 16 * K + (size_t)kc * KC * 16) * RG::EB;
             mbar_wait(empty_bar(slot), (uint32_t)((use - 1) & 1));
             mbar_arrive_expect_tx(full_bar(slot), bytes);
-            bulk_g2s(ring0 + slot * SLOT_BYTES, src, bytes, full_bar(slot));
+            bulk_g2s(ring0 + slot * RG::SLOT, src, bytes, full_bar(slot));
           }
           ++idx;
-          if (++slot == SLOTS) { slot = 0; ++use; }
+          if (++slot == RG::NSLOT) { slot = 0; ++use; }
         }
       }
     }
@@ -679,13 +748,13 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
     for (int i = 0; i < NG; ++i) {
       if (i < ng) {
         mbar_wait(full_bar(slot), par);
-        const uint8_t* base = smem + slot * SLOT_BYTES;
+        const uint8_t* base = smem + slot * RG::SLOT;
 #pragma unroll
         for (int t = 0; t < 2; ++t) {
           const int kb = warp + CWARPS * t;
           if (kb < kb_n) {
-            const uint4 wa = *reinterpret_cast<const uint4*>(base + kb * 1024 + lane * 16);          // row g
-            const uint4 wb = *reinterpret_cast<const uint4*>(base + kb * 1024 + 512 + lane * 16);    // row g + 8
+            uint4 wa, wb;                                                                              // rows g, g + 8
+            load_a<FMT>(base, kb, lane, wa, wb);
 #pragma unroll
             for (int j = 0; j < 2; ++j) {
               mma_bf16(acc[i][j], wa.x, wb.x, wa.y, wb.y, xq[t][j].x, xq[t][j].y);
@@ -695,7 +764,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(empty_bar(slot));
-        if (++slot == SLOTS) { slot = 0; par ^= 1u; }
+        if (++slot == RG::NSLOT) { slot = 0; par ^= 1u; }
       }
     }
     __syncwarp();
@@ -740,7 +809,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
     for (int lg = 0; lg < ng; ++lg) {
       const int vrow = (grp_begin + lg) * 16 + rr;
       if (b < NB && vrow < N) {
-        const float v0 = tile_sum(lg, rr * 17 + b);
+        const float v0 = row_scaled<FMT>(a, vrow, tile_sum(lg, rr * 17 + b));
         if (mode == GEMV_RES) epi_residual(e, b, vrow, v0);
         else epi_logit(e, b, vrow, v0);
       }
@@ -753,7 +822,8 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
       const int rr = 2 * pr;
       const int vrow = (grp_begin + lg) * 16 + rr;
       if (b >= NB || vrow >= N) continue;
-      const float v0 = tile_sum(lg, rr * 17 + b), v1 = tile_sum(lg, (rr + 1) * 17 + b);
+      const float v0 = row_scaled<FMT>(a, vrow, tile_sum(lg, rr * 17 + b));
+      const float v1 = row_scaled<FMT>(a, vrow + 1, tile_sum(lg, (rr + 1) * 17 + b));
       if (mode == GEMV_SWIGLU) epi_swiglu(e, b, vrow, NB, v0, v1);
       else epi_qkv_rope(e, b, vrow, col, floor, v0, v1);
     }
@@ -782,20 +852,101 @@ __global__ void gemv_tc_repack_kernel(const bf16* __restrict__ W, bf16* __restri
   }
 }
 
+// Load-time E4M3 quantizer, one CTA per row v of the decode copy (source row qkv_row(v) of a q|k|v matrix, row v
+// otherwise). With a = max |W[r, :]|, e is the smallest integer with a <= 448 * 2^e (0 for an all-zero row), so
+// the row maximum lands in (224, 448]; q = E4M3(W * 2^-e), round to nearest even with subnormals (exact scaling,
+// never above 448: torch's .to(torch.float8_e4m3fn)); W~ = q * 2^e, exactly a bf16. Writes the codes in the slot
+// order of the ring kernels (the element order of gemv_tc_repack_kernel, one byte each), scales[v] = 2^e, and W~
+// into w_deq[source row] (w_deq may be W: each element is read and then written by one thread). bad (optional):
+// bad[0] = the lowest source row with a non-finite weight, bad[1] = the lowest whose 2^e is not a normal fp32
+// number or whose W~ is not exactly a finite bf16; rows that pass leave them alone.
+__global__ void __launch_bounds__(256) gemv_quantize_fp8_kernel(const bf16* W, bf16* w_deq, uint8_t* __restrict__ codes,
+                                                                 float* __restrict__ scales, int N, int K, int qkv,
+                                                                 int* bad) {
+  __shared__ float red[8];
+  const int v = blockIdx.x, tid = threadIdx.x;
+  const long long sr = qkv ? qkv_row(v) : (long long)v;
+  const bf16* src = W + sr * K;
+  const int nch = K >> 3;
+  float amax = 0.f;
+  bool finite = true;
+  for (int c = tid; c < nch; c += 256) {
+    const uint4 u = *reinterpret_cast<const uint4*>(src + c * 8);
+    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float f0 = bf16lo(w[i]), f1 = bf16hi(w[i]);
+      finite = finite && isfinite(f0) && isfinite(f1);
+      amax = fmaxf(amax, fmaxf(fabsf(f0), fabsf(f1)));
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  if ((tid & 31) == 0) red[tid >> 5] = amax;
+  finite = __syncthreads_and(finite);
+  amax = red[0];
+#pragma unroll
+  for (int w = 1; w < 8; ++w) amax = fmaxf(amax, red[w]);
+  int e = 0;
+  if (amax > 0.f) {
+    int x;
+    const float m = frexpf(amax, &x);                  // amax = m * 2^x, 0.5 <= m < 1; 448 = 0.875 * 2^9
+    e = m <= 0.875f ? x - 9 : x - 8;
+  }
+  const bool e_ok = e >= -126 && e <= 126;
+  const int ec = e_ok ? e : 0;
+  const float s = __int_as_float((ec + 127) << 23), s_inv = __int_as_float((127 - ec) << 23);
+  bool exact = e_ok;
+  uint8_t* cg = codes + (size_t)(v >> 4) * 16 * K;     // this row's 16-row group
+  const int r = v & 15, half = r >> 3, g = r & 7;
+  for (int c = tid; c < nch; c += 256) {
+    const uint4 u = *reinterpret_cast<const uint4*>(src + c * 8);
+    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+    uint32_t q[2] = {0u, 0u}, d[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float f[2] = {bf16lo(w[i]), bf16hi(w[i])};
+      float wt[2];
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const __nv_fp8_storage_t c8 = __nv_cvt_float_to_fp8(f[j] * s_inv, __NV_SATFINITE, __NV_E4M3);
+        q[i >> 1] |= (uint32_t)c8 << (8 * (2 * (i & 1) + j));
+        wt[j] = __half2float(__half(__nv_cvt_fp8_to_halfraw(c8, __NV_E4M3))) * s;
+      }
+      d[i] = pack_bf16x2(wt[0], wt[1]);
+      exact = exact && bf16lo(d[i]) == wt[0] && bf16hi(d[i]) == wt[1] && isfinite(wt[0]) && isfinite(wt[1]);
+    }
+    *reinterpret_cast<uint4*>(w_deq + sr * K + c * 8) = make_uint4(d[0], d[1], d[2], d[3]);
+    // k = 8c: K chunk kc, 32-wide block kb, lane (g, k / 8 % 4)
+    const int k = c * 8, kc = k / KC, kin = k % KC;
+    const size_t off = (size_t)kc * KC * 16 + (kin >> 5) * 512 + half * 256 + (g * 4 + ((kin >> 3) & 3)) * 8;
+    *reinterpret_cast<uint2*>(cg + off) = make_uint2(q[0], q[1]);
+  }
+  exact = __syncthreads_and(exact);
+  if (tid == 0) {
+    scales[v] = s;
+    if (bad != nullptr && !finite) atomicMin(bad, (int)sr);
+    if (bad != nullptr && finite && !exact) atomicMin(bad + 1, (int)sr);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // launch layer
 // ---------------------------------------------------------------------------------------------
-// gemv_tc shared-memory plan on `grid` CTAs; returns the slot count (0 = does not fit)
-int plan(int nb, int N, int K, bool norm, int grid, size_t* smem_bytes, int* x_elems, int* r_cap) {
+// gemv_tc shared-memory plan on `grid` CTAs; returns the slot count (0 = does not fit). fp8 weights: slots of
+// half the size, up to twice as many
+int plan(int nb, int N, int K, bool norm, int grid, size_t* smem_bytes, int* x_elems, int* r_cap, int fmt = W_BF16) {
   if (K % 32 != 0 || K > 14336) return 0;
+  const int slot_bytes = fmt == W_FP8 ? Ring<W_FP8>::SLOT : SLOT_BYTES;
+  const int max_slots = fmt == W_FP8 ? Ring<W_FP8>::NSLOT : SLOTS;
   const int xe = K * (nb + ((nb > 1 && norm) ? 1 : 0));   // x buffer: nb vectors (+ the parked norm weights when nb > 1)
   const int rmax = (((N + 15) / 16 + grid - 1) / grid) * 16;
-  const size_t fixed = (size_t)xe * 2 + (size_t)(2 * CWARPS * 16 + rmax) * 4 * 4 + 4 * CWARPS * 4 + 2 * SLOTS * 8 + 128;
+  const size_t fixed = (size_t)xe * 2 + (size_t)(2 * CWARPS * 16 + rmax) * 4 * 4 + 4 * CWARPS * 4 + 2 * max_slots * 8 + 128;
   const size_t limit = nb > 1 ? TC_SMEM_CLIPS : TC_SMEM_ONE_CLIP;
-  if (fixed + 4 * (size_t)SLOT_BYTES > limit) return 0;
-  int slots = (int)((limit - fixed) / SLOT_BYTES);
-  if (slots > SLOTS) slots = SLOTS;
-  *smem_bytes = (size_t)slots * SLOT_BYTES + fixed;
+  if (fixed + 4 * (size_t)slot_bytes > limit) return 0;
+  int slots = (int)((limit - fixed) / slot_bytes);
+  if (slots > max_slots) slots = max_slots;
+  *smem_bytes = (size_t)slots * slot_bytes + fixed;
   *x_elems = xe; *r_cap = rmax;
   return slots;
 }
@@ -819,15 +970,26 @@ constexpr int TC_TRACE_RECORDS = 512;
 unsigned long long* g_trace = nullptr;
 int g_trace_next = 0;
 
+// the weights of a launch: the bf16 slots or the fp8 codes (with their row scales), 16-byte aligned
+int weight_format(const GemvArgs& a) {
+  VCL_REQUIRE((a.W_tiled != nullptr) != (a.W_fp8 != nullptr) && (a.W_fp8 == nullptr) == (a.w_scale == nullptr),
+              "gemv: exactly one of the bf16 copy (W_tiled) or the fp8 codes with their row scales (W_fp8, w_scale)");
+  VCL_REQUIRE((uintptr_t)a.W_tiled % 16 == 0 && (uintptr_t)a.W_fp8 % 16 == 0, "gemv: weights must be 16-byte aligned");
+  return a.W_fp8 != nullptr ? W_FP8 : W_BF16;
+}
+
 int launch_tc(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
   VCL_REQUIRE(!e.out_xwin, "gemv: the 1..4-clip kernel writes row-major outputs only (out_xwin)");
-  VCL_REQUIRE(a.W_tiled != nullptr && (uintptr_t)a.W_tiled % 16 == 0 && a.ldx % 8 == 0 &&
-              (a.embed != nullptr || (uintptr_t)a.x % 16 == 0), "gemv_tc: operands must be 16-byte aligned");
+  VCL_REQUIRE(a.ldx % 8 == 0 && (a.embed != nullptr || (uintptr_t)a.x % 16 == 0),
+              "gemv_tc: operands must be 16-byte aligned");
+  const int fmt = weight_format(a);
+  if (fmt < 0) return fmt;
   TcParams p = {};
   p.a = a; p.e = e;
   const int grid = gemv_grid(a.N);
   size_t smem = 0;
-  p.n_slots = plan(a.B, a.N, a.K, a.norm_w != nullptr, grid, &smem, &p.x_elems, &p.r_cap);
+  p.n_slots = plan(a.B, a.N, a.K, a.norm_w != nullptr, grid, &smem, &p.x_elems, &p.r_cap, fmt);
+  VCL_REQUIRE(p.n_slots >= 4, "gemv_tc: B=%d N=%d K=%d does not fit the shared-memory plan", a.B, a.N, a.K);
   static const bool tracing = getenv("VCL_TC_TRACE") != nullptr;
   if (tracing) {
     const size_t rec = (size_t)device_num_sms() * 8;
@@ -840,10 +1002,16 @@ int launch_tc(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
   }
   cudaLaunchAttribute attr[1];
   cudaLaunchConfig_t cfg = pdl_config(grid, smem, stream, attr);
-  VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, gemv_tc_kernel, p));
+  VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, fmt == W_FP8 ? gemv_tc_kernel<W_FP8> : gemv_tc_kernel<W_BF16>, p));
   count_launches(1);
   return 0;
 }
+
+typedef void (*TcwKernel)(const GemvArgs, const GemvEpilogue);
+const TcwKernel tcw_bf16[4] = {gemv_tcw_kernel<2, W_BF16>, gemv_tcw_kernel<6, W_BF16>, gemv_tcw_kernel<10, W_BF16>,
+                               gemv_tcw_kernel<TW_NG_MAX, W_BF16>};
+const TcwKernel tcw_fp8[4] = {gemv_tcw_kernel<2, W_FP8>, gemv_tcw_kernel<6, W_FP8>, gemv_tcw_kernel<10, W_FP8>,
+                              gemv_tcw_kernel<TW_NG_MAX, W_FP8>};
 
 // RES / LOGITS over more than 14 row groups per SM (the lm_head): consecutive launches over near-equal
 // row slices
@@ -851,8 +1019,9 @@ int launch_tcw(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
   VCL_REQUIRE(a.norm_w == nullptr && a.embed == nullptr && a.amax_out == nullptr,
               "gemv: the 5..16-clip kernel takes normalised activations (no fused norm, embedding gather or "
               "arg-max partials)");
-  VCL_REQUIRE(a.W_tiled != nullptr && (uintptr_t)a.x % 16 == 0 && (uintptr_t)a.W_tiled % 16 == 0,
-              "gemv_tcw: operands must be 16-byte aligned");
+  VCL_REQUIRE((uintptr_t)a.x % 16 == 0, "gemv_tcw: operands must be 16-byte aligned");
+  const int fmt = weight_format(a);
+  if (fmt < 0) return fmt;
   const int groups = (a.N + 15) / 16, sms = device_num_sms();
   const int n_slices = (groups + TW_NG_MAX * sms - 1) / (TW_NG_MAX * sms);
   for (int s = 0; s < n_slices; ++s) {
@@ -860,19 +1029,22 @@ int launch_tcw(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
     const long long r0 = (long long)g0 * 16;
     GemvArgs sa = a;
     GemvEpilogue se = e;
-    sa.W_tiled = a.W_tiled + r0 * a.K;
+    if (fmt == W_FP8) {
+      sa.W_fp8 = a.W_fp8 + r0 * a.K;
+      sa.w_scale = a.w_scale + r0;
+    } else {
+      sa.W_tiled = a.W_tiled + r0 * a.K;
+    }
     sa.N = (a.N < g1 * 16 ? a.N : g1 * 16) - (int)r0;
     if (se.out != nullptr) se.out += r0;
     if (se.res != nullptr) se.res += r0;
     if (se.logits != nullptr) se.logits += r0;
     const int grid = g1 - g0 < sms ? g1 - g0 : sms;                   // no CTA without a row group
     cudaLaunchAttribute attr[1];
-    cudaLaunchConfig_t cfg = pdl_config(grid, TW_SMEM, stream, attr);
+    cudaLaunchConfig_t cfg = pdl_config(grid, fmt == W_FP8 ? tw_smem<W_FP8>() : tw_smem<W_BF16>(), stream, attr);
     const int ng_max = (g1 - g0 + grid - 1) / grid;                  // groups of the busiest CTA
-    auto kern = gemv_tcw_kernel<TW_NG_MAX>;
-    if (ng_max <= 2) kern = gemv_tcw_kernel<2>;
-    else if (ng_max <= 6) kern = gemv_tcw_kernel<6>;
-    else if (ng_max <= 10) kern = gemv_tcw_kernel<10>;
+    const int pick = ng_max <= 2 ? 0 : ng_max <= 6 ? 1 : ng_max <= 10 ? 2 : 3;
+    auto kern = fmt == W_FP8 ? tcw_fp8[pick] : tcw_bf16[pick];
     VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, sa, se));
     count_launches(1);
   }
@@ -896,9 +1068,12 @@ extern "C" int vcl_debug_tc_trace_dump(const char* path) {
 }
 
 int init_gemv_kernels() {
-  VCL_CUDA_OK(cudaFuncSetAttribute(gemv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-  for (auto k : {gemv_tcw_kernel<2>, gemv_tcw_kernel<6>, gemv_tcw_kernel<10>, gemv_tcw_kernel<TW_NG_MAX>})
-    VCL_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
+  for (auto k : {gemv_tc_kernel<W_BF16>, gemv_tc_kernel<W_FP8>})
+    VCL_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+  for (int i = 0; i < 4; ++i) {
+    VCL_CUDA_OK(cudaFuncSetAttribute(tcw_bf16[i], cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
+    VCL_CUDA_OK(cudaFuncSetAttribute(tcw_fp8[i], cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM_FP8));
+  }
   return 0;
 }
 
@@ -908,11 +1083,11 @@ int gemv_grid(int N) {
   return n_groups < sms ? n_groups : sms;
 }
 
-bool gemv_fits(int B, int N, int K, bool norm, bool pairs) {
+bool gemv_fits(int B, int N, int K, bool norm, bool pairs, bool fp8) {
   if (B < 1 || B > 16 || N < 1) return false;
   if (B > 4) return K % 32 == 0 && (!pairs || (N + 15) / 16 <= TW_NG_MAX * device_num_sms());
   size_t smem = 0; int xe = 0, rc = 0;
-  return plan(B, N, K, norm, gemv_grid(N), &smem, &xe, &rc) >= 4;
+  return plan(B, N, K, norm, gemv_grid(N), &smem, &xe, &rc, fp8 ? W_FP8 : W_BF16) >= 4;
 }
 
 size_t gemv_tiled_elems(int N, int K) { return (size_t)((N + 15) / 16) * 16 * K; }
@@ -925,10 +1100,23 @@ int launch_gemv_repack(const bf16* W, bf16* dst, int N, int K, bool qkv_pairs, c
   return 0;
 }
 
+int launch_gemv_quantize_fp8(const bf16* W, bf16* w_deq, uint8_t* codes, float* scales, int N, int K, bool qkv_pairs,
+                             int* bad, cudaStream_t stream) {
+  VCL_REQUIRE(N >= 1 && K >= 32 && K % 32 == 0, "fp8 quantizer: N=%d K=%d (K a positive multiple of 32)", N, K);
+  VCL_REQUIRE(!qkv_pairs || N % 128 == 0, "fp8 quantizer: q/k/v rows must come in heads of 128 (N=%d)", N);
+  VCL_REQUIRE((uintptr_t)W % 16 == 0 && (uintptr_t)w_deq % 16 == 0 && (uintptr_t)codes % 16 == 0,
+              "fp8 quantizer: operands must be 16-byte aligned");
+  // the rows of the last 16-row group past N stay zero
+  VCL_CUDA_OK(cudaMemsetAsync(codes, 0, gemv_tiled_elems(N, K), stream));
+  gemv_quantize_fp8_kernel<<<N, 256, 0, stream>>>(W, w_deq, codes, scales, N, K, qkv_pairs ? 1 : 0, bad);
+  VCL_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
 int launch_gemv(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
   const bool pairs = e.mode == GEMV_SWIGLU || e.mode == GEMV_QKV;
   VCL_REQUIRE(e.mode >= GEMV_RES && e.mode <= GEMV_LOGITS, "gemv: unknown epilogue mode %d", e.mode);
-  VCL_REQUIRE(gemv_fits(a.B, a.N, a.K, a.norm_w != nullptr, pairs),
+  VCL_REQUIRE(gemv_fits(a.B, a.N, a.K, a.norm_w != nullptr, pairs, a.W_fp8 != nullptr),
               "gemv: B=%d N=%d K=%d is outside the decode kernels' range (1..16 clips, K a multiple of 32; "
               "1..4 clips: K <= 14336 and the shared-memory plan; 5..16 clips: q|k|v and gate|up at most 14 "
               "row groups of 16 per SM)", a.B, a.N, a.K);

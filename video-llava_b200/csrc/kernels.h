@@ -185,14 +185,17 @@ int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, c
 // Two ring kernels (bulk-copy ring over a slot-ordered copy of the matrix + mma.sync) behind one launcher:
 // 1..4 clips stage the activation vectors in shared memory (K <= 14336, optional fused RMSNorm and, for
 // q|k|v, a fused token-embedding gather); 5..16 clips read activations that are already normalised and
-// stored window-major ("xwin", below). Both read the copy that launch_gemv_repack builds.
+// stored window-major ("xwin", below). Both read the copy that launch_gemv_repack builds, or its fp8 twin from
+// launch_gemv_quantize_fp8 (E4M3 codes in the same order plus a power-of-two scale per row; decode_gemv.cu).
 // per-CTA partial arg-max of the logits kernel: the next step's q|k|v kernel reduces the grid's
 // partials itself (lowest index wins ties), so no arg-max kernel runs between two decode steps
 struct ArgmaxPart { float v; int idx; };
 
 struct GemvArgs {
   const bf16* x = nullptr; long long ldx = 0;   // [B][ldx] (5..16 clips: xwin layout, see below)
-  const bf16* W_tiled = nullptr;                // slot-ordered copy of the [N, K] matrix
+  const bf16* W_tiled = nullptr;                // slot-ordered copy of the [N, K] matrix ...
+  const uint8_t* W_fp8 = nullptr;               // ... or its E4M3 codes in the same order (W_tiled null) with the
+  const float* w_scale = nullptr;               //     row scales 2^e_r [N]: row r is W~[r] = code * 2^e_r
   int B = 0, N = 0, K = 0;
   const bf16* norm_w = nullptr; float eps = 0;  // 1..4 clips: optional fused RMSNorm prologue
   // 1..4 clips only. q|k|v with a fused token-embedding gather: x is row `token` of `embed` [vocab, K],
@@ -240,12 +243,20 @@ int launch_xwin_norm(const bf16* x, long long ldx, bf16* y, const bf16* w, int B
 
 int init_gemv_kernels();
 // whether a [N, K] projection of B clips has a decode kernel. norm: with the fused RMSNorm (1..4 clips);
-// pairs: a SWIGLU or QKV epilogue (5..16 clips: such a matrix has at most 14 row groups of 16 per SM)
-bool gemv_fits(int B, int N, int K, bool norm, bool pairs);
+// pairs: a SWIGLU or QKV epilogue (5..16 clips: such a matrix has at most 14 row groups of 16 per SM); fp8: the
+// kernels of fp8 weights (their shared-memory plan; they take every shape the bf16 kernels take)
+bool gemv_fits(int B, int N, int K, bool norm, bool pairs, bool fp8 = false);
 int gemv_grid(int N);                         // CTAs of a 1..4-clip launch over N rows
 size_t gemv_tiled_elems(int N, int K);        // elements of the slot-ordered copy of an [N, K] matrix
 // qkv_pairs: rows are taken in the order of the fused q/k/v epilogue (RoPE pairs adjacent)
 int launch_gemv_repack(const bf16* W, bf16* dst, int N, int K, bool qkv_pairs, cudaStream_t stream);
+// The load-time E4M3 quantizer (rule: decode_gemv.cu, gemv_quantize_fp8_kernel). codes: gemv_tiled_elems(N, K)
+// bytes in the slot order of launch_gemv_repack; scales [N] fp32 (2^e per row of that order); w_deq [N, K] bf16
+// row-major receives W~ (may be W). bad (optional, device int[2], set to INT_MAX by the caller): the lowest
+// source row with a non-finite weight, and the lowest whose W~ is not exactly a finite bf16 or whose scale is
+// not a normal fp32 number.
+int launch_gemv_quantize_fp8(const bf16* W, bf16* w_deq, uint8_t* codes, float* scales, int N, int K, bool qkv_pairs,
+                             int* bad, cudaStream_t stream);
 // 1..4 clips: gemv_tc_kernel; 5..16 clips: gemv_tcw_kernel (several launches over row slices when a RES /
 // LOGITS matrix has more than 14 row groups per SM)
 int launch_gemv(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream);

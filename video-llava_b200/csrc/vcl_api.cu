@@ -44,9 +44,17 @@ namespace {
 struct ClipLayerW {
   bf16 *ln1_w, *ln1_b, *wqkv, *bqkv, *wo, *bo, *ln2_w, *ln2_b, *w1, *b1, *w2, *b2;
 };
+// The decode kernels' copy of one streamed matrix: bf16 slots, or E4M3 codes in the same order with a power-of-two
+// scale per row (VCL_WEIGHTS_FP8_E4M3; decode_gemv.cu)
+struct DecodeW {
+  bf16* t = nullptr;
+  uint8_t* q = nullptr;
+  float* s = nullptr;
+  void into(GemvArgs& g) const { g.W_tiled = t; g.W_fp8 = q; g.w_scale = s; }
+};
 struct LlmLayerW {
   bf16 *ln1, *wqkv, *wo, *ln2, *wgu, *wd;
-  bf16 *wqkv_t = nullptr, *wo_t = nullptr, *wgu_t = nullptr, *wd_t = nullptr;   // slot-ordered copies for decode
+  DecodeW qkv_d, o_d, gu_d, dn_d;   // slot-ordered copies for decode
 };
 struct GraphEntry {
   int B, n_new;        // the positions and pad counts are read on the device (h->d_pos, h->d_npad) ...
@@ -90,7 +98,8 @@ struct vcl_handle {
   bf16 *patch_w = nullptr, *cls = nullptr, *pos = nullptr, *pre_w = nullptr, *pre_b = nullptr;
   std::vector<ClipLayerW> cl;
   // LLM weights
-  bf16 *embed = nullptr, *norm_w = nullptr, *lm_head = nullptr, *lm_head_t = nullptr;
+  bf16 *embed = nullptr, *norm_w = nullptr, *lm_head = nullptr;
+  DecodeW lm_head_d;
   bf16 *proj_w0 = nullptr, *proj_b0 = nullptr, *proj_w1 = nullptr, *proj_b1 = nullptr;
   std::vector<LlmLayerW> ll;
   // CLIP activations (rows = max_frames * (P+1))
@@ -209,6 +218,73 @@ int check_device() {
 }
 
 cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
+
+#define VCL_TRY(expr)        \
+  do {                       \
+    int _rc = (expr);        \
+    if (_rc != 0) return _rc; \
+  } while (0)
+
+int op_gemv_run(GemvArgs g, void* out, const void* res, float eps, cudaStream_t st);
+
+// VCL_WEIGHTS_FP8_E4M3: every streamed matrix is quantized in place (W~ over the row-major copy, which the prefill
+// GEMMs, the decode GEMM beyond 16 clips and the scoring lm_head read) and its decode copy is the E4M3 codes with
+// one scale per row instead of the bf16 slots. The state-dict name of a failing matrix row is reported.
+int quantize_llm_fp8(vcl_handle* h) {
+  const vcl_config& c = h->cfg;
+  const int D = c.llm_hidden, F = c.llm_inter, L = c.llm_layers, n_mats = 4 * L + 1;
+  int* bad = nullptr;                                 // [n_mats][2] (see launch_gemv_quantize_fp8)
+  VCL_CUDA_OK(cudaMalloc(&bad, (size_t)n_mats * 2 * sizeof(int)));
+  VCL_CUDA_OK(cudaMemset(bad, 0x7f, (size_t)n_mats * 2 * sizeof(int)));
+  auto quant = [&](bf16* W, DecodeW& d, int N, int K, bool qkv, int idx) -> int {
+    if (dalloc(h, &d.q, gemv_tiled_elems(N, K)) || dalloc(h, &d.s, (size_t)N)) return -2;
+    return launch_gemv_quantize_fp8(W, W, d.q, d.s, N, K, qkv, bad + 2 * idx, nullptr);
+  };
+  int rc = 0;
+  for (int l = 0; l < L && rc == 0; ++l) {
+    LlmLayerW& w = h->ll[l];
+    rc = quant(w.wqkv, w.qkv_d, 3 * D, D, true, 4 * l);
+    if (rc == 0) rc = quant(w.wo, w.o_d, D, D, false, 4 * l + 1);
+    if (rc == 0) rc = quant(w.wgu, w.gu_d, 2 * F, D, false, 4 * l + 2);
+    if (rc == 0) rc = quant(w.wd, w.dn_d, D, F, false, 4 * l + 3);
+  }
+  if (rc == 0) rc = quant(h->lm_head, h->lm_head_d, c.vocab, D, false, 4 * L);
+  std::vector<int> flags((size_t)n_mats * 2);
+  cudaError_t e = cudaDeviceSynchronize();
+  if (e == cudaSuccess) e = cudaMemcpy(flags.data(), bad, flags.size() * sizeof(int), cudaMemcpyDeviceToHost);
+  cudaFree(bad);
+  if (rc != 0) return rc;
+  if (e != cudaSuccess) {
+    set_last_error("vcl_load_llm_weights: %s", cudaGetErrorString(e));
+    return -2;
+  }
+  // matrix idx, row r of its row-major (fused) layout -> the state-dict tensor and its row
+  auto name_of = [&](int idx, int r, int* row) -> std::string {
+    if (idx == 4 * L) { *row = r; return "lm_head.weight"; }
+    const std::string lp = "model.layers." + std::to_string(idx / 4) + ".";
+    switch (idx % 4) {
+      case 0: { static const char* nm[3] = {"q_proj", "k_proj", "v_proj"};
+                *row = r % D; return lp + "self_attn." + nm[r / D] + ".weight"; }
+      case 1: *row = r; return lp + "self_attn.o_proj.weight";
+      case 2: *row = r / 2; return lp + (r % 2 ? "mlp.up_proj.weight" : "mlp.gate_proj.weight");
+      default: *row = r; return lp + "mlp.down_proj.weight";
+    }
+  };
+  for (int idx = 0; idx < n_mats; ++idx) {
+    int row = 0;
+    if (flags[2 * idx] != 0x7f7f7f7f) {
+      const std::string nm = name_of(idx, flags[2 * idx], &row);
+      VCL_REQUIRE(false, "weight '%s' has a non-finite value in row %d: the fp8 weight format needs finite weights",
+                  nm.c_str(), row);
+    }
+    if (flags[2 * idx + 1] != 0x7f7f7f7f) {
+      const std::string nm = name_of(idx, flags[2 * idx + 1], &row);
+      VCL_REQUIRE(false, "weight '%s' row %d: its fp8 row scale 2^e is not a normal fp32 number or its dequantized "
+                  "values are not exact bf16 numbers (a row maximum below ~1e-36)", nm.c_str(), row);
+    }
+  }
+  return 0;
+}
 
 }  // namespace
 
@@ -375,8 +451,29 @@ int vcl_load_clip_weights(vcl_handle* h, const vcl_tensor* tensors, int n) {
 }
 
 int vcl_load_llm_weights(vcl_handle* h, const vcl_tensor* tensors, int n) {
+  return vcl_load_llm_weights_ex(h, tensors, n, VCL_WEIGHTS_BF16);
+}
+
+int vcl_load_llm_weights_ex(vcl_handle* h, const vcl_tensor* tensors, int n, int weight_format) {
+  VCL_REQUIRE(weight_format == VCL_WEIGHTS_BF16 || weight_format == VCL_WEIGHTS_FP8_E4M3,
+              "vcl_load_llm_weights: unknown weight format %d (VCL_WEIGHTS_BF16 0, VCL_WEIGHTS_FP8_E4M3 1)",
+              weight_format);
   VCL_REQUIRE(h && tensors && n > 0, "vcl_load_llm_weights: null argument");
   VCL_REQUIRE(!h->llm_loaded, "vcl_load_llm_weights: already loaded");
+  const bool fp8 = weight_format == VCL_WEIGHTS_FP8_E4M3;
+  if (fp8) {
+    // the fp8 decode kernels take every shape the bf16 ones take (vcl_create checked those)
+    const vcl_config& c = h->cfg;
+    const int D = c.llm_hidden, F = c.llm_inter;
+    const struct { const char* name; int N, K; bool norm, pairs; } mats[5] = {
+        {"q|k|v", 3 * D, D, true, true}, {"o_proj", D, D, false, false}, {"gate|up", 2 * F, D, true, true},
+        {"down_proj", D, F, false, false}, {"lm_head", c.vocab, D, true, false}};
+    for (int B = 1; B <= c.max_batch && B <= 16; ++B)
+      for (const auto& mt : mats)
+        VCL_REQUIRE(gemv_fits(B, mt.N, mt.K, mt.norm, mt.pairs, true),
+                    "vcl_load_llm_weights: the %s projection [%d x %d] has no fp8 decode kernel for %d clips", mt.name,
+                    mt.N, mt.K, B);
+  }
   TensorMap m;
   for (int i = 0; i < n; ++i)
     if (tensors[i].name) m[tensors[i].name] = &tensors[i];
@@ -427,18 +524,23 @@ int vcl_load_llm_weights(vcl_handle* h, const vcl_tensor* tensors, int n) {
                              cudaMemcpyDeviceToDevice));
     if (load_copy(h, m, lp + "mlp.down_proj.weight", &w.wd, 2, D, F)) return -1;
   }
+  if (fp8) {
+    VCL_TRY(quantize_llm_fp8(h));
+    h->llm_loaded = true;
+    return 0;
+  }
   // Decode-only second copy of every streamed matrix in the slot order of the decode kernels (one bulk
   // copy per 16 KB slot, decode_gemv.cu). 13.2 GB more for the 7B model, 25.7 GB for 13B.
-  auto tiled = [&](const bf16* src, bf16** dst, int N, int K, bool qkv) -> int {
-    if (dalloc(h, dst, gemv_tiled_elems(N, K))) return -2;
-    return launch_gemv_repack(src, *dst, N, K, qkv, nullptr);
+  auto tiled = [&](const bf16* src, DecodeW& dst, int N, int K, bool qkv) -> int {
+    if (dalloc(h, &dst.t, gemv_tiled_elems(N, K))) return -2;
+    return launch_gemv_repack(src, dst.t, N, K, qkv, nullptr);
   };
   for (int l = 0; l < c.llm_layers; ++l) {
     LlmLayerW& w = h->ll[l];
-    if (tiled(w.wqkv, &w.wqkv_t, 3 * D, D, true) || tiled(w.wo, &w.wo_t, D, D, false) ||
-        tiled(w.wgu, &w.wgu_t, 2 * F, D, false) || tiled(w.wd, &w.wd_t, D, F, false)) return -2;
+    if (tiled(w.wqkv, w.qkv_d, 3 * D, D, true) || tiled(w.wo, w.o_d, D, D, false) ||
+        tiled(w.wgu, w.gu_d, 2 * F, D, false) || tiled(w.wd, w.dn_d, D, F, false)) return -2;
   }
-  if (tiled(h->lm_head, &h->lm_head_t, V, D, false)) return -2;
+  if (tiled(h->lm_head, h->lm_head_d, V, D, false)) return -2;
   VCL_CUDA_OK(cudaDeviceSynchronize());
   h->llm_loaded = true;
   return 0;
@@ -450,12 +552,6 @@ int vcl_load_llm_weights(vcl_handle* h, const vcl_tensor* tensors, int n) {
 // launch sequences
 // ---------------------------------------------------------------------------------------------
 namespace {
-
-#define VCL_TRY(expr)        \
-  do {                       \
-    int _rc = (expr);        \
-    if (_rc != 0) return _rc; \
-  } while (0)
 
 int gemm(const bf16* A, long long lda, const bf16* W, long long ldw, bf16* C, long long ldc,
          const bf16* bias, const bf16* res, long long ldr, int M, int N, int K, int act,
@@ -509,7 +605,7 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
   const vcl_config& c = h->cfg;
   VCL_REQUIRE(!(partials_out && smp.on), "sampled rows need the logits, not the partial arg-max");
   GemvArgs g;
-  g.W_tiled = h->lm_head_t; g.N = c.vocab; g.K = c.llm_hidden;
+  h->lm_head_d.into(g); g.N = c.vocab; g.K = c.llm_hidden;
   GemvEpilogue e;
   e.mode = GEMV_LOGITS; e.ldl = c.vocab;
   if (B <= 4) {
@@ -745,7 +841,7 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
       residual.mode = GEMV_RES; residual.out = h->d_h; residual.ldo = D; residual.res = h->d_h; residual.ldr = D;
 
       GemvArgs g;
-      g.W_tiled = w.wqkv_t; g.B = B; g.N = 3 * D; g.K = D;
+      w.qkv_d.into(g); g.B = B; g.N = 3 * D; g.K = D;
       VCL_TRY(normed(g, w.ln1));
       if (fused_embed && l == 0) {
         g.x = nullptr; g.embed = h->embed; g.vocab = c.vocab; g.h_out = h->d_h;
@@ -763,16 +859,16 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
       VCL_TRY(launch_decode_attention(h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->d_attn, D, B, H, 128,
                                       c.max_seq, pos + 1, scale, st, pd, /*o_xwin=*/wide, np));
       GemvArgs go;
-      go.x = h->d_attn; go.ldx = D; go.W_tiled = w.wo_t; go.B = B; go.N = D; go.K = D;
+      go.x = h->d_attn; go.ldx = D; w.o_d.into(go); go.B = B; go.N = D; go.K = D;
       VCL_TRY(launch_gemv(go, residual, st));
       GemvArgs gg;
-      gg.W_tiled = w.wgu_t; gg.B = B; gg.N = 2 * F; gg.K = D;
+      w.gu_d.into(gg); gg.B = B; gg.N = 2 * F; gg.K = D;
       VCL_TRY(normed(gg, w.ln2));
       GemvEpilogue swiglu;
       swiglu.mode = GEMV_SWIGLU; swiglu.out = h->d_act; swiglu.ldo = F; swiglu.out_xwin = wide;
       VCL_TRY(launch_gemv(gg, swiglu, st));
       GemvArgs gd;
-      gd.x = h->d_act; gd.ldx = F; gd.W_tiled = w.wd_t; gd.B = B; gd.N = D; gd.K = F;
+      gd.x = h->d_act; gd.ldx = F; w.dn_d.into(gd); gd.B = B; gd.N = D; gd.K = F;
       VCL_TRY(launch_gemv(gd, residual, st));
     } else {
       // B > 16: tensor-core path, the B new rows ride in one (mostly empty) 128-row tile and the
@@ -1265,6 +1361,50 @@ int vcl_op_gemv(const void* x, const void* W, void* out, const void* res, const 
     c_W = W; c_N = N; c_K = K;
   }
   g.W_tiled = c_tiled;
+  return op_gemv_run(g, out, res, eps, as_stream(stream));
+}
+
+int vcl_op_quantize_fp8(const void* W, int N, int K, void* w_deq, void* codes, float* scales, void* stream) {
+  if (check_device() != 0) return -2;
+  VCL_REQUIRE(W && w_deq && codes && scales, "vcl_op_quantize_fp8: null argument");
+  return launch_gemv_quantize_fp8(reinterpret_cast<const bf16*>(W), reinterpret_cast<bf16*>(w_deq),
+                                  reinterpret_cast<uint8_t*>(codes), scales, N, K, false, nullptr, as_stream(stream));
+}
+
+int vcl_op_gemv_fp8(const void* x, const void* W, void* out, const void* res, const void* norm_w,
+                    float eps, int B, int N, int K, void* stream) {
+  if (check_device() != 0) return -2;
+  VCL_REQUIRE(B >= 1 && B <= 16, "vcl_op_gemv_fp8: B=%d outside 1..16 (more rows take the GEMM)", B);
+  VCL_REQUIRE(gemv_fits(B, N, K, norm_w != nullptr, false, true),
+              "vcl_op_gemv_fp8: B=%d N=%d K=%d is outside the decode kernels' range", B, N, K);
+  static bool inited = false;
+  if (!inited) {
+    VCL_TRY(init_gemv_kernels());
+    inited = true;
+  }
+  // the load-time quantizer into stream-ordered scratch (W itself is left as it is), then the fp8 ring kernels
+  cudaStream_t st = as_stream(stream);
+  unsigned char* scratch = nullptr;
+  const size_t deq = (size_t)N * K * sizeof(bf16), cb = (gemv_tiled_elems(N, K) + 255) / 256 * 256;
+  VCL_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&scratch), deq + cb + (size_t)N * sizeof(float), st));
+  GemvArgs g;
+  g.x = reinterpret_cast<const bf16*>(x); g.ldx = K;
+  g.B = B; g.N = N; g.K = K; g.norm_w = reinterpret_cast<const bf16*>(norm_w); g.eps = eps;
+  g.W_fp8 = scratch + deq; g.w_scale = reinterpret_cast<float*>(scratch + deq + cb);
+  int rc = launch_gemv_quantize_fp8(reinterpret_cast<const bf16*>(W), reinterpret_cast<bf16*>(scratch),
+                                    scratch + deq, reinterpret_cast<float*>(scratch + deq + cb), N, K, false, nullptr, st);
+  if (rc == 0) rc = op_gemv_run(g, out, res, eps, st);
+  VCL_CUDA_OK(cudaFreeAsync(scratch, st));
+  return rc;
+}
+
+}  // extern "C"
+
+namespace {
+
+// out = x . W^T (+ res) by the decode kernels, with g's weights; 5..16 rows through the xwin re-layout
+int op_gemv_run(GemvArgs g, void* out, const void* res, float eps, cudaStream_t st) {
+  const int B = g.B, N = g.N, K = g.K;
   GemvEpilogue e;
   e.mode = GEMV_RES; e.out = reinterpret_cast<bf16*>(out); e.ldo = N; e.res = reinterpret_cast<const bf16*>(res); e.ldr = N;
   if (B >= 5) {
@@ -1272,16 +1412,20 @@ int vcl_op_gemv(const void* x, const void* W, void* out, const void* res, const 
     // as on the decode path
     static bf16* xn = nullptr; static size_t xn_elems = 0;
     if (xn_elems < xwin_elems(B, K)) {
-      cudaStreamSynchronize(as_stream(stream));
+      cudaStreamSynchronize(st);
       if (xn) cudaFree(xn);
       VCL_CUDA_OK(cudaMalloc(&xn, xwin_elems(B, K) * sizeof(bf16)));
       xn_elems = xwin_elems(B, K);
     }
-    VCL_TRY(launch_xwin_norm(g.x, K, xn, g.norm_w, B, K, eps, as_stream(stream)));
+    VCL_TRY(launch_xwin_norm(g.x, K, xn, g.norm_w, B, K, eps, st));
     g.x = xn; g.norm_w = nullptr;
   }
-  return launch_gemv(g, e, as_stream(stream));
+  return launch_gemv(g, e, st);
 }
+
+}  // namespace
+
+extern "C" {
 
 int vcl_op_decode_attention(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int B, int H,
                             int s_max, int kv_len, const int32_t* pos_dev, const int32_t* n_pad, float scale,

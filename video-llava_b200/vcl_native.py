@@ -20,6 +20,15 @@ PIXELS_BF16_NCHW, PIXELS_U8_NHWC = 0, 1
 PROJ_LINEAR, PROJ_MLP2X_GELU = 0, 1
 NO_VIDEO = -2 ** 31          # vid_start value of a text-only row (VCL_NO_VIDEO)
 ACT_NONE, ACT_QGELU, ACT_GELU, ACT_SWIGLU = 0, 1, 2, 3
+WEIGHTS_BF16, WEIGHTS_FP8_E4M3 = 0, 1
+WEIGHT_FORMATS = {"bf16": WEIGHTS_BF16, "fp8_e4m3": WEIGHTS_FP8_E4M3}   # the language model's weight formats
+
+
+def weight_format_code(name) -> int:
+    """"bf16" | "fp8_e4m3" -> VCL_WEIGHTS_*; anything else raises ValueError."""
+    if not isinstance(name, str) or name not in WEIGHT_FORMATS:
+        raise ValueError(f"unknown LLM weight format {name!r}: one of {sorted(WEIGHT_FORMATS)}")
+    return WEIGHT_FORMATS[name]
 
 
 class VclError(RuntimeError):
@@ -50,6 +59,7 @@ _SIGNATURES = {
     "vcl_destroy": (None, [c_void_p]),
     "vcl_load_clip_weights": (c_int, [c_void_p, POINTER(vcl_tensor), c_int]),
     "vcl_load_llm_weights": (c_int, [c_void_p, POINTER(vcl_tensor), c_int]),
+    "vcl_load_llm_weights_ex": (c_int, [c_void_p, POINTER(vcl_tensor), c_int, c_int]),
     "vcl_clip_encode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "vcl_st_pool": (c_int, [c_void_p, c_int, c_int64, c_int64, c_int, c_int, c_int, c_int, c_void_p,
                             c_int, c_void_p]),
@@ -92,6 +102,9 @@ _SIGNATURES = {
     "vcl_op_attention_vit": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "vcl_op_gemv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int,
                             c_int, c_void_p]),
+    "vcl_op_gemv_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int,
+                                c_int, c_void_p]),
+    "vcl_op_quantize_fp8": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
@@ -236,6 +249,32 @@ def op_gemv(x, w, res=None, norm_w=None, eps=0.0):
     return out
 
 
+def op_gemv_fp8(x, w, res=None, norm_w=None, eps=0.0):
+    """op_gemv with w quantized to E4M3 by the load-time quantizer and the fp8 ring kernels (vcl_op_gemv_fp8);
+    equals op_gemv(x, W~) bit for bit, W~ = op_quantize_fp8(w)[0]."""
+    B, K = x.shape
+    N = w.shape[0]
+    out = torch.empty(B, N, dtype=torch.bfloat16, device=x.device)
+    check(lib().vcl_op_gemv_fp8(ptr(x), ptr(w), ptr(out), ptr(res), ptr(norm_w), eps, B, N, K, cur_stream()))
+    return out
+
+
+def tiled_elems(N, K):
+    """elements (bytes for fp8) of the slot-ordered decode copy of an [N, K] matrix"""
+    return (N + 15) // 16 * 16 * K
+
+
+def op_quantize_fp8(w):
+    """The load-time E4M3 quantizer alone (vcl_op_quantize_fp8), rows in order: w [N, K] bf16 ->
+    (W~ [N, K] bf16, codes uint8 [tiled_elems(N, K)] in the decode kernels' slot order, scales [N] fp32 = 2^e)."""
+    N, K = w.shape
+    deq = torch.empty_like(w)
+    codes = torch.empty(tiled_elems(N, K), dtype=torch.uint8, device=w.device)
+    scales = torch.empty(N, dtype=torch.float32, device=w.device)
+    check(lib().vcl_op_quantize_fp8(ptr(w), N, K, ptr(deq), ptr(codes), ptr(scales), cur_stream()))
+    return deq, codes, scales
+
+
 XWIN_KC, XWIN_PITCH = 512, 544     # kernels.h: the window-major activation layout of the 5..16-clip decode kernels
 
 
@@ -319,11 +358,18 @@ class Engine:
         torch.cuda.synchronize()
         check(lib().vcl_load_clip_weights(self._h, arr, len(state)))
 
-    def load_llm(self, state: dict):
+    def load_llm(self, state: dict, weight_format: str = "bf16"):
+        """weight_format "bf16" (vcl_load_llm_weights) or "fp8_e4m3" (vcl_load_llm_weights_ex: the streamed
+        matrices as E4M3 codes with power-of-two row scales; the engine then computes with the dequantized
+        weights W~). Any other value raises ValueError before anything is loaded."""
+        fmt = weight_format_code(weight_format)
         keep: list = []
         arr = _tensor_array(state, keep)
         torch.cuda.synchronize()
-        check(lib().vcl_load_llm_weights(self._h, arr, len(state)))
+        if fmt == WEIGHTS_BF16:
+            check(lib().vcl_load_llm_weights(self._h, arr, len(state)))
+        else:
+            check(lib().vcl_load_llm_weights_ex(self._h, arr, len(state), fmt))
 
     # ---- vision ----
     @staticmethod

@@ -298,7 +298,12 @@ class VideoChatGPTLlamaForCausalLM:
     config_class = VideoChatGPTConfig
 
     def __init__(self, config: VideoChatGPTConfig, clip_config=None, max_batch: int = 1, max_seq: int | None = None,
-                 clip_run_layers: int | None = None):
+                 clip_run_layers: int | None = None, llm_weight_format: str = "bf16"):
+        """llm_weight_format: "bf16", or "fp8_e4m3" to hold the language model's streamed matrices as E4M3 codes
+        with power-of-two row scales (vcl_load_llm_weights_ex): decode reads half the weight bytes, and every
+        output is that of the bf16 engine on the dequantized weights."""
+        vn.weight_format_code(llm_weight_format)          # ValueError before anything else
+        self._llm_weight_format = llm_weight_format
         self.config = config
         self.clip_config = _clip_config(clip_config if clip_config is not None
                                         else getattr(config, "mm_vision_tower", None))
@@ -408,7 +413,7 @@ class VideoChatGPTLlamaForCausalLM:
             self._engine.load_clip(self._clip_state)
             self._clip_state, self._clip_loaded = None, True
         if need_llm and not self._llm_loaded:
-            self._engine.load_llm(self._state)
+            self._engine.load_llm(self._state, weight_format=self._llm_weight_format)
             self._llm_loaded = True
         return self._engine
 
