@@ -70,6 +70,9 @@ typedef struct vcl_config {
   int32_t max_frames;    /* frames per vcl_clip_encode call */
   int32_t max_batch;     /* clips per prefill / decode call */
   int32_t max_seq;       /* prompt + generated tokens per clip */
+  int32_t max_slots;     /* in-flight cache slots (vcl_llm_slot_*): 0 = min(max_batch, 16); otherwise
+                            1 .. min(max_batch, 64), anything else is rejected by vcl_create. A capacity
+                            only: the decode kernel is chosen by the clip count of each call */
 } vcl_config;
 
 /* A named tensor in the layout of the HF/reference state_dict (row-major, bf16, on the device).
@@ -223,11 +226,12 @@ int vcl_llm_generate_padded(vcl_handle* h, const int64_t* ids, const void* video
 
 /* In-flight (continuous) batching: every clip of the KV cache is a SLOT that holds its own sequence at its own
  * length, so a finished request's slot takes the next queued request while the other slots keep decoding.
- * There are min(max_batch, 16) slots (the decode ring kernels take up to 16 clips per launch). Slots are
- * unpadded.
+ * There are max_slots slots (vcl_config; 0 means min(max_batch, 16), at most min(max_batch, 64)). Slots are
+ * unpadded. Decode projections by clip count: 1..4 gemv_tc, 5..16 gemv_tcw, 17..64 gemv_tcx (the ring kernels of
+ * decode_gemv.cu, each streaming every weight byte once per step), more than 64 the prefill GEMM.
  *
  * vcl_llm_slot_prefill: vcl_llm_prefill of ONE prompt (ids [1,S], video_feats [1, n_temporal+P, 1024] or NULL,
- * vid_start [1]) into cache slot `slot` (0 <= slot < min(max_batch, 16)). The slot then holds positions
+ * vid_start [1]) into cache slot `slot` (0 <= slot < max_slots). The slot then holds positions
  * 0 .. S-1; no other slot's cache columns are read or written. next_tok [1] int32: the arg-max at the last
  * position. Like vcl_llm_prefill it clears the cache's left padding (vcl_llm_prefill_padded): the other slots
  * must be (re)started with vcl_llm_slot_prefill before they are decoded. */
@@ -241,12 +245,12 @@ int vcl_llm_slot_prefill(vcl_handle* h, int slot, const int64_t* ids, const void
  * is text only and its feature rows are ignored). Every prompt comes out exactly as vcl_llm_slot_prefill of that
  * prompt alone leaves it: the same cache bits in its slot (columns 0 .. S_i-1) and the same first token
  * next_tok[i]. No other cache column is read or written. Like vcl_llm_slot_prefill it clears the cache's left
- * padding. Rejected before any device work, the handle and cache untouched: n outside 1 .. min(max_batch, 16),
- * a slot outside 0 .. min(max_batch, 16)-1 or given twice, S_i outside 1 .. min(512, max_seq) (512: the key limit
+ * padding. Rejected before any device work, the handle and cache untouched: n outside 1 .. max_slots,
+ * a slot outside 0 .. max_slots-1 or given twice, S_i outside 1 .. min(512, max_seq) (512: the key limit
  * of the prefill attention kernel). So sum S_i never exceeds the activations (max_batch * max_seq rows). The call always
  * runs the q|k|v GEMM's fused RoPE / cache-write epilogue and the wgmma prefill attention, whatever
  * VCL_PREFILL_ROPE_SEPARATE and VCL_PREFILL_ATTN_FLASH say (those switch the other prefill entry points only).
- * Its launches do not depend on n beyond the choice of decode kernel for the lm_head (1..4 or 5..16 rows); the
+ * Its launches do not depend on n beyond the choice of decode kernel for the lm_head (1..4, 5..16 or 17..64 rows); the
  * row layout reaches the kernels through one host-to-device copy into a device map of the handle. */
 int vcl_llm_slots_prefill(vcl_handle* h, int n, const int32_t* slots_host, const int32_t* seq_len_host,
                           const int64_t* ids, const void* video_feats, const int32_t* vid_start,
@@ -258,8 +262,8 @@ int vcl_llm_slots_prefill(vcl_handle* h, int n, const int32_t* slots_host, const
  * (checked before any device work). A slot without a request is computed like any other; its tokens are
  * meaningless and it writes only its own cache columns (park it at position 0). The positions are copied to
  * a device array of the handle at a fixed address, so one CUDA graph per (n_slots, n_new) serves every set of
- * positions; it is the graph vcl_llm_decode_loop uses for (B = n_slots, n_new). 1 <= n_slots <= min(max_batch,
- * 16); a left-padded cache is rejected. */
+ * positions; it is the graph vcl_llm_decode_loop uses for (B = n_slots, n_new). 1 <= n_slots <= max_slots;
+ * a left-padded cache is rejected. */
 int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* pos_host, int n_slots, int n_new,
                         int32_t* out_tokens, void* stream);
 

@@ -1,6 +1,6 @@
 """bf16 against fp8 (E4M3) LLM weights (H100; prints one JSON line).
 
-    python tools/bench_fp8.py [--rounds 10] [--skip-13b]
+    python tools/bench_fp8.py [--rounds 10] [--skip-13b] [--batches 1,4,16] [--decode-only --formats bf16]
 
 (a) 7B decode: Vicuna-7B shapes with random bf16 weights (bench.py's), prompts of S = 448 with video, the CUDA-graph
     decode loop of 31 steps (vcl_llm_decode_loop, 32 tokens) at B = 1, 4 and 16 clips. The bf16 and the fp8 engine
@@ -13,10 +13,16 @@
     are random: this says nothing about answer quality on a trained checkpoint.
 (d) 13B (one engine at a time): resident memory of the bf16 and the fp8 engine (free device memory before and
     after creating and loading it), and the fp8 decode at B = 4.
+--batches: the clip counts of (a); above 16 they run the 17..64-clip ring kernel. --decode-only runs (a) alone, with
+the engines of --formats (one engine each; a 7B engine sized for 64 clips holds 16 GB of KV cache, so at 64 clips
+run one format per call). --compare-lib PATH (with --decode-only) also creates, for every format, an engine from another
+build of libvcl.so (e.g. the parent commit's, built side by side) and alternates the two call by call; --layers N
+shortens the model so that both engines fit on one card (the ratio of the two is what this compares).
 The card's name and power limit are printed with the numbers.
 """
 import argparse
 import gc
+import importlib.util
 import json
 import os
 import statistics
@@ -37,9 +43,18 @@ from bench_padded import card  # noqa: E402
 S, N_NEW, N_VID = 448, 32, 356
 
 
-def engine(model, fmt, max_batch=16, llm=None):
+def other_binding(lib_path):
+    """a second instance of the vcl_native module bound to another libvcl.so (same C ABI)"""
+    spec = importlib.util.spec_from_file_location("vcl_native_other", vn.__file__)
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    mod.LIB_PATH = os.path.abspath(lib_path)
+    return mod
+
+
+def engine(model, fmt, max_batch=16, llm=None, binding=None):
     m = bench.MODELS[model]
-    c = vn.vcl_config()
+    c = (binding or vn).vcl_config()
     c.clip_layers, c.clip_hidden, c.clip_inter, c.clip_heads = 0, 1024, 4096, 16
     c.image_size, c.patch_size, c.clip_ln_eps = 224, 14, 1e-5
     c.llm_layers, c.llm_hidden, c.llm_inter, c.llm_heads = m["layers"], m["hidden"], m["inter"], m["heads"]
@@ -47,7 +62,7 @@ def engine(model, fmt, max_batch=16, llm=None):
     c.proj_type, c.n_temporal = vn.PROJ_LINEAR, 100
     c.max_frames, c.max_batch, c.max_seq = 1, max_batch, S + N_NEW
     free0 = torch.cuda.mem_get_info()[0]
-    eng = vn.Engine(c)
+    eng = (binding or vn).Engine(c)
     own = llm is None
     if own:
         _, llm = bench.device_weights(model, "cuda")
@@ -87,7 +102,7 @@ def time_ms(fn, st):
     return a.elapsed_time(b)
 
 
-def decode_arm(engines, B, rounds, st, model="7b"):
+def decode_arm(engines, B, rounds, st, model="7b", fmts=None):
     ids, vf, vs = prompts(B)
     firsts = {}
     with torch.cuda.stream(st):
@@ -104,7 +119,9 @@ def decode_arm(engines, B, rounds, st, model="7b"):
     out = {}
     for k in engines:
         ms = statistics.median(times[k])
-        out[k] = dict(ms_per_step=round(ms, 3), gb_s=round((streamed_bytes(model, k) + kv) / ms / 1e6, 1))
+        fmt = fmts[k] if fmts else k
+        out[k] = dict(ms_per_step=round(ms, 3), gb_s=round((streamed_bytes(model, fmt) + kv) / ms / 1e6, 1),
+                      spread_ms=[round(min(times[k]), 3), round(max(times[k]), 3)])
     return out
 
 
@@ -112,32 +129,66 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rounds", type=int, default=10)
     ap.add_argument("--skip-13b", action="store_true")
+    ap.add_argument("--batches", default="1,4,16")
+    ap.add_argument("--decode-only", action="store_true")
+    ap.add_argument("--formats", default="bf16,fp8_e4m3")
+    ap.add_argument("--compare-lib", default=None)
+    ap.add_argument("--layers", type=int, default=None)
     args = ap.parse_args()
+    if args.layers is not None:
+        bench.MODELS["7b"] = dict(bench.MODELS["7b"], layers=args.layers)
+    batches = [int(b) for b in args.batches.split(",")]
+    formats = args.formats.split(",")
     name, power = card()
     print(f"[bench_fp8] {name}, power limit {power}")
     st = torch.cuda.Stream()
     res = {"card": name, "power_limit": power}
 
     _, llm = bench.device_weights("7b", "cuda")
+    if args.compare_lib:
+        other = other_binding(args.compare_lib)
+        res["layers"] = bench.MODELS["7b"]["layers"]
+        res["7b_decode_vs_other_lib"] = {}
+        for fmt in formats:
+            engines = {}
+            engines["this"] = engine("7b", fmt, max_batch=max(batches + [16]), llm=llm)[0]
+            engines["other"] = engine("7b", fmt, max_batch=max(batches + [16]), llm=llm, binding=other)[0]
+            for B in batches:
+                r = decode_arm(engines, B, args.rounds, st, fmts={"this": fmt, "other": fmt})
+                r["speedup"] = round(r["other"]["ms_per_step"] / r["this"]["ms_per_step"], 3)
+                res["7b_decode_vs_other_lib"][f"{fmt}_B{B}"] = r
+                print(f"[bench_fp8] {fmt} B={B}: {r}", flush=True)
+            for e in engines.values():
+                e.close()
+            del engines
+            gc.collect()
+            torch.cuda.empty_cache()
+        print(json.dumps(res))
+        return
     errs = []
     for k, v in llm.items():
         if k == "lm_head.weight" or (k.startswith("model.layers.") and k.endswith("_proj.weight")):
             d = R.dequantized(v)
             errs.append(((d.float() - v.float()).norm() ** 2).item() / (v.float().norm() ** 2).item())
     res["w_tilde_rel_err"] = round(statistics.mean(errs) ** 0.5, 4)
-    eb, mem_b = engine("7b", "bf16", llm=llm)
-    e8, mem_8 = engine("7b", "fp8_e4m3", llm=llm)
+    engines, mems = {}, {}
+    for fmt in formats:
+        engines[fmt], mems[fmt] = engine("7b", fmt, max_batch=max(batches + [16]), llm=llm)
     del llm
     gc.collect()
     torch.cuda.empty_cache()
-    engines = {"bf16": eb, "fp8_e4m3": e8}
-    res["7b_resident_gib"] = {"bf16": round(mem_b / 2 ** 30, 2), "fp8_e4m3": round(mem_8 / 2 ** 30, 2)}
+    res["7b_resident_gib"] = {k: round(v / 2 ** 30, 2) for k, v in mems.items()}
     res["7b_decode"] = {}
-    for B in (1, 4, 16):
+    for B in batches:
         r = decode_arm(engines, B, args.rounds, st)
-        r["speedup"] = round(r["bf16"]["ms_per_step"] / r["fp8_e4m3"]["ms_per_step"], 3)
+        if len(engines) == 2:
+            r["speedup"] = round(r["bf16"]["ms_per_step"] / r["fp8_e4m3"]["ms_per_step"], 3)
         res["7b_decode"][f"B{B}"] = r
         print(f"[bench_fp8] 7B decode B={B}: {r}")
+    if args.decode_only:
+        print(json.dumps(res))
+        return
+    eb, e8 = engines["bf16"], engines["fp8_e4m3"]
 
     # (b) one clip through the language model
     ids, vf, vs = prompts(1, seed=7)

@@ -2,8 +2,11 @@
 
     python tools/bench_inflight.py [--requests 64] [--min-new 16] [--max-new 384] [--slots 4,8,16]
                                    [--chunks 16] [--repeats 2] [--no-static] [--no-alone] [--out DIR]
+                                   [--llm-weight-format {bf16,fp8_e4m3}]
     python tools/bench_inflight.py --prefill-cost [--ks 1,2,4,8,16] [--iters 10] [--out DIR]
 
+More than 16 slots set max_slots on the engine (one slot per clip of max_batch = the largest slot count); the
+engine's resident memory (free device memory before and after creating and loading it) is reported.
 Vicuna-7B shapes with random-init bf16 weights (bench.device_weights, seed 0), random pooled video features, and
 prompts of 400..448 tokens (bench.synthetic_prompt_ids with a shorter text before the video). Random weights never
 produce a real EOS, so each request's seeded max_new_tokens (uniform over --min-new .. --max-new) stands in for
@@ -50,20 +53,28 @@ from video_chatgpt.model import VideoChatGPTConfig, VideoChatGPTLlamaForCausalLM
 S_MAX, N_VID = 448, 356
 
 
-def make_model(max_batch, max_seq):
+def make_model(max_batch, max_seq, weight_format="bf16"):
+    """the engine has max_batch cache slots (max_slots above 16); returns (model, engine, resident bytes: free device
+    memory before creating the engine minus after loading it)"""
     m = bench.MODELS["7b"]
     cfg = VideoChatGPTConfig(hidden_size=m["hidden"], intermediate_size=m["inter"], num_hidden_layers=m["layers"],
                              num_attention_heads=m["heads"], vocab_size=32003, use_mm_proj=True, mm_hidden_size=1024)
-    model = VideoChatGPTLlamaForCausalLM(cfg, clip_config={}, max_batch=max_batch, max_seq=max_seq)
+    model = VideoChatGPTLlamaForCausalLM(cfg, clip_config={}, max_batch=max_batch, max_seq=max_seq,
+                                         max_slots=max_batch if max_batch > 16 else None,
+                                         llm_weight_format=weight_format)
     vc = model.get_model().vision_config
     vc.vid_patch_token, vc.vid_start_token, vc.vid_end_token, vc.use_vid_start_end = 32000, 32001, 32002, True
     _, llm = bench.device_weights("7b", "cuda")
     model.load_state_dict(llm)
+    torch.cuda.synchronize()
+    free0 = torch.cuda.mem_get_info()[0]
     eng = model._ensure_engine(need_llm=True)
+    torch.cuda.synchronize()
+    resident = free0 - torch.cuda.mem_get_info()[0]
     model._state = {}
     del llm
     torch.cuda.empty_cache()
-    return model, eng
+    return model, eng, resident
 
 
 def make_requests(n, min_new, max_new, min_len=400):
@@ -198,6 +209,7 @@ def main():
     ap.add_argument("--ks", default="1,2,4,8,16")
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--out", default=None, help="also write the JSON line to DIR/bench_inflight.json")
+    ap.add_argument("--llm-weight-format", default="bf16", choices=["bf16", "fp8_e4m3"])
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_inflight.py needs an H100 (no CPU measurement)")
@@ -207,7 +219,7 @@ def main():
     chunks = [int(c) for c in a.chunks.split(",")] if a.chunks else [default_chunk]
     if a.prefill_cost:
         ks = [int(k) for k in a.ks.split(",")]
-        model, eng = make_model(max(ks), S_MAX + a.max_new)
+        model, eng, _ = make_model(max(ks), S_MAX + a.max_new, a.llm_weight_format)
         reqs = make_requests(max(ks), a.min_new, a.max_new)
         st = torch.cuda.Stream()
         with torch.cuda.stream(st):
@@ -223,7 +235,7 @@ def main():
             with open(os.path.join(a.out, "bench_prefill_cost.json"), "w") as f:
                 f.write(line + "\n")
         return
-    model, eng = make_model(max(slot_counts), S_MAX + a.max_new)
+    model, eng, resident = make_model(max(slot_counts), S_MAX + a.max_new, a.llm_weight_format)
     reqs = make_requests(a.requests, a.min_new, a.max_new)
     n_tokens = sum(r["max_new_tokens"] for r in reqs)
     # admissions: device time of every slot prefill of the in-flight arm
@@ -253,7 +265,8 @@ def main():
     st = torch.cuda.Stream()          # decode loops are captured into CUDA graphs on a non-default stream
     res = {"what": f"{a.requests} requests, prompts 400..{S_MAX} tokens with video, max_new_tokens uniform "
                    f"{a.min_new}..{a.max_new} ({n_tokens} tokens), Vicuna-7B shapes, random bf16 weights",
-           "card": name, "power_limit": power, "repeats": a.repeats, "arms": {}}
+           "card": name, "power_limit": power, "repeats": a.repeats, "llm_weight_format": a.llm_weight_format,
+           "resident_gib": round(resident / 2 ** 30, 2), "max_seq": S_MAX + a.max_new, "arms": {}}
     tokens = {}
     with torch.cuda.stream(st):
         for slots in slot_counts:

@@ -95,7 +95,7 @@ def main():
         res["kernel_us"][B] = {"us": round(us, 2), "GB_per_s": round(4 * 32003 * B / us / 1e3, 1)}
     print("[bench_sampling] (c)", res["kernel_us"], flush=True)
 
-    model, eng = make_model(16, S_MAX + 400)
+    model, eng, _ = make_model(16, S_MAX + 400)
     ids = O.make_prompt_ids(O.LlmCfg(), 356, seed=1).cuda()
     feats = (torch.randn(1, 356, 1024, generator=torch.Generator().manual_seed(2)) * 0.5).half().cuda()
     st = torch.cuda.Stream()

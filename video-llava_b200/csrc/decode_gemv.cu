@@ -1,7 +1,8 @@
-// Decode projections for 1..16 clips: out[b][n] = x[b] . W[n, :], one kernel per weight matrix, the weights
-// streamed ONCE per launch. Two kernels share the streaming machinery and the epilogues:
+// Decode projections for 1..64 clips: out[b][n] = x[b] . W[n, :], one kernel per weight matrix, the weights
+// streamed ONCE per launch. Three kernels share the streaming machinery and the epilogues:
 //   gemv_tc_kernel        1..4 clips, the activation vectors staged in shared memory
 //   gemv_tcw_kernel<NG>   5..16 clips, the activations streamed window by window next to the weights
+//   gemv_tcx_kernel       17..64 clips, gemv_tcw with the clips split across the consumer warps as well as K
 //
 // What bounds these kernels is how much of the time HBM is kept streaming:
 //   * a chain of per-matrix kernels keeps HBM busier with programmatic dependent launch (the next
@@ -830,6 +831,218 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// 17..64 clips: gemv_tcw_kernel with the clips split across the consumer warps as well as K. The 8 consumer
+// warps are CG clip groups of 16 (clip group cg = columns 16 cg .. 16 cg + 15 of the MMA B operand) x KP = 8 / CG
+// K phases (warp kp of a group takes the 32-wide K blocks kp, kp + KP, ...): CG = 2 for 17..32 clips, 4 for
+// 33..64. Each warp keeps the accumulators of its 16 clips for all NG row groups (the register budget of
+// gemv_tcw<NG>) and the B fragments of its K blocks (TPW x 8 registers) for the whole chunk; an A fragment is
+// loaded by CG warps. A 9-warp kernel has at most 168 registers per thread (3 warps share a sub-partition's
+// 16K), so the largest instance without spills is NG = 10 at CG = 2 and NG = 6 at CG = 4.
+// The same producer, slot-ordered weight copy, xwin windows (now of up to 64 clips) and epilogues as gemv_tcw.
+// Shared memory: an 80 KB ring (5 bf16 / 10 fp8 slots) and 136 KB of windows (4 of 32 clips or 2 of 64); the
+// KP partial tiles [kp][group][16][16 CG + 1] fp32 meet in the idle ring + window memory at the end (at most
+// 84 KB). Every matrix runs in row slices of at most NG groups per CTA; r0 is the slice's first row
+// (the weights and row scales of `a` start there, the epilogue addresses rows r0 + local row).
+// ---------------------------------------------------------------------------------------------
+constexpr int TX_RING = 5 * SLOT_BYTES;
+constexpr int TX_XAREA = 8 * 16 * TW_XROW;
+constexpr int TX_SMEM = TX_RING + TX_XAREA + 512;   // + barriers (at most 2 x 10 slots + 2 x 4 windows)
+template <int FMT> struct RingX {
+  static constexpr int EB = FMT == W_FP8 ? 1 : 2;
+  static constexpr int SLOT = 16 * KC * EB;
+  static constexpr int NSLOT = TX_RING / SLOT;
+};
+
+template <int NG, int CG, int FMT>
+__global__ void __launch_bounds__(THREADS, 1) gemv_tcx_kernel(const GemvArgs a, const GemvEpilogue e, const int r0) {
+  using RG = RingX<FMT>;
+  constexpr int KP = CWARPS / CG;                     // K phases
+  constexpr int TPW = KC / 32 / KP;                   // 32-wide K blocks per warp and slot
+  constexpr int NWIN = 8 / CG;                        // activation windows in flight (power of two)
+  constexpr int XBUF = 16 * CG * TW_XROW;             // one window of 16 CG clips
+  constexpr int TP = 16 * CG + 1;                     // floats per row of a partial tile
+  static_assert(NWIN * XBUF == TX_XAREA, "window area");
+  static_assert(KP * NG * 16 * TP * 4 <= TX_RING + TX_XAREA, "partial tiles");
+  extern __shared__ __align__(128) uint8_t smem[];
+  uint8_t* xs = smem + TX_RING;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(xs + TX_XAREA);
+  const uint32_t ring0 = smem_u32(smem), xs0 = smem_u32(xs), bar0 = smem_u32(bars);
+  auto full_bar = [&](int s) { return bar0 + 8u * s; };
+  auto empty_bar = [&](int s) { return bar0 + 8u * (RG::NSLOT + s); };
+  auto xfull_bar = [&](int s) { return bar0 + 8u * (2 * RG::NSLOT + s); };
+  auto xempty_bar = [&](int s) { return bar0 + 8u * (2 * RG::NSLOT + NWIN + s); };
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int K = a.K, N = a.N, NB = a.B;
+  const int nkc = (K + KC - 1) / KC;
+  int grp_begin;
+  const int ng = cta_row_groups(N, grp_begin);        // 1..NG
+
+  if (tid == 0) {
+    for (int s = 0; s < RG::NSLOT; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CWARPS); }
+    for (int s = 0; s < NWIN; ++s) { mbar_init(xfull_bar(s), 1); mbar_init(xempty_bar(s), CWARPS); }
+    mbar_fence_init();
+  }
+  // rows of the activation windows that no clip owns stay zero (their MMA columns are never stored)
+  for (int i = tid; i < TX_XAREA / 16; i += THREADS) reinterpret_cast<uint4*>(xs)[i] = make_uint4(0, 0, 0, 0);
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  __syncthreads();
+  pdl_launch_dependents();
+
+  if (warp == CWARPS) {
+    // =============================== producer (gemv_tcw's) ===============================
+    if (lane == 0) {
+      const int total = ng * nkc;
+      const int pre = total < RG::NSLOT ? total : RG::NSLOT;
+      const uint8_t* W = weight_bytes<FMT>(a);
+      {
+        int kc = 0, lg = 0;
+        for (int idx = 0; idx < pre; ++idx) {
+          const uint32_t bytes = (uint32_t)min(KC, K - kc * KC) * (16u * RG::EB);
+          const uint8_t* src = W + ((size_t)(grp_begin + lg) * 16 * K + (size_t)kc * KC * 16) * RG::EB;
+          mbar_arrive_expect_tx(full_bar(idx), bytes);
+          bulk_g2s(ring0 + idx * RG::SLOT, src, bytes, full_bar(idx));
+          if (++lg == ng) { lg = 0; ++kc; }
+        }
+      }
+      pdl_wait();
+      int idx = 0, slot = 0, use = 0;
+      const uint32_t win_bytes = (uint32_t)NB * TW_XROW;
+      for (int kc = 0; kc < nkc; ++kc) {
+        const int xb = kc & (NWIN - 1);
+        if (kc >= NWIN) mbar_wait(xempty_bar(xb), (uint32_t)(((kc / NWIN) - 1) & 1));
+        mbar_arrive_expect_tx(xfull_bar(xb), win_bytes);
+        bulk_g2s(xs0 + xb * XBUF, a.x + (size_t)kc * NB * XWIN_PITCH, win_bytes, xfull_bar(xb));
+        for (int lg = 0; lg < ng; ++lg) {
+          if (idx >= pre) {
+            const uint32_t bytes = (uint32_t)min(KC, K - kc * KC) * (16u * RG::EB);
+            const uint8_t* src = W + ((size_t)(grp_begin + lg) * 16 * K + (size_t)kc * KC * 16) * RG::EB;
+            mbar_wait(empty_bar(slot), (uint32_t)((use - 1) & 1));
+            mbar_arrive_expect_tx(full_bar(slot), bytes);
+            bulk_g2s(ring0 + slot * RG::SLOT, src, bytes, full_bar(slot));
+          }
+          ++idx;
+          if (++slot == RG::NSLOT) { slot = 0; ++use; }
+        }
+      }
+    }
+    return;
+  }
+
+  // =============================== consumers ===============================
+  pdl_wait();
+  const int g = lane >> 2, q = lane & 3;
+  const int kp = warp % KP, cg = warp / KP;
+  float acc[NG][2][4];
+#pragma unroll
+  for (int i = 0; i < NG; ++i)
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+      for (int r = 0; r < 4; ++r) acc[i][j][r] = 0.f;
+
+  int slot = 0;
+  uint32_t par = 0;
+  for (int kc = 0; kc < nkc; ++kc) {
+    const int xb = kc & (NWIN - 1);
+    const int kb_n = min(KC, K - kc * KC) >> 5;
+    mbar_wait(xfull_bar(xb), (uint32_t)((kc / NWIN) & 1));
+    const uint8_t* xw = xs + xb * XBUF;
+    // the B fragments of this warp's 16 clips and K blocks, the same for every row group
+    uint4 xq[TPW][2];
+#pragma unroll
+    for (int t = 0; t < TPW; ++t)
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        xq[t][j] = *reinterpret_cast<const uint4*>(xw + (16 * cg + 8 * j + g) * TW_XROW + (kp + KP * t) * 64 + q * 16);
+#pragma unroll
+    for (int i = 0; i < NG; ++i) {
+      if (i < ng) {
+        mbar_wait(full_bar(slot), par);
+        const uint8_t* base = smem + slot * RG::SLOT;
+#pragma unroll
+        for (int t = 0; t < TPW; ++t) {
+          const int kb = kp + KP * t;
+          if (kb < kb_n) {
+            uint4 wa, wb;
+            load_a<FMT>(base, kb, lane, wa, wb);
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+              mma_bf16(acc[i][j], wa.x, wb.x, wa.y, wb.y, xq[t][j].x, xq[t][j].y);
+              mma_bf16(acc[i][j], wa.z, wb.z, wa.w, wb.w, xq[t][j].z, xq[t][j].w);
+            }
+          }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_bar(slot));
+        if (++slot == RG::NSLOT) { slot = 0; par ^= 1u; }
+      }
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(xempty_bar(xb));
+  }
+
+  // ---------------- the KP partial tiles of every group and clip meet in the (now idle) shared memory ----------------
+  cbar();
+  float* tiles = reinterpret_cast<float*>(smem);        // [kp][group][16][TP]
+#pragma unroll
+  for (int i = 0; i < NG; ++i) {
+    if (i < ng) {
+      float* t = tiles + ((size_t)kp * NG + i) * 16 * TP + 16 * cg;
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        t[g * TP + 8 * j + 2 * q] = acc[i][j][0];
+        t[g * TP + 8 * j + 2 * q + 1] = acc[i][j][1];
+        t[(g + 8) * TP + 8 * j + 2 * q] = acc[i][j][2];
+        t[(g + 8) * TP + 8 * j + 2 * q + 1] = acc[i][j][3];
+      }
+    }
+  }
+  cbar();
+
+  // ---------------- fused epilogue (gemv_tcw's item order, one pass per clip group) ----------------
+  const int mode = e.mode;
+  const bool pairs = (mode == GEMV_SWIGLU || mode == GEMV_QKV);
+  auto tile_sum = [&](int lg, int el) {
+    float v = tiles[(size_t)lg * 16 * TP + el];
+#pragma unroll
+    for (int k2 = 1; k2 < KP; ++k2) v += tiles[((size_t)k2 * NG + lg) * 16 * TP + el];
+    return v;
+  };
+  if (!pairs) {
+    const int rr = tid & 15;
+    for (int bb = 0; bb < CG; ++bb) {
+      const int b = 16 * bb + (tid >> 4);
+#pragma unroll 2
+      for (int lg = 0; lg < ng; ++lg) {
+        const int vrow = (grp_begin + lg) * 16 + rr;
+        if (b < NB && vrow < N) {
+          const float v0 = row_scaled<FMT>(a, vrow, tile_sum(lg, rr * TP + b));
+          if (mode == GEMV_RES) epi_residual(e, b, r0 + vrow, v0);
+          else epi_logit(e, b, r0 + vrow, v0);
+        }
+      }
+    }
+  } else {
+    const int pr = tid & 7;
+    for (int bb = 0; bb < CG; ++bb) {
+      const int b = 16 * bb + ((tid >> 3) & 15);
+      int col = 0, floor = 0;
+      if (mode == GEMV_QKV && b < NB) { col = decode_col(e, b); floor = __ldg(e.n_pad + b); }
+      for (int lg = tid >> 7; lg < ng; lg += 2) {
+        const int rr = 2 * pr;
+        const int vrow = (grp_begin + lg) * 16 + rr;
+        if (b >= NB || vrow >= N) continue;
+        const float v0 = row_scaled<FMT>(a, vrow, tile_sum(lg, rr * TP + b));
+        const float v1 = row_scaled<FMT>(a, vrow + 1, tile_sum(lg, (rr + 1) * TP + b));
+        if (mode == GEMV_SWIGLU) epi_swiglu(e, b, r0 + vrow, NB, v0, v1);
+        else epi_qkv_rope(e, b, r0 + vrow, col, floor, v0, v1);
+      }
+    }
+  }
+}
+
 // row-major W[N][K] -> tiled copy. One thread per 16-byte chunk of the output.
 __global__ void gemv_tc_repack_kernel(const bf16* __restrict__ W, bf16* __restrict__ dst, int N, int K, int qkv) {
   const size_t chunks_per_group = (size_t)2 * K;                      // 16 rows x K x 2 B / 16 B
@@ -1051,6 +1264,52 @@ int launch_tcw(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
   return 0;
 }
 
+typedef void (*TcxKernel)(const GemvArgs, const GemvEpilogue, const int);
+const TcxKernel tcx_bf16[2][3] = {
+    {gemv_tcx_kernel<2, 2, W_BF16>, gemv_tcx_kernel<6, 2, W_BF16>, gemv_tcx_kernel<10, 2, W_BF16>},
+    {gemv_tcx_kernel<2, 4, W_BF16>, gemv_tcx_kernel<4, 4, W_BF16>, gemv_tcx_kernel<6, 4, W_BF16>}};
+const TcxKernel tcx_fp8[2][3] = {
+    {gemv_tcx_kernel<2, 2, W_FP8>, gemv_tcx_kernel<6, 2, W_FP8>, gemv_tcx_kernel<10, 2, W_FP8>},
+    {gemv_tcx_kernel<2, 4, W_FP8>, gemv_tcx_kernel<4, 4, W_FP8>, gemv_tcx_kernel<6, 4, W_FP8>}};
+const int tcx_ng[2][3] = {{2, 6, 10}, {2, 4, 6}};
+
+// 17..64 clips: a matrix with more row groups per SM than the largest instance takes (10 groups at 17..32 clips,
+// 6 at 33..64) runs as consecutive launches over near-equal row slices; the epilogue addresses rows by their
+// index in the whole matrix
+int launch_tcx(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
+  VCL_REQUIRE(a.norm_w == nullptr && a.embed == nullptr && a.amax_out == nullptr,
+              "gemv: the 17..64-clip kernel takes normalised activations (no fused norm, embedding gather or "
+              "arg-max partials)");
+  VCL_REQUIRE((uintptr_t)a.x % 16 == 0, "gemv_tcx: operands must be 16-byte aligned");
+  const int fmt = weight_format(a);
+  if (fmt < 0) return fmt;
+  const int cgi = a.B <= 32 ? 0 : 1;                                  // 2 or 4 clip groups of 16
+  const int groups = (a.N + 15) / 16, sms = device_num_sms();
+  const int ng_cap = tcx_ng[cgi][2];
+  const int n_slices = (groups + ng_cap * sms - 1) / (ng_cap * sms);
+  for (int s = 0; s < n_slices; ++s) {
+    const int g0 = (int)((long long)groups * s / n_slices), g1 = (int)((long long)groups * (s + 1) / n_slices);
+    const long long r0 = (long long)g0 * 16;
+    GemvArgs sa = a;
+    if (fmt == W_FP8) {
+      sa.W_fp8 = a.W_fp8 + r0 * a.K;
+      sa.w_scale = a.w_scale + r0;
+    } else {
+      sa.W_tiled = a.W_tiled + r0 * a.K;
+    }
+    sa.N = (a.N < g1 * 16 ? a.N : g1 * 16) - (int)r0;
+    const int grid = g1 - g0 < sms ? g1 - g0 : sms;
+    cudaLaunchAttribute attr[1];
+    cudaLaunchConfig_t cfg = pdl_config(grid, TX_SMEM, stream, attr);
+    const int ng_max = (g1 - g0 + grid - 1) / grid;
+    const int pick = ng_max <= tcx_ng[cgi][0] ? 0 : ng_max <= tcx_ng[cgi][1] ? 1 : 2;
+    auto kern = fmt == W_FP8 ? tcx_fp8[cgi][pick] : tcx_bf16[cgi][pick];
+    VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, sa, e, (int)r0));
+    count_launches(1);
+  }
+  return 0;
+}
+
 }  // namespace
 
 extern "C" int vcl_debug_tc_trace_dump(const char* path) {
@@ -1074,6 +1333,11 @@ int init_gemv_kernels() {
     VCL_CUDA_OK(cudaFuncSetAttribute(tcw_bf16[i], cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
     VCL_CUDA_OK(cudaFuncSetAttribute(tcw_fp8[i], cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM_FP8));
   }
+  for (int c = 0; c < 2; ++c)
+    for (int i = 0; i < 3; ++i) {
+      VCL_CUDA_OK(cudaFuncSetAttribute(tcx_bf16[c][i], cudaFuncAttributeMaxDynamicSharedMemorySize, TX_SMEM));
+      VCL_CUDA_OK(cudaFuncSetAttribute(tcx_fp8[c][i], cudaFuncAttributeMaxDynamicSharedMemorySize, TX_SMEM));
+    }
   return 0;
 }
 
@@ -1084,7 +1348,8 @@ int gemv_grid(int N) {
 }
 
 bool gemv_fits(int B, int N, int K, bool norm, bool pairs, bool fp8) {
-  if (B < 1 || B > 16 || N < 1) return false;
+  if (B < 1 || B > 64 || N < 1) return false;
+  if (B > 16) return K % 32 == 0;             // 17..64 clips: any matrix, in row slices
   if (B > 4) return K % 32 == 0 && (!pairs || (N + 15) / 16 <= TW_NG_MAX * device_num_sms());
   size_t smem = 0; int xe = 0, rc = 0;
   return plan(B, N, K, norm, gemv_grid(N), &smem, &xe, &rc, fp8 ? W_FP8 : W_BF16) >= 4;
@@ -1117,7 +1382,7 @@ int launch_gemv(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
   const bool pairs = e.mode == GEMV_SWIGLU || e.mode == GEMV_QKV;
   VCL_REQUIRE(e.mode >= GEMV_RES && e.mode <= GEMV_LOGITS, "gemv: unknown epilogue mode %d", e.mode);
   VCL_REQUIRE(gemv_fits(a.B, a.N, a.K, a.norm_w != nullptr, pairs, a.W_fp8 != nullptr),
-              "gemv: B=%d N=%d K=%d is outside the decode kernels' range (1..16 clips, K a multiple of 32; "
+              "gemv: B=%d N=%d K=%d is outside the decode kernels' range (1..64 clips, K a multiple of 32; "
               "1..4 clips: K <= 14336 and the shared-memory plan; 5..16 clips: q|k|v and gate|up at most 14 "
               "row groups of 16 per SM)", a.B, a.N, a.K);
   VCL_REQUIRE(e.mode != GEMV_SWIGLU || a.N % 2 == 0, "gemv swiglu: N must be even (interleaved gate/up rows)");
@@ -1126,7 +1391,7 @@ int launch_gemv(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
               "gemv: the q|k|v epilogue needs the key floors n_pad, and no other epilogue takes them");
   VCL_REQUIRE(a.embed == nullptr || (a.vocab > 0 && (a.tok_in != nullptr || (a.amax_in != nullptr && a.amax_n > 0))),
               "gemv: the fused embedding gather needs a token source");
-  return a.B <= 4 ? launch_tc(a, e, stream) : launch_tcw(a, e, stream);
+  return a.B <= 4 ? launch_tc(a, e, stream) : a.B <= 16 ? launch_tcw(a, e, stream) : launch_tcx(a, e, stream);
 }
 
 }  // namespace vcl

@@ -14,10 +14,10 @@ typedef __nv_bfloat16 bf16;
 // Packed prefill (vcl_llm_slots_prefill): n <= PACK_SEQ_MAX sequences of lengths S_0 .. S_{n-1} concatenated
 // without padding into M = sum S_i rows, sequence i going to cache slot slot_i. One device int array describes the
 // layout, and every kernel of a packed prefill reads it through the accessors below:
-//   [0, 16)   row offset of sequence i      [16, 32)  its length S_i
-//   [32, 48)  its cache slot                [48, 64)  its last row (offset + S_i - 1), whose logits give its token
-//   [64 + 2r] sequence of row r             [64 + 2r + 1] position of row r inside its sequence
-constexpr int PACK_SEQ_MAX = 16;
+//   [0, 64)    row offset of sequence i     [64, 128)   its length S_i
+//   [128, 192) its cache slot               [192, 256)  its last row (offset + S_i - 1), whose logits give its token
+//   [256 + 2r] sequence of row r            [256 + 2r + 1] position of row r inside its sequence
+constexpr int PACK_SEQ_MAX = 64;
 constexpr int PACK_HEAD = 4 * PACK_SEQ_MAX;
 inline size_t pack_elems(long long rows) { return PACK_HEAD + 2 * (size_t)rows; }
 template <class T> __host__ __device__ inline T* pack_off(T* p) { return p; }
@@ -181,18 +181,18 @@ int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, c
                             int kv_len, float scale, cudaStream_t stream, const int* pos_dev, bool o_xwin,
                             const int* n_pad);
 
-// ---- decode_gemv.cu : decode-time weight streaming (1..16 new tokens) -------------------------------
-// Two ring kernels (bulk-copy ring over a slot-ordered copy of the matrix + mma.sync) behind one launcher:
+// ---- decode_gemv.cu : decode-time weight streaming (1..64 new tokens) -------------------------------
+// Three ring kernels (bulk-copy ring over a slot-ordered copy of the matrix + mma.sync) behind one launcher:
 // 1..4 clips stage the activation vectors in shared memory (K <= 14336, optional fused RMSNorm and, for
-// q|k|v, a fused token-embedding gather); 5..16 clips read activations that are already normalised and
-// stored window-major ("xwin", below). Both read the copy that launch_gemv_repack builds, or its fp8 twin from
+// q|k|v, a fused token-embedding gather); 5..16 and 17..64 clips read activations that are already normalised
+// and stored window-major ("xwin", below). All three read the copy that launch_gemv_repack builds, or its fp8 twin from
 // launch_gemv_quantize_fp8 (E4M3 codes in the same order plus a power-of-two scale per row; decode_gemv.cu).
 // per-CTA partial arg-max of the logits kernel: the next step's q|k|v kernel reduces the grid's
 // partials itself (lowest index wins ties), so no arg-max kernel runs between two decode steps
 struct ArgmaxPart { float v; int idx; };
 
 struct GemvArgs {
-  const bf16* x = nullptr; long long ldx = 0;   // [B][ldx] (5..16 clips: xwin layout, see below)
+  const bf16* x = nullptr; long long ldx = 0;   // [B][ldx] (5..64 clips: xwin layout, see below)
   const bf16* W_tiled = nullptr;                // slot-ordered copy of the [N, K] matrix ...
   const uint8_t* W_fp8 = nullptr;               // ... or its E4M3 codes in the same order (W_tiled null) with the
   const float* w_scale = nullptr;               //     row scales 2^e_r [N]: row r is W~[r] = code * 2^e_r
@@ -220,7 +220,7 @@ enum GemvMode {
 struct GemvEpilogue {
   int mode = GEMV_RES;
   bf16* out = nullptr; long long ldo = 0;       // RES: out[B][ldo]; SWIGLU: out[B][ldo] ...
-  bool out_xwin = false;                        // ... or, 5..16 clips, in xwin layout (feeds down_proj)
+  bool out_xwin = false;                        // ... or, 5..64 clips, in xwin layout (feeds down_proj)
   const bf16* res = nullptr; long long ldr = 0; // RES
   bf16* q_out = nullptr; long long ldq = 0;     // QKV: q [B][ldq], cache base of the layer [B][H][s_max][128]
   bf16* kcache = nullptr; bf16* vcache = nullptr;
@@ -243,7 +243,8 @@ int launch_xwin_norm(const bf16* x, long long ldx, bf16* y, const bf16* w, int B
 
 int init_gemv_kernels();
 // whether a [N, K] projection of B clips has a decode kernel. norm: with the fused RMSNorm (1..4 clips);
-// pairs: a SWIGLU or QKV epilogue (5..16 clips: such a matrix has at most 14 row groups of 16 per SM); fp8: the
+// pairs: a SWIGLU or QKV epilogue (5..16 clips: such a matrix has at most 14 row groups of 16 per SM; 17..64
+// clips take any matrix whose K is a multiple of 32); fp8: the
 // kernels of fp8 weights (their shared-memory plan; they take every shape the bf16 kernels take)
 bool gemv_fits(int B, int N, int K, bool norm, bool pairs, bool fp8 = false);
 int gemv_grid(int N);                         // CTAs of a 1..4-clip launch over N rows
@@ -258,7 +259,8 @@ int launch_gemv_repack(const bf16* W, bf16* dst, int N, int K, bool qkv_pairs, c
 int launch_gemv_quantize_fp8(const bf16* W, bf16* w_deq, uint8_t* codes, float* scales, int N, int K, bool qkv_pairs,
                              int* bad, cudaStream_t stream);
 // 1..4 clips: gemv_tc_kernel; 5..16 clips: gemv_tcw_kernel (several launches over row slices when a RES /
-// LOGITS matrix has more than 14 row groups per SM)
+// LOGITS matrix has more than 14 row groups per SM); 17..64 clips: gemv_tcx_kernel (row slices of at most 10 / 6
+// row groups per SM at 17..32 / 33..64 clips, for every epilogue)
 int launch_gemv(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream);
 
 }  // namespace vcl

@@ -151,8 +151,15 @@ struct vcl_handle {
   }
   // rows of the row-major lm_head: vocab rounded up to the 256-wide GEMM tile, the extra rows zero
   int vocab_padded() const { return (cfg.vocab + 255) / 256 * 256; }
-  // cache slots: as many as clips the decode ring kernels take in one launch
-  int n_slots_max() const { return cfg.max_batch < 16 ? cfg.max_batch : 16; }
+  // cache slots: max_slots, or by default min(max_batch, 16)
+  int n_slots_max() const { return cfg.max_slots > 0 ? cfg.max_slots : cfg.max_batch < 16 ? cfg.max_batch : 16; }
+  // the capacity named in a slot-count rejection (the default's wording predates max_slots)
+  std::string slots_note() const {
+    char b[96];
+    if (cfg.max_slots > 0) snprintf(b, sizeof b, "max_slots %d", cfg.max_slots);
+    else snprintf(b, sizeof b, "max_batch %d, at most 16 slots", cfg.max_batch);
+    return b;
+  }
 };
 
 namespace {
@@ -309,13 +316,16 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   VCL_REQUIRE(c->clip_layers >= 0 && c->llm_layers >= 0 && c->vocab > 0, "vcl_create: bad layer/vocab counts");
   VCL_REQUIRE(c->max_frames > 0 && c->max_batch > 0 && c->max_seq > 0, "vcl_create: capacities must be > 0");
   VCL_REQUIRE(c->proj_type == VCL_PROJ_LINEAR || c->proj_type == VCL_PROJ_MLP2X_GELU, "vcl_create: proj_type");
+  VCL_REQUIRE(c->max_slots == 0 || (c->max_slots >= 1 && c->max_slots <= c->max_batch && c->max_slots <= 64),
+              "vcl_create: max_slots=%d outside 1..%d (0: min(max_batch, 16))", c->max_slots,
+              c->max_batch < 64 ? c->max_batch : 64);
   {
-    // every decode projection must have a kernel for every clip count up to 16 (beyond: the GEMM)
+    // every decode projection must have a kernel for every clip count up to 64 (beyond: the GEMM)
     const int D = c->llm_hidden, F = c->llm_inter;
     const struct { const char* name; int N, K; bool norm, pairs; } mats[5] = {
         {"q|k|v", 3 * D, D, true, true}, {"o_proj", D, D, false, false}, {"gate|up", 2 * F, D, true, true},
         {"down_proj", D, F, false, false}, {"lm_head", c->vocab, D, true, false}};
-    for (int B = 1; B <= c->max_batch && B <= 16; ++B)
+    for (int B = 1; B <= c->max_batch && B <= 64; ++B)
       for (const auto& m : mats)
         VCL_REQUIRE(gemv_fits(B, m.N, m.K, m.norm, m.pairs),
                     "vcl_create: the %s projection [%d x %d] has no decode kernel for %d clips (1..4 clips: K <= 14336 "
@@ -468,7 +478,7 @@ int vcl_load_llm_weights_ex(vcl_handle* h, const vcl_tensor* tensors, int n, int
     const struct { const char* name; int N, K; bool norm, pairs; } mats[5] = {
         {"q|k|v", 3 * D, D, true, true}, {"o_proj", D, D, false, false}, {"gate|up", 2 * F, D, true, true},
         {"down_proj", D, F, false, false}, {"lm_head", c.vocab, D, true, false}};
-    for (int B = 1; B <= c.max_batch && B <= 16; ++B)
+    for (int B = 1; B <= c.max_batch && B <= 64; ++B)
       for (const auto& mt : mats)
         VCL_REQUIRE(gemv_fits(B, mt.N, mt.K, mt.norm, mt.pairs, true),
                     "vcl_load_llm_weights: the %s projection [%d x %d] has no fp8 decode kernel for %d clips", mt.name,
@@ -616,9 +626,15 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
     }
     e.logits = h->logits;
     VCL_TRY(launch_gemv(g, e, st));
+  } else if (B <= 64) {
+    // 5..64 clips: the rows normalised into the window-major layout first, then one ring kernel over the
+    // vocabulary matrix (in row slices)
+    g.x = h->d_x; g.ldx = c.llm_hidden; g.B = B;
+    VCL_TRY(launch_xwin_norm(x, ldx, h->d_x, h->norm_w, B, c.llm_hidden, c.rms_eps, st));
+    e.logits = h->logits;
+    VCL_TRY(launch_gemv(g, e, st));
   } else {
-    // 5..16 clips per launch, the rows normalised into the window-major layout first; more clips are split
-    // into ceil(B / 16) near-equal chunks (at least 8 clips each)
+    // more than 64 rows are split into ceil(B / 16) near-equal chunks of the 5..16-clip kernel
     const int n_chunks = (B + 15) / 16;
     for (int i = 0; i < n_chunks; ++i) {
       const int b0 = B * i / n_chunks, nb = B * (i + 1) / n_chunks - b0;
@@ -823,9 +839,9 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
   if (!fused_embed) VCL_TRY(launch_embed_tokens(io.tok_in, io.in_stride, h->embed, h->d_h, B, D, c.vocab, st));
   for (int l = 0; l < c.llm_layers; ++l) {
     const LlmLayerW& w = h->ll[l];
-    if (B <= 16) {
+    if (B <= 64) {
       // the ring kernels. 1..4 clips fuse the RMSNorm into the projection (and, in layer 0, the embedding
-      // gather); 5..16 clips take their inputs window-major (kernels.h: xwin), written by launch_xwin_norm,
+      // gather); 5..64 clips take their inputs window-major (kernels.h: xwin), written by launch_xwin_norm,
       // the attention kernel and the SwiGLU epilogue. The residual stream d_h stays row-major.
       const bool wide = B > 4;
       auto normed = [&](GemvArgs& g, const bf16* ln) -> int {
@@ -871,7 +887,7 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
       gd.x = h->d_act; gd.ldx = F; w.dn_d.into(gd); gd.B = B; gd.N = D; gd.K = F;
       VCL_TRY(launch_gemv(gd, residual, st));
     } else {
-      // B > 16: tensor-core path, the B new rows ride in one (mostly empty) 128-row tile and the
+      // B > 64: tensor-core path, the B new rows ride in one (mostly empty) 128-row tile and the
       // N tile is narrowed so that every SM streams a slice of the weights
       VCL_TRY(launch_rmsnorm(h->d_h, D, h->d_x, D, w.ln1, B, D, c.rms_eps, st));
       VCL_TRY(gemm(h->d_x, D, w.wqkv, D, h->d_qkv, 3 * D, nullptr, nullptr, 0, B, 3 * D, D, ACT_NONE, st));
@@ -1069,8 +1085,8 @@ int vcl_llm_slot_prefill(vcl_handle* h, int slot, const int64_t* ids, const void
                          const int32_t* vid_start, int S, int32_t* next_tok, void* stream) {
   VCL_REQUIRE(h && ids && vid_start && next_tok, "vcl_llm_slot_prefill: null argument");
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
-  VCL_REQUIRE(slot >= 0 && slot < h->n_slots_max(), "vcl_llm_slot_prefill: slot %d outside 0..%d (max_batch %d, at "
-              "most 16 slots)", slot, h->n_slots_max() - 1, h->cfg.max_batch);
+  VCL_REQUIRE(slot >= 0 && slot < h->n_slots_max(), "vcl_llm_slot_prefill: slot %d outside 0..%d (%s)", slot,
+              h->n_slots_max() - 1, h->slots_note().c_str());
   return llm_prefill(h, ids, video_feats, vid_start, 1, S, h->cfg.llm_layers, nullptr, nullptr, next_tok, 1,
                      as_stream(stream), 0, nullptr, nullptr, slot);
 }
@@ -1080,8 +1096,8 @@ int vcl_llm_slots_prefill(vcl_handle* h, int n, const int32_t* slots_host, const
                           void* stream) {
   VCL_REQUIRE(h != nullptr, "vcl_llm_slots_prefill: null handle");
   const vcl_config& c = h->cfg;
-  VCL_REQUIRE(n >= 1 && n <= h->n_slots_max(), "vcl_llm_slots_prefill: n=%d outside 1..%d (max_batch %d, at most 16 "
-              "slots)", n, h->n_slots_max(), c.max_batch);
+  VCL_REQUIRE(n >= 1 && n <= h->n_slots_max(), "vcl_llm_slots_prefill: n=%d outside 1..%d (%s)", n, h->n_slots_max(),
+              h->slots_note().c_str());
   VCL_REQUIRE(slots_host && seq_len_host && ids && vid_start && next_tok, "vcl_llm_slots_prefill: null argument");
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
   const int s_lim = c.max_seq < 512 ? c.max_seq : 512;   // 512: the key limit of the wgmma prefill attention
@@ -1119,8 +1135,8 @@ int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* 
                         int32_t* out_tokens, void* stream) {
   VCL_REQUIRE(h && first_tok && pos_host && out_tokens, "vcl_llm_slot_decode: null argument");
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
-  VCL_REQUIRE(n_slots >= 1 && n_slots <= h->n_slots_max(), "vcl_llm_slot_decode: n_slots=%d outside 1..%d (max_batch "
-              "%d, at most 16 slots)", n_slots, h->n_slots_max(), h->cfg.max_batch);
+  VCL_REQUIRE(n_slots >= 1 && n_slots <= h->n_slots_max(), "vcl_llm_slot_decode: n_slots=%d outside 1..%d (%s)",
+              n_slots, h->n_slots_max(), h->slots_note().c_str());
   VCL_REQUIRE(!h->padded, "vcl_llm_slot_decode: the cache is left-padded; slots are unpadded (start each one with "
               "vcl_llm_slot_prefill)");
   VCL_REQUIRE(n_new >= 1 && n_new <= h->cfg.max_seq, "vcl_llm_slot_decode: n_new=%d outside 1..max_seq %d", n_new,
@@ -1335,7 +1351,7 @@ int vcl_op_attention_vit(const void* qkv, void* out, int n_frames, int S, int H,
 int vcl_op_gemv(const void* x, const void* W, void* out, const void* res, const void* norm_w,
                 float eps, int B, int N, int K, void* stream) {
   if (check_device() != 0) return -2;
-  VCL_REQUIRE(B >= 1 && B <= 16, "vcl_op_gemv: B=%d outside 1..16 (more rows take the GEMM)", B);
+  VCL_REQUIRE(B >= 1 && B <= 64, "vcl_op_gemv: B=%d outside 1..64 (more rows take the GEMM)", B);
   VCL_REQUIRE(gemv_fits(B, N, K, norm_w != nullptr, false),
               "vcl_op_gemv: B=%d N=%d K=%d is outside the decode kernels' range", B, N, K);
   static bool inited = false;
@@ -1374,7 +1390,7 @@ int vcl_op_quantize_fp8(const void* W, int N, int K, void* w_deq, void* codes, f
 int vcl_op_gemv_fp8(const void* x, const void* W, void* out, const void* res, const void* norm_w,
                     float eps, int B, int N, int K, void* stream) {
   if (check_device() != 0) return -2;
-  VCL_REQUIRE(B >= 1 && B <= 16, "vcl_op_gemv_fp8: B=%d outside 1..16 (more rows take the GEMM)", B);
+  VCL_REQUIRE(B >= 1 && B <= 64, "vcl_op_gemv_fp8: B=%d outside 1..64 (more rows take the GEMM)", B);
   VCL_REQUIRE(gemv_fits(B, N, K, norm_w != nullptr, false, true),
               "vcl_op_gemv_fp8: B=%d N=%d K=%d is outside the decode kernels' range", B, N, K);
   static bool inited = false;
@@ -1402,13 +1418,13 @@ int vcl_op_gemv_fp8(const void* x, const void* W, void* out, const void* res, co
 
 namespace {
 
-// out = x . W^T (+ res) by the decode kernels, with g's weights; 5..16 rows through the xwin re-layout
+// out = x . W^T (+ res) by the decode kernels, with g's weights; 5..64 rows through the xwin re-layout
 int op_gemv_run(GemvArgs g, void* out, const void* res, float eps, cudaStream_t st) {
   const int B = g.B, N = g.N, K = g.K;
   GemvEpilogue e;
   e.mode = GEMV_RES; e.out = reinterpret_cast<bf16*>(out); e.ldo = N; e.res = reinterpret_cast<const bf16*>(res); e.ldr = N;
   if (B >= 5) {
-    // 5..16 rows: the wide ring kernel; its input is normalised and re-laid out (xwin) by a launch of its own,
+    // 5..64 rows: the xwin ring kernels; their input is normalised and re-laid out (xwin) by a launch of its own,
     // as on the decode path
     static bf16* xn = nullptr; static size_t xn_elems = 0;
     if (xn_elems < xwin_elems(B, K)) {

@@ -7,6 +7,7 @@ calls raise.
 from __future__ import annotations
 
 import ctypes
+import operator
 import os
 from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int64, c_uint64, c_void_p
 
@@ -44,7 +45,23 @@ class vcl_config(Structure):
         ("llm_heads", c_int32), ("vocab", c_int32), ("rms_eps", c_float), ("rope_theta", c_float),
         ("proj_type", c_int32), ("n_temporal", c_int32),
         ("max_frames", c_int32), ("max_batch", c_int32), ("max_seq", c_int32),
+        ("max_slots", c_int32),    # 0: min(max_batch, 16) in-flight cache slots
     ]
+
+
+def slot_capacity(max_batch: int, max_slots=None) -> int:
+    """The engine's in-flight cache slots: max_slots, or min(max_batch, 16) for None. Raises ValueError for any
+    other value outside 1 .. min(max_batch, 64) (vcl_create would reject it; its 0 is spelled None here)."""
+    if max_slots is None:
+        return min(int(max_batch), 16)
+    try:
+        n = None if isinstance(max_slots, bool) else operator.index(max_slots)     # int, numpy integers
+    except TypeError:
+        n = None
+    if n is None or not 1 <= n <= min(int(max_batch), 64):
+        raise ValueError(f"max_slots={max_slots!r} outside 1..{min(int(max_batch), 64)} (at most 64 and at most "
+                         f"max_batch {max_batch}; None: min(max_batch, 16))")
+    return n
 
 
 class vcl_tensor(Structure):
@@ -275,7 +292,7 @@ def op_quantize_fp8(w):
     return deq, codes, scales
 
 
-XWIN_KC, XWIN_PITCH = 512, 544     # kernels.h: the window-major activation layout of the 5..16-clip decode kernels
+XWIN_KC, XWIN_PITCH = 512, 544     # kernels.h: the window-major activation layout of the 5..64-clip decode kernels
 
 
 def xwin_offset(b, k, B):

@@ -298,11 +298,15 @@ class VideoChatGPTLlamaForCausalLM:
     config_class = VideoChatGPTConfig
 
     def __init__(self, config: VideoChatGPTConfig, clip_config=None, max_batch: int = 1, max_seq: int | None = None,
-                 clip_run_layers: int | None = None, llm_weight_format: str = "bf16"):
+                 clip_run_layers: int | None = None, llm_weight_format: str = "bf16", max_slots: int | None = None):
         """llm_weight_format: "bf16", or "fp8_e4m3" to hold the language model's streamed matrices as E4M3 codes
         with power-of-two row scales (vcl_load_llm_weights_ex): decode reads half the weight bytes, and every
-        output is that of the bf16 engine on the dequantized weights."""
+        output is that of the bf16 engine on the dequantized weights.
+        max_slots: the KV-cache slots generate_requests keeps in flight, 1 .. min(max_batch, 64); None means
+        min(max_batch, 16). A capacity only: which decode kernel runs depends on the clip count of each call."""
         vn.weight_format_code(llm_weight_format)          # ValueError before anything else
+        self._n_slots = vn.slot_capacity(max_batch, max_slots)
+        self._max_slots = 0 if max_slots is None else self._n_slots
         self._llm_weight_format = llm_weight_format
         self.config = config
         self.clip_config = _clip_config(clip_config if clip_config is not None
@@ -405,6 +409,7 @@ class VideoChatGPTLlamaForCausalLM:
             k.proj_type = vn.PROJ_LINEAR if kind == "linear" else vn.PROJ_MLP2X_GELU
             k.n_temporal = 100
             k.max_frames, k.max_batch, k.max_seq = 100, self._max_batch, self._max_seq
+            k.max_slots = self._max_slots
             self._engine = vn.Engine(k)
             self._clip_loaded = self._llm_loaded = False
         if need_clip and not self._clip_loaded:
@@ -726,7 +731,8 @@ class VideoChatGPTLlamaForCausalLM:
         it for that request alone. A request ends at its first EOS, at its max_new_tokens, or at the first token
         where one of its stopping criteria fires (called token by token with the [1, S_i + k] prefix on the host,
         as a stepwise generate would call it).
-        slots: cache slots in flight, default and at most min(max_batch, 16). Requests are admitted one prefill
+        slots: cache slots in flight, default and at most the engine's slot count (max_slots; by default
+        min(max_batch, 16)). Requests are admitted one prefill
         at a time; all slots then decode _SLOT_CHUNK steps per device call. Everything is validated before any
         device work. Afterwards there is no turn for generate_continue to continue.
         packed_admission: at every admission point all free slots are filled from the queue (in queue order) by
@@ -744,9 +750,11 @@ class VideoChatGPTLlamaForCausalLM:
             if r.get("do_sample", do_sample) and r.get("seed", seed) is None:
                 raise NotImplementedError(f"request {i}: generate_requests decodes greedily unless given a seed; "
                                           "sampling in flight needs seed= (the call's or the request's own)")
-        cap = min(self._max_batch, 16)
+        cap = self._n_slots
         n_slots = cap if slots is None else int(slots)
         if not 1 <= n_slots <= cap:
+            if self._max_slots:
+                raise ValueError(f"slots={slots} outside 1..{cap} (max_slots {self._max_slots})")
             raise ValueError(f"slots={slots} outside 1..{cap} (at most 16 and at most max_batch {self._max_batch})")
         eng = self._ensure_engine(need_llm=True)
         samp = dict(do_sample=do_sample, temperature=temperature, top_k=top_k, seed=seed)
