@@ -227,8 +227,9 @@ int vcl_llm_generate_padded(vcl_handle* h, const int64_t* ids, const void* video
 /* In-flight (continuous) batching: every clip of the KV cache is a SLOT that holds its own sequence at its own
  * length, so a finished request's slot takes the next queued request while the other slots keep decoding.
  * There are max_slots slots (vcl_config; 0 means min(max_batch, 16), at most min(max_batch, 64)). Slots are
- * unpadded. Decode projections by clip count: 1..4 gemv_tc, 5..16 gemv_tcw, 17..64 gemv_tcx (the ring kernels of
- * decode_gemv.cu, each streaming every weight byte once per step), more than 64 the prefill GEMM.
+ * unpadded. Decode projections by clip count: 1..4 gemv_tc, 5..64 gemv_tcw with 1 / 2 / 4 clip groups at 5..16 /
+ * 17..32 / 33..64 clips (the ring kernels of decode_gemv.cu, each streaming every weight byte once per step), more
+ * than 64 the prefill GEMM.
  *
  * vcl_llm_slot_prefill: vcl_llm_prefill of ONE prompt (ids [1,S], video_feats [1, n_temporal+P, 1024] or NULL,
  * vid_start [1]) into cache slot `slot` (0 <= slot < max_slots). The slot then holds positions

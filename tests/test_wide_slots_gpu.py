@@ -1,4 +1,5 @@
-"""Decode of 17..64 clips by the third ring kernel (gemv_tcx) and in-flight batching with up to 64 cache slots.
+"""Decode of 17..64 clips by the window kernel (gemv_tcw with 2 or 4 clip groups) and in-flight batching with up to
+64 cache slots.
 
 - the kernel (vcl_op_gemv) at B = 17, 24, 32, 33, 48, 64 against the fp64 reference and bounds of test_gemv, at the
   7B q|k|v, o_proj, down_proj and lm_head shapes; clip b's output does not depend on the other clips' inputs; the
@@ -16,7 +17,8 @@
   cache writes and generate against the oracle there;
 - at 7B width (B = 33: q|k|v in one launch, gate|up in two row slices) and 13B width (B = 48: q|k|v and gate|up in
   row slices), decode steps teacher-forced against the bf16 oracle follow the margin rule, which checks the RoPE and
-  SwiGLU epilogues of the sliced launches against an independent reference."""
+  SwiGLU epilogues of the sliced launches against an independent reference; so do decode steps at 10240 width and
+  5..16 clips (B = 8: q|k|v in row slices of one clip group)."""
 import time
 import math
 
@@ -28,7 +30,7 @@ pytestmark = pytest.mark.gpu
 import vcl_native as vn  # noqa: E402
 import _fp8_ref as R  # noqa: E402
 from oracle import vcl_oracle as O  # noqa: E402
-from _util import teacher_forced_check, to_dev, vid_start_of  # noqa: E402
+from _util import relerr, teacher_forced_check, to_dev, vid_start_of  # noqa: E402
 from test_padded_batch_gpu import first_near_tie, padded_batch, video_feats  # noqa: E402
 from test_kv_cache_gpu import (_assert_kv, _assert_same, _caches, _check_step, _embed, _fill_sentinel, _ids,  # noqa: E402
                                _no_video, _ref_kv, _state)
@@ -38,6 +40,7 @@ DEV = "cuda"
 SMALL = O.LlmCfg(hidden=512, inter=1024, heads=4, layers=2)
 W7B = O.LlmCfg(hidden=4096, inter=11008, heads=32, layers=2)
 W13B = O.LlmCfg(hidden=5120, inter=13824, heads=40, layers=1)
+W10K = O.LlmCfg(hidden=10240, inter=2048, heads=80, layers=1)   # q|k|v: 1920 row groups > 14 per SM x 132 SMs
 WIDE_B = [17, 24, 32, 33, 48, 64]
 
 
@@ -501,4 +504,26 @@ def test_wide_width_decode_teacher_forced_against_the_oracle(cfg, B):
     ids = O.make_prompt_ids(cfg, 356, seed=620 + B, batch=B).to(DEV)
     vf = video_feats(B, 621 + B)
     teacher_forced_check(eng, sd_b, cfg, ids, vf, 4, f"{cfg.hidden} B={B}")
+    eng.close()
+
+
+@torch.no_grad()
+def test_sliced_qkv_at_5_to_16_clips_decodes_like_the_oracle():
+    """5..16 clips with q|k|v in row slices (width 10240: 1920 row groups, more than 14 per SM on 132 SMs) through the
+    RoPE and KV-append epilogue. The prefill's RMSNorm takes widths up to 8192, so the engine decodes from an empty
+    cache: steps at positions 0..3 on random tokens against the oracle's cached forward, with the margin rule."""
+    cfg, B = W10K, 8
+    sd_b = to_dev(O.random_llm_state(cfg, seed=61))
+    eng = engine(cfg, B, 16, sd=sd_b)
+    toks = torch.randint(3, 32000, (B, 4), generator=torch.Generator().manual_seed(628)).to(DEV)
+    past = None
+    for i in range(toks.shape[1]):
+        o_logits, _, past = O.llm_forward(sd_b, cfg, toks[:, i:i + 1], None, past)
+        o = o_logits[:, -1].float()
+        lg, _ = eng.decode_step(toks[:, i].to(torch.int32).contiguous(), i, want_logits=True)
+        e = relerr(lg, o)
+        assert e < 3e-2, (i, e)
+        top = torch.topk(o, 2, dim=-1)
+        clear = (top.values[:, 0] - top.values[:, 1]) / (top.values[:, 0].abs().clamp_min(2 ** -6) * 2 ** -7) >= 3
+        assert torch.equal(lg.argmax(-1)[clear], top.indices[clear, 0]), i
     eng.close()

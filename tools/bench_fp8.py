@@ -18,6 +18,8 @@ the engines of --formats (one engine each; a 7B engine sized for 64 clips holds 
 run one format per call). --compare-lib PATH (with --decode-only) also creates, for every format, an engine from another
 build of libvcl.so (e.g. the parent commit's, built side by side) and alternates the two call by call; --layers N
 shortens the model so that both engines fit on one card (the ratio of the two is what this compares).
+"tokens_equal" at each B says whether the engines' first tokens and decode_loop tokens of the last round are equal
+(for two builds of the same format: an identity check; bf16 against fp8 on the same W need not agree).
 The card's name and power limit are printed with the numbers.
 """
 import argparse
@@ -110,10 +112,10 @@ def decode_arm(engines, B, rounds, st, model="7b", fmts=None):
             firsts[k] = e.prefill(ids, vf, vs)[2]
             e.decode_loop(firsts[k], S, N_NEW)                   # capture
     st.synchronize()
-    times = {k: [] for k in engines}
+    times, toks = {k: [] for k in engines}, {}
     for _ in range(rounds):
         for k, e in engines.items():
-            times[k].append(time_ms(lambda: e.decode_loop(firsts[k], S, N_NEW), st) / (N_NEW - 1))
+            times[k].append(time_ms(lambda: toks.__setitem__(k, e.decode_loop(firsts[k], S, N_NEW)), st) / (N_NEW - 1))
     m = bench.MODELS[model]
     kv = 2 * m["layers"] * B * (S + N_NEW // 2) * m["hidden"] * 2       # K and V read per step, mean position
     out = {}
@@ -122,6 +124,10 @@ def decode_arm(engines, B, rounds, st, model="7b", fmts=None):
         fmt = fmts[k] if fmts else k
         out[k] = dict(ms_per_step=round(ms, 3), gb_s=round((streamed_bytes(model, fmt) + kv) / ms / 1e6, 1),
                       spread_ms=[round(min(times[k]), 3), round(max(times[k]), 3)])
+    if len(engines) > 1:
+        ref = next(iter(engines))
+        out["tokens_equal"] = all(torch.equal(firsts[k], firsts[ref]) and torch.equal(toks[k], toks[ref])
+                                  for k in engines)
     return out
 
 

@@ -32,7 +32,7 @@ from bench_padded import card  # noqa: E402
 def attribute(names, layers):
     """kernel names of one step in launch order -> a label per kernel"""
     labels, layer, phase = [], -1, None
-    tcx_in_phase = []
+    proj_in_phase = []
     for i, n in enumerate(names):
         if "xwin_norm" in n:
             if phase in (None, "down"):
@@ -44,16 +44,16 @@ def attribute(names, layers):
         elif "decode_attn" in n:
             labels.append("attention")
             phase = "o_proj"
-        elif "gemv_tcx" in n or "gemv_tcw" in n:
+        elif "gemv_tcw" in n:
             labels.append(phase)
             if phase == "gate|up":
-                tcx_in_phase.append(i)
+                proj_in_phase.append(i)
         else:
             labels.append("other")
         # the last projection launch before the next norm of a layer's MLP half is down_proj
-        if phase == "gate|up" and (i + 1 == len(names) or "xwin_norm" in names[i + 1]) and tcx_in_phase:
-            labels[tcx_in_phase[-1]] = "down_proj"
-            tcx_in_phase = []
+        if phase == "gate|up" and (i + 1 == len(names) or "xwin_norm" in names[i + 1]) and proj_in_phase:
+            labels[proj_in_phase[-1]] = "down_proj"
+            proj_in_phase = []
             phase = "down"
     return labels
 

@@ -1,8 +1,8 @@
 // Decode projections for 1..64 clips: out[b][n] = x[b] . W[n, :], one kernel per weight matrix, the weights
-// streamed ONCE per launch. Three kernels share the streaming machinery and the epilogues:
-//   gemv_tc_kernel        1..4 clips, the activation vectors staged in shared memory
-//   gemv_tcw_kernel<NG>   5..16 clips, the activations streamed window by window next to the weights
-//   gemv_tcx_kernel       17..64 clips, gemv_tcw with the clips split across the consumer warps as well as K
+// streamed ONCE per launch. Two kernels share the streaming machinery and the epilogues:
+//   gemv_tc_kernel            1..4 clips, the activation vectors staged in shared memory
+//   gemv_tcw_kernel<NG, CG>   5..64 clips, the activations streamed window by window next to the weights, the
+//                             clips split into CG groups of 16 across the consumer warps (CG = 1, 2, 4)
 //
 // What bounds these kernels is how much of the time HBM is kept streaming:
 //   * a chain of per-matrix kernels keeps HBM busier with programmatic dependent launch (the next
@@ -15,7 +15,7 @@
 //   * the serial latency after griddepcontrol.wait (activation fetch + norm) is dead time for HBM
 //     once the ring is full, so it is kept to one L2 round trip.
 //
-// Common structure (one CTA per SM, at most one per 16-row group; 9 warps, 8 x 16 KB ring):
+// Common structure (one CTA per SM, at most one per 16-row group; 9 warps, a ring of 16 KB slots):
 //   warp 8      producer: walks this CTA's 16-row groups and 512-k chunks and fills the ring with one bulk
 //               copy per slot. Both kernels read a decode-only copy of the matrix that the weight loader
 //               lays out slot by slot (gemv_tc_repack_kernel): [16-row group][K chunk][32-wide K block]
@@ -32,7 +32,7 @@
 // optionally RMS-normalised, or gathered from the token-embedding table) and walk the ring group by group;
 // fp32 accumulators live across the K chunks of a row group, the per-warp partials meet after every group.
 //
-// gemv_tcw_kernel<NG> (5..16 clips):
+// gemv_tcw_kernel<NG, CG> (5..64 clips):
 //   * the activations no longer fit in shared memory next to the ring (16 x 11008 x 2 B = 352 KB for
 //     down_proj), so the K dimension is walked chunk-major: for every 512-wide K chunk the producer first
 //     copies that WINDOW of the (already normalised) activations and then the slots of that chunk for all
@@ -44,16 +44,22 @@
 //     loads of the 8 clips of an MMA bank-conflict free. Whoever produces an input of this kernel writes
 //     that layout: the decode-path RMSNorm (launch_xwin_norm), the decode attention kernel and this
 //     kernel's own SwiGLU epilogue.
-//   * the accumulators of ALL row groups of the CTA (up to NG = 14 groups x 2 column blocks x 4 registers
-//     per warp) stay in registers across the K chunks; the 8 per-warp partial tiles of a group meet once,
-//     at the end, in the (then idle) ring memory. A RES / LOGITS matrix with more row groups per SM (the
-//     lm_head) is streamed by consecutive launches over near-equal row slices.
+//   * the 8 consumer warps are CG clip groups of 16 (clip group cg = columns 16 cg .. 16 cg + 15 of the MMA B
+//     operand) x KP = 8 / CG K phases (warp kp of a group takes the 32-wide K blocks kp, kp + KP, ...): CG = 1
+//     for 5..16 clips, 2 for 17..32, 4 for 33..64. An A fragment is loaded by CG warps.
+//   * the accumulators of ALL row groups of the CTA (up to NG groups x 2 column blocks x 4 registers per warp)
+//     and the B fragments of the warp's K blocks stay in registers across the K chunks; the KP partial tiles of
+//     a group meet once, at the end, in the (then idle) shared memory. A 9-warp kernel has at most 168 registers
+//     per thread (3 warps share a sub-partition's 16K), so the largest instances without spills hold NG = 14 /
+//     10 / 6 row groups at CG = 1 / 2 / 4. A matrix with more row groups per SM is streamed by consecutive
+//     launches over near-equal row slices; r0 is the slice's first row (the weights and row scales of `a` start
+//     there, the epilogue addresses rows r0 + local row).
 //   * a warp per row group (no reduction at all) keeps a slot held for ~1000 cycles by its one consumer, so
 //     only a few of the ring slots are in flight; per-row window copies make the copy engine the limit.
 //
 // Weight formats (GemvArgs): both kernels are templates over the format of the slot-ordered copy.
 //   W_BF16  the bf16 copy above.
-//   W_FP8   E4M3 codes q in the SAME order, one byte per weight (a 512-k slot is 8 KB; the ring keeps its 128 KB
+//   W_FP8   E4M3 codes q in the SAME order, one byte per weight (a 512-k slot is 8 KB; the ring keeps its size
 //           and holds twice as many slots), plus a power-of-two scale 2^e per row (w_scale). The consumers turn
 //           the codes into exactly the bf16 A fragments of q (e4m3x2_bf16x2), issue the same MMAs in the same k
 //           order and warp split, and multiply each row's fp32 dot product, after the cross-warp sum, by 2^e.
@@ -93,15 +99,6 @@ constexpr int SLOTS = 8;                            // ring depth (gemv_tc: at m
 constexpr int TC_SMEM_ONE_CLIP = 160 * 1024;
 constexpr int TC_SMEM_CLIPS = 212 * 1024;
 
-constexpr int TW_XROW = XWIN_PITCH * 2;             // 1088 bytes per activation row of a window
-constexpr int TW_XBUF = 16 * TW_XROW;               // one window of 16 clips
-constexpr int TW_XWIN = 4;                          // activation windows in flight (power of two): with two, a
-                                                    // CTA that owns 1-2 row groups (o_proj, down_proj) waited
-                                                    // an L2 round trip for a window every second chunk
-constexpr int TW_SMEM = SLOTS * SLOT_BYTES + TW_XWIN * TW_XBUF + 256;
-constexpr int TW_TILE = 16 * 17;                    // floats of one partial tile (16 rows x 16 clips, padded rows)
-constexpr int TW_NG_MAX = 14;                       // row groups per CTA of the largest instance (18 would spill)
-
 // the ring of each weight format: bytes per weight, per slot, and slots in the same 128 KB
 constexpr int W_BF16 = 0, W_FP8 = 1;
 template <int FMT> struct Ring {
@@ -109,8 +106,24 @@ template <int FMT> struct Ring {
   static constexpr int SLOT = 16 * KC * EB;
   static constexpr int NSLOT = SLOTS * 2 / EB;
 };
-constexpr int TW_SMEM_FP8 = SLOTS * SLOT_BYTES + TW_XWIN * TW_XBUF + 512;   // 16 + 16 + 8 barriers
-template <int FMT> constexpr int tw_smem() { return FMT == W_FP8 ? TW_SMEM_FP8 : TW_SMEM; }
+
+// gemv_tcw: shared-memory plan of CG clip groups (not swept on the H100): a ring of RING bytes, NWIN activation
+// windows of 16 CG clips in flight, then the barriers (full / empty per slot and per window)
+//   CG = 1: 128 KB ring (8 bf16 / 16 fp8 slots), 4 windows of 16 clips. With two windows, a CTA that owns 1-2 row
+//           groups (o_proj, down_proj) waited an L2 round trip for a window every second chunk.
+//   CG = 2:  80 KB ring (5 / 10 slots), 4 windows of 32 clips
+//   CG = 4:  80 KB ring (5 / 10 slots), 2 windows of 64 clips
+constexpr int TW_XROW = XWIN_PITCH * 2;             // 1088 bytes per activation row of a window
+template <int CG, int FMT> struct TwPlan {
+  static constexpr int RING = (CG == 1 ? 8 : 5) * SLOT_BYTES;
+  static constexpr int NSLOT = RING / Ring<FMT>::SLOT;
+  static constexpr int NWIN = CG == 4 ? 2 : 4;      // a power of two
+  static constexpr int XBUF = 16 * CG * TW_XROW;
+  static constexpr int XAREA = NWIN * XBUF;
+  static constexpr int BARS = CG == 1 && FMT == W_BF16 ? 256 : 512;
+  static constexpr int SMEM = RING + XAREA + BARS;
+  static_assert(2 * (NSLOT + NWIN) * 8 <= BARS, "barriers");
+};
 
 struct TcParams {
   GemvArgs a;                       // a.B clips (1..4) are the columns of the MMA B operand
@@ -642,22 +655,28 @@ __global__ void __launch_bounds__(THREADS, 2) gemv_tc_kernel(const TcParams p) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// 5..16 clips. NG = upper bound of the row groups a CTA owns (the accumulator arrays are sized and
-// unrolled by it); a.x holds the activations in the xwin layout
+// 5..64 clips. NG = upper bound of the row groups a CTA owns (the accumulator arrays are sized and
+// unrolled by it), CG = clip groups of 16; a.x holds the activations in the xwin layout
 // ---------------------------------------------------------------------------------------------
-template <int NG, int FMT>
-__global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, const GemvEpilogue e) {
+template <int NG, int CG, int FMT>
+__global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, const GemvEpilogue e, const int r0) {
   using RG = Ring<FMT>;
+  using P = TwPlan<CG, FMT>;
+  constexpr int KP = CWARPS / CG;                     // K phases
+  constexpr int TPW = KC / 32 / KP;                   // 32-wide K blocks per warp and slot
+  constexpr int TP = 16 * CG + 1;                     // floats per row of a partial tile (padded rows)
+  static_assert((P::NWIN & (P::NWIN - 1)) == 0 && P::SMEM <= 227 * 1024, "window area");
+  static_assert(KP * NG * 16 * TP * 4 <= P::RING + P::XAREA, "partial tiles");
   extern __shared__ __align__(128) uint8_t smem[];
-  // layout: ring[RG::NSLOT] (128 KB; after the main loop: partial tiles [warp][group]) | x windows [4][16][1088 B]
-  //         | barriers
-  uint8_t* xs = smem + SLOTS * SLOT_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(xs + TW_XWIN * TW_XBUF);
+  // layout: ring[P::NSLOT] | x windows [NWIN][16 CG][1088 B] | barriers; after the main loop the partial tiles
+  // [kp][group][16][TP] fp32 take the ring and window memory
+  uint8_t* xs = smem + P::RING;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(xs + P::XAREA);
   const uint32_t ring0 = smem_u32(smem), xs0 = smem_u32(xs), bar0 = smem_u32(bars);
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
-  auto empty_bar = [&](int s) { return bar0 + 8u * (RG::NSLOT + s); };
-  auto xfull_bar = [&](int s) { return bar0 + 8u * (2 * RG::NSLOT + s); };
-  auto xempty_bar = [&](int s) { return bar0 + 8u * (2 * RG::NSLOT + TW_XWIN + s); };
+  auto empty_bar = [&](int s) { return bar0 + 8u * (P::NSLOT + s); };
+  auto xfull_bar = [&](int s) { return bar0 + 8u * (2 * P::NSLOT + s); };
+  auto xempty_bar = [&](int s) { return bar0 + 8u * (2 * P::NSLOT + P::NWIN + s); };
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int K = a.K, N = a.N, NB = a.B;
@@ -666,12 +685,12 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
   const int ng = cta_row_groups(N, grp_begin);        // 1..NG
 
   if (tid == 0) {
-    for (int s = 0; s < RG::NSLOT; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CWARPS); }
-    for (int s = 0; s < TW_XWIN; ++s) { mbar_init(xfull_bar(s), 1); mbar_init(xempty_bar(s), CWARPS); }
+    for (int s = 0; s < P::NSLOT; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CWARPS); }
+    for (int s = 0; s < P::NWIN; ++s) { mbar_init(xfull_bar(s), 1); mbar_init(xempty_bar(s), CWARPS); }
     mbar_fence_init();
   }
   // rows of the activation windows that no clip owns stay zero (their MMA columns are never stored)
-  for (int i = tid; i < TW_XWIN * TW_XBUF / 16; i += THREADS) reinterpret_cast<uint4*>(xs)[i] = make_uint4(0, 0, 0, 0);
+  for (int i = tid; i < P::XAREA / 16; i += THREADS) reinterpret_cast<uint4*>(xs)[i] = make_uint4(0, 0, 0, 0);
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   __syncthreads();
   pdl_launch_dependents();
@@ -682,7 +701,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
     // single-lane region and the uniform-datapath code around the bulk copies then faults)
     if (lane == 0) {
       const int total = ng * nkc;
-      const int pre = total < RG::NSLOT ? total : RG::NSLOT;
+      const int pre = total < P::NSLOT ? total : P::NSLOT;
       const uint8_t* W = weight_bytes<FMT>(a);
       // the weights never depend on the previous kernel: fill the ring before the dependency wait
       {
@@ -696,13 +715,13 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
         }
       }
       pdl_wait();
-      int idx = 0, slot = 0, use = 0;                 // slot = idx % SLOTS, use = idx / SLOTS
+      int idx = 0, slot = 0, use = 0;                 // slot = idx % NSLOT, use = idx / NSLOT
       const uint32_t win_bytes = (uint32_t)NB * TW_XROW;
       for (int kc = 0; kc < nkc; ++kc) {
-        const int xb = kc & (TW_XWIN - 1);
-        if (kc >= TW_XWIN) mbar_wait(xempty_bar(xb), (uint32_t)(((kc / TW_XWIN) - 1) & 1));
+        const int xb = kc & (P::NWIN - 1);
+        if (kc >= P::NWIN) mbar_wait(xempty_bar(xb), (uint32_t)(((kc / P::NWIN) - 1) & 1));
         mbar_arrive_expect_tx(xfull_bar(xb), win_bytes);
-        bulk_g2s(xs0 + xb * TW_XBUF, a.x + (size_t)kc * NB * XWIN_PITCH, win_bytes, xfull_bar(xb));
+        bulk_g2s(xs0 + xb * P::XBUF, a.x + (size_t)kc * NB * XWIN_PITCH, win_bytes, xfull_bar(xb));
         for (int lg = 0; lg < ng; ++lg) {
           if (idx >= pre) {
             const uint32_t bytes = (uint32_t)min(KC, K - kc * KC) * (16u * RG::EB);
@@ -712,7 +731,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
             bulk_g2s(ring0 + slot * RG::SLOT, src, bytes, full_bar(slot));
           }
           ++idx;
-          if (++slot == RG::NSLOT) { slot = 0; ++use; }
+          if (++slot == P::NSLOT) { slot = 0; ++use; }
         }
       }
     }
@@ -722,6 +741,8 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
   // =============================== consumers ===============================
   pdl_wait();                                           // the epilogue reads / overwrites tensors of earlier kernels
   const int g = lane >> 2, q = lane & 3;
+  // K phase and clip group of this warp (the compiler cannot prove warp < 8 here: CG = 1 spells out kp = warp)
+  const int kp = CG == 1 ? warp : warp % KP, cg = CG == 1 ? 0 : warp / KP;
   float acc[NG][2][4];
 #pragma unroll
   for (int i = 0; i < NG; ++i)
@@ -733,223 +754,12 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcw_kernel(const GemvArgs a, 
   int slot = 0;
   uint32_t par = 0;
   for (int kc = 0; kc < nkc; ++kc) {
-    const int xb = kc & (TW_XWIN - 1);
+    const int xb = kc & (P::NWIN - 1);
     const int kb_n = min(KC, K - kc * KC) >> 5;          // 32-wide K blocks in this chunk
-    mbar_wait(xfull_bar(xb), (uint32_t)((kc / TW_XWIN) & 1));
-    const uint8_t* xw = xs + xb * TW_XBUF;
-    // this warp's share of every slot of the chunk: K blocks warp and warp + 8; the B fragments (the
-    // activations of 16 clips for those K blocks) are the same for every row group: load them once
-    uint4 xq[2][2];
-#pragma unroll
-    for (int t = 0; t < 2; ++t)
-#pragma unroll
-      for (int j = 0; j < 2; ++j)
-        xq[t][j] = *reinterpret_cast<const uint4*>(xw + (8 * j + g) * TW_XROW + (warp + CWARPS * t) * 64 + q * 16);   // clip 8j+g
-#pragma unroll
-    for (int i = 0; i < NG; ++i) {
-      if (i < ng) {
-        mbar_wait(full_bar(slot), par);
-        const uint8_t* base = smem + slot * RG::SLOT;
-#pragma unroll
-        for (int t = 0; t < 2; ++t) {
-          const int kb = warp + CWARPS * t;
-          if (kb < kb_n) {
-            uint4 wa, wb;                                                                              // rows g, g + 8
-            load_a<FMT>(base, kb, lane, wa, wb);
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-              mma_bf16(acc[i][j], wa.x, wb.x, wa.y, wb.y, xq[t][j].x, xq[t][j].y);
-              mma_bf16(acc[i][j], wa.z, wb.z, wa.w, wb.w, xq[t][j].z, xq[t][j].w);
-            }
-          }
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty_bar(slot));
-        if (++slot == RG::NSLOT) { slot = 0; par ^= 1u; }
-      }
-    }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(xempty_bar(xb));
-  }
-
-  // ---------------- the 8 per-warp partial tiles of every group meet in the (now idle) ring ----------------
-  cbar();                                               // every warp has left the ring
-  float* tiles = reinterpret_cast<float*>(smem);        // [warp][group][16][17]
-#pragma unroll
-  for (int i = 0; i < NG; ++i) {
-    if (i < ng) {
-      float* t = tiles + ((size_t)warp * NG + i) * TW_TILE;
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        t[g * 17 + 8 * j + 2 * q] = acc[i][j][0];
-        t[g * 17 + 8 * j + 2 * q + 1] = acc[i][j][1];
-        t[(g + 8) * 17 + 8 * j + 2 * q] = acc[i][j][2];
-        t[(g + 8) * 17 + 8 * j + 2 * q + 1] = acc[i][j][3];
-      }
-    }
-  }
-  cbar();
-
-  // ---------------- fused epilogue ----------------
-  // All 256 consumer threads share the items of every group: thread = (row or row pair, clip) with the ROW
-  // index fastest, so that a warp's accesses to the residual / output rows are contiguous runs (a warp per
-  // group walking (row, clip) items with the clip fastest touched 32 sectors per instruction, one dependent
-  // round trip per 32 items at the end of every launch). The 8 partial tiles are summed on the fly,
-  // in a fixed order.
-  const int mode = e.mode;
-  const bool pairs = (mode == GEMV_SWIGLU || mode == GEMV_QKV);
-  auto tile_sum = [&](int lg, int el) {
-    float v = tiles[(size_t)lg * TW_TILE + el];
-#pragma unroll
-    for (int w2 = 1; w2 < CWARPS; ++w2) v += tiles[((size_t)w2 * NG + lg) * TW_TILE + el];
-    return v;
-  };
-  if (!pairs) {
-    const int rr = tid & 15, b = tid >> 4;               // 16 rows x 16 clips of one group per pass
-#pragma unroll 2
-    for (int lg = 0; lg < ng; ++lg) {
-      const int vrow = (grp_begin + lg) * 16 + rr;
-      if (b < NB && vrow < N) {
-        const float v0 = row_scaled<FMT>(a, vrow, tile_sum(lg, rr * 17 + b));
-        if (mode == GEMV_RES) epi_residual(e, b, vrow, v0);
-        else epi_logit(e, b, vrow, v0);
-      }
-    }
-  } else {
-    const int pr = tid & 7, b = (tid >> 3) & 15;         // 8 row pairs x 16 clips of TWO groups per pass
-    int col = 0, floor = 0;                              // q|k|v: clip b's column and key floor, loaded once
-    if (mode == GEMV_QKV && b < NB) { col = decode_col(e, b); floor = __ldg(e.n_pad + b); }
-    for (int lg = tid >> 7; lg < ng; lg += 2) {
-      const int rr = 2 * pr;
-      const int vrow = (grp_begin + lg) * 16 + rr;
-      if (b >= NB || vrow >= N) continue;
-      const float v0 = row_scaled<FMT>(a, vrow, tile_sum(lg, rr * 17 + b));
-      const float v1 = row_scaled<FMT>(a, vrow + 1, tile_sum(lg, (rr + 1) * 17 + b));
-      if (mode == GEMV_SWIGLU) epi_swiglu(e, b, vrow, NB, v0, v1);
-      else epi_qkv_rope(e, b, vrow, col, floor, v0, v1);
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// 17..64 clips: gemv_tcw_kernel with the clips split across the consumer warps as well as K. The 8 consumer
-// warps are CG clip groups of 16 (clip group cg = columns 16 cg .. 16 cg + 15 of the MMA B operand) x KP = 8 / CG
-// K phases (warp kp of a group takes the 32-wide K blocks kp, kp + KP, ...): CG = 2 for 17..32 clips, 4 for
-// 33..64. Each warp keeps the accumulators of its 16 clips for all NG row groups (the register budget of
-// gemv_tcw<NG>) and the B fragments of its K blocks (TPW x 8 registers) for the whole chunk; an A fragment is
-// loaded by CG warps. A 9-warp kernel has at most 168 registers per thread (3 warps share a sub-partition's
-// 16K), so the largest instance without spills is NG = 10 at CG = 2 and NG = 6 at CG = 4.
-// The same producer, slot-ordered weight copy, xwin windows (now of up to 64 clips) and epilogues as gemv_tcw.
-// Shared memory: an 80 KB ring (5 bf16 / 10 fp8 slots) and 136 KB of windows (4 of 32 clips or 2 of 64); the
-// KP partial tiles [kp][group][16][16 CG + 1] fp32 meet in the idle ring + window memory at the end (at most
-// 84 KB). Every matrix runs in row slices of at most NG groups per CTA; r0 is the slice's first row
-// (the weights and row scales of `a` start there, the epilogue addresses rows r0 + local row).
-// ---------------------------------------------------------------------------------------------
-constexpr int TX_RING = 5 * SLOT_BYTES;
-constexpr int TX_XAREA = 8 * 16 * TW_XROW;
-constexpr int TX_SMEM = TX_RING + TX_XAREA + 512;   // + barriers (at most 2 x 10 slots + 2 x 4 windows)
-template <int FMT> struct RingX {
-  static constexpr int EB = FMT == W_FP8 ? 1 : 2;
-  static constexpr int SLOT = 16 * KC * EB;
-  static constexpr int NSLOT = TX_RING / SLOT;
-};
-
-template <int NG, int CG, int FMT>
-__global__ void __launch_bounds__(THREADS, 1) gemv_tcx_kernel(const GemvArgs a, const GemvEpilogue e, const int r0) {
-  using RG = RingX<FMT>;
-  constexpr int KP = CWARPS / CG;                     // K phases
-  constexpr int TPW = KC / 32 / KP;                   // 32-wide K blocks per warp and slot
-  constexpr int NWIN = 8 / CG;                        // activation windows in flight (power of two)
-  constexpr int XBUF = 16 * CG * TW_XROW;             // one window of 16 CG clips
-  constexpr int TP = 16 * CG + 1;                     // floats per row of a partial tile
-  static_assert(NWIN * XBUF == TX_XAREA, "window area");
-  static_assert(KP * NG * 16 * TP * 4 <= TX_RING + TX_XAREA, "partial tiles");
-  extern __shared__ __align__(128) uint8_t smem[];
-  uint8_t* xs = smem + TX_RING;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(xs + TX_XAREA);
-  const uint32_t ring0 = smem_u32(smem), xs0 = smem_u32(xs), bar0 = smem_u32(bars);
-  auto full_bar = [&](int s) { return bar0 + 8u * s; };
-  auto empty_bar = [&](int s) { return bar0 + 8u * (RG::NSLOT + s); };
-  auto xfull_bar = [&](int s) { return bar0 + 8u * (2 * RG::NSLOT + s); };
-  auto xempty_bar = [&](int s) { return bar0 + 8u * (2 * RG::NSLOT + NWIN + s); };
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int K = a.K, N = a.N, NB = a.B;
-  const int nkc = (K + KC - 1) / KC;
-  int grp_begin;
-  const int ng = cta_row_groups(N, grp_begin);        // 1..NG
-
-  if (tid == 0) {
-    for (int s = 0; s < RG::NSLOT; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CWARPS); }
-    for (int s = 0; s < NWIN; ++s) { mbar_init(xfull_bar(s), 1); mbar_init(xempty_bar(s), CWARPS); }
-    mbar_fence_init();
-  }
-  // rows of the activation windows that no clip owns stay zero (their MMA columns are never stored)
-  for (int i = tid; i < TX_XAREA / 16; i += THREADS) reinterpret_cast<uint4*>(xs)[i] = make_uint4(0, 0, 0, 0);
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  __syncthreads();
-  pdl_launch_dependents();
-
-  if (warp == CWARPS) {
-    // =============================== producer (gemv_tcw's) ===============================
-    if (lane == 0) {
-      const int total = ng * nkc;
-      const int pre = total < RG::NSLOT ? total : RG::NSLOT;
-      const uint8_t* W = weight_bytes<FMT>(a);
-      {
-        int kc = 0, lg = 0;
-        for (int idx = 0; idx < pre; ++idx) {
-          const uint32_t bytes = (uint32_t)min(KC, K - kc * KC) * (16u * RG::EB);
-          const uint8_t* src = W + ((size_t)(grp_begin + lg) * 16 * K + (size_t)kc * KC * 16) * RG::EB;
-          mbar_arrive_expect_tx(full_bar(idx), bytes);
-          bulk_g2s(ring0 + idx * RG::SLOT, src, bytes, full_bar(idx));
-          if (++lg == ng) { lg = 0; ++kc; }
-        }
-      }
-      pdl_wait();
-      int idx = 0, slot = 0, use = 0;
-      const uint32_t win_bytes = (uint32_t)NB * TW_XROW;
-      for (int kc = 0; kc < nkc; ++kc) {
-        const int xb = kc & (NWIN - 1);
-        if (kc >= NWIN) mbar_wait(xempty_bar(xb), (uint32_t)(((kc / NWIN) - 1) & 1));
-        mbar_arrive_expect_tx(xfull_bar(xb), win_bytes);
-        bulk_g2s(xs0 + xb * XBUF, a.x + (size_t)kc * NB * XWIN_PITCH, win_bytes, xfull_bar(xb));
-        for (int lg = 0; lg < ng; ++lg) {
-          if (idx >= pre) {
-            const uint32_t bytes = (uint32_t)min(KC, K - kc * KC) * (16u * RG::EB);
-            const uint8_t* src = W + ((size_t)(grp_begin + lg) * 16 * K + (size_t)kc * KC * 16) * RG::EB;
-            mbar_wait(empty_bar(slot), (uint32_t)((use - 1) & 1));
-            mbar_arrive_expect_tx(full_bar(slot), bytes);
-            bulk_g2s(ring0 + slot * RG::SLOT, src, bytes, full_bar(slot));
-          }
-          ++idx;
-          if (++slot == RG::NSLOT) { slot = 0; ++use; }
-        }
-      }
-    }
-    return;
-  }
-
-  // =============================== consumers ===============================
-  pdl_wait();
-  const int g = lane >> 2, q = lane & 3;
-  const int kp = warp % KP, cg = warp / KP;
-  float acc[NG][2][4];
-#pragma unroll
-  for (int i = 0; i < NG; ++i)
-#pragma unroll
-    for (int j = 0; j < 2; ++j)
-#pragma unroll
-      for (int r = 0; r < 4; ++r) acc[i][j][r] = 0.f;
-
-  int slot = 0;
-  uint32_t par = 0;
-  for (int kc = 0; kc < nkc; ++kc) {
-    const int xb = kc & (NWIN - 1);
-    const int kb_n = min(KC, K - kc * KC) >> 5;
-    mbar_wait(xfull_bar(xb), (uint32_t)((kc / NWIN) & 1));
-    const uint8_t* xw = xs + xb * XBUF;
-    // the B fragments of this warp's 16 clips and K blocks, the same for every row group
+    mbar_wait(xfull_bar(xb), (uint32_t)((kc / P::NWIN) & 1));
+    const uint8_t* xw = xs + xb * P::XBUF;
+    // this warp's share of every slot of the chunk: K blocks kp, kp + KP, ...; the B fragments (the activations
+    // of its 16 clips for those K blocks) are the same for every row group: load them once
     uint4 xq[TPW][2];
 #pragma unroll
     for (int t = 0; t < TPW; ++t)
@@ -965,7 +775,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcx_kernel(const GemvArgs a, 
         for (int t = 0; t < TPW; ++t) {
           const int kb = kp + KP * t;
           if (kb < kb_n) {
-            uint4 wa, wb;
+            uint4 wa, wb;                                                                              // rows g, g + 8
             load_a<FMT>(base, kb, lane, wa, wb);
 #pragma unroll
             for (int j = 0; j < 2; ++j) {
@@ -976,7 +786,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcx_kernel(const GemvArgs a, 
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(empty_bar(slot));
-        if (++slot == RG::NSLOT) { slot = 0; par ^= 1u; }
+        if (++slot == P::NSLOT) { slot = 0; par ^= 1u; }
       }
     }
     __syncwarp();
@@ -984,7 +794,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcx_kernel(const GemvArgs a, 
   }
 
   // ---------------- the KP partial tiles of every group and clip meet in the (now idle) shared memory ----------------
-  cbar();
+  cbar();                                               // every warp has left the ring and the windows
   float* tiles = reinterpret_cast<float*>(smem);        // [kp][group][16][TP]
 #pragma unroll
   for (int i = 0; i < NG; ++i) {
@@ -1001,7 +811,12 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcx_kernel(const GemvArgs a, 
   }
   cbar();
 
-  // ---------------- fused epilogue (gemv_tcw's item order, one pass per clip group) ----------------
+  // ---------------- fused epilogue ----------------
+  // All 256 consumer threads share the items of every group, one pass per clip group: thread = (row or row pair,
+  // clip) with the ROW index fastest, so that a warp's accesses to the residual / output rows are contiguous runs
+  // (a warp per group walking (row, clip) items with the clip fastest touched 32 sectors per instruction, one
+  // dependent round trip per 32 items at the end of every launch). The KP partial tiles are summed on the fly,
+  // in a fixed order.
   const int mode = e.mode;
   const bool pairs = (mode == GEMV_SWIGLU || mode == GEMV_QKV);
   auto tile_sum = [&](int lg, int el) {
@@ -1011,7 +826,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcx_kernel(const GemvArgs a, 
     return v;
   };
   if (!pairs) {
-    const int rr = tid & 15;
+    const int rr = tid & 15;                             // 16 rows x 16 clips of one group per pass
     for (int bb = 0; bb < CG; ++bb) {
       const int b = 16 * bb + (tid >> 4);
 #pragma unroll 2
@@ -1025,10 +840,10 @@ __global__ void __launch_bounds__(THREADS, 1) gemv_tcx_kernel(const GemvArgs a, 
       }
     }
   } else {
-    const int pr = tid & 7;
+    const int pr = tid & 7;                              // 8 row pairs x 16 clips of TWO groups per pass
     for (int bb = 0; bb < CG; ++bb) {
       const int b = 16 * bb + ((tid >> 3) & 15);
-      int col = 0, floor = 0;
+      int col = 0, floor = 0;                            // q|k|v: clip b's column and key floor, loaded once
       if (mode == GEMV_QKV && b < NB) { col = decode_col(e, b); floor = __ldg(e.n_pad + b); }
       for (int lg = tid >> 7; lg < ng; lg += 2) {
         const int rr = 2 * pr;
@@ -1220,72 +1035,32 @@ int launch_tc(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
   return 0;
 }
 
-typedef void (*TcwKernel)(const GemvArgs, const GemvEpilogue);
-const TcwKernel tcw_bf16[4] = {gemv_tcw_kernel<2, W_BF16>, gemv_tcw_kernel<6, W_BF16>, gemv_tcw_kernel<10, W_BF16>,
-                               gemv_tcw_kernel<TW_NG_MAX, W_BF16>};
-const TcwKernel tcw_fp8[4] = {gemv_tcw_kernel<2, W_FP8>, gemv_tcw_kernel<6, W_FP8>, gemv_tcw_kernel<10, W_FP8>,
-                              gemv_tcw_kernel<TW_NG_MAX, W_FP8>};
+typedef void (*TcwKernel)(const GemvArgs, const GemvEpilogue, const int);
+struct TcwInstance { TcwKernel kern; int ng, smem; };
+template <int NG, int CG, int FMT> TcwInstance tcw() { return {gemv_tcw_kernel<NG, CG, FMT>, NG, TwPlan<CG, FMT>::SMEM}; }
+// [format][CG = 1, 2, 4][instance], NG ascending (unused entries: ng = 0); the largest NG of a CG is the largest
+// instance without spills
+const TcwInstance tcw_kernels[2][3][4] = {
+    {{tcw<2, 1, W_BF16>(), tcw<6, 1, W_BF16>(), tcw<10, 1, W_BF16>(), tcw<14, 1, W_BF16>()},
+     {tcw<2, 2, W_BF16>(), tcw<6, 2, W_BF16>(), tcw<10, 2, W_BF16>()},
+     {tcw<2, 4, W_BF16>(), tcw<4, 4, W_BF16>(), tcw<6, 4, W_BF16>()}},
+    {{tcw<2, 1, W_FP8>(), tcw<6, 1, W_FP8>(), tcw<10, 1, W_FP8>(), tcw<14, 1, W_FP8>()},
+     {tcw<2, 2, W_FP8>(), tcw<6, 2, W_FP8>(), tcw<10, 2, W_FP8>()},
+     {tcw<2, 4, W_FP8>(), tcw<4, 4, W_FP8>(), tcw<6, 4, W_FP8>()}}};
 
-// RES / LOGITS over more than 14 row groups per SM (the lm_head): consecutive launches over near-equal
-// row slices
+// 5..64 clips: a matrix with more row groups per SM than the largest instance of its CG takes runs as consecutive
+// launches over near-equal row slices; the epilogue addresses rows by their index in the whole matrix
 int launch_tcw(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
   VCL_REQUIRE(a.norm_w == nullptr && a.embed == nullptr && a.amax_out == nullptr,
-              "gemv: the 5..16-clip kernel takes normalised activations (no fused norm, embedding gather or "
+              "gemv: the 5..64-clip kernel takes normalised activations (no fused norm, embedding gather or "
               "arg-max partials)");
   VCL_REQUIRE((uintptr_t)a.x % 16 == 0, "gemv_tcw: operands must be 16-byte aligned");
   const int fmt = weight_format(a);
   if (fmt < 0) return fmt;
+  const TcwInstance* inst = tcw_kernels[fmt][a.B <= 16 ? 0 : a.B <= 32 ? 1 : 2];   // 1, 2 or 4 clip groups of 16
+  int ng_cap = 0;
+  for (int i = 0; i < 4; ++i) ng_cap = inst[i].ng > ng_cap ? inst[i].ng : ng_cap;
   const int groups = (a.N + 15) / 16, sms = device_num_sms();
-  const int n_slices = (groups + TW_NG_MAX * sms - 1) / (TW_NG_MAX * sms);
-  for (int s = 0; s < n_slices; ++s) {
-    const int g0 = (int)((long long)groups * s / n_slices), g1 = (int)((long long)groups * (s + 1) / n_slices);
-    const long long r0 = (long long)g0 * 16;
-    GemvArgs sa = a;
-    GemvEpilogue se = e;
-    if (fmt == W_FP8) {
-      sa.W_fp8 = a.W_fp8 + r0 * a.K;
-      sa.w_scale = a.w_scale + r0;
-    } else {
-      sa.W_tiled = a.W_tiled + r0 * a.K;
-    }
-    sa.N = (a.N < g1 * 16 ? a.N : g1 * 16) - (int)r0;
-    if (se.out != nullptr) se.out += r0;
-    if (se.res != nullptr) se.res += r0;
-    if (se.logits != nullptr) se.logits += r0;
-    const int grid = g1 - g0 < sms ? g1 - g0 : sms;                   // no CTA without a row group
-    cudaLaunchAttribute attr[1];
-    cudaLaunchConfig_t cfg = pdl_config(grid, fmt == W_FP8 ? tw_smem<W_FP8>() : tw_smem<W_BF16>(), stream, attr);
-    const int ng_max = (g1 - g0 + grid - 1) / grid;                  // groups of the busiest CTA
-    const int pick = ng_max <= 2 ? 0 : ng_max <= 6 ? 1 : ng_max <= 10 ? 2 : 3;
-    auto kern = fmt == W_FP8 ? tcw_fp8[pick] : tcw_bf16[pick];
-    VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, sa, se));
-    count_launches(1);
-  }
-  return 0;
-}
-
-typedef void (*TcxKernel)(const GemvArgs, const GemvEpilogue, const int);
-const TcxKernel tcx_bf16[2][3] = {
-    {gemv_tcx_kernel<2, 2, W_BF16>, gemv_tcx_kernel<6, 2, W_BF16>, gemv_tcx_kernel<10, 2, W_BF16>},
-    {gemv_tcx_kernel<2, 4, W_BF16>, gemv_tcx_kernel<4, 4, W_BF16>, gemv_tcx_kernel<6, 4, W_BF16>}};
-const TcxKernel tcx_fp8[2][3] = {
-    {gemv_tcx_kernel<2, 2, W_FP8>, gemv_tcx_kernel<6, 2, W_FP8>, gemv_tcx_kernel<10, 2, W_FP8>},
-    {gemv_tcx_kernel<2, 4, W_FP8>, gemv_tcx_kernel<4, 4, W_FP8>, gemv_tcx_kernel<6, 4, W_FP8>}};
-const int tcx_ng[2][3] = {{2, 6, 10}, {2, 4, 6}};
-
-// 17..64 clips: a matrix with more row groups per SM than the largest instance takes (10 groups at 17..32 clips,
-// 6 at 33..64) runs as consecutive launches over near-equal row slices; the epilogue addresses rows by their
-// index in the whole matrix
-int launch_tcx(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
-  VCL_REQUIRE(a.norm_w == nullptr && a.embed == nullptr && a.amax_out == nullptr,
-              "gemv: the 17..64-clip kernel takes normalised activations (no fused norm, embedding gather or "
-              "arg-max partials)");
-  VCL_REQUIRE((uintptr_t)a.x % 16 == 0, "gemv_tcx: operands must be 16-byte aligned");
-  const int fmt = weight_format(a);
-  if (fmt < 0) return fmt;
-  const int cgi = a.B <= 32 ? 0 : 1;                                  // 2 or 4 clip groups of 16
-  const int groups = (a.N + 15) / 16, sms = device_num_sms();
-  const int ng_cap = tcx_ng[cgi][2];
   const int n_slices = (groups + ng_cap * sms - 1) / (ng_cap * sms);
   for (int s = 0; s < n_slices; ++s) {
     const int g0 = (int)((long long)groups * s / n_slices), g1 = (int)((long long)groups * (s + 1) / n_slices);
@@ -1298,13 +1073,13 @@ int launch_tcx(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
       sa.W_tiled = a.W_tiled + r0 * a.K;
     }
     sa.N = (a.N < g1 * 16 ? a.N : g1 * 16) - (int)r0;
-    const int grid = g1 - g0 < sms ? g1 - g0 : sms;
+    const int grid = g1 - g0 < sms ? g1 - g0 : sms;                   // no CTA without a row group
+    const int ng_max = (g1 - g0 + grid - 1) / grid;                  // groups of the busiest CTA
+    int pick = 0;
+    while (inst[pick].ng < ng_max) ++pick;
     cudaLaunchAttribute attr[1];
-    cudaLaunchConfig_t cfg = pdl_config(grid, TX_SMEM, stream, attr);
-    const int ng_max = (g1 - g0 + grid - 1) / grid;
-    const int pick = ng_max <= tcx_ng[cgi][0] ? 0 : ng_max <= tcx_ng[cgi][1] ? 1 : 2;
-    auto kern = fmt == W_FP8 ? tcx_fp8[cgi][pick] : tcx_bf16[cgi][pick];
-    VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, sa, e, (int)r0));
+    cudaLaunchConfig_t cfg = pdl_config(grid, inst[pick].smem, stream, attr);
+    VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, inst[pick].kern, sa, e, (int)r0));
     count_launches(1);
   }
   return 0;
@@ -1329,15 +1104,10 @@ extern "C" int vcl_debug_tc_trace_dump(const char* path) {
 int init_gemv_kernels() {
   for (auto k : {gemv_tc_kernel<W_BF16>, gemv_tc_kernel<W_FP8>})
     VCL_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-  for (int i = 0; i < 4; ++i) {
-    VCL_CUDA_OK(cudaFuncSetAttribute(tcw_bf16[i], cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM));
-    VCL_CUDA_OK(cudaFuncSetAttribute(tcw_fp8[i], cudaFuncAttributeMaxDynamicSharedMemorySize, TW_SMEM_FP8));
-  }
-  for (int c = 0; c < 2; ++c)
-    for (int i = 0; i < 3; ++i) {
-      VCL_CUDA_OK(cudaFuncSetAttribute(tcx_bf16[c][i], cudaFuncAttributeMaxDynamicSharedMemorySize, TX_SMEM));
-      VCL_CUDA_OK(cudaFuncSetAttribute(tcx_fp8[c][i], cudaFuncAttributeMaxDynamicSharedMemorySize, TX_SMEM));
-    }
+  for (const auto& by_fmt : tcw_kernels)
+    for (const auto& by_cg : by_fmt)
+      for (const TcwInstance& k : by_cg)
+        if (k.kern != nullptr) VCL_CUDA_OK(cudaFuncSetAttribute(k.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, k.smem));
   return 0;
 }
 
@@ -1347,10 +1117,9 @@ int gemv_grid(int N) {
   return n_groups < sms ? n_groups : sms;
 }
 
-bool gemv_fits(int B, int N, int K, bool norm, bool pairs, bool fp8) {
+bool gemv_fits(int B, int N, int K, bool norm, bool fp8) {
   if (B < 1 || B > 64 || N < 1) return false;
-  if (B > 16) return K % 32 == 0;             // 17..64 clips: any matrix, in row slices
-  if (B > 4) return K % 32 == 0 && (!pairs || (N + 15) / 16 <= TW_NG_MAX * device_num_sms());
+  if (B > 4) return K % 32 == 0;              // 5..64 clips: any matrix, in row slices
   size_t smem = 0; int xe = 0, rc = 0;
   return plan(B, N, K, norm, gemv_grid(N), &smem, &xe, &rc, fp8 ? W_FP8 : W_BF16) >= 4;
 }
@@ -1379,19 +1148,17 @@ int launch_gemv_quantize_fp8(const bf16* W, bf16* w_deq, uint8_t* codes, float* 
 }
 
 int launch_gemv(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream) {
-  const bool pairs = e.mode == GEMV_SWIGLU || e.mode == GEMV_QKV;
   VCL_REQUIRE(e.mode >= GEMV_RES && e.mode <= GEMV_LOGITS, "gemv: unknown epilogue mode %d", e.mode);
-  VCL_REQUIRE(gemv_fits(a.B, a.N, a.K, a.norm_w != nullptr, pairs, a.W_fp8 != nullptr),
+  VCL_REQUIRE(gemv_fits(a.B, a.N, a.K, a.norm_w != nullptr, a.W_fp8 != nullptr),
               "gemv: B=%d N=%d K=%d is outside the decode kernels' range (1..64 clips, K a multiple of 32; "
-              "1..4 clips: K <= 14336 and the shared-memory plan; 5..16 clips: q|k|v and gate|up at most 14 "
-              "row groups of 16 per SM)", a.B, a.N, a.K);
+              "1..4 clips: K <= 14336 and the shared-memory plan)", a.B, a.N, a.K);
   VCL_REQUIRE(e.mode != GEMV_SWIGLU || a.N % 2 == 0, "gemv swiglu: N must be even (interleaved gate/up rows)");
   VCL_REQUIRE(e.mode != GEMV_QKV || a.N == 3 * e.H * 128, "gemv qkv: N=%d != 3*H*128", a.N);
   VCL_REQUIRE((e.n_pad != nullptr) == (e.mode == GEMV_QKV),
               "gemv: the q|k|v epilogue needs the key floors n_pad, and no other epilogue takes them");
   VCL_REQUIRE(a.embed == nullptr || (a.vocab > 0 && (a.tok_in != nullptr || (a.amax_in != nullptr && a.amax_n > 0))),
               "gemv: the fused embedding gather needs a token source");
-  return a.B <= 4 ? launch_tc(a, e, stream) : a.B <= 16 ? launch_tcw(a, e, stream) : launch_tcx(a, e, stream);
+  return a.B <= 4 ? launch_tc(a, e, stream) : launch_tcw(a, e, stream);
 }
 
 }  // namespace vcl

@@ -182,10 +182,10 @@ int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, c
                             const int* n_pad);
 
 // ---- decode_gemv.cu : decode-time weight streaming (1..64 new tokens) -------------------------------
-// Three ring kernels (bulk-copy ring over a slot-ordered copy of the matrix + mma.sync) behind one launcher:
+// Two ring kernels (bulk-copy ring over a slot-ordered copy of the matrix + mma.sync) behind one launcher:
 // 1..4 clips stage the activation vectors in shared memory (K <= 14336, optional fused RMSNorm and, for
-// q|k|v, a fused token-embedding gather); 5..16 and 17..64 clips read activations that are already normalised
-// and stored window-major ("xwin", below). All three read the copy that launch_gemv_repack builds, or its fp8 twin from
+// q|k|v, a fused token-embedding gather); 5..64 clips read activations that are already normalised
+// and stored window-major ("xwin", below). Both read the copy that launch_gemv_repack builds, or its fp8 twin from
 // launch_gemv_quantize_fp8 (E4M3 codes in the same order plus a power-of-two scale per row; decode_gemv.cu).
 // per-CTA partial arg-max of the logits kernel: the next step's q|k|v kernel reduces the grid's
 // partials itself (lowest index wins ties), so no arg-max kernel runs between two decode steps
@@ -243,10 +243,9 @@ int launch_xwin_norm(const bf16* x, long long ldx, bf16* y, const bf16* w, int B
 
 int init_gemv_kernels();
 // whether a [N, K] projection of B clips has a decode kernel. norm: with the fused RMSNorm (1..4 clips);
-// pairs: a SWIGLU or QKV epilogue (5..16 clips: such a matrix has at most 14 row groups of 16 per SM; 17..64
-// clips take any matrix whose K is a multiple of 32); fp8: the
-// kernels of fp8 weights (their shared-memory plan; they take every shape the bf16 kernels take)
-bool gemv_fits(int B, int N, int K, bool norm, bool pairs, bool fp8 = false);
+// 5..64 clips take any matrix whose K is a multiple of 32; fp8: the kernels of fp8 weights (their shared-memory
+// plan; they take every shape the bf16 kernels take)
+bool gemv_fits(int B, int N, int K, bool norm, bool fp8 = false);
 int gemv_grid(int N);                         // CTAs of a 1..4-clip launch over N rows
 size_t gemv_tiled_elems(int N, int K);        // elements of the slot-ordered copy of an [N, K] matrix
 // qkv_pairs: rows are taken in the order of the fused q/k/v epilogue (RoPE pairs adjacent)
@@ -258,9 +257,8 @@ int launch_gemv_repack(const bf16* W, bf16* dst, int N, int K, bool qkv_pairs, c
 // not a normal fp32 number.
 int launch_gemv_quantize_fp8(const bf16* W, bf16* w_deq, uint8_t* codes, float* scales, int N, int K, bool qkv_pairs,
                              int* bad, cudaStream_t stream);
-// 1..4 clips: gemv_tc_kernel; 5..16 clips: gemv_tcw_kernel (several launches over row slices when a RES /
-// LOGITS matrix has more than 14 row groups per SM); 17..64 clips: gemv_tcx_kernel (row slices of at most 10 / 6
-// row groups per SM at 17..32 / 33..64 clips, for every epilogue)
+// 1..4 clips: gemv_tc_kernel; 5..64 clips: gemv_tcw_kernel with 1 / 2 / 4 clip groups at 5..16 / 17..32 / 33..64
+// clips (row slices of at most 14 / 10 / 6 row groups per SM, for every epilogue)
 int launch_gemv(const GemvArgs& a, const GemvEpilogue& e, cudaStream_t stream);
 
 }  // namespace vcl

@@ -322,15 +322,14 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   {
     // every decode projection must have a kernel for every clip count up to 64 (beyond: the GEMM)
     const int D = c->llm_hidden, F = c->llm_inter;
-    const struct { const char* name; int N, K; bool norm, pairs; } mats[5] = {
-        {"q|k|v", 3 * D, D, true, true}, {"o_proj", D, D, false, false}, {"gate|up", 2 * F, D, true, true},
-        {"down_proj", D, F, false, false}, {"lm_head", c->vocab, D, true, false}};
+    const struct { const char* name; int N, K; bool norm; } mats[5] = {
+        {"q|k|v", 3 * D, D, true}, {"o_proj", D, D, false}, {"gate|up", 2 * F, D, true},
+        {"down_proj", D, F, false}, {"lm_head", c->vocab, D, true}};
     for (int B = 1; B <= c->max_batch && B <= 64; ++B)
       for (const auto& m : mats)
-        VCL_REQUIRE(gemv_fits(B, m.N, m.K, m.norm, m.pairs),
+        VCL_REQUIRE(gemv_fits(B, m.N, m.K, m.norm),
                     "vcl_create: the %s projection [%d x %d] has no decode kernel for %d clips (1..4 clips: K <= 14336 "
-                    "and the shared-memory plan; 5..16 clips: q|k|v and gate|up at most 14 row groups of 16 per SM)",
-                    m.name, m.N, m.K, B);
+                    "and the shared-memory plan)", m.name, m.N, m.K, B);
   }
 
   vcl_handle* h = new vcl_handle();
@@ -475,12 +474,12 @@ int vcl_load_llm_weights_ex(vcl_handle* h, const vcl_tensor* tensors, int n, int
     // the fp8 decode kernels take every shape the bf16 ones take (vcl_create checked those)
     const vcl_config& c = h->cfg;
     const int D = c.llm_hidden, F = c.llm_inter;
-    const struct { const char* name; int N, K; bool norm, pairs; } mats[5] = {
-        {"q|k|v", 3 * D, D, true, true}, {"o_proj", D, D, false, false}, {"gate|up", 2 * F, D, true, true},
-        {"down_proj", D, F, false, false}, {"lm_head", c.vocab, D, true, false}};
+    const struct { const char* name; int N, K; bool norm; } mats[5] = {
+        {"q|k|v", 3 * D, D, true}, {"o_proj", D, D, false}, {"gate|up", 2 * F, D, true},
+        {"down_proj", D, F, false}, {"lm_head", c.vocab, D, true}};
     for (int B = 1; B <= c.max_batch && B <= 64; ++B)
       for (const auto& mt : mats)
-        VCL_REQUIRE(gemv_fits(B, mt.N, mt.K, mt.norm, mt.pairs, true),
+        VCL_REQUIRE(gemv_fits(B, mt.N, mt.K, mt.norm, true),
                     "vcl_load_llm_weights: the %s projection [%d x %d] has no fp8 decode kernel for %d clips", mt.name,
                     mt.N, mt.K, B);
   }
@@ -1352,7 +1351,7 @@ int vcl_op_gemv(const void* x, const void* W, void* out, const void* res, const 
                 float eps, int B, int N, int K, void* stream) {
   if (check_device() != 0) return -2;
   VCL_REQUIRE(B >= 1 && B <= 64, "vcl_op_gemv: B=%d outside 1..64 (more rows take the GEMM)", B);
-  VCL_REQUIRE(gemv_fits(B, N, K, norm_w != nullptr, false),
+  VCL_REQUIRE(gemv_fits(B, N, K, norm_w != nullptr),
               "vcl_op_gemv: B=%d N=%d K=%d is outside the decode kernels' range", B, N, K);
   static bool inited = false;
   if (!inited) {
@@ -1391,7 +1390,7 @@ int vcl_op_gemv_fp8(const void* x, const void* W, void* out, const void* res, co
                     float eps, int B, int N, int K, void* stream) {
   if (check_device() != 0) return -2;
   VCL_REQUIRE(B >= 1 && B <= 64, "vcl_op_gemv_fp8: B=%d outside 1..64 (more rows take the GEMM)", B);
-  VCL_REQUIRE(gemv_fits(B, N, K, norm_w != nullptr, false, true),
+  VCL_REQUIRE(gemv_fits(B, N, K, norm_w != nullptr, true),
               "vcl_op_gemv_fp8: B=%d N=%d K=%d is outside the decode kernels' range", B, N, K);
   static bool inited = false;
   if (!inited) {
