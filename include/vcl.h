@@ -73,6 +73,9 @@ typedef struct vcl_config {
   int32_t max_slots;     /* in-flight cache slots (vcl_llm_slot_*): 0 = min(max_batch, 16); otherwise
                             1 .. min(max_batch, 64), anything else is rejected by vcl_create. A capacity
                             only: the decode kernel is chosen by the clip count of each call */
+  int32_t kv_blocks;     /* 0: the contiguous KV cache, [layer][max_batch][head][max_seq][128] for K and for V.
+                            > 0: a PAGED cache of kv_blocks blocks instead (vcl_llm_set_block_table); at least 2,
+                            block 0 being the park block. A paged handle serves the slot entry points only */
 } vcl_config;
 
 /* A named tensor in the layout of the HF/reference state_dict (row-major, bf16, on the device).
@@ -288,6 +291,34 @@ int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* 
 int vcl_llm_set_sampling(vcl_handle* h, int n, const int32_t* clips_host, const float* temperature_host,
                          const int32_t* top_k_host, const uint64_t* seed_host, void* stream);
 
+/* Paged KV cache (vcl_config.kv_blocks > 0). The cache is a pool of kv_blocks BLOCKS. A block holds 128 cache columns
+ * of one sequence across all layers, [layer][K = 0 | V = 1][head][128 columns][128 dims] bf16 (2 * llm_layers *
+ * llm_heads * 32 KiB: 64 MiB at 7B, 100 MiB at 13B), one contiguous range. The BLOCK TABLE, int32
+ * [n_slots][ceil(max_seq / 128)] with n_slots the slot count (max_slots, see above), maps column c of cache slot s to
+ * block table[s][c / 128], offset c % 128. Block 0 is the PARK BLOCK: no sequence owns it, and every table entry
+ * that no sequence owns points at it, so a parked slot (position 0) writes into it and into nothing else. Usable
+ * capacity is kv_blocks - 1 blocks. The table starts all zeros. Every result is bit for bit that of the contiguous
+ * cache: only the address of a column changes. The caller makes the table cover every column a call writes that
+ * it will read again: a slot prefill of S tokens writes columns 0 .. S-1, a slot decode of n_new tokens at pos
+ * writes pos .. pos + n_new - 2.
+ *
+ * A paged handle serves vcl_llm_slots_prefill, vcl_llm_slot_prefill (run as a packed prefill of one prompt, so
+ * prompts are limited to min(512, max_seq) tokens), vcl_llm_slot_decode and vcl_llm_set_sampling. Every static
+ * entry point (vcl_llm_prefill(_padded, _states, _append), _decode_step, _decode_loop, _generate(_padded), _score)
+ * and vcl_kv_cache_copy is rejected. Its LLM activations are sized for max_batch * min(max_seq, 512) rows, the
+ * most a packed prefill uses.
+ *
+ * vcl_llm_set_block_table writes the whole table from table_host (HOST memory, n_slots * ceil(max_seq / 128)
+ * int32, row-major) with one host-to-device copy on `stream` into a device array of the handle at a fixed address,
+ * so one captured slot-decode graph serves every table. Rejected before any device work, the table unchanged: an
+ * entry outside 0 .. kv_blocks-1, or a block other than 0 that appears twice. Not a paged handle: rejected. */
+int vcl_llm_set_block_table(vcl_handle* h, const int32_t* table_host, void* stream);
+
+/* Copy block `block` (0 .. kv_blocks-1) of a paged cache whole out of the handle into buf (write = 0) or from buf
+ * into it (write = 1): one cudaMemcpyAsync on `stream`. buf is device memory or pinned host memory of the block's
+ * size (above). Swapping a sequence out to host memory and back, and reading the cache back in tests. */
+int vcl_kv_block_copy(vcl_handle* h, int block, int write, void* buf, void* stream);
+
 /* forward(input_ids, labels=..., ...) (video_chatgpt/model/video_chatgpt.py:225-239): lm_head at EVERY
  * position and, with labels, the shifted cross-entropy of CrossEntropyLoss (ignore_index -100): column s of
  * clip b is scored against labels[b, s+1]; column S-1 has no target. The prefill is vcl_llm_prefill's
@@ -347,7 +378,8 @@ int vcl_op_attention_vit(const void* qkv, void* out, int n_frames, int S, int H,
 /* Copy decoder layer `layer`'s whole K and V cache, each [max_batch][llm_heads][max_seq][128] bf16, out of the
  * handle into k / v (write = 0) or from k / v into the handle (write = 1): one cudaMemcpyAsync per tensor on
  * `stream`. Lets a test read back exactly what the RoPE / cache writers stored, or fill the cache with a sentinel
- * first to see which columns a call touches. */
+ * first to see which columns a call touches. A paged handle (vcl_config.kv_blocks > 0) rejects it: see
+ * vcl_kv_block_copy. */
 int vcl_kv_cache_copy(vcl_handle* h, int layer, int write, void* k, void* v, void* stream);
 /* The decode attention kernel on its own: q [B][q_ld] (head h at columns h*128 ..), k / v caches
  * [B][H][s_max][128], clip b's query at column c_b = kv_len - 1 + (pos_dev ? pos_dev[b] : 0) attending keys

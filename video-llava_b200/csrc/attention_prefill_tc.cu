@@ -89,9 +89,12 @@ __device__ __forceinline__ void pa_mma(float (&acc)[64], uint32_t a_base, int a_
 // PACK: packed sequences (a.pack): blockIdx.z is sequence i, whose S_i queries start at its row offset and whose keys
 // are clip slot_i of the cache (S = S_kv = S_i, q_off = 0); the grid covers the longest sequence, so a CTA whose
 // query tile starts past S_i has nothing to do.
-template <bool PAD, bool PACK>
+// PAGED (with PACK): a paged cache (a.pages). Key block kb of sequence i is the 128 columns of block
+// table[slot_i][kb], rows 128 elements apart, so one key block of this kernel is exactly one page.
+template <bool PAD, bool PACK, bool PAGED = false>
 __global__ void __launch_bounds__(PA_THREADS)
 attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
+  static_assert(!PAGED || (PACK && !PAD), "a paged cache is read by packed prefills only");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t pad = ((raw_addr + 1023u) & ~1023u) - raw_addr;
@@ -111,8 +114,23 @@ attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
     q_base = off * a.q_ss; o_base = off * a.o_ss; kv_clip = __ldg(pack_slot(a.pack) + b);
   }
   const bf16* qg = a.q + q_base + (long long)h * a.q_sh;
-  const bf16* kg = a.k + kv_clip * a.k_sb + (long long)h * a.k_sh;
-  const bf16* vg = a.v + kv_clip * a.v_sb + (long long)h * a.v_sh;
+  const bf16* kg = a.k + (PAGED ? 0 : kv_clip * a.k_sb) + (long long)h * a.k_sh;
+  const bf16* vg = a.v + (PAGED ? 0 : kv_clip * a.v_sb) + (long long)h * a.v_sh;
+  // key block kb: rows kb * 128 .. of the clip, or rows 0 .. of its page (paged; keys >= S_kv are zero either way)
+  auto load_k = [&](int kb) {
+    if constexpr (PAGED)
+      pa_load_rows<128>(smem + PA_OFF_K, kg + (long long)__ldg(a.pages.table + kv_clip * a.pages.row + kb) * a.pages.blk,
+                        a.k_ss, 0, S_kv - kb * 128);
+    else
+      pa_load_rows<128>(smem + PA_OFF_K, kg, a.k_ss, kb * 128, S_kv);
+  };
+  auto load_vt = [&](int kb) {
+    if constexpr (PAGED)
+      pa_load_vt(smem + PA_OFF_VT, vg + (long long)__ldg(a.pages.table + kv_clip * a.pages.row + kb) * a.pages.blk,
+                 a.v_ss, 0, S_kv - kb * 128);
+    else
+      pa_load_vt(smem + PA_OFF_VT, vg, a.v_ss, kb * 128, S_kv);
+  };
   // key blocks this tile touches: keys up to the absolute position of its last query
   const int last_key = min(S_kv - 1, q_off + min(q0 + 63, S - 1));
   const int n_kb = last_key / 128 + 1;
@@ -144,7 +162,7 @@ attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
   float m[2] = {-INFINITY, -INFINITY};
   for (int kb = kb0; kb < n_kb; ++kb) {
     __syncthreads();                                     // previous readers of K are done
-    pa_load_rows<128>(smem + PA_OFF_K, kg, a.k_ss, kb * 128, S_kv);
+    load_k(kb);
     fence_async_smem();
     __syncthreads();
     pa_mma(acc, sbase + PA_OFF_Q, 64 * 128, sbase + PA_OFF_K, 128 * 128, false);
@@ -163,8 +181,8 @@ attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
   float l[2] = {0.f, 0.f};
   for (int kb = kb0; kb < n_kb; ++kb) {
     __syncthreads();                                     // previous readers of K / V^T / P are done
-    pa_load_rows<128>(smem + PA_OFF_K, kg, a.k_ss, kb * 128, S_kv);
-    pa_load_vt(smem + PA_OFF_VT, vg, a.v_ss, kb * 128, S_kv);
+    load_k(kb);
+    load_vt(kb);
     fence_async_smem();
     __syncthreads();
     pa_mma(acc, sbase + PA_OFF_Q, 64 * 128, sbase + PA_OFF_K, 128 * 128, false);
@@ -212,6 +230,8 @@ int init_attention_prefill_tc_kernels() {
   VCL_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PA_SMEM));
   VCL_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, PA_SMEM));
   VCL_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, PA_SMEM));
+  VCL_CUDA_OK(cudaFuncSetAttribute(attn_prefill_tc_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   PA_SMEM));
   return 0;
 }
 
@@ -231,7 +251,9 @@ bool attention_prefill_tc_supported(const AttnArgs& a) {
 int launch_attention_prefill_tc(const AttnArgs& a, cudaStream_t stream) {
   const int S_kv = a.S_kv > 0 ? a.S_kv : a.S;
   dim3 grid((a.S + 63) / 64, a.H, a.B);
-  if (a.pack != nullptr) attn_prefill_tc_kernel<false, true><<<grid, PA_THREADS, PA_SMEM, stream>>>(a, S_kv);
+  VCL_REQUIRE(a.pages.table == nullptr || a.pack != nullptr, "prefill attention: a paged cache needs packed rows");
+  if (a.pages.table != nullptr) attn_prefill_tc_kernel<false, true, true><<<grid, PA_THREADS, PA_SMEM, stream>>>(a, S_kv);
+  else if (a.pack != nullptr) attn_prefill_tc_kernel<false, true><<<grid, PA_THREADS, PA_SMEM, stream>>>(a, S_kv);
   else if (a.n_pad != nullptr) attn_prefill_tc_kernel<true, false><<<grid, PA_THREADS, PA_SMEM, stream>>>(a, S_kv);
   else attn_prefill_tc_kernel<false, false><<<grid, PA_THREADS, PA_SMEM, stream>>>(a, S_kv);
   VCL_CUDA_OK(cudaGetLastError());

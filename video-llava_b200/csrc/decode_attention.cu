@@ -50,16 +50,23 @@ __device__ __forceinline__ float block_reduce(float v, bool is_max, float* scrat
 // DA_SPLIT = CTAs per (clip, head): 4 for few clips (latency: more CTAs than SMs are needed to fill the
 // machine at all), 2 or 1 when clips x heads alone oversubscribe it (throughput: fewer barriers per byte).
 // The keys of clip b, n_pad[b] .. kv_len + pos_dev[b] - 1 (kernels.h: decode positions), are split over the CTAs.
-template <int DA_SPLIT>
+// PAGED: a paged cache (kernels.h: KvPages; clip b is cache slot b). The slot's table row is staged in shared
+// memory, and key j of a CTA's range, at column lo + j, is read from row (lo + j) % 128 of block tbl[(lo + j) / 128].
+template <int DA_SPLIT, bool PAGED = false>
 __global__ void __launch_bounds__(DA_THREADS)
 decode_attn_cluster_kernel(const bf16* __restrict__ q, long long q_ld, const bf16* __restrict__ kcache,
                            const bf16* __restrict__ vcache, bf16* __restrict__ o, long long o_ld, int H,
                            int s_max, int kv_len, int per_cap, float scale, const int* __restrict__ pos_dev,
-                           int o_xwin, const int* __restrict__ n_pad) {
+                           int o_xwin, const int* __restrict__ n_pad, const KvPages pages) {
   extern __shared__ float sm[];
   float* sc = sm;                       // [per_cap] scores -> probabilities of my keys
   float* red = sm + per_cap;            // [16][128] partial outputs over the 16 key groups
   const int h = blockIdx.y, b = blockIdx.z;
+  int* tbl = reinterpret_cast<int*>(red + 16 * 128 + 128 + 2 + 8);   // PAGED: [pages.row] the slot's table row
+  if constexpr (PAGED) {
+    // the table is constant while a decode graph runs (written before it, like pos_dev): read before the wait
+    for (int i = threadIdx.x; i < pages.row; i += DA_THREADS) tbl[i] = __ldg(pages.table + b * pages.row + i);
+  }
   // the clip's position and key floor live on the device (one captured graph for every position and padding);
   // they are constant while the graph runs, so they can be read before the dependency wait. The first k0
   // cache columns hold pad keys, which are neither read nor split
@@ -72,12 +79,22 @@ decode_attn_cluster_kernel(const bf16* __restrict__ q, long long q_ld, const bf1
   const uint32_t rank = cluster_ctarank();
   const int lo = k0 + (int)rank * per;
   const int n_loc = max(0, min(kv_len - lo, per));
-  const long long coff = (((long long)b * H + h) * s_max + lo) * 128;
+  const long long coff = PAGED ? (long long)h * 128 * 128 : (((long long)b * H + h) * s_max + lo) * 128;
   const bf16* kc = kcache + coff;
   const bf16* vc = vcache + coff;
+  // element offset of key j of my range (relative to kc / vc)
+  auto key_off = [&](int j) -> long long {
+    if constexpr (PAGED) {
+      const int c = lo + j;
+      return (long long)tbl[c >> 7] * pages.blk + (c & 127) * 128;
+    } else {
+      return (long long)j * 128;
+    }
+  };
 
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
+  if constexpr (PAGED) __syncthreads();   // tbl is staged
 
   constexpr int U = 8;
   const int g = threadIdx.x >> 4, dc = threadIdx.x & 15;   // key slot (of 16) and 8-dim chunk
@@ -93,7 +110,7 @@ decode_attn_cluster_kernel(const bf16* __restrict__ q, long long q_ld, const bf1
 #pragma unroll
       for (int u = 0; u < U; ++u) {
         const int j = j0 + 16 * u;
-        ku[u] = (j < n_loc) ? ld_nc_v4(kc + (long long)j * 128 + dc * 8) : make_uint4(0, 0, 0, 0);
+        ku[u] = (j < n_loc) ? ld_nc_v4(kc + key_off(j) + dc * 8) : make_uint4(0, 0, 0, 0);
       }
 #pragma unroll
       for (int u = 0; u < U; ++u) {
@@ -114,7 +131,7 @@ decode_attn_cluster_kernel(const bf16* __restrict__ q, long long q_ld, const bf1
 #pragma unroll
   for (int u = 0; u < U; ++u) {
     const int j = g + 16 * u;
-    vu[u] = (j < n_loc) ? ld_nc_v4(vc + (long long)j * 128 + dc * 8) : make_uint4(0, 0, 0, 0);
+    vu[u] = (j < n_loc) ? ld_nc_v4(vc + key_off(j) + dc * 8) : make_uint4(0, 0, 0, 0);
   }
   __syncthreads();
   float mx = -INFINITY;
@@ -147,7 +164,7 @@ decode_attn_cluster_kernel(const bf16* __restrict__ q, long long q_ld, const bf1
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           const int j = j0 + 16 * u;
-          vu[u] = (j < n_loc) ? ld_nc_v4(vc + (long long)j * 128 + dc * 8) : make_uint4(0, 0, 0, 0);
+          vu[u] = (j < n_loc) ? ld_nc_v4(vc + key_off(j) + dc * 8) : make_uint4(0, 0, 0, 0);
         }
       }
 #pragma unroll
@@ -187,8 +204,11 @@ decode_attn_cluster_kernel(const bf16* __restrict__ q, long long q_ld, const bf1
 int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, const bf16* vcache,
                             bf16* o, long long o_ld, int B, int H, int head_dim, int s_max,
                             int kv_len, float scale, cudaStream_t stream, const int* pos_dev, bool o_xwin,
-                            const int* n_pad) {
+                            const int* n_pad, const KvPages& pages) {
   VCL_REQUIRE(head_dim == 128, "decode attention: head_dim must be 128");
+  const bool paged = pages.table != nullptr;
+  VCL_REQUIRE(!paged || pages.row == (s_max + 127) / 128, "decode attention: table rows of %d blocks for max_seq %d",
+              pages.row, s_max);
   VCL_REQUIRE(n_pad != nullptr, "decode attention: needs the key floors n_pad");
   VCL_REQUIRE(kv_len > 0 && kv_len <= s_max, "decode attention: kv_len %d out of range", kv_len);
   // shared memory is sized for the longest sequence when the length is only known on the device
@@ -197,7 +217,7 @@ int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, c
   const int heads = B * H;
   const int split = heads <= 2 * device_num_sms() ? 4 : (heads <= 3 * device_num_sms() ? 2 : 1);
   const int per = ((kv_cap + split - 1) / split + 15) / 16 * 16;   // keys per CTA, multiple of 16
-  const size_t smem = (size_t)(per + 16 * 128 + 128 + 2 + 8) * sizeof(float);
+  const size_t smem = (size_t)(per + 16 * 128 + 128 + 2 + 8 + (paged ? pages.row : 0)) * sizeof(float);
   VCL_REQUIRE(smem <= 48 * 1024, "decode attention: kv_len %d too long for the smem budget", kv_len);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(split, H, B);
@@ -213,11 +233,11 @@ int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, c
   attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 2;
-  auto kern = decode_attn_cluster_kernel<4>;
-  if (split == 2) kern = decode_attn_cluster_kernel<2>;
-  if (split == 1) kern = decode_attn_cluster_kernel<1>;
+  auto kern = paged ? decode_attn_cluster_kernel<4, true> : decode_attn_cluster_kernel<4>;
+  if (split == 2) kern = paged ? decode_attn_cluster_kernel<2, true> : decode_attn_cluster_kernel<2>;
+  if (split == 1) kern = paged ? decode_attn_cluster_kernel<1, true> : decode_attn_cluster_kernel<1>;
   VCL_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, q, q_ld, kcache, vcache, o, o_ld, H, s_max, kv_len, per, scale, pos_dev,
-                                 o_xwin ? 1 : 0, n_pad));
+                                 o_xwin ? 1 : 0, n_pad, pages));
   count_launches(1);
   return 0;
 }

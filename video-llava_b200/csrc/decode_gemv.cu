@@ -258,7 +258,9 @@ __device__ __forceinline__ void epi_qkv_rope(const GemvEpilogue& e, int b, int r
   const int which = hr / e.H, head = hr - which * e.H;
   const int d = (row & 127) >> 1;
   const float lo = bf16r(v0), hi = bf16r(v1);
-  const long long coff = (((long long)b * e.H + head) * e.s_max + col) * 128;
+  // a paged cache: clip b is cache slot b, its column col in block table[b][col / 128]
+  const long long coff = e.pages.table != nullptr ? kv_paged_off(e.pages, b, head, col)
+                                                  : (((long long)b * e.H + head) * e.s_max + col) * 128;
   if (which == 2) {
     e.vcache[coff + d] = __float2bfloat16_rn(lo);
     e.vcache[coff + d + 64] = __float2bfloat16_rn(hi);

@@ -201,7 +201,9 @@ __device__ __forceinline__ void gemm_epilogue_store(const uint8_t* stg, int t, i
           } else {
             gb = grow / rp.S; col_c = rp.start_pos + grow - gb * rp.S;
           }
-          dst = (which == 1 ? rp.kcache : rp.vcache) + (((long long)gb * rp.H + head) * rp.s_max + col_c) * 128 + d;
+          dst = (which == 1 ? rp.kcache : rp.vcache) + d +
+                (rp.pages.table != nullptr ? kv_paged_off(rp.pages, gb, head, col_c)   // paged: one more lookup
+                                           : (((long long)gb * rp.H + head) * rp.s_max + col_c) * 128);
         }
       } else if (RES && residual != nullptr) {
         val.x = bf16x2_add(val.x, rr[u].x); val.y = bf16x2_add(val.y, rr[u].y);

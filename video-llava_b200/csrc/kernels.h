@@ -26,6 +26,20 @@ template <class T> __host__ __device__ inline T* pack_slot(T* p) { return p + 2 
 template <class T> __host__ __device__ inline T* pack_last(T* p) { return p + 3 * PACK_SEQ_MAX; }
 template <class T> __host__ __device__ inline T* pack_row(T* p, long long r) { return p + PACK_HEAD + 2 * r; }   // [seq, pos]
 
+// Paged KV cache (vcl_config.kv_blocks > 0): one pool of blocks instead of the contiguous [clip][head][s_max][128]
+// cache of a layer. A block is 128 columns of one sequence across all layers, [layer][K = 0 | V = 1][head][128][128]
+// bf16 (blk elements). Column c of cache slot s lives in block table[s * row + c / 128] at offset c % 128, so with
+// the K (or V) base of a layer, pool + (2 * layer (+ 1)) * H * 128 * 128, element (s, head, c, d) is at
+// base + kv_paged_off(p, s, head, c) + d. A null table is the contiguous cache.
+struct KvPages {
+  const int* table = nullptr;   // [slots][row] block indices
+  int row = 0;                  // ceil(s_max / 128)
+  long long blk = 0;            // elements per block
+};
+__device__ __forceinline__ long long kv_paged_off(const KvPages& p, int slot, int head, int col) {
+  return (long long)__ldg(p.table + slot * p.row + (col >> 7)) * p.blk + ((long long)head * 128 + (col & 127)) * 128;
+}
+
 enum Act { ACT_NONE = 0, ACT_QGELU = 1, ACT_GELU = 2, ACT_SWIGLU = 3, ACT_ROPE = 4 };
 // ACT_ROPE: the GEMM is the LLaMA q|k|v projection of a prefill (N = 3 * H * 128, rows = [clip][position], or the
 // packed rows of `pack`). The epilogue rotates q and k (RoPE, every product and the sum rounded to bf16 like the
@@ -38,6 +52,7 @@ struct RopeEpilogue {
   const int* n_pad = nullptr;                                  // [clip] left padding (see below) or null
   const int* pack = nullptr;   // packed rows (above) or null: row r is rotated by its position p and lands at
                                // column p of its sequence's slot (S, start_pos and n_pad are then unused)
+  KvPages pages;               // packed rows only: a paged cache (kcache / vcache are then the layer's pool bases)
 };
 
 // Positions in the KV cache. Left padding (a batch of prompts of different lengths): clip b's first n_pad[b]
@@ -160,6 +175,9 @@ struct AttnArgs {
   // are rows offset_i .. of q / o (q_sb, o_sb unused), its keys / values clip slot_i of k / v. a.S is max S_i.
   // Always the wgmma kernel (S_i <= 512), whatever VCL_PREFILL_ATTN_FLASH says.
   const int* pack = nullptr;
+  // packed rows only: a paged cache. Key block kb of sequence i is block table[slot_i][kb] (k / v: the layer's pool
+  // bases, k_sh / v_sh the head stride inside a block, k_ss = v_ss = 128; k_sb / v_sb unused)
+  KvPages pages;
 };
 int launch_attention(const AttnArgs& a, cudaStream_t stream);     // dispatches to the wgmma prefill kernel when it applies
 int init_attention_kernels();
@@ -175,11 +193,12 @@ bool attention_vit_tc_supported(int S);
 int launch_attention_vit_tc(const bf16* qkv, bf16* out, int n_frames, int S, int H, int C, cudaStream_t stream);
 int init_attention_tc_kernels();
 // single-query attention against the cache at the decode positions above (kv_len = pos + 1):
-// q [B, H*hd] -> o [B, H*hd], written in xwin layout with o_xwin
+// q [B, H*hd] -> o [B, H*hd], written in xwin layout with o_xwin. pages.table: a paged cache (kcache / vcache the
+// layer's pool bases; clip b is cache slot b)
 int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, const bf16* vcache,
                             bf16* o, long long o_ld, int B, int H, int head_dim, int s_max,
                             int kv_len, float scale, cudaStream_t stream, const int* pos_dev, bool o_xwin,
-                            const int* n_pad);
+                            const int* n_pad, const KvPages& pages = KvPages());
 
 // ---- decode_gemv.cu : decode-time weight streaming (1..64 new tokens) -------------------------------
 // Two ring kernels (bulk-copy ring over a slot-ordered copy of the matrix + mma.sync) behind one launcher:
@@ -228,6 +247,7 @@ struct GemvEpilogue {
   int H = 0, s_max = 0, pos = 0;
   const int* pos_dev = nullptr;                 // QKV: the decode positions above (pos_dev may be null) ...
   const int* n_pad = nullptr;                   // ... and the key floors [B] (required)
+  KvPages pages;                                // QKV: a paged cache (kcache / vcache the layer's pool bases) or none
   float* logits = nullptr; long long ldl = 0;   // LOGITS
 };
 

@@ -108,6 +108,11 @@ struct vcl_handle {
   bf16 *l_h = nullptr, *l_x = nullptr, *l_qkv = nullptr, *l_attn = nullptr, *l_act = nullptr;
   bf16 *l_vid = nullptr, *l_vid_tmp = nullptr;
   bf16 *kcache = nullptr, *vcache = nullptr;   // [L][B][H][s_max][128]
+  // the paged cache (cfg.kv_blocks > 0) instead: kv_blocks blocks of [L][K | V][H][128][128] (kernels.h: KvPages),
+  // and the block table [n_slots_max()][table_row()] at a fixed device address, written whole from its host copy
+  bf16* pool = nullptr;
+  int* d_table = nullptr;
+  std::vector<int> table_host;
   bf16 *rope_cos = nullptr, *rope_sin = nullptr;
   float* logits = nullptr;                     // [max_batch, vocab]
   int32_t* tokens = nullptr;                   // [max_batch, max_seq] generated-token scratch
@@ -149,6 +154,16 @@ struct vcl_handle {
   size_t cache_layer_elems() const {
     return (size_t)cfg.max_batch * cfg.llm_heads * cfg.max_seq * 128;
   }
+  bool paged() const { return cfg.kv_blocks > 0; }
+  int table_row() const { return (cfg.max_seq + 127) / 128; }
+  size_t block_elems() const { return (size_t)2 * cfg.llm_layers * cfg.llm_heads * 128 * 128; }
+  KvPages pages() const {
+    KvPages p;
+    if (paged()) { p.table = d_table; p.row = table_row(); p.blk = (long long)block_elems(); }
+    return p;
+  }
+  // rows of the LLM activations per clip: a paged handle prefills packed prompts of at most 512 tokens only
+  int act_seq() const { return paged() && cfg.max_seq > 512 ? 512 : cfg.max_seq; }
   // rows of the row-major lm_head: vocab rounded up to the 256-wide GEMM tile, the extra rows zero
   int vocab_padded() const { return (cfg.vocab + 255) / 256 * 256; }
   // cache slots: max_slots, or by default min(max_batch, 16)
@@ -319,6 +334,8 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   VCL_REQUIRE(c->max_slots == 0 || (c->max_slots >= 1 && c->max_slots <= c->max_batch && c->max_slots <= 64),
               "vcl_create: max_slots=%d outside 1..%d (0: min(max_batch, 16))", c->max_slots,
               c->max_batch < 64 ? c->max_batch : 64);
+  VCL_REQUIRE(c->kv_blocks == 0 || c->kv_blocks >= 2,
+              "vcl_create: kv_blocks=%d: 0 (contiguous cache) or at least 2 (block 0 is the park block)", c->kv_blocks);
   {
     // every decode projection must have a kernel for every clip count up to 64 (beyond: the GEMM)
     const int D = c->llm_hidden, F = c->llm_inter;
@@ -355,7 +372,7 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   rc |= dalloc(h, &h->v_act, act_elems);
 
   const size_t D = c->llm_hidden, LF = c->llm_inter;
-  const size_t Ml = (size_t)c->max_batch * c->max_seq;
+  const size_t Ml = (size_t)c->max_batch * h->act_seq();
   rc |= dalloc(h, &h->l_h, Ml * D);
   rc |= dalloc(h, &h->l_x, Ml * D);
   rc |= dalloc(h, &h->l_qkv, Ml * 3 * D);
@@ -363,8 +380,14 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   rc |= dalloc(h, &h->l_act, Ml * LF);
   rc |= dalloc(h, &h->l_vid, (size_t)c->max_batch * h->NV * D);
   rc |= dalloc(h, &h->l_vid_tmp, (size_t)c->max_batch * h->NV * D);
-  rc |= dalloc(h, &h->kcache, (size_t)c->llm_layers * h->cache_layer_elems());
-  rc |= dalloc(h, &h->vcache, (size_t)c->llm_layers * h->cache_layer_elems());
+  if (h->paged()) {
+    rc |= dalloc(h, &h->pool, (size_t)c->kv_blocks * h->block_elems());
+    h->table_host.assign((size_t)h->n_slots_max() * h->table_row(), 0);   // every entry at the park block
+    rc |= dalloc(h, &h->d_table, h->table_host.size());
+  } else {
+    rc |= dalloc(h, &h->kcache, (size_t)c->llm_layers * h->cache_layer_elems());
+    rc |= dalloc(h, &h->vcache, (size_t)c->llm_layers * h->cache_layer_elems());
+  }
   rc |= dalloc(h, &h->rope_cos, (size_t)c->max_seq * 64);
   rc |= dalloc(h, &h->rope_sin, (size_t)c->max_seq * 64);
   rc |= dalloc(h, &h->logits, (size_t)c->max_batch * c->vocab);
@@ -386,6 +409,7 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   if (rc == 0) {
     cudaError_t e = cudaMemset(h->d_npad, 0, Bm * sizeof(int));   // the cache starts unpadded
     if (e == cudaSuccess) e = cudaMemset(h->samp, 0, Bm * 16);        // and every entry greedy
+    if (e == cudaSuccess && h->paged()) e = cudaMemset(h->d_table, 0, h->table_host.size() * sizeof(int));
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
     if (e != cudaSuccess) {
       set_last_error("vcl_create: %s", cudaGetErrorString(e));
@@ -602,8 +626,22 @@ int clip_forward(vcl_handle* h, const void* pixels, int fmt, int n_frames, int n
   return 0;
 }
 
-bf16* kc_layer(vcl_handle* h, int l) { return h->kcache + (size_t)l * h->cache_layer_elems(); }
-bf16* vc_layer(vcl_handle* h, int l) { return h->vcache + (size_t)l * h->cache_layer_elems(); }
+// the K / V cache base of layer l: its contiguous cache, or in a paged cache its place inside block 0 (h->pages()
+// adds the block offset of a column)
+bf16* kc_layer(vcl_handle* h, int l) {
+  if (h->paged()) return h->pool + (size_t)(2 * l) * h->cfg.llm_heads * 128 * 128;
+  return h->kcache + (size_t)l * h->cache_layer_elems();
+}
+bf16* vc_layer(vcl_handle* h, int l) {
+  if (h->paged()) return h->pool + (size_t)(2 * l + 1) * h->cfg.llm_heads * 128 * 128;
+  return h->vcache + (size_t)l * h->cache_layer_elems();
+}
+
+// the static entry points: a paged cache serves the slot entry points only
+#define VCL_NOT_PAGED(h, name)                                                                                   \
+  VCL_REQUIRE(!(h)->paged(), "%s: this handle has a paged KV cache (kv_blocks %d), which serves the slot entry "   \
+              "points only (generate_requests: vcl_llm_slots_prefill / vcl_llm_slot_prefill / vcl_llm_slot_decode)", \
+              name, (h)->cfg.kv_blocks)
 
 // final RMSNorm + lm_head on rows x[b*ldx .. ] (b < B), arg-max
 // partials_out: the arg-max is left as per-CTA partials in h->amax for the next step's q|k|v kernel
@@ -676,6 +714,7 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
   const vcl_config& c = h->cfg;
   const bool packed = packed_rows > 0;
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
+  VCL_REQUIRE(packed || !h->paged(), "a paged KV cache is prefilled by packed prefills only");
   VCL_REQUIRE(B > 0 && B <= c.max_batch, "B=%d outside 1..%d", B, c.max_batch);
   VCL_REQUIRE(slot == 0 || (B == 1 && slot > 0 && slot < c.max_batch), "slot %d needs B = 1 and a clip of the cache",
               slot);
@@ -750,7 +789,7 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
       g.act = ACT_ROPE;
       g.rope.cos_t = h->rope_cos; g.rope.sin_t = h->rope_sin; g.rope.kcache = kc(l); g.rope.vcache = vc(l);
       g.rope.S = S; g.rope.start_pos = start_pos; g.rope.H = H; g.rope.s_max = c.max_seq; g.rope.n_pad = np;
-      g.rope.pack = pk;
+      g.rope.pack = pk; g.rope.pages = h->pages();
       VCL_TRY(launch_gemm_bf16_tn(g, st));
     } else {
       VCL_TRY(gemm(h->l_x, D, w.wqkv, D, h->l_qkv, 3 * D, nullptr, nullptr, 0, M, 3 * D, D, ACT_NONE, st));
@@ -764,6 +803,9 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
     a.o = h->l_attn; a.o_sb = (long long)S * D; a.o_sh = 128; a.o_ss = D;
     a.B = B; a.H = H; a.S = S; a.head_dim = 128; a.scale = scale; a.causal = 1;
     a.S_kv = start_pos + S; a.q_off = start_pos; a.n_pad = np; a.pack = pk;
+    if (h->paged()) {   // heads 128 x 128 apart inside a block (kernels.h: KvPages)
+      a.k_sb = a.v_sb = 0; a.k_sh = a.v_sh = 128 * 128; a.pages = h->pages();
+    }
     VCL_TRY(launch_attention(a, st));
     VCL_TRY(gemm(h->l_attn, D, w.wo, D, h->l_h, D, nullptr, h->l_h, D, M, D, D, ACT_NONE, st));
     VCL_TRY(launch_rmsnorm(h->l_h, D, h->l_x, D, w.ln2, M, D, c.rms_eps, st));
@@ -869,10 +911,10 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
       GemvEpilogue qkv;
       qkv.mode = GEMV_QKV; qkv.q_out = h->d_q; qkv.ldq = D; qkv.kcache = kc_layer(h, l); qkv.vcache = vc_layer(h, l);
       qkv.cos_t = h->rope_cos; qkv.sin_t = h->rope_sin; qkv.H = H; qkv.s_max = c.max_seq; qkv.pos = pos; qkv.pos_dev = pd;
-      qkv.n_pad = np;
+      qkv.n_pad = np; qkv.pages = h->pages();
       VCL_TRY(launch_gemv(g, qkv, st));
       VCL_TRY(launch_decode_attention(h->d_q, D, kc_layer(h, l), vc_layer(h, l), h->d_attn, D, B, H, 128,
-                                      c.max_seq, pos + 1, scale, st, pd, /*o_xwin=*/wide, np));
+                                      c.max_seq, pos + 1, scale, st, pd, /*o_xwin=*/wide, np, h->pages()));
       GemvArgs go;
       go.x = h->d_attn; go.ldx = D; w.o_d.into(go); go.B = B; go.N = D; go.K = D;
       VCL_TRY(launch_gemv(go, residual, st));
@@ -888,6 +930,7 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
     } else {
       // B > 64: tensor-core path, the B new rows ride in one (mostly empty) 128-row tile and the
       // N tile is narrowed so that every SM streams a slice of the weights
+      VCL_REQUIRE(!h->paged(), "a paged KV cache decodes at most 64 slots");
       VCL_TRY(launch_rmsnorm(h->d_h, D, h->d_x, D, w.ln1, B, D, c.rms_eps, st));
       VCL_TRY(gemm(h->d_x, D, w.wqkv, D, h->d_qkv, 3 * D, nullptr, nullptr, 0, B, 3 * D, D, ACT_NONE, st));
       VCL_TRY(launch_rope_kv_prefill(h->d_qkv, kc_layer(h, l), vc_layer(h, l), h->rope_cos, h->rope_sin, B,
@@ -1037,6 +1080,7 @@ int vcl_llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats,
                     const int32_t* vid_start, int B, int S, int n_layers, void* hidden_out,
                     float* logits_out, int32_t* next_tok, void* stream) {
   VCL_REQUIRE(h != nullptr, "vcl_llm_prefill: null handle");
+  VCL_NOT_PAGED(h, "vcl_llm_prefill");
   return llm_prefill(h, ids, video_feats, vid_start, B, S, n_layers, hidden_out, logits_out, next_tok, 1,
                      as_stream(stream));
 }
@@ -1045,6 +1089,7 @@ int vcl_llm_prefill_states(vcl_handle* h, const int64_t* ids, const void* video_
                            const int32_t* vid_start, int B, int S, void* states_out, float* logits_out,
                            void* stream) {
   VCL_REQUIRE(h != nullptr && states_out != nullptr, "vcl_llm_prefill_states: null argument");
+  VCL_NOT_PAGED(h, "vcl_llm_prefill_states");
   return llm_prefill(h, ids, video_feats, vid_start, B, S, h->cfg.llm_layers, nullptr, logits_out, nullptr, 1,
                      as_stream(stream), 0, states_out);
 }
@@ -1052,6 +1097,7 @@ int vcl_llm_prefill_states(vcl_handle* h, const int64_t* ids, const void* video_
 int vcl_llm_prefill_append(vcl_handle* h, const int64_t* ids, int B, int S, int start_pos, void* hidden_out,
                            float* logits_out, int32_t* next_tok, void* stream) {
   VCL_REQUIRE(h != nullptr && ids != nullptr, "vcl_llm_prefill_append: null argument");
+  VCL_NOT_PAGED(h, "vcl_llm_prefill_append");
   VCL_REQUIRE(start_pos > 0, "vcl_llm_prefill_append: start_pos must be > 0 (use vcl_llm_prefill for a new sequence)");
   return llm_prefill(h, ids, nullptr, nullptr, B, S, h->cfg.llm_layers, hidden_out, logits_out, next_tok, 1,
                      as_stream(stream), start_pos);
@@ -1060,6 +1106,7 @@ int vcl_llm_prefill_append(vcl_handle* h, const int64_t* ids, int B, int S, int 
 int vcl_llm_decode_step(vcl_handle* h, const int32_t* tok_in, int B, int pos, float* logits_out,
                         int32_t* tok_out, void* stream) {
   VCL_REQUIRE(h && tok_in, "vcl_llm_decode_step: null argument");
+  VCL_NOT_PAGED(h, "vcl_llm_decode_step");
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
   VCL_REQUIRE(B > 0 && B <= h->cfg.max_batch, "B=%d outside 1..%d", B, h->cfg.max_batch);
   StepIo io;
@@ -1070,6 +1117,7 @@ int vcl_llm_decode_step(vcl_handle* h, const int32_t* tok_in, int B, int pos, fl
 int vcl_llm_decode_loop(vcl_handle* h, const int32_t* first_tok, int B, int S, int n_new,
                         int32_t* out_tokens, void* stream) {
   VCL_REQUIRE(h && first_tok && out_tokens, "vcl_llm_decode_loop: null argument");
+  VCL_NOT_PAGED(h, "vcl_llm_decode_loop");
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
   VCL_REQUIRE(B > 0 && B <= h->cfg.max_batch, "B=%d outside 1..%d", B, h->cfg.max_batch);
   VCL_REQUIRE(n_new >= 1 && S + n_new <= h->cfg.max_seq + 1, "S + n_new = %d exceeds max_seq %d", S + n_new,
@@ -1086,6 +1134,8 @@ int vcl_llm_slot_prefill(vcl_handle* h, int slot, const int64_t* ids, const void
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
   VCL_REQUIRE(slot >= 0 && slot < h->n_slots_max(), "vcl_llm_slot_prefill: slot %d outside 0..%d (%s)", slot,
               h->n_slots_max() - 1, h->slots_note().c_str());
+  // a paged cache: the packed prefill of one prompt, bit for bit the same (vcl_llm_slots_prefill)
+  if (h->paged()) return vcl_llm_slots_prefill(h, 1, &slot, &S, ids, video_feats, vid_start, next_tok, stream);
   return llm_prefill(h, ids, video_feats, vid_start, 1, S, h->cfg.llm_layers, nullptr, nullptr, next_tok, 1,
                      as_stream(stream), 0, nullptr, nullptr, slot);
 }
@@ -1112,7 +1162,7 @@ int vcl_llm_slots_prefill(vcl_handle* h, int n, const int32_t* slots_host, const
     M += len;
     S_max = len > S_max ? len : S_max;
   }
-  // n <= max_batch sequences of at most max_seq tokens: M fits the activations (max_batch * max_seq rows)
+  // n <= max_batch sequences of at most min(512, max_seq) tokens: M fits the activations (max_batch * act_seq() rows)
   std::vector<int> map(pack_elems(M), 0);
   int* p = map.data();
   for (int i = 0, r = 0; i < n; ++i) {
@@ -1181,6 +1231,7 @@ int vcl_llm_generate(vcl_handle* h, const int64_t* ids, const void* video_feats,
                      const int32_t* vid_start, int B, int S, int n_new, int32_t* out_tokens,
                      void* stream) {
   VCL_REQUIRE(h && out_tokens, "vcl_llm_generate: null argument");
+  VCL_NOT_PAGED(h, "vcl_llm_generate");
   VCL_REQUIRE(n_new >= 1 && S + n_new <= h->cfg.max_seq + 1, "S + n_new = %d exceeds max_seq %d", S + n_new,
               h->cfg.max_seq);
   cudaStream_t st = as_stream(stream);
@@ -1193,6 +1244,7 @@ int vcl_llm_prefill_padded(vcl_handle* h, const int64_t* ids, const void* video_
                            const int32_t* n_pad_host, int B, int S, int n_layers, void* hidden_out,
                            float* logits_out, int32_t* next_tok, void* stream) {
   VCL_REQUIRE(h != nullptr && n_pad_host != nullptr, "vcl_llm_prefill_padded: null argument");
+  VCL_NOT_PAGED(h, "vcl_llm_prefill_padded");
   return llm_prefill(h, ids, video_feats, vid_start, B, S, n_layers, hidden_out, logits_out, next_tok, 1,
                      as_stream(stream), 0, nullptr, n_pad_host);
 }
@@ -1200,6 +1252,7 @@ int vcl_llm_prefill_padded(vcl_handle* h, const int64_t* ids, const void* video_
 int vcl_llm_generate_padded(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
                             const int32_t* n_pad_host, int B, int S, int n_new, int32_t* out_tokens, void* stream) {
   VCL_REQUIRE(h && out_tokens && n_pad_host, "vcl_llm_generate_padded: null argument");
+  VCL_NOT_PAGED(h, "vcl_llm_generate_padded");
   VCL_REQUIRE(n_new >= 1 && S + n_new <= h->cfg.max_seq + 1, "S + n_new = %d exceeds max_seq %d", S + n_new,
               h->cfg.max_seq);
   cudaStream_t st = as_stream(stream);
@@ -1212,6 +1265,7 @@ int vcl_llm_score(vcl_handle* h, const int64_t* ids, const void* video_feats, co
                   const int32_t* n_pad_host, int B, int S, const int64_t* labels, void* logits_out, float* nll_out,
                   float* loss_out, void* stream) {
   VCL_REQUIRE(h != nullptr, "vcl_llm_score: null handle");
+  VCL_NOT_PAGED(h, "vcl_llm_score");
   VCL_REQUIRE(labels != nullptr || (nll_out == nullptr && loss_out == nullptr),
               "vcl_llm_score: nll_out / loss_out need labels");
   cudaStream_t st = as_stream(stream);
@@ -1225,6 +1279,8 @@ long long vcl_launch_count(void) { return launch_count(); }
 
 int vcl_kv_cache_copy(vcl_handle* h, int layer, int write, void* k, void* v, void* stream) {
   VCL_REQUIRE(h && k && v, "vcl_kv_cache_copy: null argument");
+  VCL_REQUIRE(!h->paged(), "vcl_kv_cache_copy: this handle has a paged KV cache (kv_blocks %d): use vcl_kv_block_copy",
+              h->cfg.kv_blocks);
   VCL_REQUIRE(layer >= 0 && layer < h->cfg.llm_layers, "vcl_kv_cache_copy: layer %d outside 0..%d", layer,
               h->cfg.llm_layers - 1);
   const size_t bytes = h->cache_layer_elems() * sizeof(bf16);
@@ -1236,6 +1292,40 @@ int vcl_kv_cache_copy(vcl_handle* h, int layer, int write, void* k, void* v, voi
     VCL_CUDA_OK(cudaMemcpyAsync(k, kc_layer(h, layer), bytes, cudaMemcpyDeviceToDevice, st));
     VCL_CUDA_OK(cudaMemcpyAsync(v, vc_layer(h, layer), bytes, cudaMemcpyDeviceToDevice, st));
   }
+  return 0;
+}
+
+int vcl_llm_set_block_table(vcl_handle* h, const int32_t* table_host, void* stream) {
+  VCL_REQUIRE(h && table_host, "vcl_llm_set_block_table: null argument");
+  VCL_REQUIRE(h->paged(), "vcl_llm_set_block_table: the handle has a contiguous KV cache (kv_blocks 0)");
+  const int nb = h->cfg.kv_blocks, row = h->table_row();
+  std::vector<int> owner(nb, -1);    // the first entry that names each block
+  for (size_t i = 0; i < h->table_host.size(); ++i) {
+    const int blk = table_host[i];
+    VCL_REQUIRE(blk >= 0 && blk < nb, "vcl_llm_set_block_table: slot %d, block %d: entry %d outside 0..%d",
+                (int)(i / row), (int)(i % row), blk, nb - 1);
+    VCL_REQUIRE(blk == 0 || owner[blk] < 0,
+                "vcl_llm_set_block_table: block %d appears twice (slot %d block %d and slot %d block %d); only the "
+                "park block 0 may be shared", blk, blk ? owner[blk] / row : 0, blk ? owner[blk] % row : 0,
+                (int)(i / row), (int)(i % row));
+    if (blk != 0) owner[blk] = (int)i;
+  }
+  memcpy(h->table_host.data(), table_host, h->table_host.size() * sizeof(int));
+  VCL_CUDA_OK(cudaMemcpyAsync(h->d_table, h->table_host.data(), h->table_host.size() * sizeof(int),
+                              cudaMemcpyHostToDevice, as_stream(stream)));
+  return 0;
+}
+
+int vcl_kv_block_copy(vcl_handle* h, int block, int write, void* buf, void* stream) {
+  VCL_REQUIRE(h && buf, "vcl_kv_block_copy: null argument");
+  VCL_REQUIRE(h->paged(), "vcl_kv_block_copy: the handle has a contiguous KV cache (kv_blocks 0)");
+  VCL_REQUIRE(block >= 0 && block < h->cfg.kv_blocks, "vcl_kv_block_copy: block %d outside 0..%d", block,
+              h->cfg.kv_blocks - 1);
+  bf16* blk = h->pool + (size_t)block * h->block_elems();
+  const size_t bytes = h->block_elems() * sizeof(bf16);
+  cudaStream_t st = as_stream(stream);
+  if (write) VCL_CUDA_OK(cudaMemcpyAsync(blk, buf, bytes, cudaMemcpyDefault, st));
+  else VCL_CUDA_OK(cudaMemcpyAsync(buf, blk, bytes, cudaMemcpyDefault, st));
   return 0;
 }
 

@@ -49,6 +49,35 @@ class vcl_config(Structure):
     ]
 
 
+class vcl_config_ex(vcl_config):
+    """The whole C vcl_config: the fields above, then the trailing kv_blocks (0: the contiguous KV cache; > 0: a paged
+    cache of that many 128-column blocks). Engine always passes this struct to vcl_create; a plain vcl_config is
+    copied into one, with kv_blocks from Engine's argument."""
+    _fields_ = [("kv_blocks", c_int32)]
+
+
+KV_BLOCK_COLS = 128          # cache columns per block of a paged KV cache
+
+
+def kv_block_bytes(llm_layers: int, llm_heads: int) -> int:
+    """Bytes of one block of a paged KV cache: [layer][K | V][head][128 columns][128 dims] bf16"""
+    return 2 * int(llm_layers) * int(llm_heads) * KV_BLOCK_COLS * 128 * 2
+
+
+def check_kv_blocks(kv_blocks):
+    """kv_blocks of a paged cache -> int (None -> 0, the contiguous cache). Raises ValueError for anything else than
+    None or an int >= 2 (block 0 is the park block)."""
+    if kv_blocks is None:
+        return 0
+    try:
+        n = None if isinstance(kv_blocks, bool) else operator.index(kv_blocks)
+    except TypeError:
+        n = None
+    if n is None or n < 2:
+        raise ValueError(f"kv_blocks={kv_blocks!r}: None (contiguous cache) or an int >= 2 (block 0 is the park block)")
+    return n
+
+
 def slot_capacity(max_batch: int, max_slots=None) -> int:
     """The engine's in-flight cache slots: max_slots, or min(max_batch, 16) for None. Raises ValueError for any
     other value outside 1 .. min(max_batch, 64) (vcl_create would reject it; its 0 is spelled None here)."""
@@ -103,6 +132,8 @@ _SIGNATURES = {
                                      POINTER(c_uint64), c_void_p]),
     "vcl_launch_count": (ctypes.c_longlong, []),
     "vcl_kv_cache_copy": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "vcl_llm_set_block_table": (c_int, [c_void_p, POINTER(c_int32), c_void_p]),
+    "vcl_kv_block_copy": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "vcl_op_decode_attention": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                         c_void_p, c_void_p, c_float, c_int, c_void_p]),
     "vcl_op_cross_entropy": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
@@ -349,8 +380,14 @@ def launch_count() -> int:
 class Engine:
     """Owns one vcl_handle (one per process / GPU)."""
 
-    def __init__(self, cfg: vcl_config):
-        self.cfg = cfg
+    def __init__(self, cfg: vcl_config, kv_blocks: int | None = None):
+        """cfg: a vcl_config (or vcl_config_ex). kv_blocks: > 0 makes the KV cache paged (vcl_config.kv_blocks);
+        None keeps cfg's own (0 for a plain vcl_config)."""
+        ex = vcl_config_ex()
+        ctypes.memmove(ctypes.addressof(ex), ctypes.addressof(cfg), ctypes.sizeof(cfg))
+        if kv_blocks is not None:
+            ex.kv_blocks = int(kv_blocks)
+        cfg = self.cfg = ex
         self._h = c_void_p()
         check(lib().vcl_create(ctypes.byref(self._h), ctypes.byref(cfg)))
         g = cfg.image_size // cfg.patch_size
@@ -555,6 +592,52 @@ class Engine:
         shape = self._cache_shape()
         assert tuple(k.shape) == shape and tuple(v.shape) == shape and k.dtype == v.dtype == torch.bfloat16
         check(lib().vcl_kv_cache_copy(self._h, int(layer), 1, ptr(k), ptr(v), cur_stream()))
+
+    # ---- paged KV cache (cfg.kv_blocks > 0) ----
+    @property
+    def kv_blocks(self) -> int:
+        return int(self.cfg.kv_blocks)
+
+    @property
+    def n_slots(self) -> int:
+        """The engine's cache slots (vcl_config.max_slots, 0 meaning min(max_batch, 16))"""
+        return int(self.cfg.max_slots) or min(int(self.cfg.max_batch), 16)
+
+    @property
+    def table_row(self) -> int:
+        """Blocks per slot in the block table: ceil(max_seq / 128)"""
+        return (int(self.cfg.max_seq) + KV_BLOCK_COLS - 1) // KV_BLOCK_COLS
+
+    @property
+    def block_bytes(self) -> int:
+        return kv_block_bytes(self.cfg.llm_layers, self.cfg.llm_heads)
+
+    def block_shape(self):
+        """A block as a tensor shape: [layers, 2 (K, V), heads, 128 columns, 128 dims] bf16"""
+        c = self.cfg
+        return (c.llm_layers, 2, c.llm_heads, KV_BLOCK_COLS, 128)
+
+    def set_block_table(self, table):
+        """Write the whole block table (vcl_llm_set_block_table): n_slots rows of table_row block indices (nested
+        lists, a numpy array or a tensor on any device). Column c of slot s then lives in block table[s][c // 128]."""
+        vals = table.tolist() if hasattr(table, "tolist") else table
+        flat = [int(b) for row in vals for b in row]
+        if len(vals) != self.n_slots or len(flat) != self.n_slots * self.table_row:
+            raise VclError(f"the block table is [{self.n_slots}][{self.table_row}]")
+        n = len(flat)
+        check(lib().vcl_llm_set_block_table(self._h, (c_int32 * n)(*flat), cur_stream()))
+
+    def swap_buffer(self):
+        """A pinned host buffer for one block (kv_block_copy), [block_shape()] bf16"""
+        return torch.empty(self.block_shape(), dtype=torch.bfloat16, pin_memory=True)
+
+    def kv_block_copy(self, block, buf, write=False):
+        """Copy block `block` whole into buf (write=False) or from buf into the pool (vcl_kv_block_copy). buf: a
+        contiguous CUDA tensor or pinned host tensor of block_bytes bytes (e.g. torch.empty(block_shape(), bf16))."""
+        assert buf.is_contiguous() and buf.numel() * buf.element_size() == self.block_bytes
+        assert buf.is_cuda or buf.is_pinned(), "the block buffer must be device memory or pinned host memory"
+        check(lib().vcl_kv_block_copy(self._h, int(block), int(bool(write)), c_void_p(buf.data_ptr()), cur_stream()))
+        return buf
 
     # ---- cache slots (in-flight batching) ----
     def slot_prefill(self, slot, ids, video_feats, vid_start, tok_out=None):

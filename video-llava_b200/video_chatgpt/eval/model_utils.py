@@ -62,13 +62,13 @@ def _load_weight_files(directory):
 
 
 def initialize_model(model_name, projection_path=None, max_batch=1, max_seq=2048, llm_weight_format="bf16",
-                     max_slots=None):
+                     max_slots=None, kv_blocks=None):
     from transformers import AutoTokenizer, CLIPImageProcessor
     model_name = os.path.expanduser(model_name)
     tokenizer = AutoTokenizer.from_pretrained(model_name)
     model = VideoChatGPTLlamaForCausalLM.from_pretrained(model_name, use_cache=True, max_batch=max_batch,
                                                          max_seq=max_seq, llm_weight_format=llm_weight_format,
-                                                         max_slots=max_slots)
+                                                         max_slots=max_slots, kv_blocks=kv_blocks)
     tower_dir = model.config.mm_vision_tower
     image_processor = CLIPImageProcessor.from_pretrained(tower_dir)
 

@@ -298,13 +298,21 @@ class VideoChatGPTLlamaForCausalLM:
     config_class = VideoChatGPTConfig
 
     def __init__(self, config: VideoChatGPTConfig, clip_config=None, max_batch: int = 1, max_seq: int | None = None,
-                 clip_run_layers: int | None = None, llm_weight_format: str = "bf16", max_slots: int | None = None):
+                 clip_run_layers: int | None = None, llm_weight_format: str = "bf16", max_slots: int | None = None,
+                 kv_blocks: int | None = None):
         """llm_weight_format: "bf16", or "fp8_e4m3" to hold the language model's streamed matrices as E4M3 codes
         with power-of-two row scales (vcl_load_llm_weights_ex): decode reads half the weight bytes, and every
         output is that of the bf16 engine on the dequantized weights.
         max_slots: the KV-cache slots generate_requests keeps in flight, 1 .. min(max_batch, 64); None means
-        min(max_batch, 16). A capacity only: which decode kernel runs depends on the clip count of each call."""
+        min(max_batch, 16). A capacity only: which decode kernel runs depends on the clip count of each call.
+        kv_blocks: None keeps the contiguous KV cache (every slot holds max_seq columns). An int >= 2 makes the cache
+        PAGED: a pool of kv_blocks blocks of 128 columns (vcl_config.kv_blocks), which the running requests of
+        generate_requests take as they grow; block 0 is the park block, so kv_blocks - 1 are usable. A paged model
+        serves generate_requests only (generate / forward / generate_continue raise NotImplementedError), with
+        prompts of at most 512 tokens, and returns exactly what the contiguous model returns."""
         vn.weight_format_code(llm_weight_format)          # ValueError before anything else
+        self._kv_blocks = vn.check_kv_blocks(kv_blocks)
+        self.last_kv_stats = None
         self._n_slots = vn.slot_capacity(max_batch, max_slots)
         self._max_slots = 0 if max_slots is None else self._n_slots
         self._llm_weight_format = llm_weight_format
@@ -410,7 +418,8 @@ class VideoChatGPTLlamaForCausalLM:
             k.n_temporal = 100
             k.max_frames, k.max_batch, k.max_seq = 100, self._max_batch, self._max_seq
             k.max_slots = self._max_slots
-            self._engine = vn.Engine(k)
+            # a paged cache is the trailing vcl_config.kv_blocks (vcl_native.vcl_config_ex)
+            self._engine = vn.Engine(k, kv_blocks=self._kv_blocks) if self._kv_blocks else vn.Engine(k)
             self._clip_loaded = self._llm_loaded = False
         if need_clip and not self._clip_loaded:
             if not self._clip_state:
@@ -462,6 +471,11 @@ class VideoChatGPTLlamaForCausalLM:
         return torch.tensor(starts, dtype=torch.int32, device="cuda")
 
     # ---- forward / generate ----------------------------------------------------------------
+    def _not_paged(self, what):
+        if self._kv_blocks:
+            raise NotImplementedError(f"{what}: this model has a paged KV cache (kv_blocks={self._kv_blocks}), which "
+                                      "serves generate_requests only")
+
     @torch.no_grad()
     def forward(self, input_ids=None, attention_mask=None, past_key_values=None, inputs_embeds=None, labels=None,
                 use_cache=None, output_attentions=None, output_hidden_states=None,
@@ -469,6 +483,7 @@ class VideoChatGPTLlamaForCausalLM:
         """logits_to_keep (transformers 5.x's name): 1, the default, returns the last position's logits [B,1,V];
         0 returns every position's [B,S,V]. labels [B,S] (train.py's IGNORE_INDEX -100 on prompt and padding)
         returns the reference's loss, a 0-d bf16 tensor, with the logits of every position (vcl_llm_score)."""
+        self._not_paged("forward")
         if inputs_embeds is not None or output_attentions:
             raise NotImplementedError("inference path only: input_ids in, logits out")
         if logits_to_keep not in (0, 1):
@@ -602,6 +617,7 @@ class VideoChatGPTLlamaForCausalLM:
         and stopping criteria are applied on the host between loops of _GREEDY_CHUNK tokens, token by token as
         the stepwise path does. Each row's tokens depend on its seed and positions only. Without a seed,
         do_sample=True keeps the stepwise path and torch's RNG (torch.manual_seed)."""
+        self._not_paged("generate")
         seeded = do_sample and seed is not None
         if seeded:
             temperature, top_k, seed = self._sampling_args(temperature, top_k, seed)
@@ -744,7 +760,10 @@ class VideoChatGPTLlamaForCausalLM:
         admitted slots' entries of the engine's sampling table with one set_sampling call, and every slot is
         greedy again when the call returns. A request's tokens depend on its seed and positions only: not on its
         slot, its neighbours, the queue order or the admission mode. Sampling without any seed is not supported
-        in flight (only the stepwise generate draws from torch's RNG)."""
+        in flight (only the stepwise generate draws from torch's RNG).
+        A paged model (kv_blocks) gives each request only the 128-column blocks it has written, so the requests in
+        flight follow their actual lengths: see _schedule_paged. The results are the same bit for bit; afterwards
+        self.last_kv_stats holds the preemptions, the bytes swapped out and the peak blocks in use."""
         for i, r in enumerate(requests):
             r = r if isinstance(r, dict) else {}
             if r.get("do_sample", do_sample) and r.get("seed", seed) is None:
@@ -759,11 +778,15 @@ class VideoChatGPTLlamaForCausalLM:
         eng = self._ensure_engine(need_llm=True)
         samp = dict(do_sample=do_sample, temperature=temperature, top_k=top_k, seed=seed)
         reqs = [self._request(i, r, max_new_tokens, stopping_criteria, eng.NV, samp) for i, r in enumerate(requests)]
+        if self._kv_blocks:
+            self._check_paged(reqs)
         sampling = any(r.temperature > 0 for r in reqs)
         eos, _ = self._eos_pad(eos_token_id, None)
         self._last_out, self._pos = None, 0
         n_slots = min(n_slots, len(reqs))
         try:
+            if self._kv_blocks:
+                return self._schedule_paged(eng, reqs, n_slots, packed_admission, sampling, eos)
             return self._schedule(eng, reqs, n_slots, packed_admission, sampling, eos)
         finally:
             if sampling:
@@ -839,6 +862,151 @@ class VideoChatGPTLlamaForCausalLM:
                                     [r.vid_start for _, r in packed])
             first[torch.tensor(slots, device=dev)] = tok
 
+    def _check_paged(self, reqs):
+        """The requests a paged cache takes, checked on the host before any device work: a prompt of at most
+        min(512, max_seq) tokens (a paged engine prefills packed), and at most kv_blocks - 1 blocks for the prompt and
+        every new token, so that a request alone always fits the pool and the scheduler always makes progress."""
+        C, usable = vn.KV_BLOCK_COLS, self._kv_blocks - 1
+        s_lim = min(self._PACKED_MAX_S, self._max_seq)
+        for i, r in enumerate(reqs):
+            if r.S > s_lim:
+                raise ValueError(f"request {i}: prompt of {r.S} tokens; a paged KV cache takes prompts of at most "
+                                 f"{s_lim} tokens (the packed prefill)")
+            need = -(-(r.S + r.n) // C)
+            if need > usable:
+                raise ValueError(f"request {i}: prompt {r.S} + max_new_tokens {r.n} needs {need} blocks of {C} columns, "
+                                 f"more than the pool's {usable} (kv_blocks {self._kv_blocks}, block 0 is the park block)")
+
+    def _schedule_paged(self, eng, reqs, n_slots, packed_admission, sampling, eos):
+        """The admission / decode loop of generate_requests on a paged KV cache. The host keeps a free list and each
+        slot's row of the block table (block 0, the park block, wherever no request owns a block), and writes the
+        whole table to the engine before every prefill and every decode chunk.
+        - Blocks. A running request at position pos, decoding a chunk of m steps, owns the blocks of columns
+          0 .. min(pos + m, S + n) - 1: every column the chunk writes that the request can still read (past S + n - 1
+          the request has all its tokens; those columns of a chunk land in the park block or in its own last block).
+        - Admission. Swapped-out requests resume first, oldest admission first, then queued requests in queue order
+          (none overtakes another): each into a free slot when the free list covers its blocks for one chunk.
+        - Preemption. When a chunk's growth is not covered, the most recently admitted running request is swapped out
+          (its written blocks copied to pinned host memory, its blocks freed, its slot parked) until it is. Its
+          position, pending token and sampling entry stay on the host; it resumes into any free slot and free blocks,
+          restored exactly, and its tokens depend on its seed and positions only.
+        _check_paged guarantees that the oldest running request alone always fits."""
+        dev, C, K = self.device, vn.KV_BLOCK_COLS, self._SLOT_CHUNK
+        table = [[0] * eng.table_row for _ in range(eng.n_slots)]    # every slot of the engine, parked
+        free = list(range(eng.kv_blocks - 1, 0, -1))                  # pop() takes the lowest block
+        results = [None] * len(reqs)
+        queue = collections.deque(range(len(reqs)))
+        owner = [None] * n_slots            # request of each slot
+        pos = [0] * n_slots                 # tokens in each slot's cache; a slot without a request is parked at 0
+        unseen = [False] * n_slots          # the slot's first token has not reached the host yet
+        order = [0] * n_slots               # admission stamp of the slot's request (the latest is preempted first)
+        blocks = [[] for _ in range(n_slots)]
+        gen = {}
+        swapped = {}                        # request -> (pos, pending token, unseen, host copies of its blocks)
+        released = []                       # host buffers whose copy back may still be in flight
+        stats = dict(preemptions=0, swapped_bytes=0, peak_blocks=0, kv_blocks=eng.kv_blocks)
+        first = torch.zeros(n_slots, dtype=torch.int32, device=dev)     # the token each slot is fed next
+        stamp = 0
+
+        def cover(i, p, m):                 # blocks of columns 0 .. min(p + m, S + n) - 1
+            r = reqs[i]
+            return -(-min(p + m, r.S + r.n) // C)
+
+        def take(s, want):
+            while len(blocks[s]) < want:
+                blocks[s].append(free.pop())
+            table[s][:len(blocks[s])] = blocks[s]
+            stats["peak_blocks"] = max(stats["peak_blocks"], eng.kv_blocks - 1 - len(free))
+
+        def release(s):
+            free.extend(reversed(blocks[s]))
+            blocks[s], table[s] = [], [0] * eng.table_row
+            owner[s], pos[s] = None, 0
+
+        def swap_out(s):
+            i = owner[s]
+            saved = []
+            for b in blocks[s][:-(-pos[s] // C)]:        # the blocks that hold written columns
+                buf = eng.swap_buffer()
+                eng.kv_block_copy(b, buf)
+                saved.append(buf)
+            swapped[i] = (pos[s], int(first[s]), unseen[s], saved)
+            stats["preemptions"] += 1
+            stats["swapped_bytes"] += len(saved) * eng.block_bytes
+            release(s)
+
+        while True:
+            idle = [s for s in range(n_slots) if owner[s] is None]
+            admitted, resumed = [], []
+            while swapped and idle:
+                i = min(swapped)            # requests are first admitted in queue (= index) order
+                p, tok, uns, saved = swapped[i]
+                if len(free) < cover(i, p, K):
+                    break
+                s = idle.pop(0)
+                del swapped[i]
+                stamp += 1
+                owner[s], pos[s], unseen[s], order[s] = i, p, uns, stamp
+                take(s, cover(i, p, K))
+                for b, buf in zip(blocks[s], saved):
+                    eng.kv_block_copy(b, buf, write=True)
+                released.extend(saved)
+                first[s] = tok
+                resumed.append((s, i))
+            while not swapped and idle and queue:
+                i = queue[0]
+                if len(free) < cover(i, reqs[i].S, K):
+                    break
+                queue.popleft()
+                s = idle.pop(0)
+                stamp += 1
+                owner[s], pos[s], unseen[s], order[s], gen[i] = i, reqs[i].S, True, stamp, []
+                take(s, cover(i, reqs[i].S, K))
+                admitted.append((s, i))
+            if admitted or resumed:
+                eng.set_block_table(table)
+            if sampling and (admitted or resumed):
+                rs = [(s, reqs[i]) for s, i in admitted + resumed]
+                eng.set_sampling([s for s, _ in rs], [r.temperature for _, r in rs], [r.top_k for _, r in rs],
+                                 [r.seed for _, r in rs])
+            if admitted and packed_admission:
+                self._admit_packed(eng, [(s, reqs[i]) for s, i in admitted], first)
+            elif admitted:
+                for s, i in admitted:
+                    r = reqs[i]
+                    feats = None if r.feats is None else r.feats.to(dev)
+                    vs = torch.tensor([r.vid_start], dtype=torch.int32, device=dev)
+                    eng.slot_prefill(s, r.ids.to(dev), feats, vs, tok_out=first[s:s + 1])
+            active = [s for s in range(n_slots) if owner[s] is not None]
+            if not active:
+                eng.set_block_table(table)      # every slot parked again
+                self.last_kv_stats = stats
+                return results
+            m = min([K] + [self._max_seq - pos[s] for s in active])
+            # growth, oldest admission first; preempt the latest running request while the free list falls short
+            for s in sorted(active, key=lambda t: order[t]):
+                while owner[s] is not None and len(free) < cover(owner[s], pos[s], m) - len(blocks[s]):
+                    swap_out(max((t for t in range(n_slots) if owner[t] is not None), key=lambda t: order[t]))
+                if owner[s] is not None:
+                    take(s, cover(owner[s], pos[s], m))
+            active = [s for s in active if owner[s] is not None]
+            eng.set_block_table(table)
+            out = eng.slot_decode(first, pos, m + 1)
+            first = out[:, m].contiguous()
+            host = out.tolist()
+            released.clear()                # the stream has passed every copy enqueued before the decode
+            for s in active:
+                i = owner[s]
+                r = reqs[i]
+                pos[s] += m
+                for t in (host[s] if unseen[s] else host[s][1:]):
+                    gen[i].append(t)
+                    if self._request_done(r, gen[i], eos):
+                        results[i] = torch.cat([r.ids, torch.tensor(gen[i], dtype=torch.int64)])[None].to(dev)
+                        release(s)
+                        break
+                unseen[s] = False
+
     def _request(self, i, r, max_new_tokens, stopping_criteria, n_vid, samp=None):
         """One request of generate_requests, checked on the host -> (ids [S] int64 on the host, S, n, feats,
         vid_start, criteria, and its sampling-table entry: temperature (0: greedy), top_k, seed)"""
@@ -894,6 +1062,7 @@ class VideoChatGPTLlamaForCausalLM:
         After a left-padded generate the cache stays padded, so every row continues its own positions; the
         new text of every row has the same length S_new (no padding inside a turn).
         seed: do_sample=True samples on the device as generate(seed=...) does."""
+        self._not_paged("generate_continue")
         if getattr(self, "_last_out", None) is None:
             raise ValueError("generate_continue: no previous generate() to continue")
         seeded = do_sample and seed is not None
