@@ -260,6 +260,28 @@ int vcl_llm_slots_prefill(vcl_handle* h, int n, const int32_t* slots_host, const
                           const int64_t* ids, const void* video_feats, const int32_t* vid_start,
                           int32_t* next_tok, void* stream);
 
+/* Chunked prefill on a PAGED cache (vcl_config.kv_blocks > 0; rejected otherwise): prompts longer than 512 tokens
+ * run through the layer stack in chunks of at most 512 rows, each attending the cache columns its earlier chunks
+ * left there. Sequence i is rows start_host[i] .. start_host[i] + len_host[i] - 1 of a prompt of total_host[i]
+ * tokens in slot slots_host[i] (all HOST memory, [n] int32); columns 0 .. start_host[i] - 1 of that slot must hold
+ * the prompt's earlier chunks. ids is the packed [sum len_i] int64 of the chunks. video_feats / vid_start are those
+ * of vcl_llm_slots_prefill, vid_start[i] counted from the prompt's first token: row p of the prompt takes feature row
+ * p - vid_start[i] - 1 when that lies in the span, so a span may straddle a chunk boundary. RoPE positions and cache
+ * columns are absolute (start_i + j). The attention follows the contiguous engine's choice for the whole prompt:
+ * total_i > 512 runs the mma.sync flash kernel of a one-shot prefill over more than 512 keys, with each key tile read
+ * through the block table; total_i <= 512 needs start_i = 0 and len_i = total_i (vcl_llm_slots_prefill) and runs the
+ * wgmma kernel; one launch per kernel kind present. So after the last chunk the slot's columns 0 .. total_i - 1 and
+ * its first token equal vcl_llm_slot_prefill of the whole prompt on a contiguous handle, bit for bit, however the
+ * prompt was cut. next_tok [n] int32: the token at each chunk's last row, drawn with entry slots_host[i] of the
+ * sampling table at counter start_i + len_i (only the last chunk's token is the prompt's first token). Rejected
+ * before any device work, the handle untouched: n outside 1 .. max_slots, a slot outside 0 .. max_slots-1 or given
+ * twice, start_i not a multiple of 64, len_i outside 1 .. 512, start_i + len_i > total_i, total_i > max_seq, a
+ * prompt of at most 512 tokens that is not whole, and sum len_i beyond the activations (max_batch * min(max_seq,
+ * 512) rows). */
+int vcl_llm_slots_prefill_chunk(vcl_handle* h, int n, const int32_t* slots_host, const int32_t* start_host,
+                                const int32_t* len_host, const int32_t* total_host, const int64_t* ids,
+                                const void* video_feats, const int32_t* vid_start, int32_t* next_tok, void* stream);
+
 /* vcl_llm_decode_loop with a position per slot: slot b (0 <= b < n_slots) is fed first_tok[b] at position
  * pos_host[b] (HOST memory: the number of tokens its cache holds), then runs n_new-1 greedy steps;
  * out_tokens is [n_slots, n_new] int32, first_tok included. Every pos_host[b] + n_new - 1 must be <= max_seq
@@ -303,7 +325,8 @@ int vcl_llm_set_sampling(vcl_handle* h, int n, const int32_t* clips_host, const 
  * writes pos .. pos + n_new - 2.
  *
  * A paged handle serves vcl_llm_slots_prefill, vcl_llm_slot_prefill (run as a packed prefill of one prompt, so
- * prompts are limited to min(512, max_seq) tokens), vcl_llm_slot_decode and vcl_llm_set_sampling. Every static
+ * prompts are limited to min(512, max_seq) tokens), vcl_llm_slots_prefill_chunk (prompts up to max_seq tokens, in
+ * chunks of at most 512 rows), vcl_llm_slot_decode and vcl_llm_set_sampling. Every static
  * entry point (vcl_llm_prefill(_padded, _states, _append), _decode_step, _decode_loop, _generate(_padded), _score)
  * and vcl_kv_cache_copy is rejected. Its LLM activations are sized for max_batch * min(max_seq, 512) rows, the
  * most a packed prefill uses.

@@ -2,6 +2,7 @@
 
     python tools/bench_paged.py --model {7b,13b} --arm {contig,paged} [--requests 256] [--max-new 1024]
                                 [--stop-min 32] [--stop-max 512] [--budget-gib G] [--out DIR]
+                                [--transcript-tokens LO-HI]
 
 The workload is video_chatgpt_infer's: max_new_tokens 1024, sampling at temperature 0.2 with top-k 50 (seeded on the
 device), and prompts of 400..448 tokens with video (bench.synthetic_prompt_ids, random pooled features). Random
@@ -19,6 +20,13 @@ Each arm runs generate_requests once as a warm-up over the first 64 requests, th
 clock ended by a stream synchronise. Prints one JSON line: the card name and power limit, slots, kv_blocks,
 requests/s, generated tokens/s, the engine's resident memory, and (paged) preemptions, bytes swapped to host memory
 and the peak blocks in use.
+
+--transcript-tokens LO-HI: the --use_asr prompts of the reference's eval scripts. Each prompt gets a transcript of a
+seeded LO..HI tokens appended, max_seq is 2048, and max_new_tokens is capped so that the longest prompt fits. The paged
+arm then runs generate_requests(chunked_prefill=True) and also reports the chunked prompts and chunk calls. Both arms
+then also report the share of the wall time spent in prefill calls (each one timed between two stream synchronises),
+and the time of one 1024-token prompt: the contiguous engine's one-shot slot_prefill, or the paged engine's two
+512-row chunk calls (median of 10 after a warm-up).
 """
 import argparse
 import json
@@ -73,12 +81,15 @@ class StopAt:
         return ids.shape[1] - self.start >= self.n
 
 
-def make_requests(n, stop_min, stop_max, max_new):
+def make_requests(n, stop_min, stop_max, max_new, transcript=None):
     rnd = random.Random(0)
     reqs = []
     for i in range(n):
         S = rnd.randint(400, S_MAX)
         ids = bench.synthetic_prompt_ids(seed=1 + i, n_pre=63 - (S_MAX - S))[0]
+        if transcript:
+            t = rnd.randint(*transcript)
+            ids = torch.cat([ids, torch.randint(3, 32000, (t,), generator=torch.Generator().manual_seed(5000 + i))])
         feats = (torch.randn(N_VID, 1024, device="cuda", generator=torch.Generator(device="cuda").manual_seed(100 + i))
                  * 0.5).to(torch.bfloat16)
         reqs.append(dict(input_ids=ids, video_spatio_temporal_features=feats, max_new_tokens=max_new,
@@ -88,6 +99,36 @@ def make_requests(n, stop_min, stop_max, max_new):
 
 def with_criteria(reqs):
     return [dict({k: v for k, v in r.items() if k != "stop"}, stopping_criteria=[StopAt(r["stop"])]) for r in reqs]
+
+
+def time_1024(model, paged, reps=10):
+    """ms of one 1024-token text prompt into slot 0: one-shot slot_prefill (contiguous) or two 512-row chunk calls
+    into a fresh table row (paged), median of reps after a warm-up"""
+    eng = model._engine
+    ids = torch.randint(3, 32000, (1024,), generator=torch.Generator().manual_seed(7)).to("cuda")
+    vs = torch.tensor([vn.NO_VIDEO], dtype=torch.int32, device="cuda")
+    if paged:
+        table = [[0] * eng.table_row for _ in range(eng.n_slots)]
+        table[0][:8] = list(range(1, 9))
+        eng.set_block_table(table)
+
+    def once():
+        if paged:
+            for st in (0, 512):
+                eng.slots_prefill_chunk([0], [st], [1024], [ids[st:st + 512]], [None], [0])
+        else:
+            eng.slot_prefill(0, ids[None], None, vs)
+    once()
+    times = []
+    for _ in range(reps):
+        torch.cuda.synchronize()
+        t = time.perf_counter()
+        once()
+        torch.cuda.synchronize()
+        times.append((time.perf_counter() - t) * 1e3)
+    if paged:
+        eng.set_block_table([[0] * eng.table_row for _ in range(eng.n_slots)])
+    return sorted(times)[reps // 2]
 
 
 def main():
@@ -100,7 +141,14 @@ def main():
     ap.add_argument("--stop-max", type=int, default=512)
     ap.add_argument("--budget-gib", type=float, default=None)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--transcript-tokens", default=None, metavar="LO-HI")
     a = ap.parse_args()
+    transcript = tuple(int(x) for x in a.transcript_tokens.split("-")) if a.transcript_tokens else None
+    max_seq = 2048 if transcript else MAX_SEQ
+    if transcript:
+        a.max_new = min(a.max_new, max_seq - S_MAX - transcript[1])
+        a.stop_max = min(a.stop_max, a.max_new)
+        a.stop_min = min(a.stop_min, a.stop_max)
     torch.cuda.init()
     D, F, L, H = shapes(a.model)
     free0 = torch.cuda.mem_get_info()[0]
@@ -109,7 +157,7 @@ def main():
     budget = int(a.budget_gib * GIB) if a.budget_gib else free0 - 2 * GIB - weights_in
     col = 2 * L * H * 128 * 2                                  # one cache column of one sequence, K and V
     if a.arm == "contig":
-        per_slot = col * MAX_SEQ + MAX_SEQ * act_row_bytes(a.model)
+        per_slot = col * max_seq + max_seq * act_row_bytes(a.model)
         slots = min(64, (budget - fixed_bytes(a.model, 64)) // per_slot)
         max_batch, kv_blocks = slots, None
     else:
@@ -120,7 +168,7 @@ def main():
         raise SystemExit(f"budget {budget / GIB:.1f} GiB leaves no cache")
     cfg = VideoChatGPTConfig(hidden_size=D, intermediate_size=F, num_hidden_layers=L, num_attention_heads=H,
                              vocab_size=V, use_mm_proj=True, mm_hidden_size=1024)
-    model = VideoChatGPTLlamaForCausalLM(cfg, clip_config={}, max_batch=int(max_batch), max_seq=MAX_SEQ,
+    model = VideoChatGPTLlamaForCausalLM(cfg, clip_config={}, max_batch=int(max_batch), max_seq=max_seq,
                                          max_slots=int(slots), kv_blocks=None if kv_blocks is None else int(kv_blocks))
     vc = model.get_model().vision_config
     vc.vid_patch_token, vc.vid_start_token, vc.vid_end_token, vc.use_vid_start_end = 32000, 32001, 32002, True
@@ -134,10 +182,24 @@ def main():
     del llm
     torch.cuda.empty_cache()
 
-    reqs = make_requests(a.requests, a.stop_min, a.stop_max, a.max_new)
+    reqs = make_requests(a.requests, a.stop_min, a.stop_max, a.max_new, transcript)
     kw = dict(eos_token_id=None, do_sample=True, temperature=0.2, top_k=50, seed=1234, packed_admission=True)
+    if transcript and kv_blocks:
+        kw["chunked_prefill"] = True
     model.generate_requests(with_criteria(reqs[:64]), **kw)            # warm-up: graphs, allocator
     torch.cuda.synchronize()
+    eng = model._engine
+    prefill_s = [0.0]
+    if transcript:                                   # time every prefill call between two stream synchronises
+        for name in ("slot_prefill", "slots_prefill", "slots_prefill_chunk"):
+            def timed(*args, _f=getattr(eng, name), **kwargs):
+                torch.cuda.synchronize()
+                t = time.perf_counter()
+                r = _f(*args, **kwargs)
+                torch.cuda.synchronize()
+                prefill_s[0] += time.perf_counter() - t
+                return r
+            setattr(eng, name, timed)
     t0 = time.perf_counter()
     outs = model.generate_requests(with_criteria(reqs), **kw)
     torch.cuda.synchronize()
@@ -152,7 +214,11 @@ def main():
     if kv_blocks:
         st = model.last_kv_stats
         res.update(preemptions=st["preemptions"], swapped_gb=round(st["swapped_bytes"] / 1e9, 2),
-                   peak_blocks=st["peak_blocks"])
+                   peak_blocks=st["peak_blocks"], chunked_prefills=st["chunked_prefills"],
+                   chunk_calls=st["chunk_calls"])
+    if transcript:
+        res.update(transcript_tokens=a.transcript_tokens, max_new=a.max_new,
+                   prefill_share=round(prefill_s[0] / wall, 3), prompt_1024_ms=round(time_1024(model, kv_blocks), 2))
     line = json.dumps(res)
     print(line)
     if a.out:

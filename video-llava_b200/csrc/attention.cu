@@ -10,7 +10,9 @@
 //     bf16 before the PV matmul. The score roundings are reproduced; the probabilities are rounded
 //     to bf16 un-normalised (flash form), the one place this kernel differs from eager by design.
 //     It serves the 336-px ViT tower (S = 577, read straight out of the fused q|k|v activation,
-//     launch_attention_vit), longer prompts and continued prefills beyond 512 keys; the ViT's S = 257 runs in
+//     launch_attention_vit), longer prompts and continued prefills beyond 512 keys, and the chunks of prompts over
+//     512 tokens in a paged cache (vcl_llm_slots_prefill_chunk: packed, each key tile read through the block
+//     table, the same tiles and arithmetic as the one-shot prefill of the whole prompt); the ViT's S = 257 runs in
 //     attention_tc.cu, the causal hd-128 prefill up to 512 keys in attention_prefill_tc.cu (both wgmma, exact
 //     full-row softmax).
 //
@@ -77,8 +79,17 @@ __device__ __forceinline__ void load_tile(uint32_t sbase, const bf16* g, long lo
 // PAD (causal only): left-padded clips (a.n_pad): a real query (cache column >= n_pad[b]) attends keys n_pad[b] ..
 // its own column, and a tile of real queries starts at the first key tile that holds a real key; a pad query
 // attends causally
-template <int HD, bool CAUSAL, bool PAD = false>
+// PACK: packed sequences (a.pack, kernels.h) on a paged cache (PAGED, a.pages): blockIdx.z is sequence i, whose
+// pack_end_i - pack_start_i queries start at its row offset and sit at absolute positions start_i .. ; its keys are
+// columns 0 .. end_i - 1 of slot_i (q_off = start_i, S_kv = end_i). Sequences with pack_len > 0 belong to the wgmma
+// kernel and are skipped. Key tile jt is the 64 columns at offset (jt % 2) * 64 of block table[slot_i][jt / 2].
+// With start_i a multiple of 64 a query tile covers the rows, walks the key tiles and applies the masks of the same
+// tile of a one-shot prefill of the whole prompt (S = S_kv = end, q_off = 0): keys past end_i are past every query
+// of the chunk too, so both mask them causally, and the zero-filled columns past end_i only meet P = 0.
+template <int HD, bool CAUSAL, bool PAD = false, bool PACK = false, bool PAGED = false>
 __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
+  static_assert(PACK == PAGED && (!PACK || (CAUSAL && !PAD && HD == 128)),
+                "packed sequences: causal, unpadded hd-128 attention on a paged cache");
   extern __shared__ __align__(128) uint8_t smem[];
   constexpr int TILE_BYTES = 64 * HD * 2;
   const uint32_t sQ = smem_u32(smem);
@@ -87,13 +98,37 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
 
   const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int S = a.S;                                  // queries
-  const int S_kv = a.S_kv > 0 ? a.S_kv : a.S;         // keys (a continued prefill attends to the cache too)
-  const int q_off = a.q_off;                          // absolute position of query 0 (causal mask)
+  int S = a.S;                                        // queries
+  int S_kv = a.S_kv > 0 ? a.S_kv : a.S;               // keys (a continued prefill attends to the cache too)
+  int q_off = a.q_off;                                // absolute position of query 0 (causal mask)
   const int q0 = qt * 64;
-  const bf16* qg = a.q + (long long)b * a.q_sb + (long long)h * a.q_sh;
-  const bf16* kg = a.k + (long long)b * a.k_sb + (long long)h * a.k_sh;
-  const bf16* vg = a.v + (long long)b * a.v_sb + (long long)h * a.v_sh;
+  long long q_base = (long long)b * a.q_sb, o_base = (long long)b * a.o_sb;
+  int slot = 0;
+  if constexpr (PACK) {
+    if (__ldg(pack_len(a.pack) + b) != 0) return;     // a wgmma sequence (before the first barrier: the CTA leaves)
+    q_off = __ldg(pack_start(a.pack) + b);
+    S_kv = __ldg(pack_end(a.pack) + b);
+    S = S_kv - q_off;
+    if (q0 >= S) return;
+    const long long off = __ldg(pack_off(a.pack) + b);
+    q_base = off * a.q_ss; o_base = off * a.o_ss;
+    slot = __ldg(pack_slot(a.pack) + b);
+  }
+  const bf16* qg = a.q + q_base + (long long)h * a.q_sh;
+  const bf16* kg = a.k + (PAGED ? 0 : (long long)b * a.k_sb) + (long long)h * a.k_sh;
+  const bf16* vg = a.v + (PAGED ? 0 : (long long)b * a.v_sb) + (long long)h * a.v_sh;
+  // key tile jt (keys jt * 64 ..; keys >= S_kv are zero-filled, never read)
+  auto load_kv = [&](uint32_t sk, uint32_t sv, int jt) {
+    if constexpr (PAGED) {
+      const long long pg = (long long)__ldg(a.pages.table + slot * a.pages.row + (jt >> 1)) * a.pages.blk +
+                           (long long)(jt & 1) * 64 * a.k_ss;
+      load_tile<HD>(sk, kg + pg, a.k_ss, 0, S_kv - jt * 64);
+      load_tile<HD>(sv, vg + pg, a.v_ss, 0, S_kv - jt * 64);
+    } else {
+      load_tile<HD>(sk, kg, a.k_ss, jt * 64, S_kv);
+      load_tile<HD>(sv, vg, a.v_ss, jt * 64, S_kv);
+    }
+  };
 
   const int n_tiles_all = (S_kv + 63) / 64;
   const int n_tiles = CAUSAL ? min(n_tiles_all, (q_off + q0 + 63) / 64 + 1) : n_tiles_all;
@@ -101,8 +136,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
   const int jt0 = (PAD && q_off + q0 >= k_pad) ? k_pad / 64 : 0;     // key tiles below hold pad keys only
 
   load_tile<HD>(sQ, qg, a.q_ss, q0, S);
-  load_tile<HD>(sK, kg, a.k_ss, jt0 * 64, S_kv);
-  load_tile<HD>(sV, vg, a.v_ss, jt0 * 64, S_kv);
+  load_kv(sK, sV, jt0);
   cp_async_commit();
 
   uint32_t qf[HD / 16][4];
@@ -122,8 +156,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
   for (int jt = jt0; jt < n_tiles; ++jt) {
     const int buf = (jt - jt0) & 1;
     if (jt + 1 < n_tiles) {
-      load_tile<HD>(sK + (buf ^ 1) * TILE_BYTES, kg, a.k_ss, (jt + 1) * 64, S_kv);
-      load_tile<HD>(sV + (buf ^ 1) * TILE_BYTES, vg, a.v_ss, (jt + 1) * 64, S_kv);
+      load_kv(sK + (buf ^ 1) * TILE_BYTES, sV + (buf ^ 1) * TILE_BYTES, jt + 1);
       cp_async_commit();
       cp_async_wait<1>();
     } else {
@@ -231,7 +264,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
     l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
     l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
   }
-  bf16* og = a.o + (long long)b * a.o_sb + (long long)h * a.o_sh;
+  bf16* og = a.o + (PACK ? o_base : (long long)b * a.o_sb) + (long long)h * a.o_sh;
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int qrow = qrow0 + r * 8;
@@ -247,10 +280,10 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
   }
 }
 
-template <int HD, bool CAUSAL, bool PAD = false>
+template <int HD, bool CAUSAL, bool PAD = false, bool PACK = false>
 int launch_attn_t(const AttnArgs& a, cudaStream_t stream) {
   constexpr int SMEM = 5 * 64 * HD * 2;
-  auto kern = attn_fwd_kernel<HD, CAUSAL, PAD>;
+  auto kern = attn_fwd_kernel<HD, CAUSAL, PAD, PACK, PACK>;
   dim3 grid((a.S + 63) / 64, a.H, a.B);
   kern<<<grid, 128, SMEM, stream>>>(a);
   VCL_CUDA_OK(cudaGetLastError());
@@ -266,6 +299,8 @@ int init_attention_kernels() {
   VCL_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 64 * 128 * 2));
   VCL_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 64 * 128 * 2));
   VCL_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<128, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 64 * 128 * 2));
+  VCL_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<128, true, false, true, true>,
+                                   cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 64 * 128 * 2));
   if (init_attention_tc_kernels() != 0) return -2;
   return init_attention_prefill_tc_kernels();
 }
@@ -279,8 +314,14 @@ int launch_attention(const AttnArgs& a, cudaStream_t stream) {
   VCL_REQUIRE(a.n_pad == nullptr || (a.causal && a.head_dim == 128), "attention: left padding needs causal hd-128 attention");
   VCL_REQUIRE(a.pack == nullptr || (a.causal && a.head_dim == 128 && a.n_pad == nullptr && a.S <= 512),
               "attention: packed sequences need causal hd-128 attention over at most 512 keys, unpadded");
+  VCL_REQUIRE(a.pack == nullptr || a.pack_tc || a.pack_flash, "attention: a packed launch runs at least one kernel");
+  VCL_REQUIRE(a.pack == nullptr || !a.pack_flash || a.pages.table != nullptr,
+              "attention: the packed flash kernel reads a paged cache");
   if (a.B <= 0 || a.H <= 0 || a.S <= 0) return 0;
-  if (a.pack != nullptr) return launch_attention_prefill_tc(a, stream);   // the only kernel with packed sequences
+  if (a.pack != nullptr) {   // wgmma: whole prompts of at most 512 tokens; flash: chunks of longer prompts
+    if (a.pack_tc && launch_attention_prefill_tc(a, stream) != 0) return -1;
+    return a.pack_flash ? launch_attn_t<128, true, false, true>(a, stream) : 0;
+  }
   if (attention_prefill_tc_supported(a)) return launch_attention_prefill_tc(a, stream);   // LLaMA prefill up to 512 keys
   if (a.n_pad != nullptr) return launch_attn_t<128, true, true>(a, stream);
   if (a.head_dim == 64) {

@@ -11,19 +11,25 @@ namespace vcl {
 
 typedef __nv_bfloat16 bf16;
 
-// Packed prefill (vcl_llm_slots_prefill): n <= PACK_SEQ_MAX sequences of lengths S_0 .. S_{n-1} concatenated
-// without padding into M = sum S_i rows, sequence i going to cache slot slot_i. One device int array describes the
-// layout, and every kernel of a packed prefill reads it through the accessors below:
-//   [0, 64)    row offset of sequence i     [64, 128)   its length S_i
+// Packed prefill (vcl_llm_slots_prefill / vcl_llm_slots_prefill_chunk): n <= PACK_SEQ_MAX sequences of lengths
+// S_0 .. S_{n-1} concatenated without padding into M = sum S_i rows, sequence i going to cache slot slot_i. Sequence
+// i is the rows start_i .. start_i + S_i - 1 of its prompt (start_i = 0 for a whole prompt; a chunk of a longer
+// prompt attends the columns 0 .. start_i - 1 its earlier chunks left in the cache). One device int array describes
+// the layout, and every kernel of a packed prefill reads it through the accessors below:
+//   [0, 64)    row offset of sequence i     [64, 128)   S_i when the wgmma prefill attention attends it, 0 when the
+//                                                       flash kernel does (a chunk of a prompt over 512 tokens)
 //   [128, 192) its cache slot               [192, 256)  its last row (offset + S_i - 1), whose logits give its token
-//   [256 + 2r] sequence of row r            [256 + 2r + 1] position of row r inside its sequence
+//   [256, 320) start_i                      [320, 384)  start_i + S_i: the position of the token its last row gives
+//   [384 + 2r] sequence of row r            [384 + 2r + 1] position of row r in its prompt (start_i + row in sequence)
 constexpr int PACK_SEQ_MAX = 64;
-constexpr int PACK_HEAD = 4 * PACK_SEQ_MAX;
+constexpr int PACK_HEAD = 6 * PACK_SEQ_MAX;
 inline size_t pack_elems(long long rows) { return PACK_HEAD + 2 * (size_t)rows; }
 template <class T> __host__ __device__ inline T* pack_off(T* p) { return p; }
 template <class T> __host__ __device__ inline T* pack_len(T* p) { return p + PACK_SEQ_MAX; }
 template <class T> __host__ __device__ inline T* pack_slot(T* p) { return p + 2 * PACK_SEQ_MAX; }
 template <class T> __host__ __device__ inline T* pack_last(T* p) { return p + 3 * PACK_SEQ_MAX; }
+template <class T> __host__ __device__ inline T* pack_start(T* p) { return p + 4 * PACK_SEQ_MAX; }
+template <class T> __host__ __device__ inline T* pack_end(T* p) { return p + 5 * PACK_SEQ_MAX; }
 template <class T> __host__ __device__ inline T* pack_row(T* p, long long r) { return p + PACK_HEAD + 2 * r; }   // [seq, pos]
 
 // Paged KV cache (vcl_config.kv_blocks > 0): one pool of blocks instead of the contiguous [clip][head][s_max][128]
@@ -173,11 +179,15 @@ struct AttnArgs {
   const int* n_pad = nullptr;   // causal only: [B] left padding, the key floor of real queries (or null)
   // packed rows (kernels.h, above) or null. Sequence i (i < B) has S = S_kv = S_i, q_off 0: its queries / outputs
   // are rows offset_i .. of q / o (q_sb, o_sb unused), its keys / values clip slot_i of k / v. a.S is max S_i.
-  // Always the wgmma kernel (S_i <= 512), whatever VCL_PREFILL_ATTN_FLASH says.
+  // The wgmma kernel (S_i <= 512) whatever VCL_PREFILL_ATTN_FLASH says, for every sequence with pack_len S_i > 0.
   const int* pack = nullptr;
   // packed rows only: a paged cache. Key block kb of sequence i is block table[slot_i][kb] (k / v: the layer's pool
   // bases, k_sh / v_sh the head stride inside a block, k_ss = v_ss = 128; k_sb / v_sb unused)
   KvPages pages;
+  // packed rows on a paged cache: which kernels run. pack_tc: the wgmma kernel for the sequences with pack_len > 0;
+  // pack_flash: the flash kernel (attention.cu) for those with pack_len 0, whose queries start_i .. end_i - 1 attend
+  // keys 0 .. their own position (one launch per kernel, each over every sequence; the other kind's CTAs leave)
+  bool pack_tc = true, pack_flash = false;
 };
 int launch_attention(const AttnArgs& a, cudaStream_t stream);     // dispatches to the wgmma prefill kernel when it applies
 int init_attention_kernels();

@@ -162,7 +162,8 @@ struct vcl_handle {
     if (paged()) { p.table = d_table; p.row = table_row(); p.blk = (long long)block_elems(); }
     return p;
   }
-  // rows of the LLM activations per clip: a paged handle prefills packed prompts of at most 512 tokens only
+  // rows of the LLM activations per clip: a paged handle prefills packed prompts, or chunks of longer prompts, of
+  // at most 512 tokens only
   int act_seq() const { return paged() && cfg.max_seq > 512 ? 512 : cfg.max_seq; }
   // rows of the row-major lm_head: vocab rounded up to the 256-wide GEMM tile, the extra rows zero
   int vocab_padded() const { return (cfg.vocab + 255) / 256 * 256; }
@@ -706,11 +707,13 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
 // clips, and no other clip's columns are read or written.
 // packed_rows > 0: B new sequences packed without padding into packed_rows rows, each into its own cache slot, as
 // the map in h->d_pack (kernels.h) describes them; S is the longest. Every row is computed as it would be in a
-// prefill of its sequence alone; next_tok [B] receives each sequence's first token.
+// prefill of its sequence alone; next_tok [B] receives each sequence's first token. pack_attn: which packed
+// attention kernels run (1: wgmma, the sequences with pack_len > 0; 2: flash, chunks of longer prompts; 3: both).
 int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
                 int B, int S, int n_layers, void* hidden_out, float* logits_out, int32_t* next_tok,
                 long long tok_stride, cudaStream_t st, int start_pos = 0, void* states_out = nullptr,
-                const int32_t* n_pad_host = nullptr, int slot = 0, int packed_rows = 0, bool pack_sampled = false) {
+                const int32_t* n_pad_host = nullptr, int slot = 0, int packed_rows = 0, bool pack_sampled = false,
+                int pack_attn = 1) {
   const vcl_config& c = h->cfg;
   const bool packed = packed_rows > 0;
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
@@ -805,6 +808,7 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
     a.S_kv = start_pos + S; a.q_off = start_pos; a.n_pad = np; a.pack = pk;
     if (h->paged()) {   // heads 128 x 128 apart inside a block (kernels.h: KvPages)
       a.k_sb = a.v_sb = 0; a.k_sh = a.v_sh = 128 * 128; a.pages = h->pages();
+      a.pack_tc = (pack_attn & 1) != 0; a.pack_flash = (pack_attn & 2) != 0;
     }
     VCL_TRY(launch_attention(a, st));
     VCL_TRY(gemm(h->l_attn, D, w.wo, D, h->l_h, D, nullptr, h->l_h, D, M, D, D, ACT_NONE, st));
@@ -818,9 +822,9 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
   if (packed && next_tok != nullptr) {
     // each sequence's last row, gathered into B contiguous rows of l_x (dead after the last layer)
     VCL_TRY(launch_embed_tokens(pack_last(pk), 1, h->l_h, h->l_x, B, D, M, st));
-    // sequence i samples with its slot's entry; its token takes column S_i
+    // sequence i samples with its slot's entry; its token takes column start_i + S_i
     SampleAt smp;
-    smp.on = pack_sampled; smp.rowmap = pack_slot(pk); smp.col_dev = pack_len(pk);
+    smp.on = pack_sampled; smp.rowmap = pack_slot(pk); smp.col_dev = pack_end(pk);
     return lm_head_argmax(h, h->l_x, D, B, nullptr, next_tok, tok_stride, st, false, smp);
   }
   if (logits_out != nullptr || next_tok != nullptr) {
@@ -1140,6 +1144,32 @@ int vcl_llm_slot_prefill(vcl_handle* h, int slot, const int64_t* ids, const void
                      as_stream(stream), 0, nullptr, nullptr, slot);
 }
 
+// The packed prefill of n checked sequences (kernels.h): sequence i is rows start_i .. start_i + len_i - 1 of its
+// prompt (start_host null: 0) into slot slots_host[i]; flash_host[i] (null: none) puts it on the flash attention
+// kernel. One host-to-device copy of the map, then the layer stack.
+static int packed_prefill(vcl_handle* h, int n, const int32_t* slots_host, const int32_t* start_host,
+                   const int32_t* len_host, const int* flash_host, long long M, int S_max, const int64_t* ids,
+                   const void* video_feats, const int32_t* vid_start, int32_t* next_tok, cudaStream_t st) {
+  std::vector<int> map(pack_elems(M), 0);
+  int* p = map.data();
+  int pack_attn = 0;
+  for (int i = 0, r = 0; i < n; ++i) {
+    const int start = start_host ? start_host[i] : 0, len = len_host[i];
+    const bool fl = flash_host != nullptr && flash_host[i];
+    pack_attn |= fl ? 2 : 1;
+    pack_off(p)[i] = r; pack_len(p)[i] = fl ? 0 : len; pack_slot(p)[i] = slots_host[i];
+    pack_last(p)[i] = r + len - 1; pack_start(p)[i] = start; pack_end(p)[i] = start + len;
+    for (int j = 0; j < len; ++j, ++r) {
+      pack_row(p, r)[0] = i; pack_row(p, r)[1] = start + j;
+    }
+  }
+  VCL_CUDA_OK(cudaMemcpyAsync(h->d_pack, p, map.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  bool sampled = false;
+  for (int i = 0; i < n; ++i) sampled = sampled || h->sampling(slots_host[i], 1);
+  return llm_prefill(h, ids, video_feats, vid_start, n, S_max, h->cfg.llm_layers, nullptr, nullptr, next_tok, 1, st,
+                     0, nullptr, nullptr, 0, (int)M, sampled, pack_attn);
+}
+
 int vcl_llm_slots_prefill(vcl_handle* h, int n, const int32_t* slots_host, const int32_t* seq_len_host,
                           const int64_t* ids, const void* video_feats, const int32_t* vid_start, int32_t* next_tok,
                           void* stream) {
@@ -1163,21 +1193,48 @@ int vcl_llm_slots_prefill(vcl_handle* h, int n, const int32_t* slots_host, const
     S_max = len > S_max ? len : S_max;
   }
   // n <= max_batch sequences of at most min(512, max_seq) tokens: M fits the activations (max_batch * act_seq() rows)
-  std::vector<int> map(pack_elems(M), 0);
-  int* p = map.data();
-  for (int i = 0, r = 0; i < n; ++i) {
-    pack_off(p)[i] = r; pack_len(p)[i] = seq_len_host[i]; pack_slot(p)[i] = slots_host[i];
-    pack_last(p)[i] = r + seq_len_host[i] - 1;
-    for (int j = 0; j < seq_len_host[i]; ++j, ++r) {
-      pack_row(p, r)[0] = i; pack_row(p, r)[1] = j;
-    }
+  return packed_prefill(h, n, slots_host, nullptr, seq_len_host, nullptr, M, S_max, ids, video_feats, vid_start,
+                        next_tok, as_stream(stream));
+}
+
+int vcl_llm_slots_prefill_chunk(vcl_handle* h, int n, const int32_t* slots_host, const int32_t* start_host,
+                                const int32_t* len_host, const int32_t* total_host, const int64_t* ids,
+                                const void* video_feats, const int32_t* vid_start, int32_t* next_tok, void* stream) {
+  VCL_REQUIRE(h != nullptr, "vcl_llm_slots_prefill_chunk: null handle");
+  const vcl_config& c = h->cfg;
+  VCL_REQUIRE(h->paged(), "vcl_llm_slots_prefill_chunk: the handle has a contiguous KV cache (kv_blocks 0), which "
+              "prefills long prompts in one pass (vcl_llm_slot_prefill)");
+  VCL_REQUIRE(n >= 1 && n <= h->n_slots_max(), "vcl_llm_slots_prefill_chunk: n=%d outside 1..%d (%s)", n,
+              h->n_slots_max(), h->slots_note().c_str());
+  VCL_REQUIRE(slots_host && start_host && len_host && total_host && ids && vid_start && next_tok,
+              "vcl_llm_slots_prefill_chunk: null argument");
+  VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
+  long long M = 0;
+  int S_max = 0;
+  for (int i = 0; i < n; ++i) {
+    const int s = slots_host[i], st0 = start_host[i], len = len_host[i], tot = total_host[i];
+    VCL_REQUIRE(s >= 0 && s < h->n_slots_max(), "vcl_llm_slots_prefill_chunk: slot %d outside 0..%d", s,
+                h->n_slots_max() - 1);
+    for (int j = 0; j < i; ++j)
+      VCL_REQUIRE(slots_host[j] != s, "vcl_llm_slots_prefill_chunk: slot %d is given twice", s);
+    VCL_REQUIRE(st0 >= 0 && st0 % 64 == 0, "vcl_llm_slots_prefill_chunk: sequence %d starts at %d, not a multiple of "
+                "64 (the query tiles of a chunk must be those of the whole prompt)", i, st0);
+    VCL_REQUIRE(len >= 1 && len <= 512, "vcl_llm_slots_prefill_chunk: sequence %d has %d rows, outside 1..512", i, len);
+    VCL_REQUIRE(st0 + len <= tot, "vcl_llm_slots_prefill_chunk: sequence %d: rows %d..%d past its prompt of %d tokens",
+                i, st0, st0 + len - 1, tot);
+    VCL_REQUIRE(tot <= c.max_seq, "vcl_llm_slots_prefill_chunk: sequence %d: prompt of %d tokens exceeds max_seq %d",
+                i, tot, c.max_seq);
+    VCL_REQUIRE(tot > 512 || (st0 == 0 && len == tot), "vcl_llm_slots_prefill_chunk: sequence %d: a prompt of %d <= "
+                "512 tokens is prefilled whole (start 0, length %d), as vcl_llm_slots_prefill does", i, tot, tot);
+    M += len;
+    S_max = len > S_max ? len : S_max;
   }
-  cudaStream_t st = as_stream(stream);
-  VCL_CUDA_OK(cudaMemcpyAsync(h->d_pack, p, map.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-  bool sampled = false;
-  for (int i = 0; i < n; ++i) sampled = sampled || h->sampling(slots_host[i], 1);
-  return llm_prefill(h, ids, video_feats, vid_start, n, S_max, c.llm_layers, nullptr, nullptr, next_tok, 1, st, 0,
-                     nullptr, nullptr, 0, (int)M, sampled);
+  VCL_REQUIRE(M <= (long long)c.max_batch * h->act_seq(), "vcl_llm_slots_prefill_chunk: %lld rows exceed the "
+              "activations (max_batch %d * %d)", M, c.max_batch, h->act_seq());
+  std::vector<int> flash(n);
+  for (int i = 0; i < n; ++i) flash[i] = total_host[i] > 512;
+  return packed_prefill(h, n, slots_host, start_host, len_host, flash.data(), M, S_max, ids, video_feats, vid_start,
+                        next_tok, as_stream(stream));
 }
 
 int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* pos_host, int n_slots, int n_new,

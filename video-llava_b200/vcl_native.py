@@ -127,6 +127,8 @@ _SIGNATURES = {
     "vcl_llm_slot_prefill": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "vcl_llm_slots_prefill": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), c_void_p, c_void_p,
                                       c_void_p, c_void_p, c_void_p]),
+    "vcl_llm_slots_prefill_chunk": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32),
+                                            POINTER(c_int32), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "vcl_llm_slot_decode": (c_int, [c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_void_p, c_void_p]),
     "vcl_llm_set_sampling": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_float), POINTER(c_int32),
                                      POINTER(c_uint64), c_void_p]),
@@ -662,7 +664,13 @@ class Engine:
         n = len(slots)
         if not (len(ids_list) == len(feats_list) == len(vid_starts) == n):
             raise VclError(f"{n} slots, {len(ids_list)} prompts, {len(feats_list)} features, {len(vid_starts)} vid_starts")
-        dev = "cuda"
+        ids, lens, packed, vf, vs, tok = self._packed_args(ids_list, feats_list, vid_starts, tok_out)
+        check(lib().vcl_llm_slots_prefill(self._h, n, (c_int32 * n)(*[int(s) for s in slots]), (c_int32 * n)(*lens),
+                                          ptr(packed), ptr(vf), ptr(vs), ptr(tok), cur_stream()))
+        return tok
+
+    def _packed_args(self, ids_list, feats_list, vid_starts, tok_out):
+        n, dev = len(ids_list), "cuda"
         ids = [torch.as_tensor(t).reshape(-1) for t in ids_list]
         lens = [t.numel() for t in ids]
         packed = torch.cat([t.to(dev, torch.int64) for t in ids]) if n else torch.empty(0, dtype=torch.int64, device=dev)
@@ -675,8 +683,23 @@ class Engine:
         vs = torch.tensor([int(v) if f is not None else NO_VIDEO for v, f in zip(vid_starts, feats_list)],
                           dtype=torch.int32, device=dev)
         tok = tok_out if tok_out is not None else torch.empty(n, dtype=torch.int32, device=dev)
-        check(lib().vcl_llm_slots_prefill(self._h, n, (c_int32 * n)(*[int(s) for s in slots]), (c_int32 * n)(*lens),
-                                          ptr(packed), ptr(vf), ptr(vs), ptr(tok), cur_stream()))
+        return ids, lens, packed, vf, vs, tok
+
+    def slots_prefill_chunk(self, slots, starts, totals, ids_list, feats_list, vid_starts, tok_out=None):
+        """Chunks of prompts into the cache slots of a paged engine, all in one packed pass
+        (vcl_llm_slots_prefill_chunk): ids_list[i] ([len_i] or [1, len_i]) is rows starts[i] .. starts[i] + len_i - 1
+        of a prompt of totals[i] tokens in slot slots[i], whose earlier rows the slot already holds. feats_list[i] /
+        vid_starts[i]: the whole prompt's video features and span start (counted from its first token), as in
+        slots_prefill. Returns the token at each chunk's last row, [n] int32 on the device; after a prompt's last
+        chunk its slot and that token equal slot_prefill of the whole prompt on a contiguous engine."""
+        n = len(slots)
+        if not (len(starts) == len(totals) == len(ids_list) == len(feats_list) == len(vid_starts) == n):
+            raise VclError(f"{n} slots, {len(starts)} starts, {len(totals)} totals, {len(ids_list)} chunks, "
+                           f"{len(feats_list)} features, {len(vid_starts)} vid_starts")
+        ids, lens, packed, vf, vs, tok = self._packed_args(ids_list, feats_list, vid_starts, tok_out)
+        arr = lambda v: (c_int32 * n)(*[int(x) for x in v])   # noqa: E731
+        check(lib().vcl_llm_slots_prefill_chunk(self._h, n, arr(slots), arr(starts), arr(lens), arr(totals),
+                                                ptr(packed), ptr(vf), ptr(vs), ptr(tok), cur_stream()))
         return tok
 
     def slot_decode(self, first_tok, positions, n_new, out=None):

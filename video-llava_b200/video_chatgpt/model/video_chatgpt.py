@@ -733,7 +733,8 @@ class VideoChatGPTLlamaForCausalLM:
 
     @torch.no_grad()
     def generate_requests(self, requests, max_new_tokens=32, eos_token_id="config", stopping_criteria=None,
-                          slots=None, do_sample=False, packed_admission=False, temperature=1.0, top_k=50, seed=None):
+                          slots=None, do_sample=False, packed_admission=False, temperature=1.0, top_k=50, seed=None,
+                          chunked_prefill=False):
         """Greedy generation for many independent requests by in-flight (continuous) batching: every request
         owns a slot of the KV cache while it runs, and a finished request's slot takes the next queued one at
         once while the other slots keep decoding (a static batch decodes until its longest row finishes).
@@ -763,7 +764,11 @@ class VideoChatGPTLlamaForCausalLM:
         in flight (only the stepwise generate draws from torch's RNG).
         A paged model (kv_blocks) gives each request only the 128-column blocks it has written, so the requests in
         flight follow their actual lengths: see _schedule_paged. The results are the same bit for bit; afterwards
-        self.last_kv_stats holds the preemptions, the bytes swapped out and the peak blocks in use."""
+        self.last_kv_stats holds the preemptions, the bytes swapped out and the peak blocks in use.
+        chunked_prefill: on a paged model, prompts longer than _PACKED_MAX_S tokens (up to max_seq - max_new_tokens)
+        are prefilled in chunks of _PACKED_MAX_S rows (_prefill_chunked) instead of being rejected; last_kv_stats
+        then also counts the chunked prompts and the chunk calls. The results are those of a contiguous model.
+        A contiguous model accepts the flag and ignores it: it prefills any prompt up to max_seq in one pass."""
         for i, r in enumerate(requests):
             r = r if isinstance(r, dict) else {}
             if r.get("do_sample", do_sample) and r.get("seed", seed) is None:
@@ -779,14 +784,14 @@ class VideoChatGPTLlamaForCausalLM:
         samp = dict(do_sample=do_sample, temperature=temperature, top_k=top_k, seed=seed)
         reqs = [self._request(i, r, max_new_tokens, stopping_criteria, eng.NV, samp) for i, r in enumerate(requests)]
         if self._kv_blocks:
-            self._check_paged(reqs)
+            self._check_paged(reqs, chunked_prefill)
         sampling = any(r.temperature > 0 for r in reqs)
         eos, _ = self._eos_pad(eos_token_id, None)
         self._last_out, self._pos = None, 0
         n_slots = min(n_slots, len(reqs))
         try:
             if self._kv_blocks:
-                return self._schedule_paged(eng, reqs, n_slots, packed_admission, sampling, eos)
+                return self._schedule_paged(eng, reqs, n_slots, packed_admission, sampling, eos, chunked_prefill)
             return self._schedule(eng, reqs, n_slots, packed_admission, sampling, eos)
         finally:
             if sampling:
@@ -862,22 +867,45 @@ class VideoChatGPTLlamaForCausalLM:
                                     [r.vid_start for _, r in packed])
             first[torch.tensor(slots, device=dev)] = tok
 
-    def _check_paged(self, reqs):
+    def _prefill_chunked(self, eng, group, first, packed):
+        """Prefill the (slot, request) pairs of one admission point whose prompts are longer than _PACKED_MAX_S on a
+        paged engine: each prompt runs as consecutive chunks of _PACKED_MAX_S rows (Engine.slots_prefill_chunk),
+        every chunk attending the columns its earlier chunks left in the slot's blocks. packed: chunk k of every
+        prompt of the group goes into one call (at most n_slots * 512 rows, which the activations hold); otherwise
+        each prompt runs alone. A slot's first token (first[slot]) is the one its last chunk gives. Returns the
+        number of chunk calls."""
+        dev, L = first.device, self._PACKED_MAX_S
+        calls = 0
+        for batch in ([group] if packed else [[g] for g in group]):
+            for start in range(0, max(r.S for _, r in batch), L):
+                live = [(s, r) for s, r in batch if start < r.S]
+                tok = eng.slots_prefill_chunk([s for s, _ in live], [start] * len(live), [r.S for _, r in live],
+                                              [r.ids[start:start + L] for _, r in live],
+                                              [None if r.feats is None else r.feats.to(dev) for _, r in live],
+                                              [r.vid_start for _, r in live])
+                calls += 1
+                for j, (s, r) in enumerate(live):
+                    if start + L >= r.S:
+                        first[s] = tok[j]
+        return calls
+
+    def _check_paged(self, reqs, chunked=False):
         """The requests a paged cache takes, checked on the host before any device work: a prompt of at most
-        min(512, max_seq) tokens (a paged engine prefills packed), and at most kv_blocks - 1 blocks for the prompt and
-        every new token, so that a request alone always fits the pool and the scheduler always makes progress."""
+        min(512, max_seq) tokens (a paged engine prefills packed) unless `chunked` (any prompt _request accepts), and
+        at most kv_blocks - 1 blocks for the prompt and every new token, so that a request alone always fits the pool
+        and the scheduler always makes progress."""
         C, usable = vn.KV_BLOCK_COLS, self._kv_blocks - 1
         s_lim = min(self._PACKED_MAX_S, self._max_seq)
         for i, r in enumerate(reqs):
-            if r.S > s_lim:
+            if r.S > s_lim and not chunked:
                 raise ValueError(f"request {i}: prompt of {r.S} tokens; a paged KV cache takes prompts of at most "
-                                 f"{s_lim} tokens (the packed prefill)")
+                                 f"{s_lim} tokens (the packed prefill); chunked_prefill=True takes longer ones")
             need = -(-(r.S + r.n) // C)
             if need > usable:
                 raise ValueError(f"request {i}: prompt {r.S} + max_new_tokens {r.n} needs {need} blocks of {C} columns, "
                                  f"more than the pool's {usable} (kv_blocks {self._kv_blocks}, block 0 is the park block)")
 
-    def _schedule_paged(self, eng, reqs, n_slots, packed_admission, sampling, eos):
+    def _schedule_paged(self, eng, reqs, n_slots, packed_admission, sampling, eos, chunked=False):
         """The admission / decode loop of generate_requests on a paged KV cache. The host keeps a free list and each
         slot's row of the block table (block 0, the park block, wherever no request owns a block), and writes the
         whole table to the engine before every prefill and every decode chunk.
@@ -890,6 +918,9 @@ class VideoChatGPTLlamaForCausalLM:
           (its written blocks copied to pinned host memory, its blocks freed, its slot parked) until it is. Its
           position, pending token and sampling entry stay on the host; it resumes into any free slot and free blocks,
           restored exactly, and its tokens depend on its seed and positions only.
+        - Chunked prefill (`chunked`). A prompt over _PACKED_MAX_S tokens is admitted by the same rule (its prompt's
+          blocks plus one chunk's growth) and prefilled at its admission point by _prefill_chunked, before the next
+          decode chunk; so a request that is swapped out always holds its whole prompt.
         _check_paged guarantees that the oldest running request alone always fits."""
         dev, C, K = self.device, vn.KV_BLOCK_COLS, self._SLOT_CHUNK
         table = [[0] * eng.table_row for _ in range(eng.n_slots)]    # every slot of the engine, parked
@@ -904,7 +935,8 @@ class VideoChatGPTLlamaForCausalLM:
         gen = {}
         swapped = {}                        # request -> (pos, pending token, unseen, host copies of its blocks)
         released = []                       # host buffers whose copy back may still be in flight
-        stats = dict(preemptions=0, swapped_bytes=0, peak_blocks=0, kv_blocks=eng.kv_blocks)
+        stats = dict(preemptions=0, swapped_bytes=0, peak_blocks=0, kv_blocks=eng.kv_blocks, chunked_prefills=0,
+                     chunk_calls=0)
         first = torch.zeros(n_slots, dtype=torch.int32, device=dev)     # the token each slot is fed next
         stamp = 0
 
@@ -969,6 +1001,12 @@ class VideoChatGPTLlamaForCausalLM:
                 rs = [(s, reqs[i]) for s, i in admitted + resumed]
                 eng.set_sampling([s for s, _ in rs], [r.temperature for _, r in rs], [r.top_k for _, r in rs],
                                  [r.seed for _, r in rs])
+            if chunked and admitted:
+                long = [(s, reqs[i]) for s, i in admitted if reqs[i].S > self._PACKED_MAX_S]
+                admitted = [(s, i) for s, i in admitted if reqs[i].S <= self._PACKED_MAX_S]
+                if long:
+                    stats["chunked_prefills"] += len(long)
+                    stats["chunk_calls"] += self._prefill_chunked(eng, long, first, packed_admission)
             if admitted and packed_admission:
                 self._admit_packed(eng, [(s, reqs[i]) for s, i in admitted], first)
             elif admitted:
