@@ -282,6 +282,22 @@ int vcl_llm_slots_prefill_chunk(vcl_handle* h, int n, const int32_t* slots_host,
                                 const int32_t* len_host, const int32_t* total_host, const int64_t* ids,
                                 const void* video_feats, const int32_t* vid_start, int32_t* next_tok, void* stream);
 
+/* Continued prefill on a PAGED cache (vcl_config.kv_blocks > 0; rejected otherwise): vcl_llm_prefill_append for
+ * several slots in one packed pass. Sequence i is the text-only tail of len_host[i] tokens at positions
+ * start_host[i] .. start_host[i] + len_host[i] - 1 of slot slots_host[i] (all HOST memory, [n] int32), whose
+ * columns 0 .. start_host[i] - 1 the slot already holds (a kept conversation: its prompt, the answer's decoded
+ * columns). ids is the packed [sum len_i] int64 of the tails. Each tail runs the attention kernel the contiguous
+ * continued prefill runs at the same start and length: the wgmma kernel when start_i + len_i <= 512, the flash kernel
+ * otherwise, with the same tiles and masks (VCL_PREFILL_ATTN_FLASH does not apply); one launch per kernel kind
+ * present. So the slot's columns start_i .. start_i + len_i - 1 and next_tok[i] equal vcl_llm_prefill_append(ids_i,
+ * B = 1, S = len_i, start_pos = start_i) on a contiguous handle holding the same columns 0 .. start_i - 1, bit for
+ * bit. next_tok [n] int32 is drawn with entry slots_host[i] of the sampling table at counter start_i + len_i.
+ * Rejected before any device work, the handle untouched: n outside 1 .. max_slots, a slot outside 0 .. max_slots-1
+ * or given twice, start_i < 1, len_i outside 1 .. 512, start_i + len_i > max_seq, and sum len_i beyond the
+ * activations (max_batch * min(max_seq, 512) rows). */
+int vcl_llm_slots_prefill_append(vcl_handle* h, int n, const int32_t* slots_host, const int32_t* start_host,
+                                 const int32_t* len_host, const int64_t* ids, int32_t* next_tok, void* stream);
+
 /* vcl_llm_decode_loop with a position per slot: slot b (0 <= b < n_slots) is fed first_tok[b] at position
  * pos_host[b] (HOST memory: the number of tokens its cache holds), then runs n_new-1 greedy steps;
  * out_tokens is [n_slots, n_new] int32, first_tok included. Every pos_host[b] + n_new - 1 must be <= max_seq
@@ -326,7 +342,7 @@ int vcl_llm_set_sampling(vcl_handle* h, int n, const int32_t* clips_host, const 
  *
  * A paged handle serves vcl_llm_slots_prefill, vcl_llm_slot_prefill (run as a packed prefill of one prompt, so
  * prompts are limited to min(512, max_seq) tokens), vcl_llm_slots_prefill_chunk (prompts up to max_seq tokens, in
- * chunks of at most 512 rows), vcl_llm_slot_decode and vcl_llm_set_sampling. Every static
+ * chunks of at most 512 rows), vcl_llm_slots_prefill_append (text tails of kept conversations), vcl_llm_slot_decode and vcl_llm_set_sampling. Every static
  * entry point (vcl_llm_prefill(_padded, _states, _append), _decode_step, _decode_loop, _generate(_padded), _score)
  * and vcl_kv_cache_copy is rejected. Its LLM activations are sized for max_batch * min(max_seq, 512) rows, the
  * most a packed prefill uses.

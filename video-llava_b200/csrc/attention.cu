@@ -12,7 +12,9 @@
 //     It serves the 336-px ViT tower (S = 577, read straight out of the fused q|k|v activation,
 //     launch_attention_vit), longer prompts and continued prefills beyond 512 keys, and the chunks of prompts over
 //     512 tokens in a paged cache (vcl_llm_slots_prefill_chunk: packed, each key tile read through the block
-//     table, the same tiles and arithmetic as the one-shot prefill of the whole prompt); the ViT's S = 257 runs in
+//     table, the same tiles and arithmetic as the one-shot prefill of the whole prompt) and text tails appended to
+//     a paged slot past 512 keys (vcl_llm_slots_prefill_append: those of the contiguous continued prefill); the
+//     ViT's S = 257 runs in
 //     attention_tc.cu, the causal hd-128 prefill up to 512 keys in attention_prefill_tc.cu (both wgmma, exact
 //     full-row softmax).
 //
@@ -83,8 +85,10 @@ __device__ __forceinline__ void load_tile(uint32_t sbase, const bf16* g, long lo
 // pack_end_i - pack_start_i queries start at its row offset and sit at absolute positions start_i .. ; its keys are
 // columns 0 .. end_i - 1 of slot_i (q_off = start_i, S_kv = end_i). Sequences with pack_len > 0 belong to the wgmma
 // kernel and are skipped. Key tile jt is the 64 columns at offset (jt % 2) * 64 of block table[slot_i][jt / 2].
-// With start_i a multiple of 64 a query tile covers the rows, walks the key tiles and applies the masks of the same
-// tile of a one-shot prefill of the whole prompt (S = S_kv = end, q_off = 0): keys past end_i are past every query
+// A query tile covers the rows, walks the key tiles and applies the masks of the same tile of the contiguous kernel
+// at the same q_off, S_kv: a continued prefill (vcl_llm_slots_prefill_append: a text tail at any start_i). For a
+// chunk of a prompt (vcl_llm_slots_prefill_chunk), start_i is a multiple of 64, so these are also the tiles and
+// masks of a one-shot prefill of the whole prompt (S = S_kv = end, q_off = 0): keys past end_i are past every query
 // of the chunk too, so both mask them causally, and the zero-filled columns past end_i only meet P = 0.
 template <int HD, bool CAUSAL, bool PAD = false, bool PACK = false, bool PAGED = false>
 __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {

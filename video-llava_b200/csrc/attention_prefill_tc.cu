@@ -86,9 +86,11 @@ __device__ __forceinline__ void pa_mma(float (&acc)[64], uint32_t a_base, int a_
 
 // PAD: left-padded clips (a.n_pad): a real query (cache column >= n_pad[b]) attends keys n_pad[b] .. its own column,
 // and a tile of real queries starts at the first key block that holds a real key; a pad query attends causally.
-// PACK: packed sequences (a.pack): blockIdx.z is sequence i, whose S_i queries start at its row offset and whose keys
-// are clip slot_i of the cache (S = S_kv = S_i, q_off = 0); the grid covers the longest sequence, so a CTA whose
-// query tile starts past S_i has nothing to do.
+// PACK: packed sequences (a.pack): blockIdx.z is sequence i, whose S_i = pack_len_i queries start at its row offset,
+// sit at absolute positions start_i .. end_i - 1 and attend keys 0 .. their own position of clip slot_i of the cache
+// (S = S_i, q_off = start_i, S_kv = end_i): a whole prompt (start 0, end S_i) or a text tail appended to a cached
+// sequence, each walking the tiles of the contiguous prefill at the same q_off; the grid covers the longest
+// sequence, so a CTA whose query tile starts past S_i has nothing to do.
 // PAGED (with PACK): a paged cache (a.pages). Key block kb of sequence i is the 128 columns of block
 // table[slot_i][kb], rows 128 elements apart, so one key block of this kernel is exactly one page.
 template <bool PAD, bool PACK, bool PAGED = false>
@@ -110,7 +112,7 @@ attn_prefill_tc_kernel(const AttnArgs a, int S_kv) {
     S = __ldg(pack_len(a.pack) + b);
     if (q0 >= S) return;                                 // before the first barrier: the whole CTA leaves
     const long long off = __ldg(pack_off(a.pack) + b);
-    S_kv = S; q_off = 0;
+    S_kv = __ldg(pack_end(a.pack) + b); q_off = __ldg(pack_start(a.pack) + b);
     q_base = off * a.q_ss; o_base = off * a.o_ss; kv_clip = __ldg(pack_slot(a.pack) + b);
   }
   const bf16* qg = a.q + q_base + (long long)h * a.q_sh;

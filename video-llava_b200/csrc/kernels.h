@@ -11,13 +11,15 @@ namespace vcl {
 
 typedef __nv_bfloat16 bf16;
 
-// Packed prefill (vcl_llm_slots_prefill / vcl_llm_slots_prefill_chunk): n <= PACK_SEQ_MAX sequences of lengths
+// Packed prefill (vcl_llm_slots_prefill / _chunk / _append): n <= PACK_SEQ_MAX sequences of lengths
 // S_0 .. S_{n-1} concatenated without padding into M = sum S_i rows, sequence i going to cache slot slot_i. Sequence
 // i is the rows start_i .. start_i + S_i - 1 of its prompt (start_i = 0 for a whole prompt; a chunk of a longer
-// prompt attends the columns 0 .. start_i - 1 its earlier chunks left in the cache). One device int array describes
+// prompt, or a text tail appended to a kept conversation, attends the columns 0 .. start_i - 1 already in the
+// cache). One device int array describes
 // the layout, and every kernel of a packed prefill reads it through the accessors below:
 //   [0, 64)    row offset of sequence i     [64, 128)   S_i when the wgmma prefill attention attends it, 0 when the
-//                                                       flash kernel does (a chunk of a prompt over 512 tokens)
+//                                                       flash kernel does (a chunk of a prompt over 512 tokens,
+//                                                       or an appended tail that ends past 512 keys)
 //   [128, 192) its cache slot               [192, 256)  its last row (offset + S_i - 1), whose logits give its token
 //   [256, 320) start_i                      [320, 384)  start_i + S_i: the position of the token its last row gives
 //   [384 + 2r] sequence of row r            [384 + 2r + 1] position of row r in its prompt (start_i + row in sequence)
@@ -177,8 +179,9 @@ struct AttnArgs {
   int S_kv = 0;      // number of keys (0: = S); > S when the queries continue a cached sequence
   int q_off = 0;     // absolute position of query 0 for the causal mask (S_kv - S for a continuation)
   const int* n_pad = nullptr;   // causal only: [B] left padding, the key floor of real queries (or null)
-  // packed rows (kernels.h, above) or null. Sequence i (i < B) has S = S_kv = S_i, q_off 0: its queries / outputs
-  // are rows offset_i .. of q / o (q_sb, o_sb unused), its keys / values clip slot_i of k / v. a.S is max S_i.
+  // packed rows (kernels.h, above) or null. Sequence i (i < B) has S = S_i, q_off = start_i, S_kv = start_i + S_i:
+  // its queries / outputs are rows offset_i .. of q / o (q_sb, o_sb unused), its keys / values clip slot_i of k / v.
+  // a.S is max S_i.
   // The wgmma kernel (S_i <= 512) whatever VCL_PREFILL_ATTN_FLASH says, for every sequence with pack_len S_i > 0.
   const int* pack = nullptr;
   // packed rows only: a paged cache. Key block kb of sequence i is block table[slot_i][kb] (k / v: the layer's pool

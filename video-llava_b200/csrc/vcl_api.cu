@@ -727,7 +727,8 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
   VCL_REQUIRE(S > 0 && start_pos >= 0 && start_pos + S <= c.max_seq, "positions %d..%d outside the cache (max_seq %d)",
               start_pos, start_pos + S - 1, c.max_seq);
   VCL_REQUIRE(n_layers >= 0 && n_layers <= c.llm_layers, "n_layers=%d outside 0..%d", n_layers, c.llm_layers);
-  VCL_REQUIRE(ids != nullptr && (vid_start != nullptr || start_pos > 0), "ids / vid_start are required");
+  VCL_REQUIRE(ids != nullptr && (vid_start != nullptr || start_pos > 0 || (packed && video_feats == nullptr)),
+              "ids / vid_start are required");
   VCL_REQUIRE(start_pos == 0 || video_feats == nullptr, "a continuation cannot carry a video span");
   VCL_REQUIRE((logits_out == nullptr && next_tok == nullptr) || n_layers == c.llm_layers,
               "logits / next token need the full stack (n_layers == %d)", c.llm_layers);
@@ -1234,6 +1235,41 @@ int vcl_llm_slots_prefill_chunk(vcl_handle* h, int n, const int32_t* slots_host,
   std::vector<int> flash(n);
   for (int i = 0; i < n; ++i) flash[i] = total_host[i] > 512;
   return packed_prefill(h, n, slots_host, start_host, len_host, flash.data(), M, S_max, ids, video_feats, vid_start,
+                        next_tok, as_stream(stream));
+}
+
+int vcl_llm_slots_prefill_append(vcl_handle* h, int n, const int32_t* slots_host, const int32_t* start_host,
+                                 const int32_t* len_host, const int64_t* ids, int32_t* next_tok, void* stream) {
+  VCL_REQUIRE(h != nullptr, "vcl_llm_slots_prefill_append: null handle");
+  const vcl_config& c = h->cfg;
+  VCL_REQUIRE(h->paged(), "vcl_llm_slots_prefill_append: the handle has a contiguous KV cache (kv_blocks 0), which "
+              "continues a sequence with vcl_llm_prefill_append");
+  VCL_REQUIRE(n >= 1 && n <= h->n_slots_max(), "vcl_llm_slots_prefill_append: n=%d outside 1..%d (%s)", n,
+              h->n_slots_max(), h->slots_note().c_str());
+  VCL_REQUIRE(slots_host && start_host && len_host && ids && next_tok, "vcl_llm_slots_prefill_append: null argument");
+  VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
+  long long M = 0;
+  int S_max = 0;
+  for (int i = 0; i < n; ++i) {
+    const int s = slots_host[i], st0 = start_host[i], len = len_host[i];
+    VCL_REQUIRE(s >= 0 && s < h->n_slots_max(), "vcl_llm_slots_prefill_append: slot %d outside 0..%d", s,
+                h->n_slots_max() - 1);
+    for (int j = 0; j < i; ++j)
+      VCL_REQUIRE(slots_host[j] != s, "vcl_llm_slots_prefill_append: slot %d is given twice", s);
+    VCL_REQUIRE(st0 >= 1, "vcl_llm_slots_prefill_append: sequence %d starts at %d; a tail continues a cached "
+                "sequence (start >= 1; vcl_llm_slots_prefill takes new prompts)", i, st0);
+    VCL_REQUIRE(len >= 1 && len <= 512, "vcl_llm_slots_prefill_append: sequence %d has %d rows, outside 1..512", i, len);
+    VCL_REQUIRE(st0 + len <= c.max_seq, "vcl_llm_slots_prefill_append: sequence %d: rows %d..%d outside the cache "
+                "(max_seq %d)", i, st0, st0 + len - 1, c.max_seq);
+    M += len;
+    S_max = len > S_max ? len : S_max;
+  }
+  VCL_REQUIRE(M <= (long long)c.max_batch * h->act_seq(), "vcl_llm_slots_prefill_append: %lld rows exceed the "
+              "activations (max_batch %d * %d)", M, c.max_batch, h->act_seq());
+  // the kernel of the contiguous continued prefill (attention_prefill_tc_supported): wgmma up to 512 keys
+  std::vector<int> flash(n);
+  for (int i = 0; i < n; ++i) flash[i] = start_host[i] + len_host[i] > 512;
+  return packed_prefill(h, n, slots_host, start_host, len_host, flash.data(), M, S_max, ids, nullptr, nullptr,
                         next_tok, as_stream(stream));
 }
 

@@ -129,6 +129,8 @@ _SIGNATURES = {
                                       c_void_p, c_void_p, c_void_p]),
     "vcl_llm_slots_prefill_chunk": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32),
                                             POINTER(c_int32), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "vcl_llm_slots_prefill_append": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32),
+                                             c_void_p, c_void_p, c_void_p]),
     "vcl_llm_slot_decode": (c_int, [c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_void_p, c_void_p]),
     "vcl_llm_set_sampling": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_float), POINTER(c_int32),
                                      POINTER(c_uint64), c_void_p]),
@@ -700,6 +702,21 @@ class Engine:
         arr = lambda v: (c_int32 * n)(*[int(x) for x in v])   # noqa: E731
         check(lib().vcl_llm_slots_prefill_chunk(self._h, n, arr(slots), arr(starts), arr(lens), arr(totals),
                                                 ptr(packed), ptr(vf), ptr(vs), ptr(tok), cur_stream()))
+        return tok
+
+    def slots_prefill_append(self, slots, starts, ids_list, tok_out=None):
+        """Text tails appended to the cached sequences of a paged engine's slots, all in one packed pass
+        (vcl_llm_slots_prefill_append): ids_list[i] ([len_i] or [1, len_i]) takes positions starts[i] .. of slot
+        slots[i], whose columns 0 .. starts[i] - 1 the slot already holds. Returns the token after each tail, [n] int32
+        on the device (tok_out if given); it and the slot's new columns equal prefill_append of that tail on a
+        contiguous engine holding the same columns."""
+        n = len(slots)
+        if not (len(starts) == len(ids_list) == n):
+            raise VclError(f"{n} slots, {len(starts)} starts, {len(ids_list)} tails")
+        ids, lens, packed, _, _, tok = self._packed_args(ids_list, [None] * n, [0] * n, tok_out)
+        arr = lambda v: (c_int32 * n)(*[int(x) for x in v])   # noqa: E731
+        check(lib().vcl_llm_slots_prefill_append(self._h, n, arr(slots), arr(starts), arr(lens), ptr(packed), ptr(tok),
+                                                 cur_stream()))
         return tok
 
     def slot_decode(self, first_tok, positions, n_new, out=None):

@@ -313,6 +313,8 @@ class VideoChatGPTLlamaForCausalLM:
         vn.weight_format_code(llm_weight_format)          # ValueError before anything else
         self._kv_blocks = vn.check_kv_blocks(kv_blocks)
         self.last_kv_stats = None
+        self._sessions: dict = {}      # kept conversations of generate_requests (paged): key -> _schedule_paged's state
+        self._session_clock = 0        # last-use stamps of the kept conversations (the least recent is swapped first)
         self._n_slots = vn.slot_capacity(max_batch, max_slots)
         self._max_slots = 0 if max_slots is None else self._n_slots
         self._llm_weight_format = llm_weight_format
@@ -751,7 +753,8 @@ class VideoChatGPTLlamaForCausalLM:
         slots: cache slots in flight, default and at most the engine's slot count (max_slots; by default
         min(max_batch, 16)). Requests are admitted one prefill
         at a time; all slots then decode _SLOT_CHUNK steps per device call. Everything is validated before any
-        device work. Afterwards there is no turn for generate_continue to continue.
+        device work. Afterwards there is no turn for generate_continue to continue; on a paged model a conversation
+        continues through the sessions below.
         packed_admission: at every admission point all free slots are filled from the queue (in queue order) by
         one packed prefill (Engine.slots_prefill) instead of one prefill each; a prompt longer than
         _PACKED_MAX_S is admitted alone. The results are the same either way.
@@ -768,9 +771,25 @@ class VideoChatGPTLlamaForCausalLM:
         chunked_prefill: on a paged model, prompts longer than _PACKED_MAX_S tokens (up to max_seq - max_new_tokens)
         are prefilled in chunks of _PACKED_MAX_S rows (_prefill_chunked) instead of being rejected; last_kv_stats
         then also counts the chunked prompts and the chunk calls. The results are those of a contiguous model.
-        A contiguous model accepts the flag and ignores it: it prefills any prompt up to max_seq in one pass."""
+        A contiguous model accepts the flag and ignores it: it prefills any prompt up to max_seq in one pass.
+        Sessions (paged models only; a contiguous model raises ValueError). A request with "session": key (any
+        hashable) starts a conversation: when it ends, its tokens [L] and the cache blocks of columns 0 .. L - 2 are
+        kept under key, across calls, until end_session(key). A request with "continues": key is the next turn of
+        that conversation: its input_ids are the new text only (as generate_continue's new_input_ids), only the last
+        kept token and that text are prefilled (at most _PACKED_MAX_S rows), it returns the whole conversation
+        [1, L + S_new + n] (which its stopping criteria see too) and the conversation stays kept under key. Every turn
+        returns what generate followed by generate_continue (B = 1, same arguments) returns on a contiguous model.
+        Kept conversations are swapped to host memory, least recently used first, before a running request is
+        preempted (_schedule_paged). Rejected before any device work: an unknown key to continue, a session key
+        already kept, a key started and continued in one call, a key continued twice in one call, video features on
+        a continuation, and a continuation that overflows max_seq or the pool. last_kv_stats then also counts the
+        continuations, the prefill rows they did not recompute (reused_rows), the conversations swapped out
+        (session_swaps, session_swapped_bytes) and the conversations kept, resident and swapped at the end."""
         for i, r in enumerate(requests):
             r = r if isinstance(r, dict) else {}
+            if not self._kv_blocks and (r.get("session") is not None or r.get("continues") is not None):
+                raise ValueError(f"request {i}: conversation sessions (\"session\" / \"continues\") need a paged KV "
+                                 "cache (kv_blocks=...); on this model use generate and generate_continue")
             if r.get("do_sample", do_sample) and r.get("seed", seed) is None:
                 raise NotImplementedError(f"request {i}: generate_requests decodes greedily unless given a seed; "
                                           "sampling in flight needs seed= (the call's or the request's own)")
@@ -784,6 +803,7 @@ class VideoChatGPTLlamaForCausalLM:
         samp = dict(do_sample=do_sample, temperature=temperature, top_k=top_k, seed=seed)
         reqs = [self._request(i, r, max_new_tokens, stopping_criteria, eng.NV, samp) for i, r in enumerate(requests)]
         if self._kv_blocks:
+            self._bind_sessions(reqs)
             self._check_paged(reqs, chunked_prefill)
         sampling = any(r.temperature > 0 for r in reqs)
         eos, _ = self._eos_pad(eos_token_id, None)
@@ -897,10 +917,14 @@ class VideoChatGPTLlamaForCausalLM:
         C, usable = vn.KV_BLOCK_COLS, self._kv_blocks - 1
         s_lim = min(self._PACKED_MAX_S, self._max_seq)
         for i, r in enumerate(reqs):
-            if r.S > s_lim and not chunked:
+            if r.start == 0 and r.S > s_lim and not chunked:
                 raise ValueError(f"request {i}: prompt of {r.S} tokens; a paged KV cache takes prompts of at most "
                                  f"{s_lim} tokens (the packed prefill); chunked_prefill=True takes longer ones")
             need = -(-(r.S + r.n) // C)
+            if need > usable and r.start > 0:
+                raise ValueError(f"request {i}: conversation of {r.S} tokens + max_new_tokens {r.n} needs {need} blocks "
+                                 f"of {C} columns, more than the pool's {usable} (kv_blocks {self._kv_blocks}, block 0 "
+                                 "is the park block)")
             if need > usable:
                 raise ValueError(f"request {i}: prompt {r.S} + max_new_tokens {r.n} needs {need} blocks of {C} columns, "
                                  f"more than the pool's {usable} (kv_blocks {self._kv_blocks}, block 0 is the park block)")
@@ -921,10 +945,20 @@ class VideoChatGPTLlamaForCausalLM:
         - Chunked prefill (`chunked`). A prompt over _PACKED_MAX_S tokens is admitted by the same rule (its prompt's
           blocks plus one chunk's growth) and prefilled at its admission point by _prefill_chunked, before the next
           decode chunk; so a request that is swapped out always holds its whole prompt.
+        - Sessions. A request with a "session" or "continues" key keeps its conversation when it ends (self._sessions):
+          its tokens [L] and the blocks of columns 0 .. L - 2, which stay out of the free list, also across calls;
+          its other blocks are freed. A continuation is admitted by the same rule with its conversation's blocks in
+          its slot's row (copied back into fresh blocks first if they were swapped out) and prefills its tail, the
+          columns L - 1 .. S - 1, through Engine.slots_prefill_append.
+        - Eviction. Kept conversations are idle: when an admission, a resume or a chunk's growth is short of blocks,
+          the least recently used one that is resident is swapped to pinned host memory (its blocks freed) before
+          anything waits or any running request is preempted.
         _check_paged guarantees that the oldest running request alone always fits."""
         dev, C, K = self.device, vn.KV_BLOCK_COLS, self._SLOT_CHUNK
+        sessions = self._sessions
         table = [[0] * eng.table_row for _ in range(eng.n_slots)]    # every slot of the engine, parked
-        free = list(range(eng.kv_blocks - 1, 0, -1))                  # pop() takes the lowest block
+        kept = {b for ss in sessions.values() if ss.blocks is not None for b in ss.blocks}
+        free = [b for b in range(eng.kv_blocks - 1, 0, -1) if b not in kept]   # pop() takes the lowest block
         results = [None] * len(reqs)
         queue = collections.deque(range(len(reqs)))
         owner = [None] * n_slots            # request of each slot
@@ -936,7 +970,7 @@ class VideoChatGPTLlamaForCausalLM:
         swapped = {}                        # request -> (pos, pending token, unseen, host copies of its blocks)
         released = []                       # host buffers whose copy back may still be in flight
         stats = dict(preemptions=0, swapped_bytes=0, peak_blocks=0, kv_blocks=eng.kv_blocks, chunked_prefills=0,
-                     chunk_calls=0)
+                     chunk_calls=0, continuations=0, reused_rows=0, session_swaps=0, session_swapped_bytes=0)
         first = torch.zeros(n_slots, dtype=torch.int32, device=dev)     # the token each slot is fed next
         stamp = 0
 
@@ -950,10 +984,27 @@ class VideoChatGPTLlamaForCausalLM:
             table[s][:len(blocks[s])] = blocks[s]
             stats["peak_blocks"] = max(stats["peak_blocks"], eng.kv_blocks - 1 - len(free))
 
-        def release(s):
-            free.extend(reversed(blocks[s]))
+        def release(s, keep=0):             # the first `keep` blocks stay with a kept conversation
+            free.extend(reversed(blocks[s][keep:]))
             blocks[s], table[s] = [], [0] * eng.table_row
             owner[s], pos[s] = None, 0
+
+        def evict_session(spare=None):
+            """swap the least recently used resident conversation (not `spare`) to host memory; False if none"""
+            keys = [k for k, ss in sessions.items() if ss.blocks is not None and k != spare]
+            if not keys:
+                return False
+            ss = sessions[min(keys, key=lambda k: sessions[k].used)]
+            ss.saved = []
+            for b in ss.blocks:
+                buf = eng.swap_buffer()
+                eng.kv_block_copy(b, buf)
+                ss.saved.append(buf)
+            free.extend(reversed(ss.blocks))
+            ss.blocks = None
+            stats["session_swaps"] += 1
+            stats["session_swapped_bytes"] += len(ss.saved) * eng.block_bytes
+            return True
 
         def swap_out(s):
             i = owner[s]
@@ -969,10 +1020,12 @@ class VideoChatGPTLlamaForCausalLM:
 
         while True:
             idle = [s for s in range(n_slots) if owner[s] is None]
-            admitted, resumed = [], []
+            admitted, resumed, tails = [], [], []
             while swapped and idle:
                 i = min(swapped)            # requests are first admitted in queue (= index) order
                 p, tok, uns, saved = swapped[i]
+                while len(free) < cover(i, p, K) and evict_session():
+                    pass
                 if len(free) < cover(i, p, K):
                     break
                 s = idle.pop(0)
@@ -987,20 +1040,43 @@ class VideoChatGPTLlamaForCausalLM:
                 resumed.append((s, i))
             while not swapped and idle and queue:
                 i = queue[0]
-                if len(free) < cover(i, reqs[i].S, K):
+                r = reqs[i]
+                ss = sessions[r.continues] if r.continues is not None else None
+                own = ss.blocks if ss is not None and ss.blocks is not None else []
+                need = cover(i, r.S, K) - len(own)
+                while len(free) < need and evict_session(spare=r.continues):
+                    pass
+                if len(free) < need:
                     break
                 queue.popleft()
                 s = idle.pop(0)
                 stamp += 1
-                owner[s], pos[s], unseen[s], order[s], gen[i] = i, reqs[i].S, True, stamp, []
-                take(s, cover(i, reqs[i].S, K))
-                admitted.append((s, i))
-            if admitted or resumed:
+                owner[s], pos[s], unseen[s], order[s], gen[i] = i, r.S, True, stamp, []
+                if ss is None:
+                    take(s, cover(i, r.S, K))
+                    admitted.append((s, i))
+                    continue
+                del sessions[r.continues]
+                blocks[s] = list(own)
+                take(s, cover(i, r.S, K))
+                if ss.saved is not None:    # swapped out: copied back into the slot's first blocks
+                    for b, buf in zip(blocks[s], ss.saved):
+                        eng.kv_block_copy(b, buf, write=True)
+                    released.extend(ss.saved)
+                tails.append((s, i))
+                stats["continuations"] += 1
+                stats["reused_rows"] += r.start
+            if admitted or resumed or tails:
                 eng.set_block_table(table)
-            if sampling and (admitted or resumed):
-                rs = [(s, reqs[i]) for s, i in admitted + resumed]
+            if sampling and (admitted or resumed or tails):
+                rs = [(s, reqs[i]) for s, i in admitted + resumed + tails]
                 eng.set_sampling([s for s, _ in rs], [r.temperature for _, r in rs], [r.top_k for _, r in rs],
                                  [r.seed for _, r in rs])
+            # continuations: the tails admitted here in one call under packed_admission, one call each otherwise
+            for group in ([tails] if packed_admission and tails else [[t] for t in tails]):
+                tok = eng.slots_prefill_append([s for s, _ in group], [reqs[i].start for _, i in group],
+                                               [reqs[i].ids[reqs[i].start:] for _, i in group])
+                first[torch.tensor([s for s, _ in group], device=dev)] = tok
             if chunked and admitted:
                 long = [(s, reqs[i]) for s, i in admitted if reqs[i].S > self._PACKED_MAX_S]
                 admitted = [(s, i) for s, i in admitted if reqs[i].S <= self._PACKED_MAX_S]
@@ -1018,12 +1094,18 @@ class VideoChatGPTLlamaForCausalLM:
             active = [s for s in range(n_slots) if owner[s] is not None]
             if not active:
                 eng.set_block_table(table)      # every slot parked again
+                stats["sessions"] = len(sessions)
+                stats["sessions_resident"] = sum(ss.blocks is not None for ss in sessions.values())
+                stats["sessions_swapped"] = stats["sessions"] - stats["sessions_resident"]
                 self.last_kv_stats = stats
                 return results
             m = min([K] + [self._max_seq - pos[s] for s in active])
-            # growth, oldest admission first; preempt the latest running request while the free list falls short
+            # growth, oldest admission first; while the free list falls short, swap out a kept conversation, else
+            # preempt the latest running request
             for s in sorted(active, key=lambda t: order[t]):
                 while owner[s] is not None and len(free) < cover(owner[s], pos[s], m) - len(blocks[s]):
+                    if evict_session():
+                        continue
                     swap_out(max((t for t in range(n_slots) if owner[t] is not None), key=lambda t: order[t]))
                 if owner[s] is not None:
                     take(s, cover(owner[s], pos[s], m))
@@ -1040,8 +1122,16 @@ class VideoChatGPTLlamaForCausalLM:
                 for t in (host[s] if unseen[s] else host[s][1:]):
                     gen[i].append(t)
                     if self._request_done(r, gen[i], eos):
-                        results[i] = torch.cat([r.ids, torch.tensor(gen[i], dtype=torch.int64)])[None].to(dev)
-                        release(s)
+                        seq = torch.cat([r.ids, torch.tensor(gen[i], dtype=torch.int64)])
+                        results[i] = seq[None].to(dev)
+                        key = r.continues if r.continues is not None else r.session
+                        keep = 0
+                        if key is not None:     # kept: columns 0 .. L - 2, generate_continue's cache
+                            keep = -(-(seq.numel() - 1) // C)
+                            self._session_clock += 1
+                            sessions[key] = SimpleNamespace(ids=seq, blocks=blocks[s][:keep], saved=None,
+                                                            used=self._session_clock)
+                        release(s, keep)
                         break
                 unseen[s] = False
 
@@ -1059,6 +1149,8 @@ class VideoChatGPTLlamaForCausalLM:
         if n < 1 or S + n > self._max_seq:
             raise ValueError(f"request {i}: prompt length {S} + max_new_tokens {n} does not fit max_seq {self._max_seq}")
         feats, vs = r.get("video_spatio_temporal_features"), vn.NO_VIDEO
+        if feats is not None and r.get("continues") is not None:
+            raise ValueError(f"request {i}: a continuation carries text only (its video is in the kept cache)")
         if feats is not None:
             if feats.dim() == 3 and feats.shape[0] == 1:
                 feats = feats[0]
@@ -1077,7 +1169,59 @@ class VideoChatGPTLlamaForCausalLM:
             if T == 0:
                 k, seed = 0, 0
         return SimpleNamespace(ids=ids, S=S, n=n, feats=feats, vid_start=vs, criteria=list(crit or []),
-                               temperature=T, top_k=k, seed=seed)
+                               temperature=T, top_k=k, seed=seed, session=r.get("session"),
+                               continues=r.get("continues"), start=0)
+
+    def _bind_sessions(self, reqs):
+        """The "session" / "continues" keys of generate_requests' requests, checked on the host before any device
+        work. A continuation's ids become the whole conversation (the kept tokens, then its new turn), its S their
+        length and its start the first column its tail prefill writes: the kept position L - 1, where
+        generate_continue would start."""
+        started, continued = {}, {}
+        for i, r in enumerate(reqs):
+            if r.session is not None and r.continues is not None:
+                raise ValueError(f"request {i}: a request starts a conversation (\"session\") or continues one "
+                                 "(\"continues\"), not both")
+            if r.session is not None:
+                if r.session in self._sessions:
+                    raise ValueError(f"request {i}: a conversation is already kept under session key {r.session!r} "
+                                     "(continue it, or end_session it first)")
+                if r.session in started:
+                    raise ValueError(f"request {i}: session key {r.session!r} is also started by request "
+                                     f"{started[r.session]}")
+                started[r.session] = i
+            if r.continues is not None:
+                if r.continues in continued:
+                    raise ValueError(f"request {i}: conversation {r.continues!r} is also continued by request "
+                                     f"{continued[r.continues]}; one turn per conversation and call")
+                continued[r.continues] = i
+        for key, i in continued.items():
+            r = reqs[i]
+            if key in started:
+                raise ValueError(f"request {i}: conversation {key!r} is started by request {started[key]} in the same "
+                                 "call; a turn's text depends on the previous answer, so continue it in a later call")
+            if key not in self._sessions:
+                raise ValueError(f"request {i}: no conversation is kept under key {key!r}")
+            if r.S + 1 > self._PACKED_MAX_S:
+                raise ValueError(f"request {i}: the continuation's tail (the last kept token and {r.S} new tokens) "
+                                 f"has {r.S + 1} rows, more than {self._PACKED_MAX_S}")
+            conv = self._sessions[key].ids
+            L = conv.numel()
+            if L + r.S + r.n > self._max_seq:
+                raise ValueError(f"request {i}: conversation of {L} tokens + {r.S} new + max_new_tokens {r.n} does not "
+                                 f"fit max_seq {self._max_seq}")
+            r.ids, r.start = torch.cat([conv, r.ids]), L - 1
+            r.S = r.ids.numel()
+
+    def end_session(self, key=None):
+        """Forget the conversation kept under `key` (every kept conversation when None): its cache blocks return to
+        the free list of the next generate_requests call, and a copy swapped to host memory is dropped."""
+        if key is None:
+            self._sessions.clear()
+            return
+        if key not in self._sessions:
+            raise ValueError(f"end_session: no conversation is kept under key {key!r}")
+        del self._sessions[key]
 
     @staticmethod
     def _request_done(r, gen, eos):
