@@ -329,6 +329,38 @@ int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* 
 int vcl_llm_set_sampling(vcl_handle* h, int n, const int32_t* clips_host, const float* temperature_host,
                          const int32_t* top_k_host, const uint64_t* seed_host, void* stream);
 
+/* Log-probabilities of generated tokens: what HF returns as generate(output_scores=True) followed by
+ * compute_transition_scores(sequences, scores, normalize_logits=True) ($TF/generation/utils.py), plus the top-n
+ * alternatives of each step, computed on the device by the sampler next to the token it picks. For the token of
+ * an entry that asks, with s the processed scores HF's `scores` holds (greedy: the logits; sampled: logits / T over
+ * the tokens top-k keeps, -inf elsewhere; a NaN logit is never kept), m = max s and W = sum of exp(s - m) over the
+ * kept tokens (for a sampled row the sum the draw uses, in its order): lp(j) = (s_j - m) - logf(W). The exact rules
+ * are in DESIGN.md section 3. A row's values depend on its logits row and its entry only.
+ *
+ * vcl_llm_set_logprobs writes n entries of the handle's sampling table: clip / slot clips_host[i] gets
+ * top_n_host[i] (HOST memory, [n]): -1 off (every entry after vcl_create), 0 the chosen token only, 1 ..
+ * VCL_LOGPROBS_MAX that many alternatives as well. One host-to-device copy on `stream`. Every token-producing call
+ * (the list at vcl_llm_set_sampling, on a contiguous or a paged handle) then writes, for each entry that asks, 1 +
+ * VCL_LOGPROBS_MAX pairs (int32 id, f32 lp) at (entry, RoPE position of the token) of a buffer the handle owns,
+ * [max_batch][max_seq + 1][1 + VCL_LOGPROBS_MAX] ids and as many log-probs, allocated by the first call that turns an
+ * entry on (22 MB at max_batch 64, max_seq 2048; a handle that never asks holds none). Place 0 is the chosen token; places 1 .. top_n
+ * the top_n kept tokens of largest s (ties: lowest index), -1 / -inf where fewer are kept; a row without a finite
+ * maximum (the arg-max fallback) has NaN everywhere and id -1 at places 1 .. top_n; places past top_n are not
+ * written. A call whose entries are all greedy with log-probs off runs the kernels it ran before; otherwise the
+ * sampler replaces the arg-max kernels, with the same tokens (a greedy entry's token is the arg-max either way).
+ * Rejected before any device work: n outside 1 .. max_batch, a clip outside 0 .. max_batch-1 or given twice, a
+ * top_n outside -1 .. VCL_LOGPROBS_MAX. */
+#define VCL_LOGPROBS_MAX 20
+int vcl_llm_set_logprobs(vcl_handle* h, int n, const int32_t* clips_host, const int32_t* top_n_host, void* stream);
+
+/* Copy the log-prob rows of positions first_pos .. first_pos + count - 1 of entry `entry` out of the handle's buffer:
+ * ids_out [count][1 + VCL_LOGPROBS_MAX] int32 and lp_out [count][1 + VCL_LOGPROBS_MAX] f32, host or device memory,
+ * ordered on `stream`. The token generated at position p of entry b (a prefill of S tokens into clip b: p = S -
+ * n_pad[b]; decode tokens follow at p + 1, ...) is row p. Rejected before any device work: a null argument, a handle
+ * whose buffer was never allocated, an entry outside 0 .. max_batch-1, positions outside 0 .. max_seq. */
+int vcl_llm_read_logprobs(vcl_handle* h, int entry, int first_pos, int count, int32_t* ids_out, float* lp_out,
+                          void* stream);
+
 /* Paged KV cache (vcl_config.kv_blocks > 0). The cache is a pool of kv_blocks BLOCKS. A block holds 128 cache columns
  * of one sequence across all layers, [layer][K = 0 | V = 1][head][128 columns][128 dims] bf16 (2 * llm_layers *
  * llm_heads * 32 KiB: 64 MiB at 7B, 100 MiB at 13B), one contiguous range. The BLOCK TABLE, int32
@@ -405,6 +437,14 @@ int vcl_op_cross_entropy(const void* logits, int64_t ld, const int64_t* labels, 
 int vcl_op_sample(const float* logits, int64_t ld, int B, int V, const float* temperature_host,
                   const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host, int32_t* tok_out,
                   void* stream);
+/* vcl_op_sample with log-probs (compute_transition_scores(normalize_logits=True) on HF's output_scores, and the
+ * top-n alternatives; see vcl_llm_set_logprobs): row b also writes places 0 .. top_n_host[b] (HOST memory, [B],
+ * -1 .. VCL_LOGPROBS_MAX; -1 writes none) of ids_out / lp_out [B][1 + VCL_LOGPROBS_MAX] (device int32 / f32).
+ * tok_out equals vcl_op_sample's bit for bit. */
+int vcl_op_sample_logprobs(const float* logits, int64_t ld, int B, int V, const float* temperature_host,
+                           const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
+                           const int32_t* top_n_host, int32_t* tok_out, int32_t* ids_out, float* lp_out,
+                           void* stream);
 int vcl_op_layernorm(const void* x, void* y, const void* w, const void* b, int rows, int D, float eps,
                      void* stream);
 int vcl_op_rmsnorm(const void* x, void* y, const void* w, int rows, int D, float eps, void* stream);

@@ -156,12 +156,21 @@ int launch_nll_mean(const float* nll, const long long* labels, long long rows, i
 // sampling.cu. Row r uses entry t = entry0 + (rowmap ? rowmap[r] : r) of the sampling table (temperature, top_k,
 // seed: device arrays; temperature 0 is greedy) and draws at counter p = col + (col_dev ? col_dev[r] : 0) -
 // (n_pad ? n_pad[t] : 0), the RoPE position its token takes. out[r * out_stride] receives the token.
+// Log-probs: an entry with top_n[t] >= 0 (top_n null: none) also writes places 0 .. top_n[t] of its row (place 0 the
+// chosen token, then the alternatives), place q of the token at position p (0 <= p < lp_rows) at index
+// t * lp_entry + p * lp_pos + q of lp_id / lp_val.
+#ifndef VCL_LOGPROBS_MAX
+#define VCL_LOGPROBS_MAX 20   // include/vcl.h
+#endif
 struct SampleArgs {
   const float* logits = nullptr; long long ld = 0; int V = 0, B = 0;
   const float* temperature = nullptr; const int* top_k = nullptr; const unsigned long long* seed = nullptr;
   int entry0 = 0; const int* rowmap = nullptr;
   int col = 0; const int* col_dev = nullptr; const int* n_pad = nullptr;
   int* out = nullptr; long long out_stride = 1;
+  const int* top_n = nullptr;
+  int* lp_id = nullptr; float* lp_val = nullptr;
+  long long lp_entry = 0, lp_pos = 0; int lp_rows = 0;
 };
 int launch_sample(const SampleArgs& a, cudaStream_t stream);
 

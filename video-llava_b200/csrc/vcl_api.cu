@@ -58,7 +58,8 @@ struct LlmLayerW {
 };
 struct GraphEntry {
   int B, n_new;        // the positions and pad counts are read on the device (h->d_pos, h->d_npad) ...
-  bool sampled;        // ... and so is the sampling table: a sampled graph serves every temperature / top_k / seed
+  bool sampled;        // ... and so is the sampling table: a graph of the sampler serves every temperature / top_k /
+                       // seed / top_n
   cudaGraphExec_t exec;
   long long kernels;   // kernel nodes in the graph (for vcl_launch_count)
   unsigned long long last_use;
@@ -74,13 +75,15 @@ struct StepIo {
   float* logits_out = nullptr;
   int32_t* tok_out = nullptr; long long out_stride = 1;
   const int* pos_dev = nullptr;   // clip b at position pos + pos_dev[b] (null: pos)
-  bool sampled = false;           // the sampler picks tok_out (entry b of the sampling table for clip b)
+  bool sampled = false;           // the sampler picks tok_out (entry b of the sampling table for clip b) and writes
+                                  // the log-probs of the entries that ask for them
 };
 
 // which sampling-table entries the rows of an lm_head call use, and the cache column their tokens take
 // (SampleArgs in kernels.h; the counter subtracts the clip's left padding)
 struct SampleAt {
-  bool on = false;                              // some entry samples: the sampler replaces the arg-max kernel
+  bool on = false;                              // some entry samples or wants log-probs: the sampler replaces
+                                                // the arg-max kernel
   int entry0 = 0; const int* rowmap = nullptr;  // row r: entry entry0 + (rowmap ? rowmap[r] : r)
   int col = 0; const int* col_dev = nullptr;    // row r: column col + (col_dev ? col_dev[r] : 0)
 };
@@ -134,22 +137,30 @@ struct vcl_handle {
   ArgmaxPart* amax = nullptr;                  // [gemv_grid(vocab)][max_batch] per-CTA partial arg-max of the logits kernel
   int* d_pack = nullptr;                       // pack_elems(max_batch * max_seq): the packed-row map of kernels.h,
                                                // written by each vcl_llm_slots_prefill with one host-to-device copy
-  // The sampling table (vcl_llm_set_sampling): entry b belongs to clip b / cache slot b. One device block at a
-  // fixed address, [max_batch] seeds (u64), temperatures (f32), top_k (i32), so one sampled decode graph serves
-  // every setting; samp_host is its host copy, written whole by one host-to-device copy per call. All zeros
-  // (greedy) at vcl_create.
+  // The sampling table (vcl_llm_set_sampling, vcl_llm_set_logprobs): entry b belongs to clip b / cache slot b. One
+  // device block at a fixed address, [max_batch] seeds (u64), temperatures (f32), top_k (i32), top_n (i32), so one
+  // sampled decode graph serves every setting; samp_host is its host copy, written whole by one host-to-device copy
+  // per call. Greedy without log-probs (top_n -1) at vcl_create.
   unsigned char* samp = nullptr;
   std::vector<unsigned char> samp_host;
   unsigned long long* samp_seed(unsigned char* base) const { return reinterpret_cast<unsigned long long*>(base); }
   float* samp_temp(unsigned char* base) const { return reinterpret_cast<float*>(base + 8 * cfg.max_batch); }
   int* samp_topk(unsigned char* base) const { return reinterpret_cast<int*>(base + 12 * cfg.max_batch); }
-  // whether entry first .. first + n - 1 samples (a temperature above 0)
-  bool sampling(int first, int n) {
+  int* samp_topn(unsigned char* base) const { return reinterpret_cast<int*>(base + 16 * cfg.max_batch); }
+  // whether entry first .. first + n - 1 needs the sampler: it samples (a temperature above 0) or wants log-probs
+  bool sampler(int first, int n) {
     const float* t = samp_temp(samp_host.data());
+    const int* tn = samp_topn(samp_host.data());
     for (int b = first; b < first + n; ++b)
-      if (t[b] > 0.f) return true;
+      if (t[b] > 0.f || tn[b] >= 0) return true;
     return false;
   }
+  // The log-prob buffer: two planes, int32 ids then f32 log-probs, each [max_batch][lp_rows()][1 + VCL_LOGPROBS_MAX],
+  // indexed by entry and the RoPE position of the token (so a read is one contiguous copy per plane); allocated by the
+  // first vcl_llm_set_logprobs that turns an entry on.
+  unsigned char* lp = nullptr;
+  int lp_rows() const { return cfg.max_seq + 1; }   // a decode loop's last token may take position max_seq
+  size_t lp_plane() const { return (size_t)cfg.max_batch * lp_rows() * (1 + VCL_LOGPROBS_MAX); }   // elements
 
   size_t cache_layer_elems() const {
     return (size_t)cfg.max_batch * cfg.llm_heads * cfg.max_seq * 128;
@@ -404,12 +415,14 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   rc |= dalloc(h, &h->d_npad, Bm);
   rc |= dalloc(h, &h->amax, (size_t)device_num_sms() * Bm);
   rc |= dalloc(h, &h->d_pack, pack_elems((long long)Ml));
-  rc |= dalloc(h, &h->samp, Bm * 16);
-  h->samp_host.assign(Bm * 16, 0);
+  rc |= dalloc(h, &h->samp, Bm * 20);
+  h->samp_host.assign(Bm * 20, 0);
+  for (size_t b = 0; b < Bm; ++b) h->samp_topn(h->samp_host.data())[b] = -1;
   if (rc == 0) rc = launch_rope_table(h->rope_cos, h->rope_sin, c->max_seq, 128, c->rope_theta, 0);
   if (rc == 0) {
     cudaError_t e = cudaMemset(h->d_npad, 0, Bm * sizeof(int));   // the cache starts unpadded
-    if (e == cudaSuccess) e = cudaMemset(h->samp, 0, Bm * 16);        // and every entry greedy
+    if (e == cudaSuccess)                                             // and every entry greedy, log-probs off
+      e = cudaMemcpy(h->samp, h->samp_host.data(), h->samp_host.size(), cudaMemcpyHostToDevice);
     if (e == cudaSuccess && h->paged()) e = cudaMemset(h->d_table, 0, h->table_host.size() * sizeof(int));
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
     if (e != cudaSuccess) {
@@ -691,6 +704,12 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
     sa.temperature = h->samp_temp(h->samp); sa.top_k = h->samp_topk(h->samp); sa.seed = h->samp_seed(h->samp);
     sa.entry0 = smp.entry0; sa.rowmap = smp.rowmap; sa.col = smp.col; sa.col_dev = smp.col_dev; sa.n_pad = h->d_npad;
     sa.out = tok_out; sa.out_stride = tok_stride;
+    if (h->lp != nullptr) {   // (every top_n entry is -1 until the buffer exists)
+      sa.top_n = h->samp_topn(h->samp);
+      sa.lp_id = reinterpret_cast<int*>(h->lp); sa.lp_val = reinterpret_cast<float*>(h->lp) + h->lp_plane();
+      sa.lp_entry = (long long)h->lp_rows() * (1 + VCL_LOGPROBS_MAX); sa.lp_pos = 1 + VCL_LOGPROBS_MAX;
+      sa.lp_rows = h->lp_rows();
+    }
     return launch_sample(sa, st);
   }
   if (tok_out != nullptr) VCL_TRY(launch_argmax(h->logits, tok_out, tok_stride, B, c.vocab, st));
@@ -830,7 +849,7 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
   }
   if (logits_out != nullptr || next_tok != nullptr) {
     SampleAt smp;   // clip b (slot `slot` for B = 1) samples with its entry; its token takes column start_pos + S
-    smp.on = next_tok != nullptr && h->sampling(slot, B); smp.entry0 = slot; smp.col = start_pos + S;
+    smp.on = next_tok != nullptr && h->sampler(slot, B); smp.entry0 = slot; smp.col = start_pos + S;
     VCL_TRY(lm_head_argmax(h, h->l_h + (size_t)(S - 1) * D, (long long)S * D, B, logits_out, next_tok,
                            tok_stride, st, false, smp));
   }
@@ -1028,14 +1047,14 @@ int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t 
 }
 
 // The loop of vcl_llm_decode_loop and vcl_llm_slot_decode, with h->d_pos written by the caller: first_tok
-// [B] is fed, n_new - 1 steps follow, and [B, n_new] tokens (first_tok included) go to out_tokens. Greedy unless
-// one of the entries 0 .. B-1 of the sampling table samples.
+// [B] is fed, n_new - 1 steps follow, and [B, n_new] tokens (first_tok included) go to out_tokens. The arg-max
+// kernels unless one of the entries 0 .. B-1 of the sampling table samples or wants log-probs.
 int decode_loop(vcl_handle* h, const int32_t* first_tok, int B, int n_new, int32_t* out_tokens, cudaStream_t st) {
   int32_t* tk = h->tokens;  // [B, n_new] row-major scratch
   if (first_tok != tk)
     VCL_CUDA_OK(cudaMemcpy2DAsync(tk, (size_t)n_new * sizeof(int32_t), first_tok, sizeof(int32_t),
                                   sizeof(int32_t), B, cudaMemcpyDeviceToDevice, st));
-  if (n_new > 1) VCL_TRY(run_decode_steps(h, tk, B, n_new, st, h->sampling(0, B)));
+  if (n_new > 1) VCL_TRY(run_decode_steps(h, tk, B, n_new, st, h->sampler(0, B)));
   VCL_CUDA_OK(cudaMemcpyAsync(out_tokens, tk, (size_t)B * n_new * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
@@ -1115,7 +1134,7 @@ int vcl_llm_decode_step(vcl_handle* h, const int32_t* tok_in, int B, int pos, fl
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
   VCL_REQUIRE(B > 0 && B <= h->cfg.max_batch, "B=%d outside 1..%d", B, h->cfg.max_batch);
   StepIo io;
-  io.tok_in = tok_in; io.logits_out = logits_out; io.tok_out = tok_out; io.sampled = h->sampling(0, B);
+  io.tok_in = tok_in; io.logits_out = logits_out; io.tok_out = tok_out; io.sampled = h->sampler(0, B);
   return llm_decode_step(h, io, B, pos, as_stream(stream));
 }
 
@@ -1166,7 +1185,7 @@ static int packed_prefill(vcl_handle* h, int n, const int32_t* slots_host, const
   }
   VCL_CUDA_OK(cudaMemcpyAsync(h->d_pack, p, map.size() * sizeof(int), cudaMemcpyHostToDevice, st));
   bool sampled = false;
-  for (int i = 0; i < n; ++i) sampled = sampled || h->sampling(slots_host[i], 1);
+  for (int i = 0; i < n; ++i) sampled = sampled || h->sampler(slots_host[i], 1);
   return llm_prefill(h, ids, video_feats, vid_start, n, S_max, h->cfg.llm_layers, nullptr, nullptr, next_tok, 1, st,
                      0, nullptr, nullptr, 0, (int)M, sampled, pack_attn);
 }
@@ -1320,6 +1339,55 @@ int vcl_llm_set_sampling(vcl_handle* h, int n, const int32_t* clips_host, const 
   return 0;
 }
 
+int vcl_llm_set_logprobs(vcl_handle* h, int n, const int32_t* clips_host, const int32_t* top_n_host, void* stream) {
+  VCL_REQUIRE(h != nullptr, "vcl_llm_set_logprobs: null handle");
+  const int mb = h->cfg.max_batch;
+  VCL_REQUIRE(n >= 1 && n <= mb, "vcl_llm_set_logprobs: n=%d outside 1..%d", n, mb);
+  VCL_REQUIRE(clips_host && top_n_host, "vcl_llm_set_logprobs: null argument");
+  bool on = false;
+  for (int i = 0; i < n; ++i) {
+    const int b = clips_host[i], k = top_n_host[i];
+    VCL_REQUIRE(b >= 0 && b < mb, "vcl_llm_set_logprobs: clip %d outside 0..%d", b, mb - 1);
+    for (int j = 0; j < i; ++j)
+      VCL_REQUIRE(clips_host[j] != b, "vcl_llm_set_logprobs: clip %d is given twice", b);
+    VCL_REQUIRE(k >= -1 && k <= VCL_LOGPROBS_MAX, "vcl_llm_set_logprobs: top_n %d of clip %d outside -1..%d", k, b,
+                VCL_LOGPROBS_MAX);
+    on = on || k >= 0;
+  }
+  if (on && h->lp == nullptr) {
+    VCL_TRY(dalloc(h, &h->lp, h->lp_plane() * 8));
+    // the sampler graphs captured so far carry no log-prob buffer: capture them again
+    for (size_t i = h->graphs.size(); i-- > 0;)
+      if (h->graphs[i].sampled) {
+        cudaGraphExecDestroy(h->graphs[i].exec);
+        h->graphs.erase(h->graphs.begin() + i);
+      }
+  }
+  unsigned char* hb = h->samp_host.data();
+  for (int i = 0; i < n; ++i) h->samp_topn(hb)[clips_host[i]] = top_n_host[i];
+  VCL_CUDA_OK(cudaMemcpyAsync(h->samp, hb, h->samp_host.size(), cudaMemcpyHostToDevice, as_stream(stream)));
+  return 0;
+}
+
+int vcl_llm_read_logprobs(vcl_handle* h, int entry, int first_pos, int count, int32_t* ids_out, float* lp_out,
+                          void* stream) {
+  VCL_REQUIRE(h && ids_out && lp_out, "vcl_llm_read_logprobs: null argument");
+  VCL_REQUIRE(h->lp != nullptr, "vcl_llm_read_logprobs: no log-probs were ever turned on for this handle "
+              "(vcl_llm_set_logprobs)");
+  VCL_REQUIRE(entry >= 0 && entry < h->cfg.max_batch, "vcl_llm_read_logprobs: entry %d outside 0..%d", entry,
+              h->cfg.max_batch - 1);
+  VCL_REQUIRE(first_pos >= 0 && count >= 1 && (long long)first_pos + count <= h->lp_rows(),
+              "vcl_llm_read_logprobs: positions %d..%lld outside 0..%d", first_pos, (long long)first_pos + count - 1,
+              h->lp_rows() - 1);
+  constexpr int P = 1 + VCL_LOGPROBS_MAX;
+  const size_t off = ((size_t)entry * h->lp_rows() + first_pos) * P, bytes = (size_t)count * P * 4;
+  cudaStream_t st = as_stream(stream);
+  VCL_CUDA_OK(cudaMemcpyAsync(ids_out, reinterpret_cast<const int*>(h->lp) + off, bytes, cudaMemcpyDefault, st));
+  VCL_CUDA_OK(cudaMemcpyAsync(lp_out, reinterpret_cast<const float*>(h->lp) + h->lp_plane() + off, bytes,
+                              cudaMemcpyDefault, st));
+  return 0;
+}
+
 int vcl_llm_generate(vcl_handle* h, const int64_t* ids, const void* video_feats,
                      const int32_t* vid_start, int B, int S, int n_new, int32_t* out_tokens,
                      void* stream) {
@@ -1454,23 +1522,33 @@ int vcl_op_cross_entropy(const void* logits, int64_t ld, const int64_t* labels, 
   return loss_out != nullptr ? launch_nll_mean(nll_out, lab, rows, 0, nullptr, loss_out, as_stream(stream)) : 0;
 }
 
-int vcl_op_sample(const float* logits, int64_t ld, int B, int V, const float* temperature_host,
-                  const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host, int32_t* tok_out,
-                  void* stream) {
+}  // extern "C"
+
+namespace {
+
+// vcl_op_sample / vcl_op_sample_logprobs: top_n_host null, or log-prob rows [B][1 + VCL_LOGPROBS_MAX] to ids_out / lp_out
+int op_sample(const char* name, const float* logits, int64_t ld, int B, int V, const float* temperature_host,
+              const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
+              const int32_t* top_n_host, int32_t* tok_out, int32_t* ids_out, float* lp_out, void* stream) {
   if (check_device() != 0) return -2;
-  VCL_REQUIRE(logits && temperature_host && top_k_host && seed_host && counter_host && tok_out,
-              "vcl_op_sample: null argument");
-  VCL_REQUIRE(B >= 1, "vcl_op_sample: B=%d", B);
+  VCL_REQUIRE(logits && temperature_host && top_k_host && seed_host && counter_host && tok_out, "%s: null argument",
+              name);
+  VCL_REQUIRE(B >= 1, "%s: B=%d", name, B);
   for (int b = 0; b < B; ++b)
     VCL_REQUIRE(isfinite(temperature_host[b]) && temperature_host[b] >= 0.f && top_k_host[b] >= 0 &&
-                counter_host[b] >= 0, "vcl_op_sample: row %d: temperature %g, top_k %d, counter %d", b,
+                counter_host[b] >= 0, "%s: row %d: temperature %g, top_k %d, counter %d", name, b,
                 (double)temperature_host[b], top_k_host[b], counter_host[b]);
-  // the per-row settings in one stream-ordered block: [B] seeds, temperatures, top_k, counters
-  std::vector<unsigned char> hb((size_t)B * 20);
+  if (top_n_host != nullptr)
+    for (int b = 0; b < B; ++b)
+      VCL_REQUIRE(top_n_host[b] >= -1 && top_n_host[b] <= VCL_LOGPROBS_MAX, "%s: row %d: top_n %d outside -1..%d",
+                  name, b, top_n_host[b], VCL_LOGPROBS_MAX);
+  // the per-row settings in one stream-ordered block: [B] seeds, temperatures, top_k, counters, top_n
+  std::vector<unsigned char> hb((size_t)B * 24);
   memcpy(hb.data(), seed_host, (size_t)B * 8);
   memcpy(hb.data() + (size_t)B * 8, temperature_host, (size_t)B * 4);
   memcpy(hb.data() + (size_t)B * 12, top_k_host, (size_t)B * 4);
   memcpy(hb.data() + (size_t)B * 16, counter_host, (size_t)B * 4);
+  if (top_n_host != nullptr) memcpy(hb.data() + (size_t)B * 20, top_n_host, (size_t)B * 4);
   cudaStream_t st = as_stream(stream);
   unsigned char* d = nullptr;
   VCL_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&d), hb.size(), st));
@@ -1482,9 +1560,33 @@ int vcl_op_sample(const float* logits, int64_t ld, int B, int V, const float* te
   sa.top_k = reinterpret_cast<const int*>(d + (size_t)B * 12);
   sa.col_dev = reinterpret_cast<const int*>(d + (size_t)B * 16);
   sa.out = tok_out;
+  if (top_n_host != nullptr) {   // row b's places at ids_out / lp_out + b * (1 + VCL_LOGPROBS_MAX), any counter
+    sa.top_n = reinterpret_cast<const int*>(d + (size_t)B * 20);
+    sa.lp_id = ids_out; sa.lp_val = lp_out; sa.lp_entry = 1 + VCL_LOGPROBS_MAX; sa.lp_pos = 0; sa.lp_rows = 0x7fffffff;
+  }
   const int rc = launch_sample(sa, st);
   VCL_CUDA_OK(cudaFreeAsync(d, st));
   return rc;
+}
+
+}  // namespace
+
+extern "C" {
+
+int vcl_op_sample(const float* logits, int64_t ld, int B, int V, const float* temperature_host,
+                  const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host, int32_t* tok_out,
+                  void* stream) {
+  return op_sample("vcl_op_sample", logits, ld, B, V, temperature_host, top_k_host, seed_host, counter_host, nullptr,
+                   tok_out, nullptr, nullptr, stream);
+}
+
+int vcl_op_sample_logprobs(const float* logits, int64_t ld, int B, int V, const float* temperature_host,
+                           const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
+                           const int32_t* top_n_host, int32_t* tok_out, int32_t* ids_out, float* lp_out,
+                           void* stream) {
+  VCL_REQUIRE(top_n_host && ids_out && lp_out, "vcl_op_sample_logprobs: null argument");
+  return op_sample("vcl_op_sample_logprobs", logits, ld, B, V, temperature_host, top_k_host, seed_host, counter_host,
+                   top_n_host, tok_out, ids_out, lp_out, stream);
 }
 
 int vcl_op_layernorm(const void* x, void* y, const void* w, const void* b, int rows, int D, float eps,

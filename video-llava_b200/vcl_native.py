@@ -134,6 +134,8 @@ _SIGNATURES = {
     "vcl_llm_slot_decode": (c_int, [c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_void_p, c_void_p]),
     "vcl_llm_set_sampling": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_float), POINTER(c_int32),
                                      POINTER(c_uint64), c_void_p]),
+    "vcl_llm_set_logprobs": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), c_void_p]),
+    "vcl_llm_read_logprobs": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_launch_count": (ctypes.c_longlong, []),
     "vcl_kv_cache_copy": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_llm_set_block_table": (c_int, [c_void_p, POINTER(c_int32), c_void_p]),
@@ -147,6 +149,9 @@ _SIGNATURES = {
                                c_int64, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "vcl_op_sample": (c_int, [c_void_p, c_int64, c_int, c_int, POINTER(c_float), POINTER(c_int32), POINTER(c_uint64),
                               POINTER(c_int32), c_void_p, c_void_p]),
+    "vcl_op_sample_logprobs": (c_int, [c_void_p, c_int64, c_int, c_int, POINTER(c_float), POINTER(c_int32),
+                                       POINTER(c_uint64), POINTER(c_int32), POINTER(c_int32), c_void_p, c_void_p,
+                                       c_void_p, c_void_p]),
     "vcl_op_layernorm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "vcl_op_rmsnorm": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "vcl_op_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
@@ -291,6 +296,29 @@ def op_sample(logits, temperature, top_k, seed, counter):
                               (c_float * B)(*[float(t) for t in vals[0]]), (c_int32 * B)(*[int(k) for k in vals[1]]),
                               _seeds(seed, B), (c_int32 * B)(*[int(c) for c in vals[2]]), ptr(out), cur_stream()))
     return out
+
+
+LOGPROBS_MAX = 20              # include/vcl.h: VCL_LOGPROBS_MAX, the most alternatives per token
+LOGPROB_PLACES = 1 + LOGPROBS_MAX
+
+
+def op_sample_logprobs(logits, temperature, top_k, seed, counter, top_n):
+    """The sampling kernel with log-probs (vcl_op_sample_logprobs): op_sample's arguments plus top_n, B host ints
+    (-1 .. LOGPROBS_MAX). Returns (tokens [B] int32, ids [B, LOGPROB_PLACES] int32, lp [B, LOGPROB_PLACES] f32) on
+    the device: place 0 the chosen token, places 1 .. top_n[b] the alternatives; places past top_n[b] are -1 / NaN."""
+    B, ld = logits.shape
+    assert logits.dtype == torch.float32 and logits.stride(1) == 1
+    vals = [list(v) for v in (temperature, top_k, counter, top_n)]
+    if not all(len(v) == B for v in vals):
+        raise VclError(f"temperature / top_k / counter / top_n need {B} entries each")
+    out = torch.empty(B, dtype=torch.int32, device=logits.device)
+    ids = torch.full((B, LOGPROB_PLACES), -1, dtype=torch.int32, device=logits.device)
+    lp = torch.full((B, LOGPROB_PLACES), float("nan"), dtype=torch.float32, device=logits.device)
+    ints = lambda v: (c_int32 * B)(*[int(x) for x in v])   # noqa: E731
+    check(lib().vcl_op_sample_logprobs(c_void_p(logits.data_ptr()), logits.stride(0), B, ld,
+                                       (c_float * B)(*[float(t) for t in vals[0]]), ints(vals[1]), _seeds(seed, B),
+                                       ints(vals[2]), ints(vals[3]), ptr(out), ptr(ids), ptr(lp), cur_stream()))
+    return out, ids, lp
 
 
 def op_gemv(x, w, res=None, norm_w=None, eps=0.0):
@@ -578,6 +606,32 @@ class Engine:
         check(lib().vcl_llm_set_sampling(self._h, n, (c_int32 * n)(*[int(b) for b in clips]),
                                          (c_float * n)(*[float(t) for t in temperature]),
                                          (c_int32 * n)(*[int(k) for k in top_k]), _seeds(seed, n), cur_stream()))
+
+    # ---- log-probs of generated tokens ----
+    sample_logprobs_op = staticmethod(op_sample_logprobs)
+
+    def set_logprobs(self, clips, top_n):
+        """Entries `clips` of the sampling table report log-probs (vcl_llm_set_logprobs): top_n[i] -1 (off), 0 (the
+        chosen token) or 1 .. LOGPROBS_MAX alternatives as well. Host lists of equal length."""
+        n = len(clips)
+        if len(top_n) != n:
+            raise VclError(f"{n} clips, {len(top_n)} top_n")
+        check(lib().vcl_llm_set_logprobs(self._h, n, (c_int32 * n)(*[int(b) for b in clips]),
+                                         (c_int32 * n)(*[int(k) for k in top_n]), cur_stream()))
+
+    def read_logprobs(self, entry, first_pos, count, ids_out=None, lp_out=None):
+        """The log-prob rows of positions first_pos .. first_pos + count - 1 of entry `entry` (vcl_llm_read_logprobs):
+        (ids [count, LOGPROB_PLACES] int32, lp [count, LOGPROB_PLACES] f32), device tensors unless given (any
+        contiguous device or host tensors of that size)."""
+        if ids_out is None:
+            ids_out = torch.empty(int(count), LOGPROB_PLACES, dtype=torch.int32, device="cuda")
+        if lp_out is None:
+            lp_out = torch.empty(int(count), LOGPROB_PLACES, dtype=torch.float32, device="cuda")
+        for t, dt in ((ids_out, torch.int32), (lp_out, torch.float32)):
+            assert t.dtype == dt and t.is_contiguous() and t.numel() == int(count) * LOGPROB_PLACES
+        check(lib().vcl_llm_read_logprobs(self._h, int(entry), int(first_pos), int(count), c_void_p(ids_out.data_ptr()),
+                                          c_void_p(lp_out.data_ptr()), cur_stream()))
+        return ids_out, lp_out
 
     # ---- KV cache read-back (tests) ----
     def _cache_shape(self):

@@ -313,6 +313,8 @@ class VideoChatGPTLlamaForCausalLM:
         vn.weight_format_code(llm_weight_format)          # ValueError before anything else
         self._kv_blocks = vn.check_kv_blocks(kv_blocks)
         self.last_kv_stats = None
+        self.last_logprobs = None      # generate / generate_continue / generate_requests(logprobs=...): per row or request
+        self._pads = None              # the left padding of the last generate (log-prob positions of generate_continue)
         self._sessions: dict = {}      # kept conversations of generate_requests (paged): key -> _schedule_paged's state
         self._session_clock = 0        # last-use stamps of the kept conversations (the least recent is swapped first)
         self._n_slots = vn.slot_capacity(max_batch, max_slots)
@@ -600,10 +602,56 @@ class VideoChatGPTLlamaForCausalLM:
         finally:
             eng.set_sampling(clips, [0.0] * len(clips), [0] * len(clips), [0] * len(clips))
 
+    @staticmethod
+    def _logprobs_arg(v, what):
+        """Checks a logprobs setting on the host: None (off) or an int 0 .. vn.LOGPROBS_MAX"""
+        if v is None:
+            return None
+        if isinstance(v, bool) or not isinstance(v, int) or not 0 <= v <= vn.LOGPROBS_MAX:
+            raise ValueError(f"{what}: logprobs {v!r} must be None or an int 0..{vn.LOGPROBS_MAX} (the alternatives "
+                             "reported per token besides the chosen one)")
+        return v
+
+    @contextlib.contextmanager
+    def _logprobs(self, eng, clips, top_n):
+        """Entries `clips` report top_n alternatives (None: nothing changes) for the duration of the block and are off
+        again afterwards, also when the block raises."""
+        if top_n is None:
+            yield
+            return
+        eng.set_logprobs(clips, [top_n] * len(clips))
+        try:
+            yield
+        finally:
+            eng.set_logprobs(clips, [-1] * len(clips))
+
+    @staticmethod
+    def _logprob_entry(ids, lp, k):
+        """host rows ids / lp [n, 1 + LOGPROBS_MAX] -> one entry of last_logprobs"""
+        return dict(token_logprobs=lp[:, 0].clone(), top_ids=ids[:, 1:1 + k].to(torch.int64),
+                    top_logprobs=lp[:, 1:1 + k].clone())
+
+    def _read_logprobs(self, eng, new, p0, k, eos):
+        """last_logprobs of a static batch: row b's new tokens new[b] [n] took positions p0[b] .. p0[b] + n - 1 of
+        entry b. Positions after a row's first EOS (its padding) hold NaN / -1."""
+        B, n = new.shape
+        out = []
+        for b in range(B):
+            ids, lp = eng.read_logprobs(b, p0[b], n)
+            e = self._logprob_entry(ids.cpu(), lp.cpu(), k)
+            hit = (new[b] == eos).nonzero() if eos is not None else []
+            if len(hit):
+                f = int(hit[0]) + 1
+                e["token_logprobs"][f:] = float("nan")
+                e["top_ids"][f:] = -1
+                e["top_logprobs"][f:] = float("nan")
+            out.append(e)
+        return out
+
     @torch.no_grad()
     def generate(self, input_ids, video_spatio_temporal_features=None, do_sample=False, temperature=1.0,
                  max_new_tokens=32, stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50,
-                 attention_mask=None, seed=None, **kw):
+                 attention_mask=None, seed=None, logprobs=None, **kw):
         """Returns [B, S+n] int64 INCLUDING the prompt, like HF generate (inference.py:105-120), and
         like HF it stops at EOS (config.eos_token_id unless eos_token_id is given; None disables it):
         finished rows are padded, the call returns when every row has finished.
@@ -618,12 +666,23 @@ class VideoChatGPTLlamaForCausalLM:
         top-k rules, row b with seed + b (mod 2**64), through the prefill and the CUDA-graph loops; EOS, padding
         and stopping criteria are applied on the host between loops of _GREEDY_CHUNK tokens, token by token as
         the stepwise path does. Each row's tokens depend on its seed and positions only. Without a seed,
-        do_sample=True keeps the stepwise path and torch's RNG (torch.manual_seed)."""
+        do_sample=True keeps the stepwise path and torch's RNG (torch.manual_seed).
+        logprobs (an int 0 .. 20): self.last_logprobs gets, per row, the log-probabilities of its new tokens as
+        compute_transition_scores(normalize_logits=True) gives them on HF's scores (DESIGN.md section 3):
+        token_logprobs f32 [n_new], and the `logprobs` most likely tokens of each step, top_ids int64 [n_new, k] and
+        top_logprobs f32 [n_new, k]; positions after a row's EOS hold NaN / -1. They are computed on the device next
+        to the token, so greedy calls take the device loops (the seeded path's, with greedy entries) and return the
+        same tokens; unseeded sampling cannot report them (NotImplementedError: pass seed=)."""
         self._not_paged("generate")
+        lp_n = self._logprobs_arg(logprobs, "generate")
+        if lp_n is not None and do_sample and seed is None:
+            raise NotImplementedError("generate: logprobs are computed by the device sampler, and sampling there needs "
+                                      "seed= (unseeded do_sample=True draws from torch's RNG on the host)")
         seeded = do_sample and seed is not None
         if seeded:
             temperature, top_k, seed = self._sampling_args(temperature, top_k, seed)
         pads = left_padding(attention_mask, input_ids.shape)
+        self.last_logprobs = None
         eng = self._ensure_engine(need_llm=True)
         ids = input_ids.cuda().to(torch.int64)
         B, S = ids.shape
@@ -635,9 +694,12 @@ class VideoChatGPTLlamaForCausalLM:
         if n <= 0:
             raise ValueError(f"prompt length {S} leaves no room in max_seq {self._max_seq}")
         eos, pad = self._eos_pad(eos_token_id, pad_token_id)
-        if seeded:
+        self._pads = pads
+        if seeded or lp_n is not None:
             clips = list(range(B))
-            with self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips]):
+            samp = (self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips]) if seeded
+                    else contextlib.nullcontext())
+            with samp, self._logprobs(eng, clips, lp_n):
                 if eos is None and not stopping_criteria:
                     new = eng.generate(ids, feats, vs, n, n_pad=pads)
                     self._pos = S + n - 1
@@ -645,6 +707,9 @@ class VideoChatGPTLlamaForCausalLM:
                 else:
                     first = eng.generate(ids, feats, vs, min(n, self._GREEDY_CHUNK), n_pad=pads)
                     self._last_out = self._host_stops(eng, ids, first, n, stopping_criteria, eos, pad)
+            if lp_n is not None:   # the token after the prompt takes position S - n_pad[b]
+                self.last_logprobs = self._read_logprobs(eng, self._last_out[:, S:].cpu(),
+                                                         [S - (pads[b] if pads else 0) for b in range(B)], lp_n, eos)
             return self._last_out
         if do_sample or stopping_criteria:
             _, logits, _ = eng.prefill(ids, feats, vs, want_logits=True, want_token=False, n_pad=pads)
@@ -736,7 +801,7 @@ class VideoChatGPTLlamaForCausalLM:
     @torch.no_grad()
     def generate_requests(self, requests, max_new_tokens=32, eos_token_id="config", stopping_criteria=None,
                           slots=None, do_sample=False, packed_admission=False, temperature=1.0, top_k=50, seed=None,
-                          chunked_prefill=False):
+                          chunked_prefill=False, logprobs=None):
         """Greedy generation for many independent requests by in-flight (continuous) batching: every request
         owns a slot of the KV cache while it runs, and a finished request's slot takes the next queued one at
         once while the other slots keep decoding (a static batch decodes until its longest row finishes).
@@ -784,9 +849,16 @@ class VideoChatGPTLlamaForCausalLM:
         already kept, a key started and continued in one call, a key continued twice in one call, video features on
         a continuation, and a continuation that overflows max_seq or the pool. last_kv_stats then also counts the
         continuations, the prefill rows they did not recompute (reused_rows), the conversations swapped out
-        (session_swaps, session_swapped_bytes) and the conversations kept, resident and swapped at the end."""
+        (session_swaps, session_swapped_bytes) and the conversations kept, resident and swapped at the end.
+        logprobs (an int 0 .. 20, or a request's own "logprobs" key): self.last_logprobs[i] holds request i's
+        log-probabilities as generate(logprobs=...) reports them, for its new tokens only (a continuation: this
+        turn's), or None when the request did not ask. Each admission writes the admitted slots' log-prob entries
+        (a slot without a request is off), and each decode chunk's rows come back in one copy; the values do not
+        depend on slot, neighbours, queue order, admission mode, paging or preemption."""
+        self._logprobs_arg(logprobs, "generate_requests")
         for i, r in enumerate(requests):
             r = r if isinstance(r, dict) else {}
+            self._logprobs_arg(r.get("logprobs", logprobs), f"request {i}")
             if not self._kv_blocks and (r.get("session") is not None or r.get("continues") is not None):
                 raise ValueError(f"request {i}: conversation sessions (\"session\" / \"continues\") need a paged KV "
                                  "cache (kv_blocks=...); on this model use generate and generate_continue")
@@ -800,25 +872,33 @@ class VideoChatGPTLlamaForCausalLM:
                 raise ValueError(f"slots={slots} outside 1..{cap} (max_slots {self._max_slots})")
             raise ValueError(f"slots={slots} outside 1..{cap} (at most 16 and at most max_batch {self._max_batch})")
         eng = self._ensure_engine(need_llm=True)
-        samp = dict(do_sample=do_sample, temperature=temperature, top_k=top_k, seed=seed)
+        samp = dict(do_sample=do_sample, temperature=temperature, top_k=top_k, seed=seed, logprobs=logprobs)
         reqs = [self._request(i, r, max_new_tokens, stopping_criteria, eng.NV, samp) for i, r in enumerate(requests)]
         if self._kv_blocks:
             self._bind_sessions(reqs)
             self._check_paged(reqs, chunked_prefill)
         sampling = any(r.temperature > 0 for r in reqs)
         eos, _ = self._eos_pad(eos_token_id, None)
-        self._last_out, self._pos = None, 0
+        self._last_out, self._pos, self.last_logprobs = None, 0, None
         n_slots = min(n_slots, len(reqs))
+        lps = _RequestLogprobs(eng, reqs, n_slots, self.device)
         try:
             if self._kv_blocks:
-                return self._schedule_paged(eng, reqs, n_slots, packed_admission, sampling, eos, chunked_prefill)
-            return self._schedule(eng, reqs, n_slots, packed_admission, sampling, eos)
+                out = self._schedule_paged(eng, reqs, n_slots, packed_admission, sampling, eos, chunked_prefill, lps)
+            else:
+                out = self._schedule(eng, reqs, n_slots, packed_admission, sampling, eos, lps)
+            if lps.on:
+                self.last_logprobs = lps.result()
+            return out
         finally:
             if sampling:
                 eng.set_sampling(list(range(n_slots)), [0.0] * n_slots, [0] * n_slots, [0] * n_slots)
+            if lps.on:
+                eng.set_logprobs(list(range(n_slots)), [-1] * n_slots)
 
-    def _schedule(self, eng, reqs, n_slots, packed_admission, sampling, eos):
+    def _schedule(self, eng, reqs, n_slots, packed_admission, sampling, eos, lps=None):
         """The admission / decode loop of generate_requests"""
+        lps = lps or _RequestLogprobs(eng, reqs, n_slots, self.device)
         dev = self.device
         results = [None] * len(reqs)
         queue = collections.deque(range(len(reqs)))
@@ -838,6 +918,7 @@ class VideoChatGPTLlamaForCausalLM:
                 rs = [reqs[i] for _, i in admitted]
                 eng.set_sampling([s for s, _ in admitted], [r.temperature for r in rs], [r.top_k for r in rs],
                                  [r.seed for r in rs])
+            lps.sync(owner)
             if admitted and packed_admission:
                 self._admit_packed(eng, [(s, reqs[i]) for s, i in admitted], first)
             elif admitted:
@@ -854,6 +935,7 @@ class VideoChatGPTLlamaForCausalLM:
             out = eng.slot_decode(first, pos, m + 1)
             first = out[:, m].contiguous()
             host = out.tolist()
+            running = [(s, owner[s]) for s in active]
             for s in active:
                 i = owner[s]
                 r = reqs[i]
@@ -865,6 +947,7 @@ class VideoChatGPTLlamaForCausalLM:
                         owner[s], pos[s] = None, 0
                         break
                 unseen[s] = False
+            lps.collect([(s, i, len(gen[i])) for s, i in running])
 
     def _admit_packed(self, eng, group, first):
         """Prefill the (slot, request) pairs of one admission point: prompts longer than _PACKED_MAX_S one at a time
@@ -929,7 +1012,7 @@ class VideoChatGPTLlamaForCausalLM:
                 raise ValueError(f"request {i}: prompt {r.S} + max_new_tokens {r.n} needs {need} blocks of {C} columns, "
                                  f"more than the pool's {usable} (kv_blocks {self._kv_blocks}, block 0 is the park block)")
 
-    def _schedule_paged(self, eng, reqs, n_slots, packed_admission, sampling, eos, chunked=False):
+    def _schedule_paged(self, eng, reqs, n_slots, packed_admission, sampling, eos, chunked=False, lps=None):
         """The admission / decode loop of generate_requests on a paged KV cache. The host keeps a free list and each
         slot's row of the block table (block 0, the park block, wherever no request owns a block), and writes the
         whole table to the engine before every prefill and every decode chunk.
@@ -953,8 +1036,11 @@ class VideoChatGPTLlamaForCausalLM:
         - Eviction. Kept conversations are idle: when an admission, a resume or a chunk's growth is short of blocks,
           the least recently used one that is resident is swapped to pinned host memory (its blocks freed) before
           anything waits or any running request is preempted.
+        - Log-probs (lps). A request swapped out before its first token reached the host takes that token's row
+          along (it lives in its old slot's entry); every other row is read after the chunk that produced it.
         _check_paged guarantees that the oldest running request alone always fits."""
         dev, C, K = self.device, vn.KV_BLOCK_COLS, self._SLOT_CHUNK
+        lps = lps or _RequestLogprobs(eng, reqs, n_slots, self.device)
         sessions = self._sessions
         table = [[0] * eng.table_row for _ in range(eng.n_slots)]    # every slot of the engine, parked
         kept = {b for ss in sessions.values() if ss.blocks is not None for b in ss.blocks}
@@ -1008,6 +1094,8 @@ class VideoChatGPTLlamaForCausalLM:
 
         def swap_out(s):
             i = owner[s]
+            if unseen[s]:
+                lps.collect([(s, i, 1)])
             saved = []
             for b in blocks[s][:-(-pos[s] // C)]:        # the blocks that hold written columns
                 buf = eng.swap_buffer()
@@ -1072,6 +1160,7 @@ class VideoChatGPTLlamaForCausalLM:
                 rs = [(s, reqs[i]) for s, i in admitted + resumed + tails]
                 eng.set_sampling([s for s, _ in rs], [r.temperature for _, r in rs], [r.top_k for _, r in rs],
                                  [r.seed for _, r in rs])
+            lps.sync(owner)
             # continuations: the tails admitted here in one call under packed_admission, one call each otherwise
             for group in ([tails] if packed_admission and tails else [[t] for t in tails]):
                 tok = eng.slots_prefill_append([s for s, _ in group], [reqs[i].start for _, i in group],
@@ -1111,10 +1200,12 @@ class VideoChatGPTLlamaForCausalLM:
                     take(s, cover(owner[s], pos[s], m))
             active = [s for s in active if owner[s] is not None]
             eng.set_block_table(table)
+            lps.sync(owner)
             out = eng.slot_decode(first, pos, m + 1)
             first = out[:, m].contiguous()
             host = out.tolist()
             released.clear()                # the stream has passed every copy enqueued before the decode
+            running = [(s, owner[s]) for s in active]
             for s in active:
                 i = owner[s]
                 r = reqs[i]
@@ -1134,6 +1225,7 @@ class VideoChatGPTLlamaForCausalLM:
                         release(s, keep)
                         break
                 unseen[s] = False
+            lps.collect([(s, i, len(gen[i])) for s, i in running])
 
     def _request(self, i, r, max_new_tokens, stopping_criteria, n_vid, samp=None):
         """One request of generate_requests, checked on the host -> (ids [S] int64 on the host, S, n, feats,
@@ -1170,7 +1262,7 @@ class VideoChatGPTLlamaForCausalLM:
                 k, seed = 0, 0
         return SimpleNamespace(ids=ids, S=S, n=n, feats=feats, vid_start=vs, criteria=list(crit or []),
                                temperature=T, top_k=k, seed=seed, session=r.get("session"),
-                               continues=r.get("continues"), start=0)
+                               continues=r.get("continues"), start=0, lp=r.get("logprobs", samp.get("logprobs")))
 
     def _bind_sessions(self, reqs):
         """The "session" / "continues" keys of generate_requests' requests, checked on the host before any device
@@ -1236,17 +1328,24 @@ class VideoChatGPTLlamaForCausalLM:
         return len(gen) >= r.n
 
     def generate_continue(self, new_input_ids, do_sample=False, temperature=1.0, max_new_tokens=32,
-                          stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50, seed=None):
+                          stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50, seed=None,
+                          logprobs=None):
         """Next turn about the SAME video(s): `new_input_ids` [B, S_new] follow everything generated
         so far. Only the tokens the KV cache does not hold yet (the last generated token and the new
         text) are prefilled (vcl_llm_prefill_append); the reference re-runs the tower and the whole
         prompt every turn (chat.py:137-154). Returns the full sequence [B, S_total + n] like generate.
         After a left-padded generate the cache stays padded, so every row continues its own positions; the
         new text of every row has the same length S_new (no padding inside a turn).
-        seed: do_sample=True samples on the device as generate(seed=...) does."""
+        seed: do_sample=True samples on the device as generate(seed=...) does. logprobs: as in generate, for the new
+        tokens of this turn."""
         self._not_paged("generate_continue")
         if getattr(self, "_last_out", None) is None:
             raise ValueError("generate_continue: no previous generate() to continue")
+        lp_n = self._logprobs_arg(logprobs, "generate_continue")
+        if lp_n is not None and do_sample and seed is None:
+            raise NotImplementedError("generate_continue: logprobs are computed by the device sampler, and sampling "
+                                      "there needs seed= (unseeded do_sample=True draws from torch's RNG on the host)")
+        self.last_logprobs = None
         seeded = do_sample and seed is not None
         if seeded:
             temperature, top_k, seed = self._sampling_args(temperature, top_k, seed, "generate_continue")
@@ -1259,13 +1358,19 @@ class VideoChatGPTLlamaForCausalLM:
         if n <= 0:
             raise ValueError(f"context length {ctx.shape[1]} leaves no room in max_seq {self._max_seq}")
         eos, pad = self._eos_pad(eos_token_id, pad_token_id)
-        if seeded:
-            B = ctx.shape[0]
+        if seeded or lp_n is not None:
+            B, L = ctx.shape
             clips = list(range(B))
-            with self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips]):
+            samp = (self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips]) if seeded
+                    else contextlib.nullcontext())
+            with samp, self._logprobs(eng, clips, lp_n):
                 _, _, tok = eng.prefill_append(tail, start)
                 first = eng.decode_loop(tok, ctx.shape[1], min(n, self._GREEDY_CHUNK))
                 self._last_out = self._host_stops(eng, ctx, first, n, stopping_criteria, eos, pad)
+            if lp_n is not None:   # the cache keeps the padding of the generate it continues
+                pads = self._pads
+                self.last_logprobs = self._read_logprobs(eng, self._last_out[:, L:].cpu(),
+                                                         [L - (pads[b] if pads else 0) for b in range(B)], lp_n, eos)
             return self._last_out
         _, logits, _ = eng.prefill_append(tail, start, want_logits=True, want_token=False)
         self._pos = ctx.shape[1]
@@ -1298,4 +1403,55 @@ class VideoChatGPTLlamaForCausalLM:
                 break
             logits, _ = eng.decode_step(nxt.to(torch.int32).contiguous(), self._pos, want_logits=True)
             self._pos += 1
+        return out
+
+
+class _RequestLogprobs:
+    """The log-probs of one generate_requests call: the slots' entries as the engine holds them, and each request's
+    rows read so far (blocks of rows, one row per new token, in order). Request i's k-th new token took position
+    reqs[i].S + k of its slot's entry."""
+
+    def __init__(self, eng, reqs, n_slots, dev):
+        self.eng, self.reqs, self.dev = eng, reqs, dev
+        self.on = any(r.lp is not None for r in reqs)
+        self.written = [-1] * n_slots
+        self.rows = {i: [] for i, r in enumerate(reqs) if r.lp is not None}
+        self.have = {i: 0 for i in self.rows}
+
+    def sync(self, owner):
+        """One set_logprobs call for the slots whose entry changed: the top_n of the slot's request, -1 without one"""
+        if not self.on:
+            return
+        want = [-1 if i is None or self.reqs[i].lp is None else self.reqs[i].lp for i in owner]
+        changed = [s for s, w in enumerate(want) if w != self.written[s]]
+        if changed:
+            self.eng.set_logprobs(changed, [want[s] for s in changed])
+            for s in changed:
+                self.written[s] = want[s]
+
+    def collect(self, running):
+        """(slot, request, its new tokens so far): read the rows the host does not hold yet, all in one copy"""
+        reads = [(s, i, self.have[i], n - self.have[i]) for s, i, n in running if i in self.rows and n > self.have[i]]
+        if not reads:
+            return
+        total = sum(c for *_, c in reads)
+        ids = torch.empty(total, vn.LOGPROB_PLACES, dtype=torch.int32, device=self.dev)
+        lp = torch.empty(total, vn.LOGPROB_PLACES, dtype=torch.float32, device=self.dev)
+        o = 0
+        for s, i, had, c in reads:
+            self.eng.read_logprobs(s, self.reqs[i].S + had, c, ids_out=ids[o:o + c], lp_out=lp[o:o + c])
+            o += c
+        ids, lp = ids.cpu(), lp.cpu()
+        o = 0
+        for s, i, had, c in reads:
+            self.rows[i].append((ids[o:o + c], lp[o:o + c]))
+            self.have[i] += c
+            o += c
+
+    def result(self):
+        out = [None] * len(self.reqs)
+        for i, rows in self.rows.items():
+            ids = torch.cat([a for a, _ in rows])
+            lp = torch.cat([b for _, b in rows])
+            out[i] = VideoChatGPTLlamaForCausalLM._logprob_entry(ids, lp, self.reqs[i].lp)
         return out
