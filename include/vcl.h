@@ -329,6 +329,39 @@ int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* 
 int vcl_llm_set_sampling(vcl_handle* h, int n, const int32_t* clips_host, const float* temperature_host,
                          const int32_t* top_k_host, const uint64_t* seed_host, void* stream);
 
+/* Top-p (nucleus) sampling and the repetition penalty (HF's TopPLogitsWarper and RepetitionPenaltyLogitsProcessor,
+ * in HF's order: penalty, temperature, top-k, top-p). vcl_llm_set_sampling_ex is vcl_llm_set_sampling plus, per
+ * entry, top_p_host[i] (0 .. 1; 1 off) and repetition_penalty_host[i] (> 0; 1 off); vcl_llm_set_sampling itself sets
+ * both to 1. The penalty applies to greedy and sampled entries: a logit x of a token in the entry's TOKEN SET becomes
+ * x < 0 ? x * r : x / r (fp32) before the temperature. Top-p applies to sampled entries: of the tokens top-k keeps,
+ * those whose mass strictly above them (fixed-point, in key order) is below top_p times the kept mass, ties whole
+ * and the largest always kept; the draw and the log-probs then use that final set. The exact rules are in DESIGN.md
+ * section 3. An entry with either setting takes a 32-bit sampler that adds the token it picks to the entry's token
+ * set, so a decode loop keeps it current on the device; a call uses it when one of its entries has a penalty, or
+ * samples with top_p < 1, and then launches it instead of the arg-max kernels (a sampled decode loop of these entries
+ * has its own CUDA graph per (B, n_new)). Calls whose entries all have top_p 1 and penalty 1 launch what they
+ * launched before. The first call that turns a penalty on allocates the token sets, one bitmap of ceil(vocab / 32)
+ * int32 words per entry (256 KB at max_batch 64, vocab 32003). Rejected before any device work: what
+ * vcl_llm_set_sampling rejects, a top_p outside [0, 1] or NaN, a penalty <= 0 or not finite, and either setting on
+ * a vocabulary over VCL_SAMPLE_WIDE_MAX_V (the 32-bit sampler stages a row of 4-byte keys in shared memory). */
+#define VCL_SAMPLE_WIDE_MAX_V 57344
+int vcl_llm_set_sampling_ex(vcl_handle* h, int n, const int32_t* clips_host, const float* temperature_host,
+                            const int32_t* top_k_host, const uint64_t* seed_host, const float* top_p_host,
+                            const float* repetition_penalty_host, void* stream);
+
+/* The token set of entry `entry` (HF's input_ids of its row: the prompt with its video placeholder and pad ids, then
+ * every token generated so far; for a continued conversation the whole conversation): cleared, then ids[0 .. n)
+ * (DEVICE int64; ids outside 0 .. vocab-1 are ignored) marked, in one kernel on `stream`. Set it before the call that
+ * produces the entry's first token with a penalty; the sampler then adds each token it picks. Rejected before any
+ * device work: an entry outside 0 .. max_batch-1, n < 0, null ids with n > 0, a vocabulary over
+ * VCL_SAMPLE_WIDE_MAX_V. */
+int vcl_llm_set_token_set(vcl_handle* h, int entry, const int64_t* ids, int n, void* stream);
+
+/* Copy entry `entry`'s token set, ceil(vocab / 32) uint32 words (bit i & 31 of word i >> 5: token i), to bits_out
+ * (host or device memory), ordered on `stream`. Rejected: a null argument, an entry outside 0 .. max_batch-1, a
+ * handle that never allocated its token sets. */
+int vcl_llm_read_token_set(vcl_handle* h, int entry, uint32_t* bits_out, void* stream);
+
 /* Log-probabilities of generated tokens: what HF returns as generate(output_scores=True) followed by
  * compute_transition_scores(sequences, scores, normalize_logits=True) ($TF/generation/utils.py), plus the top-n
  * alternatives of each step, computed on the device by the sampler next to the token it picks. For the token of
@@ -445,6 +478,15 @@ int vcl_op_sample_logprobs(const float* logits, int64_t ld, int B, int V, const 
                            const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
                            const int32_t* top_n_host, int32_t* tok_out, int32_t* ids_out, float* lp_out,
                            void* stream);
+/* The 32-bit sampler on its own (vcl_llm_set_sampling_ex): vcl_op_sample with top_p_host[b] and
+ * repetition_penalty_host[b] (HOST memory, [B]), token_sets [B][ceil(V / 32)] uint32 on the device (null: every
+ * set empty; row b's picked token is added to its set) and, when top_n_host is not null, vcl_op_sample_logprobs'
+ * log-probs. A row with top_p 1 and penalty 1 gives vcl_op_sample(_logprobs)'s token and values bit for bit.
+ * V <= VCL_SAMPLE_WIDE_MAX_V. */
+int vcl_op_sample_ex(const float* logits, int64_t ld, int B, int V, const float* temperature_host,
+                     const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
+                     const float* top_p_host, const float* repetition_penalty_host, uint32_t* token_sets,
+                     const int32_t* top_n_host, int32_t* tok_out, int32_t* ids_out, float* lp_out, void* stream);
 int vcl_op_layernorm(const void* x, void* y, const void* w, const void* b, int rows, int D, float eps,
                      void* stream);
 int vcl_op_rmsnorm(const void* x, void* y, const void* w, int rows, int D, float eps, void* stream);

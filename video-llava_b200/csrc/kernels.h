@@ -162,6 +162,12 @@ int launch_nll_mean(const float* nll, const long long* labels, long long rows, i
 #ifndef VCL_LOGPROBS_MAX
 #define VCL_LOGPROBS_MAX 20   // include/vcl.h
 #endif
+// The 32-bit path (top_p set; V <= VCL_SAMPLE_WIDE_MAX_V): entry t also has top_p[t] (1: off) and the repetition
+// penalty rep[t] (1: off), applied to the tokens of its set, bitmap tset[t * tset_words ..] (null: every set empty),
+// to which the sampler adds the token it picks.
+#ifndef VCL_SAMPLE_WIDE_MAX_V
+#define VCL_SAMPLE_WIDE_MAX_V 57344   // include/vcl.h
+#endif
 struct SampleArgs {
   const float* logits = nullptr; long long ld = 0; int V = 0, B = 0;
   const float* temperature = nullptr; const int* top_k = nullptr; const unsigned long long* seed = nullptr;
@@ -171,8 +177,13 @@ struct SampleArgs {
   const int* top_n = nullptr;
   int* lp_id = nullptr; float* lp_val = nullptr;
   long long lp_entry = 0, lp_pos = 0; int lp_rows = 0;
+  const float* top_p = nullptr; const float* rep = nullptr;
+  unsigned int* tset = nullptr; int tset_words = 0;
 };
 int launch_sample(const SampleArgs& a, cudaStream_t stream);
+// one token set: dst[0 .. words) cleared, then the bits of ids[0 .. n) (device int64; ids outside 0 .. V-1 ignored)
+// set, in one launch
+int launch_token_set(unsigned int* dst, int words, const long long* ids, int n, int V, cudaStream_t stream);
 
 // ---- attention.cu -------------------------------------------------------------------------------
 // softmax(Q K^T * scale [+ causal]) V for S_q == S_kv, bf16, fp32 softmax; element (b,h,s,d) of

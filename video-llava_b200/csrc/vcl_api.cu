@@ -12,6 +12,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <map>
 #include <string>
 #include <vector>
@@ -58,8 +59,9 @@ struct LlmLayerW {
 };
 struct GraphEntry {
   int B, n_new;        // the positions and pad counts are read on the device (h->d_pos, h->d_npad) ...
-  bool sampled;        // ... and so is the sampling table: a graph of the sampler serves every temperature / top_k /
-                       // seed / top_n
+  int sampled;         // ... and so is the sampling table: a graph of the sampler serves every temperature / top_k /
+                       // seed / top_n (h->sampler: 0 the arg-max, 1 the 16-bit sampler, 2 the 32-bit one, whose
+                       // graphs serve every top_p / repetition penalty too)
   cudaGraphExec_t exec;
   long long kernels;   // kernel nodes in the graph (for vcl_launch_count)
   unsigned long long last_use;
@@ -75,15 +77,15 @@ struct StepIo {
   float* logits_out = nullptr;
   int32_t* tok_out = nullptr; long long out_stride = 1;
   const int* pos_dev = nullptr;   // clip b at position pos + pos_dev[b] (null: pos)
-  bool sampled = false;           // the sampler picks tok_out (entry b of the sampling table for clip b) and writes
+  int sampled = 0;                // (h->sampler) the sampler picks tok_out (entry b of the sampling table for clip b) and writes
                                   // the log-probs of the entries that ask for them
 };
 
 // which sampling-table entries the rows of an lm_head call use, and the cache column their tokens take
 // (SampleArgs in kernels.h; the counter subtracts the clip's left padding)
 struct SampleAt {
-  bool on = false;                              // some entry samples or wants log-probs: the sampler replaces
-                                                // the arg-max kernel
+  int on = 0;                                   // some entry samples or wants log-probs: the sampler replaces
+                                                // the arg-max kernel (h->sampler: 2 the 32-bit sampler)
   int entry0 = 0; const int* rowmap = nullptr;  // row r: entry entry0 + (rowmap ? rowmap[r] : r)
   int col = 0; const int* col_dev = nullptr;    // row r: column col + (col_dev ? col_dev[r] : 0)
 };
@@ -137,24 +139,38 @@ struct vcl_handle {
   ArgmaxPart* amax = nullptr;                  // [gemv_grid(vocab)][max_batch] per-CTA partial arg-max of the logits kernel
   int* d_pack = nullptr;                       // pack_elems(max_batch * max_seq): the packed-row map of kernels.h,
                                                // written by each vcl_llm_slots_prefill with one host-to-device copy
-  // The sampling table (vcl_llm_set_sampling, vcl_llm_set_logprobs): entry b belongs to clip b / cache slot b. One
-  // device block at a fixed address, [max_batch] seeds (u64), temperatures (f32), top_k (i32), top_n (i32), so one
-  // sampled decode graph serves every setting; samp_host is its host copy, written whole by one host-to-device copy
-  // per call. Greedy without log-probs (top_n -1) at vcl_create.
+  // The sampling table (vcl_llm_set_sampling(_ex), vcl_llm_set_logprobs): entry b belongs to clip b / cache slot b.
+  // One device block at a fixed address, [max_batch] seeds (u64), temperatures (f32), top_k (i32), top_n (i32),
+  // top_p (f32), repetition penalties (f32), so one sampled decode graph serves every setting; samp_host is its host
+  // copy, written whole by one host-to-device copy per call. Greedy without log-probs (top_n -1), top_p 1 and
+  // penalty 1 at vcl_create.
+  static constexpr int SAMP_BYTES = 28;   // per entry
   unsigned char* samp = nullptr;
   std::vector<unsigned char> samp_host;
   unsigned long long* samp_seed(unsigned char* base) const { return reinterpret_cast<unsigned long long*>(base); }
   float* samp_temp(unsigned char* base) const { return reinterpret_cast<float*>(base + 8 * cfg.max_batch); }
   int* samp_topk(unsigned char* base) const { return reinterpret_cast<int*>(base + 12 * cfg.max_batch); }
   int* samp_topn(unsigned char* base) const { return reinterpret_cast<int*>(base + 16 * cfg.max_batch); }
-  // whether entry first .. first + n - 1 needs the sampler: it samples (a temperature above 0) or wants log-probs
-  bool sampler(int first, int n) {
-    const float* t = samp_temp(samp_host.data());
-    const int* tn = samp_topn(samp_host.data());
-    for (int b = first; b < first + n; ++b)
-      if (t[b] > 0.f || tn[b] >= 0) return true;
-    return false;
+  float* samp_topp(unsigned char* base) const { return reinterpret_cast<float*>(base + 20 * cfg.max_batch); }
+  float* samp_rep(unsigned char* base) const { return reinterpret_cast<float*>(base + 24 * cfg.max_batch); }
+  // what entry b needs: 0 the arg-max, 1 the sampler (it samples, with a temperature above 0, or wants log-probs),
+  // 2 the 32-bit sampler (a repetition penalty, or top-p on a sampled entry)
+  int sampler_of(int b) {
+    unsigned char* hb = samp_host.data();
+    const float T = samp_temp(hb)[b];
+    if (samp_rep(hb)[b] != 1.f || (T > 0.f && samp_topp(hb)[b] < 1.f)) return 2;
+    return T > 0.f || samp_topn(hb)[b] >= 0 ? 1 : 0;
   }
+  // ... and what entries first .. first + n - 1 need together
+  int sampler(int first, int n) {
+    int m = 0;
+    for (int b = first; b < first + n; ++b) m = std::max(m, sampler_of(b));
+    return m;
+  }
+  // The token sets of the repetition penalty (vcl_llm_set_token_set): a bitmap of tset_words() words per entry,
+  // [max_batch][tset_words()], allocated by the first call that turns a penalty on or sets a token set
+  unsigned int* tset = nullptr;
+  int tset_words() const { return (cfg.vocab + 31) / 32; }
   // The log-prob buffer: two planes, int32 ids then f32 log-probs, each [max_batch][lp_rows()][1 + VCL_LOGPROBS_MAX],
   // indexed by entry and the RoPE position of the token (so a read is one contiguous copy per plane); allocated by the
   // first vcl_llm_set_logprobs that turns an entry on.
@@ -415,9 +431,13 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
   rc |= dalloc(h, &h->d_npad, Bm);
   rc |= dalloc(h, &h->amax, (size_t)device_num_sms() * Bm);
   rc |= dalloc(h, &h->d_pack, pack_elems((long long)Ml));
-  rc |= dalloc(h, &h->samp, Bm * 20);
-  h->samp_host.assign(Bm * 20, 0);
-  for (size_t b = 0; b < Bm; ++b) h->samp_topn(h->samp_host.data())[b] = -1;
+  rc |= dalloc(h, &h->samp, Bm * vcl_handle::SAMP_BYTES);
+  h->samp_host.assign(Bm * vcl_handle::SAMP_BYTES, 0);
+  for (size_t b = 0; b < Bm; ++b) {
+    h->samp_topn(h->samp_host.data())[b] = -1;
+    h->samp_topp(h->samp_host.data())[b] = 1.f;
+    h->samp_rep(h->samp_host.data())[b] = 1.f;
+  }
   if (rc == 0) rc = launch_rope_table(h->rope_cos, h->rope_sin, c->max_seq, 128, c->rope_theta, 0);
   if (rc == 0) {
     cudaError_t e = cudaMemset(h->d_npad, 0, Bm * sizeof(int));   // the cache starts unpadded
@@ -710,6 +730,10 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
       sa.lp_entry = (long long)h->lp_rows() * (1 + VCL_LOGPROBS_MAX); sa.lp_pos = 1 + VCL_LOGPROBS_MAX;
       sa.lp_rows = h->lp_rows();
     }
+    if (smp.on == 2) {   // the 32-bit sampler: top_p, the penalties and the token sets
+      sa.top_p = h->samp_topp(h->samp); sa.rep = h->samp_rep(h->samp);
+      sa.tset = h->tset; sa.tset_words = h->tset_words();
+    }
     return launch_sample(sa, st);
   }
   if (tok_out != nullptr) VCL_TRY(launch_argmax(h->logits, tok_out, tok_stride, B, c.vocab, st));
@@ -731,7 +755,7 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
 int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
                 int B, int S, int n_layers, void* hidden_out, float* logits_out, int32_t* next_tok,
                 long long tok_stride, cudaStream_t st, int start_pos = 0, void* states_out = nullptr,
-                const int32_t* n_pad_host = nullptr, int slot = 0, int packed_rows = 0, bool pack_sampled = false,
+                const int32_t* n_pad_host = nullptr, int slot = 0, int packed_rows = 0, int pack_sampled = 0,
                 int pack_attn = 1) {
   const vcl_config& c = h->cfg;
   const bool packed = packed_rows > 0;
@@ -849,7 +873,7 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
   }
   if (logits_out != nullptr || next_tok != nullptr) {
     SampleAt smp;   // clip b (slot `slot` for B = 1) samples with its entry; its token takes column start_pos + S
-    smp.on = next_tok != nullptr && h->sampler(slot, B); smp.entry0 = slot; smp.col = start_pos + S;
+    smp.on = next_tok != nullptr ? h->sampler(slot, B) : 0; smp.entry0 = slot; smp.col = start_pos + S;
     VCL_TRY(lm_head_argmax(h, h->l_h + (size_t)(S - 1) * D, (long long)S * D, B, logits_out, next_tok,
                            tok_stride, st, false, smp));
   }
@@ -979,7 +1003,7 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
 // its embedding row. Step i feeds clip b at position h->d_pos[b] + i - 1.
 // sampled: the sampler writes tk[:, i] from the full logits, and the next step gathers from tk (fused into
 // layer 0 for 1..4 clips, the embedding kernel otherwise).
-int decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, bool sampled) {
+int decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, int sampled) {
   const bool hand_off = B <= 4 && h->cfg.llm_layers > 0 && !sampled;
   for (int i = 1; i < n_new; ++i) {
     StepIo io;
@@ -997,11 +1021,11 @@ int decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, 
   return 0;
 }
 
-// decode_steps from one captured graph per (B, n_new, sampled). The positions (h->d_pos, written by the caller),
+// decode_steps from one captured graph per (B, n_new, sampled), sampled as h->sampler gives it. The positions (h->d_pos, written by the caller),
 // the pad counts (h->d_npad) and the sampling table are read on the device, so new positions, padding or sampling
 // settings replay the same graph. Bounded LRU cache (an entry holds thousands of nodes). A stream that cannot be
 // captured runs the steps eagerly.
-int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, bool sampled) {
+int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, int sampled) {
   GraphEntry* ge = nullptr;
   for (auto& g : h->graphs)
     if (g.B == B && g.n_new == n_new && g.sampled == sampled) ge = &g;
@@ -1184,8 +1208,8 @@ static int packed_prefill(vcl_handle* h, int n, const int32_t* slots_host, const
     }
   }
   VCL_CUDA_OK(cudaMemcpyAsync(h->d_pack, p, map.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-  bool sampled = false;
-  for (int i = 0; i < n; ++i) sampled = sampled || h->sampler(slots_host[i], 1);
+  int sampled = 0;
+  for (int i = 0; i < n; ++i) sampled = std::max(sampled, h->sampler(slots_host[i], 1));
   return llm_prefill(h, ids, video_feats, vid_start, n, S_max, h->cfg.llm_layers, nullptr, nullptr, next_tok, 1, st,
                      0, nullptr, nullptr, 0, (int)M, sampled, pack_attn);
 }
@@ -1334,8 +1358,90 @@ int vcl_llm_set_sampling(vcl_handle* h, int n, const int32_t* clips_host, const 
     h->samp_seed(hb)[b] = seed_host[i];
     h->samp_temp(hb)[b] = temperature_host[i];
     h->samp_topk(hb)[b] = top_k_host[i];
+    h->samp_topp(hb)[b] = 1.f;
+    h->samp_rep(hb)[b] = 1.f;
   }
   VCL_CUDA_OK(cudaMemcpyAsync(h->samp, hb, h->samp_host.size(), cudaMemcpyHostToDevice, as_stream(stream)));
+  return 0;
+}
+
+// the token-set bitmap, all sets empty; the 32-bit sampler graphs captured without it are captured again
+static int ensure_token_sets(vcl_handle* h, cudaStream_t st) {
+  if (h->tset != nullptr) return 0;
+  const size_t words = (size_t)h->cfg.max_batch * h->tset_words();
+  VCL_TRY(dalloc(h, &h->tset, words));
+  VCL_CUDA_OK(cudaMemsetAsync(h->tset, 0, words * 4, st));
+  for (size_t i = h->graphs.size(); i-- > 0;)
+    if (h->graphs[i].sampled == 2) {
+      cudaGraphExecDestroy(h->graphs[i].exec);
+      h->graphs.erase(h->graphs.begin() + i);
+    }
+  return 0;
+}
+
+int vcl_llm_set_sampling_ex(vcl_handle* h, int n, const int32_t* clips_host, const float* temperature_host,
+                            const int32_t* top_k_host, const uint64_t* seed_host, const float* top_p_host,
+                            const float* repetition_penalty_host, void* stream) {
+  VCL_REQUIRE(h != nullptr, "vcl_llm_set_sampling_ex: null handle");
+  const int mb = h->cfg.max_batch;
+  VCL_REQUIRE(n >= 1 && n <= mb, "vcl_llm_set_sampling_ex: n=%d outside 1..%d", n, mb);
+  VCL_REQUIRE(clips_host && temperature_host && top_k_host && seed_host && top_p_host && repetition_penalty_host,
+              "vcl_llm_set_sampling_ex: null argument");
+  bool penalty = false;
+  for (int i = 0; i < n; ++i) {
+    const int b = clips_host[i];
+    const float T = temperature_host[i], p = top_p_host[i], r = repetition_penalty_host[i];
+    VCL_REQUIRE(b >= 0 && b < mb, "vcl_llm_set_sampling_ex: clip %d outside 0..%d", b, mb - 1);
+    for (int j = 0; j < i; ++j)
+      VCL_REQUIRE(clips_host[j] != b, "vcl_llm_set_sampling_ex: clip %d is given twice", b);
+    VCL_REQUIRE(isfinite(T) && T >= 0.f, "vcl_llm_set_sampling_ex: temperature %g of clip %d is not a finite value "
+                ">= 0", (double)T, b);
+    VCL_REQUIRE(top_k_host[i] >= 0, "vcl_llm_set_sampling_ex: top_k %d of clip %d is negative", top_k_host[i], b);
+    VCL_REQUIRE(p >= 0.f && p <= 1.f, "vcl_llm_set_sampling_ex: top_p %g of clip %d outside [0, 1]", (double)p, b);
+    VCL_REQUIRE(isfinite(r) && r > 0.f, "vcl_llm_set_sampling_ex: repetition_penalty %g of clip %d is not a finite "
+                "value > 0", (double)r, b);
+    VCL_REQUIRE((p == 1.f && r == 1.f) || h->cfg.vocab <= VCL_SAMPLE_WIDE_MAX_V,
+                "vcl_llm_set_sampling_ex: clip %d: top_p and repetition_penalty take a vocabulary of at most %d "
+                "tokens (the sampler's shared memory), this model has %d", b, VCL_SAMPLE_WIDE_MAX_V, h->cfg.vocab);
+    penalty = penalty || r != 1.f;
+  }
+  cudaStream_t st = as_stream(stream);
+  if (penalty) VCL_TRY(ensure_token_sets(h, st));
+  unsigned char* hb = h->samp_host.data();
+  for (int i = 0; i < n; ++i) {
+    const int b = clips_host[i];
+    h->samp_seed(hb)[b] = seed_host[i];
+    h->samp_temp(hb)[b] = temperature_host[i];
+    h->samp_topk(hb)[b] = top_k_host[i];
+    h->samp_topp(hb)[b] = top_p_host[i];
+    h->samp_rep(hb)[b] = repetition_penalty_host[i];
+  }
+  VCL_CUDA_OK(cudaMemcpyAsync(h->samp, hb, h->samp_host.size(), cudaMemcpyHostToDevice, st));
+  return 0;
+}
+
+int vcl_llm_set_token_set(vcl_handle* h, int entry, const int64_t* ids, int n, void* stream) {
+  VCL_REQUIRE(h != nullptr, "vcl_llm_set_token_set: null handle");
+  VCL_REQUIRE(entry >= 0 && entry < h->cfg.max_batch, "vcl_llm_set_token_set: entry %d outside 0..%d", entry,
+              h->cfg.max_batch - 1);
+  VCL_REQUIRE(n >= 0 && (n == 0 || ids != nullptr), "vcl_llm_set_token_set: n=%d with %s ids", n,
+              ids ? "given" : "null");
+  VCL_REQUIRE(h->cfg.vocab <= VCL_SAMPLE_WIDE_MAX_V, "vcl_llm_set_token_set: the repetition penalty takes a "
+              "vocabulary of at most %d tokens, this model has %d", VCL_SAMPLE_WIDE_MAX_V, h->cfg.vocab);
+  cudaStream_t st = as_stream(stream);
+  VCL_TRY(ensure_token_sets(h, st));
+  return launch_token_set(h->tset + (size_t)entry * h->tset_words(), h->tset_words(),
+                          reinterpret_cast<const long long*>(ids), n, h->cfg.vocab, st);
+}
+
+int vcl_llm_read_token_set(vcl_handle* h, int entry, uint32_t* bits_out, void* stream) {
+  VCL_REQUIRE(h && bits_out, "vcl_llm_read_token_set: null argument");
+  VCL_REQUIRE(entry >= 0 && entry < h->cfg.max_batch, "vcl_llm_read_token_set: entry %d outside 0..%d", entry,
+              h->cfg.max_batch - 1);
+  VCL_REQUIRE(h->tset != nullptr, "vcl_llm_read_token_set: no token set was ever set for this handle "
+              "(vcl_llm_set_token_set, or a repetition penalty in vcl_llm_set_sampling_ex)");
+  VCL_CUDA_OK(cudaMemcpyAsync(bits_out, h->tset + (size_t)entry * h->tset_words(), (size_t)h->tset_words() * 4,
+                              cudaMemcpyDefault, as_stream(stream)));
   return 0;
 }
 
@@ -1526,14 +1632,27 @@ int vcl_op_cross_entropy(const void* logits, int64_t ld, const int64_t* labels, 
 
 namespace {
 
-// vcl_op_sample / vcl_op_sample_logprobs: top_n_host null, or log-prob rows [B][1 + VCL_LOGPROBS_MAX] to ids_out / lp_out
+// vcl_op_sample / vcl_op_sample_logprobs / vcl_op_sample_ex: top_n_host null, or log-prob rows
+// [B][1 + VCL_LOGPROBS_MAX] to ids_out / lp_out; top_p_host null (the 16-bit sampler), or the 32-bit sampler with
+// top_p_host, rep_host and the token sets tset [B][ceil(V / 32)] (device, may be null)
 int op_sample(const char* name, const float* logits, int64_t ld, int B, int V, const float* temperature_host,
               const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
-              const int32_t* top_n_host, int32_t* tok_out, int32_t* ids_out, float* lp_out, void* stream) {
+              const int32_t* top_n_host, int32_t* tok_out, int32_t* ids_out, float* lp_out, void* stream,
+              const float* top_p_host = nullptr, const float* rep_host = nullptr, uint32_t* tset = nullptr) {
   if (check_device() != 0) return -2;
   VCL_REQUIRE(logits && temperature_host && top_k_host && seed_host && counter_host && tok_out, "%s: null argument",
               name);
   VCL_REQUIRE(B >= 1, "%s: B=%d", name, B);
+  const bool wide = top_p_host != nullptr;
+  if (wide) {
+    VCL_REQUIRE(rep_host != nullptr, "%s: null argument", name);
+    VCL_REQUIRE(V >= 1 && V <= VCL_SAMPLE_WIDE_MAX_V, "%s: V=%d outside 1..%d (the 32-bit sampler's shared memory)",
+                name, V, VCL_SAMPLE_WIDE_MAX_V);
+    for (int b = 0; b < B; ++b)
+      VCL_REQUIRE(top_p_host[b] >= 0.f && top_p_host[b] <= 1.f && isfinite(rep_host[b]) && rep_host[b] > 0.f,
+                  "%s: row %d: top_p %g outside [0, 1] or repetition_penalty %g not a finite value > 0", name, b,
+                  (double)top_p_host[b], (double)rep_host[b]);
+  }
   for (int b = 0; b < B; ++b)
     VCL_REQUIRE(isfinite(temperature_host[b]) && temperature_host[b] >= 0.f && top_k_host[b] >= 0 &&
                 counter_host[b] >= 0, "%s: row %d: temperature %g, top_k %d, counter %d", name, b,
@@ -1542,13 +1661,17 @@ int op_sample(const char* name, const float* logits, int64_t ld, int B, int V, c
     for (int b = 0; b < B; ++b)
       VCL_REQUIRE(top_n_host[b] >= -1 && top_n_host[b] <= VCL_LOGPROBS_MAX, "%s: row %d: top_n %d outside -1..%d",
                   name, b, top_n_host[b], VCL_LOGPROBS_MAX);
-  // the per-row settings in one stream-ordered block: [B] seeds, temperatures, top_k, counters, top_n
-  std::vector<unsigned char> hb((size_t)B * 24);
+  // the per-row settings in one stream-ordered block: [B] seeds, temperatures, top_k, counters, top_n, top_p, penalties
+  std::vector<unsigned char> hb((size_t)B * (wide ? 32 : 24));
   memcpy(hb.data(), seed_host, (size_t)B * 8);
   memcpy(hb.data() + (size_t)B * 8, temperature_host, (size_t)B * 4);
   memcpy(hb.data() + (size_t)B * 12, top_k_host, (size_t)B * 4);
   memcpy(hb.data() + (size_t)B * 16, counter_host, (size_t)B * 4);
   if (top_n_host != nullptr) memcpy(hb.data() + (size_t)B * 20, top_n_host, (size_t)B * 4);
+  if (wide) {
+    memcpy(hb.data() + (size_t)B * 24, top_p_host, (size_t)B * 4);
+    memcpy(hb.data() + (size_t)B * 28, rep_host, (size_t)B * 4);
+  }
   cudaStream_t st = as_stream(stream);
   unsigned char* d = nullptr;
   VCL_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&d), hb.size(), st));
@@ -1563,6 +1686,11 @@ int op_sample(const char* name, const float* logits, int64_t ld, int B, int V, c
   if (top_n_host != nullptr) {   // row b's places at ids_out / lp_out + b * (1 + VCL_LOGPROBS_MAX), any counter
     sa.top_n = reinterpret_cast<const int*>(d + (size_t)B * 20);
     sa.lp_id = ids_out; sa.lp_val = lp_out; sa.lp_entry = 1 + VCL_LOGPROBS_MAX; sa.lp_pos = 0; sa.lp_rows = 0x7fffffff;
+  }
+  if (wide) {
+    sa.top_p = reinterpret_cast<const float*>(d + (size_t)B * 24);
+    sa.rep = reinterpret_cast<const float*>(d + (size_t)B * 28);
+    sa.tset = tset; sa.tset_words = (V + 31) / 32;
   }
   const int rc = launch_sample(sa, st);
   VCL_CUDA_OK(cudaFreeAsync(d, st));
@@ -1587,6 +1715,16 @@ int vcl_op_sample_logprobs(const float* logits, int64_t ld, int B, int V, const 
   VCL_REQUIRE(top_n_host && ids_out && lp_out, "vcl_op_sample_logprobs: null argument");
   return op_sample("vcl_op_sample_logprobs", logits, ld, B, V, temperature_host, top_k_host, seed_host, counter_host,
                    top_n_host, tok_out, ids_out, lp_out, stream);
+}
+
+int vcl_op_sample_ex(const float* logits, int64_t ld, int B, int V, const float* temperature_host,
+                     const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
+                     const float* top_p_host, const float* repetition_penalty_host, uint32_t* token_sets,
+                     const int32_t* top_n_host, int32_t* tok_out, int32_t* ids_out, float* lp_out, void* stream) {
+  VCL_REQUIRE(top_p_host && repetition_penalty_host, "vcl_op_sample_ex: null argument");
+  VCL_REQUIRE(top_n_host == nullptr || (ids_out && lp_out), "vcl_op_sample_ex: log-probs need ids_out and lp_out");
+  return op_sample("vcl_op_sample_ex", logits, ld, B, V, temperature_host, top_k_host, seed_host, counter_host,
+                   top_n_host, tok_out, ids_out, lp_out, stream, top_p_host, repetition_penalty_host, token_sets);
 }
 
 int vcl_op_layernorm(const void* x, void* y, const void* w, const void* b, int rows, int D, float eps,

@@ -134,6 +134,10 @@ _SIGNATURES = {
     "vcl_llm_slot_decode": (c_int, [c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_void_p, c_void_p]),
     "vcl_llm_set_sampling": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_float), POINTER(c_int32),
                                      POINTER(c_uint64), c_void_p]),
+    "vcl_llm_set_sampling_ex": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_float), POINTER(c_int32),
+                                        POINTER(c_uint64), POINTER(c_float), POINTER(c_float), c_void_p]),
+    "vcl_llm_set_token_set": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),
+    "vcl_llm_read_token_set": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "vcl_llm_set_logprobs": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), c_void_p]),
     "vcl_llm_read_logprobs": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_launch_count": (ctypes.c_longlong, []),
@@ -152,6 +156,9 @@ _SIGNATURES = {
     "vcl_op_sample_logprobs": (c_int, [c_void_p, c_int64, c_int, c_int, POINTER(c_float), POINTER(c_int32),
                                        POINTER(c_uint64), POINTER(c_int32), POINTER(c_int32), c_void_p, c_void_p,
                                        c_void_p, c_void_p]),
+    "vcl_op_sample_ex": (c_int, [c_void_p, c_int64, c_int, c_int, POINTER(c_float), POINTER(c_int32), POINTER(c_uint64),
+                                 POINTER(c_int32), POINTER(c_float), POINTER(c_float), c_void_p, POINTER(c_int32),
+                                 c_void_p, c_void_p, c_void_p, c_void_p]),
     "vcl_op_layernorm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "vcl_op_rmsnorm": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "vcl_op_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
@@ -319,6 +326,43 @@ def op_sample_logprobs(logits, temperature, top_k, seed, counter, top_n):
                                        (c_float * B)(*[float(t) for t in vals[0]]), ints(vals[1]), _seeds(seed, B),
                                        ints(vals[2]), ints(vals[3]), ptr(out), ptr(ids), ptr(lp), cur_stream()))
     return out, ids, lp
+
+
+SAMPLE_WIDE_MAX_V = 57344     # include/vcl.h: VCL_SAMPLE_WIDE_MAX_V, the vocabulary limit of top_p / repetition_penalty
+
+
+def token_set_words(V):
+    """int32 words of one token-set bitmap over a vocabulary of V tokens"""
+    return (V + 31) // 32
+
+
+def op_sample_ex(logits, temperature, top_k, seed, counter, top_p, repetition_penalty, token_sets=None, top_n=None):
+    """The 32-bit sampler alone (vcl_op_sample_ex): op_sample's arguments plus top_p and repetition_penalty (B host
+    values each), token_sets (None, or [B, token_set_words(V)] int32 on the device; each row's picked token is added
+    to it) and top_n (None, or B host ints as in op_sample_logprobs). Returns tokens [B] int32, or (tokens, ids, lp)
+    with top_n."""
+    B, ld = logits.shape
+    assert logits.dtype == torch.float32 and logits.stride(1) == 1
+    vals = [list(v) for v in (temperature, top_k, counter, top_p, repetition_penalty)]
+    if top_n is not None:
+        vals.append(list(top_n))
+    if not all(len(v) == B for v in vals):
+        raise VclError(f"temperature / top_k / counter / top_p / repetition_penalty (/ top_n) need {B} entries each")
+    if token_sets is not None:
+        assert token_sets.is_cuda and token_sets.dtype == torch.int32 and token_sets.is_contiguous()
+        assert tuple(token_sets.shape) == (B, token_set_words(ld))
+    out = torch.empty(B, dtype=torch.int32, device=logits.device)
+    ids = lp = None
+    if top_n is not None:
+        ids = torch.full((B, LOGPROB_PLACES), -1, dtype=torch.int32, device=logits.device)
+        lp = torch.full((B, LOGPROB_PLACES), float("nan"), dtype=torch.float32, device=logits.device)
+    ints = lambda v: (c_int32 * B)(*[int(x) for x in v])   # noqa: E731
+    flts = lambda v: (c_float * B)(*[float(x) for x in v])   # noqa: E731
+    check(lib().vcl_op_sample_ex(c_void_p(logits.data_ptr()), logits.stride(0), B, ld, flts(vals[0]), ints(vals[1]),
+                                 _seeds(seed, B), ints(vals[2]), flts(vals[3]), flts(vals[4]), ptr(token_sets),
+                                 ints(vals[5]) if top_n is not None else None, ptr(out), ptr(ids), ptr(lp),
+                                 cur_stream()))
+    return out if top_n is None else (out, ids, lp)
 
 
 def op_gemv(x, w, res=None, norm_w=None, eps=0.0):
@@ -606,6 +650,33 @@ class Engine:
         check(lib().vcl_llm_set_sampling(self._h, n, (c_int32 * n)(*[int(b) for b in clips]),
                                          (c_float * n)(*[float(t) for t in temperature]),
                                          (c_int32 * n)(*[int(k) for k in top_k]), _seeds(seed, n), cur_stream()))
+
+    def set_sampling_ex(self, clips, temperature, top_k, seed, top_p, repetition_penalty):
+        """set_sampling plus top_p[i] (0 .. 1, 1: off) and repetition_penalty[i] (> 0, 1: off) per entry
+        (vcl_llm_set_sampling_ex). Host lists of equal length."""
+        n = len(clips)
+        if not (len(temperature) == len(top_k) == len(top_p) == len(repetition_penalty) == n):
+            raise VclError(f"{n} clips, {len(temperature)} temperatures, {len(top_k)} top_k, {len(top_p)} top_p, "
+                           f"{len(repetition_penalty)} repetition_penalty")
+        flts = lambda v: (c_float * n)(*[float(x) for x in v])   # noqa: E731
+        check(lib().vcl_llm_set_sampling_ex(self._h, n, (c_int32 * n)(*[int(b) for b in clips]), flts(temperature),
+                                            (c_int32 * n)(*[int(k) for k in top_k]), _seeds(seed, n), flts(top_p),
+                                            flts(repetition_penalty), cur_stream()))
+
+    def set_token_set(self, entry, ids):
+        """Entry `entry`'s token set of the repetition penalty becomes the ids of `ids` (any int tensor or list;
+        vcl_llm_set_token_set)"""
+        t = torch.as_tensor(ids).reshape(-1).to(device="cuda", dtype=torch.int64).contiguous()
+        check(lib().vcl_llm_set_token_set(self._h, int(entry), ptr(t) if t.numel() else None, t.numel(), cur_stream()))
+
+    def read_token_set(self, entry):
+        """Entry `entry`'s token set (vcl_llm_read_token_set) as a sorted int64 tensor of token ids on the host"""
+        words = token_set_words(self.cfg.vocab)
+        bits = torch.empty(words, dtype=torch.int32, device="cuda")
+        check(lib().vcl_llm_read_token_set(self._h, int(entry), c_void_p(bits.data_ptr()), cur_stream()))
+        b = bits.cpu().to(torch.int64) & 0xFFFFFFFF
+        on = ((b[:, None] >> torch.arange(32)) & 1).reshape(-1)
+        return on.nonzero()[:, 0]
 
     # ---- log-probs of generated tokens ----
     sample_logprobs_op = staticmethod(op_sample_logprobs)

@@ -66,13 +66,16 @@ class VideoFeatureCache:
 
 def video_chatgpt_infer(video_frames, question, conv_mode, model, vision_tower, tokenizer, image_processor,
                         video_token_len, transcript=None, do_sample=True, temperature=0.2, max_new_tokens=1024,
-                        video_key=None, feature_cache: "VideoFeatureCache | None" = None, seed=None):
+                        video_key=None, feature_cache: "VideoFeatureCache | None" = None, seed=None, top_p=1.0,
+                        repetition_penalty=1.0):
     """Same flow as the reference: prompt -> tokenizer -> image processor -> tower -> pool -> generate
     -> decode. `do_sample/temperature/max_new_tokens` default to the reference's hard-coded values.
     Extension (off by default): with `video_key` and a `VideoFeatureCache`, the pooled features of a
     video are computed once and reused on later turns.
     seed (off by default): with do_sample, the tokens are sampled on the device (generate(seed=...)), reproducible
-    from the seed; without one, generate samples step by step from torch's RNG as before."""
+    from the seed; without one, generate samples step by step from torch's RNG as before.
+    top_p / repetition_penalty (off by default, 1.0): HF's nucleus sampling and repetition penalty, passed to
+    generate."""
     if model.get_model().vision_config.use_vid_start_end:
         qs = question + "\n" + DEFAULT_VID_START_TOKEN + DEFAULT_VIDEO_PATCH_TOKEN * video_token_len + DEFAULT_VID_END_TOKEN
     else:
@@ -106,7 +109,8 @@ def video_chatgpt_infer(video_frames, question, conv_mode, model, vision_tower, 
         output_ids = model.generate(input_ids, video_spatio_temporal_features=feats.unsqueeze(0),
                                     do_sample=do_sample, temperature=temperature, max_new_tokens=max_new_tokens,
                                     stopping_criteria=[stopping], eos_token_id=eos if eos is not None else "config",
-                                    pad_token_id=getattr(tokenizer, "pad_token_id", None), seed=seed)
+                                    pad_token_id=getattr(tokenizer, "pad_token_id", None), seed=seed, top_p=top_p,
+                                    repetition_penalty=repetition_penalty)
     n_diff = (input_ids != output_ids[:, :input_ids.shape[1]]).sum().item()
     if n_diff > 0:
         print(f"[Warning] {n_diff} output_ids are not the same as the input_ids")

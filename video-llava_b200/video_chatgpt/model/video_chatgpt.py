@@ -592,15 +592,46 @@ class VideoChatGPTLlamaForCausalLM:
             raise ValueError(f"{what}: seed {seed!r} must be an int")
         return t, k, None if seed is None else seed % 2 ** 64
 
+    def _nucleus_args(self, top_p, repetition_penalty, what="generate", sampled=True, device=True):
+        """Checks top_p and repetition_penalty on the host -> (top_p, repetition_penalty) as floats; 1.0 is off. The
+        device sampler's vocabulary limit applies when the call runs there (`device`) and turns a setting on: the
+        penalty, or top_p on a `sampled` call (a greedy one ignores top_p, as HF does)."""
+        p, r = float(top_p), float(repetition_penalty)
+        if not 0.0 <= p <= 1.0:
+            raise ValueError(f"{what}: top_p {top_p} must lie in [0, 1] (1: off)")
+        if not math.isfinite(r) or r <= 0:
+            raise ValueError(f"{what}: repetition_penalty {repetition_penalty} must be a finite value > 0 (1: off)")
+        V = self.config.vocab_size
+        if device and (r != 1.0 or (sampled and p != 1.0)) and V > vn.SAMPLE_WIDE_MAX_V:
+            raise ValueError(f"{what}: top_p and repetition_penalty take a vocabulary of at most {vn.SAMPLE_WIDE_MAX_V} "
+                             f"tokens on the device sampler, this model has {V}")
+        return p, r
+
+    @staticmethod
+    def _set_entries(eng, clips, temperature, top_k, seeds, top_p, penalty):
+        """One sampling-table write: set_sampling when every entry has top_p 1 and penalty 1 (what a call without
+        them always made), set_sampling_ex otherwise"""
+        if all(p == 1.0 for p in top_p) and all(r == 1.0 for r in penalty):
+            eng.set_sampling(clips, temperature, top_k, seeds)
+        else:
+            eng.set_sampling_ex(clips, temperature, top_k, seeds, top_p, penalty)
+
     @contextlib.contextmanager
-    def _sampling(self, eng, clips, temperature, top_k, seeds):
-        """Entries `clips` of the engine's sampling table sample for the duration of the block and are greedy
-        again afterwards, also when the block raises."""
-        eng.set_sampling(clips, temperature, top_k, seeds)
+    def _sampling(self, eng, clips, temperature, top_k, seeds, top_p=1.0, penalty=1.0):
+        """Entries `clips` of the engine's sampling table sample (temperature 0: greedy, with the penalty) for the
+        duration of the block and are greedy, without top-p or penalty, again afterwards, also when the block raises."""
+        n = len(clips)
+        self._set_entries(eng, clips, temperature, top_k, seeds, [top_p] * n, [penalty] * n)
         try:
             yield
         finally:
-            eng.set_sampling(clips, [0.0] * len(clips), [0] * len(clips), [0] * len(clips))
+            eng.set_sampling(clips, [0.0] * n, [0] * n, [0] * n)
+
+    @staticmethod
+    def _token_sets(eng, rows):
+        """(entry, ids) pairs: each entry's token set of the repetition penalty becomes its ids, one call each"""
+        for b, ids in rows:
+            eng.set_token_set(b, ids)
 
     @staticmethod
     def _logprobs_arg(v, what):
@@ -651,7 +682,7 @@ class VideoChatGPTLlamaForCausalLM:
     @torch.no_grad()
     def generate(self, input_ids, video_spatio_temporal_features=None, do_sample=False, temperature=1.0,
                  max_new_tokens=32, stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50,
-                 attention_mask=None, seed=None, logprobs=None, **kw):
+                 attention_mask=None, seed=None, logprobs=None, top_p=1.0, repetition_penalty=1.0, **kw):
         """Returns [B, S+n] int64 INCLUDING the prompt, like HF generate (inference.py:105-120), and
         like HF it stops at EOS (config.eos_token_id unless eos_token_id is given; None disables it):
         finished rows are padded, the call returns when every row has finished.
@@ -672,12 +703,19 @@ class VideoChatGPTLlamaForCausalLM:
         token_logprobs f32 [n_new], and the `logprobs` most likely tokens of each step, top_ids int64 [n_new, k] and
         top_logprobs f32 [n_new, k]; positions after a row's EOS hold NaN / -1. They are computed on the device next
         to the token, so greedy calls take the device loops (the seeded path's, with greedy entries) and return the
-        same tokens; unseeded sampling cannot report them (NotImplementedError: pass seed=)."""
+        same tokens; unseeded sampling cannot report them (NotImplementedError: pass seed=).
+        top_p (1.0: off) and repetition_penalty (1.0: off): HF's TopPLogitsWarper and RepetitionPenaltyLogitsProcessor,
+        in HF's order (penalty, temperature, top-k, top-p; DESIGN.md section 3). The penalty divides (multiplies, when
+        negative) the logits of every token of the row's input_ids so far (prompt, padding, new tokens); top-p only
+        applies when sampling. Seeded sampling applies both on the device; a greedy call with a penalty takes the
+        device loops with greedy entries; unseeded sampling applies them on the host, step by step, as HF does."""
         self._not_paged("generate")
         lp_n = self._logprobs_arg(logprobs, "generate")
         if lp_n is not None and do_sample and seed is None:
             raise NotImplementedError("generate: logprobs are computed by the device sampler, and sampling there needs "
                                       "seed= (unseeded do_sample=True draws from torch's RNG on the host)")
+        top_p, penalty = self._nucleus_args(top_p, repetition_penalty, "generate", do_sample,
+                                            device=not do_sample or seed is not None)
         seeded = do_sample and seed is not None
         if seeded:
             temperature, top_k, seed = self._sampling_args(temperature, top_k, seed)
@@ -695,10 +733,17 @@ class VideoChatGPTLlamaForCausalLM:
             raise ValueError(f"prompt length {S} leaves no room in max_seq {self._max_seq}")
         eos, pad = self._eos_pad(eos_token_id, pad_token_id)
         self._pads = pads
-        if seeded or lp_n is not None:
+        if seeded or lp_n is not None or (penalty != 1.0 and not do_sample):
             clips = list(range(B))
-            samp = (self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips]) if seeded
-                    else contextlib.nullcontext())
+            if seeded:
+                samp = self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips], top_p,
+                                      penalty)
+            elif penalty != 1.0:   # greedy entries with the penalty
+                samp = self._sampling(eng, clips, [0.0] * B, [0] * B, [0] * B, 1.0, penalty)
+            else:
+                samp = contextlib.nullcontext()
+            if penalty != 1.0:
+                self._token_sets(eng, [(b, ids[b]) for b in clips])
             with samp, self._logprobs(eng, clips, lp_n):
                 if eos is None and not stopping_criteria:
                     new = eng.generate(ids, feats, vs, n, n_pad=pads)
@@ -715,7 +760,7 @@ class VideoChatGPTLlamaForCausalLM:
             _, logits, _ = eng.prefill(ids, feats, vs, want_logits=True, want_token=False, n_pad=pads)
             self._pos = S
             self._last_out = self._stepwise(eng, ids, logits, n, do_sample, temperature, stopping_criteria, eos, pad,
-                                            top_k)
+                                            top_k, top_p, penalty)
             return self._last_out
         if eos is None:
             new = eng.generate(ids, feats, vs, n, n_pad=pads).to(torch.int64)
@@ -801,7 +846,7 @@ class VideoChatGPTLlamaForCausalLM:
     @torch.no_grad()
     def generate_requests(self, requests, max_new_tokens=32, eos_token_id="config", stopping_criteria=None,
                           slots=None, do_sample=False, packed_admission=False, temperature=1.0, top_k=50, seed=None,
-                          chunked_prefill=False, logprobs=None):
+                          chunked_prefill=False, logprobs=None, top_p=1.0, repetition_penalty=1.0):
         """Greedy generation for many independent requests by in-flight (continuous) batching: every request
         owns a slot of the KV cache while it runs, and a finished request's slot takes the next queued one at
         once while the other slots keep decoding (a static batch decodes until its longest row finishes).
@@ -854,7 +899,13 @@ class VideoChatGPTLlamaForCausalLM:
         log-probabilities as generate(logprobs=...) reports them, for its new tokens only (a continuation: this
         turn's), or None when the request did not ask. Each admission writes the admitted slots' log-prob entries
         (a slot without a request is off), and each decode chunk's rows come back in one copy; the values do not
-        depend on slot, neighbours, queue order, admission mode, paging or preemption."""
+        depend on slot, neighbours, queue order, admission mode, paging or preemption.
+        top_p / repetition_penalty (1.0: off), or a request's own "top_p" / "repetition_penalty" keys: as in generate,
+        on the device. top_p applies to sampled requests; the penalty to greedy and sampled ones, over the request's own
+        prompt (a continuation: the whole conversation) and its new tokens. The slot's token set is written when the
+        request is admitted (before each chunk of a chunked prompt) and rebuilt from the prompt and the tokens the host
+        holds when it resumes after a preemption; nothing carries over from the slot's earlier requests. Requests
+        without either setting write the sampling table with set_sampling and launch what they launched before."""
         self._logprobs_arg(logprobs, "generate_requests")
         for i, r in enumerate(requests):
             r = r if isinstance(r, dict) else {}
@@ -865,6 +916,8 @@ class VideoChatGPTLlamaForCausalLM:
             if r.get("do_sample", do_sample) and r.get("seed", seed) is None:
                 raise NotImplementedError(f"request {i}: generate_requests decodes greedily unless given a seed; "
                                           "sampling in flight needs seed= (the call's or the request's own)")
+            self._nucleus_args(r.get("top_p", top_p), r.get("repetition_penalty", repetition_penalty), f"request {i}",
+                               r.get("do_sample", do_sample))
         cap = self._n_slots
         n_slots = cap if slots is None else int(slots)
         if not 1 <= n_slots <= cap:
@@ -872,12 +925,13 @@ class VideoChatGPTLlamaForCausalLM:
                 raise ValueError(f"slots={slots} outside 1..{cap} (max_slots {self._max_slots})")
             raise ValueError(f"slots={slots} outside 1..{cap} (at most 16 and at most max_batch {self._max_batch})")
         eng = self._ensure_engine(need_llm=True)
-        samp = dict(do_sample=do_sample, temperature=temperature, top_k=top_k, seed=seed, logprobs=logprobs)
+        samp = dict(do_sample=do_sample, temperature=temperature, top_k=top_k, seed=seed, logprobs=logprobs, top_p=top_p,
+                    repetition_penalty=repetition_penalty)
         reqs = [self._request(i, r, max_new_tokens, stopping_criteria, eng.NV, samp) for i, r in enumerate(requests)]
         if self._kv_blocks:
             self._bind_sessions(reqs)
             self._check_paged(reqs, chunked_prefill)
-        sampling = any(r.temperature > 0 for r in reqs)
+        sampling = any(r.temperature > 0 or r.penalty != 1.0 for r in reqs)
         eos, _ = self._eos_pad(eos_token_id, None)
         self._last_out, self._pos, self.last_logprobs = None, 0, None
         n_slots = min(n_slots, len(reqs))
@@ -915,9 +969,7 @@ class VideoChatGPTLlamaForCausalLM:
                     admitted.append((s, i))
                     owner[s], pos[s], unseen[s], gen[i] = i, reqs[i].S, True, []
             if admitted and sampling:
-                rs = [reqs[i] for _, i in admitted]
-                eng.set_sampling([s for s, _ in admitted], [r.temperature for r in rs], [r.top_k for r in rs],
-                                 [r.seed for r in rs])
+                self._admit_sampling(eng, [(s, reqs[i]) for s, i in admitted])
             lps.sync(owner)
             if admitted and packed_admission:
                 self._admit_packed(eng, [(s, reqs[i]) for s, i in admitted], first)
@@ -949,6 +1001,17 @@ class VideoChatGPTLlamaForCausalLM:
                 unseen[s] = False
             lps.collect([(s, i, len(gen[i])) for s, i in running])
 
+    def _admit_sampling(self, eng, group, resumed=()):
+        """The sampling-table entries of the (slot, request) pairs admitted at one point, in one write, and the token
+        set of each penalized one: its ids; for a (slot, request, tokens) of `resumed`, its ids then those tokens."""
+        rows = list(group) + [(s, r) for s, r, _ in resumed]
+        self._set_entries(eng, [s for s, _ in rows], [r.temperature for _, r in rows], [r.top_k for _, r in rows],
+                          [r.seed for _, r in rows], [r.top_p for _, r in rows], [r.penalty for _, r in rows])
+        sets = [(s, r.ids) for s, r in group if r.penalty != 1.0]
+        sets += [(s, torch.cat([r.ids, torch.tensor(toks, dtype=torch.int64)])) for s, r, toks in resumed
+                 if r.penalty != 1.0]
+        self._token_sets(eng, sets)
+
     def _admit_packed(self, eng, group, first):
         """Prefill the (slot, request) pairs of one admission point: prompts longer than _PACKED_MAX_S one at a time
         (slot_prefill), all others in one slots_prefill. Each slot's first token goes to first[slot]. The packed
@@ -970,18 +1033,21 @@ class VideoChatGPTLlamaForCausalLM:
                                     [r.vid_start for _, r in packed])
             first[torch.tensor(slots, device=dev)] = tok
 
-    def _prefill_chunked(self, eng, group, first, packed):
+    def _prefill_chunked(self, eng, group, first, packed, sampling=False):
         """Prefill the (slot, request) pairs of one admission point whose prompts are longer than _PACKED_MAX_S on a
         paged engine: each prompt runs as consecutive chunks of _PACKED_MAX_S rows (Engine.slots_prefill_chunk),
         every chunk attending the columns its earlier chunks left in the slot's blocks. packed: chunk k of every
         prompt of the group goes into one call (at most n_slots * 512 rows, which the activations hold); otherwise
         each prompt runs alone. A slot's first token (first[slot]) is the one its last chunk gives. Returns the
-        number of chunk calls."""
+        number of chunk calls. Every chunk call also draws a token for each of its prompts (only the last one's is
+        kept), which a penalized slot adds to its token set: so the set is written again before each later call."""
         dev, L = first.device, self._PACKED_MAX_S
         calls = 0
         for batch in ([group] if packed else [[g] for g in group]):
             for start in range(0, max(r.S for _, r in batch), L):
                 live = [(s, r) for s, r in batch if start < r.S]
+                if sampling and start > 0:   # (chunk 0 follows the admission's write)
+                    self._token_sets(eng, [(s, r.ids) for s, r in live if r.penalty != 1.0])
                 tok = eng.slots_prefill_chunk([s for s, _ in live], [start] * len(live), [r.S for _, r in live],
                                               [r.ids[start:start + L] for _, r in live],
                                               [None if r.feats is None else r.feats.to(dev) for _, r in live],
@@ -1157,9 +1223,10 @@ class VideoChatGPTLlamaForCausalLM:
             if admitted or resumed or tails:
                 eng.set_block_table(table)
             if sampling and (admitted or resumed or tails):
-                rs = [(s, reqs[i]) for s, i in admitted + resumed + tails]
-                eng.set_sampling([s for s, _ in rs], [r.temperature for _, r in rs], [r.top_k for _, r in rs],
-                                 [r.seed for _, r in rs])
+                # a resumed request's token set: its prompt and its tokens, the pending one too when the host has
+                # not seen it yet (its prefill's token)
+                self._admit_sampling(eng, [(s, reqs[i]) for s, i in admitted + tails],
+                                     [(s, reqs[i], gen[i] + ([int(first[s])] if unseen[s] else [])) for s, i in resumed])
             lps.sync(owner)
             # continuations: the tails admitted here in one call under packed_admission, one call each otherwise
             for group in ([tails] if packed_admission and tails else [[t] for t in tails]):
@@ -1171,7 +1238,7 @@ class VideoChatGPTLlamaForCausalLM:
                 admitted = [(s, i) for s, i in admitted if reqs[i].S <= self._PACKED_MAX_S]
                 if long:
                     stats["chunked_prefills"] += len(long)
-                    stats["chunk_calls"] += self._prefill_chunked(eng, long, first, packed_admission)
+                    stats["chunk_calls"] += self._prefill_chunked(eng, long, first, packed_admission, sampling)
             if admitted and packed_admission:
                 self._admit_packed(eng, [(s, reqs[i]) for s, i in admitted], first)
             elif admitted:
@@ -1253,6 +1320,9 @@ class VideoChatGPTLlamaForCausalLM:
         crit = r.get("stopping_criteria", stopping_criteria)
         samp = samp or dict(do_sample=False, temperature=1.0, top_k=50, seed=None)
         T, k, seed = 0.0, 0, 0
+        top_p, penalty = self._nucleus_args(r.get("top_p", samp.get("top_p", 1.0)),
+                                            r.get("repetition_penalty", samp.get("repetition_penalty", 1.0)),
+                                            f"request {i}", r.get("do_sample", samp["do_sample"]))
         if r.get("do_sample", samp["do_sample"]):
             own = r.get("seed") is not None       # a seed is there (generate_requests checks it first)
             T, k, seed = self._sampling_args(r.get("temperature", samp["temperature"]), r.get("top_k", samp["top_k"]),
@@ -1260,8 +1330,10 @@ class VideoChatGPTLlamaForCausalLM:
             seed = seed if own else (seed + i) % 2 ** 64
             if T == 0:
                 k, seed = 0, 0
+        if T == 0:
+            top_p = 1.0                           # HF adds no warpers when greedy
         return SimpleNamespace(ids=ids, S=S, n=n, feats=feats, vid_start=vs, criteria=list(crit or []),
-                               temperature=T, top_k=k, seed=seed, session=r.get("session"),
+                               temperature=T, top_k=k, seed=seed, top_p=top_p, penalty=penalty, session=r.get("session"),
                                continues=r.get("continues"), start=0, lp=r.get("logprobs", samp.get("logprobs")))
 
     def _bind_sessions(self, reqs):
@@ -1329,7 +1401,7 @@ class VideoChatGPTLlamaForCausalLM:
 
     def generate_continue(self, new_input_ids, do_sample=False, temperature=1.0, max_new_tokens=32,
                           stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50, seed=None,
-                          logprobs=None):
+                          logprobs=None, top_p=1.0, repetition_penalty=1.0):
         """Next turn about the SAME video(s): `new_input_ids` [B, S_new] follow everything generated
         so far. Only the tokens the KV cache does not hold yet (the last generated token and the new
         text) are prefilled (vcl_llm_prefill_append); the reference re-runs the tower and the whole
@@ -1337,7 +1409,8 @@ class VideoChatGPTLlamaForCausalLM:
         After a left-padded generate the cache stays padded, so every row continues its own positions; the
         new text of every row has the same length S_new (no padding inside a turn).
         seed: do_sample=True samples on the device as generate(seed=...) does. logprobs: as in generate, for the new
-        tokens of this turn."""
+        tokens of this turn. top_p / repetition_penalty: as in generate; the penalty's tokens are the whole
+        conversation (every earlier turn, its answers as returned, and the new text)."""
         self._not_paged("generate_continue")
         if getattr(self, "_last_out", None) is None:
             raise ValueError("generate_continue: no previous generate() to continue")
@@ -1346,6 +1419,8 @@ class VideoChatGPTLlamaForCausalLM:
             raise NotImplementedError("generate_continue: logprobs are computed by the device sampler, and sampling "
                                       "there needs seed= (unseeded do_sample=True draws from torch's RNG on the host)")
         self.last_logprobs = None
+        top_p, penalty = self._nucleus_args(top_p, repetition_penalty, "generate_continue", do_sample,
+                                            device=not do_sample or seed is not None)
         seeded = do_sample and seed is not None
         if seeded:
             temperature, top_k, seed = self._sampling_args(temperature, top_k, seed, "generate_continue")
@@ -1358,11 +1433,18 @@ class VideoChatGPTLlamaForCausalLM:
         if n <= 0:
             raise ValueError(f"context length {ctx.shape[1]} leaves no room in max_seq {self._max_seq}")
         eos, pad = self._eos_pad(eos_token_id, pad_token_id)
-        if seeded or lp_n is not None:
+        if seeded or lp_n is not None or (penalty != 1.0 and not do_sample):
             B, L = ctx.shape
             clips = list(range(B))
-            samp = (self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips]) if seeded
-                    else contextlib.nullcontext())
+            if seeded:
+                samp = self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips], top_p,
+                                      penalty)
+            elif penalty != 1.0:   # greedy entries with the penalty
+                samp = self._sampling(eng, clips, [0.0] * B, [0] * B, [0] * B, 1.0, penalty)
+            else:
+                samp = contextlib.nullcontext()
+            if penalty != 1.0:
+                self._token_sets(eng, [(b, ctx[b]) for b in clips])
             with samp, self._logprobs(eng, clips, lp_n):
                 _, _, tok = eng.prefill_append(tail, start)
                 first = eng.decode_loop(tok, ctx.shape[1], min(n, self._GREEDY_CHUNK))
@@ -1374,22 +1456,45 @@ class VideoChatGPTLlamaForCausalLM:
             return self._last_out
         _, logits, _ = eng.prefill_append(tail, start, want_logits=True, want_token=False)
         self._pos = ctx.shape[1]
-        self._last_out = self._stepwise(eng, ctx, logits, n, do_sample, temperature, stopping_criteria, eos, pad, top_k)
+        self._last_out = self._stepwise(eng, ctx, logits, n, do_sample, temperature, stopping_criteria, eos, pad, top_k,
+                                        top_p, penalty)
         return self._last_out
 
-    def _stepwise(self, eng, out, logits, n, do_sample, temperature, stopping_criteria, eos, pad, top_k=50):
+    @staticmethod
+    def _host_processors(out, logits, sampled, temperature, top_k, top_p, penalty):
+        """HF's logits processors of the stepwise path, in HF's order, on logits [B, V] fp32 after the ids `out`
+        [B, L]: RepetitionPenaltyLogitsProcessor, then (sampled only) TemperatureLogitsWarper, TopKLogitsWarper and
+        TopPLogitsWarper (min_tokens_to_keep 1); a dropped token is -inf"""
+        if penalty != 1.0:
+            ids = out.to(logits.device)
+            sc = torch.gather(logits, 1, ids)
+            sc = torch.where(sc < 0, sc * penalty, sc / penalty)
+            logits = logits.scatter(1, ids, sc)
+        if not sampled:
+            return logits
+        lg = logits / temperature
+        if top_k and top_k < lg.shape[-1]:
+            kth = torch.topk(lg, top_k, dim=-1).values[:, -1:]
+            lg = lg.masked_fill(lg < kth, float("-inf"))
+        if top_p < 1.0:
+            srt, idx = torch.sort(lg, descending=False)
+            drop = srt.softmax(dim=-1).cumsum(dim=-1) <= (1 - top_p)
+            drop[..., -1:] = False
+            lg = lg.masked_fill(drop.scatter(1, idx, drop), float("-inf"))
+        return lg
+
+    def _stepwise(self, eng, out, logits, n, do_sample, temperature, stopping_criteria, eos, pad, top_k=50, top_p=1.0,
+                  penalty=1.0):
         """One token per C-ABI call. After the loop the cache holds every returned token but the last
-        (self._pos = out.shape[1] - 1), the state generate_continue starts from."""
+        (self._pos = out.shape[1] - 1), the state generate_continue starts from. The logits go through HF's
+        processors in HF's order: repetition penalty (over `out` so far), then temperature, top-k and top-p."""
         unfinished = torch.ones(out.shape[0], dtype=torch.bool, device=out.device)
         for step in range(n):
+            lg = self._host_processors(out, logits, do_sample and temperature > 0, temperature, top_k, top_p, penalty)
             if do_sample and temperature > 0:
-                lg = logits / temperature
-                if top_k and top_k < lg.shape[-1]:            # HF's default warpers: temperature, then top-k 50
-                    kth = torch.topk(lg, top_k, dim=-1).values[:, -1:]
-                    lg = lg.masked_fill(lg < kth, float("-inf"))
                 nxt = torch.multinomial(torch.softmax(lg, dim=-1), 1)[:, 0]
             else:
-                nxt = logits.argmax(-1)
+                nxt = lg.argmax(-1)
             if eos is not None:
                 nxt = torch.where(unfinished, nxt, torch.full_like(nxt, pad))
             out = torch.cat([out, nxt[:, None].to(torch.int64)], dim=1)
