@@ -394,6 +394,41 @@ int vcl_llm_set_logprobs(vcl_handle* h, int n, const int32_t* clips_host, const 
 int vcl_llm_read_logprobs(vcl_handle* h, int entry, int first_pos, int count, int32_t* ids_out, float* lp_out,
                           void* stream);
 
+/* Beam search: transformers' _beam_search with do_sample=False (video_chatgpt/inference.py:105-112 calls HF
+ * generate; DESIGN.md section 3, "Beam search"). Per step and item, with k = num_beams beams and K = 2k:
+ *   lp       the greedy log-prob rule of vcl_op_sample_logprobs on each running beam's logits, bit for bit
+ *   score    fp32(lp + the beam's running score); before the first step beam 0 has 0, the others -1e9
+ *   top K    the K best scores of the item's k * V, ties to the lowest flat index beam * V + token
+ *   hit      the token is eos_token, or the step is the last (step t of n_new: t + 1 == n_new, HF's max_length)
+ *   running  the k best of score + hit * -1e9, ties to the lower index
+ * One RECORD per candidate: vcl_beam_record, [step][B][K], best first; one PICK per running beam: the index of its
+ * candidate in the item's K, [step][B][k]. Steps 4-6 of _beam_search (finished hypotheses, length penalty, early
+ * stopping, the returned sequences) are the caller's, on these records.
+ * The B prompts are prefilled once each into clips 0 .. B-1; item i's k beams hold cache clips of their own (B * k
+ * <= max_batch), and a new beam that does not continue its parent's clip gets a copy of the parent's columns [S, the
+ * last one written] (after the prefill: [0, S)) in a freed clip, on the device. Each clip keeps its item's left
+ * padding. Requires a contiguous cache, 2 <= num_beams <= VCL_BEAM_MAX and 2k <= vocab <= VCL_SAMPLE_WIDE_MAX_V. */
+#define VCL_BEAM_MAX 8
+typedef struct vcl_beam_record {
+  float score;     /* the accumulated score of the candidate */
+  int32_t beam;    /* its parent: the running beam (0 .. k-1) it continues */
+  int32_t token;
+} vcl_beam_record;
+/* Prefill the B prompts (n_pad_host null: unpadded, else as vcl_llm_prefill_padded) and run step 0 on their logits:
+ * records_out [B][2k] and picks_out [B][k], host or device memory, ordered on `stream`. n_new: the steps of the call
+ * (S + n_new <= max_seq + 1); eos_token -1 for none. Rejected before any device work: a null argument, a paged
+ * handle, num_beams outside 2 .. VCL_BEAM_MAX, B * num_beams > max_batch, a vocabulary outside 2k ..
+ * VCL_SAMPLE_WIDE_MAX_V, S + n_new > max_seq + 1, an eos_token or n_pad outside its range. */
+int vcl_llm_beam_start(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
+                       const int32_t* n_pad_host, int B, int S, int num_beams, int n_new, int eos_token,
+                       void* records_out, int32_t* picks_out, void* stream);
+/* The next n_steps steps of the beam search vcl_llm_beam_start began: one CUDA graph per (B * k, n_steps, k) of
+ * decode steps, each followed by the selection and the forks. records_out [n_steps][B][2k], picks_out
+ * [n_steps][B][k]. Rejected before any device work: a null argument, a paged handle, no running call, steps past
+ * the call's n_new. Any other entry point may run afterwards; a new prefill ends the beam search (its decode calls are
+ * then rejected). */
+int vcl_llm_beam_decode(vcl_handle* h, int n_steps, void* records_out, int32_t* picks_out, void* stream);
+
 /* Paged KV cache (vcl_config.kv_blocks > 0). The cache is a pool of kv_blocks BLOCKS. A block holds 128 cache columns
  * of one sequence across all layers, [layer][K = 0 | V = 1][head][128 columns][128 dims] bf16 (2 * llm_layers *
  * llm_heads * 32 KiB: 64 MiB at 7B, 100 MiB at 13B), one contiguous range. The BLOCK TABLE, int32
@@ -487,6 +522,12 @@ int vcl_op_sample_ex(const float* logits, int64_t ld, int B, int V, const float*
                      const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
                      const float* top_p_host, const float* repetition_penalty_host, uint32_t* token_sets,
                      const int32_t* top_n_host, int32_t* tok_out, int32_t* ids_out, float* lp_out, void* stream);
+/* One beam-search step on its own (vcl_llm_beam_start's rules): B items of num_beams beams, beam r = i * num_beams +
+ * j reading logits row r [ld] (device f32, bf16 values) with the running score scores[r] (device f32). last_step:
+ * every candidate hits (the max-length step). records_out [B][2 num_beams] and picks_out [B][num_beams] on the device.
+ * 2 num_beams <= V <= VCL_SAMPLE_WIDE_MAX_V. */
+int vcl_op_beam_select(const float* logits, int64_t ld, int B, int num_beams, int V, const float* scores, int eos_token,
+                       int last_step, void* records_out, int32_t* picks_out, void* stream);
 int vcl_op_layernorm(const void* x, void* y, const void* w, const void* b, int rows, int D, float eps,
                      void* stream);
 int vcl_op_rmsnorm(const void* x, void* y, const void* w, int rows, int D, float eps, void* stream);

@@ -185,6 +185,38 @@ int launch_sample(const SampleArgs& a, cudaStream_t stream);
 // set, in one launch
 int launch_token_set(unsigned int* dst, int words, const long long* ids, int n, int V, cudaStream_t stream);
 
+// ---- beam.cu ------------------------------------------------------------------------------------
+// One step of beam search (HF _beam_search, greedy; DESIGN.md section 3) over B items of k beams (2 <= k <=
+// VCL_BEAM_MAX), K = 2k candidates per item. Beam r = item i * k + j reads logits row `first ? i : (map ? map[r] :
+// r)` [ld] (first V columns, V <= VCL_SAMPLE_WIDE_MAX_V) and adds its running score (first: 0 for j = 0, -1e9 for
+// the others) to the greedy log-probs of the row. Step t = ctl[0] + step; ctl = {t0, n_total, eos (-1: none), S}
+// on the device. A candidate hits the stopping criteria when its token is eos or t + 1 >= n_total.
+// Outputs: rec [B][K] the item's candidates best first (score desc, then flat index beam * V + token asc), pick
+// [B][k] the running beams as indices into rec, score_out [B*k] their running scores (may alias score). With map
+// (beam -> cache clip, updated in place): tok_out[clip] the token each running beam feeds next, and fork [B*k] the
+// (src, dst) clip pairs to copy (-1: none); a parent keeps its clip for its first child. Without map: tok_out
+// [B*k] in beam order (optional).
+#ifndef VCL_BEAM_MAX
+#define VCL_BEAM_MAX 8   // include/vcl.h
+#endif
+struct BeamRec { float score; int beam; int token; };
+struct BeamArgs {
+  const float* logits = nullptr; long long ld = 0; int V = 0;
+  int B = 0, k = 0, first = 0, step = 0;
+  const int* ctl = nullptr;
+  const float* score = nullptr; float* score_out = nullptr;
+  int* map = nullptr; int* tok_out = nullptr; int2* fork = nullptr;
+  BeamRec* rec = nullptr; int* pick = nullptr;
+  unsigned int* cand_key = nullptr; int* cand_tok = nullptr;   // scratch [B*k][K]
+};
+int launch_beam_select(const BeamArgs& a, cudaStream_t stream);
+// The forks of a beam step: for every fork (src, dst) of fork[0 .. n), the columns [first ? 0 : S, S + t - 1]
+// (t = ctl[0] + step, S = ctl[3]) of clip src are copied to clip dst, in every layer, K and V, every head. The
+// cache is [L][clip][H][s_max][128] bf16 (layer stride layer_elems). Sources are kept clips and destinations freed
+// ones, so the copy is in place.
+int launch_kv_fork(bf16* kcache, bf16* vcache, long long layer_elems, int L, int H, int s_max, const int2* fork, int n,
+                   const int* ctl, int step, int first, cudaStream_t stream);
+
 // ---- attention.cu -------------------------------------------------------------------------------
 // softmax(Q K^T * scale [+ causal]) V for S_q == S_kv, bf16, fp32 softmax; element (b,h,s,d) of
 // each operand lives at base + b*sb + h*sh + s*ss + d.

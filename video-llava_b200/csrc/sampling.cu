@@ -43,13 +43,14 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "select.cuh"
 
 namespace vcl {
 
 namespace {
 
-constexpr int SM_THREADS = 512;
-constexpr int SM_WARPS = SM_THREADS / 32;
+constexpr int SM_THREADS = SEL_THREADS;
+constexpr int SM_WARPS = SEL_WARPS;
 constexpr int SM_MAX_V = 80 * 1024;   // the staged row of 16-bit keys: 160 KB of shared memory
 constexpr int SM_MAX_V_WIDE = VCL_SAMPLE_WIDE_MAX_V;   // 32-bit keys: 224 KB, of the 227 KB a block may take
 
@@ -68,64 +69,7 @@ __device__ __forceinline__ float key_value(uint32_t k) {
 }
 constexpr uint32_t KEY_NEG_INF = 0x007fu;   // order_key(-inf)
 
-// the same over all 32 bits of any fp32 value
-__device__ __forceinline__ uint32_t order_key32(float x) {
-  if (x != x) return 0u;
-  const uint32_t b = x == 0.f ? 0u : __float_as_uint(x);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float key_value32(uint32_t k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-constexpr uint32_t KEY32_NEG_INF = 0x007fffffu;   // order_key32(-inf)
-
-// The need-th largest key of skey[0 .. V) (1 <= need <= V): PASSES 8-bit histogram passes from the high byte
-// down, each inside the bytes chosen so far. *left receives the rank left inside that key: the key's ties to take,
-// counting from the lowest index, after the keys above it.
-template <int PASSES, class Key>
-__device__ __forceinline__ uint32_t radix_select(const Key* skey, int V, uint32_t need, uint32_t* s_hist,
-                                                 uint32_t* s_wcnt, uint32_t* s_sel, uint32_t* left) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  uint32_t prefix = 0;   // the bytes found so far
-  for (int pass = 0; pass < PASSES; ++pass) {
-    const int shift = 8 * (PASSES - 1 - pass);
-    if (tid < 256) s_hist[tid] = 0;
-    __syncthreads();
-    for (int i = tid; i < V; i += SM_THREADS) {
-      const uint32_t key = skey[i];
-      if (pass == 0) atomicAdd(&s_hist[key >> shift], 1u);
-      else if ((key >> (shift + 8)) == prefix) atomicAdd(&s_hist[(key >> shift) & 0xffu], 1u);
-    }
-    __syncthreads();
-    // threads 0..255 take the bins from the top down; an inclusive scan of the counts finds the bin in which
-    // the count from the top reaches `need`
-    uint32_t h = 0, incl = 0;
-    if (tid < 256) {
-      h = s_hist[255 - tid];
-      incl = h;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t n = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += n;
-      }
-      if (lane == 31) s_wcnt[warp] = incl;
-    }
-    __syncthreads();
-    if (tid < 256) {
-      for (int w = 0; w < warp; ++w) incl += s_wcnt[w];
-      if (incl >= need && incl - h < need) {
-        s_sel[0] = 255 - tid;           // the bin
-        s_sel[1] = need - (incl - h);   // the rank left inside it
-      }
-    }
-    __syncthreads();
-    prefix = pass == 0 ? s_sel[0] : ((prefix << 8) | s_sel[0]);
-    need = s_sel[1];
-    __syncthreads();                    // s_sel and s_hist are rewritten by the next pass
-  }
-  *left = need;
-  return prefix;
-}
+// (the 32-bit keys, order_key32 / key_value32, and radix_select are in select.cuh)
 
 // fixed-point mass of a kept token: q = rint(w * 2^36), w = exp(z - z_max) in fp32 (so q <= 2^36 and the masses of
 // a row of up to 2^17 tokens sum exactly, below 2^53, in any order)
@@ -366,31 +310,10 @@ sample_kernel(SampleArgs a) {
   // Prefix sum of index j (in run t): P_j = excl_t + (the run's own running sum up to j)
   const int run = (V + SM_THREADS - 1) / SM_THREADS;
   const int i_beg = tid * run, i_end = min(i_beg + run, V);
-  float s = 0.f;
-  int last = -1;                   // the run's last index with a nonzero weight
-  for (int i = i_beg; i < i_end; ++i) {
-    const float z = zval(skey[i]);
-    if (z >= zthr) {
-      const float w = expf(z - zmax);
-      s += w;
-      if (w > 0.f) last = i;
-    }
-  }
-  float incl = s;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const float n = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += n;
-  }
-  if (lane == 31) s_sum[warp] = incl;
   if (tid == 0) { s_pick[0] = 0x7fffffff; s_pick[1] = -1; }
-  __syncthreads();
-  float excl = incl - s, W = 0.f;
-#pragma unroll
-  for (int w = 0; w < SM_WARPS; ++w) {
-    if (w < warp) excl += s_sum[w];
-    W += s_sum[w];
-  }
+  float s, excl, W;
+  int last;                        // the run's last index with a nonzero weight
+  kept_weights(skey, i_beg, i_end, zval, zthr, zmax, s_sum, &s, &excl, &W, &last);
 
   int tok = amax;
   if (!greedy) {
@@ -439,34 +362,8 @@ sample_kernel(SampleArgs a) {
   if (tid == 0) put_lp(a, row, 0, tok, (zval(skey[tok]) - zmax) - lw);
   if (n_lp == 0) return;
   const int n_sel = min(n_lp, V);
-  // the n_sel largest keys: every key above the n_sel-th largest, then its ties from the lowest index (each run's
-  // first tie rank from a block scan of the per-run tie counts; the runs are in index order)
-  uint32_t take;
-  const uint32_t kn = radix_select<WIDE ? 4 : 2>(skey, V, (uint32_t)n_sel, s_hist, s_wcnt, s_sel, &take);
-  uint32_t eq = 0;
-  for (int i = i_beg; i < i_end; ++i) eq += skey[i] == kn;
-  uint32_t eincl = eq;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t n = __shfl_up_sync(0xffffffffu, eincl, o);
-    if (lane >= o) eincl += n;
-  }
-  if (lane == 31) s_cnt[warp] = eincl;
-  if (tid == 0) s_ntop = 0;
-  __syncthreads();
-  uint32_t rank = eincl - eq;
-  for (int w = 0; w < warp; ++w) rank += s_cnt[w];
-  for (int i = i_beg; i < i_end; ++i) {
-    const uint32_t key = skey[i];
-    bool sel = key > kn;
-    if (key == kn) sel = rank++ < take;
-    if (sel) {
-      const int q = atomicAdd(&s_ntop, 1);
-      s_top_key[q] = key;
-      s_top_idx[q] = i;
-    }
-  }
-  __syncthreads();
+  // the n_sel largest keys (ties: the lowest index first)
+  collect_top<WIDE ? 4 : 2>(skey, V, n_sel, i_beg, i_end, s_hist, s_wcnt, s_sel, s_cnt, &s_ntop, s_top_key, s_top_idx);
   // one warp sorts them: key descending, then index ascending. A token the top-k / top-p rules drop (or a NaN) is
   // reported as -1 / -inf; those sort after every kept token, since a larger key never has a smaller s
   if (warp == 0 && lane < n_lp) {

@@ -62,6 +62,8 @@ struct GraphEntry {
   int sampled;         // ... and so is the sampling table: a graph of the sampler serves every temperature / top_k /
                        // seed / top_n (h->sampler: 0 the arg-max, 1 the 16-bit sampler, 2 the 32-bit one, whose
                        // graphs serve every top_p / repetition penalty too)
+  int beam;            // beam search with this many beams per item (0: none); its step counter, scores and clip map
+                       // are read on the device too (vcl_llm_beam_decode)
   cudaGraphExec_t exec;
   long long kernels;   // kernel nodes in the graph (for vcl_launch_count)
   unsigned long long last_use;
@@ -79,6 +81,8 @@ struct StepIo {
   const int* pos_dev = nullptr;   // clip b at position pos + pos_dev[b] (null: pos)
   int sampled = 0;                // (h->sampler) the sampler picks tok_out (entry b of the sampling table for clip b) and writes
                                   // the log-probs of the entries that ask for them
+  bool beam = false;              // beam search: the logits go to beam_select and kv_fork (beam_step), which write the
+  int beam_step = 0;              // tokens of the next step; beam_step is this step's index in the chunk
 };
 
 // which sampling-table entries the rows of an lm_head call use, and the cache column their tokens take
@@ -175,6 +179,21 @@ struct vcl_handle {
   // indexed by entry and the RoPE position of the token (so a read is one contiguous copy per plane); allocated by the
   // first vcl_llm_set_logprobs that turns an entry on.
   unsigned char* lp = nullptr;
+  // Beam search (vcl_llm_beam_start / vcl_llm_beam_decode), allocated by the first call. Item i's k beams live in the
+  // cache clips beam_map[i * k .. i * k + k - 1]; the prompt is prefilled into clip i and forked to the others.
+  // beam_ctl {t0, n_total, eos, S} is written by the host before each chunk, so one captured graph per (B * k,
+  // n_steps, k) serves every call. Records [max_seq][2 max_batch] and picks [max_seq][max_batch] hold one chunk.
+  int* beam_ctl = nullptr;
+  int* beam_map = nullptr;                      // [max_batch]
+  float* beam_score = nullptr;                  // [max_batch] running scores, beam order
+  int* beam_tok = nullptr;                      // [max_batch] the token each clip feeds next
+  int2* beam_fork = nullptr;                    // [max_batch]
+  unsigned int* beam_ckey = nullptr;            // [max_batch][2 VCL_BEAM_MAX] row candidates
+  int* beam_ctok = nullptr;
+  BeamRec* beam_rec = nullptr;
+  int* beam_pick = nullptr;
+  int beam_ctl_host[4] = {0, 0, -1, 0};
+  int beam_B = 0, beam_k = 0, beam_t = 0;       // the running call (beam_k 0: none); beam_t the next step
   int lp_rows() const { return cfg.max_seq + 1; }   // a decode loop's last token may take position max_seq
   size_t lp_plane() const { return (size_t)cfg.max_batch * lp_rows() * (1 + VCL_LOGPROBS_MAX); }   // elements
 
@@ -776,6 +795,7 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
   VCL_REQUIRE((logits_out == nullptr && next_tok == nullptr) || n_layers == c.llm_layers,
               "logits / next token need the full stack (n_layers == %d)", c.llm_layers);
   if (start_pos == 0) {
+    h->beam_k = 0;   // a new sequence ends any running beam search (vcl_llm_beam_decode refuses to continue it)
     int npad_max = 0;
     if (n_pad_host != nullptr) {
       for (int b = 0; b < B; ++b) {
@@ -911,6 +931,21 @@ int score_tail(vcl_handle* h, int B, int S, const int64_t* labels, bf16* logits_
   return 0;
 }
 
+// One beam-search step on the logits in h->logits (rows by cache clip; after the prefill: by item): beam_select
+// writes the records and picks of chunk step `step`, the next tokens (h->beam_tok) and the forks, which kv_fork copies.
+int beam_step(vcl_handle* h, int step, bool first, cudaStream_t st) {
+  const int B = h->beam_B, k = h->beam_k;
+  BeamArgs a;
+  a.logits = h->logits; a.ld = h->cfg.vocab; a.V = h->cfg.vocab; a.B = B; a.k = k; a.first = first; a.step = step;
+  a.ctl = h->beam_ctl; a.score = h->beam_score; a.score_out = h->beam_score;
+  a.map = h->beam_map; a.tok_out = h->beam_tok; a.fork = h->beam_fork;
+  a.rec = h->beam_rec + (size_t)step * 2 * B * k; a.pick = h->beam_pick + (size_t)step * B * k;
+  a.cand_key = h->beam_ckey; a.cand_tok = h->beam_ctok;
+  VCL_TRY(launch_beam_select(a, st));
+  return launch_kv_fork(h->kcache, h->vcache, (long long)h->cache_layer_elems(), h->cfg.llm_layers, h->cfg.llm_heads,
+                        h->cfg.max_seq, h->beam_fork, B * k, h->beam_ctl, step, first, st);
+}
+
 // One decode step: the token of io is fed to clip b at position pos (+ io.pos_dev[b]), key floor h->d_npad[b].
 int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_t st) {
   const vcl_config& c = h->cfg;
@@ -994,6 +1029,7 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
   SampleAt smp;   // the token fed at column c_b is followed by one at column c_b + 1
   smp.on = io.sampled; smp.col = pos + 1; smp.col_dev = pd;
   VCL_TRY(lm_head_argmax(h, h->d_h, D, B, io.logits_out, io.tok_out, io.out_stride, st, io.partials_out, smp));
+  if (io.beam) VCL_TRY(beam_step(h, io.beam_step, false, st));
   return 0;
 }
 
@@ -1021,14 +1057,30 @@ int decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, 
   return 0;
 }
 
-// decode_steps from one captured graph per (B, n_new, sampled), sampled as h->sampler gives it. The positions (h->d_pos, written by the caller),
+// n_new beam-search steps over the B * k clips of the running call: step i feeds h->beam_tok[b] to clip b at position
+// h->d_pos[b] + i, then beam_select / kv_fork (beam_step) pick the next tokens. The 1..4-clip arg-max hand-off is off:
+// beam_select needs the logits.
+int beam_steps(vcl_handle* h, int Bk, int n_new, cudaStream_t st) {
+  for (int i = 0; i < n_new; ++i) {
+    StepIo io;
+    io.pos_dev = h->d_pos;
+    io.tok_in = h->beam_tok;
+    io.beam = true; io.beam_step = i;
+    VCL_TRY(llm_decode_step(h, io, Bk, i, st));
+  }
+  return 0;
+}
+
+// decode_steps from one captured graph per (B, n_new, sampled), sampled as h->sampler gives it (beam > 0: beam_steps
+// with that many beams per item, one graph per (B, n_new, beam)). The positions (h->d_pos, written by the caller),
 // the pad counts (h->d_npad) and the sampling table are read on the device, so new positions, padding or sampling
 // settings replay the same graph. Bounded LRU cache (an entry holds thousands of nodes). A stream that cannot be
 // captured runs the steps eagerly.
-int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, int sampled) {
+int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, int sampled, int beam = 0) {
+  auto steps = [&]() { return beam ? beam_steps(h, B, n_new, st) : decode_steps(h, tk, B, n_new, st, sampled); };
   GraphEntry* ge = nullptr;
   for (auto& g : h->graphs)
-    if (g.B == B && g.n_new == n_new && g.sampled == sampled) ge = &g;
+    if (g.B == B && g.n_new == n_new && g.sampled == sampled && g.beam == beam) ge = &g;
   const bool can_capture = (st != nullptr) && (st != cudaStreamLegacy);
   if (ge == nullptr && can_capture) {
     if (h->graphs.size() >= MAX_DECODE_GRAPHS) {
@@ -1040,7 +1092,7 @@ int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t 
     }
     const long long before = launch_count();
     VCL_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    const int rc = decode_steps(h, tk, B, n_new, st, sampled);
+    const int rc = steps();
     cudaGraph_t graph = nullptr;
     cudaError_t e = cudaStreamEndCapture(st, &graph);
     const long long nodes = launch_count() - before;
@@ -1060,10 +1112,10 @@ int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t 
       set_last_error("decode graph instantiate failed: %s", cudaGetErrorString(e));
       return -2;
     }
-    h->graphs.push_back({B, n_new, sampled, exec, nodes, 0});
+    h->graphs.push_back({B, n_new, sampled, beam, exec, nodes, 0});
     ge = &h->graphs.back();
   }
-  if (ge == nullptr) return decode_steps(h, tk, B, n_new, st, sampled);
+  if (ge == nullptr) return steps();
   ge->last_use = ++h->graph_clock;
   VCL_CUDA_OK(cudaGraphLaunch(ge->exec, st));
   count_launches(ge->kernels);
@@ -1528,6 +1580,89 @@ int vcl_llm_generate_padded(vcl_handle* h, const int64_t* ids, const void* video
   return vcl_llm_decode_loop(h, h->tokens, B, S, n_new, out_tokens, stream);
 }
 
+// Beam search (video_chatgpt/inference.py:105-112 calls HF generate; generate(num_beams=k) is HF's _beam_search):
+// one prefill of the B prompts, then the first beam step on the prefill logits and the fork of the prompt columns.
+int vcl_llm_beam_start(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
+                       const int32_t* n_pad_host, int B, int S, int num_beams, int n_new, int eos_token,
+                       void* records_out, int32_t* picks_out, void* stream) {
+  VCL_REQUIRE(h && ids && vid_start && records_out && picks_out, "vcl_llm_beam_start: null argument");
+  VCL_NOT_PAGED(h, "vcl_llm_beam_start");
+  const vcl_config& c = h->cfg;
+  const int k = num_beams;
+  VCL_REQUIRE(k >= 2 && k <= VCL_BEAM_MAX, "vcl_llm_beam_start: num_beams=%d outside 2..%d", k, VCL_BEAM_MAX);
+  VCL_REQUIRE(B >= 1 && (long long)B * k <= c.max_batch, "vcl_llm_beam_start: B * num_beams = %lld outside 1..%d "
+              "(max_batch: every beam takes a cache clip)", (long long)B * k, c.max_batch);
+  VCL_REQUIRE(c.vocab <= VCL_SAMPLE_WIDE_MAX_V && c.vocab >= 2 * k, "vcl_llm_beam_start: beam search takes a "
+              "vocabulary of %d..%d tokens (the selection's shared memory), this model has %d", 2 * k,
+              VCL_SAMPLE_WIDE_MAX_V, c.vocab);
+  VCL_REQUIRE(S >= 1 && n_new >= 1 && S + n_new <= c.max_seq + 1, "vcl_llm_beam_start: S + n_new = %d exceeds max_seq %d",
+              S + n_new, c.max_seq);
+  VCL_REQUIRE(eos_token >= -1 && eos_token < c.vocab, "vcl_llm_beam_start: eos_token %d outside -1..%d", eos_token,
+              c.vocab - 1);
+  if (n_pad_host != nullptr)
+    for (int b = 0; b < B; ++b)
+      VCL_REQUIRE(n_pad_host[b] >= 0 && n_pad_host[b] < S, "vcl_llm_beam_start: n_pad[%d] = %d outside 0..%d", b,
+                  n_pad_host[b], S - 1);
+  VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
+  cudaStream_t st = as_stream(stream);
+  if (h->beam_ctl == nullptr) {
+    const size_t mb = c.max_batch;
+    VCL_TRY(dalloc(h, &h->beam_ctl, 4));
+    VCL_TRY(dalloc(h, &h->beam_map, mb));
+    VCL_TRY(dalloc(h, &h->beam_score, mb));
+    VCL_TRY(dalloc(h, &h->beam_tok, mb));
+    VCL_TRY(dalloc(h, &h->beam_fork, mb));
+    VCL_TRY(dalloc(h, &h->beam_ckey, mb * 2 * VCL_BEAM_MAX));
+    VCL_TRY(dalloc(h, &h->beam_ctok, mb * 2 * VCL_BEAM_MAX));
+    VCL_TRY(dalloc(h, &h->beam_rec, (size_t)c.max_seq * 2 * mb));
+    VCL_TRY(dalloc(h, &h->beam_pick, (size_t)c.max_seq * mb));
+  }
+  h->beam_k = 0;   // (no running call until this one has started)
+  VCL_TRY(llm_prefill(h, ids, video_feats, vid_start, B, S, c.llm_layers, nullptr, h->logits, nullptr, 1, st, 0,
+                      nullptr, n_pad_host));
+  // clips: beam (i, 0) is the prompt's clip i, beam (i, j > 0) clip B + i * (k - 1) + j - 1, with item i's padding
+  const int Bk = B * k;
+  std::vector<int> map(Bk), npad(Bk);
+  for (int i = 0; i < B; ++i)
+    for (int j = 0; j < k; ++j) {
+      const int clip = j == 0 ? i : B + i * (k - 1) + j - 1;
+      map[i * k + j] = clip;
+      npad[clip] = n_pad_host != nullptr ? n_pad_host[i] : 0;
+    }
+  VCL_CUDA_OK(cudaMemcpyAsync(h->beam_map, map.data(), Bk * sizeof(int), cudaMemcpyHostToDevice, st));
+  if (h->padded)
+    VCL_CUDA_OK(cudaMemcpyAsync(h->d_npad, npad.data(), Bk * sizeof(int), cudaMemcpyHostToDevice, st));
+  h->beam_ctl_host[0] = 0; h->beam_ctl_host[1] = n_new; h->beam_ctl_host[2] = eos_token; h->beam_ctl_host[3] = S;
+  VCL_CUDA_OK(cudaMemcpyAsync(h->beam_ctl, h->beam_ctl_host, sizeof(h->beam_ctl_host), cudaMemcpyHostToDevice, st));
+  h->beam_B = B; h->beam_k = k; h->beam_t = 1;
+  VCL_TRY(beam_step(h, 0, true, st));
+  VCL_CUDA_OK(cudaMemcpyAsync(records_out, h->beam_rec, (size_t)2 * Bk * sizeof(BeamRec), cudaMemcpyDefault, st));
+  VCL_CUDA_OK(cudaMemcpyAsync(picks_out, h->beam_pick, (size_t)Bk * sizeof(int), cudaMemcpyDefault, st));
+  return 0;
+}
+
+// The next n_steps steps of the running beam search, from one captured graph per (B * k, n_steps, k).
+int vcl_llm_beam_decode(vcl_handle* h, int n_steps, void* records_out, int32_t* picks_out, void* stream) {
+  VCL_REQUIRE(h && records_out && picks_out, "vcl_llm_beam_decode: null argument");
+  VCL_NOT_PAGED(h, "vcl_llm_beam_decode");
+  VCL_REQUIRE(h->beam_k > 0, "vcl_llm_beam_decode: no beam search is running (vcl_llm_beam_start)");
+  const int n_total = h->beam_ctl_host[1];
+  VCL_REQUIRE(n_steps >= 1 && h->beam_t + n_steps <= n_total, "vcl_llm_beam_decode: steps %d..%d outside the call's "
+              "%d steps", h->beam_t, h->beam_t + n_steps - 1, n_total);
+  cudaStream_t st = as_stream(stream);
+  const int Bk = h->beam_B * h->beam_k, t0 = h->beam_t;
+  h->beam_ctl_host[0] = t0;
+  VCL_CUDA_OK(cudaMemcpyAsync(h->beam_ctl, h->beam_ctl_host, sizeof(int), cudaMemcpyHostToDevice, st));
+  // step t feeds the token picked at step t - 1 at column S + t - 1
+  VCL_TRY(launch_fill_int(h->d_pos, h->beam_ctl_host[3] + t0 - 1, Bk, st));
+  VCL_TRY(run_decode_steps(h, nullptr, Bk, n_steps, st, 0, h->beam_k));
+  h->beam_t += n_steps;
+  VCL_CUDA_OK(cudaMemcpyAsync(records_out, h->beam_rec, (size_t)n_steps * 2 * Bk * sizeof(BeamRec), cudaMemcpyDefault,
+                              st));
+  VCL_CUDA_OK(cudaMemcpyAsync(picks_out, h->beam_pick, (size_t)n_steps * Bk * sizeof(int), cudaMemcpyDefault, st));
+  return 0;
+}
+
 int vcl_llm_score(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
                   const int32_t* n_pad_host, int B, int S, const int64_t* labels, void* logits_out, float* nll_out,
                   float* loss_out, void* stream) {
@@ -1700,6 +1835,38 @@ int op_sample(const char* name, const float* logits, int64_t ld, int B, int V, c
 }  // namespace
 
 extern "C" {
+
+// beam_select alone (HF _beam_search's steps 1-3, inference.py:105-112): item i's beams are logits rows i * k ..
+// i * k + k - 1 with running scores scores[i * k + j] (device)
+int vcl_op_beam_select(const float* logits, int64_t ld, int B, int num_beams, int V, const float* scores, int eos_token,
+                       int last_step, void* records_out, int32_t* picks_out, void* stream) {
+  VCL_REQUIRE(logits && scores && records_out && picks_out, "vcl_op_beam_select: null argument");
+  if (check_device() != 0) return -2;
+  const int k = num_beams;
+  VCL_REQUIRE(k >= 2 && k <= VCL_BEAM_MAX, "vcl_op_beam_select: num_beams=%d outside 2..%d", k, VCL_BEAM_MAX);
+  VCL_REQUIRE(B >= 1, "vcl_op_beam_select: B=%d", B);
+  VCL_REQUIRE(V >= 2 * k && V <= VCL_SAMPLE_WIDE_MAX_V && ld >= V, "vcl_op_beam_select: V=%d outside %d..%d or row "
+              "pitch %lld < V", V, 2 * k, VCL_SAMPLE_WIDE_MAX_V, (long long)ld);
+  VCL_REQUIRE(eos_token >= -1 && eos_token < V, "vcl_op_beam_select: eos_token %d outside -1..%d", eos_token, V - 1);
+  cudaStream_t st = as_stream(stream);
+  const size_t Bk = (size_t)B * k, cand = Bk * 2 * k;
+  unsigned char* scratch = nullptr;
+  VCL_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&scratch), 16 + cand * 8, st));
+  const int ctl[4] = {0, last_step ? 1 : 2, eos_token, 0};   // step 0 of 1 (the max-length step) or of 2
+  BeamArgs a;
+  a.logits = logits; a.ld = ld; a.V = V; a.B = B; a.k = k; a.step = 0;
+  a.ctl = reinterpret_cast<int*>(scratch); a.score = scores;
+  a.rec = reinterpret_cast<BeamRec*>(records_out); a.pick = picks_out;
+  a.cand_key = reinterpret_cast<unsigned int*>(scratch + 16); a.cand_tok = reinterpret_cast<int*>(scratch + 16 + cand * 4);
+  int rc = 0;
+  if (cudaMemcpyAsync(scratch, ctl, sizeof(ctl), cudaMemcpyHostToDevice, st) != cudaSuccess) {
+    set_last_error("vcl_op_beam_select: control copy failed");
+    rc = -2;
+  }
+  if (rc == 0) rc = launch_beam_select(a, st);
+  cudaFreeAsync(scratch, st);
+  return rc;
+}
 
 int vcl_op_sample(const float* logits, int64_t ld, int B, int V, const float* temperature_host,
                   const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host, int32_t* tok_out,

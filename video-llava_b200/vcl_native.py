@@ -140,6 +140,9 @@ _SIGNATURES = {
     "vcl_llm_read_token_set": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "vcl_llm_set_logprobs": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), c_void_p]),
     "vcl_llm_read_logprobs": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "vcl_llm_beam_start": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_int, c_int,
+                                   c_int, c_void_p, c_void_p, c_void_p]),
+    "vcl_llm_beam_decode": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_launch_count": (ctypes.c_longlong, []),
     "vcl_kv_cache_copy": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_llm_set_block_table": (c_int, [c_void_p, POINTER(c_int32), c_void_p]),
@@ -159,6 +162,8 @@ _SIGNATURES = {
     "vcl_op_sample_ex": (c_int, [c_void_p, c_int64, c_int, c_int, POINTER(c_float), POINTER(c_int32), POINTER(c_uint64),
                                  POINTER(c_int32), POINTER(c_float), POINTER(c_float), c_void_p, POINTER(c_int32),
                                  c_void_p, c_void_p, c_void_p, c_void_p]),
+    "vcl_op_beam_select": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                   c_void_p]),
     "vcl_op_layernorm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "vcl_op_rmsnorm": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "vcl_op_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
@@ -363,6 +368,32 @@ def op_sample_ex(logits, temperature, top_k, seed, counter, top_p, repetition_pe
                                  ints(vals[5]) if top_n is not None else None, ptr(out), ptr(ids), ptr(lp),
                                  cur_stream()))
     return out if top_n is None else (out, ids, lp)
+
+
+BEAM_MAX = 8                  # include/vcl.h: VCL_BEAM_MAX, the most beams per item
+
+
+def beam_records(rec):
+    """records int32 [..., K, 3] (vcl_beam_record: f32 score bits, beam, token) -> (score f32, beam int64, token
+    int64), each [..., K]"""
+    return rec[..., 0].view(torch.float32), rec[..., 1].to(torch.int64), rec[..., 2].to(torch.int64)
+
+
+def op_beam_select(logits, scores, num_beams, eos=-1, last_step=False):
+    """One beam-search step alone (vcl_op_beam_select): logits [B * k, ld] fp32 on the device (bf16 values), scores
+    [B * k] fp32 running scores. Returns (records int32 [B, 2k, 3], picks int32 [B, k]) on the device (beam_records
+    unpacks the records)."""
+    Bk, ld = logits.shape
+    k = int(num_beams)
+    assert logits.dtype == torch.float32 and logits.stride(1) == 1 and Bk % k == 0
+    sc = scores.to(device=logits.device, dtype=torch.float32).contiguous()
+    assert sc.numel() == Bk
+    B = Bk // k
+    rec = torch.empty(B, 2 * k, 3, dtype=torch.int32, device=logits.device)
+    picks = torch.empty(B, k, dtype=torch.int32, device=logits.device)
+    check(lib().vcl_op_beam_select(c_void_p(logits.data_ptr()), logits.stride(0), B, k, ld, ptr(sc), int(eos),
+                                   int(bool(last_step)), ptr(rec), ptr(picks), cur_stream()))
+    return rec, picks
 
 
 def op_gemv(x, w, res=None, norm_w=None, eps=0.0):
@@ -703,6 +734,34 @@ class Engine:
         check(lib().vcl_llm_read_logprobs(self._h, int(entry), int(first_pos), int(count), c_void_p(ids_out.data_ptr()),
                                           c_void_p(lp_out.data_ptr()), cur_stream()))
         return ids_out, lp_out
+
+    # ---- beam search ----
+    def beam_start(self, ids, video_feats, vid_start, num_beams, n_new, eos=-1, n_pad=None):
+        """Prefill the B prompts once and run beam step 0 (vcl_llm_beam_start): num_beams beams per prompt, n_new
+        steps in all, eos -1 for none, n_pad as in prefill. Returns (records int32 [1, B, 2k, 3], picks int32
+        [1, B, k]) on the device."""
+        B, S = ids.shape
+        k = int(num_beams)
+        rec = torch.empty(1, B, 2 * k, 3, dtype=torch.int32, device=ids.device)
+        picks = torch.empty(1, B, k, dtype=torch.int32, device=ids.device)
+        vf = None
+        if video_feats is not None:
+            vf = video_feats.to(torch.bfloat16).contiguous()
+            assert vf.shape == (B, self.NV, self.cfg.clip_hidden), vf.shape
+        pads = None if n_pad is None else _host_pads(n_pad, B)
+        check(lib().vcl_llm_beam_start(self._h, ptr(ids.contiguous()), ptr(vf), ptr(vid_start.contiguous()), pads, B, S,
+                                       k, int(n_new), int(eos), ptr(rec), ptr(picks), cur_stream()))
+        self._beam_shape = (B, k)
+        return rec, picks
+
+    def beam_decode(self, n_steps):
+        """The next n_steps steps of the running beam search (vcl_llm_beam_decode): (records int32 [n, B, 2k, 3],
+        picks int32 [n, B, k]) on the device."""
+        B, k = self._beam_shape
+        rec = torch.empty(int(n_steps), B, 2 * k, 3, dtype=torch.int32, device="cuda")
+        picks = torch.empty(int(n_steps), B, k, dtype=torch.int32, device="cuda")
+        check(lib().vcl_llm_beam_decode(self._h, int(n_steps), ptr(rec), ptr(picks), cur_stream()))
+        return rec, picks
 
     # ---- KV cache read-back (tests) ----
     def _cache_shape(self):

@@ -294,6 +294,99 @@ class VideoChatGPTLlamaModel:
         return dict(num_patches=(vc.frame_size // vc.patch_size) ** 2, vision_config=vc)
 
 
+class _BeamReplay:
+    """Steps 4-6 of transformers' _beam_search (generation/utils.py, do_sample=False) replayed in fp32 torch on the
+    host, one step per device record, for B prompts of k beams, prompt length S (with its left padding, HF's
+    decoder_prompt_len) and n new tokens at most (max_length = S + n). Per step t (cur_len = S + t) it takes the K = 2k
+    candidates (score, parent beam, token), best first, and the device's k running picks:
+      hit       token == eos, or cur_len + 1 >= max_length
+      finished  the hits among the first k candidates, score / (cur_len + 1 - S) ** length_penalty, with -1e9 added
+                when the item's k finished slots are full and early_stopping is True, when the early-stop heuristic
+                is satisfied, and to every candidate that did not just finish; merged with the kept finished set by
+                top k
+      running   the picked candidates, with score + hit * -1e9
+      heuristic HF's _check_early_stop_heuristic, and the call ends when no item can improve, or (early_stopping
+                True) every finished set is full, or every candidate hit.
+    Sequences are the generated tokens only, filled with (pad or eos) when eos is set, else -1, as HF fills them."""
+
+    def __init__(self, B, k, S, n, eos, pad, length_penalty, early_stopping):
+        self.B, self.k, self.S, self.n = B, k, S, n
+        self.eos, self.lp, self.early = eos, float(length_penalty), early_stopping
+        self.max_length = S + n
+        fill = (pad if pad else eos) if eos is not None else -1
+        self.run_seq = torch.full((B, k, n), fill, dtype=torch.int64)
+        self.fin_seq = torch.full((B, k, n), fill, dtype=torch.int64)
+        self.fin_score = torch.full((B, k), -1.0e9, dtype=torch.float32)
+        self.fin_len = torch.zeros((B, k), dtype=torch.int64)          # generated tokens of a finished hypothesis
+        self.is_fin = torch.zeros((B, k), dtype=torch.bool)
+        self.unsat = torch.ones((B, 1), dtype=torch.bool)              # the early-stop heuristic is unsatisfied
+        self.first_k = torch.arange(2 * k) < k
+        self.t = 0                                                      # steps replayed
+
+    @staticmethod
+    def _take(x, idx):
+        """x [B, M, ...] gathered along dim 1 by idx [B, N]"""
+        while idx.dim() < x.dim():
+            idx = idx.unsqueeze(-1)
+        return torch.take_along_dim(x, idx, dim=1)
+
+    def step(self, score, beam, tok, pick):
+        """One step: score f32 [B, K], beam / tok int64 [B, K], pick int64 [B, k]. Returns True when HF stops."""
+        t, S = self.t, self.S
+        cur_len = S + t
+        cand_seq = self._take(self.run_seq, beam).clone()
+        cand_seq[:, :, t] = tok
+        hit = torch.full_like(tok, cur_len + 1 >= self.max_length, dtype=torch.bool)
+        if self.eos is not None:
+            hit = hit | (tok == self.eos)
+        # finished hypotheses
+        just = hit & self.first_k[None, :]
+        fin = score / ((cur_len + 1 - S) ** self.lp)
+        full = torch.all(self.is_fin, dim=-1, keepdim=True) & (self.early is True)
+        fin = fin + full.to(torch.float32) * -1.0e9
+        fin = fin + (~self.unsat).to(torch.float32) * -1.0e9
+        fin = fin + (~just).to(torch.float32) * -1.0e9
+        merged = torch.cat([self.fin_score, fin], dim=1)
+        keep = torch.topk(merged, k=self.k, dim=1)[1]
+        self.fin_seq = self._take(torch.cat([self.fin_seq, cand_seq], dim=1), keep)
+        self.fin_score = self._take(merged, keep)
+        self.fin_len = self._take(torch.cat([self.fin_len, torch.full_like(tok, t + 1)], dim=1), keep)
+        self.is_fin = self._take(torch.cat([self.is_fin, just], dim=1), keep)
+        # running beams: the device's picks
+        run_score = self._take(score + hit.to(torch.float32) * -1.0e9, pick)
+        self.run_seq = self._take(cand_seq, pick)
+        self.t = t + 1
+        cur_len += 1
+        # early stopping
+        if self.early == "never" and self.lp > 0.0:
+            best_len = self.max_length - S
+        else:
+            best_len = cur_len - S
+        best = run_score[:, :1] / (best_len ** self.lp)
+        worst = torch.where(self.is_fin, torch.min(self.fin_score, dim=1, keepdim=True)[0], -1.0e9)
+        self.unsat = self.unsat & torch.any(best > worst, dim=-1, keepdim=True)
+        improvable = bool(self.unsat.any())
+        open_beam = not (bool(self.is_fin.all()) and self.early is True)
+        return not (improvable and open_beam and not bool(hit.all()))
+
+    def steps(self, rec, picks):
+        """The records [n, B, K, 3] and picks [n, B, k] of a chunk, step by step; True once HF stops (later steps of
+        the chunk are discarded)"""
+        rec, picks = rec.cpu(), picks.cpu().to(torch.int64)
+        score, beam, tok = vn.beam_records(rec)
+        for i in range(rec.shape[0]):
+            if self.step(score[i], beam[i], tok[i], picks[i]):
+                return True
+        return False
+
+    def result(self, m):
+        """(sequences int64 [B * m, longest], sequences_scores f32 [B * m]): each prompt's m best finished
+        hypotheses, best first, cut at the longest of them"""
+        length = int(self.fin_len[:, :m].max())
+        seqs = self.fin_seq[:, :m].reshape(self.B * m, self.n)[:, :length]
+        return seqs, self.fin_score[:, :m].reshape(-1).clone()
+
+
 class VideoChatGPTLlamaForCausalLM:
     config_class = VideoChatGPTConfig
 
@@ -314,6 +407,8 @@ class VideoChatGPTLlamaForCausalLM:
         self._kv_blocks = vn.check_kv_blocks(kv_blocks)
         self.last_kv_stats = None
         self.last_logprobs = None      # generate / generate_continue / generate_requests(logprobs=...): per row or request
+        self.last_beam_scores = None   # generate(num_beams > 1): HF's sequences_scores, f32 [B * num_return_sequences]
+        self._after_beams = False      # the last generate ran beam search: there is no single turn to continue
         self._pads = None              # the left padding of the last generate (log-prob positions of generate_continue)
         self._sessions: dict = {}      # kept conversations of generate_requests (paged): key -> _schedule_paged's state
         self._session_clock = 0        # last-use stamps of the kept conversations (the least recent is swapped first)
@@ -470,9 +565,9 @@ class VideoChatGPTLlamaForCausalLM:
                                  f"({n_pad[b]} columns)")
         return starts
 
-    def _spans_dev(self, ids, feats, n_vid, n_pad=None):
+    def _spans_dev(self, ids, feats, n_vid, n_pad=None, device="cuda"):
         starts = self._video_spans(ids, n_vid, n_pad) if feats is not None else [vn.NO_VIDEO] * ids.shape[0]
-        return torch.tensor(starts, dtype=torch.int32, device="cuda")
+        return torch.tensor(starts, dtype=torch.int32, device=device)
 
     # ---- forward / generate ----------------------------------------------------------------
     def _not_paged(self, what):
@@ -682,7 +777,8 @@ class VideoChatGPTLlamaForCausalLM:
     @torch.no_grad()
     def generate(self, input_ids, video_spatio_temporal_features=None, do_sample=False, temperature=1.0,
                  max_new_tokens=32, stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50,
-                 attention_mask=None, seed=None, logprobs=None, top_p=1.0, repetition_penalty=1.0, **kw):
+                 attention_mask=None, seed=None, logprobs=None, top_p=1.0, repetition_penalty=1.0, num_beams=1,
+                 num_return_sequences=1, length_penalty=1.0, early_stopping=False, **kw):
         """Returns [B, S+n] int64 INCLUDING the prompt, like HF generate (inference.py:105-120), and
         like HF it stops at EOS (config.eos_token_id unless eos_token_id is given; None disables it):
         finished rows are padded, the call returns when every row has finished.
@@ -708,8 +804,21 @@ class VideoChatGPTLlamaForCausalLM:
         in HF's order (penalty, temperature, top-k, top-p; DESIGN.md section 3). The penalty divides (multiplies, when
         negative) the logits of every token of the row's input_ids so far (prompt, padding, new tokens); top-p only
         applies when sampling. Seeded sampling applies both on the device; a greedy call with a penalty takes the
-        device loops with greedy entries; unseeded sampling applies them on the host, step by step, as HF does."""
+        device loops with greedy entries; unseeded sampling applies them on the host, step by step, as HF does.
+        num_beams > 1: HF's beam search (do_sample=False), with HF's num_return_sequences, length_penalty and
+        early_stopping (True, False or "never"); see _beam_generate. It returns [B * num_return_sequences, S + m], the
+        best hypotheses of each prompt first, and sets self.last_beam_scores (HF's sequences_scores). Sampling, seed,
+        logprobs, top_p, repetition_penalty and stopping criteria are not supported with beams (NotImplementedError), and
+        a beam call must fit max_seq whole (S + max_new_tokens <= max_seq: a shorter call would move HF's max-length
+        step and so change the search). num_beams must be an int 1 .. 8 on every call (a ValueError otherwise, rather
+        than a silently greedy call); num_return_sequences without beams is ignored, as it always was."""
         self._not_paged("generate")
+        beams = self._beam_args(num_beams, num_return_sequences, length_penalty, early_stopping, do_sample, seed,
+                                logprobs, top_p, repetition_penalty, stopping_criteria)
+        if beams is not None:
+            return self._beam_generate(input_ids, video_spatio_temporal_features, attention_mask, max_new_tokens,
+                                       eos_token_id, pad_token_id, *beams)
+        self._after_beams, self.last_beam_scores = False, None
         lp_n = self._logprobs_arg(logprobs, "generate")
         if lp_n is not None and do_sample and seed is None:
             raise NotImplementedError("generate: logprobs are computed by the device sampler, and sampling there needs "
@@ -781,6 +890,80 @@ class VideoChatGPTLlamaForCausalLM:
         self._pos = S + new.shape[1] - 1
         self._last_out = torch.cat([ids, new], dim=1)
         return self._last_out
+
+    # beam-search steps per vcl_llm_beam_decode call between two host-side replays (see _beam_generate). Measured with
+    # tools/bench_beams.py (7B shapes, one clip at S = 448, 4 beams, 256 tokens, H100 at 700 W): 6.38 / 6.11 / 6.06 /
+    # 5.96 ms per token at 4 / 8 / 16 / 32 (an earlier run: 6.24 / 5.89 / 5.91 / 5.83) -- 8 and longer are within
+    # run-to-run spread, and 16 wastes at most 15 steps after an early stop
+    _BEAM_CHUNK = 16
+
+    def _beam_args(self, num_beams, num_return_sequences, length_penalty, early_stopping, do_sample, seed, logprobs,
+                   top_p, repetition_penalty, stopping_criteria):
+        """Checks the beam-search arguments of generate on the host -> None (no beams), or (num_beams,
+        num_return_sequences, length_penalty, early_stopping)"""
+        if isinstance(num_beams, bool) or not isinstance(num_beams, int) or num_beams < 1:
+            raise ValueError(f"generate: num_beams {num_beams!r} must be an int >= 1")
+        if num_beams == 1:
+            return None                         # (num_return_sequences keeps its old treatment: ignored)
+        v = num_return_sequences
+        if isinstance(v, bool) or not isinstance(v, int) or v < 1:
+            raise ValueError(f"generate: num_return_sequences {v!r} must be an int >= 1")
+        if num_beams > vn.BEAM_MAX:
+            raise ValueError(f"generate: num_beams {num_beams} exceeds {vn.BEAM_MAX}, the most the device keeps per prompt")
+        if num_return_sequences > num_beams:
+            raise ValueError(f"generate: num_return_sequences ({num_return_sequences}) has to be smaller or equal to "
+                             f"num_beams ({num_beams})")
+        if not (early_stopping is True or early_stopping is False or early_stopping == "never"):
+            raise ValueError(f"generate: early_stopping {early_stopping!r} must be True, False or \"never\"")
+        lp = float(length_penalty)
+        if not math.isfinite(lp):
+            raise ValueError(f"generate: length_penalty {length_penalty} must be finite")
+        for name, bad in (("do_sample=True", do_sample), ("seed", seed is not None), ("logprobs", logprobs is not None),
+                          ("top_p", float(top_p) < 1.0), ("repetition_penalty", float(repetition_penalty) != 1.0),
+                          ("stopping_criteria", bool(stopping_criteria))):
+            if bad:
+                raise NotImplementedError(f"generate: {name} is not supported with num_beams > 1 (beam search runs "
+                                          "greedy, do_sample=False, without logits processors or stopping criteria)")
+        if self.config.vocab_size > vn.SAMPLE_WIDE_MAX_V:
+            raise ValueError(f"generate: beam search takes a vocabulary of at most {vn.SAMPLE_WIDE_MAX_V} tokens on the "
+                             f"device, this model has {self.config.vocab_size}")
+        return num_beams, num_return_sequences, lp, early_stopping
+
+    def _beam_generate(self, input_ids, feats, attention_mask, max_new_tokens, eos_token_id, pad_token_id, k, m,
+                       length_penalty, early_stopping):
+        """generate(num_beams=k): HF's _beam_search (do_sample=False). The device prefills each prompt once, runs the
+        per-step selection (steps 1-3 of DESIGN.md section 3, "Beam search") and forks the KV cache, in chunks of
+        _BEAM_CHUNK steps from one CUDA graph; after each chunk _BeamReplay replays steps 4-6 (finished hypotheses,
+        length penalty, early stopping) in fp32 torch on the records it read back, and the call stops where HF stops.
+        The running beams come from the device's picks, so host and cache cannot disagree. Steps the device ran past
+        HF's stop are discarded."""
+        pads = left_padding(attention_mask, input_ids.shape)
+        self.last_logprobs = self.last_beam_scores = None
+        B, S = input_ids.shape
+        if B * k > self._max_batch:
+            raise ValueError(f"generate: {B} prompts x num_beams {k} = {B * k} beams exceed max_batch {self._max_batch} "
+                             "(every beam takes a cache clip)")
+        n = int(max_new_tokens)
+        if n < 1 or S + n > self._max_seq:
+            # (greedy calls cut max_new_tokens to fit; a beam call cannot: max_length decides when every candidate
+            # finishes and normalizes the length penalty, so a shorter call is a different search)
+            raise ValueError(f"generate: prompt length {S} + max_new_tokens {max_new_tokens} must fit max_seq "
+                             f"{self._max_seq} with beams")
+        eng = self._ensure_engine(need_llm=True)
+        dev = self.device
+        ids = input_ids.to(dev).to(torch.int64)
+        vs = self._spans_dev(ids, feats, eng.NV, pads, device=dev)
+        if feats is not None:
+            feats = feats.to(dev)
+        eos, pad = self._eos_pad(eos_token_id, pad_token_id)
+        replay = _BeamReplay(B, k, S, n, eos, pad, length_penalty, early_stopping)
+        self._last_out, self._after_beams = None, True
+        rec, picks = eng.beam_start(ids, feats, vs, k, n, -1 if eos is None else eos, n_pad=pads)
+        while not replay.steps(rec, picks):
+            rec, picks = eng.beam_decode(min(self._BEAM_CHUNK, n - replay.t))
+        seqs, scores = replay.result(m)
+        self.last_beam_scores = scores
+        return torch.cat([ids.repeat_interleave(m, dim=0), seqs.to(dev)], dim=1)
 
     def _host_stops(self, eng, out, new, n, stopping_criteria, eos, pad):
         """The device-sampled loop of generate / generate_continue: `new` [B, c] int32 holds the first c tokens
@@ -1412,6 +1595,10 @@ class VideoChatGPTLlamaForCausalLM:
         tokens of this turn. top_p / repetition_penalty: as in generate; the penalty's tokens are the whole
         conversation (every earlier turn, its answers as returned, and the new text)."""
         self._not_paged("generate_continue")
+        self.last_beam_scores = None
+        if getattr(self, "_after_beams", False):
+            raise ValueError("generate_continue: the last generate() ran beam search (num_beams > 1), which returns "
+                             "several hypotheses per prompt and leaves no single turn to continue")
         if getattr(self, "_last_out", None) is None:
             raise ValueError("generate_continue: no previous generate() to continue")
         lp_n = self._logprobs_arg(logprobs, "generate_continue")
