@@ -27,7 +27,6 @@ conventions. Differences from the reference, all documented where they occur:
 """
 from __future__ import annotations
 
-import collections
 import contextlib
 import json
 import math
@@ -44,6 +43,7 @@ import vcl_native as vn  # noqa: E402
 
 from ..constants import (DEFAULT_VID_END_TOKEN, DEFAULT_VID_START_TOKEN,  # noqa: E402
                          DEFAULT_VIDEO_PATCH_TOKEN)
+from . import inflight  # noqa: E402
 from .multimodal_projector.builder import build_vision_projector  # noqa: E402
 
 
@@ -410,7 +410,7 @@ class VideoChatGPTLlamaForCausalLM:
         self.last_beam_scores = None   # generate(num_beams > 1): HF's sequences_scores, f32 [B * num_return_sequences]
         self._after_beams = False      # the last generate ran beam search: there is no single turn to continue
         self._pads = None              # the left padding of the last generate (log-prob positions of generate_continue)
-        self._sessions: dict = {}      # kept conversations of generate_requests (paged): key -> _schedule_paged's state
+        self._sessions: dict = {}      # kept conversations of generate_requests (paged): key -> inflight.PagedSlots' state
         self._session_clock = 0        # last-use stamps of the kept conversations (the least recent is swapped first)
         self._n_slots = vn.slot_capacity(max_batch, max_slots)
         self._max_slots = 0 if max_slots is None else self._n_slots
@@ -1059,10 +1059,10 @@ class VideoChatGPTLlamaForCausalLM:
         slot, its neighbours, the queue order or the admission mode. Sampling without any seed is not supported
         in flight (only the stepwise generate draws from torch's RNG).
         A paged model (kv_blocks) gives each request only the 128-column blocks it has written, so the requests in
-        flight follow their actual lengths: see _schedule_paged. The results are the same bit for bit; afterwards
+        flight follow their actual lengths: see inflight.PagedSlots. The results are the same bit for bit; afterwards
         self.last_kv_stats holds the preemptions, the bytes swapped out and the peak blocks in use.
         chunked_prefill: on a paged model, prompts longer than _PACKED_MAX_S tokens (up to max_seq - max_new_tokens)
-        are prefilled in chunks of _PACKED_MAX_S rows (_prefill_chunked) instead of being rejected; last_kv_stats
+        are prefilled in chunks of _PACKED_MAX_S rows (inflight.prefill_chunked), not rejected; last_kv_stats
         then also counts the chunked prompts and the chunk calls. The results are those of a contiguous model.
         A contiguous model accepts the flag and ignores it: it prefills any prompt up to max_seq in one pass.
         Sessions (paged models only; a contiguous model raises ValueError). A request with "session": key (any
@@ -1073,7 +1073,7 @@ class VideoChatGPTLlamaForCausalLM:
         [1, L + S_new + n] (which its stopping criteria see too) and the conversation stays kept under key. Every turn
         returns what generate followed by generate_continue (B = 1, same arguments) returns on a contiguous model.
         Kept conversations are swapped to host memory, least recently used first, before a running request is
-        preempted (_schedule_paged). Rejected before any device work: an unknown key to continue, a session key
+        preempted (inflight.PagedSlots). Rejected before any device work: an unknown key to continue, a session key
         already kept, a key started and continued in one call, a key continued twice in one call, video features on
         a continuation, and a continuation that overflows max_seq or the pool. last_kv_stats then also counts the
         continuations, the prefill rows they did not recompute (reused_rows), the conversations swapped out
@@ -1110,20 +1110,19 @@ class VideoChatGPTLlamaForCausalLM:
         eng = self._ensure_engine(need_llm=True)
         samp = dict(do_sample=do_sample, temperature=temperature, top_k=top_k, seed=seed, logprobs=logprobs, top_p=top_p,
                     repetition_penalty=repetition_penalty)
-        reqs = [self._request(i, r, max_new_tokens, stopping_criteria, eng.NV, samp) for i, r in enumerate(requests)]
+        reqs = [inflight.request(self, i, r, max_new_tokens, stopping_criteria, eng.NV, samp)
+                for i, r in enumerate(requests)]
         if self._kv_blocks:
-            self._bind_sessions(reqs)
-            self._check_paged(reqs, chunked_prefill)
+            inflight.bind_sessions(self, reqs)
+            inflight.check_paged(self, reqs, chunked_prefill)
         sampling = any(r.temperature > 0 or r.penalty != 1.0 for r in reqs)
         eos, _ = self._eos_pad(eos_token_id, None)
         self._last_out, self._pos, self.last_logprobs = None, 0, None
         n_slots = min(n_slots, len(reqs))
-        lps = _RequestLogprobs(eng, reqs, n_slots, self.device)
+        lps = inflight.RequestLogprobs(self, eng, reqs, n_slots)
         try:
-            if self._kv_blocks:
-                out = self._schedule_paged(eng, reqs, n_slots, packed_admission, sampling, eos, chunked_prefill, lps)
-            else:
-                out = self._schedule(eng, reqs, n_slots, packed_admission, sampling, eos, lps)
+            out = inflight.schedule(self, eng, reqs, n_slots, packed_admission, sampling, eos,
+                                    chunked_prefill and bool(self._kv_blocks), lps)
             if lps.on:
                 self.last_logprobs = lps.result()
             return out
@@ -1132,433 +1131,6 @@ class VideoChatGPTLlamaForCausalLM:
                 eng.set_sampling(list(range(n_slots)), [0.0] * n_slots, [0] * n_slots, [0] * n_slots)
             if lps.on:
                 eng.set_logprobs(list(range(n_slots)), [-1] * n_slots)
-
-    def _schedule(self, eng, reqs, n_slots, packed_admission, sampling, eos, lps=None):
-        """The admission / decode loop of generate_requests"""
-        lps = lps or _RequestLogprobs(eng, reqs, n_slots, self.device)
-        dev = self.device
-        results = [None] * len(reqs)
-        queue = collections.deque(range(len(reqs)))
-        owner = [None] * n_slots            # request of each slot
-        pos = [0] * n_slots                 # tokens in each slot's cache; a slot without a request is parked at 0
-        unseen = [False] * n_slots          # the slot's first token (from its prefill) has not reached the host yet
-        gen = {}                            # request -> its new tokens so far
-        first = torch.zeros(n_slots, dtype=torch.int32, device=dev)     # the token each slot is fed next
-        while True:
-            admitted = []
-            for s in range(n_slots):
-                if owner[s] is None and queue:
-                    i = queue.popleft()
-                    admitted.append((s, i))
-                    owner[s], pos[s], unseen[s], gen[i] = i, reqs[i].S, True, []
-            if admitted and sampling:
-                self._admit_sampling(eng, [(s, reqs[i]) for s, i in admitted])
-            lps.sync(owner)
-            if admitted and packed_admission:
-                self._admit_packed(eng, [(s, reqs[i]) for s, i in admitted], first)
-            elif admitted:
-                for s, i in admitted:
-                    r = reqs[i]
-                    feats = None if r.feats is None else r.feats.to(dev)
-                    vs = torch.tensor([r.vid_start], dtype=torch.int32, device=dev)
-                    eng.slot_prefill(s, r.ids.to(dev), feats, vs, tok_out=first[s:s + 1])
-            active = [s for s in range(n_slots) if owner[s] is not None]
-            if not active:
-                return results
-            # shorter than a chunk only when a slot nears max_seq
-            m = min([self._SLOT_CHUNK] + [self._max_seq - pos[s] for s in active])
-            out = eng.slot_decode(first, pos, m + 1)
-            first = out[:, m].contiguous()
-            host = out.tolist()
-            running = [(s, owner[s]) for s in active]
-            for s in active:
-                i = owner[s]
-                r = reqs[i]
-                pos[s] += m
-                for t in (host[s] if unseen[s] else host[s][1:]):
-                    gen[i].append(t)
-                    if self._request_done(r, gen[i], eos):
-                        results[i] = torch.cat([r.ids, torch.tensor(gen[i], dtype=torch.int64)])[None].to(dev)
-                        owner[s], pos[s] = None, 0
-                        break
-                unseen[s] = False
-            lps.collect([(s, i, len(gen[i])) for s, i in running])
-
-    def _admit_sampling(self, eng, group, resumed=()):
-        """The sampling-table entries of the (slot, request) pairs admitted at one point, in one write, and the token
-        set of each penalized one: its ids; for a (slot, request, tokens) of `resumed`, its ids then those tokens."""
-        rows = list(group) + [(s, r) for s, r, _ in resumed]
-        self._set_entries(eng, [s for s, _ in rows], [r.temperature for _, r in rows], [r.top_k for _, r in rows],
-                          [r.seed for _, r in rows], [r.top_p for _, r in rows], [r.penalty for _, r in rows])
-        sets = [(s, r.ids) for s, r in group if r.penalty != 1.0]
-        sets += [(s, torch.cat([r.ids, torch.tensor(toks, dtype=torch.int64)])) for s, r, toks in resumed
-                 if r.penalty != 1.0]
-        self._token_sets(eng, sets)
-
-    def _admit_packed(self, eng, group, first):
-        """Prefill the (slot, request) pairs of one admission point: prompts longer than _PACKED_MAX_S one at a time
-        (slot_prefill), all others in one slots_prefill. Each slot's first token goes to first[slot]. The packed
-        prompts always fit the activations (max_batch * max_seq tokens): there are at most max_batch of them, each
-        shorter than max_seq (_request)."""
-        dev = first.device
-        packed = []
-        for s, r in group:
-            if r.S > self._PACKED_MAX_S:
-                feats = None if r.feats is None else r.feats.to(dev)
-                vs = torch.tensor([r.vid_start], dtype=torch.int32, device=dev)
-                eng.slot_prefill(s, r.ids.to(dev), feats, vs, tok_out=first[s:s + 1])
-            else:
-                packed.append((s, r))
-        if packed:
-            slots = [s for s, _ in packed]
-            tok = eng.slots_prefill(slots, [r.ids for _, r in packed],
-                                    [None if r.feats is None else r.feats.to(dev) for _, r in packed],
-                                    [r.vid_start for _, r in packed])
-            first[torch.tensor(slots, device=dev)] = tok
-
-    def _prefill_chunked(self, eng, group, first, packed, sampling=False):
-        """Prefill the (slot, request) pairs of one admission point whose prompts are longer than _PACKED_MAX_S on a
-        paged engine: each prompt runs as consecutive chunks of _PACKED_MAX_S rows (Engine.slots_prefill_chunk),
-        every chunk attending the columns its earlier chunks left in the slot's blocks. packed: chunk k of every
-        prompt of the group goes into one call (at most n_slots * 512 rows, which the activations hold); otherwise
-        each prompt runs alone. A slot's first token (first[slot]) is the one its last chunk gives. Returns the
-        number of chunk calls. Every chunk call also draws a token for each of its prompts (only the last one's is
-        kept), which a penalized slot adds to its token set: so the set is written again before each later call."""
-        dev, L = first.device, self._PACKED_MAX_S
-        calls = 0
-        for batch in ([group] if packed else [[g] for g in group]):
-            for start in range(0, max(r.S for _, r in batch), L):
-                live = [(s, r) for s, r in batch if start < r.S]
-                if sampling and start > 0:   # (chunk 0 follows the admission's write)
-                    self._token_sets(eng, [(s, r.ids) for s, r in live if r.penalty != 1.0])
-                tok = eng.slots_prefill_chunk([s for s, _ in live], [start] * len(live), [r.S for _, r in live],
-                                              [r.ids[start:start + L] for _, r in live],
-                                              [None if r.feats is None else r.feats.to(dev) for _, r in live],
-                                              [r.vid_start for _, r in live])
-                calls += 1
-                for j, (s, r) in enumerate(live):
-                    if start + L >= r.S:
-                        first[s] = tok[j]
-        return calls
-
-    def _check_paged(self, reqs, chunked=False):
-        """The requests a paged cache takes, checked on the host before any device work: a prompt of at most
-        min(512, max_seq) tokens (a paged engine prefills packed) unless `chunked` (any prompt _request accepts), and
-        at most kv_blocks - 1 blocks for the prompt and every new token, so that a request alone always fits the pool
-        and the scheduler always makes progress."""
-        C, usable = vn.KV_BLOCK_COLS, self._kv_blocks - 1
-        s_lim = min(self._PACKED_MAX_S, self._max_seq)
-        for i, r in enumerate(reqs):
-            if r.start == 0 and r.S > s_lim and not chunked:
-                raise ValueError(f"request {i}: prompt of {r.S} tokens; a paged KV cache takes prompts of at most "
-                                 f"{s_lim} tokens (the packed prefill); chunked_prefill=True takes longer ones")
-            need = -(-(r.S + r.n) // C)
-            if need > usable and r.start > 0:
-                raise ValueError(f"request {i}: conversation of {r.S} tokens + max_new_tokens {r.n} needs {need} blocks "
-                                 f"of {C} columns, more than the pool's {usable} (kv_blocks {self._kv_blocks}, block 0 "
-                                 "is the park block)")
-            if need > usable:
-                raise ValueError(f"request {i}: prompt {r.S} + max_new_tokens {r.n} needs {need} blocks of {C} columns, "
-                                 f"more than the pool's {usable} (kv_blocks {self._kv_blocks}, block 0 is the park block)")
-
-    def _schedule_paged(self, eng, reqs, n_slots, packed_admission, sampling, eos, chunked=False, lps=None):
-        """The admission / decode loop of generate_requests on a paged KV cache. The host keeps a free list and each
-        slot's row of the block table (block 0, the park block, wherever no request owns a block), and writes the
-        whole table to the engine before every prefill and every decode chunk.
-        - Blocks. A running request at position pos, decoding a chunk of m steps, owns the blocks of columns
-          0 .. min(pos + m, S + n) - 1: every column the chunk writes that the request can still read (past S + n - 1
-          the request has all its tokens; those columns of a chunk land in the park block or in its own last block).
-        - Admission. Swapped-out requests resume first, oldest admission first, then queued requests in queue order
-          (none overtakes another): each into a free slot when the free list covers its blocks for one chunk.
-        - Preemption. When a chunk's growth is not covered, the most recently admitted running request is swapped out
-          (its written blocks copied to pinned host memory, its blocks freed, its slot parked) until it is. Its
-          position, pending token and sampling entry stay on the host; it resumes into any free slot and free blocks,
-          restored exactly, and its tokens depend on its seed and positions only.
-        - Chunked prefill (`chunked`). A prompt over _PACKED_MAX_S tokens is admitted by the same rule (its prompt's
-          blocks plus one chunk's growth) and prefilled at its admission point by _prefill_chunked, before the next
-          decode chunk; so a request that is swapped out always holds its whole prompt.
-        - Sessions. A request with a "session" or "continues" key keeps its conversation when it ends (self._sessions):
-          its tokens [L] and the blocks of columns 0 .. L - 2, which stay out of the free list, also across calls;
-          its other blocks are freed. A continuation is admitted by the same rule with its conversation's blocks in
-          its slot's row (copied back into fresh blocks first if they were swapped out) and prefills its tail, the
-          columns L - 1 .. S - 1, through Engine.slots_prefill_append.
-        - Eviction. Kept conversations are idle: when an admission, a resume or a chunk's growth is short of blocks,
-          the least recently used one that is resident is swapped to pinned host memory (its blocks freed) before
-          anything waits or any running request is preempted.
-        - Log-probs (lps). A request swapped out before its first token reached the host takes that token's row
-          along (it lives in its old slot's entry); every other row is read after the chunk that produced it.
-        _check_paged guarantees that the oldest running request alone always fits."""
-        dev, C, K = self.device, vn.KV_BLOCK_COLS, self._SLOT_CHUNK
-        lps = lps or _RequestLogprobs(eng, reqs, n_slots, self.device)
-        sessions = self._sessions
-        table = [[0] * eng.table_row for _ in range(eng.n_slots)]    # every slot of the engine, parked
-        kept = {b for ss in sessions.values() if ss.blocks is not None for b in ss.blocks}
-        free = [b for b in range(eng.kv_blocks - 1, 0, -1) if b not in kept]   # pop() takes the lowest block
-        results = [None] * len(reqs)
-        queue = collections.deque(range(len(reqs)))
-        owner = [None] * n_slots            # request of each slot
-        pos = [0] * n_slots                 # tokens in each slot's cache; a slot without a request is parked at 0
-        unseen = [False] * n_slots          # the slot's first token has not reached the host yet
-        order = [0] * n_slots               # admission stamp of the slot's request (the latest is preempted first)
-        blocks = [[] for _ in range(n_slots)]
-        gen = {}
-        swapped = {}                        # request -> (pos, pending token, unseen, host copies of its blocks)
-        released = []                       # host buffers whose copy back may still be in flight
-        stats = dict(preemptions=0, swapped_bytes=0, peak_blocks=0, kv_blocks=eng.kv_blocks, chunked_prefills=0,
-                     chunk_calls=0, continuations=0, reused_rows=0, session_swaps=0, session_swapped_bytes=0)
-        first = torch.zeros(n_slots, dtype=torch.int32, device=dev)     # the token each slot is fed next
-        stamp = 0
-
-        def cover(i, p, m):                 # blocks of columns 0 .. min(p + m, S + n) - 1
-            r = reqs[i]
-            return -(-min(p + m, r.S + r.n) // C)
-
-        def take(s, want):
-            while len(blocks[s]) < want:
-                blocks[s].append(free.pop())
-            table[s][:len(blocks[s])] = blocks[s]
-            stats["peak_blocks"] = max(stats["peak_blocks"], eng.kv_blocks - 1 - len(free))
-
-        def release(s, keep=0):             # the first `keep` blocks stay with a kept conversation
-            free.extend(reversed(blocks[s][keep:]))
-            blocks[s], table[s] = [], [0] * eng.table_row
-            owner[s], pos[s] = None, 0
-
-        def evict_session(spare=None):
-            """swap the least recently used resident conversation (not `spare`) to host memory; False if none"""
-            keys = [k for k, ss in sessions.items() if ss.blocks is not None and k != spare]
-            if not keys:
-                return False
-            ss = sessions[min(keys, key=lambda k: sessions[k].used)]
-            ss.saved = []
-            for b in ss.blocks:
-                buf = eng.swap_buffer()
-                eng.kv_block_copy(b, buf)
-                ss.saved.append(buf)
-            free.extend(reversed(ss.blocks))
-            ss.blocks = None
-            stats["session_swaps"] += 1
-            stats["session_swapped_bytes"] += len(ss.saved) * eng.block_bytes
-            return True
-
-        def swap_out(s):
-            i = owner[s]
-            if unseen[s]:
-                lps.collect([(s, i, 1)])
-            saved = []
-            for b in blocks[s][:-(-pos[s] // C)]:        # the blocks that hold written columns
-                buf = eng.swap_buffer()
-                eng.kv_block_copy(b, buf)
-                saved.append(buf)
-            swapped[i] = (pos[s], int(first[s]), unseen[s], saved)
-            stats["preemptions"] += 1
-            stats["swapped_bytes"] += len(saved) * eng.block_bytes
-            release(s)
-
-        while True:
-            idle = [s for s in range(n_slots) if owner[s] is None]
-            admitted, resumed, tails = [], [], []
-            while swapped and idle:
-                i = min(swapped)            # requests are first admitted in queue (= index) order
-                p, tok, uns, saved = swapped[i]
-                while len(free) < cover(i, p, K) and evict_session():
-                    pass
-                if len(free) < cover(i, p, K):
-                    break
-                s = idle.pop(0)
-                del swapped[i]
-                stamp += 1
-                owner[s], pos[s], unseen[s], order[s] = i, p, uns, stamp
-                take(s, cover(i, p, K))
-                for b, buf in zip(blocks[s], saved):
-                    eng.kv_block_copy(b, buf, write=True)
-                released.extend(saved)
-                first[s] = tok
-                resumed.append((s, i))
-            while not swapped and idle and queue:
-                i = queue[0]
-                r = reqs[i]
-                ss = sessions[r.continues] if r.continues is not None else None
-                own = ss.blocks if ss is not None and ss.blocks is not None else []
-                need = cover(i, r.S, K) - len(own)
-                while len(free) < need and evict_session(spare=r.continues):
-                    pass
-                if len(free) < need:
-                    break
-                queue.popleft()
-                s = idle.pop(0)
-                stamp += 1
-                owner[s], pos[s], unseen[s], order[s], gen[i] = i, r.S, True, stamp, []
-                if ss is None:
-                    take(s, cover(i, r.S, K))
-                    admitted.append((s, i))
-                    continue
-                del sessions[r.continues]
-                blocks[s] = list(own)
-                take(s, cover(i, r.S, K))
-                if ss.saved is not None:    # swapped out: copied back into the slot's first blocks
-                    for b, buf in zip(blocks[s], ss.saved):
-                        eng.kv_block_copy(b, buf, write=True)
-                    released.extend(ss.saved)
-                tails.append((s, i))
-                stats["continuations"] += 1
-                stats["reused_rows"] += r.start
-            if admitted or resumed or tails:
-                eng.set_block_table(table)
-            if sampling and (admitted or resumed or tails):
-                # a resumed request's token set: its prompt and its tokens, the pending one too when the host has
-                # not seen it yet (its prefill's token)
-                self._admit_sampling(eng, [(s, reqs[i]) for s, i in admitted + tails],
-                                     [(s, reqs[i], gen[i] + ([int(first[s])] if unseen[s] else [])) for s, i in resumed])
-            lps.sync(owner)
-            # continuations: the tails admitted here in one call under packed_admission, one call each otherwise
-            for group in ([tails] if packed_admission and tails else [[t] for t in tails]):
-                tok = eng.slots_prefill_append([s for s, _ in group], [reqs[i].start for _, i in group],
-                                               [reqs[i].ids[reqs[i].start:] for _, i in group])
-                first[torch.tensor([s for s, _ in group], device=dev)] = tok
-            if chunked and admitted:
-                long = [(s, reqs[i]) for s, i in admitted if reqs[i].S > self._PACKED_MAX_S]
-                admitted = [(s, i) for s, i in admitted if reqs[i].S <= self._PACKED_MAX_S]
-                if long:
-                    stats["chunked_prefills"] += len(long)
-                    stats["chunk_calls"] += self._prefill_chunked(eng, long, first, packed_admission, sampling)
-            if admitted and packed_admission:
-                self._admit_packed(eng, [(s, reqs[i]) for s, i in admitted], first)
-            elif admitted:
-                for s, i in admitted:
-                    r = reqs[i]
-                    feats = None if r.feats is None else r.feats.to(dev)
-                    vs = torch.tensor([r.vid_start], dtype=torch.int32, device=dev)
-                    eng.slot_prefill(s, r.ids.to(dev), feats, vs, tok_out=first[s:s + 1])
-            active = [s for s in range(n_slots) if owner[s] is not None]
-            if not active:
-                eng.set_block_table(table)      # every slot parked again
-                stats["sessions"] = len(sessions)
-                stats["sessions_resident"] = sum(ss.blocks is not None for ss in sessions.values())
-                stats["sessions_swapped"] = stats["sessions"] - stats["sessions_resident"]
-                self.last_kv_stats = stats
-                return results
-            m = min([K] + [self._max_seq - pos[s] for s in active])
-            # growth, oldest admission first; while the free list falls short, swap out a kept conversation, else
-            # preempt the latest running request
-            for s in sorted(active, key=lambda t: order[t]):
-                while owner[s] is not None and len(free) < cover(owner[s], pos[s], m) - len(blocks[s]):
-                    if evict_session():
-                        continue
-                    swap_out(max((t for t in range(n_slots) if owner[t] is not None), key=lambda t: order[t]))
-                if owner[s] is not None:
-                    take(s, cover(owner[s], pos[s], m))
-            active = [s for s in active if owner[s] is not None]
-            eng.set_block_table(table)
-            lps.sync(owner)
-            out = eng.slot_decode(first, pos, m + 1)
-            first = out[:, m].contiguous()
-            host = out.tolist()
-            released.clear()                # the stream has passed every copy enqueued before the decode
-            running = [(s, owner[s]) for s in active]
-            for s in active:
-                i = owner[s]
-                r = reqs[i]
-                pos[s] += m
-                for t in (host[s] if unseen[s] else host[s][1:]):
-                    gen[i].append(t)
-                    if self._request_done(r, gen[i], eos):
-                        seq = torch.cat([r.ids, torch.tensor(gen[i], dtype=torch.int64)])
-                        results[i] = seq[None].to(dev)
-                        key = r.continues if r.continues is not None else r.session
-                        keep = 0
-                        if key is not None:     # kept: columns 0 .. L - 2, generate_continue's cache
-                            keep = -(-(seq.numel() - 1) // C)
-                            self._session_clock += 1
-                            sessions[key] = SimpleNamespace(ids=seq, blocks=blocks[s][:keep], saved=None,
-                                                            used=self._session_clock)
-                        release(s, keep)
-                        break
-                unseen[s] = False
-            lps.collect([(s, i, len(gen[i])) for s, i in running])
-
-    def _request(self, i, r, max_new_tokens, stopping_criteria, n_vid, samp=None):
-        """One request of generate_requests, checked on the host -> (ids [S] int64 on the host, S, n, feats,
-        vid_start, criteria, and its sampling-table entry: temperature (0: greedy), top_k, seed)"""
-        if isinstance(r, torch.Tensor):
-            r = {"input_ids": r}
-        ids = torch.as_tensor(r["input_ids"]).detach().cpu().to(torch.int64)
-        if ids.dim() == 2 and ids.shape[0] == 1:
-            ids = ids[0]
-        if ids.dim() != 1 or ids.numel() == 0:
-            raise ValueError(f"request {i}: input_ids must be [S] or [1, S], got shape {tuple(ids.shape)}")
-        S, n = ids.numel(), int(r.get("max_new_tokens", max_new_tokens))
-        if n < 1 or S + n > self._max_seq:
-            raise ValueError(f"request {i}: prompt length {S} + max_new_tokens {n} does not fit max_seq {self._max_seq}")
-        feats, vs = r.get("video_spatio_temporal_features"), vn.NO_VIDEO
-        if feats is not None and r.get("continues") is not None:
-            raise ValueError(f"request {i}: a continuation carries text only (its video is in the kept cache)")
-        if feats is not None:
-            if feats.dim() == 3 and feats.shape[0] == 1:
-                feats = feats[0]
-            if feats.dim() != 2 or feats.shape[0] != n_vid:
-                raise ValueError(f"request {i}: video_spatio_temporal_features must be [{n_vid}, C], got "
-                                 f"{tuple(feats.shape)}")
-            vs = self._video_spans(ids[None], n_vid)[0]
-        crit = r.get("stopping_criteria", stopping_criteria)
-        samp = samp or dict(do_sample=False, temperature=1.0, top_k=50, seed=None)
-        T, k, seed = 0.0, 0, 0
-        top_p, penalty = self._nucleus_args(r.get("top_p", samp.get("top_p", 1.0)),
-                                            r.get("repetition_penalty", samp.get("repetition_penalty", 1.0)),
-                                            f"request {i}", r.get("do_sample", samp["do_sample"]))
-        if r.get("do_sample", samp["do_sample"]):
-            own = r.get("seed") is not None       # a seed is there (generate_requests checks it first)
-            T, k, seed = self._sampling_args(r.get("temperature", samp["temperature"]), r.get("top_k", samp["top_k"]),
-                                             r["seed"] if own else samp["seed"], f"request {i}")
-            seed = seed if own else (seed + i) % 2 ** 64
-            if T == 0:
-                k, seed = 0, 0
-        if T == 0:
-            top_p = 1.0                           # HF adds no warpers when greedy
-        return SimpleNamespace(ids=ids, S=S, n=n, feats=feats, vid_start=vs, criteria=list(crit or []),
-                               temperature=T, top_k=k, seed=seed, top_p=top_p, penalty=penalty, session=r.get("session"),
-                               continues=r.get("continues"), start=0, lp=r.get("logprobs", samp.get("logprobs")))
-
-    def _bind_sessions(self, reqs):
-        """The "session" / "continues" keys of generate_requests' requests, checked on the host before any device
-        work. A continuation's ids become the whole conversation (the kept tokens, then its new turn), its S their
-        length and its start the first column its tail prefill writes: the kept position L - 1, where
-        generate_continue would start."""
-        started, continued = {}, {}
-        for i, r in enumerate(reqs):
-            if r.session is not None and r.continues is not None:
-                raise ValueError(f"request {i}: a request starts a conversation (\"session\") or continues one "
-                                 "(\"continues\"), not both")
-            if r.session is not None:
-                if r.session in self._sessions:
-                    raise ValueError(f"request {i}: a conversation is already kept under session key {r.session!r} "
-                                     "(continue it, or end_session it first)")
-                if r.session in started:
-                    raise ValueError(f"request {i}: session key {r.session!r} is also started by request "
-                                     f"{started[r.session]}")
-                started[r.session] = i
-            if r.continues is not None:
-                if r.continues in continued:
-                    raise ValueError(f"request {i}: conversation {r.continues!r} is also continued by request "
-                                     f"{continued[r.continues]}; one turn per conversation and call")
-                continued[r.continues] = i
-        for key, i in continued.items():
-            r = reqs[i]
-            if key in started:
-                raise ValueError(f"request {i}: conversation {key!r} is started by request {started[key]} in the same "
-                                 "call; a turn's text depends on the previous answer, so continue it in a later call")
-            if key not in self._sessions:
-                raise ValueError(f"request {i}: no conversation is kept under key {key!r}")
-            if r.S + 1 > self._PACKED_MAX_S:
-                raise ValueError(f"request {i}: the continuation's tail (the last kept token and {r.S} new tokens) "
-                                 f"has {r.S + 1} rows, more than {self._PACKED_MAX_S}")
-            conv = self._sessions[key].ids
-            L = conv.numel()
-            if L + r.S + r.n > self._max_seq:
-                raise ValueError(f"request {i}: conversation of {L} tokens + {r.S} new + max_new_tokens {r.n} does not "
-                                 f"fit max_seq {self._max_seq}")
-            r.ids, r.start = torch.cat([conv, r.ids]), L - 1
-            r.S = r.ids.numel()
 
     def end_session(self, key=None):
         """Forget the conversation kept under `key` (every kept conversation when None): its cache blocks return to
@@ -1569,18 +1141,6 @@ class VideoChatGPTLlamaForCausalLM:
         if key not in self._sessions:
             raise ValueError(f"end_session: no conversation is kept under key {key!r}")
         del self._sessions[key]
-
-    @staticmethod
-    def _request_done(r, gen, eos):
-        """Whether the request ends with its newest token gen[-1]: EOS, then the stopping criteria, then the
-        length limit, in the order of _stepwise"""
-        if eos is not None and gen[-1] == eos:
-            return True
-        if r.criteria:
-            seq = torch.cat([r.ids, torch.tensor(gen, dtype=torch.int64)])[None]
-            if any(c(seq, None) for c in r.criteria):
-                return True
-        return len(gen) >= r.n
 
     def generate_continue(self, new_input_ids, do_sample=False, temperature=1.0, max_new_tokens=32,
                           stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50, seed=None,
@@ -1695,55 +1255,4 @@ class VideoChatGPTLlamaForCausalLM:
                 break
             logits, _ = eng.decode_step(nxt.to(torch.int32).contiguous(), self._pos, want_logits=True)
             self._pos += 1
-        return out
-
-
-class _RequestLogprobs:
-    """The log-probs of one generate_requests call: the slots' entries as the engine holds them, and each request's
-    rows read so far (blocks of rows, one row per new token, in order). Request i's k-th new token took position
-    reqs[i].S + k of its slot's entry."""
-
-    def __init__(self, eng, reqs, n_slots, dev):
-        self.eng, self.reqs, self.dev = eng, reqs, dev
-        self.on = any(r.lp is not None for r in reqs)
-        self.written = [-1] * n_slots
-        self.rows = {i: [] for i, r in enumerate(reqs) if r.lp is not None}
-        self.have = {i: 0 for i in self.rows}
-
-    def sync(self, owner):
-        """One set_logprobs call for the slots whose entry changed: the top_n of the slot's request, -1 without one"""
-        if not self.on:
-            return
-        want = [-1 if i is None or self.reqs[i].lp is None else self.reqs[i].lp for i in owner]
-        changed = [s for s, w in enumerate(want) if w != self.written[s]]
-        if changed:
-            self.eng.set_logprobs(changed, [want[s] for s in changed])
-            for s in changed:
-                self.written[s] = want[s]
-
-    def collect(self, running):
-        """(slot, request, its new tokens so far): read the rows the host does not hold yet, all in one copy"""
-        reads = [(s, i, self.have[i], n - self.have[i]) for s, i, n in running if i in self.rows and n > self.have[i]]
-        if not reads:
-            return
-        total = sum(c for *_, c in reads)
-        ids = torch.empty(total, vn.LOGPROB_PLACES, dtype=torch.int32, device=self.dev)
-        lp = torch.empty(total, vn.LOGPROB_PLACES, dtype=torch.float32, device=self.dev)
-        o = 0
-        for s, i, had, c in reads:
-            self.eng.read_logprobs(s, self.reqs[i].S + had, c, ids_out=ids[o:o + c], lp_out=lp[o:o + c])
-            o += c
-        ids, lp = ids.cpu(), lp.cpu()
-        o = 0
-        for s, i, had, c in reads:
-            self.rows[i].append((ids[o:o + c], lp[o:o + c]))
-            self.have[i] += c
-            o += c
-
-    def result(self):
-        out = [None] * len(self.reqs)
-        for i, rows in self.rows.items():
-            ids = torch.cat([a for a, _ in rows])
-            lp = torch.cat([b for _, b in rows])
-            out[i] = VideoChatGPTLlamaForCausalLM._logprob_entry(ids, lp, self.reqs[i].lp)
         return out
