@@ -551,6 +551,29 @@ int vcl_kv_cache_copy(vcl_handle* h, int layer, int write, void* k, void* v, voi
 int vcl_op_decode_attention(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int B, int H,
                             int s_max, int kv_len, const int32_t* pos_dev, const int32_t* n_pad, float scale,
                             int o_xwin, void* stream);
+/* The prefill attention over the KV cache on its own, with the arguments a prefill of vcl_llm_prefill(_padded) or
+ * vcl_llm_prefill_append builds (scale 128^-1/2, causal): clip b's S queries sit at positions start_pos ..
+ * start_pos + S - 1, q [B*S][q_ld] (head h at columns h*128 ..; q_ld >= H*128, a multiple of 8), k / v caches
+ * [B][H][s_max][128], o [B*S][H*128]. n_pad_host (HOST memory, [B], or NULL: none) is each clip's left padding
+ * (vcl_llm_prefill_padded: a real query at column c attends keys n_pad[b] .. c, a pad query keys 0 .. c); with
+ * start_pos > 0 every pad count must be below start_pos. The kernel is the one the engine takes: the wgmma kernel up
+ * to 512 keys, the flash kernel beyond, and the flash kernel whenever VCL_PREFILL_ATTN_FLASH is set (read per
+ * call). Every argument is checked before any device work. Scratch is stream-ordered. */
+int vcl_op_attention_cached(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int B, int H,
+                            int s_max, int start_pos, int S, const int32_t* n_pad_host, void* stream);
+/* The packed prefill attention on its own (vcl_llm_slots_prefill / _chunk / _append): n <= 64 sequences, sequence i
+ * the len_host[i] (1..512) queries at positions start_host[i] .. of cache slot slots_host[i] (0 .. n_slots - 1),
+ * attending keys 0 .. their own position; its rows follow sequence i - 1's in q [sum len][q_ld] and o [sum
+ * len][H*128]. flash_host[i] (NULL: all 0) puts it on the flash kernel (a paged cache only), else on the wgmma kernel
+ * (start + len <= 512). Keys: table_host NULL, the contiguous caches k / v [n_slots][H][s_max][128]; otherwise a
+ * paged pool, k / v the K / V bases of one layer inside block 0 and column c of slot s in block table_host[s *
+ * table_row + c / 128] (table_row >= ceil(s_max / 128), every entry a sequence reads in 0 .. n_blocks - 1), blocks
+ * blk elements apart, heads 128 x 128 apart inside a block. One launch per kernel kind. Every argument is checked
+ * before any device work. Scratch is stream-ordered. */
+int vcl_op_attention_packed(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int H, int s_max,
+                            int n_slots, int n, const int32_t* slots_host, const int32_t* start_host,
+                            const int32_t* len_host, const int32_t* flash_host, const int32_t* table_host,
+                            int table_row, int n_blocks, int64_t blk, void* stream);
 /* out[b,n] = x[b,:].W[n,:] (+res) with optional RMSNorm of x: B <= 4 the ring kernel of the single-clip
  * decode path (fused norm), 5 <= B <= 16 the wide ring kernel (norm + window-major re-layout by a launch of
  * its own, as on the decode path) */

@@ -30,6 +30,7 @@ pytestmark = pytest.mark.gpu
 import vcl_native as vn  # noqa: E402
 from oracle import vcl_oracle as O  # noqa: E402
 from _util import make_engine, to_dev  # noqa: E402
+from _attn_ref import attn_ref  # noqa: E402
 
 DEV = "cuda"
 SMALL = O.LlmCfg(hidden=512, inter=1024, heads=4, layers=2)
@@ -313,19 +314,10 @@ def test_slot_prefill_touches_only_its_slot(eng17):
 # ------------------------------------------------------------------------------------------
 # 6. decode attention against fp64
 def _attn_ref(q, k, v, kv_len, n_pad, pos, scale):
-    """[B, H, 128] fp64: scores bf16(bf16(q.k) * scale), fp32 softmax over keys n_pad[b] .. c_b, p rounded to bf16,
-    p . v accumulated exactly"""
-    B, H = k.shape[:2]
-    out = torch.empty(B, H, 128, dtype=torch.float64, device=q.device)
-    for b in range(B):
-        c = kv_len - 1 + pos[b]
-        qb = q[b, :H * 128].view(H, 1, 128).double()
-        kb, vb = k[b, :, n_pad[b]:c + 1].double(), v[b, :, n_pad[b]:c + 1].double()
-        s = (qb @ kb.transpose(1, 2)).bfloat16().float()
-        s = (s * torch.tensor(scale, dtype=torch.float32)).bfloat16().float()
-        p = torch.softmax(s, -1).bfloat16().double()
-        out[b] = (p @ vb)[:, 0]
-    return out
+    """[B, H, 128] fp64 (tests/_attn_ref.py): clip b's query at column c_b = kv_len - 1 + pos[b] attends keys
+    n_pad[b] .. c_b"""
+    B = k.shape[0]
+    return attn_ref(q, k, v, list(range(B)), [kv_len - 1 + pos[b] for b in range(B)], list(n_pad), scale)
 
 
 def _attn_case(B, H, s_max, kv_len, n_pad, pos, kind="random", q_ld_heads=1, seed=0):

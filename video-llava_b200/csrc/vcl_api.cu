@@ -759,6 +759,49 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
   return 0;
 }
 
+// The prefill attention of one layer (llm_prefill, and vcl_op_attention_cached / _packed, which test exactly this
+// launch): head h of query row r is q[r * q_ld + h * 128 ..], its output o[r * o_ld + h * 128 ..]; rows are
+// [B][S] (clip b's queries at positions start_pos .. start_pos + S - 1), or the packed rows of `pack` (kernels.h;
+// S is then the longest sequence and start_pos 0). Keys and values: the contiguous cache [clip][H][s_max][128] at
+// kc / vc, or with pages.table the layer's K / V bases in a paged pool, heads 128 x 128 apart inside a block
+// (kernels.h: KvPages); pack_attn then says which packed kernels run (1: wgmma, 2: flash, 3: both).
+AttnArgs prefill_attn_args(const bf16* q, long long q_ld, const bf16* kc, const bf16* vc, bf16* o, long long o_ld,
+                           int B, int H, int S, int s_max, int start_pos, const int* n_pad, const int* pack,
+                           const KvPages& pages, int pack_attn) {
+  AttnArgs a;
+  a.q = q; a.q_sb = (long long)S * q_ld; a.q_sh = 128; a.q_ss = q_ld;
+  a.k = kc; a.k_sb = (long long)H * s_max * 128; a.k_sh = (long long)s_max * 128; a.k_ss = 128;
+  a.v = vc; a.v_sb = a.k_sb; a.v_sh = a.k_sh; a.v_ss = 128;
+  a.o = o; a.o_sb = (long long)S * o_ld; a.o_sh = 128; a.o_ss = o_ld;
+  a.B = B; a.H = H; a.S = S; a.head_dim = 128; a.scale = 0.08838834764831845f; a.causal = 1;   // 128 ^ -1/2
+  a.S_kv = start_pos + S; a.q_off = start_pos; a.n_pad = n_pad; a.pack = pack;
+  if (pages.table != nullptr) {
+    a.k_sb = a.v_sb = 0; a.k_sh = a.v_sh = 128 * 128; a.pages = pages;
+    a.pack_tc = (pack_attn & 1) != 0; a.pack_flash = (pack_attn & 2) != 0;
+  }
+  return a;
+}
+
+// The packed-row map (kernels.h) of n sequences into p (pack_elems(sum of len_host) ints, zeroed): sequence i is
+// rows start_i .. start_i + len_host[i] - 1 of its prompt (start_host null: 0) into cache slot slots_host[i], on the
+// flash kernel when flash_host[i] (null: none) is set. Returns the packed kernels that run (prefill_attn_args'
+// pack_attn).
+int fill_pack_map(int* p, int n, const int32_t* slots_host, const int32_t* start_host, const int32_t* len_host,
+                  const int* flash_host) {
+  int pack_attn = 0;
+  for (int i = 0, r = 0; i < n; ++i) {
+    const int start = start_host ? start_host[i] : 0, len = len_host[i];
+    const bool fl = flash_host != nullptr && flash_host[i];
+    pack_attn |= fl ? 2 : 1;
+    pack_off(p)[i] = r; pack_len(p)[i] = fl ? 0 : len; pack_slot(p)[i] = slots_host[i];
+    pack_last(p)[i] = r + len - 1; pack_start(p)[i] = start; pack_end(p)[i] = start + len;
+    for (int j = 0; j < len; ++j, ++r) {
+      pack_row(p, r)[0] = i; pack_row(p, r)[1] = start + j;
+    }
+  }
+  return pack_attn;
+}
+
 // start_pos > 0 continues a cached sequence: the S new tokens take positions start_pos .. start_pos+S-1
 // and attend to the whole cache (multi-turn reuse; no video span in a continuation).
 // states_out (optional): [n_layers + 1][B][S][D], entry i = HF's hidden_states[i] (the raw output of
@@ -835,7 +878,6 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
   }
   VCL_TRY(launch_embed_splice(reinterpret_cast<const long long*>(ids), h->embed, h->l_vid, vid_start,
                               h->l_h, B, S, D, video_feats ? NV : 0, c.vocab, st, pk, M));
-  const float scale = 0.08838834764831845f;  // 128 ^ -1/2
   auto keep_state = [&](int i) -> int {
     if (states_out == nullptr) return 0;
     VCL_CUDA_OK(cudaMemcpyAsync(reinterpret_cast<bf16*>(states_out) + (size_t)i * M * D, h->l_h, (size_t)M * D * 2,
@@ -863,18 +905,8 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
       VCL_TRY(launch_rope_kv_prefill(h->l_qkv, kc(l), vc(l), h->rope_cos, h->rope_sin, B,
                                      S, H, 128, c.max_seq, start_pos, st, nullptr, np));
     }
-    AttnArgs a;
-    a.q = h->l_qkv; a.q_sb = (long long)S * 3 * D; a.q_sh = 128; a.q_ss = 3 * D;
-    a.k = kc(l); a.k_sb = (long long)H * c.max_seq * 128; a.k_sh = (long long)c.max_seq * 128; a.k_ss = 128;
-    a.v = vc(l); a.v_sb = a.k_sb; a.v_sh = a.k_sh; a.v_ss = 128;
-    a.o = h->l_attn; a.o_sb = (long long)S * D; a.o_sh = 128; a.o_ss = D;
-    a.B = B; a.H = H; a.S = S; a.head_dim = 128; a.scale = scale; a.causal = 1;
-    a.S_kv = start_pos + S; a.q_off = start_pos; a.n_pad = np; a.pack = pk;
-    if (h->paged()) {   // heads 128 x 128 apart inside a block (kernels.h: KvPages)
-      a.k_sb = a.v_sb = 0; a.k_sh = a.v_sh = 128 * 128; a.pages = h->pages();
-      a.pack_tc = (pack_attn & 1) != 0; a.pack_flash = (pack_attn & 2) != 0;
-    }
-    VCL_TRY(launch_attention(a, st));
+    VCL_TRY(launch_attention(prefill_attn_args(h->l_qkv, 3 * D, kc(l), vc(l), h->l_attn, D, B, H, S, c.max_seq,
+                                               start_pos, np, pk, h->pages(), pack_attn), st));
     VCL_TRY(gemm(h->l_attn, D, w.wo, D, h->l_h, D, nullptr, h->l_h, D, M, D, D, ACT_NONE, st));
     VCL_TRY(launch_rmsnorm(h->l_h, D, h->l_x, D, w.ln2, M, D, c.rms_eps, st));
     VCL_TRY(gemm(h->l_x, D, w.wgu, D, h->l_act, F, nullptr, nullptr, 0, M, 2 * F, D, ACT_SWIGLU, st));
@@ -1247,19 +1279,8 @@ static int packed_prefill(vcl_handle* h, int n, const int32_t* slots_host, const
                    const int32_t* len_host, const int* flash_host, long long M, int S_max, const int64_t* ids,
                    const void* video_feats, const int32_t* vid_start, int32_t* next_tok, cudaStream_t st) {
   std::vector<int> map(pack_elems(M), 0);
-  int* p = map.data();
-  int pack_attn = 0;
-  for (int i = 0, r = 0; i < n; ++i) {
-    const int start = start_host ? start_host[i] : 0, len = len_host[i];
-    const bool fl = flash_host != nullptr && flash_host[i];
-    pack_attn |= fl ? 2 : 1;
-    pack_off(p)[i] = r; pack_len(p)[i] = fl ? 0 : len; pack_slot(p)[i] = slots_host[i];
-    pack_last(p)[i] = r + len - 1; pack_start(p)[i] = start; pack_end(p)[i] = start + len;
-    for (int j = 0; j < len; ++j, ++r) {
-      pack_row(p, r)[0] = i; pack_row(p, r)[1] = start + j;
-    }
-  }
-  VCL_CUDA_OK(cudaMemcpyAsync(h->d_pack, p, map.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  const int pack_attn = fill_pack_map(map.data(), n, slots_host, start_host, len_host, flash_host);
+  VCL_CUDA_OK(cudaMemcpyAsync(h->d_pack, map.data(), map.size() * sizeof(int), cudaMemcpyHostToDevice, st));
   int sampled = 0;
   for (int i = 0; i < n; ++i) sampled = std::max(sampled, h->sampler(slots_host[i], 1));
   return llm_prefill(h, ids, video_feats, vid_start, n, S_max, h->cfg.llm_layers, nullptr, nullptr, next_tok, 1, st,
@@ -2042,6 +2063,127 @@ int vcl_op_decode_attention(const void* q, int64_t q_ld, const void* k, const vo
   return launch_decode_attention(reinterpret_cast<const bf16*>(q), q_ld, reinterpret_cast<const bf16*>(k),
                                  reinterpret_cast<const bf16*>(v), reinterpret_cast<bf16*>(o), (long long)H * 128, B,
                                  H, 128, s_max, kv_len, scale, as_stream(stream), pos_dev, o_xwin != 0, n_pad);
+}
+
+}  // extern "C"
+
+namespace {
+
+int op_attention_init() {
+  static bool inited = false;
+  if (!inited) {
+    VCL_TRY(init_attention_kernels());
+    inited = true;
+  }
+  return 0;
+}
+
+bool aligned16(const void* p) { return ((uintptr_t)p % 16) == 0; }
+
+}  // namespace
+
+extern "C" {
+
+int vcl_op_attention_cached(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int B, int H,
+                            int s_max, int start_pos, int S, const int32_t* n_pad_host, void* stream) {
+  if (check_device() != 0) return -2;
+  VCL_REQUIRE(q && k && v && o, "vcl_op_attention_cached: q, k, v and o are required");
+  VCL_REQUIRE(aligned16(q) && aligned16(k) && aligned16(v) && aligned16(o),
+              "vcl_op_attention_cached: q, k, v and o must be 16-byte aligned");
+  VCL_REQUIRE(B >= 1 && H >= 1, "vcl_op_attention_cached: B=%d H=%d", B, H);
+  VCL_REQUIRE(q_ld >= (int64_t)H * 128 && q_ld % 8 == 0, "vcl_op_attention_cached: q_ld=%lld is below H*128 = %d or "
+              "not a multiple of 8", (long long)q_ld, H * 128);
+  VCL_REQUIRE(S >= 1 && start_pos >= 0 && start_pos + S <= s_max, "vcl_op_attention_cached: positions %d..%d "
+              "(start_pos %d, S %d) outside the cache (s_max %d)", start_pos, start_pos + S - 1, start_pos, S, s_max);
+  // llm_prefill's rule: a new sequence keeps a real token per clip, a continuation starts past every clip's padding
+  int npad_max = 0;
+  if (n_pad_host != nullptr) {
+    for (int b = 0; b < B; ++b) {
+      VCL_REQUIRE(n_pad_host[b] >= 0 && n_pad_host[b] < start_pos + S, "vcl_op_attention_cached: n_pad[%d] = %d "
+                  "outside 0..%d", b, n_pad_host[b], start_pos + S - 1);
+      npad_max = n_pad_host[b] > npad_max ? n_pad_host[b] : npad_max;
+    }
+    VCL_REQUIRE(start_pos == 0 || start_pos > npad_max, "vcl_op_attention_cached: start_pos %d lies inside the left "
+                "padding (%d columns)", start_pos, npad_max);
+  }
+  VCL_TRY(op_attention_init());
+  cudaStream_t st = as_stream(stream);
+  int* d_npad = nullptr;   // as in llm_prefill: no padding array when every clip is unpadded
+  if (npad_max > 0) {
+    VCL_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&d_npad), (size_t)B * sizeof(int), st));
+    VCL_CUDA_OK(cudaMemcpyAsync(d_npad, n_pad_host, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, st));
+  }
+  const int rc = launch_attention(
+      prefill_attn_args(reinterpret_cast<const bf16*>(q), q_ld, reinterpret_cast<const bf16*>(k),
+                        reinterpret_cast<const bf16*>(v), reinterpret_cast<bf16*>(o), (long long)H * 128, B, H, S,
+                        s_max, start_pos, d_npad, nullptr, KvPages(), 1),
+      st);
+  if (d_npad != nullptr) VCL_CUDA_OK(cudaFreeAsync(d_npad, st));
+  return rc;
+}
+
+int vcl_op_attention_packed(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int H, int s_max,
+                            int n_slots, int n, const int32_t* slots_host, const int32_t* start_host,
+                            const int32_t* len_host, const int32_t* flash_host, const int32_t* table_host,
+                            int table_row, int n_blocks, int64_t blk, void* stream) {
+  if (check_device() != 0) return -2;
+  VCL_REQUIRE(q && k && v && o && slots_host && start_host && len_host,
+              "vcl_op_attention_packed: q, k, v, o, slots, starts and lengths are required");
+  VCL_REQUIRE(aligned16(q) && aligned16(k) && aligned16(v) && aligned16(o),
+              "vcl_op_attention_packed: q, k, v and o must be 16-byte aligned");
+  VCL_REQUIRE(H >= 1 && s_max >= 1 && n_slots >= 1, "vcl_op_attention_packed: H=%d s_max=%d n_slots=%d", H, s_max,
+              n_slots);
+  VCL_REQUIRE(q_ld >= (int64_t)H * 128 && q_ld % 8 == 0, "vcl_op_attention_packed: q_ld=%lld is below H*128 = %d or "
+              "not a multiple of 8", (long long)q_ld, H * 128);
+  VCL_REQUIRE(n >= 1 && n <= PACK_SEQ_MAX, "vcl_op_attention_packed: n=%d sequences outside 1..%d", n, PACK_SEQ_MAX);
+  const bool paged = table_host != nullptr;
+  if (paged) {
+    VCL_REQUIRE(table_row >= (s_max + 127) / 128 && n_blocks >= 1 && blk >= (int64_t)H * 128 * 128 && blk % 8 == 0,
+                "vcl_op_attention_packed: table_row=%d (needs >= %d), n_blocks=%d or blk=%lld (needs a multiple of 8 "
+                ">= H*128*128) out of range", table_row, (s_max + 127) / 128, n_blocks, (long long)blk);
+  }
+  long long M = 0;
+  int S_max = 0;
+  for (int i = 0; i < n; ++i) {
+    const int s = slots_host[i], st0 = start_host[i], len = len_host[i];
+    const bool fl = flash_host != nullptr && flash_host[i];
+    VCL_REQUIRE(s >= 0 && s < n_slots, "vcl_op_attention_packed: sequence %d: slot %d outside 0..%d", i, s,
+                n_slots - 1);
+    VCL_REQUIRE(len >= 1 && len <= 512, "vcl_op_attention_packed: sequence %d has %d rows, outside 1..512", i, len);
+    VCL_REQUIRE(st0 >= 0 && st0 + len <= s_max, "vcl_op_attention_packed: sequence %d: positions %d..%d outside the "
+                "cache (s_max %d)", i, st0, st0 + len - 1, s_max);
+    VCL_REQUIRE(fl || st0 + len <= 512, "vcl_op_attention_packed: sequence %d ends at %d keys; the wgmma kernel "
+                "attends at most 512", i, st0 + len);
+    VCL_REQUIRE(!fl || paged, "vcl_op_attention_packed: sequence %d is on the flash kernel, which reads a paged "
+                "cache only", i);
+    if (paged) {
+      for (int kb = 0; kb < (st0 + len + 127) / 128; ++kb) {
+        const int blk_id = table_host[(size_t)s * table_row + kb];
+        VCL_REQUIRE(blk_id >= 0 && blk_id < n_blocks, "vcl_op_attention_packed: table[%d][%d] = %d outside the pool "
+                    "(0..%d)", s, kb, blk_id, n_blocks - 1);
+      }
+    }
+    M += len;
+    S_max = len > S_max ? len : S_max;
+  }
+  VCL_TRY(op_attention_init());
+  // one stream-ordered block: the packed-row map, then (paged) the block table
+  std::vector<int> hb(pack_elems(M) + (paged ? (size_t)n_slots * table_row : 0), 0);
+  const int pack_attn = fill_pack_map(hb.data(), n, slots_host, start_host, len_host, flash_host);
+  if (paged) memcpy(hb.data() + pack_elems(M), table_host, (size_t)n_slots * table_row * sizeof(int));
+  cudaStream_t st = as_stream(stream);
+  int* d = nullptr;
+  VCL_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&d), hb.size() * sizeof(int), st));
+  VCL_CUDA_OK(cudaMemcpyAsync(d, hb.data(), hb.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  KvPages pages;
+  if (paged) { pages.table = d + pack_elems(M); pages.row = table_row; pages.blk = blk; }
+  const int rc = launch_attention(
+      prefill_attn_args(reinterpret_cast<const bf16*>(q), q_ld, reinterpret_cast<const bf16*>(k),
+                        reinterpret_cast<const bf16*>(v), reinterpret_cast<bf16*>(o), (long long)H * 128, n, H,
+                        S_max, s_max, 0, nullptr, d, pages, pack_attn),
+      st);
+  VCL_CUDA_OK(cudaFreeAsync(d, st));
+  return rc;
 }
 
 }  // extern "C"

@@ -149,6 +149,11 @@ _SIGNATURES = {
     "vcl_kv_block_copy": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "vcl_op_decode_attention": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                         c_void_p, c_void_p, c_float, c_int, c_void_p]),
+    "vcl_op_attention_cached": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                        c_int, POINTER(c_int32), c_void_p]),
+    "vcl_op_attention_packed": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                        POINTER(c_int32), POINTER(c_int32), POINTER(c_int32), POINTER(c_int32),
+                                        POINTER(c_int32), c_int, c_int, c_int64, c_void_p]),
     "vcl_op_cross_entropy": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_op_gemm": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
                             c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -450,6 +455,59 @@ def op_decode_attention(q, k, v, kv_len, n_pad, pos_dev=None, scale=128 ** -0.5,
         o = torch.empty(B, H * 128, dtype=torch.bfloat16, device=q.device)
     check(lib().vcl_op_decode_attention(ptr(q), q.stride(0), ptr(k), ptr(v), ptr(o), B, H, s_max, int(kv_len),
                                         ptr(pos_dev), ptr(n_pad), scale, int(o_xwin), cur_stream()))
+    return o
+
+
+def _rows_view(t, what):
+    """a [rows, ld] bf16 device tensor with unit column stride -> (pointer, row pitch)"""
+    assert t.is_cuda and t.dtype == torch.bfloat16 and t.dim() == 2 and t.stride(1) == 1, what
+    return c_void_p(t.data_ptr()), t.stride(0)
+
+
+def _ints(vals):
+    vals = [int(x) for x in vals]
+    return (c_int32 * len(vals))(*vals)
+
+
+def op_attention_cached(q, k, v, start_pos, n_pad=None, out=None):
+    """The prefill attention over the cache alone (vcl_op_attention_cached): q [B*S, q_ld] bf16 (head h at columns
+    h*128 ..), k / v [B, H, s_max, 128] bf16 caches, the queries at positions start_pos .. start_pos + S - 1,
+    n_pad None or B host ints. Returns o [B*S, H*128] (out if given)."""
+    B, H, s_max, hd = k.shape
+    assert hd == 128 and v.shape == k.shape and k.is_contiguous() and v.is_contiguous()
+    qp, q_ld = _rows_view(q, "q")
+    S = q.shape[0] // B
+    o = out if out is not None else torch.empty(B * S, H * 128, dtype=torch.bfloat16, device=q.device)
+    pads = None if n_pad is None else _host_pads(n_pad, B)
+    check(lib().vcl_op_attention_cached(qp, q_ld, ptr(k), ptr(v), ptr(o), B, H, s_max, int(start_pos), S, pads,
+                                        cur_stream()))
+    return o
+
+
+def op_attention_packed(q, k, v, slots, starts, lens, flash=None, table=None, n_blocks=0, blk=0, s_max=None,
+                        out=None):
+    """The packed prefill attention alone (vcl_op_attention_packed): sequence i is lens[i] query rows of q [sum lens,
+    q_ld] at positions starts[i] .. of slot slots[i] (host ints), on the flash kernel when flash[i] (paged only).
+    Contiguous cache (table None): k / v [n_slots, H, s_max, 128]. Paged: k / v are one layer's K / V planes of block 0
+    of a pool (any [.., H, 128, 128] views), table [n_slots, table_row] host ints, n_blocks blocks blk elements apart,
+    s_max the columns a slot may hold. Returns o [sum lens, H*128] (out if given)."""
+    n = len(slots)
+    qp, q_ld = _rows_view(q, "q")
+    H = k.shape[-3]
+    if table is None:
+        n_slots, _, s_max, _ = k.shape
+        assert k.is_contiguous() and v.shape == k.shape and v.is_contiguous()
+        tab, row = None, 0
+    else:
+        vals = table.tolist() if hasattr(table, "tolist") else table
+        n_slots, row = len(vals), len(vals[0])
+        tab = _ints([b for r in vals for b in r])
+    o = out if out is not None else torch.empty(sum(int(x) for x in lens), H * 128, dtype=torch.bfloat16,
+                                                device=q.device)
+    check(lib().vcl_op_attention_packed(qp, q_ld, c_void_p(k.data_ptr()), c_void_p(v.data_ptr()), ptr(o), H,
+                                        int(s_max), n_slots, n, _ints(slots), _ints(starts), _ints(lens),
+                                        None if flash is None else _ints(flash), tab, row, int(n_blocks), int(blk),
+                                        cur_stream()))
     return o
 
 
