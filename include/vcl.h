@@ -362,6 +362,48 @@ int vcl_llm_set_token_set(vcl_handle* h, int entry, const int64_t* ids, int n, v
  * handle that never allocated its token sets. */
 int vcl_llm_read_token_set(vcl_handle* h, int entry, uint32_t* bits_out, void* stream);
 
+/* Banned tokens: HF's NoRepeatNGramLogitsProcessor, NoBadWordsLogitsProcessor and MinNewTokensLengthLogitsProcessor on
+ * the device. Each only sets logits to -inf, so they commute with each other and with the penalty, and the sampler
+ * applies them after the penalty and the temperature, before top-k: HF's order. For a draw at cache column c with the
+ * entry's TOKEN HISTORY h[0 .. c) (HF's input_ids of its row, left padding and video placeholders included):
+ *   n-gram n > 0   if c + 1 >= n, ban h[i + n - 1] for every i in 0 .. c - n with h[i .. i + n - 2] = h[c - n + 1 ..
+ *                  c - 1] (n = 1 bans every id of the row)
+ *   bad words      a one-id word is always banned; a word w of L > 1 ids bans w[L - 1] when L <= c and
+ *                  h[c - L + 1 .. c - 1] = w[0 .. L - 2]
+ *   EOS            banned while c < eos_from_col (min_new_tokens m: eos_from_col = the first new token's column + m)
+ * A banned token's value becomes -inf; the maximum, top-k, top-p, the draw and the log-probs then follow as before,
+ * and a row with every token banned takes the arg-max fallback (token 0). The logits buffer is not written. The exact
+ * rules are in DESIGN.md section 3, "Banned tokens".
+ *
+ * vcl_llm_set_bans writes n entries of the ban table (HOST memory, [n] each): clip clips_host[i] gets the n-gram
+ * size ngram_host[i] (0: off), eos_host[i] (-1: off) with eos_from_col_host[i], and its bad words
+ * words_host[i * VCL_BAN_WORDS_MAX ..]: records (L, id_0 .. id_{L-1}) up to an L of 0 or the end of the
+ * VCL_BAN_WORDS_MAX int32. One host-to-device copy on `stream`. Every entry is off after vcl_create. An entry with a
+ * ban takes the 32-bit sampler (vcl_llm_set_sampling_ex) with the ban stage, and a decode loop of such entries has a
+ * CUDA graph of its own per (B, n_new), replayed for any settings; calls whose entries have no ban launch what they
+ * launched before. The first call that turns a ban on allocates the ban table and the token histories,
+ * [max_batch][max_seq + 1] int32 (512 KB at 64 x 2048). Rejected before any device work: n outside 1 .. max_batch, a
+ * clip outside 0 .. max_batch-1 or given twice, a negative n-gram size or eos_from_col, an EOS outside -1 ..
+ * vocab-1, a word of length < 0 or running past the list, an id outside 0 .. vocab-1, a ban on a vocabulary over
+ * VCL_SAMPLE_WIDE_MAX_V. */
+#define VCL_BAN_WORDS_MAX 1024
+int vcl_llm_set_bans(vcl_handle* h, int n, const int32_t* clips_host, const int32_t* ngram_host,
+                     const int32_t* eos_host, const int32_t* eos_from_col_host, const int32_t* words_host,
+                     void* stream);
+
+/* Entry `entry`'s token history, columns 0 .. n - 1, becomes ids[0 .. n) (DEVICE int64), in one kernel on `stream`;
+ * the sampler of a banning entry writes each token it picks at its column. Set it wherever the entry's row of input_ids
+ * changes other than by a drawn token: before the call that draws its first token, and again after anything that
+ * draws into it a token the row does not keep (a chunk of a chunked prompt). Rejected before any device work: an
+ * entry outside 0 .. max_batch-1, n outside 0 .. max_seq + 1, null ids with n > 0, a vocabulary over
+ * VCL_SAMPLE_WIDE_MAX_V. */
+int vcl_llm_set_token_history(vcl_handle* h, int entry, const int64_t* ids, int n, void* stream);
+
+/* Copy columns first_col .. first_col + count - 1 of entry `entry`'s token history (int32) to out (host or device
+ * memory), ordered on `stream`. Rejected: a null argument, an entry or columns outside the history, a handle that never
+ * allocated its histories. */
+int vcl_llm_read_token_history(vcl_handle* h, int entry, int first_col, int count, int32_t* out, void* stream);
+
 /* Log-probabilities of generated tokens: what HF returns as generate(output_scores=True) followed by
  * compute_transition_scores(sequences, scores, normalize_logits=True) ($TF/generation/utils.py), plus the top-n
  * alternatives of each step, computed on the device by the sampler next to the token it picks. For the token of
@@ -522,6 +564,17 @@ int vcl_op_sample_ex(const float* logits, int64_t ld, int B, int V, const float*
                      const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
                      const float* top_p_host, const float* repetition_penalty_host, uint32_t* token_sets,
                      const int32_t* top_n_host, int32_t* tok_out, int32_t* ids_out, float* lp_out, void* stream);
+/* The 32-bit sampler with the ban stage on its own (vcl_llm_set_bans): vcl_op_sample_ex where row b also has a token
+ * history histories[b * hist_ld ..] (device int32), and the ban settings ngram_host[b], eos_host[b],
+ * eos_from_col_host[b] and words_host[b * VCL_BAN_WORDS_MAX ..] (HOST memory, vcl_llm_set_bans' format). Row b draws
+ * at column counter_host[b] (< hist_ld) and writes its token there. Its tokens and log-probs equal vcl_op_sample_ex's
+ * on the same row with the banned ids' logits set to -inf, bit for bit. */
+int vcl_op_sample_bans(const float* logits, int64_t ld, int B, int V, const float* temperature_host,
+                       const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
+                       const float* top_p_host, const float* repetition_penalty_host, uint32_t* token_sets,
+                       int32_t* histories, int64_t hist_ld, const int32_t* ngram_host, const int32_t* eos_host,
+                       const int32_t* eos_from_col_host, const int32_t* words_host, const int32_t* top_n_host,
+                       int32_t* tok_out, int32_t* ids_out, float* lp_out, void* stream);
 /* One beam-search step on its own (vcl_llm_beam_start's rules): B items of num_beams beams, beam r = i * num_beams +
  * j reading logits row r [ld] (device f32, bf16 values) with the running score scores[r] (device f32). last_step:
  * every candidate hits (the max-length step). records_out [B][2 num_beams] and picks_out [B][num_beams] on the device.

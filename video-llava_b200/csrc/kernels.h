@@ -179,8 +179,22 @@ struct SampleArgs {
   long long lp_entry = 0, lp_pos = 0; int lp_rows = 0;
   const float* top_p = nullptr; const float* rep = nullptr;
   unsigned int* tset = nullptr; int tset_words = 0;
+  // Banned tokens (32-bit path, bans set): entry t's row of the ban table, bans + t * VCL_BAN_ROW: {n-gram size (0:
+  // off), EOS id, the first column at which EOS is allowed, w = the int32 used of its bad-words list}, then the list
+  // at [4 .. 4 + w): records (-L, id_0 .. id_{L-1}), the length negated so that any thread can tell a record's start.
+  // hist[t * hist_ld ..] is the entry's token history (HF's input_ids of its row, cache column = index); the
+  // sampler bans the tokens of the rules at the top of sampling.cu for a draw at column c (< hist_ld) and writes the
+  // token it picks at hist[t * hist_ld + c].
+  int* hist = nullptr; long long hist_ld = 0;
+  const int* bans = nullptr;
 };
+#ifndef VCL_BAN_WORDS_MAX
+#define VCL_BAN_WORDS_MAX 1024   // include/vcl.h
+#endif
+constexpr int VCL_BAN_ROW = 4 + VCL_BAN_WORDS_MAX;
 int launch_sample(const SampleArgs& a, cudaStream_t stream);
+// one token history: dst[i] = (int32) ids[i] for i in 0 .. n (device int64), in one launch
+int launch_token_history(int* dst, const long long* ids, int n, cudaStream_t stream);
 // one token set: dst[0 .. words) cleared, then the bits of ids[0 .. n) (device int64; ids outside 0 .. V-1 ignored)
 // set, in one launch
 int launch_token_set(unsigned int* dst, int words, const long long* ids, int n, int V, cudaStream_t stream);

@@ -37,6 +37,13 @@
 //          passes, then the top-p threshold; V <= VCL_SAMPLE_WIDE_MAX_V. For r = 1 and p = 1 its tokens and
 //          log-probs are the 16-bit instance's bit for bit (z of a larger x is never smaller, so the k-th largest z
 //          is fp32(k-th largest x / T)). The sampler adds the token it picks to the entry's token set.
+//          With a ban table (SampleArgs::bans) it also bans tokens, HF's NoRepeatNGram / NoBadWords /
+//          MinNewTokensLength processors over the entry's token history h[0 .. c) for a draw at cache column c:
+//            n-gram n > 0   h[i + n - 1] for every i in 0 .. c - n with h[i .. i + n - 2] = h[c - n + 1 .. c - 1]
+//            bad words      a one-id word always; a word w of L > 1 ids: w[L - 1] when L <= c and h ends with w[:-1]
+//            EOS            while c < the entry's eos_from_col
+//          A banned token's x' is -inf (after the penalty; the arg-max fallback, the maximum, top-k, top-p, the draw
+//          and the log-probs follow), and the token picked is written at h[c] (DESIGN.md section 3, "Banned tokens").
 #include <math.h>
 
 #include <type_traits>
@@ -191,6 +198,49 @@ sample_kernel(SampleArgs a) {
     rep = a.rep[t];
     if (a.tset != nullptr) tset = a.tset + (long long)t * a.tset_words;
   }
+  // the cache column the token takes (its RoPE position plus the entry's left padding)
+  const int col = a.col + (a.col_dev != nullptr ? a.col_dev[r] : 0);
+
+  // banned tokens (32-bit path, a ban table; DESIGN.md section 3, "Banned tokens"): the staged row is cleared, each
+  // banned id is marked (a nonzero key), and the staging below reads the mark before it overwrites it, staging
+  // x' = -inf there. The history h[0 .. col) is read from global memory, the logits row is never written
+  bool ban_row = false;
+  if constexpr (WIDE) {
+    if (a.bans != nullptr) {
+      const int* bt = a.bans + (long long)t * VCL_BAN_ROW;
+      const int ng = bt[0], eos = bt[1], nw = bt[3];
+      const bool eos_ban = eos >= 0 && col < bt[2];
+      if (ng > 0 || eos_ban || nw > 0) {
+        ban_row = true;
+        for (int i = tid; i < V; i += SM_THREADS) skey[i] = 0u;
+        __syncthreads();
+        const int* h = a.hist + (long long)t * a.hist_ld;
+        auto mark = [&](int id) {
+          if (id >= 0 && id < V) skey[id] = 1u;
+        };
+        if (tid == 0 && eos_ban) mark(eos);
+        // n-gram: ban h[i + n - 1] for every i in 0 .. col - n with h[i .. i + n - 2] = h[col - n + 1 .. col - 1]
+        for (int i = tid; i <= col - ng; i += SM_THREADS) {
+          int j = 0;
+          while (j < ng - 1 && h[i + j] == h[col - ng + 1 + j]) ++j;
+          if (j == ng - 1) mark(h[i + ng - 1]);
+        }
+        // bad words: a one-id word always; a word of L <= col ids when h[col - L + 1 .. col - 1] is its prefix
+        for (int i = tid; i < nw; i += SM_THREADS) {
+          const int* w = bt + 4 + i;
+          const int L = -w[0];
+          if (L == 1) {
+            mark(w[1]);
+          } else if (L > 1 && L <= col) {
+            int j = 0;
+            while (j < L - 1 && w[1 + j] == h[col - L + 1 + j]) ++j;
+            if (j == L - 1) mark(w[L]);
+          }
+        }
+        __syncthreads();
+      }
+    }
+  }
 
   // stage the keys; the largest key with its lowest index (the arg-max, packed so that a max-reduce finds it). The
   // 32-bit path also finds the arg-max of x' itself: z = x' / T can tie (or overflow) where x' does not, and the
@@ -213,6 +263,7 @@ sample_kernel(SampleArgs a) {
           float xp = v[u];
           if (rep != 1.f && tset != nullptr && ((__ldg(tset + (i >> 5)) >> (i & 31)) & 1u))
             xp = xp < 0.f ? __fmul_rn(xp, rep) : __fdiv_rn(xp, rep);
+          if (ban_row && skey[i] != 0u) xp = -INFINITY;
           k = order_key32(__fdiv_rn(xp, T_stage));
           const unsigned long long px = ((unsigned long long)order_key32(xp) << 32) | (0xffffffffu - (uint32_t)i);
           best_x = px > best_x ? px : best_x;
@@ -252,11 +303,13 @@ sample_kernel(SampleArgs a) {
     amax = (uint32_t)(best_x >> 32) > KEY32_NEG_INF ? (int)(0xffffffffu - (uint32_t)best_x) : 0;
   }
 
-  // the token: to the output, and on the 32-bit path into the entry's token set (one row per entry and launch)
+  // the token: to the output, and on the 32-bit path into the entry's token set and its history (one row per entry
+  // and launch)
   auto emit = [&](int tok) {
     a.out[(long long)r * a.out_stride] = tok;
     if constexpr (WIDE) {
       if (a.tset != nullptr) atomicOr(a.tset + (long long)t * a.tset_words + (tok >> 5), 1u << (tok & 31));
+      if (a.hist != nullptr && col >= 0 && col < a.hist_ld) a.hist[(long long)t * a.hist_ld + col] = tok;
     }
   };
 
@@ -270,9 +323,7 @@ sample_kernel(SampleArgs a) {
     if constexpr (WIDE) return key_value32(key);
     else return __fdiv_rn(key_value(key), T);
   };
-  auto position = [&]() {
-    return a.col + (a.col_dev != nullptr ? a.col_dev[r] : 0) - (a.n_pad != nullptr ? a.n_pad[t] : 0);
-  };
+  auto position = [&]() { return col - (a.n_pad != nullptr ? a.n_pad[t] : 0); };
   const float zmax = zval(kmax);
   if ((greedy && n_lp < 0) || !isfinite(zmax)) {   // greedy entry, or no finite scaled maximum: the arg-max
     if (tid == 0) emit(amax);
@@ -395,6 +446,12 @@ __global__ void token_set_kernel(uint32_t* dst, int words, const long long* ids,
   }
 }
 
+// dst[i] = ids[i] for i in 0 .. n (a token history, vcl_llm_set_token_history)
+__global__ void token_history_kernel(int* dst, const long long* ids, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = (int)ids[i];
+}
+
 }  // namespace
 
 int launch_sample(const SampleArgs& a, cudaStream_t stream) {
@@ -406,6 +463,8 @@ int launch_sample(const SampleArgs& a, cudaStream_t stream) {
   VCL_REQUIRE(a.top_n == nullptr || (a.lp_id && a.lp_val), "sample: log-probs need their outputs");
   VCL_REQUIRE(!wide || (a.rep && (a.tset == nullptr || a.tset_words >= (a.V + 31) / 32)),
               "sample: the 32-bit path needs the repetition penalties and a token set of %d words", (a.V + 31) / 32);
+  VCL_REQUIRE(a.bans == nullptr || (wide && a.hist != nullptr && a.hist_ld > 0),
+              "sample: a ban table needs the 32-bit path and the token histories");
   if (a.B == 0) return 0;
   if (wide) {
     static bool attr = false;
@@ -426,6 +485,14 @@ int launch_sample(const SampleArgs& a, cudaStream_t stream) {
     const size_t smem = ((size_t)a.V * 2 + 15) / 16 * 16;
     sample_kernel<false><<<a.B, SM_THREADS, smem, stream>>>(a);
   }
+  VCL_CUDA_OK(cudaGetLastError());
+  count_launches(1);
+  return 0;
+}
+
+int launch_token_history(int* dst, const long long* ids, int n, cudaStream_t stream) {
+  if (n == 0) return 0;
+  token_history_kernel<<<(n + 255) / 256, 256, 0, stream>>>(dst, ids, n);
   VCL_CUDA_OK(cudaGetLastError());
   count_launches(1);
   return 0;

@@ -61,7 +61,8 @@ struct GraphEntry {
   int B, n_new;        // the positions and pad counts are read on the device (h->d_pos, h->d_npad) ...
   int sampled;         // ... and so is the sampling table: a graph of the sampler serves every temperature / top_k /
                        // seed / top_n (h->sampler: 0 the arg-max, 1 the 16-bit sampler, 2 the 32-bit one, whose
-                       // graphs serve every top_p / repetition penalty too)
+                       // graphs serve every top_p / repetition penalty too, 3 the 32-bit one with the ban table and
+                       // the token histories, whose graphs serve every ban setting)
   int beam;            // beam search with this many beams per item (0: none); its step counter, scores and clip map
                        // are read on the device too (vcl_llm_beam_decode)
   cudaGraphExec_t exec;
@@ -158,10 +159,11 @@ struct vcl_handle {
   float* samp_topp(unsigned char* base) const { return reinterpret_cast<float*>(base + 20 * cfg.max_batch); }
   float* samp_rep(unsigned char* base) const { return reinterpret_cast<float*>(base + 24 * cfg.max_batch); }
   // what entry b needs: 0 the arg-max, 1 the sampler (it samples, with a temperature above 0, or wants log-probs),
-  // 2 the 32-bit sampler (a repetition penalty, or top-p on a sampled entry)
+  // 2 the 32-bit sampler (a repetition penalty, or top-p on a sampled entry), 3 the 32-bit sampler with bans
   int sampler_of(int b) {
     unsigned char* hb = samp_host.data();
     const float T = samp_temp(hb)[b];
+    if (!bans_host.empty() && ban_on(b)) return 3;
     if (samp_rep(hb)[b] != 1.f || (T > 0.f && samp_topp(hb)[b] < 1.f)) return 2;
     return T > 0.f || samp_topn(hb)[b] >= 0 ? 1 : 0;
   }
@@ -175,6 +177,17 @@ struct vcl_handle {
   // [max_batch][tset_words()], allocated by the first call that turns a penalty on or sets a token set
   unsigned int* tset = nullptr;
   int tset_words() const { return (cfg.vocab + 31) / 32; }
+  // Banned tokens (vcl_llm_set_bans, vcl_llm_set_token_history): the ban table [max_batch][VCL_BAN_ROW] int32
+  // (kernels.h: SampleArgs::bans; all zero: off), bans_host its host copy, and the token histories [max_batch]
+  // [lp_rows()] int32, both at fixed addresses and allocated by the first call that turns a ban on or writes a
+  // history (a handle that never bans holds neither)
+  int* bans = nullptr;
+  std::vector<int> bans_host;
+  int* hist = nullptr;
+  bool ban_on(int b) const {
+    const int* e = bans_host.data() + (size_t)b * VCL_BAN_ROW;
+    return e[0] > 0 || e[1] >= 0 || e[3] > 0;
+  }
   // The log-prob buffer: two planes, int32 ids then f32 log-probs, each [max_batch][lp_rows()][1 + VCL_LOGPROBS_MAX],
   // indexed by entry and the RoPE position of the token (so a read is one contiguous copy per plane); allocated by the
   // first vcl_llm_set_logprobs that turns an entry on.
@@ -749,9 +762,12 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
       sa.lp_entry = (long long)h->lp_rows() * (1 + VCL_LOGPROBS_MAX); sa.lp_pos = 1 + VCL_LOGPROBS_MAX;
       sa.lp_rows = h->lp_rows();
     }
-    if (smp.on == 2) {   // the 32-bit sampler: top_p, the penalties and the token sets
+    if (smp.on >= 2) {   // the 32-bit sampler: top_p, the penalties and the token sets
       sa.top_p = h->samp_topp(h->samp); sa.rep = h->samp_rep(h->samp);
       sa.tset = h->tset; sa.tset_words = h->tset_words();
+    }
+    if (smp.on == 3) {   // ... and the bans, over the token histories
+      sa.bans = h->bans; sa.hist = h->hist; sa.hist_ld = h->lp_rows();
     }
     return launch_sample(sa, st);
   }
@@ -1445,7 +1461,7 @@ static int ensure_token_sets(vcl_handle* h, cudaStream_t st) {
   VCL_TRY(dalloc(h, &h->tset, words));
   VCL_CUDA_OK(cudaMemsetAsync(h->tset, 0, words * 4, st));
   for (size_t i = h->graphs.size(); i-- > 0;)
-    if (h->graphs[i].sampled == 2) {
+    if (h->graphs[i].sampled >= 2) {
       cudaGraphExecDestroy(h->graphs[i].exec);
       h->graphs.erase(h->graphs.begin() + i);
     }
@@ -1505,6 +1521,106 @@ int vcl_llm_set_token_set(vcl_handle* h, int entry, const int64_t* ids, int n, v
   VCL_TRY(ensure_token_sets(h, st));
   return launch_token_set(h->tset + (size_t)entry * h->tset_words(), h->tset_words(),
                           reinterpret_cast<const long long*>(ids), n, h->cfg.vocab, st);
+}
+
+// the ban table (every entry off) and the token histories, on first use
+static int ensure_bans(vcl_handle* h, cudaStream_t st) {
+  if (h->bans != nullptr) return 0;
+  const size_t n = (size_t)h->cfg.max_batch * VCL_BAN_ROW;
+  VCL_TRY(dalloc(h, &h->bans, n));
+  VCL_TRY(dalloc(h, &h->hist, (size_t)h->cfg.max_batch * h->lp_rows()));
+  VCL_CUDA_OK(cudaMemsetAsync(h->bans, 0, n * 4, st));
+  VCL_CUDA_OK(cudaMemsetAsync(h->hist, 0, (size_t)h->cfg.max_batch * h->lp_rows() * 4, st));
+  h->bans_host.assign(n, 0);
+  for (int b = 0; b < h->cfg.max_batch; ++b) h->bans_host[(size_t)b * VCL_BAN_ROW + 1] = -1;
+  return 0;
+}
+
+// One entry's ban settings checked and packed into its ban-table row `row` (kernels.h: SampleArgs::bans); words:
+// VCL_BAN_WORDS_MAX int32, records (L, id_0 .. id_{L-1}) up to an L of 0 or the end
+static int pack_bans(const char* name, int b, int V, int ngram, int eos, int eos_from, const int32_t* words,
+                     int* row) {
+  VCL_REQUIRE(ngram >= 0, "%s: no_repeat_ngram_size %d of entry %d is negative", name, ngram, b);
+  VCL_REQUIRE(eos >= -1 && eos < V, "%s: eos %d of entry %d outside -1..%d", name, eos, b, V - 1);
+  VCL_REQUIRE(eos_from >= 0, "%s: eos_from_col %d of entry %d is negative", name, eos_from, b);
+  int w = 0;
+  while (w < VCL_BAN_WORDS_MAX && words[w] != 0) {
+    const int L = words[w];
+    VCL_REQUIRE(L > 0 && L < VCL_BAN_WORDS_MAX - w, "%s: entry %d: bad word at %d of length %d overruns the list of "
+                "%d int32 (VCL_BAN_WORDS_MAX)", name, b, w, L, VCL_BAN_WORDS_MAX);
+    for (int j = 1; j <= L; ++j)
+      VCL_REQUIRE(words[w + j] >= 0 && words[w + j] < V, "%s: entry %d: bad-word id %d outside 0..%d", name, b,
+                  words[w + j], V - 1);
+    w += 1 + L;
+  }
+  row[0] = ngram; row[1] = eos; row[2] = eos_from; row[3] = w;
+  for (int i = 0; i < w; ++i) row[4 + i] = words[i];
+  for (int i = 0; i < w; i += 1 + words[i]) row[4 + i] = -words[i];   // the lengths negated (record starts)
+  for (int i = w; i < VCL_BAN_WORDS_MAX; ++i) row[4 + i] = 0;
+  return 0;
+}
+
+int vcl_llm_set_bans(vcl_handle* h, int n, const int32_t* clips_host, const int32_t* ngram_host,
+                     const int32_t* eos_host, const int32_t* eos_from_col_host, const int32_t* words_host,
+                     void* stream) {
+  VCL_REQUIRE(h != nullptr, "vcl_llm_set_bans: null handle");
+  const int mb = h->cfg.max_batch;
+  VCL_REQUIRE(n >= 1 && n <= mb, "vcl_llm_set_bans: n=%d outside 1..%d", n, mb);
+  VCL_REQUIRE(clips_host && ngram_host && eos_host && eos_from_col_host && words_host,
+              "vcl_llm_set_bans: null argument");
+  std::vector<int> rows((size_t)n * VCL_BAN_ROW);
+  bool on = false;
+  int lo = mb, hi = -1;
+  for (int i = 0; i < n; ++i) {
+    const int b = clips_host[i];
+    VCL_REQUIRE(b >= 0 && b < mb, "vcl_llm_set_bans: clip %d outside 0..%d", b, mb - 1);
+    for (int j = 0; j < i; ++j) VCL_REQUIRE(clips_host[j] != b, "vcl_llm_set_bans: clip %d is given twice", b);
+    int* row = rows.data() + (size_t)i * VCL_BAN_ROW;
+    VCL_TRY(pack_bans("vcl_llm_set_bans", b, h->cfg.vocab, ngram_host[i], eos_host[i], eos_from_col_host[i],
+                      words_host + (size_t)i * VCL_BAN_WORDS_MAX, row));
+    const bool e_on = row[0] > 0 || row[1] >= 0 || row[3] > 0;
+    VCL_REQUIRE(!e_on || h->cfg.vocab <= VCL_SAMPLE_WIDE_MAX_V, "vcl_llm_set_bans: clip %d: bans take a vocabulary "
+                "of at most %d tokens (the sampler's shared memory), this model has %d", b, VCL_SAMPLE_WIDE_MAX_V,
+                h->cfg.vocab);
+    on = on || e_on;
+    lo = std::min(lo, b); hi = std::max(hi, b);
+  }
+  if (!on && h->bans == nullptr) return 0;   // every entry is off already
+  cudaStream_t st = as_stream(stream);
+  VCL_TRY(ensure_bans(h, st));
+  for (int i = 0; i < n; ++i)
+    memcpy(h->bans_host.data() + (size_t)clips_host[i] * VCL_BAN_ROW, rows.data() + (size_t)i * VCL_BAN_ROW,
+           VCL_BAN_ROW * 4);
+  const size_t off = (size_t)lo * VCL_BAN_ROW;
+  VCL_CUDA_OK(cudaMemcpyAsync(h->bans + off, h->bans_host.data() + off, (size_t)(hi - lo + 1) * VCL_BAN_ROW * 4,
+                              cudaMemcpyHostToDevice, st));
+  return 0;
+}
+
+int vcl_llm_set_token_history(vcl_handle* h, int entry, const int64_t* ids, int n, void* stream) {
+  VCL_REQUIRE(h != nullptr, "vcl_llm_set_token_history: null handle");
+  VCL_REQUIRE(entry >= 0 && entry < h->cfg.max_batch, "vcl_llm_set_token_history: entry %d outside 0..%d", entry,
+              h->cfg.max_batch - 1);
+  VCL_REQUIRE(n >= 0 && n <= h->lp_rows() && (n == 0 || ids != nullptr), "vcl_llm_set_token_history: n=%d outside "
+              "0..%d, or null ids", n, h->lp_rows());
+  VCL_REQUIRE(h->cfg.vocab <= VCL_SAMPLE_WIDE_MAX_V, "vcl_llm_set_token_history: bans take a vocabulary of at most "
+              "%d tokens, this model has %d", VCL_SAMPLE_WIDE_MAX_V, h->cfg.vocab);
+  cudaStream_t st = as_stream(stream);
+  VCL_TRY(ensure_bans(h, st));
+  return launch_token_history(h->hist + (size_t)entry * h->lp_rows(), reinterpret_cast<const long long*>(ids), n, st);
+}
+
+int vcl_llm_read_token_history(vcl_handle* h, int entry, int first_col, int count, int32_t* out, void* stream) {
+  VCL_REQUIRE(h && out, "vcl_llm_read_token_history: null argument");
+  VCL_REQUIRE(entry >= 0 && entry < h->cfg.max_batch, "vcl_llm_read_token_history: entry %d outside 0..%d", entry,
+              h->cfg.max_batch - 1);
+  VCL_REQUIRE(first_col >= 0 && count >= 0 && first_col + count <= h->lp_rows(), "vcl_llm_read_token_history: "
+              "columns %d .. %d outside 0..%d", first_col, first_col + count - 1, h->lp_rows() - 1);
+  VCL_REQUIRE(h->hist != nullptr, "vcl_llm_read_token_history: no history was ever set for this handle "
+              "(vcl_llm_set_token_history, or a ban in vcl_llm_set_bans)");
+  VCL_CUDA_OK(cudaMemcpyAsync(out, h->hist + (size_t)entry * h->lp_rows() + first_col, (size_t)count * 4,
+                              cudaMemcpyDefault, as_stream(stream)));
+  return 0;
 }
 
 int vcl_llm_read_token_set(vcl_handle* h, int entry, uint32_t* bits_out, void* stream) {
@@ -1794,7 +1910,10 @@ namespace {
 int op_sample(const char* name, const float* logits, int64_t ld, int B, int V, const float* temperature_host,
               const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
               const int32_t* top_n_host, int32_t* tok_out, int32_t* ids_out, float* lp_out, void* stream,
-              const float* top_p_host = nullptr, const float* rep_host = nullptr, uint32_t* tset = nullptr) {
+              const float* top_p_host = nullptr, const float* rep_host = nullptr, uint32_t* tset = nullptr,
+              int32_t* hist = nullptr, int64_t hist_ld = 0, const int32_t* ngram_host = nullptr,
+              const int32_t* eos_host = nullptr, const int32_t* eos_from_host = nullptr,
+              const int32_t* words_host = nullptr) {
   if (check_device() != 0) return -2;
   VCL_REQUIRE(logits && temperature_host && top_k_host && seed_host && counter_host && tok_out, "%s: null argument",
               name);
@@ -1817,8 +1936,19 @@ int op_sample(const char* name, const float* logits, int64_t ld, int B, int V, c
     for (int b = 0; b < B; ++b)
       VCL_REQUIRE(top_n_host[b] >= -1 && top_n_host[b] <= VCL_LOGPROBS_MAX, "%s: row %d: top_n %d outside -1..%d",
                   name, b, top_n_host[b], VCL_LOGPROBS_MAX);
-  // the per-row settings in one stream-ordered block: [B] seeds, temperatures, top_k, counters, top_n, top_p, penalties
-  std::vector<unsigned char> hb((size_t)B * (wide ? 32 : 24));
+  // the per-row settings in one stream-ordered block: [B] seeds, temperatures, top_k, counters, top_n, top_p,
+  // penalties, then the ban table [B][VCL_BAN_ROW]
+  const bool bans = hist != nullptr;
+  std::vector<unsigned char> hb((size_t)B * (wide ? 32 : 24) + (bans ? (size_t)B * VCL_BAN_ROW * 4 : 0));
+  if (bans) {
+    for (int b = 0; b < B; ++b) {
+      VCL_REQUIRE(counter_host[b] < hist_ld, "%s: row %d: column %d outside the history of %lld columns", name, b,
+                  counter_host[b], (long long)hist_ld);
+      VCL_TRY(pack_bans(name, b, V, ngram_host[b], eos_host[b], eos_from_host[b],
+                        words_host + (size_t)b * VCL_BAN_WORDS_MAX,
+                        reinterpret_cast<int*>(hb.data() + (size_t)B * 32) + (size_t)b * VCL_BAN_ROW));
+    }
+  }
   memcpy(hb.data(), seed_host, (size_t)B * 8);
   memcpy(hb.data() + (size_t)B * 8, temperature_host, (size_t)B * 4);
   memcpy(hb.data() + (size_t)B * 12, top_k_host, (size_t)B * 4);
@@ -1847,6 +1977,10 @@ int op_sample(const char* name, const float* logits, int64_t ld, int B, int V, c
     sa.top_p = reinterpret_cast<const float*>(d + (size_t)B * 24);
     sa.rep = reinterpret_cast<const float*>(d + (size_t)B * 28);
     sa.tset = tset; sa.tset_words = (V + 31) / 32;
+  }
+  if (bans) {   // row b: entry b, its history hist[b * hist_ld ..] and the draw at column counter[b]
+    sa.bans = reinterpret_cast<const int*>(d + (size_t)B * 32);
+    sa.hist = hist; sa.hist_ld = hist_ld;
   }
   const int rc = launch_sample(sa, st);
   VCL_CUDA_OK(cudaFreeAsync(d, st));
@@ -1913,6 +2047,21 @@ int vcl_op_sample_ex(const float* logits, int64_t ld, int B, int V, const float*
   VCL_REQUIRE(top_n_host == nullptr || (ids_out && lp_out), "vcl_op_sample_ex: log-probs need ids_out and lp_out");
   return op_sample("vcl_op_sample_ex", logits, ld, B, V, temperature_host, top_k_host, seed_host, counter_host,
                    top_n_host, tok_out, ids_out, lp_out, stream, top_p_host, repetition_penalty_host, token_sets);
+}
+
+int vcl_op_sample_bans(const float* logits, int64_t ld, int B, int V, const float* temperature_host,
+                       const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
+                       const float* top_p_host, const float* repetition_penalty_host, uint32_t* token_sets,
+                       int32_t* histories, int64_t hist_ld, const int32_t* ngram_host, const int32_t* eos_host,
+                       const int32_t* eos_from_col_host, const int32_t* words_host, const int32_t* top_n_host,
+                       int32_t* tok_out, int32_t* ids_out, float* lp_out, void* stream) {
+  VCL_REQUIRE(top_p_host && repetition_penalty_host && histories && ngram_host && eos_host && eos_from_col_host &&
+              words_host, "vcl_op_sample_bans: null argument");
+  VCL_REQUIRE(hist_ld >= 1, "vcl_op_sample_bans: hist_ld=%lld", (long long)hist_ld);
+  VCL_REQUIRE(top_n_host == nullptr || (ids_out && lp_out), "vcl_op_sample_bans: log-probs need ids_out and lp_out");
+  return op_sample("vcl_op_sample_bans", logits, ld, B, V, temperature_host, top_k_host, seed_host, counter_host,
+                   top_n_host, tok_out, ids_out, lp_out, stream, top_p_host, repetition_penalty_host, token_sets,
+                   histories, hist_ld, ngram_host, eos_host, eos_from_col_host, words_host);
 }
 
 int vcl_op_layernorm(const void* x, void* y, const void* w, const void* b, int rows, int D, float eps,

@@ -138,6 +138,10 @@ _SIGNATURES = {
                                         POINTER(c_uint64), POINTER(c_float), POINTER(c_float), c_void_p]),
     "vcl_llm_set_token_set": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "vcl_llm_read_token_set": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "vcl_llm_set_bans": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32),
+                                 POINTER(c_int32), POINTER(c_int32), c_void_p]),
+    "vcl_llm_set_token_history": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),
+    "vcl_llm_read_token_history": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "vcl_llm_set_logprobs": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), c_void_p]),
     "vcl_llm_read_logprobs": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_llm_beam_start": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_int, c_int,
@@ -161,6 +165,10 @@ _SIGNATURES = {
                                c_int64, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "vcl_op_sample": (c_int, [c_void_p, c_int64, c_int, c_int, POINTER(c_float), POINTER(c_int32), POINTER(c_uint64),
                               POINTER(c_int32), c_void_p, c_void_p]),
+    "vcl_op_sample_bans": (c_int, [c_void_p, c_int64, c_int, c_int, POINTER(c_float), POINTER(c_int32),
+                                   POINTER(c_uint64), POINTER(c_int32), POINTER(c_float), POINTER(c_float), c_void_p,
+                                   c_void_p, c_int64, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32),
+                                   POINTER(c_int32), POINTER(c_int32), c_void_p, c_void_p, c_void_p, c_void_p]),
     "vcl_op_sample_logprobs": (c_int, [c_void_p, c_int64, c_int, c_int, POINTER(c_float), POINTER(c_int32),
                                        POINTER(c_uint64), POINTER(c_int32), POINTER(c_int32), c_void_p, c_void_p,
                                        c_void_p, c_void_p]),
@@ -372,6 +380,55 @@ def op_sample_ex(logits, temperature, top_k, seed, counter, top_p, repetition_pe
                                  _seeds(seed, B), ints(vals[2]), flts(vals[3]), flts(vals[4]), ptr(token_sets),
                                  ints(vals[5]) if top_n is not None else None, ptr(out), ptr(ids), ptr(lp),
                                  cur_stream()))
+    return out if top_n is None else (out, ids, lp)
+
+
+BAN_WORDS_MAX = 1024          # include/vcl.h: VCL_BAN_WORDS_MAX, the int32 of one entry's bad-words list
+
+
+def ban_words(words):
+    """A list of bad words (each a non-empty list of ids) -> the BAN_WORDS_MAX int32 of vcl_llm_set_bans' format:
+    records (L, id_0 .. id_{L-1}), then zeros"""
+    flat = []
+    for w in words:
+        flat += [len(w)] + [int(x) for x in w]
+    if len(flat) > BAN_WORDS_MAX:
+        raise VclError(f"bad words take {len(flat)} int32 (a length and the ids of each word), more than the "
+                       f"{BAN_WORDS_MAX} of one entry")
+    return flat + [0] * (BAN_WORDS_MAX - len(flat))
+
+
+def op_sample_bans(logits, temperature, top_k, seed, counter, top_p, repetition_penalty, histories, ngram, eos,
+                   eos_from_col, words, token_sets=None, top_n=None):
+    """The 32-bit sampler with the ban stage alone (vcl_op_sample_bans): op_sample_ex's arguments plus histories
+    [B, hist_ld] int32 on the device (row b draws at column counter[b] < hist_ld, after h[0 .. counter[b]), and writes
+    its token there), and per row the n-gram size ngram[b] (0: off), eos[b] (-1: off) with eos_from_col[b], and
+    words[b], a list of bad words (lists of ids). Returns what op_sample_ex returns."""
+    B, ld = logits.shape
+    assert logits.dtype == torch.float32 and logits.stride(1) == 1
+    vals = [list(v) for v in (temperature, top_k, counter, top_p, repetition_penalty, ngram, eos, eos_from_col, words)]
+    if top_n is not None:
+        vals.append(list(top_n))
+    if not all(len(v) == B for v in vals):
+        raise VclError(f"every per-row setting needs {B} entries")
+    assert histories.is_cuda and histories.dtype == torch.int32 and histories.dim() == 2 and histories.shape[0] == B
+    assert histories.stride(1) == 1
+    if token_sets is not None:
+        assert token_sets.is_cuda and token_sets.dtype == torch.int32 and token_sets.is_contiguous()
+        assert tuple(token_sets.shape) == (B, token_set_words(ld))
+    out = torch.empty(B, dtype=torch.int32, device=logits.device)
+    ids = lp = None
+    if top_n is not None:
+        ids = torch.full((B, LOGPROB_PLACES), -1, dtype=torch.int32, device=logits.device)
+        lp = torch.full((B, LOGPROB_PLACES), float("nan"), dtype=torch.float32, device=logits.device)
+    ints = lambda v: (c_int32 * len(v))(*[int(x) for x in v])   # noqa: E731
+    flts = lambda v: (c_float * B)(*[float(x) for x in v])   # noqa: E731
+    flat = [x for w in vals[8] for x in ban_words(w)]
+    check(lib().vcl_op_sample_bans(c_void_p(logits.data_ptr()), logits.stride(0), B, ld, flts(vals[0]), ints(vals[1]),
+                                   _seeds(seed, B), ints(vals[2]), flts(vals[3]), flts(vals[4]), ptr(token_sets),
+                                   ptr(histories), histories.stride(0), ints(vals[5]), ints(vals[6]), ints(vals[7]),
+                                   ints(flat), ints(vals[9]) if top_n is not None else None, ptr(out), ptr(ids),
+                                   ptr(lp), cur_stream()))
     return out if top_n is None else (out, ids, lp)
 
 
@@ -766,6 +823,35 @@ class Engine:
         b = bits.cpu().to(torch.int64) & 0xFFFFFFFF
         on = ((b[:, None] >> torch.arange(32)) & 1).reshape(-1)
         return on.nonzero()[:, 0]
+
+    # ---- banned tokens ----
+    def set_bans(self, clips, ngram, eos, eos_from_col, words):
+        """Entries `clips` of the ban table (vcl_llm_set_bans): clip / slot clips[i] bans by the n-gram size ngram[i]
+        (0: off), EOS eos[i] (-1: off) before column eos_from_col[i], and the bad words words[i] (a list of lists of
+        ids). Host lists of equal length."""
+        n = len(clips)
+        if not (len(ngram) == len(eos) == len(eos_from_col) == len(words) == n):
+            raise VclError(f"{n} clips, {len(ngram)} ngram, {len(eos)} eos, {len(eos_from_col)} eos_from_col, "
+                           f"{len(words)} words")
+        ints = lambda v: (c_int32 * len(v))(*[int(x) for x in v])   # noqa: E731
+        flat = [x for w in words for x in ban_words(w)]
+        check(lib().vcl_llm_set_bans(self._h, n, ints(clips), ints(ngram), ints(eos), ints(eos_from_col), ints(flat),
+                                     cur_stream()))
+
+    def set_token_history(self, entry, ids):
+        """Entry `entry`'s token history, columns 0 .. len(ids) - 1, becomes `ids` (any int tensor or list;
+        vcl_llm_set_token_history)"""
+        t = torch.as_tensor(ids).reshape(-1).to(device="cuda", dtype=torch.int64).contiguous()
+        check(lib().vcl_llm_set_token_history(self._h, int(entry), ptr(t) if t.numel() else None, t.numel(),
+                                              cur_stream()))
+
+    def read_token_history(self, entry, first_col, count):
+        """Columns first_col .. first_col + count - 1 of entry `entry`'s token history (vcl_llm_read_token_history)
+        as an int64 tensor on the host"""
+        out = torch.empty(count, dtype=torch.int32, device="cuda")
+        check(lib().vcl_llm_read_token_history(self._h, int(entry), int(first_col), int(count),
+                                               c_void_p(out.data_ptr()), cur_stream()))
+        return out.cpu().to(torch.int64)
 
     # ---- log-probs of generated tokens ----
     sample_logprobs_op = staticmethod(op_sample_logprobs)

@@ -10,7 +10,8 @@ import vcl_native as vn
 
 def request(model, i, r, max_new_tokens, stopping_criteria, n_vid, samp):
     """One request of generate_requests, checked on the host -> (ids [S] int64 on the host, S, n, feats,
-    vid_start, criteria, and its sampling-table entry: temperature (0: greedy), top_k, seed)"""
+    vid_start, criteria, its sampling-table entry: temperature (0: greedy), top_k, seed, top_p, penalty, and its bans
+    (model._ban_args; None: none))"""
     if isinstance(r, torch.Tensor):
         r = {"input_ids": r}
     ids = torch.as_tensor(r["input_ids"]).detach().cpu().to(torch.int64)
@@ -45,8 +46,12 @@ def request(model, i, r, max_new_tokens, stopping_criteria, n_vid, samp):
             k, seed = 0, 0
     if T == 0:
         top_p = 1.0                           # HF adds no warpers when greedy
+    bans = model._ban_args(r.get("no_repeat_ngram_size", samp.get("no_repeat_ngram_size")),
+                           r.get("bad_words_ids", samp.get("bad_words_ids")),
+                           r.get("min_new_tokens", samp.get("min_new_tokens")), samp.get("eos"), f"request {i}")
     return SimpleNamespace(ids=ids, S=S, n=n, feats=feats, vid_start=vs, criteria=list(crit or []),
-                           temperature=T, top_k=k, seed=seed, top_p=top_p, penalty=penalty, session=r.get("session"),
+                           temperature=T, top_k=k, seed=seed, top_p=top_p, penalty=penalty, bans=bans,
+                           session=r.get("session"),
                            continues=r.get("continues"), start=0, lp=r.get("logprobs", samp.get("logprobs")))
 
 
@@ -122,16 +127,21 @@ def request_done(r, gen, eos):
     return len(gen) >= r.n
 
 
-def admit_sampling(model, eng, group, resumed):
+def admit_sampling(model, eng, group, resumed, banning=False, eos=None):
     """The sampling-table entries of the (slot, request) pairs admitted at one point, in one write, and the token
-    set of each penalized one: its ids; for a (slot, request, tokens) of `resumed`, its ids then those tokens."""
+    set of each penalized one: its ids; for a (slot, request, tokens) of `resumed`, its ids then those tokens. Under
+    `banning` (some request of the call bans) also the ban-table entries of every pair, in one write (EOS allowed
+    from column S + min_new_tokens), and the token history of each banning one, from the same ids."""
     rows = list(group) + [(s, r) for s, r, _ in resumed]
     model._set_entries(eng, [s for s, _ in rows], [r.temperature for _, r in rows], [r.top_k for _, r in rows],
                        [r.seed for _, r in rows], [r.top_p for _, r in rows], [r.penalty for _, r in rows])
-    sets = [(s, r.ids) for s, r in group if r.penalty != 1.0]
-    sets += [(s, torch.cat([r.ids, torch.tensor(toks, dtype=torch.int64)])) for s, r, toks in resumed
-             if r.penalty != 1.0]
-    model._token_sets(eng, sets)
+    ids = [(s, r, r.ids) for s, r in group]
+    ids += [(s, r, torch.cat([r.ids, torch.tensor(toks, dtype=torch.int64)])) for s, r, toks in resumed]
+    model._token_sets(eng, [(s, t) for s, r, t in ids if r.penalty != 1.0])
+    if banning:
+        model._set_bans(eng, [s for s, _ in rows], [r.bans for _, r in rows], eos,
+                        [r.S + r.bans.min_new if r.bans else 0 for _, r in rows])
+        model._histories(eng, [(s, t) for s, r, t in ids if r.bans is not None])
 
 
 def prefill(model, eng, group, first, packed):
@@ -160,7 +170,8 @@ def prefill_chunked(model, eng, group, first, packed, sampling, stats):
     prompt of the group goes into one call (at most n_slots * 512 rows, which the activations hold); otherwise
     each prompt runs alone. A slot's first token (first[slot]) is the one its last chunk gives; stats counts the
     prompts and the calls. Every chunk call also draws a token for each of its prompts (only the last one's is
-    kept), which a penalized slot adds to its token set: so the set is written again before each later call."""
+    kept), which a penalized slot adds to its token set and a banning one writes into its history: so both are
+    written again before each later call."""
     dev, L = first.device, model._PACKED_MAX_S
     stats["chunked_prefills"] += len(group)
     for batch in ([group] if packed else [[g] for g in group]):
@@ -168,6 +179,7 @@ def prefill_chunked(model, eng, group, first, packed, sampling, stats):
             live = [(s, r) for s, r in batch if start < r.S]
             if sampling and start > 0:   # (chunk 0 follows the admission's write)
                 model._token_sets(eng, [(s, r.ids) for s, r in live if r.penalty != 1.0])
+                model._histories(eng, [(s, r.ids) for s, r in live if r.bans is not None])
             tok = eng.slots_prefill_chunk([s for s, _ in live], [start] * len(live), [r.S for _, r in live],
                                           [r.ids[start:start + L] for _, r in live],
                                           [None if r.feats is None else r.feats.to(dev) for _, r in live],
@@ -188,6 +200,7 @@ def schedule(model, eng, reqs, n_slots, packed, sampling, eos, chunked, lps):
     results = [None] * len(reqs)
     queue = collections.deque(range(len(reqs)))
     gen = {}                            # request -> its new tokens so far
+    banning = any(r.bans is not None for r in reqs)
     while True:
         admitted, resumed, tails = slots.admit(queue)
         for _, i in admitted + tails:
@@ -196,7 +209,8 @@ def schedule(model, eng, reqs, n_slots, packed, sampling, eos, chunked, lps):
             # a resumed request's token set: its prompt and its tokens, the pending one too when the host has
             # not seen it yet (its prefill's token)
             admit_sampling(model, eng, [(s, reqs[i]) for s, i in admitted + tails],
-                           [(s, reqs[i], gen[i] + ([int(slots.first[s])] if unseen[s] else [])) for s, i in resumed])
+                           [(s, reqs[i], gen[i] + ([int(slots.first[s])] if unseen[s] else [])) for s, i in resumed],
+                           banning, eos)
         lps.sync(owner)
         # continuations: the tails admitted here in one call under packed admission, one call each otherwise
         for group in ([tails] if packed and tails else [[t] for t in tails]):

@@ -30,6 +30,7 @@ from __future__ import annotations
 import contextlib
 import json
 import math
+import numbers
 import os
 import sys
 from types import SimpleNamespace
@@ -728,6 +729,112 @@ class VideoChatGPTLlamaForCausalLM:
         for b, ids in rows:
             eng.set_token_set(b, ids)
 
+    def _ban_args(self, no_repeat_ngram_size, bad_words_ids, min_new_tokens, eos, what="generate", device=True):
+        """Checks the banned-token settings on the host, with HF's messages -> None when none is on, else
+        SimpleNamespace(ngram (0: off), words (the bad words as HF keeps them: [eos] dropped, duplicates once; None when
+        bad_words_ids is None), min_new (0 when off or EOS is disabled), eos). HF adds each processor when: n-gram size > 0,
+        bad_words_ids given, min_new_tokens > 0 with an EOS."""
+        n = 0 if no_repeat_ngram_size is None else no_repeat_ngram_size
+        if isinstance(n, bool) or not isinstance(n, int) or n < 0:
+            raise ValueError(f"{what}: `ngram_size` has to be a strictly positive integer, but is {n}")
+        m = 0 if min_new_tokens is None else min_new_tokens
+        if isinstance(m, bool) or not isinstance(m, int) or m < 0:
+            raise ValueError(f"{what}: `min_new_tokens` has to be a positive integer, but is {m}")
+        words = None
+        if bad_words_ids is not None:
+            b = bad_words_ids
+            if not isinstance(b, list) or len(b) == 0:
+                raise ValueError(f"{what}: `bad_words_ids` has to be a non-empty list, but is {b}.")
+            if any(not isinstance(w, list) for w in b):
+                raise ValueError(f"{what}: `bad_words_ids` has to be a list of lists, but is {b}.")
+            if any(any(isinstance(t, bool) or not isinstance(t, numbers.Integral) or t < 0 for t in w) for w in b):
+                raise ValueError(f"{what}: Each list in `bad_words_ids` has to be a list of positive integers, but is "
+                                 f"{b}.")
+            if any(len(w) == 0 for w in b):
+                raise ValueError(f"{what}: Each list in `bad_words_ids` has to be a non-empty list of token ids, but "
+                                 f"is {b}.")
+            keep = {}                              # HF: {tuple(word): -inf} without [eos], in order
+            for w in b:
+                if eos is None or list(w) != [eos]:
+                    keep.setdefault(tuple(int(t) for t in w), None)
+            V = self.config.vocab_size
+            bad = [t for w in keep for t in w if t >= V]
+            if bad:
+                raise ValueError(f"{what}: The model vocabulary size is {V}, but the following tokens were being "
+                                 f"biased: {bad}")
+            words = [list(w) for w in keep]
+            size = sum(1 + len(w) for w in words)
+            if size > vn.BAN_WORDS_MAX:
+                raise ValueError(f"{what}: bad_words_ids take {size} int32 on the device (a length and the ids of each "
+                                 f"word), more than {vn.BAN_WORDS_MAX}")
+        if eos is None:
+            m = 0                                  # HF adds no MinNewTokensLengthLogitsProcessor without an EOS
+        if n == 0 and words is None and m == 0:
+            return None
+        V = self.config.vocab_size
+        if device and V > vn.SAMPLE_WIDE_MAX_V:
+            raise ValueError(f"{what}: no_repeat_ngram_size, bad_words_ids and min_new_tokens take a vocabulary of at "
+                             f"most {vn.SAMPLE_WIDE_MAX_V} tokens on the device sampler, this model has {V}")
+        return SimpleNamespace(ngram=n, words=words, min_new=m, eos=eos)
+
+    @staticmethod
+    def _set_bans(eng, clips, bans, eos, eos_from):
+        """One ban-table write: clip clips[i] bans by bans[i] (None: off), EOS before column eos_from[i]"""
+        eng.set_bans(clips, [b.ngram if b else 0 for b in bans],
+                     [eos if b and b.min_new else -1 for b in bans], [e if b else 0 for b, e in zip(bans, eos_from)],
+                     [b.words or [] if b else [] for b in bans])
+
+    @contextlib.contextmanager
+    def _banning(self, eng, clips, bans, eos, eos_from):
+        """Entries `clips` ban by `bans` (None: nothing changes) for the duration of the block and are off again
+        afterwards, also when the block raises"""
+        if bans is None:
+            yield
+            return
+        n = len(clips)
+        self._set_bans(eng, clips, [bans] * n, eos, [eos_from] * n)
+        try:
+            yield
+        finally:
+            self._set_bans(eng, clips, [None] * n, eos, [0] * n)
+
+    @staticmethod
+    def _histories(eng, rows):
+        """(entry, ids) pairs: each entry's token history becomes its ids, one call each"""
+        for b, ids in rows:
+            eng.set_token_history(b, ids)
+
+    @staticmethod
+    def _host_bans(out, logits, bans, S):
+        """HF's NoRepeatNGramLogitsProcessor, NoBadWordsLogitsProcessor and MinNewTokensLengthLogitsProcessor, in that
+        order, on logits [B, V] fp32 after the ids `out` [B, c] of a call whose first new token took column S (each
+        as HF computes it: the n-gram and EOS bans assign -inf, the bad words add a bias of 0 / -inf)"""
+        c = out.shape[1]
+        rows = out.tolist()
+        if bans.ngram:
+            n = bans.ngram
+            logits = logits.clone()
+            if c + 1 >= n:
+                for b, h in enumerate(rows):
+                    key = h[c - n + 1:c]
+                    banned = [h[i + n - 1] for i in range(c - n + 1) if h[i:i + n - 1] == key]
+                    logits[b, banned] = float("-inf")
+        if bans.words is not None:
+            bias = torch.zeros_like(logits)
+            for w in bans.words:
+                if len(w) == 1:
+                    bias[:, w[0]] = float("-inf")
+            for w in bans.words:
+                if 1 < len(w) <= c:
+                    for b, h in enumerate(rows):
+                        if h[c - len(w) + 1:] == w[:-1]:
+                            bias[b, w[-1]] += float("-inf")
+            logits = logits + bias
+        if bans.min_new and c - S < bans.min_new:
+            logits = logits.clone()
+            logits[:, bans.eos] = float("-inf")
+        return logits
+
     @staticmethod
     def _logprobs_arg(v, what):
         """Checks a logprobs setting on the host: None (off) or an int 0 .. vn.LOGPROBS_MAX"""
@@ -778,7 +885,8 @@ class VideoChatGPTLlamaForCausalLM:
     def generate(self, input_ids, video_spatio_temporal_features=None, do_sample=False, temperature=1.0,
                  max_new_tokens=32, stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50,
                  attention_mask=None, seed=None, logprobs=None, top_p=1.0, repetition_penalty=1.0, num_beams=1,
-                 num_return_sequences=1, length_penalty=1.0, early_stopping=False, **kw):
+                 num_return_sequences=1, length_penalty=1.0, early_stopping=False, no_repeat_ngram_size=None,
+                 bad_words_ids=None, min_new_tokens=None, **kw):
         """Returns [B, S+n] int64 INCLUDING the prompt, like HF generate (inference.py:105-120), and
         like HF it stops at EOS (config.eos_token_id unless eos_token_id is given; None disables it):
         finished rows are padded, the call returns when every row has finished.
@@ -805,16 +913,24 @@ class VideoChatGPTLlamaForCausalLM:
         negative) the logits of every token of the row's input_ids so far (prompt, padding, new tokens); top-p only
         applies when sampling. Seeded sampling applies both on the device; a greedy call with a penalty takes the
         device loops with greedy entries; unseeded sampling applies them on the host, step by step, as HF does.
+        no_repeat_ngram_size (None or 0: off), bad_words_ids (None: off) and min_new_tokens (None or 0: off): HF's
+        NoRepeatNGramLogitsProcessor, NoBadWordsLogitsProcessor and MinNewTokensLengthLogitsProcessor, checked with
+        HF's messages. They set the logits of banned tokens to -inf after the penalty, over the row's input_ids so far
+        (padding and prompt included); min_new_tokens bans EOS until that many new tokens are out (nothing without
+        an EOS). Seeded sampling and greedy calls apply them on the device (DESIGN.md section 3, "Banned tokens");
+        unseeded sampling on the host, step by step.
         num_beams > 1: HF's beam search (do_sample=False), with HF's num_return_sequences, length_penalty and
         early_stopping (True, False or "never"); see _beam_generate. It returns [B * num_return_sequences, S + m], the
         best hypotheses of each prompt first, and sets self.last_beam_scores (HF's sequences_scores). Sampling, seed,
-        logprobs, top_p, repetition_penalty and stopping criteria are not supported with beams (NotImplementedError), and
+        logprobs, top_p, repetition_penalty, the banned-token settings and stopping criteria are not supported with
+        beams (NotImplementedError), and
         a beam call must fit max_seq whole (S + max_new_tokens <= max_seq: a shorter call would move HF's max-length
         step and so change the search). num_beams must be an int 1 .. 8 on every call (a ValueError otherwise, rather
         than a silently greedy call); num_return_sequences without beams is ignored, as it always was."""
         self._not_paged("generate")
         beams = self._beam_args(num_beams, num_return_sequences, length_penalty, early_stopping, do_sample, seed,
-                                logprobs, top_p, repetition_penalty, stopping_criteria)
+                                logprobs, top_p, repetition_penalty, stopping_criteria,
+                                (no_repeat_ngram_size, bad_words_ids, min_new_tokens))
         if beams is not None:
             return self._beam_generate(input_ids, video_spatio_temporal_features, attention_mask, max_new_tokens,
                                        eos_token_id, pad_token_id, *beams)
@@ -825,6 +941,9 @@ class VideoChatGPTLlamaForCausalLM:
                                       "seed= (unseeded do_sample=True draws from torch's RNG on the host)")
         top_p, penalty = self._nucleus_args(top_p, repetition_penalty, "generate", do_sample,
                                             device=not do_sample or seed is not None)
+        eos, pad = self._eos_pad(eos_token_id, pad_token_id)
+        bans = self._ban_args(no_repeat_ngram_size, bad_words_ids, min_new_tokens, eos, "generate",
+                              device=not do_sample or seed is not None)
         seeded = do_sample and seed is not None
         if seeded:
             temperature, top_k, seed = self._sampling_args(temperature, top_k, seed)
@@ -840,9 +959,8 @@ class VideoChatGPTLlamaForCausalLM:
         n = min(max_new_tokens, self._max_seq - S)
         if n <= 0:
             raise ValueError(f"prompt length {S} leaves no room in max_seq {self._max_seq}")
-        eos, pad = self._eos_pad(eos_token_id, pad_token_id)
         self._pads = pads
-        if seeded or lp_n is not None or (penalty != 1.0 and not do_sample):
+        if seeded or lp_n is not None or ((penalty != 1.0 or bans) and not do_sample):
             clips = list(range(B))
             if seeded:
                 samp = self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips], top_p,
@@ -853,7 +971,10 @@ class VideoChatGPTLlamaForCausalLM:
                 samp = contextlib.nullcontext()
             if penalty != 1.0:
                 self._token_sets(eng, [(b, ids[b]) for b in clips])
-            with samp, self._logprobs(eng, clips, lp_n):
+            if bans:
+                self._histories(eng, [(b, ids[b]) for b in clips])
+            with samp, self._banning(eng, clips, bans, eos, S + (bans.min_new if bans else 0)), \
+                    self._logprobs(eng, clips, lp_n):
                 if eos is None and not stopping_criteria:
                     new = eng.generate(ids, feats, vs, n, n_pad=pads)
                     self._pos = S + n - 1
@@ -869,7 +990,7 @@ class VideoChatGPTLlamaForCausalLM:
             _, logits, _ = eng.prefill(ids, feats, vs, want_logits=True, want_token=False, n_pad=pads)
             self._pos = S
             self._last_out = self._stepwise(eng, ids, logits, n, do_sample, temperature, stopping_criteria, eos, pad,
-                                            top_k, top_p, penalty)
+                                            top_k, top_p, penalty, bans)
             return self._last_out
         if eos is None:
             new = eng.generate(ids, feats, vs, n, n_pad=pads).to(torch.int64)
@@ -898,7 +1019,7 @@ class VideoChatGPTLlamaForCausalLM:
     _BEAM_CHUNK = 16
 
     def _beam_args(self, num_beams, num_return_sequences, length_penalty, early_stopping, do_sample, seed, logprobs,
-                   top_p, repetition_penalty, stopping_criteria):
+                   top_p, repetition_penalty, stopping_criteria, bans=(None, None, None)):
         """Checks the beam-search arguments of generate on the host -> None (no beams), or (num_beams,
         num_return_sequences, length_penalty, early_stopping)"""
         if isinstance(num_beams, bool) or not isinstance(num_beams, int) or num_beams < 1:
@@ -920,7 +1041,8 @@ class VideoChatGPTLlamaForCausalLM:
             raise ValueError(f"generate: length_penalty {length_penalty} must be finite")
         for name, bad in (("do_sample=True", do_sample), ("seed", seed is not None), ("logprobs", logprobs is not None),
                           ("top_p", float(top_p) < 1.0), ("repetition_penalty", float(repetition_penalty) != 1.0),
-                          ("stopping_criteria", bool(stopping_criteria))):
+                          ("stopping_criteria", bool(stopping_criteria)), ("no_repeat_ngram_size", bool(bans[0])),
+                          ("bad_words_ids", bans[1] is not None), ("min_new_tokens", bool(bans[2]))):
             if bad:
                 raise NotImplementedError(f"generate: {name} is not supported with num_beams > 1 (beam search runs "
                                           "greedy, do_sample=False, without logits processors or stopping criteria)")
@@ -1029,7 +1151,8 @@ class VideoChatGPTLlamaForCausalLM:
     @torch.no_grad()
     def generate_requests(self, requests, max_new_tokens=32, eos_token_id="config", stopping_criteria=None,
                           slots=None, do_sample=False, packed_admission=False, temperature=1.0, top_k=50, seed=None,
-                          chunked_prefill=False, logprobs=None, top_p=1.0, repetition_penalty=1.0):
+                          chunked_prefill=False, logprobs=None, top_p=1.0, repetition_penalty=1.0, no_repeat_ngram_size=None,
+                          bad_words_ids=None, min_new_tokens=None):
         """Greedy generation for many independent requests by in-flight (continuous) batching: every request
         owns a slot of the KV cache while it runs, and a finished request's slot takes the next queued one at
         once while the other slots keep decoding (a static batch decodes until its longest row finishes).
@@ -1088,7 +1211,11 @@ class VideoChatGPTLlamaForCausalLM:
         prompt (a continuation: the whole conversation) and its new tokens. The slot's token set is written when the
         request is admitted (before each chunk of a chunked prompt) and rebuilt from the prompt and the tokens the host
         holds when it resumes after a preemption; nothing carries over from the slot's earlier requests. Requests
-        without either setting write the sampling table with set_sampling and launch what they launched before."""
+        without either setting write the sampling table with set_sampling and launch what they launched before.
+        no_repeat_ngram_size / bad_words_ids / min_new_tokens, or a request's own keys of those names: as in generate,
+        on the device, over the request's own input_ids (a continuation: the whole conversation, whose length is where
+        min_new_tokens starts counting). The slot's token history is written where its token set is; a call in which
+        no request bans writes no ban table and launches what it launched before."""
         self._logprobs_arg(logprobs, "generate_requests")
         for i, r in enumerate(requests):
             r = r if isinstance(r, dict) else {}
@@ -1101,6 +1228,11 @@ class VideoChatGPTLlamaForCausalLM:
                                           "sampling in flight needs seed= (the call's or the request's own)")
             self._nucleus_args(r.get("top_p", top_p), r.get("repetition_penalty", repetition_penalty), f"request {i}",
                                r.get("do_sample", do_sample))
+        eos, _ = self._eos_pad(eos_token_id, None)
+        for i, r in enumerate(requests):
+            r = r if isinstance(r, dict) else {}
+            self._ban_args(r.get("no_repeat_ngram_size", no_repeat_ngram_size), r.get("bad_words_ids", bad_words_ids),
+                           r.get("min_new_tokens", min_new_tokens), eos, f"request {i}")
         cap = self._n_slots
         n_slots = cap if slots is None else int(slots)
         if not 1 <= n_slots <= cap:
@@ -1109,14 +1241,15 @@ class VideoChatGPTLlamaForCausalLM:
             raise ValueError(f"slots={slots} outside 1..{cap} (at most 16 and at most max_batch {self._max_batch})")
         eng = self._ensure_engine(need_llm=True)
         samp = dict(do_sample=do_sample, temperature=temperature, top_k=top_k, seed=seed, logprobs=logprobs, top_p=top_p,
-                    repetition_penalty=repetition_penalty)
+                    repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size,
+                    bad_words_ids=bad_words_ids, min_new_tokens=min_new_tokens, eos=eos)
         reqs = [inflight.request(self, i, r, max_new_tokens, stopping_criteria, eng.NV, samp)
                 for i, r in enumerate(requests)]
         if self._kv_blocks:
             inflight.bind_sessions(self, reqs)
             inflight.check_paged(self, reqs, chunked_prefill)
-        sampling = any(r.temperature > 0 or r.penalty != 1.0 for r in reqs)
-        eos, _ = self._eos_pad(eos_token_id, None)
+        sampling = any(r.temperature > 0 or r.penalty != 1.0 or r.bans is not None for r in reqs)
+        banning = any(r.bans is not None for r in reqs)
         self._last_out, self._pos, self.last_logprobs = None, 0, None
         n_slots = min(n_slots, len(reqs))
         lps = inflight.RequestLogprobs(self, eng, reqs, n_slots)
@@ -1129,6 +1262,8 @@ class VideoChatGPTLlamaForCausalLM:
         finally:
             if sampling:
                 eng.set_sampling(list(range(n_slots)), [0.0] * n_slots, [0] * n_slots, [0] * n_slots)
+            if banning:
+                self._set_bans(eng, list(range(n_slots)), [None] * n_slots, eos, [0] * n_slots)
             if lps.on:
                 eng.set_logprobs(list(range(n_slots)), [-1] * n_slots)
 
@@ -1144,7 +1279,8 @@ class VideoChatGPTLlamaForCausalLM:
 
     def generate_continue(self, new_input_ids, do_sample=False, temperature=1.0, max_new_tokens=32,
                           stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50, seed=None,
-                          logprobs=None, top_p=1.0, repetition_penalty=1.0):
+                          logprobs=None, top_p=1.0, repetition_penalty=1.0, no_repeat_ngram_size=None, bad_words_ids=None,
+                          min_new_tokens=None):
         """Next turn about the SAME video(s): `new_input_ids` [B, S_new] follow everything generated
         so far. Only the tokens the KV cache does not hold yet (the last generated token and the new
         text) are prefilled (vcl_llm_prefill_append); the reference re-runs the tower and the whole
@@ -1153,7 +1289,9 @@ class VideoChatGPTLlamaForCausalLM:
         new text of every row has the same length S_new (no padding inside a turn).
         seed: do_sample=True samples on the device as generate(seed=...) does. logprobs: as in generate, for the new
         tokens of this turn. top_p / repetition_penalty: as in generate; the penalty's tokens are the whole
-        conversation (every earlier turn, its answers as returned, and the new text)."""
+        conversation (every earlier turn, its answers as returned, and the new text). no_repeat_ngram_size /
+        bad_words_ids / min_new_tokens: as in generate, over the whole conversation; min_new_tokens counts this turn's
+        tokens (HF's prompt length is the conversation's)."""
         self._not_paged("generate_continue")
         self.last_beam_scores = None
         if getattr(self, "_after_beams", False):
@@ -1168,6 +1306,9 @@ class VideoChatGPTLlamaForCausalLM:
         self.last_logprobs = None
         top_p, penalty = self._nucleus_args(top_p, repetition_penalty, "generate_continue", do_sample,
                                             device=not do_sample or seed is not None)
+        eos, pad = self._eos_pad(eos_token_id, pad_token_id)
+        bans = self._ban_args(no_repeat_ngram_size, bad_words_ids, min_new_tokens, eos, "generate_continue",
+                              device=not do_sample or seed is not None)
         seeded = do_sample and seed is not None
         if seeded:
             temperature, top_k, seed = self._sampling_args(temperature, top_k, seed, "generate_continue")
@@ -1179,8 +1320,7 @@ class VideoChatGPTLlamaForCausalLM:
         n = min(max_new_tokens, self._max_seq - ctx.shape[1])
         if n <= 0:
             raise ValueError(f"context length {ctx.shape[1]} leaves no room in max_seq {self._max_seq}")
-        eos, pad = self._eos_pad(eos_token_id, pad_token_id)
-        if seeded or lp_n is not None or (penalty != 1.0 and not do_sample):
+        if seeded or lp_n is not None or ((penalty != 1.0 or bans) and not do_sample):
             B, L = ctx.shape
             clips = list(range(B))
             if seeded:
@@ -1192,7 +1332,10 @@ class VideoChatGPTLlamaForCausalLM:
                 samp = contextlib.nullcontext()
             if penalty != 1.0:
                 self._token_sets(eng, [(b, ctx[b]) for b in clips])
-            with samp, self._logprobs(eng, clips, lp_n):
+            if bans:
+                self._histories(eng, [(b, ctx[b]) for b in clips])
+            with samp, self._banning(eng, clips, bans, eos, L + (bans.min_new if bans else 0)), \
+                    self._logprobs(eng, clips, lp_n):
                 _, _, tok = eng.prefill_append(tail, start)
                 first = eng.decode_loop(tok, ctx.shape[1], min(n, self._GREEDY_CHUNK))
                 self._last_out = self._host_stops(eng, ctx, first, n, stopping_criteria, eos, pad)
@@ -1204,19 +1347,22 @@ class VideoChatGPTLlamaForCausalLM:
         _, logits, _ = eng.prefill_append(tail, start, want_logits=True, want_token=False)
         self._pos = ctx.shape[1]
         self._last_out = self._stepwise(eng, ctx, logits, n, do_sample, temperature, stopping_criteria, eos, pad, top_k,
-                                        top_p, penalty)
+                                        top_p, penalty, bans)
         return self._last_out
 
     @staticmethod
-    def _host_processors(out, logits, sampled, temperature, top_k, top_p, penalty):
+    def _host_processors(out, logits, sampled, temperature, top_k, top_p, penalty, bans=None, S=0):
         """HF's logits processors of the stepwise path, in HF's order, on logits [B, V] fp32 after the ids `out`
-        [B, L]: RepetitionPenaltyLogitsProcessor, then (sampled only) TemperatureLogitsWarper, TopKLogitsWarper and
+        [B, L]: RepetitionPenaltyLogitsProcessor, the banned tokens (_host_bans, with `bans` from _ban_args; the call's
+        first new token at column S), then (sampled only) TemperatureLogitsWarper, TopKLogitsWarper and
         TopPLogitsWarper (min_tokens_to_keep 1); a dropped token is -inf"""
         if penalty != 1.0:
             ids = out.to(logits.device)
             sc = torch.gather(logits, 1, ids)
             sc = torch.where(sc < 0, sc * penalty, sc / penalty)
             logits = logits.scatter(1, ids, sc)
+        if bans is not None:
+            logits = VideoChatGPTLlamaForCausalLM._host_bans(out, logits, bans, S)
         if not sampled:
             return logits
         lg = logits / temperature
@@ -1231,13 +1377,16 @@ class VideoChatGPTLlamaForCausalLM:
         return lg
 
     def _stepwise(self, eng, out, logits, n, do_sample, temperature, stopping_criteria, eos, pad, top_k=50, top_p=1.0,
-                  penalty=1.0):
+                  penalty=1.0, bans=None):
         """One token per C-ABI call. After the loop the cache holds every returned token but the last
         (self._pos = out.shape[1] - 1), the state generate_continue starts from. The logits go through HF's
-        processors in HF's order: repetition penalty (over `out` so far), then temperature, top-k and top-p."""
+        processors in HF's order: repetition penalty (over `out` so far), the banned tokens, then temperature, top-k
+        and top-p."""
+        S = out.shape[1]
         unfinished = torch.ones(out.shape[0], dtype=torch.bool, device=out.device)
         for step in range(n):
-            lg = self._host_processors(out, logits, do_sample and temperature > 0, temperature, top_k, top_p, penalty)
+            lg = self._host_processors(out, logits, do_sample and temperature > 0, temperature, top_k, top_p, penalty,
+                                       bans, S)
             if do_sample and temperature > 0:
                 nxt = torch.multinomial(torch.softmax(lg, dim=-1), 1)[:, 0]
             else:
