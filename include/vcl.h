@@ -627,9 +627,9 @@ int vcl_op_attention_packed(const void* q, int64_t q_ld, const void* k, const vo
                             int n_slots, int n, const int32_t* slots_host, const int32_t* start_host,
                             const int32_t* len_host, const int32_t* flash_host, const int32_t* table_host,
                             int table_row, int n_blocks, int64_t blk, void* stream);
-/* out[b,n] = x[b,:].W[n,:] (+res) with optional RMSNorm of x: B <= 4 the ring kernel of the single-clip
- * decode path (fused norm), 5 <= B <= 16 the wide ring kernel (norm + window-major re-layout by a launch of
- * its own, as on the decode path) */
+/* out[b,n] = x[b,:].W[n,:] (+res) with optional RMSNorm of x: vcl_op_gemv_ex below with mode 0 (RES) and bf16
+ * weights. 1 <= B <= 4 the ring kernel of the 1..4-clip decode path (fused norm), 5 <= B <= 64 the window kernel
+ * (norm + window-major re-layout by a launch of its own, as on the decode path) */
 int vcl_op_gemv(const void* x, const void* W, void* out, const void* res, const void* norm_w,
                 float eps, int B, int N, int K, void* stream);
 /* The load-time quantizer of VCL_WEIGHTS_FP8_E4M3 on its own, rows in order: W [N,K] bf16 (K a multiple of 32)
@@ -641,6 +641,21 @@ int vcl_op_quantize_fp8(const void* W, int N, int K, void* w_deq, void* codes, f
  * fp8 instances of the ring kernels run; equals vcl_op_gemv on W~ bit for bit. */
 int vcl_op_gemv_fp8(const void* x, const void* W, void* out, const void* res, const void* norm_w,
                     float eps, int B, int N, int K, void* stream);
+/* One decode projection (x [B][K] bf16 . W^T, W [N][K] bf16 row-major) through the ring kernels and one of the
+ * fused epilogues of the decode step, launched as vcl_llm_decode_step launches them. fp8 != 0: W is quantized by
+ * the quantizer above (into scratch) and the fp8 kernels run; the result equals the bf16 launch on W~ bit for bit.
+ * 1 <= B <= 64; norm_w (or NULL): RMSNorm of x (eps), fused into the projection at B <= 4, a launch of its own (the
+ * window-major re-layout) at 5..64. mode:
+ *   0 RES     out [B][N] bf16 = bf16(x.W) (+ res [B][N], or NULL)
+ *   1 SWIGLU  N even, rows 2j / 2j+1 = gate_j / up_j: out = bf16(bf16(silu(bf16(gate))) * bf16(up)), [B][N/2]
+ *             row-major at B <= 4, in the window-major layout of B rows at 5..64 (element (b, j) at
+ *             ((j / 512) * B + b) * 544 + j % 512, a buffer of ceil(N/2 / 512) * B * 544 elements)
+ *   3 LOGITS  logits [B][N] fp32 (the bf16-rounded values, or NULL) and, at B <= 4, partials (or NULL): the arg-max
+ *             {float value; int32 index} of each CTA's rows, [min(ceil(N/16), SMs)][B], lowest index on ties; out
+ *             and res NULL, logits or partials given.
+ * Scratch is stream-ordered. */
+int vcl_op_gemv_ex(const void* x, const void* W, int fp8, int mode, void* out, const void* res, float* logits,
+                   void* partials, const void* norm_w, float eps, int B, int N, int K, void* stream);
 
 #ifdef __cplusplus
 }

@@ -46,6 +46,14 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
 }
+// num / (1 + e^-x) in fp32 with the fast intrinsics: silu (num = x) and the sigmoid (num = 1) of the activation
+// epilogues. __fdividef(a, d) returns 0 for 2^126 < |d| < 2^128 (x in about -88.7 .. -87.3), where the quotient is a
+// normal number; there both operands are scaled by 1/4 first (exactly), and every other x keeps the plain quotient.
+__device__ __forceinline__ float act_sigmoid_div(float num, float x) {
+  const float d = 1.0f + __expf(-x);
+  const float s = d > 0x1p126f ? 0.25f : 1.0f;
+  return __fdividef(num * s, d * s);
+}
 __device__ __forceinline__ float bf16lo(uint32_t v) { return __uint_as_float(v << 16); }
 __device__ __forceinline__ float bf16hi(uint32_t v) { return __uint_as_float(v & 0xffff0000u); }
 

@@ -240,7 +240,7 @@ __device__ __forceinline__ void epi_logit(const GemvEpilogue& e, int b, int row,
 // layout of nb clips
 __device__ __forceinline__ void epi_swiglu(const GemvEpilogue& e, int b, int row, int nb, float gate, float up) {
   const float gt = bf16r(gate);
-  const float sg = bf16r(__fdividef(gt, 1.0f + __expf(-gt)));
+  const float sg = bf16r(act_sigmoid_div(gt, gt));
   const int col = row >> 1;
   const long long o = e.out_xwin ? (long long)xwin_offset(b, col, nb) : (long long)b * e.ldo + col;
   e.out[o] = __float2bfloat16_rn(sg * bf16r(up));

@@ -126,7 +126,7 @@ __device__ __forceinline__ void gemm_epilogue_stage(const float (&acc)[BLOCK_N /
         const float x0 = acc[4 * j + 2 * h] + b0, x1 = acc[4 * j + 2 * h + 1] + b1;
         if constexpr (ACT == ACT_SWIGLU) {
           const float g = bf16r(x0);
-          const bf16 s = __float2bfloat16_rn(__fdividef(g, 1.0f + __expf(-g)));       // silu (bf16)
+          const bf16 s = __float2bfloat16_rn(act_sigmoid_div(g, g));                  // silu (bf16)
           const bf16 o = __hmul(s, __float2bfloat16_rn(x1));                           // * up (bf16)
           *reinterpret_cast<bf16*>(stg + r * Cfg::OUT_PITCH + col) = o;                // output column col / 2
         } else {
@@ -135,8 +135,7 @@ __device__ __forceinline__ void gemm_epilogue_stage(const float (&acc)[BLOCK_N /
             // x*sigmoid(1.702x): the three bf16 tensors of the reference are materialised
             const uint32_t x2 = pack_bf16x2(x0, x1);
             const uint32_t t2 = pack_bf16x2(1.702f * bf16lo(x2), 1.702f * bf16hi(x2));
-            const uint32_t s2 = pack_bf16x2(__fdividef(1.0f, 1.0f + __expf(-bf16lo(t2))),
-                                            __fdividef(1.0f, 1.0f + __expf(-bf16hi(t2))));
+            const uint32_t s2 = pack_bf16x2(act_sigmoid_div(1.0f, bf16lo(t2)), act_sigmoid_div(1.0f, bf16hi(t2)));
             o = bf16x2_mul(x2, s2);
           } else if constexpr (ACT == ACT_GELU) {
             o = pack_bf16x2(act_gelu_erf(x0), act_gelu_erf(x1));

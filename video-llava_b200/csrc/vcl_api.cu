@@ -307,8 +307,6 @@ cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
     if (_rc != 0) return _rc; \
   } while (0)
 
-int op_gemv_run(GemvArgs g, void* out, const void* res, float eps, cudaStream_t st);
-
 // VCL_WEIGHTS_FP8_E4M3: every streamed matrix is quantized in place (W~ over the row-major copy, which the prefill
 // GEMMs, the decode GEMM beyond 16 clips and the scoring lm_head read) and its decode copy is the E4M3 codes with
 // one scale per row instead of the bf16 slots. The state-dict name of a failing matrix row is reported.
@@ -2109,34 +2107,7 @@ int vcl_op_attention_vit(const void* qkv, void* out, int n_frames, int S, int H,
 
 int vcl_op_gemv(const void* x, const void* W, void* out, const void* res, const void* norm_w,
                 float eps, int B, int N, int K, void* stream) {
-  if (check_device() != 0) return -2;
-  VCL_REQUIRE(B >= 1 && B <= 64, "vcl_op_gemv: B=%d outside 1..64 (more rows take the GEMM)", B);
-  VCL_REQUIRE(gemv_fits(B, N, K, norm_w != nullptr),
-              "vcl_op_gemv: B=%d N=%d K=%d is outside the decode kernels' range", B, N, K);
-  static bool inited = false;
-  if (!inited) {
-    VCL_TRY(init_gemv_kernels());
-    inited = true;
-  }
-  GemvArgs g;
-  g.x = reinterpret_cast<const bf16*>(x); g.ldx = K;
-  g.B = B; g.N = N; g.K = K; g.norm_w = reinterpret_cast<const bf16*>(norm_w); g.eps = eps;
-  // the decode kernels read the slot-ordered copy of the matrix. It is built here and kept for the next call
-  // with the same matrix (this entry point is a test / micro-benchmark hook, not a hot path); the copy is only
-  // REUSED when VCL_OP_GEMV_CACHE is set (tools/microbench.py), because a caller may hand in a different
-  // matrix at a recycled address
-  static const void* c_W = nullptr; static int c_N = 0, c_K = 0; static bf16* c_tiled = nullptr;
-  if (c_W != W || c_N != N || c_K != K || getenv("VCL_OP_GEMV_CACHE") == nullptr) {
-    cudaStreamSynchronize(as_stream(stream));
-    if (c_tiled != nullptr) cudaFree(c_tiled);
-    c_tiled = nullptr; c_W = nullptr;
-    VCL_CUDA_OK(cudaMalloc(&c_tiled, gemv_tiled_elems(N, K) * sizeof(bf16)));
-    const int rc0 = launch_gemv_repack(reinterpret_cast<const bf16*>(W), c_tiled, N, K, false, as_stream(stream));
-    if (rc0 != 0) { cudaFree(c_tiled); c_tiled = nullptr; return rc0; }
-    c_W = W; c_N = N; c_K = K;
-  }
-  g.W_tiled = c_tiled;
-  return op_gemv_run(g, out, res, eps, as_stream(stream));
+  return vcl_op_gemv_ex(x, W, 0, GEMV_RES, out, res, nullptr, nullptr, norm_w, eps, B, N, K, stream);
 }
 
 int vcl_op_quantize_fp8(const void* W, int N, int K, void* w_deq, void* codes, float* scales, void* stream) {
@@ -2148,40 +2119,66 @@ int vcl_op_quantize_fp8(const void* W, int N, int K, void* w_deq, void* codes, f
 
 int vcl_op_gemv_fp8(const void* x, const void* W, void* out, const void* res, const void* norm_w,
                     float eps, int B, int N, int K, void* stream) {
+  return vcl_op_gemv_ex(x, W, 1, GEMV_RES, out, res, nullptr, nullptr, norm_w, eps, B, N, K, stream);
+}
+
+int vcl_op_gemv_ex(const void* x, const void* W, int fp8, int mode, void* out, const void* res, float* logits,
+                   void* partials, const void* norm_w, float eps, int B, int N, int K, void* stream) {
   if (check_device() != 0) return -2;
-  VCL_REQUIRE(B >= 1 && B <= 64, "vcl_op_gemv_fp8: B=%d outside 1..64 (more rows take the GEMM)", B);
-  VCL_REQUIRE(gemv_fits(B, N, K, norm_w != nullptr, true),
-              "vcl_op_gemv_fp8: B=%d N=%d K=%d is outside the decode kernels' range", B, N, K);
+  VCL_REQUIRE(x != nullptr && W != nullptr, "vcl_op_gemv: x and W are required");
+  VCL_REQUIRE(B >= 1 && B <= 64, "vcl_op_gemv: B=%d outside 1..64 (more rows take the GEMM)", B);
+  VCL_REQUIRE(gemv_fits(B, N, K, norm_w != nullptr, fp8 != 0),
+              "vcl_op_gemv: B=%d N=%d K=%d is outside the decode kernels' range", B, N, K);
+  VCL_REQUIRE(mode == GEMV_RES || mode == GEMV_SWIGLU || mode == GEMV_LOGITS,
+              "vcl_op_gemv: mode %d is none of RES (0), SWIGLU (1), LOGITS (3)", mode);
+  VCL_REQUIRE(mode == GEMV_LOGITS ? out == nullptr && (logits != nullptr || partials != nullptr)
+                                  : out != nullptr && logits == nullptr && partials == nullptr,
+              "vcl_op_gemv: RES and SWIGLU write out; LOGITS writes logits and / or the arg-max partials");
+  VCL_REQUIRE(res == nullptr || mode == GEMV_RES, "vcl_op_gemv: only RES adds a residual");
+  VCL_REQUIRE(partials == nullptr || B <= 4, "vcl_op_gemv: B=%d: the arg-max partials need 1..4 rows", B);
   static bool inited = false;
   if (!inited) {
     VCL_TRY(init_gemv_kernels());
     inited = true;
   }
-  // the load-time quantizer into stream-ordered scratch (W itself is left as it is), then the fp8 ring kernels
   cudaStream_t st = as_stream(stream);
-  unsigned char* scratch = nullptr;
-  const size_t deq = (size_t)N * K * sizeof(bf16), cb = (gemv_tiled_elems(N, K) + 255) / 256 * 256;
-  VCL_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&scratch), deq + cb + (size_t)N * sizeof(float), st));
   GemvArgs g;
   g.x = reinterpret_cast<const bf16*>(x); g.ldx = K;
   g.B = B; g.N = N; g.K = K; g.norm_w = reinterpret_cast<const bf16*>(norm_w); g.eps = eps;
-  g.W_fp8 = scratch + deq; g.w_scale = reinterpret_cast<float*>(scratch + deq + cb);
-  int rc = launch_gemv_quantize_fp8(reinterpret_cast<const bf16*>(W), reinterpret_cast<bf16*>(scratch),
-                                    scratch + deq, reinterpret_cast<float*>(scratch + deq + cb), N, K, false, nullptr, st);
-  if (rc == 0) rc = op_gemv_run(g, out, res, eps, st);
-  VCL_CUDA_OK(cudaFreeAsync(scratch, st));
-  return rc;
-}
-
-}  // extern "C"
-
-namespace {
-
-// out = x . W^T (+ res) by the decode kernels, with g's weights; 5..64 rows through the xwin re-layout
-int op_gemv_run(GemvArgs g, void* out, const void* res, float eps, cudaStream_t st) {
-  const int B = g.B, N = g.N, K = g.K;
+  g.amax_out = reinterpret_cast<ArgmaxPart*>(partials);
   GemvEpilogue e;
-  e.mode = GEMV_RES; e.out = reinterpret_cast<bf16*>(out); e.ldo = N; e.res = reinterpret_cast<const bf16*>(res); e.ldr = N;
+  e.mode = mode;
+  e.out = reinterpret_cast<bf16*>(out); e.ldo = mode == GEMV_SWIGLU ? N / 2 : N; e.out_xwin = mode == GEMV_SWIGLU && B > 4;
+  e.res = reinterpret_cast<const bf16*>(res); e.ldr = N;
+  e.logits = logits; e.ldl = N;
+  // the decode kernels read the slot-ordered copy of the matrix (bf16) or its E4M3 codes (fp8)
+  unsigned char* scratch = nullptr;
+  if (fp8) {
+    // the load-time quantizer into stream-ordered scratch (W itself is left as it is)
+    const size_t deq = (size_t)N * K * sizeof(bf16), cb = (gemv_tiled_elems(N, K) + 255) / 256 * 256;
+    VCL_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&scratch), deq + cb + (size_t)N * sizeof(float), st));
+    g.W_fp8 = scratch + deq; g.w_scale = reinterpret_cast<float*>(scratch + deq + cb);
+    const int rc = launch_gemv_quantize_fp8(reinterpret_cast<const bf16*>(W), reinterpret_cast<bf16*>(scratch),
+                                            scratch + deq, reinterpret_cast<float*>(scratch + deq + cb), N, K, false,
+                                            nullptr, st);
+    if (rc != 0) { cudaFreeAsync(scratch, st); return rc; }
+  } else {
+    // The bf16 copy is built here and kept for the next call with the same matrix (this entry point is a test /
+    // micro-benchmark hook, not a hot path); the copy is only REUSED when VCL_OP_GEMV_CACHE is set
+    // (tools/microbench.py), because a caller may hand in a different matrix at a recycled address
+    static const void* c_W = nullptr; static int c_N = 0, c_K = 0; static bf16* c_tiled = nullptr;
+    if (c_W != W || c_N != N || c_K != K || getenv("VCL_OP_GEMV_CACHE") == nullptr) {
+      cudaStreamSynchronize(st);
+      if (c_tiled != nullptr) cudaFree(c_tiled);
+      c_tiled = nullptr; c_W = nullptr;
+      VCL_CUDA_OK(cudaMalloc(&c_tiled, gemv_tiled_elems(N, K) * sizeof(bf16)));
+      const int rc0 = launch_gemv_repack(reinterpret_cast<const bf16*>(W), c_tiled, N, K, false, st);
+      if (rc0 != 0) { cudaFree(c_tiled); c_tiled = nullptr; return rc0; }
+      c_W = W; c_N = N; c_K = K;
+    }
+    g.W_tiled = c_tiled;
+  }
+  int rc = 0;
   if (B >= 5) {
     // 5..64 rows: the xwin ring kernels; their input is normalised and re-laid out (xwin) by a launch of its own,
     // as on the decode path
@@ -2189,18 +2186,21 @@ int op_gemv_run(GemvArgs g, void* out, const void* res, float eps, cudaStream_t 
     if (xn_elems < xwin_elems(B, K)) {
       cudaStreamSynchronize(st);
       if (xn) cudaFree(xn);
-      VCL_CUDA_OK(cudaMalloc(&xn, xwin_elems(B, K) * sizeof(bf16)));
-      xn_elems = xwin_elems(B, K);
+      xn = nullptr; xn_elems = 0;
+      if (cudaMalloc(&xn, xwin_elems(B, K) * sizeof(bf16)) != cudaSuccess) {
+        set_last_error("vcl_op_gemv: out of device memory for the xwin rows");
+        rc = -2;
+      } else {
+        xn_elems = xwin_elems(B, K);
+      }
     }
-    VCL_TRY(launch_xwin_norm(g.x, K, xn, g.norm_w, B, K, eps, st));
+    if (rc == 0) rc = launch_xwin_norm(g.x, K, xn, g.norm_w, B, K, eps, st);
     g.x = xn; g.norm_w = nullptr;
   }
-  return launch_gemv(g, e, st);
+  if (rc == 0) rc = launch_gemv(g, e, st);
+  if (scratch != nullptr) VCL_CUDA_OK(cudaFreeAsync(scratch, st));
+  return rc;
 }
-
-}  // namespace
-
-extern "C" {
 
 int vcl_op_decode_attention(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int B, int H,
                             int s_max, int kv_len, const int32_t* pos_dev, const int32_t* n_pad, float scale,

@@ -187,6 +187,8 @@ _SIGNATURES = {
     "vcl_op_gemv_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int,
                                 c_int, c_void_p]),
     "vcl_op_quantize_fp8": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "vcl_op_gemv_ex": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                               c_float, c_int, c_int, c_int, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
@@ -474,6 +476,36 @@ def op_gemv_fp8(x, w, res=None, norm_w=None, eps=0.0):
     out = torch.empty(B, N, dtype=torch.bfloat16, device=x.device)
     check(lib().vcl_op_gemv_fp8(ptr(x), ptr(w), ptr(out), ptr(res), ptr(norm_w), eps, B, N, K, cur_stream()))
     return out
+
+
+GEMV_RES, GEMV_SWIGLU, GEMV_LOGITS = 0, 1, 3   # vcl_op_gemv_ex: the fused epilogues of the decode projections
+
+
+def gemv_grid(N):
+    """CTAs of a 1..4-row decode projection over N rows: the rows of the arg-max partials of vcl_op_gemv_ex"""
+    return min((N + 15) // 16, torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count)
+
+
+def op_gemv_ex(x, w, mode, fp8=False, norm_w=None, eps=0.0, out=None, logits=True, partials=False):
+    """One decode projection through a fused epilogue (vcl_op_gemv_ex), x [B, K] bf16, w [N, K] bf16; fp8: the
+    E4M3 kernels on the quantized w (equal to the bf16 launch on W~ = op_quantize_fp8(w)[0]).
+    RES (no residual): returns out [B, N] bf16. SWIGLU: out [B, N/2] bf16 at B <= 4, the flat xwin buffer at 5..64
+    (see xwin_offset; `out` may be given, e.g. pre-filled with a sentinel). LOGITS: returns (logits [B, N] fp32 or
+    None, partials int32 [gemv_grid(N), B, 2] or None: the value's bits and the row of each CTA's arg-max)."""
+    B, K = x.shape
+    N = w.shape[0]
+    lg = pt = None
+    if mode == GEMV_LOGITS:
+        lg = torch.empty(B, N, dtype=torch.float32, device=x.device) if logits else None
+        pt = torch.empty(gemv_grid(N), B, 2, dtype=torch.int32, device=x.device) if partials else None
+    elif out is None:
+        if mode == GEMV_SWIGLU and B > 4:
+            out = torch.empty((N // 2 + XWIN_KC - 1) // XWIN_KC * B * XWIN_PITCH, dtype=torch.bfloat16, device=x.device)
+        else:
+            out = torch.empty(B, N // 2 if mode == GEMV_SWIGLU else N, dtype=torch.bfloat16, device=x.device)
+    check(lib().vcl_op_gemv_ex(ptr(x), ptr(w), int(bool(fp8)), mode, ptr(out), None, ptr(lg), ptr(pt), ptr(norm_w),
+                               eps, B, N, K, cur_stream()))
+    return (lg, pt) if mode == GEMV_LOGITS else out
 
 
 def tiled_elems(N, K):
