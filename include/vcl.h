@@ -298,6 +298,31 @@ int vcl_llm_slots_prefill_chunk(vcl_handle* h, int n, const int32_t* slots_host,
 int vcl_llm_slots_prefill_append(vcl_handle* h, int n, const int32_t* slots_host, const int32_t* start_host,
                                  const int32_t* len_host, const int64_t* ids, int32_t* next_tok, void* stream);
 
+/* Candidate scoring, step 2 (VideoChatGPTLlamaForCausalLM.score_candidates; it replaces one reference forward per
+ * prompt + option, video_chatgpt/model/video_chatgpt.py:193-239, whose shared prompt rows repeat for every option):
+ * copy columns 0 .. cols_host[i] - 1 of cache slot src_host[i] into slot dst_host[i], every layer, K and V, on the
+ * CONTIGUOUS cache (a paged handle is rejected). All HOST memory, [n] int32. The copy is kv_fork_kernel (beam search's
+ * fork), one launch per distinct column count. Rejected before any device work: n outside 0 .. max_slots, a slot
+ * outside 0 .. max_slots-1, cols outside 0 .. max_seq, a destination given twice or also a source. */
+int vcl_llm_slots_fork(vcl_handle* h, int n, const int32_t* src_host, const int32_t* dst_host, const int32_t* cols_host,
+                       void* stream);
+
+/* Candidate scoring, step 3: one packed continuation of cached sequences on the CONTIGUOUS cache (a paged handle is
+ * rejected), scored at every row. Sequence i is len_host[i] tokens at positions start_host[i] .. of slot slots_host[i]
+ * (HOST memory, [n] int32), whose columns 0 .. start_host[i] - 1 the slot already holds (start 0: a sequence new to
+ * its slot, as in vcl_llm_slots_prefill; a one-token prompt's options start there); ids [sum len_i] int64 packs them. Each sequence runs the attention kernel the contiguous continued prefill (vcl_llm_prefill_append) runs at the
+ * same start and length: the wgmma kernel up to 512 keys, the flash kernel past them, so its cache columns and rows are
+ * those of vcl_llm_prefill_append bit for bit (at start 0, those of vcl_llm_slots_prefill). No token is sampled. Then the final RMSNorm and the lm_head GEMM run
+ * over every row in chunks (vcl_llm_score's tail), and row r of the packed rows is scored against labels[r] (device
+ * int64 [sum len_i]): lp_out[r] (device f32) = the greedy log-prob rule of vcl_op_sample_logprobs at that token,
+ * (x_label - m) - logf(W), and greedy_out[r] (device uint8) = 1 when the label is the lowest-index arg-max of the
+ * row (vcl_op_label_logprobs). A row without a finite maximum, or a label outside 0 .. vocab-1, gives NaN and 0.
+ * Rejected before any device work: n outside 1 .. max_slots, a slot outside 0 .. max_slots-1 or given twice,
+ * start_i < 0, len_i outside 1 .. 512, start_i + len_i > max_seq, and sum len_i beyond the activations. */
+int vcl_llm_slots_score_append(vcl_handle* h, int n, const int32_t* slots_host, const int32_t* start_host,
+                               const int32_t* len_host, const int64_t* ids, const int64_t* labels, float* lp_out,
+                               uint8_t* greedy_out, void* stream);
+
 /* vcl_llm_decode_loop with a position per slot: slot b (0 <= b < n_slots) is fed first_tok[b] at position
  * pos_host[b] (HOST memory: the number of tokens its cache holds), then runs n_new-1 greedy steps;
  * out_tokens is [n_slots, n_new] int32, first_tok included. Every pos_host[b] + n_new - 1 must be <= max_seq
@@ -541,6 +566,15 @@ int vcl_op_gemm_ex(const void* A, int64_t lda, const void* W, int64_t ldw, void*
  * (required) and, optionally, loss_out [1] fp32, the mean over the rows whose label is not -100. */
 int vcl_op_cross_entropy(const void* logits, int64_t ld, const int64_t* labels, int rows, int V,
                          float* nll_out, float* loss_out, void* stream);
+/* The scoring kernel of vcl_llm_slots_score_append on its own (log_softmax(logits)[label] of the reference's
+ * forward, video_chatgpt/model/video_chatgpt.py:225-239, in the sampler's fp32 rule): row r of logits [rows, ld] bf16
+ * (first V columns, V <= VCL_SAMPLE_WIDE_MAX_V) with labels[r] (device int64) -> lp_out[r] (device f32) =
+ * (x_label - m) - logf(W), m the largest non-NaN value and W the sum of exp(x - m) over the non-NaN values in the
+ * sampler's fixed order, so it equals vcl_op_sample_logprobs' value for that token bit for bit; greedy_out[r] (device
+ * uint8) = 1 when labels[r] is the lowest index of the largest value. A row without a finite maximum, or a label
+ * outside 0 .. V-1, gives NaN and 0. */
+int vcl_op_label_logprobs(const void* logits, int64_t ld, int rows, int V, const int64_t* labels, float* lp_out,
+                          uint8_t* greedy_out, void* stream);
 /* The sampling kernel on its own: row b of logits [B, ld] fp32 (first V columns; bf16-representable values, as
  * the lm_head writes them) is sampled with temperature_host[b] (0: greedy), top_k_host[b], seed_host[b] and the
  * Philox counter counter_host[b] (all HOST memory, [B]); tok_out [B] int32 on the device. V <= 81920. */
@@ -627,6 +661,12 @@ int vcl_op_attention_packed(const void* q, int64_t q_ld, const void* k, const vo
                             int n_slots, int n, const int32_t* slots_host, const int32_t* start_host,
                             const int32_t* len_host, const int32_t* flash_host, const int32_t* table_host,
                             int table_row, int n_blocks, int64_t blk, void* stream);
+/* The attention of vcl_llm_slots_score_append on its own: vcl_op_attention_packed on a contiguous cache k / v
+ * [n_slots][H][s_max][128], sequence i on the wgmma kernel when start_host[i] + len_host[i] <= 512 and on the flash
+ * kernel otherwise, as the contiguous continued prefill (vcl_op_attention_cached at the same start) chooses. */
+int vcl_op_attention_appended(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int H, int s_max,
+                              int n_slots, int n, const int32_t* slots_host, const int32_t* start_host,
+                              const int32_t* len_host, void* stream);
 /* out[b,n] = x[b,:].W[n,:] (+res) with optional RMSNorm of x: vcl_op_gemv_ex below with mode 0 (RES) and bf16
  * weights. 1 <= B <= 4 the ring kernel of the 1..4-clip decode path (fused norm), 5 <= B <= 64 the window kernel
  * (norm + window-major re-layout by a launch of its own, as on the decode path) */

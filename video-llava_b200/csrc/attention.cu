@@ -13,7 +13,9 @@
 //     launch_attention_vit), longer prompts and continued prefills beyond 512 keys, and the chunks of prompts over
 //     512 tokens in a paged cache (vcl_llm_slots_prefill_chunk: packed, each key tile read through the block
 //     table, the same tiles and arithmetic as the one-shot prefill of the whole prompt) and text tails appended to
-//     a paged slot past 512 keys (vcl_llm_slots_prefill_append: those of the contiguous continued prefill); the
+//     a paged slot past 512 keys (vcl_llm_slots_prefill_append: those of the contiguous continued prefill), and the
+//     packed option continuations of candidate scoring past 512 keys on the contiguous cache
+//     (vcl_llm_slots_score_append, the same tiles and masks again); the
 //     ViT's S = 257 runs in
 //     attention_tc.cu, the causal hd-128 prefill up to 512 keys in attention_prefill_tc.cu (both wgmma, exact
 //     full-row softmax).
@@ -81,10 +83,12 @@ __device__ __forceinline__ void load_tile(uint32_t sbase, const bf16* g, long lo
 // PAD (causal only): left-padded clips (a.n_pad): a real query (cache column >= n_pad[b]) attends keys n_pad[b] ..
 // its own column, and a tile of real queries starts at the first key tile that holds a real key; a pad query
 // attends causally
-// PACK: packed sequences (a.pack, kernels.h) on a paged cache (PAGED, a.pages): blockIdx.z is sequence i, whose
-// pack_end_i - pack_start_i queries start at its row offset and sit at absolute positions start_i .. ; its keys are
-// columns 0 .. end_i - 1 of slot_i (q_off = start_i, S_kv = end_i). Sequences with pack_len > 0 belong to the wgmma
-// kernel and are skipped. Key tile jt is the 64 columns at offset (jt % 2) * 64 of block table[slot_i][jt / 2].
+// PACK: packed sequences (a.pack, kernels.h): blockIdx.z is sequence i, whose pack_end_i - pack_start_i queries start
+// at its row offset and sit at absolute positions start_i .. ; its keys are columns 0 .. end_i - 1 of slot_i (q_off =
+// start_i, S_kv = end_i). Sequences with pack_len > 0 belong to the wgmma kernel and are skipped. On a paged cache
+// (PAGED, a.pages) key tile jt is the 64 columns at offset (jt % 2) * 64 of block table[slot_i][jt / 2]; on the
+// contiguous cache it is columns jt * 64 .. of clip slot_i (vcl_llm_slots_score_append: option continuations that
+// end past 512 keys).
 // A query tile covers the rows, walks the key tiles and applies the masks of the same tile of the contiguous kernel
 // at the same q_off, S_kv: a continued prefill (vcl_llm_slots_prefill_append: a text tail at any start_i). For a
 // chunk of a prompt (vcl_llm_slots_prefill_chunk), start_i is a multiple of 64, so these are also the tiles and
@@ -92,8 +96,8 @@ __device__ __forceinline__ void load_tile(uint32_t sbase, const bf16* g, long lo
 // of the chunk too, so both mask them causally, and the zero-filled columns past end_i only meet P = 0.
 template <int HD, bool CAUSAL, bool PAD = false, bool PACK = false, bool PAGED = false>
 __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
-  static_assert(PACK == PAGED && (!PACK || (CAUSAL && !PAD && HD == 128)),
-                "packed sequences: causal, unpadded hd-128 attention on a paged cache");
+  static_assert((!PAGED || PACK) && (!PACK || (CAUSAL && !PAD && HD == 128)),
+                "packed sequences: causal, unpadded hd-128 attention; a paged cache is read by packed sequences only");
   extern __shared__ __align__(128) uint8_t smem[];
   constexpr int TILE_BYTES = 64 * HD * 2;
   const uint32_t sQ = smem_u32(smem);
@@ -119,8 +123,8 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
     slot = __ldg(pack_slot(a.pack) + b);
   }
   const bf16* qg = a.q + q_base + (long long)h * a.q_sh;
-  const bf16* kg = a.k + (PAGED ? 0 : (long long)b * a.k_sb) + (long long)h * a.k_sh;
-  const bf16* vg = a.v + (PAGED ? 0 : (long long)b * a.v_sb) + (long long)h * a.v_sh;
+  const bf16* kg = a.k + (PAGED ? 0 : (long long)(PACK ? slot : b) * a.k_sb) + (long long)h * a.k_sh;
+  const bf16* vg = a.v + (PAGED ? 0 : (long long)(PACK ? slot : b) * a.v_sb) + (long long)h * a.v_sh;
   // key tile jt (keys jt * 64 ..; keys >= S_kv are zero-filled, never read)
   auto load_kv = [&](uint32_t sk, uint32_t sv, int jt) {
     if constexpr (PAGED) {
@@ -284,10 +288,10 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(const AttnArgs a) {
   }
 }
 
-template <int HD, bool CAUSAL, bool PAD = false, bool PACK = false>
+template <int HD, bool CAUSAL, bool PAD = false, bool PACK = false, bool PAGED = false>
 int launch_attn_t(const AttnArgs& a, cudaStream_t stream) {
   constexpr int SMEM = 5 * 64 * HD * 2;
-  auto kern = attn_fwd_kernel<HD, CAUSAL, PAD, PACK, PACK>;
+  auto kern = attn_fwd_kernel<HD, CAUSAL, PAD, PACK, PAGED>;
   dim3 grid((a.S + 63) / 64, a.H, a.B);
   kern<<<grid, 128, SMEM, stream>>>(a);
   VCL_CUDA_OK(cudaGetLastError());
@@ -305,6 +309,8 @@ int init_attention_kernels() {
   VCL_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<128, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 64 * 128 * 2));
   VCL_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<128, true, false, true, true>,
                                    cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 64 * 128 * 2));
+  VCL_CUDA_OK(cudaFuncSetAttribute(attn_fwd_kernel<128, true, false, true, false>,
+                                   cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * 64 * 128 * 2));
   if (init_attention_tc_kernels() != 0) return -2;
   return init_attention_prefill_tc_kernels();
 }
@@ -319,12 +325,12 @@ int launch_attention(const AttnArgs& a, cudaStream_t stream) {
   VCL_REQUIRE(a.pack == nullptr || (a.causal && a.head_dim == 128 && a.n_pad == nullptr && a.S <= 512),
               "attention: packed sequences need causal hd-128 attention over at most 512 keys, unpadded");
   VCL_REQUIRE(a.pack == nullptr || a.pack_tc || a.pack_flash, "attention: a packed launch runs at least one kernel");
-  VCL_REQUIRE(a.pack == nullptr || !a.pack_flash || a.pages.table != nullptr,
-              "attention: the packed flash kernel reads a paged cache");
   if (a.B <= 0 || a.H <= 0 || a.S <= 0) return 0;
-  if (a.pack != nullptr) {   // wgmma: whole prompts of at most 512 tokens; flash: chunks of longer prompts
+  if (a.pack != nullptr) {   // wgmma: up to 512 keys; flash: chunks of longer prompts, tails past 512 keys
     if (a.pack_tc && launch_attention_prefill_tc(a, stream) != 0) return -1;
-    return a.pack_flash ? launch_attn_t<128, true, false, true>(a, stream) : 0;
+    if (!a.pack_flash) return 0;
+    return a.pages.table != nullptr ? launch_attn_t<128, true, false, true, true>(a, stream)
+                                    : launch_attn_t<128, true, false, true, false>(a, stream);
   }
   if (attention_prefill_tc_supported(a)) return launch_attention_prefill_tc(a, stream);   // LLaMA prefill up to 512 keys
   if (a.n_pad != nullptr) return launch_attn_t<128, true, true>(a, stream);

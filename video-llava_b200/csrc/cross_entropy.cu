@@ -14,10 +14,17 @@
 // exponentials from shared memory and, when asked, writes the compact [rows, V] copy from shared memory with
 // 16-byte stores aligned to the destination. A second kernel (one CTA) takes the mean over the counted rows in
 // a fixed order (fp64 accumulation, no atomics), so the loss is identical from run to run.
+//
+// label_logprobs_kernel (candidate scoring, vcl_llm_slots_score_append): the greedy log-prob rule of the sampler
+// (DESIGN.md section 3) at a given label instead of the chosen token, lp = (x_label - m) - logf(W) in fp32, and
+// whether the label is the lowest-index arg-max. One CTA of SEL_THREADS per row, the row staged as 32-bit order keys
+// (select.cuh), W from kept_weights over the same contiguous runs as the sampler, so lp equals
+// vcl_op_sample_logprobs' value for that token bit for bit.
 #include <math.h>
 
 #include "common.cuh"
 #include "kernels.h"
+#include "select.cuh"
 
 namespace vcl {
 
@@ -158,7 +165,82 @@ nll_mean_kernel(const float* __restrict__ nll, const long long* __restrict__ lab
     *loss_out = scnt[0] > 0 ? (float)(ssum[0] / (double)scnt[0]) : __int_as_float(0x7fc00000);
 }
 
+constexpr int LP_MAX_V = VCL_SAMPLE_WIDE_MAX_V;   // the staged row of 32-bit keys: 224 KB of shared memory
+
+__global__ void __launch_bounds__(SEL_THREADS, 1)
+label_logprobs_kernel(const uint16_t* __restrict__ logits, long long ld, int V, const long long* __restrict__ labels,
+                      float* __restrict__ lp, uint8_t* __restrict__ greedy) {
+  extern __shared__ __align__(16) uint32_t skey[];
+  __shared__ uint32_t s_max[SEL_WARPS];
+  __shared__ float s_sum[SEL_WARPS];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const long long r = blockIdx.x;
+  const uint16_t* x = logits + r * ld;
+  const long long label = labels[r];
+
+  // stage the keys of the row and find the largest
+  uint32_t best = 0;
+  for (int i = tid; i < V; i += SEL_THREADS) {
+    const uint32_t key = order_key32(__uint_as_float((uint32_t)x[i] << 16));
+    skey[i] = key;
+    best = key > best ? key : best;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const uint32_t q = __shfl_xor_sync(0xffffffffu, best, o);
+    best = q > best ? q : best;
+  }
+  if (lane == 0) s_max[warp] = best;
+  __syncthreads();
+  best = s_max[0];
+#pragma unroll
+  for (int w = 1; w < SEL_WARPS; ++w) best = s_max[w] > best ? s_max[w] : best;
+  const float m = key_value32(best);
+  const bool finite = isfinite(m);                  // (uniform)
+  const bool ok = label >= 0 && label < V;          // (uniform)
+
+  const int run = (V + SEL_THREADS - 1) / SEL_THREADS;
+  const int i_beg = tid * run, i_end = min(i_beg + run, V);
+  float W = 0.f;
+  if (finite) {
+    float s, excl;
+    int last;
+    kept_weights(skey, i_beg, i_end, [](uint32_t key) { return key_value32(key); }, -INFINITY, m, s_sum, &s, &excl, &W,
+                 &last);
+  }
+  // the lowest-index arg-max: no key before the label's is >= it, none after it is larger
+  int beaten = 0;
+  if (ok) {
+    const uint32_t kl = skey[label];
+    for (int i = i_beg; i < i_end; ++i) beaten |= i < label ? skey[i] >= kl : skey[i] > kl;
+  }
+  beaten = __syncthreads_or(beaten);
+  if (tid == 0) {
+    lp[r] = finite && ok ? (key_value32(skey[label]) - m) - logf(W) : __int_as_float(0x7fc00000);
+    greedy[r] = finite && ok && !beaten;
+  }
+}
+
 }  // namespace
+
+int launch_label_logprobs(const bf16* logits, long long ld, int V, const long long* labels, int rows, float* lp,
+                          uint8_t* greedy, cudaStream_t stream) {
+  VCL_REQUIRE(V >= 1 && V <= LP_MAX_V && ld >= V && rows >= 0, "label_logprobs: V=%d outside 1..%d, row pitch %lld or "
+              "rows %d", V, LP_MAX_V, ld, rows);
+  VCL_REQUIRE(logits && labels && lp && greedy, "label_logprobs: null argument");
+  if (rows == 0) return 0;
+  static bool attr = false;
+  if (!attr) {
+    VCL_CUDA_OK(cudaFuncSetAttribute(label_logprobs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LP_MAX_V * 4));
+    attr = true;
+  }
+  const size_t smem = ((size_t)V * 4 + 15) / 16 * 16;
+  label_logprobs_kernel<<<rows, SEL_THREADS, smem, stream>>>(reinterpret_cast<const uint16_t*>(logits), ld, V, labels,
+                                                            lp, greedy);
+  VCL_CUDA_OK(cudaGetLastError());
+  count_launches(1);
+  return 0;
+}
 
 int launch_cross_entropy(const bf16* logits, long long ld, int V, const long long* labels, long long row0, int rows,
                          int seg, float* nll, bf16* logits_out, cudaStream_t stream) {

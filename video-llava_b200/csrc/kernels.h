@@ -150,6 +150,14 @@ int launch_cross_entropy(const bf16* logits, long long ld, int V, const long lon
 // nll_out (optional): a copy of nll, [rows] (seg == 0) or [clip][seg - 1] (the last column of each clip dropped)
 int launch_nll_mean(const float* nll, const long long* labels, long long rows, int seg, float* nll_out,
                     float* loss_out, cudaStream_t stream);
+// The greedy log-prob of a given label per row (DESIGN.md section 3): row r of logits [rows, ld] bf16 (first V
+// columns, V <= VCL_SAMPLE_WIDE_MAX_V) and its label labels[r] give lp[r] = (x_label - m) - logf(W), m the row's
+// largest non-NaN value and W the sampler's kept-weight sum in its fixed order (select.cuh: kept_weights), so lp is
+// vcl_op_sample_logprobs' value for that token bit for bit; greedy[r] = 1 when the label is the lowest index of the
+// largest value. A row without a finite maximum, or a label outside 0 .. V-1, gives NaN and 0 (a NaN logit at the
+// label gives NaN).
+int launch_label_logprobs(const bf16* logits, long long ld, int V, const long long* labels, int rows, float* lp,
+                          uint8_t* greedy, cudaStream_t stream);
 
 // ---- sampling.cu --------------------------------------------------------------------------------
 // Next token of each logits row [B][ld] (first V columns; bf16 values in fp32 storage) by the rules at the top of
@@ -253,9 +261,9 @@ struct AttnArgs {
   // packed rows only: a paged cache. Key block kb of sequence i is block table[slot_i][kb] (k / v: the layer's pool
   // bases, k_sh / v_sh the head stride inside a block, k_ss = v_ss = 128; k_sb / v_sb unused)
   KvPages pages;
-  // packed rows on a paged cache: which kernels run. pack_tc: the wgmma kernel for the sequences with pack_len > 0;
-  // pack_flash: the flash kernel (attention.cu) for those with pack_len 0, whose queries start_i .. end_i - 1 attend
-  // keys 0 .. their own position (one launch per kernel, each over every sequence; the other kind's CTAs leave)
+  // packed rows: which kernels run. pack_tc: the wgmma kernel for the sequences with pack_len > 0; pack_flash: the
+  // flash kernel (attention.cu) for those with pack_len 0, whose queries start_i .. end_i - 1 attend keys 0 .. their
+  // own position (one launch per kernel, each over every sequence; the other kind's CTAs leave)
   bool pack_tc = true, pack_flash = false;
 };
 int launch_attention(const AttnArgs& a, cudaStream_t stream);     // dispatches to the wgmma prefill kernel when it applies

@@ -789,10 +789,8 @@ AttnArgs prefill_attn_args(const bf16* q, long long q_ld, const bf16* kc, const 
   a.o = o; a.o_sb = (long long)S * o_ld; a.o_sh = 128; a.o_ss = o_ld;
   a.B = B; a.H = H; a.S = S; a.head_dim = 128; a.scale = 0.08838834764831845f; a.causal = 1;   // 128 ^ -1/2
   a.S_kv = start_pos + S; a.q_off = start_pos; a.n_pad = n_pad; a.pack = pack;
-  if (pages.table != nullptr) {
-    a.k_sb = a.v_sb = 0; a.k_sh = a.v_sh = 128 * 128; a.pages = pages;
-    a.pack_tc = (pack_attn & 1) != 0; a.pack_flash = (pack_attn & 2) != 0;
-  }
+  a.pack_tc = (pack_attn & 1) != 0; a.pack_flash = (pack_attn & 2) != 0;
+  if (pages.table != nullptr) { a.k_sb = a.v_sb = 0; a.k_sh = a.v_sh = 128 * 128; a.pages = pages; }
   return a;
 }
 
@@ -953,26 +951,36 @@ int score_chunk_rows(const vcl_handle* h) {
   return (int)(cap >= 128 ? cap / 128 * 128 : cap);
 }
 
-// Scoring tail after a full-depth prefill (h->l_h: the last layer's output, B*S rows): the final RMSNorm over
-// every row into l_x, then per chunk of rows the lm_head GEMM into l_qkv (dead after the last layer) and the
-// cross-entropy kernel over it. The per-row NLL waits in l_attn (also dead) for the mean over all rows. The KV
-// cache is not touched. labels [B,S] (HF's shift: column s is scored against labels[b, s+1]) or null.
-int score_tail(vcl_handle* h, int B, int S, const int64_t* labels, bf16* logits_out, float* nll_out,
-               float* loss_out, cudaStream_t st) {
+// The vocabulary tail of scoring after a full-depth prefill (h->l_h: the last layer's output, M rows): the final
+// RMSNorm over every row into l_x, then per chunk of rows the lm_head GEMM into l_qkv (dead after the last layer,
+// [m][vocab_padded]) and rows(r0, m), a per-row kernel over that chunk. The KV cache is not touched.
+template <class Rows>
+int vocab_tail(vcl_handle* h, long long M, Rows rows, cudaStream_t st) {
   const vcl_config& c = h->cfg;
-  const int D = c.llm_hidden, V = c.vocab, Vp = h->vocab_padded();
-  const long long M = (long long)B * S;
+  const int D = c.llm_hidden, Vp = h->vocab_padded();
   const int chunk = score_chunk_rows(h);
   VCL_REQUIRE(chunk > 0, "scoring needs max_batch * max_seq * 3 * llm_hidden >= %d (one padded vocabulary row)", Vp);
-  const long long* lab = reinterpret_cast<const long long*>(labels);
-  float* nll = labels != nullptr ? reinterpret_cast<float*>(h->l_attn) : nullptr;
   VCL_TRY(launch_rmsnorm(h->l_h, D, h->l_x, D, h->norm_w, (int)M, D, c.rms_eps, st));
   for (long long r0 = 0; r0 < M; r0 += chunk) {
     const int m = (int)(M - r0 < chunk ? M - r0 : chunk);
     VCL_TRY(gemm(h->l_x + r0 * D, D, h->lm_head, D, h->l_qkv, Vp, nullptr, nullptr, 0, m, Vp, D, ACT_NONE, st));
-    VCL_TRY(launch_cross_entropy(h->l_qkv, Vp, V, lab, r0, m, S, nll != nullptr ? nll + r0 : nullptr,
-                                 logits_out != nullptr ? logits_out + r0 * V : nullptr, st));
+    VCL_TRY(rows(r0, m));
   }
+  return 0;
+}
+
+// Scoring tail of vcl_llm_score (B*S rows): the cross-entropy kernel over each chunk; the per-row NLL waits in l_attn
+// (dead) for the mean over all rows. labels [B,S] (HF's shift: column s is scored against labels[b, s+1]) or null.
+int score_tail(vcl_handle* h, int B, int S, const int64_t* labels, bf16* logits_out, float* nll_out,
+               float* loss_out, cudaStream_t st) {
+  const int V = h->cfg.vocab, Vp = h->vocab_padded();
+  const long long M = (long long)B * S;
+  const long long* lab = reinterpret_cast<const long long*>(labels);
+  float* nll = labels != nullptr ? reinterpret_cast<float*>(h->l_attn) : nullptr;
+  VCL_TRY(vocab_tail(h, M, [&](long long r0, int m) {
+    return launch_cross_entropy(h->l_qkv, Vp, V, lab, r0, m, S, nll != nullptr ? nll + r0 : nullptr,
+                                logits_out != nullptr ? logits_out + r0 * V : nullptr, st);
+  }, st));
   if (labels != nullptr) VCL_TRY(launch_nll_mean(nll, lab, M, S, nll_out, loss_out, st));
   return 0;
 }
@@ -1368,6 +1376,37 @@ int vcl_llm_slots_prefill_chunk(vcl_handle* h, int n, const int32_t* slots_host,
                         next_tok, as_stream(stream));
 }
 
+// The checks of a packed continuation of cached sequences (vcl_llm_slots_prefill_append, vcl_llm_slots_score_append):
+// sequence i is len_host[i] rows at start_host[i] .. of slot slots_host[i]; slots distinct, start >= 1 (new_ok: >= 0,
+// a sequence new to its slot), 1..512 rows inside max_seq, and all rows inside the activations. M / S_max: the rows
+// and the longest sequence.
+static int check_tails(vcl_handle* h, const char* name, int n, const int32_t* slots_host, const int32_t* start_host,
+                       const int32_t* len_host, bool new_ok, long long* M_out, int* S_max_out) {
+  const vcl_config& c = h->cfg;
+  long long M = 0;
+  int S_max = 0;
+  for (int i = 0; i < n; ++i) {
+    const int s = slots_host[i], st0 = start_host[i], len = len_host[i];
+    VCL_REQUIRE(s >= 0 && s < h->n_slots_max(), "%s: slot %d outside 0..%d", name, s, h->n_slots_max() - 1);
+    for (int j = 0; j < i; ++j) VCL_REQUIRE(slots_host[j] != s, "%s: slot %d is given twice", name, s);
+    if (new_ok)
+      VCL_REQUIRE(st0 >= 0, "%s: sequence %d starts at %d, below 0", name, i, st0);
+    else
+      VCL_REQUIRE(st0 >= 1, "%s: sequence %d starts at %d; a tail continues a cached sequence (start >= 1; "
+                  "vcl_llm_slots_prefill takes new prompts)", name, i, st0);
+    VCL_REQUIRE(len >= 1 && len <= 512, "%s: sequence %d has %d rows, outside 1..512", name, i, len);
+    VCL_REQUIRE(st0 + len <= c.max_seq, "%s: sequence %d: rows %d..%d outside the cache (max_seq %d)", name, i, st0,
+                st0 + len - 1, c.max_seq);
+    M += len;
+    S_max = len > S_max ? len : S_max;
+  }
+  VCL_REQUIRE(M <= (long long)c.max_batch * h->act_seq(), "%s: %lld rows exceed the activations (max_batch %d * %d)",
+              name, M, c.max_batch, h->act_seq());
+  *M_out = M;
+  *S_max_out = S_max;
+  return 0;
+}
+
 int vcl_llm_slots_prefill_append(vcl_handle* h, int n, const int32_t* slots_host, const int32_t* start_host,
                                  const int32_t* len_host, const int64_t* ids, int32_t* next_tok, void* stream) {
   VCL_REQUIRE(h != nullptr, "vcl_llm_slots_prefill_append: null handle");
@@ -1380,27 +1419,94 @@ int vcl_llm_slots_prefill_append(vcl_handle* h, int n, const int32_t* slots_host
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
   long long M = 0;
   int S_max = 0;
-  for (int i = 0; i < n; ++i) {
-    const int s = slots_host[i], st0 = start_host[i], len = len_host[i];
-    VCL_REQUIRE(s >= 0 && s < h->n_slots_max(), "vcl_llm_slots_prefill_append: slot %d outside 0..%d", s,
-                h->n_slots_max() - 1);
-    for (int j = 0; j < i; ++j)
-      VCL_REQUIRE(slots_host[j] != s, "vcl_llm_slots_prefill_append: slot %d is given twice", s);
-    VCL_REQUIRE(st0 >= 1, "vcl_llm_slots_prefill_append: sequence %d starts at %d; a tail continues a cached "
-                "sequence (start >= 1; vcl_llm_slots_prefill takes new prompts)", i, st0);
-    VCL_REQUIRE(len >= 1 && len <= 512, "vcl_llm_slots_prefill_append: sequence %d has %d rows, outside 1..512", i, len);
-    VCL_REQUIRE(st0 + len <= c.max_seq, "vcl_llm_slots_prefill_append: sequence %d: rows %d..%d outside the cache "
-                "(max_seq %d)", i, st0, st0 + len - 1, c.max_seq);
-    M += len;
-    S_max = len > S_max ? len : S_max;
-  }
-  VCL_REQUIRE(M <= (long long)c.max_batch * h->act_seq(), "vcl_llm_slots_prefill_append: %lld rows exceed the "
-              "activations (max_batch %d * %d)", M, c.max_batch, h->act_seq());
+  VCL_TRY(check_tails(h, "vcl_llm_slots_prefill_append", n, slots_host, start_host, len_host, false, &M, &S_max));
   // the kernel of the contiguous continued prefill (attention_prefill_tc_supported): wgmma up to 512 keys
   std::vector<int> flash(n);
   for (int i = 0; i < n; ++i) flash[i] = start_host[i] + len_host[i] > 512;
   return packed_prefill(h, n, slots_host, start_host, len_host, flash.data(), M, S_max, ids, nullptr, nullptr,
                         next_tok, as_stream(stream));
+}
+
+int vcl_llm_slots_fork(vcl_handle* h, int n, const int32_t* src_host, const int32_t* dst_host, const int32_t* cols_host,
+                       void* stream) {
+  VCL_REQUIRE(h != nullptr, "vcl_llm_slots_fork: null handle");
+  VCL_REQUIRE(!h->paged(), "vcl_llm_slots_fork: this handle has a paged KV cache (kv_blocks %d); forks copy slots of "
+              "the contiguous cache", h->cfg.kv_blocks);
+  VCL_REQUIRE(n >= 0 && n <= h->n_slots_max(), "vcl_llm_slots_fork: n=%d outside 0..%d (%s)", n, h->n_slots_max(),
+              h->slots_note().c_str());
+  VCL_REQUIRE(n == 0 || (src_host && dst_host && cols_host), "vcl_llm_slots_fork: null argument");
+  for (int i = 0; i < n; ++i) {
+    const int s = src_host[i], d = dst_host[i], c = cols_host[i];
+    VCL_REQUIRE(s >= 0 && s < h->n_slots_max() && d >= 0 && d < h->n_slots_max(), "vcl_llm_slots_fork: fork %d: slots "
+                "%d -> %d outside 0..%d", i, s, d, h->n_slots_max() - 1);
+    VCL_REQUIRE(c >= 0 && c <= h->cfg.max_seq, "vcl_llm_slots_fork: fork %d: %d columns outside 0..max_seq %d", i, c,
+                h->cfg.max_seq);
+    for (int j = 0; j < n; ++j) {
+      VCL_REQUIRE(d != src_host[j], "vcl_llm_slots_fork: slot %d is both a destination (fork %d) and a source (fork "
+                  "%d)", d, i, j);
+      VCL_REQUIRE(j >= i || d != dst_host[j], "vcl_llm_slots_fork: slot %d is the destination of forks %d and %d", d, j,
+                  i);
+    }
+  }
+  if (n == 0 || h->cfg.llm_layers == 0) return 0;
+  // kv_fork_kernel (beam.cu) copies columns 0 .. ctl[3] - 1 of its forks at first = 1, step 0, ctl[0] = 0: one launch
+  // per distinct column count, each with its control block {0, 0, -1, cols} and its (src, dst) list
+  std::vector<int> cols;
+  for (int i = 0; i < n; ++i)
+    if (cols_host[i] > 0 && std::find(cols.begin(), cols.end(), cols_host[i]) == cols.end()) cols.push_back(cols_host[i]);
+  if (cols.empty()) return 0;
+  const size_t g = cols.size();
+  std::vector<int> hb(4 * g + 2 * (size_t)n);
+  std::vector<int> first(g), count(g, 0);
+  int2* pairs = reinterpret_cast<int2*>(hb.data() + 4 * g);
+  for (size_t k = 0, e = 0; k < g; ++k) {
+    hb[4 * k] = 0; hb[4 * k + 1] = 0; hb[4 * k + 2] = -1; hb[4 * k + 3] = cols[k];
+    first[k] = (int)e;
+    for (int i = 0; i < n; ++i)
+      if (cols_host[i] == cols[k]) { pairs[e++] = make_int2(src_host[i], dst_host[i]); ++count[k]; }
+  }
+  cudaStream_t st = as_stream(stream);
+  int* d = nullptr;
+  VCL_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&d), hb.size() * sizeof(int), st));
+  int rc = 0;
+  if (cudaMemcpyAsync(d, hb.data(), hb.size() * sizeof(int), cudaMemcpyHostToDevice, st) != cudaSuccess) {
+    set_last_error("vcl_llm_slots_fork: control copy failed");
+    rc = -2;
+  }
+  for (size_t k = 0; k < g && rc == 0; ++k)
+    rc = launch_kv_fork(h->kcache, h->vcache, (long long)h->cache_layer_elems(), h->cfg.llm_layers, h->cfg.llm_heads,
+                        h->cfg.max_seq, reinterpret_cast<const int2*>(d + 4 * g) + first[k], count[k], d + 4 * k, 0, 1,
+                        st);
+  cudaFreeAsync(d, st);
+  return rc;
+}
+
+int vcl_llm_slots_score_append(vcl_handle* h, int n, const int32_t* slots_host, const int32_t* start_host,
+                               const int32_t* len_host, const int64_t* ids, const int64_t* labels, float* lp_out,
+                               uint8_t* greedy_out, void* stream) {
+  VCL_REQUIRE(h != nullptr, "vcl_llm_slots_score_append: null handle");
+  const vcl_config& c = h->cfg;
+  VCL_REQUIRE(!h->paged(), "vcl_llm_slots_score_append: this handle has a paged KV cache (kv_blocks %d); candidate "
+              "scoring runs on the contiguous cache", c.kv_blocks);
+  VCL_REQUIRE(n >= 1 && n <= h->n_slots_max(), "vcl_llm_slots_score_append: n=%d outside 1..%d (%s)", n,
+              h->n_slots_max(), h->slots_note().c_str());
+  VCL_REQUIRE(slots_host && start_host && len_host && ids && labels && lp_out && greedy_out,
+              "vcl_llm_slots_score_append: null argument");
+  VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
+  long long M = 0;
+  int S_max = 0;
+  VCL_TRY(check_tails(h, "vcl_llm_slots_score_append", n, slots_host, start_host, len_host, true, &M, &S_max));
+  // the kernel of the contiguous continued prefill: wgmma up to 512 keys, the packed flash instance past them; no
+  // token is sampled (next_tok null), the tail below scores every row
+  std::vector<int> flash(n);
+  for (int i = 0; i < n; ++i) flash[i] = start_host[i] + len_host[i] > 512;
+  cudaStream_t st = as_stream(stream);
+  VCL_TRY(packed_prefill(h, n, slots_host, start_host, len_host, flash.data(), M, S_max, ids, nullptr, nullptr, nullptr,
+                         st));
+  const long long* lab = reinterpret_cast<const long long*>(labels);
+  return vocab_tail(h, M, [&](long long r0, int m) {
+    return launch_label_logprobs(h->l_qkv, h->vocab_padded(), c.vocab, lab + r0, m, lp_out + r0, greedy_out + r0, st);
+  }, st);
 }
 
 int vcl_llm_slot_decode(vcl_handle* h, const int32_t* first_tok, const int32_t* pos_host, int n_slots, int n_new,
@@ -1887,6 +1993,15 @@ int vcl_op_gemm_ex(const void* A, int64_t lda, const void* W, int64_t ldw, void*
               reinterpret_cast<const bf16*>(residual), ldr, M, N, K, act, as_stream(stream), block_n, cluster);
 }
 
+int vcl_op_label_logprobs(const void* logits, int64_t ld, int rows, int V, const int64_t* labels, float* lp_out,
+                          uint8_t* greedy_out, void* stream) {
+  if (check_device() != 0) return -2;
+  VCL_REQUIRE(logits && labels && lp_out && greedy_out, "vcl_op_label_logprobs: null argument");
+  VCL_REQUIRE(rows >= 0, "vcl_op_label_logprobs: rows=%d", rows);
+  return launch_label_logprobs(reinterpret_cast<const bf16*>(logits), ld, V, reinterpret_cast<const long long*>(labels),
+                               rows, lp_out, greedy_out, as_stream(stream));
+}
+
 int vcl_op_cross_entropy(const void* logits, int64_t ld, const int64_t* labels, int rows, int V, float* nll_out,
                          float* loss_out, void* stream) {
   if (check_device() != 0) return -2;
@@ -2271,45 +2386,52 @@ int vcl_op_attention_cached(const void* q, int64_t q_ld, const void* k, const vo
   return rc;
 }
 
-int vcl_op_attention_packed(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int H, int s_max,
-                            int n_slots, int n, const int32_t* slots_host, const int32_t* start_host,
-                            const int32_t* len_host, const int32_t* flash_host, const int32_t* table_host,
-                            int table_row, int n_blocks, int64_t blk, void* stream) {
+}  // extern "C"
+
+namespace {
+
+// vcl_op_attention_packed (flash_host as given: the flash kernel on a paged cache only) and vcl_op_attention_appended
+// (appended: the contiguous cache, each sequence on the kernel of the contiguous continued prefill, the flash kernel
+// when it ends past 512 keys)
+int op_attention_packed(const char* name, const void* q, int64_t q_ld, const void* k, const void* v, void* o, int H,
+                        int s_max, int n_slots, int n, const int32_t* slots_host, const int32_t* start_host,
+                        const int32_t* len_host, const int32_t* flash_host, const int32_t* table_host, int table_row,
+                        int n_blocks, int64_t blk, bool appended, void* stream) {
   if (check_device() != 0) return -2;
   VCL_REQUIRE(q && k && v && o && slots_host && start_host && len_host,
-              "vcl_op_attention_packed: q, k, v, o, slots, starts and lengths are required");
+              "%s: q, k, v, o, slots, starts and lengths are required", name);
   VCL_REQUIRE(aligned16(q) && aligned16(k) && aligned16(v) && aligned16(o),
-              "vcl_op_attention_packed: q, k, v and o must be 16-byte aligned");
-  VCL_REQUIRE(H >= 1 && s_max >= 1 && n_slots >= 1, "vcl_op_attention_packed: H=%d s_max=%d n_slots=%d", H, s_max,
-              n_slots);
-  VCL_REQUIRE(q_ld >= (int64_t)H * 128 && q_ld % 8 == 0, "vcl_op_attention_packed: q_ld=%lld is below H*128 = %d or "
-              "not a multiple of 8", (long long)q_ld, H * 128);
-  VCL_REQUIRE(n >= 1 && n <= PACK_SEQ_MAX, "vcl_op_attention_packed: n=%d sequences outside 1..%d", n, PACK_SEQ_MAX);
+              "%s: q, k, v and o must be 16-byte aligned", name);
+  VCL_REQUIRE(H >= 1 && s_max >= 1 && n_slots >= 1, "%s: H=%d s_max=%d n_slots=%d", name, H, s_max, n_slots);
+  VCL_REQUIRE(q_ld >= (int64_t)H * 128 && q_ld % 8 == 0, "%s: q_ld=%lld is below H*128 = %d or not a multiple of 8",
+              name, (long long)q_ld, H * 128);
+  VCL_REQUIRE(n >= 1 && n <= PACK_SEQ_MAX, "%s: n=%d sequences outside 1..%d", name, n, PACK_SEQ_MAX);
   const bool paged = table_host != nullptr;
   if (paged) {
     VCL_REQUIRE(table_row >= (s_max + 127) / 128 && n_blocks >= 1 && blk >= (int64_t)H * 128 * 128 && blk % 8 == 0,
-                "vcl_op_attention_packed: table_row=%d (needs >= %d), n_blocks=%d or blk=%lld (needs a multiple of 8 "
-                ">= H*128*128) out of range", table_row, (s_max + 127) / 128, n_blocks, (long long)blk);
+                "%s: table_row=%d (needs >= %d), n_blocks=%d or blk=%lld (needs a multiple of 8 >= H*128*128) out of "
+                "range", name, table_row, (s_max + 127) / 128, n_blocks, (long long)blk);
   }
+  std::vector<int> flash(n);
   long long M = 0;
   int S_max = 0;
   for (int i = 0; i < n; ++i) {
     const int s = slots_host[i], st0 = start_host[i], len = len_host[i];
-    const bool fl = flash_host != nullptr && flash_host[i];
-    VCL_REQUIRE(s >= 0 && s < n_slots, "vcl_op_attention_packed: sequence %d: slot %d outside 0..%d", i, s,
-                n_slots - 1);
-    VCL_REQUIRE(len >= 1 && len <= 512, "vcl_op_attention_packed: sequence %d has %d rows, outside 1..512", i, len);
-    VCL_REQUIRE(st0 >= 0 && st0 + len <= s_max, "vcl_op_attention_packed: sequence %d: positions %d..%d outside the "
-                "cache (s_max %d)", i, st0, st0 + len - 1, s_max);
-    VCL_REQUIRE(fl || st0 + len <= 512, "vcl_op_attention_packed: sequence %d ends at %d keys; the wgmma kernel "
-                "attends at most 512", i, st0 + len);
-    VCL_REQUIRE(!fl || paged, "vcl_op_attention_packed: sequence %d is on the flash kernel, which reads a paged "
-                "cache only", i);
+    const bool fl = appended ? st0 + len > 512 : flash_host != nullptr && flash_host[i];
+    flash[i] = fl;
+    VCL_REQUIRE(s >= 0 && s < n_slots, "%s: sequence %d: slot %d outside 0..%d", name, i, s, n_slots - 1);
+    VCL_REQUIRE(len >= 1 && len <= 512, "%s: sequence %d has %d rows, outside 1..512", name, i, len);
+    VCL_REQUIRE(st0 >= 0 && st0 + len <= s_max, "%s: sequence %d: positions %d..%d outside the cache (s_max %d)", name,
+                i, st0, st0 + len - 1, s_max);
+    VCL_REQUIRE(fl || st0 + len <= 512, "%s: sequence %d ends at %d keys; the wgmma kernel attends at most 512", name,
+                i, st0 + len);
+    VCL_REQUIRE(!fl || paged || appended, "%s: sequence %d is on the flash kernel, which reads a paged cache only",
+                name, i);
     if (paged) {
       for (int kb = 0; kb < (st0 + len + 127) / 128; ++kb) {
         const int blk_id = table_host[(size_t)s * table_row + kb];
-        VCL_REQUIRE(blk_id >= 0 && blk_id < n_blocks, "vcl_op_attention_packed: table[%d][%d] = %d outside the pool "
-                    "(0..%d)", s, kb, blk_id, n_blocks - 1);
+        VCL_REQUIRE(blk_id >= 0 && blk_id < n_blocks, "%s: table[%d][%d] = %d outside the pool (0..%d)", name, s, kb,
+                    blk_id, n_blocks - 1);
       }
     }
     M += len;
@@ -2318,7 +2440,7 @@ int vcl_op_attention_packed(const void* q, int64_t q_ld, const void* k, const vo
   VCL_TRY(op_attention_init());
   // one stream-ordered block: the packed-row map, then (paged) the block table
   std::vector<int> hb(pack_elems(M) + (paged ? (size_t)n_slots * table_row : 0), 0);
-  const int pack_attn = fill_pack_map(hb.data(), n, slots_host, start_host, len_host, flash_host);
+  const int pack_attn = fill_pack_map(hb.data(), n, slots_host, start_host, len_host, flash.data());
   if (paged) memcpy(hb.data() + pack_elems(M), table_host, (size_t)n_slots * table_row * sizeof(int));
   cudaStream_t st = as_stream(stream);
   int* d = nullptr;
@@ -2333,6 +2455,25 @@ int vcl_op_attention_packed(const void* q, int64_t q_ld, const void* k, const vo
       st);
   VCL_CUDA_OK(cudaFreeAsync(d, st));
   return rc;
+}
+
+}  // namespace
+
+extern "C" {
+
+int vcl_op_attention_packed(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int H, int s_max,
+                            int n_slots, int n, const int32_t* slots_host, const int32_t* start_host,
+                            const int32_t* len_host, const int32_t* flash_host, const int32_t* table_host,
+                            int table_row, int n_blocks, int64_t blk, void* stream) {
+  return op_attention_packed("vcl_op_attention_packed", q, q_ld, k, v, o, H, s_max, n_slots, n, slots_host, start_host,
+                             len_host, flash_host, table_host, table_row, n_blocks, blk, false, stream);
+}
+
+int vcl_op_attention_appended(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int H, int s_max,
+                              int n_slots, int n, const int32_t* slots_host, const int32_t* start_host,
+                              const int32_t* len_host, void* stream) {
+  return op_attention_packed("vcl_op_attention_appended", q, q_ld, k, v, o, H, s_max, n_slots, n, slots_host,
+                             start_host, len_host, nullptr, nullptr, 0, 0, 0, true, stream);
 }
 
 }  // extern "C"

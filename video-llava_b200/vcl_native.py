@@ -131,6 +131,9 @@ _SIGNATURES = {
                                             POINTER(c_int32), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "vcl_llm_slots_prefill_append": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32),
                                              c_void_p, c_void_p, c_void_p]),
+    "vcl_llm_slots_fork": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32), c_void_p]),
+    "vcl_llm_slots_score_append": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32),
+                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "vcl_llm_slot_decode": (c_int, [c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_void_p, c_void_p]),
     "vcl_llm_set_sampling": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_float), POINTER(c_int32),
                                      POINTER(c_uint64), c_void_p]),
@@ -159,6 +162,9 @@ _SIGNATURES = {
                                         POINTER(c_int32), POINTER(c_int32), POINTER(c_int32), POINTER(c_int32),
                                         POINTER(c_int32), c_int, c_int, c_int64, c_void_p]),
     "vcl_op_cross_entropy": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "vcl_op_label_logprobs": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "vcl_op_attention_appended": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                          POINTER(c_int32), POINTER(c_int32), POINTER(c_int32), c_void_p]),
     "vcl_op_gemm": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
                             c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "vcl_op_gemm_ex": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
@@ -300,6 +306,20 @@ def op_cross_entropy(logits, labels, V=None, want_loss=True):
     check(lib().vcl_op_cross_entropy(c_void_p(logits.data_ptr()), logits.stride(0), ptr(lab), rows,
                                      ld if V is None else V, ptr(nll), ptr(loss), cur_stream()))
     return nll, loss
+
+
+def op_label_logprobs(logits, labels, V=None):
+    """The scoring kernel of candidate scoring alone (vcl_op_label_logprobs): logits [rows, ld] bf16 (the first V
+    columns, default all), labels [rows] int64 -> (lp [rows] fp32, greedy [rows] bool) on the device: the greedy
+    log-prob rule at each label, and whether it is the lowest-index arg-max of its row."""
+    rows, ld = logits.shape
+    assert logits.dtype == torch.bfloat16 and logits.stride(1) == 1
+    lab = labels.to(device=logits.device, dtype=torch.int64).contiguous()
+    lp = torch.empty(rows, dtype=torch.float32, device=logits.device)
+    greedy = torch.empty(rows, dtype=torch.uint8, device=logits.device)
+    check(lib().vcl_op_label_logprobs(c_void_p(logits.data_ptr()), logits.stride(0), rows, ld if V is None else V,
+                                      ptr(lab), ptr(lp), ptr(greedy), cur_stream()))
+    return lp, greedy.bool()
 
 
 def _seeds(seeds, n):
@@ -597,6 +617,20 @@ def op_attention_packed(q, k, v, slots, starts, lens, flash=None, table=None, n_
                                         int(s_max), n_slots, n, _ints(slots), _ints(starts), _ints(lens),
                                         None if flash is None else _ints(flash), tab, row, int(n_blocks), int(blk),
                                         cur_stream()))
+    return o
+
+
+def op_attention_appended(q, k, v, slots, starts, lens, out=None):
+    """The attention of candidate scoring alone (vcl_op_attention_appended): op_attention_packed on a contiguous cache
+    k / v [n_slots, H, s_max, 128], each sequence on the kernel the contiguous continued prefill takes (flash past 512
+    keys). Returns o [sum lens, H*128] (out if given)."""
+    n_slots, H, s_max, _ = k.shape
+    assert k.is_contiguous() and v.shape == k.shape and v.is_contiguous()
+    qp, q_ld = _rows_view(q, "q")
+    o = out if out is not None else torch.empty(sum(int(x) for x in lens), H * 128, dtype=torch.bfloat16,
+                                                device=q.device)
+    check(lib().vcl_op_attention_appended(qp, q_ld, ptr(k), ptr(v), ptr(o), H, int(s_max), n_slots, len(slots),
+                                          _ints(slots), _ints(starts), _ints(lens), cur_stream()))
     return o
 
 
@@ -1078,6 +1112,34 @@ class Engine:
         check(lib().vcl_llm_slots_prefill_append(self._h, n, arr(slots), arr(starts), arr(lens), ptr(packed), ptr(tok),
                                                  cur_stream()))
         return tok
+
+    def slots_fork(self, src, dst, cols):
+        """Copy columns 0 .. cols[i] - 1 of cache slot src[i] into slot dst[i], every layer, K and V (vcl_llm_slots_fork;
+        contiguous cache). Host lists of equal length."""
+        n = len(src)
+        if not (len(dst) == len(cols) == n):
+            raise VclError(f"{n} sources, {len(dst)} destinations, {len(cols)} column counts")
+        arr = lambda v: (c_int32 * max(n, 1))(*[int(x) for x in v])   # noqa: E731
+        check(lib().vcl_llm_slots_fork(self._h, n, arr(src), arr(dst), arr(cols), cur_stream()))
+
+    def slots_score_append(self, slots, starts, ids_list, labels_list, lp_out=None, greedy_out=None):
+        """Continue slot slots[i]'s cached columns 0 .. starts[i] - 1 with ids_list[i] ([len_i]) and score row t of it
+        against labels_list[i][t], all in one packed pass (vcl_llm_slots_score_append; contiguous cache). Returns
+        (lp [sum len_i] fp32, greedy [sum len_i] uint8) on the device, sequence i's rows after sequence i - 1's."""
+        n = len(slots)
+        if not (len(starts) == len(ids_list) == len(labels_list) == n):
+            raise VclError(f"{n} slots, {len(starts)} starts, {len(ids_list)} sequences, {len(labels_list)} labels")
+        ids, lens, packed, _, _, _ = self._packed_args(ids_list, [None] * n, [0] * n, None)
+        lab = torch.cat([torch.as_tensor(t).reshape(-1).to("cuda", torch.int64) for t in labels_list])
+        if lab.numel() != packed.numel():
+            raise VclError(f"{lab.numel()} labels for {packed.numel()} rows")
+        M = packed.numel()
+        lp = lp_out if lp_out is not None else torch.empty(M, dtype=torch.float32, device="cuda")
+        greedy = greedy_out if greedy_out is not None else torch.empty(M, dtype=torch.uint8, device="cuda")
+        arr = lambda v: (c_int32 * n)(*[int(x) for x in v])   # noqa: E731
+        check(lib().vcl_llm_slots_score_append(self._h, n, arr(slots), arr(starts), arr(lens), ptr(packed), ptr(lab),
+                                               ptr(lp), ptr(greedy), cur_stream()))
+        return lp, greedy
 
     def slot_decode(self, first_tok, positions, n_new, out=None):
         """Slot b is fed first_tok[b] (device int32 [n_slots]) at positions[b] (host ints: the tokens its cache

@@ -45,6 +45,7 @@ import vcl_native as vn  # noqa: E402
 from ..constants import (DEFAULT_VID_END_TOKEN, DEFAULT_VID_START_TOKEN,  # noqa: E402
                          DEFAULT_VIDEO_PATCH_TOKEN)
 from . import inflight  # noqa: E402
+from . import candidates as candidate_scoring  # noqa: E402
 from .multimodal_projector.builder import build_vision_projector  # noqa: E402
 
 
@@ -1266,6 +1267,34 @@ class VideoChatGPTLlamaForCausalLM:
                 self._set_bans(eng, list(range(n_slots)), [None] * n_slots, eos, [0] * n_slots)
             if lps.on:
                 eng.set_logprobs(list(range(n_slots)), [-1] * n_slots)
+
+    @torch.no_grad()
+    def score_candidates(self, input_ids, candidates, video_spatio_temporal_features=None, attention_mask=None):
+        """Rank candidate answers by log-likelihood with one prefill per prompt (multiple-choice video QA).
+
+        input_ids: B prompts, a [B, S] tensor (left-padded with attention_mask, as generate takes them; the padding is
+        stripped on the host) or a list of B 1-D prompts. candidates[b]: the n_b >= 1 options of prompt b, each a 1-D
+        sequence of at least one token id (text only). video_spatio_temporal_features: None, [B, NV, C], or a list of B
+        entries (each [NV, C] or None).
+        Returns, per prompt, dict(logprob=float64 [n_b], greedy=bool [n_b], token_logprobs=[float32 [L_bj], ...]):
+        lm-eval's loglikelihood (the summed log-prob and whether every token is greedy) plus the per-token values. The
+        log-prob of option token c_t is the greedy log-prob rule of generate(logprobs=...) on the bf16 logits row that
+        predicts it, (x - m) - logf(W) in fp32; greedy means every c_t is the lowest-index arg-max of its row; a row
+        without a finite maximum gives NaN and greedy False; logprob sums the per-token values in float64, in order.
+        Each prompt is prefilled once into a cache slot, its columns are copied into the slots of its other options,
+        and the options of up to max_slots sequences run as one packed continuation (candidates.py). An option's values
+        do not depend on its slot, its neighbours, the prompt order or how the call is split into rounds.
+        Rejected before any device work, naming the prompt and option: an empty option list or option, an id outside
+        the vocabulary, a video placeholder id inside an option, an option over 512 tokens, a prompt plus option longer
+        than max_seq, and features whose shapes do not match the prompts. Afterwards there is no turn for
+        generate_continue to continue. A paged model raises NotImplementedError."""
+        self._not_paged("score_candidates")
+        eng = self._ensure_engine(need_llm=True)
+        q = candidate_scoring.check(self, input_ids, candidates, video_spatio_temporal_features, attention_mask,
+                                    eng.NV)
+        self._last_out, self._pos, self.last_logprobs = None, 0, None
+        self._after_beams, self.last_beam_scores = False, None
+        return candidate_scoring.score(self, eng, q)
 
     def end_session(self, key=None):
         """Forget the conversation kept under `key` (every kept conversation when None): its cache blocks return to
