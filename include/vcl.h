@@ -618,6 +618,17 @@ int vcl_op_beam_select(const float* logits, int64_t ld, int B, int num_beams, in
 int vcl_op_layernorm(const void* x, void* y, const void* w, const void* b, int rows, int D, float eps,
                      void* stream);
 int vcl_op_rmsnorm(const void* x, void* y, const void* w, int rows, int D, float eps, void* stream);
+/* The patch gather of vcl_clip_encode on its own: n_frames frames of image x image pixels (fmt VCL_PIXELS_BF16_NCHW:
+ * normalised bf16 [n][3][image][image]; VCL_PIXELS_U8_NHWC: raw uint8 [n][image][image][3], normalised with the CLIP
+ * mean / std) -> out [n_frames * P][KP] bf16, P = (image / patch)^2. Row n * P + py * G + px is patch (py, px) of
+ * frame n, column c * patch^2 + i * patch + j its pixel (channel c, row i, column j); columns 3 * patch^2 .. KP - 1
+ * are zero. KP >= 3 * patch^2. */
+int vcl_op_im2col(const void* pixels, int fmt, void* out, int n_frames, int image, int patch, int KP, void* stream);
+/* The CLIP embedding and pre-LayerNorm of vcl_clip_encode on its own: row n * (P + 1) + t of h [n_frames * (P + 1)][D]
+ * is LayerNorm(bf16(src + pos[t])) with weight w, bias b and eps, where src is cls [D] for t = 0 and row n * P + t - 1
+ * of patch_out [n_frames * P][D] otherwise; pos [P + 1][D]. All bf16; D a multiple of 8, at most 8192. */
+int vcl_op_clip_embed_ln(const void* patch_out, const void* cls, const void* pos, const void* w, const void* b,
+                         void* h, int n_frames, int P, int D, float eps, void* stream);
 /* q,k,v,o: [B,S,H,hd] contiguous bf16 */
 int vcl_op_attention(const void* q, const void* k, const void* v, void* o, int B, int S, int H,
                      int head_dim, float scale, int causal, void* stream);

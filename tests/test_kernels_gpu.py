@@ -120,6 +120,29 @@ def test_layernorm_rmsnorm(rows, D):
     assert frac > 0.999, frac
 
 
+@pytest.mark.parametrize("rows,D", [(7, 1024), (25700, 1024), (300, 768)])
+def test_layernorm_offset_and_outlier_rows(rows, D):
+    """LayerNorm of rows on a large common offset and of rows with a few outlier channels (magnitude ~1000), as
+    CLIP's residual stream carries them into layer_norm1 / 2: a one-pass variance E[x^2] - E[x]^2 loses them. At
+    D = 1024 this is the warp-per-row kernel of the encoder's layer norms, at 768 the block kernel. Bar as for the
+    CLIP pre-LN (_vit_ref.ln_check): 1 bf16 ulp of the fp64 value, at least 99 % bit-identical."""
+    import _vit_ref as V
+    g = torch.Generator(device=_dev()).manual_seed(rows + D)
+    x = torch.randn(rows, D, device=_dev(), generator=g)
+    r = torch.arange(rows, device=_dev())
+    x[r % 4 == 0] = 700 + 8 * x[r % 4 == 0]
+    x[r % 4 == 2] = 1000 + 3 * x[r % 4 == 2]
+    ch = torch.randint(0, D, (rows, 4), device=_dev(), generator=g)
+    odd = (r % 3 == 1).nonzero()[:, 0]
+    x[odd[:, None], ch[odd]] = -1000 + 100 * torch.rand(len(odd), 4, device=_dev(), generator=g)
+    x = x.bfloat16()
+    w = (1 + 0.05 * torch.randn(D, device=_dev(), generator=g)).bfloat16()
+    b = (0.02 * torch.randn(D, device=_dev(), generator=g)).bfloat16()
+    y = vn.op_layernorm(x, w, b, 1e-5)
+    torch.cuda.synchronize()
+    V.ln_check(y, x, w, b, 1e-5, f"layernorm rows={rows} D={D}")
+
+
 @pytest.mark.parametrize("B,S,H,hd,causal", [(3, 257, 16, 64, False), (2, 448, 4, 128, True),
                                              (1, 64, 2, 128, True), (5, 577, 2, 64, False),
                                              (1, 100, 3, 128, True),
@@ -165,25 +188,6 @@ def test_attention_prefill_tcgen05_vs_mma_sync(B, S, H):
     per_row = (o_tc.float() - o_mma.float()).flatten(2).norm(dim=2) / o_mma.float().flatten(2).norm(dim=2)
     assert rel < 4e-3 and per_row.max().item() < 2e-2, (rel, per_row.max().item())
     assert not torch.equal(o_tc, o_mma) or S <= 16      # two different kernels did run
-
-
-@pytest.mark.parametrize("n,S,H", [(3, 257, 16), (2, 257, 2), (4, 200, 3), (2, 129, 1), (2, 256, 2), (100, 257, 16)])
-def test_attention_vit_tcgen05(n, S, H):
-    torch.manual_seed(S + H)
-    dev = _dev()
-    C = H * 64
-    qkv = torch.randn(n * S, 3 * C, device=dev).bfloat16()
-    o = vn.op_attention_vit(qkv, n, S, H)
-    q, k, v = [qkv[:, i * C:(i + 1) * C].float().view(n, S, H, 64).permute(0, 2, 1, 3) for i in range(3)]
-    s = ((q @ k.transpose(-1, -2)).bfloat16().float() * 0.125).bfloat16().float()
-    p = torch.softmax(s, -1).bfloat16().float()
-    ref = (p @ v).permute(0, 2, 1, 3).reshape(n * S, C)
-    d = (o.float() - ref).abs()
-    rel = _rel(o, ref)
-    per_row = (o.float() - ref).norm(dim=1) / ref.norm(dim=1)
-    worst = per_row.argmax().item()
-    assert rel < 6e-3, f"rel={rel:.3e} worst row {worst} (token {worst % S}) err {per_row[worst].item():.3e} maxabs {d.max().item():.3e}"
-    assert per_row.max().item() < 3e-2, f"worst row {worst} (token {worst % S}) err {per_row[worst].item():.3e}"
 
 
 @pytest.mark.parametrize("B,N,K,norm,res", [(1, 4096, 4096, False, True), (1, 12288, 4096, True, False),

@@ -2191,6 +2191,25 @@ int vcl_op_rmsnorm(const void* x, void* y, const void* w, int rows, int D, float
                         reinterpret_cast<const bf16*>(w), rows, D, eps, as_stream(stream));
 }
 
+int vcl_op_im2col(const void* pixels, int fmt, void* out, int n_frames, int image, int patch, int KP, void* stream) {
+  if (check_device() != 0) return -2;
+  VCL_REQUIRE(pixels && out, "vcl_op_im2col: null argument");
+  VCL_REQUIRE(n_frames >= 0 && patch >= 1 && image >= patch, "vcl_op_im2col: n_frames=%d image=%d patch=%d", n_frames,
+              image, patch);
+  return launch_im2col(pixels, fmt, reinterpret_cast<bf16*>(out), n_frames, image, patch, KP, as_stream(stream));
+}
+
+int vcl_op_clip_embed_ln(const void* patch_out, const void* cls, const void* pos, const void* w, const void* b,
+                         void* h, int n_frames, int P, int D, float eps, void* stream) {
+  if (check_device() != 0) return -2;
+  VCL_REQUIRE(patch_out && cls && pos && w && b && h, "vcl_op_clip_embed_ln: null argument");
+  VCL_REQUIRE(n_frames >= 0 && P >= 1, "vcl_op_clip_embed_ln: n_frames=%d P=%d", n_frames, P);
+  return launch_clip_embed_ln(reinterpret_cast<const bf16*>(patch_out), reinterpret_cast<const bf16*>(cls),
+                              reinterpret_cast<const bf16*>(pos), reinterpret_cast<const bf16*>(w),
+                              reinterpret_cast<const bf16*>(b), reinterpret_cast<bf16*>(h), n_frames, P, D, eps,
+                              as_stream(stream));
+}
+
 int vcl_op_attention(const void* q, const void* k, const void* v, void* o, int B, int S, int H,
                      int head_dim, float scale, int causal, void* stream) {
   if (check_device() != 0) return -2;

@@ -185,6 +185,9 @@ _SIGNATURES = {
                                    c_void_p]),
     "vcl_op_layernorm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "vcl_op_rmsnorm": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
+    "vcl_op_im2col": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "vcl_op_clip_embed_ln": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                     c_float, c_void_p]),
     "vcl_op_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                  c_float, c_int, c_void_p]),
     "vcl_op_attention_vit": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
@@ -288,9 +291,33 @@ def op_attention(q, k, v, scale, causal):
     return o
 
 
-def op_attention_vit(qkv, n_frames, S, H):
-    """qkv: [n_frames*S, 3*H*64] bf16 -> [n_frames*S, H*64] (ViT attention)."""
-    out = torch.empty(n_frames * S, H * 64, dtype=torch.bfloat16, device=qkv.device)
+def op_im2col(pixels, fmt, KP, patch=14, out=None):
+    """The patch gather alone (vcl_op_im2col): pixels [N,3,I,I] bf16 (fmt PIXELS_BF16_NCHW) or [N,I,I,3] uint8
+    (PIXELS_U8_NHWC) -> [N * (I / patch)^2, KP] bf16 (out if given)."""
+    n, image = pixels.shape[0], pixels.shape[2]
+    P = (image // patch) ** 2
+    if out is None:
+        out = torch.empty(n * P, KP, dtype=torch.bfloat16, device=pixels.device)
+    check(lib().vcl_op_im2col(ptr(pixels), fmt, ptr(out), n, image, patch, KP, cur_stream()))
+    return out
+
+
+def op_clip_embed_ln(patch_out, cls, pos, w, b, n_frames, eps, out=None):
+    """The CLIP embedding + pre-LN alone (vcl_op_clip_embed_ln): patch_out [n_frames * P, D], cls [D], pos [P + 1, D],
+    w / b [D], all bf16 -> h [n_frames * (P + 1), D] bf16 (out if given)."""
+    D = cls.shape[-1]
+    P = pos.shape[0] - 1
+    if out is None:
+        out = torch.empty(n_frames * (P + 1), D, dtype=torch.bfloat16, device=cls.device)
+    check(lib().vcl_op_clip_embed_ln(ptr(patch_out), ptr(cls), ptr(pos), ptr(w), ptr(b), ptr(out), n_frames, P, D, eps,
+                                     cur_stream()))
+    return out
+
+
+def op_attention_vit(qkv, n_frames, S, H, out=None):
+    """qkv: [n_frames*S, 3*H*64] bf16 -> [n_frames*S, H*64] (ViT attention; out if given)."""
+    if out is None:
+        out = torch.empty(n_frames * S, H * 64, dtype=torch.bfloat16, device=qkv.device)
     check(lib().vcl_op_attention_vit(ptr(qkv), ptr(out), n_frames, S, H, cur_stream()))
     return out
 
