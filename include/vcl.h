@@ -36,6 +36,9 @@ extern "C" {
 #define VCL_PIXELS_BF16_NCHW 0 /* [N,3,H,W] bf16, already CLIP-normalised (inference.py:86-89)   */
 #define VCL_PIXELS_U8_NHWC 1   /* [N,H,W,3] uint8 raw frames; (x/255-mean)/std applied on device */
 
+#define VCL_RESIZE_NEAREST 0   /* torch.nn.functional.interpolate(mode="nearest"): load_video's resize           */
+#define VCL_RESIZE_BICUBIC 1   /* PIL.Image.resize(BICUBIC): CLIPImageProcessor's shortest-edge resize           */
+
 #define VCL_WEIGHTS_BF16 0     /* the checkpoint's bf16 weights, as loaded (the default)                      */
 #define VCL_WEIGHTS_FP8_E4M3 1 /* the language model's streamed matrices as E4M3 codes with power-of-two row
                                   scales (vcl_load_llm_weights_ex)                                            */
@@ -125,7 +128,9 @@ int vcl_load_llm_weights_ex(vcl_handle* h, const vcl_tensor* tensors, int n, int
  * hidden_states[0], the post-pre_layrnorm embeddings). hidden_out is [n_frames, 1+P, C] bf16 with
  * the CLS row kept, as in HF; callers slice [:, 1:]. frame_h / frame_w are the height and width of
  * the frames behind `pixels`: they must equal image_size (the image processor of the reference
- * resizes and crops, inference.py:86; raw frames of another size are an error, never read out of bounds). */
+ * resizes and crops, inference.py:86; frames of another size are an error, never read out of bounds). Raw frames of
+ * another size go through vcl_resize_frames first: its bicubic resize and center crop are the processor's, bit for
+ * bit, so the tower sees exactly the pixels the CPU-preprocessed path gives it. */
 int vcl_clip_encode(vcl_handle* h, const void* pixels, int pixel_format, int n_frames, int frame_h, int frame_w,
                     int n_layers, void* hidden_out, void* stream);
 
@@ -135,6 +140,24 @@ int vcl_clip_encode(vcl_handle* h, const void* pixels, int pixel_format, int n_f
  * [T,1+P,C] hidden state can be pooled in place by pointing at row 1. out is [n_temporal+P, C]. */
 int vcl_st_pool(const void* feats, int in_dtype, int64_t frame_stride, int64_t patch_stride, int T,
                 int P, int C, int n_temporal, void* out, int out_dtype, void* stream);
+
+/* Resize raw frames on the device: in [n, in_h, in_w, 3] uint8 -> out [n, crop_h, crop_w, 3] uint8, equal to
+ * resize(in)[:, crop_top : crop_top + crop_h, crop_left : crop_left + crop_w] where resize makes them out_h x out_w.
+ *   VCL_RESIZE_NEAREST  torch.nn.functional.interpolate(mode="nearest") on CPU tensors, as load_video runs it on its
+ *                       frames (video_chatgpt/eval/model_utils.py:39-44): src = min(floor(fp32(dst) * fp32(in) /
+ *                       fp32(out)), in - 1). Bit for bit.
+ *   VCL_RESIZE_BICUBIC  PIL.Image.resize(BICUBIC), CLIPImageProcessor's resize (inference.py:86): separable passes
+ *                       with PIL's double-precision weights and 22-bit fixed point, uint8 between the passes, a pass
+ *                       whose size does not change skipped. Bit for bit.
+ * Only the crop window is computed. ws is device scratch of at least vcl_resize_frames_workspace_bytes(...) bytes,
+ * 16-byte aligned (0 bytes, and ws may be null, for nearest or a same-size bicubic). Rejected with a message, before
+ * any device work: an unknown mode; n, a frame side or an output side outside 1..8192; a crop that is empty or not
+ * inside the resized frame; a too small workspace; a null pointer. The workspace-size entry returns SIZE_MAX for
+ * arguments the resize rejects (vcl_last_error says why). Neither call synchronises or allocates. */
+size_t vcl_resize_frames_workspace_bytes(int n, int in_h, int in_w, int mode, int out_h, int out_w, int crop_top,
+                                         int crop_left, int crop_h, int crop_w);
+int vcl_resize_frames(const uint8_t* in, int n, int in_h, int in_w, int mode, int out_h, int out_w, int crop_top,
+                      int crop_left, int crop_h, int crop_w, uint8_t* out, void* ws, size_t ws_bytes, void* stream);
 
 /* vcl_clip_encode(clip_layers) + CLS drop + vcl_st_pool in one call: the per-video body of
  * scripts/save_spatio_temporal_clip_features.py:105-123 and inference.py:93-95. */

@@ -138,6 +138,14 @@ int launch_st_pool(const void* feats, int in_dtype, long long frame_stride, long
                    int T, int P, int C, int n_temporal, void* out, int out_dtype,
                    cudaStream_t stream);
 
+// ---- frame_resize.cu ----------------------------------------------------------------------------
+// vcl_resize_frames: the arguments are checked here (SIZE_MAX / -1 with the message set when they are bad)
+size_t resize_frames_workspace(int n, int in_h, int in_w, int mode, int out_h, int out_w, int crop_top, int crop_left,
+                               int crop_h, int crop_w);
+int launch_resize_frames(const uint8_t* in, int n, int in_h, int in_w, int mode, int out_h, int out_w, int crop_top,
+                         int crop_left, int crop_h, int crop_w, uint8_t* out, void* ws, size_t ws_bytes,
+                         cudaStream_t stream);
+
 // ---- cross_entropy.cu ---------------------------------------------------------------------------
 // Rows row0 .. row0+rows-1 of a labelled batch whose logits [rows, ld] (first V columns) are at `logits`:
 // nll[i] = -bf16(log_softmax(row i)[label]) (0 for label -100 or no target, NaN for a label outside 0..V-1),

@@ -2,6 +2,7 @@
 // sequences for the three stages of the hot path (SURVEY.md section 3.2):
 //   vcl_clip_encode    CLIP ViT over the sampled frames
 //   vcl_st_pool        spatio-temporal mean pool
+//   vcl_resize_frames  raw frames to the tower's size (load_video's and the image processor's resizes)
 //   vcl_llm_prefill / vcl_llm_decode_step / vcl_llm_generate   projector + splice + LLaMA
 // Host code here only sequences kernels on the caller's stream; it never synchronises on the
 // compute path and never touches a CPU implementation.
@@ -1212,6 +1213,19 @@ int vcl_st_pool(const void* feats, int in_dtype, int64_t frame_stride, int64_t p
   if (check_device() != 0) return -2;
   return launch_st_pool(feats, in_dtype, frame_stride, patch_stride, T, P, C, n_temporal, out, out_dtype,
                         as_stream(stream));
+}
+
+size_t vcl_resize_frames_workspace_bytes(int n, int in_h, int in_w, int mode, int out_h, int out_w, int crop_top,
+                                         int crop_left, int crop_h, int crop_w) {
+  return resize_frames_workspace(n, in_h, in_w, mode, out_h, out_w, crop_top, crop_left, crop_h, crop_w);
+}
+
+int vcl_resize_frames(const uint8_t* in, int n, int in_h, int in_w, int mode, int out_h, int out_w, int crop_top,
+                      int crop_left, int crop_h, int crop_w, uint8_t* out, void* ws, size_t ws_bytes, void* stream) {
+  VCL_REQUIRE(in && out, "vcl_resize_frames: null argument (%s)", in ? "out" : "in");
+  if (check_device() != 0) return -2;
+  return launch_resize_frames(in, n, in_h, in_w, mode, out_h, out_w, crop_top, crop_left, crop_h, crop_w, out, ws,
+                              ws_bytes, as_stream(stream));
 }
 
 int vcl_clip_features(vcl_handle* h, const void* pixels, int pixel_format, int n_frames, int frame_h, int frame_w,

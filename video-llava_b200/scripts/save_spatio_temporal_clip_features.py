@@ -5,7 +5,8 @@
 
 The per-video device work is ONE C-ABI call (vcl_clip_features: ViT over all sampled frames + CLS
 drop + pool), instead of the reference's 32-frame chunks with a D2H copy of every chunk; the on-disk
-format is unchanged (pickle of a [100+P, 1024] float16 ndarray, resume-by-skip, flush every 512).
+format is unchanged (pickle of a [100+P, 1024] float16 ndarray, resume-by-skip, flush every 512). The sampled
+frames are resized on the GPU (load_video(..., device="cuda")) rather than on the CPU, with identical pixels.
 """
 import argparse
 import os
@@ -31,9 +32,9 @@ def get_spatio_temporal_features(features, num_temporal_tokens=100):
     return vn.st_pool(f, num_temporal_tokens, torch.float16).cpu().numpy()
 
 
-def extract_video(engine, frames_u8: np.ndarray) -> np.ndarray:
-    """frames_u8 [T,H,W,3] uint8 (T <= 100) -> pooled [100+P, 1024] float16 ndarray."""
-    px = torch.from_numpy(np.ascontiguousarray(frames_u8)).cuda()
+def extract_video(engine, frames_u8) -> np.ndarray:
+    """frames_u8 [T,H,W,3] uint8 ndarray or CUDA tensor (T <= 100) -> pooled [100+P, 1024] float16 ndarray."""
+    px = frames_u8 if isinstance(frames_u8, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(frames_u8)).cuda()
     return engine.clip_features(px, torch.float16).cpu().numpy()
 
 
@@ -73,7 +74,8 @@ def main():
         if os.path.exists(f"{args.clip_feat_path}/{vid}.pkl"):
             continue
         try:
-            frames = np.stack([np.asarray(im) for im in load_video(f"{args.video_dir_path}/{name}", shape=(size, size))])
+            # the native frames go to the GPU and are resized there (load_video's nearest rule, bit for bit)
+            frames = load_video(f"{args.video_dir_path}/{name}", shape=(size, size), device="cuda")
             pending[vid] = extract_video(engine, frames)
             counter += 1
         except Exception as e:

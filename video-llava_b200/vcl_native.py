@@ -18,6 +18,7 @@ LIB_PATH = os.path.join(_HERE, "libvcl.so")
 
 DTYPE_F16, DTYPE_BF16 = 0, 1
 PIXELS_BF16_NCHW, PIXELS_U8_NHWC = 0, 1
+RESIZE_MODES = {"nearest": 0, "bicubic": 1}   # VCL_RESIZE_NEAREST (load_video's torch rule), VCL_RESIZE_BICUBIC (PIL's)
 PROJ_LINEAR, PROJ_MLP2X_GELU = 0, 1
 NO_VIDEO = -2 ** 31          # vid_start value of a text-only row (VCL_NO_VIDEO)
 ACT_NONE, ACT_QGELU, ACT_GELU, ACT_SWIGLU = 0, 1, 2, 3
@@ -110,6 +111,9 @@ _SIGNATURES = {
     "vcl_st_pool": (c_int, [c_void_p, c_int, c_int64, c_int64, c_int, c_int, c_int, c_int, c_void_p,
                             c_int, c_void_p]),
     "vcl_clip_features": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
+    "vcl_resize_frames_workspace_bytes": (ctypes.c_size_t, [c_int] * 10),
+    "vcl_resize_frames": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                  c_void_p, c_void_p, ctypes.c_size_t, c_void_p]),
     "vcl_llm_prefill": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
                                 c_void_p, c_void_p, c_void_p]),
     "vcl_llm_prefill_states": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
@@ -256,6 +260,32 @@ def st_pool(features: torch.Tensor, n_temporal: int = 100, out_dtype: torch.dtyp
     check(lib().vcl_st_pool(c_void_p(features.data_ptr()), _dtype_code(features.dtype),
                             features.stride(0), features.stride(1), T, P, C, n_temporal,
                             ptr(out), _dtype_code(out_dtype), cur_stream()))
+    return out
+
+
+def resize_frames(frames: torch.Tensor, size, mode: str, crop=None) -> torch.Tensor:
+    """Resize raw frames on the device (vcl_resize_frames): frames uint8 [T,H,W,3] CUDA -> the frames resized to
+    size = (h, w) with mode "nearest" (torch.nn.functional.interpolate's rule, as load_video) or "bicubic" (PIL's
+    BICUBIC, as CLIPImageProcessor), then cut to crop = (top, left, crop_h, crop_w) (default: the whole frame):
+    uint8 [T, crop_h, crop_w, 3], bit for bit what the CPU resize gives."""
+    if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
+        raise VclError("resize_frames: frames must be a uint8 [T,H,W,3] tensor, got "
+                       f"{getattr(frames, 'dtype', type(frames))} {tuple(getattr(frames, 'shape', ()))}")
+    if not frames.is_cuda:
+        raise VclError("resize_frames: frames must live on the GPU (no CPU fallback)")
+    if mode not in RESIZE_MODES:
+        raise VclError(f"resize_frames: unknown mode {mode!r}: one of {sorted(RESIZE_MODES)}")
+    frames = frames.contiguous()
+    n, in_h, in_w = frames.shape[:3]
+    out_h, out_w = (int(v) for v in size)
+    top, left, crop_h, crop_w = (0, 0, out_h, out_w) if crop is None else (int(v) for v in crop)
+    geo = (n, in_h, in_w, RESIZE_MODES[mode], out_h, out_w, top, left, crop_h, crop_w)
+    ws_bytes = lib().vcl_resize_frames_workspace_bytes(*geo)
+    if ws_bytes == ctypes.c_size_t(-1).value:
+        raise VclError(f"libvcl error: {lib().vcl_last_error().decode()}")
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=frames.device) if ws_bytes else None
+    out = torch.empty(n, crop_h, crop_w, 3, dtype=torch.uint8, device=frames.device)
+    check(lib().vcl_resize_frames(ptr(frames), *geo, ptr(out), ptr(ws), ws_bytes, cur_stream()))
     return out
 
 

@@ -1,7 +1,7 @@
 """Model / tower / tokenizer construction and frame sampling
 (reference: video_chatgpt/eval/model_utils.py).
 
-    load_video(vis_path, n_clips=1, num_frm=100, shape=(224,224))   :12-52
+    load_video(vis_path, n_clips=1, num_frm=100, shape=(224,224))   :12-52  (+ device=: resize on the GPU)
     get_seq_frames(total_num_frames, desired_num_frames)            :55-79
     initialize_model(model_name, projection_path=None)              :82-150
 
@@ -15,6 +15,8 @@ import os
 import numpy as np
 import torch
 
+import vcl_native as vn
+
 from ..constants import DEFAULT_VID_END_TOKEN, DEFAULT_VID_START_TOKEN, DEFAULT_VIDEO_PATCH_TOKEN
 from ..model import VideoChatGPTLlamaForCausalLM
 
@@ -26,8 +28,11 @@ def get_seq_frames(total_num_frames, desired_num_frames):
     return [(edges[i] + edges[i + 1]) // 2 for i in range(desired_num_frames)]
 
 
-def load_video(vis_path, n_clips=1, num_frm=100, shape=(224, 224)):
-    """<= num_frm uniformly sampled frames as PIL images, nearest-neighbour resized to `shape`."""
+def load_video(vis_path, n_clips=1, num_frm=100, shape=(224, 224), device=None):
+    """<= num_frm uniformly sampled frames as PIL images, nearest-neighbour resized to `shape`.
+    With a device (e.g. "cuda"), the sampled frames are uploaded at their native size and resized there
+    (vcl_resize_frames): the result is a uint8 [T,h,w,3] tensor on the device, equal to
+    np.stack(load_video(...)) of the default path."""
     try:
         from decord import VideoReader, cpu
     except ImportError as e:                                   # decord is not in this image
@@ -40,6 +45,11 @@ def load_video(vis_path, n_clips=1, num_frm=100, shape=(224, 224)):
     n = min(total, num_frm)
     arr = vr.get_batch(get_seq_frames(total, n)).asnumpy()
     h, w = shape
+    if device is not None:
+        t = torch.from_numpy(np.ascontiguousarray(arr)).to(device)
+        if t.shape[1] != h or t.shape[2] != w:
+            t = vn.resize_frames(t, (h, w), "nearest")
+        return t
     if arr.shape[-3] != h or arr.shape[-2] != w:
         t = torch.from_numpy(arr).permute(0, 3, 1, 2).float()
         t = torch.nn.functional.interpolate(t, size=(h, w))

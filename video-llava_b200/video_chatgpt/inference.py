@@ -13,6 +13,7 @@ import vcl_native as vn
 from .constants import (DEFAULT_TRANSCRIPT_START, DEFAULT_VID_END_TOKEN, DEFAULT_VID_START_TOKEN,
                         DEFAULT_VIDEO_PATCH_TOKEN)
 from .model.utils import KeywordsStoppingCriteria
+from .preprocess import processor_resize
 from .video_conversation import SeparatorStyle, conv_templates
 
 
@@ -76,7 +77,10 @@ def video_chatgpt_infer(video_frames, question, conv_mode, model, vision_tower, 
     from the seed; without one, generate samples step by step from torch's RNG as before.
     top_p / repetition_penalty (off by default, 1.0): HF's nucleus sampling and repetition penalty, passed to
     generate. no_repeat_ngram_size / bad_words_ids / min_new_tokens (off by default, None): HF's banned tokens, passed
-    to generate."""
+    to generate.
+    video_frames: a list of PIL images, as in the reference, or the raw frames as a uint8 [T,H,W,3] tensor at any
+    size (e.g. load_video(..., device="cuda")), whose resize and crop then run on the device, bit for bit those of
+    the image processor (video_chatgpt.preprocess)."""
     if model.get_model().vision_config.use_vid_start_end:
         qs = question + "\n" + DEFAULT_VID_START_TOKEN + DEFAULT_VIDEO_PATCH_TOKEN * video_token_len + DEFAULT_VID_END_TOKEN
     else:
@@ -91,8 +95,12 @@ def video_chatgpt_infer(video_frames, question, conv_mode, model, vision_tower, 
 
     feats = feature_cache.get(video_key) if (feature_cache is not None and video_key is not None) else None
     if feats is None:
-        image_tensor = image_processor.preprocess(video_frames, return_tensors="pt")["pixel_values"]
-        image_tensor = image_tensor.to(torch.bfloat16).cuda()
+        if isinstance(video_frames, torch.Tensor):
+            # raw frames: the processor's resize and crop on the device, normalised by the tower's uint8 path
+            image_tensor = processor_resize(video_frames, image_processor, vision_tower.config.image_size)
+        else:
+            image_tensor = image_processor.preprocess(video_frames, return_tensors="pt")["pixel_values"]
+            image_tensor = image_tensor.to(torch.bfloat16).cuda()
         with torch.no_grad():
             outs = vision_tower(image_tensor, output_hidden_states=True)
             frame_features = outs.hidden_states[-2][:, 1:]
