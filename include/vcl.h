@@ -72,7 +72,10 @@ typedef struct vcl_config {
   /* capacities */
   int32_t max_frames;    /* frames per vcl_clip_encode call */
   int32_t max_batch;     /* clips per prefill / decode call */
-  int32_t max_seq;       /* prompt + generated tokens per clip */
+  int32_t max_seq;       /* prompt + generated tokens per clip. vcl_create rejects a max_seq whose scores decode
+                            attention cannot hold in shared memory at some clip count 1 .. max_batch (on 132
+                            SMs: 40384 / 20192 / 10096 columns at 4 / 2 / 1 CTAs per head, 39168 / 19872 / 10016
+                            paged; one CTA per head once clips x heads exceeds 3 x the SMs) */
   int32_t max_slots;     /* in-flight cache slots (vcl_llm_slot_*): 0 = min(max_batch, 16); otherwise
                             1 .. min(max_batch, 64), anything else is rejected by vcl_create. A capacity
                             only: the decode kernel is chosen by the clip count of each call */
@@ -672,6 +675,14 @@ int vcl_kv_cache_copy(vcl_handle* h, int layer, int write, void* k, void* v, voi
 int vcl_op_decode_attention(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int B, int H,
                             int s_max, int kv_len, const int32_t* pos_dev, const int32_t* n_pad, float scale,
                             int o_xwin, void* stream);
+/* vcl_op_decode_attention on a paged pool, the kernel of a paged engine's decode: k / v are the K / V bases of one
+ * layer inside block 0 of the pool, and column c of clip b lives in block table_host[b * ceil(s_max / 128) + c / 128]
+ * (HOST memory, B rows of ceil(s_max / 128) entries, each in 0 .. n_blocks - 1; copied to the device), blocks blk
+ * elements apart, heads 128 x 128 apart inside a block. Every argument is checked before any device work. Scratch
+ * is stream-ordered. */
+int vcl_op_decode_attention_paged(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int B, int H,
+                                  int s_max, int kv_len, const int32_t* pos_dev, const int32_t* n_pad, float scale,
+                                  int o_xwin, const int32_t* table_host, int n_blocks, int64_t blk, void* stream);
 /* The prefill attention over the KV cache on its own, with the arguments a prefill of vcl_llm_prefill(_padded) or
  * vcl_llm_prefill_append builds (scale 128^-1/2, causal): clip b's S queries sit at positions start_pos ..
  * start_pos + S - 1, q [B*S][q_ld] (head h at columns h*128 ..; q_ld >= H*128, a multiple of 8), k / v caches

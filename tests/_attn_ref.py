@@ -89,6 +89,46 @@ def mean_ref(v, clip, pos, kmin):
     return out
 
 
+def equal_weight_ref(v, clip, pos, kmin):
+    """The decode kernel's exact output when all scores are equal (q = 0) and v holds small integers (the counting
+    and probe inputs), [R, H, 128] fp64 holding bf16 values. Every key then weighs e = exp(0) = 1, the fp32 sum is
+    n, p = bf16(fp32(1 / n)), and the fp32 accumulator holds c_d * p exactly (c_d the sum of the attended keys'
+    values at d, below 2^16), so element d is bf16(c_d * p)."""
+    H = v.shape[1]
+    out = torch.empty(len(clip), H, 128, dtype=torch.float64, device=v.device)
+    for c, rows, n, m in _groups(clip, pos, kmin, v.device):
+        vv = _attended(v, c, n, m.any(0), "v")
+        cnt = torch.einsum("rn,hnd->rhd", m.double(), vv)
+        assert cnt.abs().max() < 2 ** 16 and torch.equal(cnt, cnt.round()), "not an exact input"
+        p = (torch.ones((), dtype=torch.float32, device=v.device) / m.sum(1).float()).bfloat16().double()
+        out[rows] = (cnt * p[:, None, None]).bfloat16().double()
+    return out
+
+
+def probe_plan(keys, n_sets=None):
+    """The probe input's schedule for one (clip, head): the sorted keys to probe are dealt round robin over
+    n_sets >= 2 sets (default: as few as hold 128 each), so that neighbouring keys never share a set. Returns
+    [[(key, dimension), ...] per set]; key i of the list is set i % n_sets, dimension i // n_sets."""
+    keys = sorted(set(int(j) for j in keys))
+    n = max(2, (len(keys) + 127) // 128) if n_sets is None else n_sets
+    assert n >= 2 and len(keys) <= 128 * n
+    return [[(j, i // n) for i, j in enumerate(keys) if i % n == s] for s in range(n)]
+
+
+def probe_values(C, H, cols, sets, device="cpu"):
+    """v [C, H, cols, 128] bf16 for the probe input: zero, except key j of clip c, head h is one-hot at dimension d
+    for each (j, d) in sets[c][h] (None or missing: no probe). With q = 0 an output element is then 0, bf16(p) or
+    bf16(2 p): its probe was skipped, read once or read twice, and a read from the wrong address lights the wrong
+    dimension (equal_weight_ref gives the expected output)."""
+    v = torch.zeros(C, H, cols, 128, dtype=torch.bfloat16, device=device)
+    for c, per_head in enumerate(sets):
+        for h, s in enumerate(per_head):
+            if s:
+                j, d = (torch.tensor(t, device=device) for t in zip(*s))
+                v[c, h, j, d] = 1.0
+    return v
+
+
 def counting_values(C, H, cols, n_pad=None, pad_value=100.0, device="cpu"):
     """v [C, H, cols, 128] bf16 for the counting input: column j of head h is one-hot at d = (7 j + 3 h) % 128, of
     value 1 (pad_value in clip c's first n_pad[c] columns). With q = 0 every attended key weighs exactly 1 / n, so
@@ -96,11 +136,11 @@ def counting_values(C, H, cols, n_pad=None, pad_value=100.0, device="cpu"):
     j = torch.arange(cols)
     h = torch.arange(H)
     d = (7 * j[None, :] + 3 * h[:, None]) % 128                                    # [H, cols]
-    v = torch.zeros(C, H, cols, 128, dtype=torch.float32)
-    v.scatter_(3, d[None, :, :, None].expand(C, H, cols, 1), 1.0)
+    v = torch.zeros(C, H, cols, 128, dtype=torch.bfloat16, device=device)
+    v.scatter_(3, d.to(device)[None, :, :, None].expand(C, H, cols, 1), 1.0)
     for c, npd in enumerate(n_pad or []):
         v[c, :, :npd] *= pad_value
-    return v.to(device=device, dtype=torch.bfloat16)
+    return v
 
 
 def bf16_ulp(x):

@@ -141,3 +141,72 @@ def test_bf16_ulp():
     x = torch.tensor([1.0, 1.5, 0.75, 3.0e-3, 0.0, -2.0], dtype=torch.float64)
     want = torch.tensor([2 ** -7, 2 ** -7, 2 ** -8, 2.0 ** -16, 2.0 ** -133, 2 ** -6], dtype=torch.float64)
     assert torch.equal(R.bf16_ulp(x), want)
+
+
+def _bf16_p(n):
+    """the decode kernel's weight of one of n equal keys: bf16(fp32(1) / fp32(n))"""
+    return float(torch.tensor(1.0, dtype=torch.float32).div(torch.tensor(float(n), dtype=torch.float32)).bfloat16())
+
+
+def _decode_rows(kv_len, pos, n_pad):
+    """decode rows (clip b, pos = kv_len - 1 + pos[b], kmin = n_pad[b]) as test_decode_attention_gpu.py builds them"""
+    B = len(pos)
+    return (torch.arange(B), torch.tensor([kv_len - 1 + p for p in pos]), torch.tensor(n_pad))
+
+
+@pytest.mark.parametrize("kv_len,pos,n_pad", [(1, [0, 0], [0, 0]), (30, [0, 170, 3], [0, 29, 5]),
+                                              (300, [0, 77], [128, 1])])
+def test_equal_weight_closed_form_counts(kv_len, pos, n_pad):
+    """counting input, pad and out-of-range columns NaN: equal_weight_ref against a key-by-key count of the classes
+    (7 j + 3 h) % 128 over keys n_pad .. c and the rounding bf16(c_d * bf16(fp32(1 / n)))"""
+    H = 3
+    clip, p, kmin = _decode_rows(kv_len, pos, n_pad)
+    cols = int(p.max()) + 5
+    v = R.counting_values(len(pos), H, cols)
+    for b in range(len(pos)):
+        v[b, :, :n_pad[b]] = float("nan")
+        v[b, :, int(p[b]) + 1:] = float("nan")
+    got = R.equal_weight_ref(v, clip, p, kmin)
+    for b in range(len(pos)):
+        keys = range(n_pad[b], int(p[b]) + 1)
+        pb = _bf16_p(len(keys))
+        for h in range(H):
+            cnt = [0] * 128
+            for j in keys:
+                cnt[(7 * j + 3 * h) % 128] += 1
+            want = torch.tensor([c * pb for c in cnt], dtype=torch.float64).bfloat16().double()
+            assert torch.equal(got[b, h], want), (b, h)
+
+
+def test_probe_plan_covers_every_key_once_with_neighbours_apart():
+    for keys in ([5], [0, 1], list(range(3, 260)), list(range(1000, 1000 + 128 * 9 + 1)), [7, 9, 130, 131, 4000]):
+        plan = R.probe_plan(keys)
+        got = sorted(j for s in plan for j, _ in s)
+        assert got == sorted(keys)
+        where = {j: i for i, s in enumerate(plan) for j, _ in s}
+        for s in plan:
+            assert len(s) <= 128 and len({d for _, d in s}) == len(s)
+        for a, b in zip(sorted(keys), sorted(keys)[1:]):
+            assert where[a] != where[b], (a, b)
+
+
+def test_probe_closed_form():
+    """probe input: an attended probe gives bf16(p) at its dimension, an unattended one (below the floor, past the
+    last key) nothing; a probe read twice would give bf16(2 p), which is a different bf16 number"""
+    B, H, kv_len, pos, n_pad = 2, 2, 200, [0, 57], [10, 0]
+    clip, p, kmin = _decode_rows(kv_len, pos, n_pad)
+    cols = 300
+    sets = [[[(3, 0), (10, 1), (11, 2), (199, 3), (200, 4)], [(150, 127)]],
+            [[(0, 5), (256, 6), (257, 7)], None]]
+    v = R.probe_values(B, H, cols, sets)
+    got = R.equal_weight_ref(v, clip, p, kmin)
+    for b in range(B):
+        lo, hi = n_pad[b], int(p[b])
+        pb = _bf16_p(hi - lo + 1)
+        for h in range(H):
+            want = torch.zeros(128, dtype=torch.float64)
+            for j, d in sets[b][h] or []:
+                if lo <= j <= hi:
+                    want[d] += pb
+            assert torch.equal(got[b, h], want), (b, h)
+        assert float(torch.tensor(2 * pb).bfloat16()) != pb

@@ -199,7 +199,27 @@ decode_attn_cluster_kernel(const bf16* __restrict__ q, long long q_ld, const bf1
   cluster_sync_all();   // keep every CTA's shared memory alive until rank 0 has read it
 }
 
+// CTAs per (clip, head): enough CTAs to cover the SMs a few times over, no more
+int decode_split(int B, int H) {
+  const long long heads = (long long)B * H;
+  return heads <= 2 * device_num_sms() ? 4 : (heads <= 3 * device_num_sms() ? 2 : 1);
+}
+
+// dynamic shared memory of a launch whose CTAs hold the scores of up to kv_cap keys between them: the scores of a
+// CTA's share, the 16 x 128 partial outputs, its partial output, the statistics, the reduction scratch and, paged,
+// the slot's table row
+size_t decode_smem(int split, int kv_cap, int table_row) {
+  const int per = ((kv_cap + split - 1) / split + 15) / 16 * 16;   // keys per CTA, multiple of 16
+  return (size_t)(per + 16 * 128 + 128 + 2 + 8 + table_row) * sizeof(float);
+}
+
+constexpr size_t DA_SMEM_MAX = 48 * 1024;
+
 }  // namespace
+
+bool decode_attention_fits(int B, int H, int s_max, bool paged) {
+  return decode_smem(decode_split(B, H), s_max, paged ? (s_max + 127) / 128 : 0) <= DA_SMEM_MAX;
+}
 
 int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, const bf16* vcache,
                             bf16* o, long long o_ld, int B, int H, int head_dim, int s_max,
@@ -213,12 +233,12 @@ int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, c
   VCL_REQUIRE(kv_len > 0 && kv_len <= s_max, "decode attention: kv_len %d out of range", kv_len);
   // shared memory is sized for the longest sequence when the length is only known on the device
   const int kv_cap = pos_dev != nullptr ? s_max : kv_len;
-  // CTAs per head: enough CTAs to cover the SMs a few times over, no more
-  const int heads = B * H;
-  const int split = heads <= 2 * device_num_sms() ? 4 : (heads <= 3 * device_num_sms() ? 2 : 1);
+  const int split = decode_split(B, H);
   const int per = ((kv_cap + split - 1) / split + 15) / 16 * 16;   // keys per CTA, multiple of 16
-  const size_t smem = (size_t)(per + 16 * 128 + 128 + 2 + 8 + (paged ? pages.row : 0)) * sizeof(float);
-  VCL_REQUIRE(smem <= 48 * 1024, "decode attention: kv_len %d too long for the smem budget", kv_len);
+  const size_t smem = decode_smem(split, kv_cap, paged ? pages.row : 0);
+  VCL_REQUIRE(smem <= DA_SMEM_MAX, "decode attention: %s %d too long for the smem budget (%zu of %zu bytes at %d "
+              "CTAs per head for %d clips x %d heads%s)", pos_dev != nullptr ? "s_max" : "kv_len", kv_cap, smem,
+              DA_SMEM_MAX, split, B, H, paged ? ", paged" : "");
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(split, H, B);
   cfg.blockDim = dim3(DA_THREADS);

@@ -294,6 +294,9 @@ int launch_decode_attention(const bf16* q, long long q_ld, const bf16* kcache, c
                             bf16* o, long long o_ld, int B, int H, int head_dim, int s_max,
                             int kv_len, float scale, cudaStream_t stream, const int* pos_dev, bool o_xwin,
                             const int* n_pad, const KvPages& pages = KvPages());
+// whether launch_decode_attention takes B clips x H heads with pos_dev over a cache of s_max columns (its shared
+// memory is then sized for s_max keys; paged: plus the table row of ceil(s_max / 128) blocks)
+bool decode_attention_fits(int B, int H, int s_max, bool paged);
 
 // ---- decode_gemv.cu : decode-time weight streaming (1..64 new tokens) -------------------------------
 // Two ring kernels (bulk-copy ring over a slot-ordered copy of the matrix + mma.sync) behind one launcher:

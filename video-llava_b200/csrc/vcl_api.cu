@@ -406,6 +406,20 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
         VCL_REQUIRE(gemv_fits(B, m.N, m.K, m.norm),
                     "vcl_create: the %s projection [%d x %d] has no decode kernel for %d clips (1..4 clips: K <= 14336 "
                     "and the shared-memory plan)", m.name, m.N, m.K, B);
+    // the decode graphs, slot decode and in-flight batching read the positions on the device, so decode attention
+    // sizes its shared memory for max_seq keys at every clip count
+    const bool paged = c->kv_blocks > 0;
+    for (int B = 1; B <= c->max_batch; ++B) {
+      if (decode_attention_fits(B, c->llm_heads, c->max_seq, paged)) continue;
+      int lo = 1, hi = c->max_seq - 1;   // the largest max_seq that fits: fits() falls with s_max
+      while (lo < hi) {
+        const int mid = lo + (hi - lo + 1) / 2;
+        if (decode_attention_fits(B, c->llm_heads, mid, paged)) lo = mid; else hi = mid - 1;
+      }
+      VCL_REQUIRE(false, "vcl_create: max_seq %d is too long for decode attention at %d clips x %d heads%s: its "
+                  "shared memory holds at most max_seq %d there", c->max_seq, B, c->llm_heads,
+                  paged ? " (paged)" : "", lo);
+    }
   }
 
   vcl_handle* h = new vcl_handle();
@@ -2360,6 +2374,39 @@ int vcl_op_decode_attention(const void* q, int64_t q_ld, const void* k, const vo
   return launch_decode_attention(reinterpret_cast<const bf16*>(q), q_ld, reinterpret_cast<const bf16*>(k),
                                  reinterpret_cast<const bf16*>(v), reinterpret_cast<bf16*>(o), (long long)H * 128, B,
                                  H, 128, s_max, kv_len, scale, as_stream(stream), pos_dev, o_xwin != 0, n_pad);
+}
+
+int vcl_op_decode_attention_paged(const void* q, int64_t q_ld, const void* k, const void* v, void* o, int B, int H,
+                                  int s_max, int kv_len, const int32_t* pos_dev, const int32_t* n_pad, float scale,
+                                  int o_xwin, const int32_t* table_host, int n_blocks, int64_t blk, void* stream) {
+  if (check_device() != 0) return -2;
+  VCL_REQUIRE(q && k && v && o && n_pad && table_host,
+              "vcl_op_decode_attention_paged: q, k, v, o, n_pad and the table are required");
+  VCL_REQUIRE(B > 0 && H > 0 && q_ld >= (int64_t)H * 128 && q_ld % 8 == 0,
+              "vcl_op_decode_attention_paged: B=%d H=%d q_ld=%lld", B, H, (long long)q_ld);
+  VCL_REQUIRE(s_max > 0 && n_blocks >= 1 && blk >= (int64_t)H * 128 * 128 && blk % 8 == 0,
+              "vcl_op_decode_attention_paged: s_max=%d, n_blocks=%d or blk=%lld (needs a multiple of 8 >= H*128*128) "
+              "out of range", s_max, n_blocks, (long long)blk);
+  // the clips' last keys are on the device: every entry of the table may be read
+  const int row = (s_max + 127) / 128;
+  for (int b = 0; b < B; ++b)
+    for (int kb = 0; kb < row; ++kb) {
+      const int id = table_host[(size_t)b * row + kb];
+      VCL_REQUIRE(id >= 0 && id < n_blocks, "vcl_op_decode_attention_paged: table[%d][%d] = %d outside the pool "
+                  "(0..%d)", b, kb, id, n_blocks - 1);
+    }
+  cudaStream_t st = as_stream(stream);
+  int* d_table = nullptr;
+  VCL_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&d_table), (size_t)B * row * sizeof(int), st));
+  VCL_CUDA_OK(cudaMemcpyAsync(d_table, table_host, (size_t)B * row * sizeof(int), cudaMemcpyHostToDevice, st));
+  KvPages pages;
+  pages.table = d_table; pages.row = row; pages.blk = blk;
+  const int rc = launch_decode_attention(reinterpret_cast<const bf16*>(q), q_ld, reinterpret_cast<const bf16*>(k),
+                                         reinterpret_cast<const bf16*>(v), reinterpret_cast<bf16*>(o),
+                                         (long long)H * 128, B, H, 128, s_max, kv_len, scale, st, pos_dev, o_xwin != 0,
+                                         n_pad, pages);
+  VCL_CUDA_OK(cudaFreeAsync(d_table, st));
+  return rc;
 }
 
 }  // extern "C"

@@ -160,6 +160,9 @@ _SIGNATURES = {
     "vcl_kv_block_copy": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "vcl_op_decode_attention": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                         c_void_p, c_void_p, c_float, c_int, c_void_p]),
+    "vcl_op_decode_attention_paged": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                              c_int, c_void_p, c_void_p, c_float, c_int, POINTER(c_int32), c_int,
+                                              c_int64, c_void_p]),
     "vcl_op_attention_cached": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                         c_int, POINTER(c_int32), c_void_p]),
     "vcl_op_attention_packed": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
@@ -609,18 +612,34 @@ def xwin_offset(b, k, B):
     return ((k // XWIN_KC) * B + b) * XWIN_PITCH + k % XWIN_KC
 
 
-def op_decode_attention(q, k, v, kv_len, n_pad, pos_dev=None, scale=128 ** -0.5, o_xwin=False):
+def op_decode_attention(q, k, v, kv_len, n_pad, pos_dev=None, scale=128 ** -0.5, o_xwin=False, table=None,
+                        n_blocks=0, blk=0, s_max=None, out=None):
     """The decode attention kernel alone (vcl_op_decode_attention). q [B, q_ld] bf16 (head h at columns
-    h*128 ..; q_ld >= H*128), k / v [B, H, s_max, 128] bf16 caches, n_pad / pos_dev int32 [B] on the device
-    (pos_dev optional). Returns o [B, H*128], or with o_xwin the flat xwin buffer (see xwin_offset)."""
-    B, H, s_max, hd = k.shape
-    assert hd == 128 and q.shape[0] == B and q.stride(1) == 1 and v.shape == k.shape
-    if o_xwin:
+    h*128 ..; q_ld >= H*128), n_pad / pos_dev int32 [B] on the device (pos_dev optional). Contiguous cache (table
+    None): k / v [B, H, s_max, 128] bf16. Paged (vcl_op_decode_attention_paged): k / v are one layer's K / V planes of
+    block 0 of a pool (any [.., H, 128, 128] views), table [B, ceil(s_max / 128)] host ints, n_blocks blocks blk
+    elements apart, s_max the columns a clip may hold. Returns o [B, H*128], or with o_xwin the flat xwin buffer (see
+    xwin_offset); out if given."""
+    B = q.shape[0]
+    H = k.shape[-3]
+    assert k.shape[-1] == 128 and q.stride(1) == 1 and v.shape == k.shape
+    if out is not None:
+        o = out
+    elif o_xwin:
         o = torch.empty((H * 128 + XWIN_KC - 1) // XWIN_KC * B * XWIN_PITCH, dtype=torch.bfloat16, device=q.device)
     else:
         o = torch.empty(B, H * 128, dtype=torch.bfloat16, device=q.device)
-    check(lib().vcl_op_decode_attention(ptr(q), q.stride(0), ptr(k), ptr(v), ptr(o), B, H, s_max, int(kv_len),
-                                        ptr(pos_dev), ptr(n_pad), scale, int(o_xwin), cur_stream()))
+    if table is None:
+        assert k.dim() == 4 and k.shape[0] == B
+        check(lib().vcl_op_decode_attention(ptr(q), q.stride(0), ptr(k), ptr(v), ptr(o), B, H, k.shape[2],
+                                            int(kv_len), ptr(pos_dev), ptr(n_pad), scale, int(o_xwin), cur_stream()))
+    else:
+        vals = table.tolist() if hasattr(table, "tolist") else table
+        assert len(vals) == B and all(len(r) == (int(s_max) + 127) // 128 for r in vals)
+        check(lib().vcl_op_decode_attention_paged(ptr(q), q.stride(0), c_void_p(k.data_ptr()), c_void_p(v.data_ptr()),
+                                                  ptr(o), B, H, int(s_max), int(kv_len), ptr(pos_dev), ptr(n_pad),
+                                                  scale, int(o_xwin), _ints([b for r in vals for b in r]),
+                                                  int(n_blocks), int(blk), cur_stream()))
     return o
 
 
