@@ -487,6 +487,26 @@ int vcl_llm_set_logprobs(vcl_handle* h, int n, const int32_t* clips_host, const 
 int vcl_llm_read_logprobs(vcl_handle* h, int entry, int first_pos, int count, int32_t* ids_out, float* lp_out,
                           void* stream);
 
+/* Classifier-free guidance (transformers' UnbatchedClassifierFreeGuidanceLogitsProcessor; DESIGN.md section 3,
+ * "Classifier-free guidance"). vcl_llm_set_guidance writes n entries of the handle's guidance table: clip
+ * clips_host[i] is guided by the unconditional clip partner_host[i] (-1: not guided, every clip after vcl_create)
+ * with scale scale_host[i] (HOST memory, [n] each). The table lives at a fixed device address (one host-to-device
+ * copy on `stream`; allocated by the first call that guides a clip), so one captured decode graph per (clips, steps,
+ * sampler, guided) serves every setting. Every call that produces the tokens of clips 0 .. B-1 (vcl_llm_prefill(_padded)
+ * and vcl_llm_generate(_padded) with a token, vcl_llm_decode_step, vcl_llm_decode_loop, vcl_llm_slot_decode) where a
+ * clip b < B has a partner u < B then, after the logits: replaces row b with g * (lc - lu) + lu in place (lc / lu the
+ * fp32 log-softmax of the rows of b / u; vcl_op_guidance), picks the tokens (the 32-bit sampler when some entry
+ * samples or asks for log-probs or bans, vcl_llm_set_sampling_ex; the arg-max kernel otherwise), and writes b's token
+ * as u's as well, so u decodes the token b chose. logits_out receives the logits before the combination. The 1..4-clip
+ * arg-max hand-off between decode steps is off in guided calls. A table without a guided clip launches exactly the
+ * kernels of a handle that never guided. Packed and single-slot prefills are never guided.
+ * Rejected before any device work: n outside 1 .. max_batch, a clip outside 0 .. max_batch-1 or given twice, a partner
+ * below -1, outside 0 .. max_batch-1 or the clip itself, a partner that is guided itself or partners another clip (in
+ * the table as this call leaves it), a guided clip's scale that is not finite, a guided clip on a vocabulary over
+ * VCL_SAMPLE_WIDE_MAX_V. */
+int vcl_llm_set_guidance(vcl_handle* h, int n, const int32_t* clips_host, const int32_t* partner_host,
+                         const float* scale_host, void* stream);
+
 /* Beam search: transformers' _beam_search with do_sample=False (video_chatgpt/inference.py:105-112 calls HF
  * generate; DESIGN.md section 3, "Beam search"). Per step and item, with k = num_beams beams and K = 2k:
  *   lp       the greedy log-prob rule of vcl_op_sample_logprobs on each running beam's logits, bit for bit
@@ -601,6 +621,13 @@ int vcl_op_cross_entropy(const void* logits, int64_t ld, const int64_t* labels, 
  * outside 0 .. V-1, gives NaN and 0. */
 int vcl_op_label_logprobs(const void* logits, int64_t ld, int rows, int V, const int64_t* labels, float* lp_out,
                           uint8_t* greedy_out, void* stream);
+/* Classifier-free guidance on its own (vcl_llm_set_guidance's combination): out [B][ld] (device f32, the first V
+ * columns written) = logits [B][ld] (device f32), then every row b with partner_host[b] = u >= 0 (HOST memory, [B];
+ * -1: left as it is) replaced by scale_host[b] * (lc - lu) + lu, the rule of DESIGN.md section 3. Row u must not be
+ * guided itself nor partner another row; a guided row's scale must be finite; V <= VCL_SAMPLE_WIDE_MAX_V. Bit for bit
+ * the combination the decode paths run. */
+int vcl_op_guidance(const float* logits, int64_t ld, int B, int V, const int32_t* partner_host,
+                    const float* scale_host, float* out, void* stream);
 /* The sampling kernel on its own: row b of logits [B, ld] fp32 (first V columns; bf16-representable values, as
  * the lm_head writes them) is sampled with temperature_host[b] (0: greedy), top_k_host[b], seed_host[b] and the
  * Philox counter counter_host[b] (all HOST memory, [B]); tok_out [B] int32 on the device. V <= 81920. */

@@ -215,6 +215,15 @@ int launch_token_history(int* dst, const long long* ids, int n, cudaStream_t str
 // set, in one launch
 int launch_token_set(unsigned int* dst, int words, const long long* ids, int n, int V, cudaStream_t stream);
 
+// ---- guidance.cu --------------------------------------------------------------------------------
+// Classifier-free guidance (DESIGN.md section 3): every row b of logits [B][ld] (first V columns, V <=
+// VCL_SAMPLE_WIDE_MAX_V) whose partner[b] is a row u in 0 .. B-1 becomes scale[b] * (lc - lu) + lu in place, lc / lu
+// the fp32 log-softmax of rows b / u (the rule at the top of guidance.cu); one CTA per row, the others exit at once
+int launch_guidance(float* logits, long long ld, int B, int V, const int* partner, const float* scale,
+                    cudaStream_t stream);
+// tok[partner[b] * stride] = tok[b * stride] for every row b with a partner in 0 .. B-1, in one launch
+int launch_guidance_handoff(int* tok, long long stride, int B, const int* partner, cudaStream_t stream);
+
 // ---- beam.cu ------------------------------------------------------------------------------------
 // One step of beam search (HF _beam_search, greedy; DESIGN.md section 3) over B items of k beams (2 <= k <=
 // VCL_BEAM_MAX), K = 2k candidates per item. Beam r = item i * k + j reads logits row `first ? i : (map ? map[r] :

@@ -66,6 +66,8 @@ struct GraphEntry {
                        // the token histories, whose graphs serve every ban setting)
   int beam;            // beam search with this many beams per item (0: none); its step counter, scores and clip map
                        // are read on the device too (vcl_llm_beam_decode)
+  int guided;          // the guidance table has a guided clip: its graphs combine paired rows and hand the tokens on;
+                       // the partners and scales are read on the device, so one graph serves every guidance setting
   cudaGraphExec_t exec;
   long long kernels;   // kernel nodes in the graph (for vcl_launch_count)
   unsigned long long last_use;
@@ -85,6 +87,7 @@ struct StepIo {
                                   // the log-probs of the entries that ask for them
   bool beam = false;              // beam search: the logits go to beam_select and kv_fork (beam_step), which write the
   int beam_step = 0;              // tokens of the next step; beam_step is this step's index in the chunk
+  bool guided = false;            // classifier-free guidance of the clips of the guidance table (SampleAt::guided)
 };
 
 // which sampling-table entries the rows of an lm_head call use, and the cache column their tokens take
@@ -94,6 +97,9 @@ struct SampleAt {
                                                 // the arg-max kernel (h->sampler: 2 the 32-bit sampler)
   int entry0 = 0; const int* rowmap = nullptr;  // row r: entry entry0 + (rowmap ? rowmap[r] : r)
   int col = 0; const int* col_dev = nullptr;    // row r: column col + (col_dev ? col_dev[r] : 0)
+  bool guided = false;                          // rows are clips 0 .. B-1 (entry0 0, no rowmap) and the guidance
+                                                // table guides some: the rows are combined before the token is
+                                                // picked, which then goes to each guided row's partner too
 };
 
 }  // namespace
@@ -208,6 +214,26 @@ struct vcl_handle {
   int* beam_pick = nullptr;
   int beam_ctl_host[4] = {0, 0, -1, 0};
   int beam_B = 0, beam_k = 0, beam_t = 0;       // the running call (beam_k 0: none); beam_t the next step
+  // Classifier-free guidance (vcl_llm_set_guidance): [max_batch] partner clips (int32, -1: not guided) then
+  // [max_batch] scales (f32) at a fixed device address, allocated by the first call; guid_host its host copy, written
+  // whole by one host-to-device copy per call. A handle that never guides holds none and launches what it did before.
+  int* guid = nullptr;
+  std::vector<int> guid_host;
+  const int* guid_partner() const { return guid; }
+  const float* guid_scale() const { return reinterpret_cast<const float*>(guid + cfg.max_batch); }
+  // some clip of 0 .. B-1 is guided by a partner inside 0 .. B-1
+  bool guided(int B) const {
+    if (guid_host.empty()) return false;
+    for (int b = 0; b < B && b < cfg.max_batch; ++b)
+      if (guid_host[b] >= 0 && guid_host[b] < B) return true;
+    return false;
+  }
+  // the sampler a call over clips 0 .. B-1 runs: guided scores are not bf16 values, so a guided call that samples
+  // takes the 32-bit sampler (and the arg-max kernel otherwise)
+  int step_sampler(int B, bool guided_call) {
+    const int s = sampler(0, B);
+    return guided_call && s == 1 ? 2 : s;
+  }
   int lp_rows() const { return cfg.max_seq + 1; }   // a decode loop's last token may take position max_seq
   size_t lp_plane() const { return (size_t)cfg.max_batch * lp_rows() * (1 + VCL_LOGPROBS_MAX); }   // elements
 
@@ -729,7 +755,10 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
                    int32_t* tok_out, long long tok_stride, cudaStream_t st, bool partials_out = false,
                    const SampleAt& smp = SampleAt()) {
   const vcl_config& c = h->cfg;
-  VCL_REQUIRE(!(partials_out && smp.on), "sampled rows need the logits, not the partial arg-max");
+  VCL_REQUIRE(!(partials_out && (smp.on || smp.guided)), "sampled or guided rows need the logits, not the partial "
+              "arg-max");
+  VCL_REQUIRE(!smp.guided || (smp.on != 1 && smp.entry0 == 0 && smp.rowmap == nullptr),
+              "guided rows are clips 0 .. B-1 on the 32-bit sampler or the arg-max");
   GemvArgs g;
   h->lm_head_d.into(g); g.N = c.vocab; g.K = c.llm_hidden;
   GemvEpilogue e;
@@ -763,6 +792,12 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
   if (logits_out != nullptr && logits_out != h->logits)
     VCL_CUDA_OK(cudaMemcpyAsync(logits_out, h->logits, (size_t)B * c.vocab * sizeof(float),
                                 cudaMemcpyDeviceToDevice, st));
+  // guided rows: the scores the token is picked from (logits_out keeps the raw logits of both rows)
+  if (smp.guided) VCL_TRY(launch_guidance(h->logits, c.vocab, B, c.vocab, h->guid_partner(), h->guid_scale(), st));
+  auto hand_off = [&]() {
+    return smp.guided && tok_out != nullptr ? launch_guidance_handoff(tok_out, tok_stride, B, h->guid_partner(), st)
+                                            : 0;
+  };
   if (tok_out != nullptr && smp.on) {
     SampleArgs sa;
     sa.logits = h->logits; sa.ld = c.vocab; sa.V = c.vocab; sa.B = B;
@@ -782,10 +817,11 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
     if (smp.on == 3) {   // ... and the bans, over the token histories
       sa.bans = h->bans; sa.hist = h->hist; sa.hist_ld = h->lp_rows();
     }
-    return launch_sample(sa, st);
+    VCL_TRY(launch_sample(sa, st));
+    return hand_off();
   }
   if (tok_out != nullptr) VCL_TRY(launch_argmax(h->logits, tok_out, tok_stride, B, c.vocab, st));
-  return 0;
+  return hand_off();
 }
 
 // The prefill attention of one layer (llm_prefill, and vcl_op_attention_cached / _packed, which test exactly this
@@ -952,7 +988,9 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
   }
   if (logits_out != nullptr || next_tok != nullptr) {
     SampleAt smp;   // clip b (slot `slot` for B = 1) samples with its entry; its token takes column start_pos + S
-    smp.on = next_tok != nullptr ? h->sampler(slot, B) : 0; smp.entry0 = slot; smp.col = start_pos + S;
+    smp.guided = next_tok != nullptr && slot == 0 && h->guided(B);
+    smp.on = next_tok == nullptr ? 0 : slot == 0 ? h->step_sampler(B, smp.guided) : h->sampler(slot, B);
+    smp.entry0 = slot; smp.col = start_pos + S;
     VCL_TRY(lm_head_argmax(h, h->l_h + (size_t)(S - 1) * D, (long long)S * D, B, logits_out, next_tok,
                            tok_stride, st, false, smp));
   }
@@ -1096,7 +1134,7 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
     }
   }
   SampleAt smp;   // the token fed at column c_b is followed by one at column c_b + 1
-  smp.on = io.sampled; smp.col = pos + 1; smp.col_dev = pd;
+  smp.on = io.sampled; smp.col = pos + 1; smp.col_dev = pd; smp.guided = io.guided;
   VCL_TRY(lm_head_argmax(h, h->d_h, D, B, io.logits_out, io.tok_out, io.out_stride, st, io.partials_out, smp));
   if (io.beam) VCL_TRY(beam_step(h, io.beam_step, false, st));
   return 0;
@@ -1107,13 +1145,14 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
 // per-CTA partials, the next step's first q|k|v kernel reduces them, records the token and gathers
 // its embedding row. Step i feeds clip b at position h->d_pos[b] + i - 1.
 // sampled: the sampler writes tk[:, i] from the full logits, and the next step gathers from tk (fused into
-// layer 0 for 1..4 clips, the embedding kernel otherwise).
-int decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, int sampled) {
-  const bool hand_off = B <= 4 && h->cfg.llm_layers > 0 && !sampled;
+// layer 0 for 1..4 clips, the embedding kernel otherwise). guided: so do guided calls, whose rows are combined first
+// and whose tokens are handed to the partner clips.
+int decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, int sampled, bool guided) {
+  const bool hand_off = B <= 4 && h->cfg.llm_layers > 0 && !sampled && !guided;
   for (int i = 1; i < n_new; ++i) {
     StepIo io;
     io.pos_dev = h->d_pos;
-    io.sampled = sampled;
+    io.sampled = sampled; io.guided = guided;
     if (hand_off && i > 1) {
       io.tok_from_partials = true; io.tok_store = tk + (i - 1); io.store_stride = n_new;
     } else {
@@ -1140,16 +1179,19 @@ int beam_steps(vcl_handle* h, int Bk, int n_new, cudaStream_t st) {
   return 0;
 }
 
-// decode_steps from one captured graph per (B, n_new, sampled), sampled as h->sampler gives it (beam > 0: beam_steps
+// decode_steps from one captured graph per (B, n_new, sampled, guided), sampled as h->step_sampler gives it (beam > 0: beam_steps
 // with that many beams per item, one graph per (B, n_new, beam)). The positions (h->d_pos, written by the caller),
 // the pad counts (h->d_npad) and the sampling table are read on the device, so new positions, padding or sampling
 // settings replay the same graph. Bounded LRU cache (an entry holds thousands of nodes). A stream that cannot be
 // captured runs the steps eagerly.
-int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, int sampled, int beam = 0) {
-  auto steps = [&]() { return beam ? beam_steps(h, B, n_new, st) : decode_steps(h, tk, B, n_new, st, sampled); };
+int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, int sampled, int beam = 0,
+                     bool guided = false) {
+  auto steps = [&]() {
+    return beam ? beam_steps(h, B, n_new, st) : decode_steps(h, tk, B, n_new, st, sampled, guided);
+  };
   GraphEntry* ge = nullptr;
   for (auto& g : h->graphs)
-    if (g.B == B && g.n_new == n_new && g.sampled == sampled && g.beam == beam) ge = &g;
+    if (g.B == B && g.n_new == n_new && g.sampled == sampled && g.beam == beam && g.guided == (int)guided) ge = &g;
   const bool can_capture = (st != nullptr) && (st != cudaStreamLegacy);
   if (ge == nullptr && can_capture) {
     if (h->graphs.size() >= MAX_DECODE_GRAPHS) {
@@ -1181,7 +1223,7 @@ int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t 
       set_last_error("decode graph instantiate failed: %s", cudaGetErrorString(e));
       return -2;
     }
-    h->graphs.push_back({B, n_new, sampled, beam, exec, nodes, 0});
+    h->graphs.push_back({B, n_new, sampled, beam, (int)guided, exec, nodes, 0});
     ge = &h->graphs.back();
   }
   if (ge == nullptr) return steps();
@@ -1199,7 +1241,8 @@ int decode_loop(vcl_handle* h, const int32_t* first_tok, int B, int n_new, int32
   if (first_tok != tk)
     VCL_CUDA_OK(cudaMemcpy2DAsync(tk, (size_t)n_new * sizeof(int32_t), first_tok, sizeof(int32_t),
                                   sizeof(int32_t), B, cudaMemcpyDeviceToDevice, st));
-  if (n_new > 1) VCL_TRY(run_decode_steps(h, tk, B, n_new, st, h->sampler(0, B)));
+  const bool guided = h->guided(B);
+  if (n_new > 1) VCL_TRY(run_decode_steps(h, tk, B, n_new, st, h->step_sampler(B, guided), 0, guided));
   VCL_CUDA_OK(cudaMemcpyAsync(out_tokens, tk, (size_t)B * n_new * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
@@ -1292,7 +1335,8 @@ int vcl_llm_decode_step(vcl_handle* h, const int32_t* tok_in, int B, int pos, fl
   VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
   VCL_REQUIRE(B > 0 && B <= h->cfg.max_batch, "B=%d outside 1..%d", B, h->cfg.max_batch);
   StepIo io;
-  io.tok_in = tok_in; io.logits_out = logits_out; io.tok_out = tok_out; io.sampled = h->sampler(0, B);
+  io.tok_in = tok_in; io.logits_out = logits_out; io.tok_out = tok_out;
+  io.guided = h->guided(B); io.sampled = h->step_sampler(B, io.guided);
   return llm_decode_step(h, io, B, pos, as_stream(stream));
 }
 
@@ -1796,6 +1840,56 @@ int vcl_llm_set_logprobs(vcl_handle* h, int n, const int32_t* clips_host, const 
   return 0;
 }
 
+// The partner / scale checks of a guidance table (vcl_llm_set_guidance, vcl_op_guidance): partner[b] -1 or another
+// row of 0 .. n-1 that is not guided itself and partners no other row; a guided row's scale finite
+static int check_guidance(const char* name, int n, const int* partner, const float* scale) {
+  std::vector<int> owner(n, -1);
+  for (int b = 0; b < n; ++b) {
+    const int u = partner[b];
+    if (u < 0) continue;
+    VCL_REQUIRE(u < n && u != b, "%s: clip %d: partner %d outside 0..%d or the clip itself", name, b, u, n - 1);
+    VCL_REQUIRE(partner[u] < 0, "%s: clip %d: partner %d is guided itself", name, b, u);
+    VCL_REQUIRE(owner[u] < 0, "%s: clip %d: partner %d is already the partner of clip %d", name, b, u, owner[u]);
+    VCL_REQUIRE(isfinite(scale[b]), "%s: clip %d: guidance scale %g is not finite", name, b, (double)scale[b]);
+    owner[u] = b;
+  }
+  return 0;
+}
+
+int vcl_llm_set_guidance(vcl_handle* h, int n, const int32_t* clips_host, const int32_t* partner_host,
+                         const float* scale_host, void* stream) {
+  VCL_REQUIRE(h != nullptr, "vcl_llm_set_guidance: null handle");
+  const int mb = h->cfg.max_batch;
+  VCL_REQUIRE(n >= 1 && n <= mb, "vcl_llm_set_guidance: n=%d outside 1..%d", n, mb);
+  VCL_REQUIRE(clips_host && partner_host && scale_host, "vcl_llm_set_guidance: null argument");
+  std::vector<int> tab = h->guid_host;
+  if (tab.empty()) {
+    tab.assign((size_t)2 * mb, 0);
+    for (int b = 0; b < mb; ++b) tab[b] = -1;
+  }
+  float* sc = reinterpret_cast<float*>(tab.data() + mb);
+  bool on = false;
+  for (int i = 0; i < n; ++i) {
+    const int b = clips_host[i];
+    VCL_REQUIRE(b >= 0 && b < mb, "vcl_llm_set_guidance: clip %d outside 0..%d", b, mb - 1);
+    for (int j = 0; j < i; ++j) VCL_REQUIRE(clips_host[j] != b, "vcl_llm_set_guidance: clip %d is given twice", b);
+    VCL_REQUIRE(partner_host[i] >= -1, "vcl_llm_set_guidance: clip %d: partner %d", b, partner_host[i]);
+    tab[b] = partner_host[i];
+    sc[b] = partner_host[i] >= 0 ? scale_host[i] : 1.f;
+    on = on || partner_host[i] >= 0;
+  }
+  VCL_TRY(check_guidance("vcl_llm_set_guidance", mb, tab.data(), sc));
+  VCL_REQUIRE(!on || h->cfg.vocab <= VCL_SAMPLE_WIDE_MAX_V, "vcl_llm_set_guidance: guidance takes a vocabulary of at "
+              "most %d tokens (the combination's shared memory), this model has %d", VCL_SAMPLE_WIDE_MAX_V,
+              h->cfg.vocab);
+  if (!on && h->guid == nullptr) return 0;   // every clip is off already
+  if (h->guid == nullptr) VCL_TRY(dalloc(h, &h->guid, (size_t)2 * mb));
+  h->guid_host = tab;
+  VCL_CUDA_OK(cudaMemcpyAsync(h->guid, h->guid_host.data(), (size_t)2 * mb * 4, cudaMemcpyHostToDevice,
+                              as_stream(stream)));
+  return 0;
+}
+
 int vcl_llm_read_logprobs(vcl_handle* h, int entry, int first_pos, int count, int32_t* ids_out, float* lp_out,
                           void* stream) {
   VCL_REQUIRE(h && ids_out && lp_out, "vcl_llm_read_logprobs: null argument");
@@ -2161,6 +2255,35 @@ int vcl_op_beam_select(const float* logits, int64_t ld, int B, int num_beams, in
   }
   if (rc == 0) rc = launch_beam_select(a, st);
   cudaFreeAsync(scratch, st);
+  return rc;
+}
+
+// guidance alone: out = logits, then the guided rows combined in place, with the table in stream-ordered scratch
+int vcl_op_guidance(const float* logits, int64_t ld, int B, int V, const int32_t* partner_host,
+                    const float* scale_host, float* out, void* stream) {
+  VCL_REQUIRE(logits && partner_host && scale_host && out, "vcl_op_guidance: null argument");
+  if (check_device() != 0) return -2;
+  VCL_REQUIRE(B >= 1, "vcl_op_guidance: B=%d", B);
+  VCL_REQUIRE(V >= 1 && V <= VCL_SAMPLE_WIDE_MAX_V && ld >= V, "vcl_op_guidance: V=%d outside 1..%d or row pitch "
+              "%lld < V", V, VCL_SAMPLE_WIDE_MAX_V, (long long)ld);
+  for (int b = 0; b < B; ++b)
+    VCL_REQUIRE(partner_host[b] >= -1, "vcl_op_guidance: row %d: partner %d", b, partner_host[b]);
+  VCL_TRY(check_guidance("vcl_op_guidance", B, partner_host, scale_host));
+  cudaStream_t st = as_stream(stream);
+  std::vector<int> tab((size_t)2 * B);
+  memcpy(tab.data(), partner_host, (size_t)B * 4);
+  memcpy(tab.data() + B, scale_host, (size_t)B * 4);
+  int* d = nullptr;
+  VCL_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&d), tab.size() * 4, st));
+  int rc = 0;
+  if (cudaMemcpyAsync(d, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+      cudaMemcpy2DAsync(out, (size_t)ld * 4, logits, (size_t)ld * 4, (size_t)V * 4, B, cudaMemcpyDeviceToDevice, st) !=
+          cudaSuccess) {
+    set_last_error("vcl_op_guidance: copy failed");
+    rc = -2;
+  }
+  if (rc == 0) rc = launch_guidance(out, ld, B, V, d, reinterpret_cast<const float*>(d + B), st);
+  cudaFreeAsync(d, st);
   return rc;
 }
 

@@ -151,6 +151,7 @@ _SIGNATURES = {
     "vcl_llm_read_token_history": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "vcl_llm_set_logprobs": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), c_void_p]),
     "vcl_llm_read_logprobs": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "vcl_llm_set_guidance": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), POINTER(c_float), c_void_p]),
     "vcl_llm_beam_start": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_int, c_int,
                                    c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_llm_beam_decode": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
@@ -188,6 +189,8 @@ _SIGNATURES = {
     "vcl_op_sample_ex": (c_int, [c_void_p, c_int64, c_int, c_int, POINTER(c_float), POINTER(c_int32), POINTER(c_uint64),
                                  POINTER(c_int32), POINTER(c_float), POINTER(c_float), c_void_p, POINTER(c_int32),
                                  c_void_p, c_void_p, c_void_p, c_void_p]),
+    "vcl_op_guidance": (c_int, [c_void_p, c_int64, c_int, c_int, POINTER(c_int32), POINTER(c_float), c_void_p,
+                                c_void_p]),
     "vcl_op_beam_select": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                    c_void_p]),
     "vcl_op_layernorm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
@@ -466,6 +469,23 @@ def op_sample_ex(logits, temperature, top_k, seed, counter, top_p, repetition_pe
 
 
 BAN_WORDS_MAX = 1024          # include/vcl.h: VCL_BAN_WORDS_MAX, the int32 of one entry's bad-words list
+
+
+def op_guidance(logits, partner, scale):
+    """Classifier-free guidance alone (vcl_op_guidance): logits [B, V] fp32 on the device; partner / scale B host
+    values (partner -1: the row is left as it is). Returns a new [B, V] fp32 tensor whose guided rows b hold
+    scale[b] * (log_softmax(row b) - log_softmax(row partner[b])) + log_softmax(row partner[b]) by the fp32 rule of
+    DESIGN.md section 3."""
+    B, V = logits.shape
+    assert logits.dtype == torch.float32 and logits.stride(1) == 1
+    if len(partner) != B or len(scale) != B:
+        raise VclError(f"partner / scale need {B} entries each")
+    out = torch.empty_like(logits, memory_format=torch.contiguous_format)
+    if logits.stride(0) != V:
+        logits = logits.contiguous()
+    check(lib().vcl_op_guidance(c_void_p(logits.data_ptr()), V, B, V, (c_int32 * B)(*[int(u) for u in partner]),
+                                (c_float * B)(*[float(g) for g in scale]), ptr(out), cur_stream()))
+    return out
 
 
 def ban_words(words):
@@ -1006,6 +1026,17 @@ class Engine:
             raise VclError(f"{n} clips, {len(top_n)} top_n")
         check(lib().vcl_llm_set_logprobs(self._h, n, (c_int32 * n)(*[int(b) for b in clips]),
                                          (c_int32 * n)(*[int(k) for k in top_n]), cur_stream()))
+
+    # ---- classifier-free guidance ----
+    def set_guidance(self, clips, partner, scale):
+        """Entries `clips` of the guidance table (vcl_llm_set_guidance): clip clips[i] is guided by the unconditional
+        clip partner[i] (-1: off) with scale[i]. Host lists of equal length."""
+        n = len(clips)
+        if not (len(partner) == len(scale) == n):
+            raise VclError(f"{n} clips, {len(partner)} partners, {len(scale)} scales")
+        check(lib().vcl_llm_set_guidance(self._h, n, (c_int32 * n)(*[int(b) for b in clips]),
+                                         (c_int32 * n)(*[int(u) for u in partner]),
+                                         (c_float * n)(*[float(g) for g in scale]), cur_stream()))
 
     def read_logprobs(self, entry, first_pos, count, ids_out=None, lp_out=None):
         """The log-prob rows of positions first_pos .. first_pos + count - 1 of entry `entry` (vcl_llm_read_logprobs):

@@ -65,10 +65,29 @@ class VideoFeatureCache:
         return len(self._items)
 
 
+def build_prompt(question, conv_mode, video_token_len, use_vid_start_end, transcript=None, with_video=True):
+    """The conversation prompt video_chatgpt_infer sends: the question, the video span (with_video) and the transcript
+    (if any) as the user's turn of `conv_mode`. Without the video the span and the newline before it are left out;
+    the transcript is kept."""
+    qs = question
+    if with_video:
+        if use_vid_start_end:
+            qs = qs + "\n" + DEFAULT_VID_START_TOKEN + DEFAULT_VIDEO_PATCH_TOKEN * video_token_len + DEFAULT_VID_END_TOKEN
+        else:
+            qs = qs + "\n" + DEFAULT_VIDEO_PATCH_TOKEN * video_token_len
+    if transcript:
+        qs = f'{qs}\n{DEFAULT_TRANSCRIPT_START}\n"{transcript}"'
+    conv = conv_templates[conv_mode].copy()
+    conv.append_message(conv.roles[0], qs)
+    conv.append_message(conv.roles[1], None)
+    return conv.get_prompt(), conv
+
+
 def video_chatgpt_infer(video_frames, question, conv_mode, model, vision_tower, tokenizer, image_processor,
                         video_token_len, transcript=None, do_sample=True, temperature=0.2, max_new_tokens=1024,
                         video_key=None, feature_cache: "VideoFeatureCache | None" = None, seed=None, top_p=1.0,
-                        repetition_penalty=1.0, no_repeat_ngram_size=None, bad_words_ids=None, min_new_tokens=None):
+                        repetition_penalty=1.0, no_repeat_ngram_size=None, bad_words_ids=None, min_new_tokens=None,
+                        guidance_scale=None):
     """Same flow as the reference: prompt -> tokenizer -> image processor -> tower -> pool -> generate
     -> decode. `do_sample/temperature/max_new_tokens` default to the reference's hard-coded values.
     Extension (off by default): with `video_key` and a `VideoFeatureCache`, the pooled features of a
@@ -80,18 +99,17 @@ def video_chatgpt_infer(video_frames, question, conv_mode, model, vision_tower, 
     to generate.
     video_frames: a list of PIL images, as in the reference, or the raw frames as a uint8 [T,H,W,3] tensor at any
     size (e.g. load_video(..., device="cuda")), whose resize and crop then run on the device, bit for bit those of
-    the image processor (video_chatgpt.preprocess)."""
-    if model.get_model().vision_config.use_vid_start_end:
-        qs = question + "\n" + DEFAULT_VID_START_TOKEN + DEFAULT_VIDEO_PATCH_TOKEN * video_token_len + DEFAULT_VID_END_TOKEN
-    else:
-        qs = question + "\n" + DEFAULT_VIDEO_PATCH_TOKEN * video_token_len
-    if transcript:
-        qs = f'{qs}\n{DEFAULT_TRANSCRIPT_START}\n"{transcript}"'
-    conv = conv_templates[conv_mode].copy()
-    conv.append_message(conv.roles[0], qs)
-    conv.append_message(conv.roles[1], None)
-    prompt = conv.get_prompt()
+    the image processor (video_chatgpt.preprocess).
+    guidance_scale (off by default, None): classifier-free guidance against the same conversation built without the
+    video span (the transcript is kept), passed to generate as negative_prompt_ids, so every answer token is pushed
+    toward what the video, not the text alone, makes likely (visual contrastive decoding)."""
+    use_se = model.get_model().vision_config.use_vid_start_end
+    prompt, conv = build_prompt(question, conv_mode, video_token_len, use_se, transcript)
     inputs = tokenizer([prompt])
+    neg_ids = None
+    if guidance_scale is not None:
+        neg_prompt, _ = build_prompt(question, conv_mode, video_token_len, use_se, transcript, with_video=False)
+        neg_ids = torch.as_tensor(tokenizer([neg_prompt]).input_ids).cuda()
 
     feats = feature_cache.get(video_key) if (feature_cache is not None and video_key is not None) else None
     if feats is None:
@@ -120,7 +138,8 @@ def video_chatgpt_infer(video_frames, question, conv_mode, model, vision_tower, 
                                     stopping_criteria=[stopping], eos_token_id=eos if eos is not None else "config",
                                     pad_token_id=getattr(tokenizer, "pad_token_id", None), seed=seed, top_p=top_p,
                                     repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size,
-                                    bad_words_ids=bad_words_ids, min_new_tokens=min_new_tokens)
+                                    bad_words_ids=bad_words_ids, min_new_tokens=min_new_tokens,
+                                    guidance_scale=guidance_scale, negative_prompt_ids=neg_ids)
     n_diff = (input_ids != output_ids[:, :input_ids.shape[1]]).sum().item()
     if n_diff > 0:
         print(f"[Warning] {n_diff} output_ids are not the same as the input_ids")

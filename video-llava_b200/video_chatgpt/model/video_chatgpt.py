@@ -882,12 +882,99 @@ class VideoChatGPTLlamaForCausalLM:
             out.append(e)
         return out
 
+    def _guidance_args(self, guidance_scale, neg_ids, neg_mask, neg_feats, input_ids, num_beams):
+        """Checks the classifier-free guidance settings of generate on the host -> None (off: guidance_scale None or
+        1.0, as HF adds no processor then) or the scale as a float"""
+        if guidance_scale is None:
+            return None
+        g = float(guidance_scale)
+        if not math.isfinite(g):
+            raise ValueError(f"generate: guidance_scale {guidance_scale} must be a finite value (None or 1.0: off)")
+        if g == 1.0:
+            return None
+        if not (isinstance(num_beams, int) and num_beams == 1):
+            raise NotImplementedError(f"generate: guidance_scale is not supported with num_beams={num_beams!r}")
+        B = input_ids.shape[0]
+        if 2 * B > self._max_batch:
+            raise ValueError(f"generate: guidance_scale with {B} prompts needs {2 * B} cache clips (every negative "
+                             f"prompt takes one), more than max_batch {self._max_batch}")
+        V = self.config.vocab_size
+        if V > vn.SAMPLE_WIDE_MAX_V:
+            raise ValueError(f"generate: guidance_scale takes a vocabulary of at most {vn.SAMPLE_WIDE_MAX_V} tokens on "
+                             f"the device, this model has {V}")
+        if neg_ids is not None and (neg_ids.dim() != 2 or neg_ids.shape[0] != B or neg_ids.shape[1] < 1):
+            raise ValueError(f"generate: negative_prompt_ids {tuple(neg_ids.shape)} must be [B, S_neg] with B = {B}")
+        if neg_mask is not None:
+            if neg_ids is None:
+                raise ValueError("generate: negative_prompt_attention_mask needs negative_prompt_ids")
+            if tuple(neg_mask.shape) != tuple(neg_ids.shape):
+                raise ValueError(f"generate: negative_prompt_attention_mask {tuple(neg_mask.shape)} does not match "
+                                 f"negative_prompt_ids {tuple(neg_ids.shape)}")
+        if neg_feats is not None:
+            if neg_ids is None:
+                raise ValueError("generate: negative_video_spatio_temporal_features needs negative_prompt_ids with a "
+                                 "video span")
+            if neg_feats.dim() != 3 or neg_feats.shape[0] != B:
+                raise ValueError(f"generate: negative_video_spatio_temporal_features {tuple(neg_feats.shape)} must be "
+                                 f"[B, tokens, channels] with B = {B}, one row per negative prompt")
+        return g
+
+    def _guided_batch(self, ids, pads, feats, neg_ids, neg_mask, neg_feats, n_vid):
+        """The 2B rows of a guided prefill: the B prompts, then the B negative prompts (HF's default without one:
+        each prompt's last token alone), all left-padded to the longest, each negative row with its own video span
+        (negative features) or none. -> (ids2 [2B, S2], pads2 (None when nothing is padded), spans [2B], feats
+        [2B, ., .] or None, shift = S2 - S). The prompts keep their tokens; the shift extra columns in front of a
+        prompt repeat its first token and are padding."""
+        B, S = ids.shape
+        neg = ids[:, -1:] if neg_ids is None else neg_ids.to(ids.device, torch.int64)
+        Sn = neg.shape[1]
+        npad = left_padding(neg_mask, (B, Sn)) if neg_mask is not None else None
+        S2 = max(S, Sn)
+        shift = S2 - S
+        cond = torch.cat([ids[:, :1].expand(B, shift), ids], dim=1)
+        negp = torch.cat([neg[:, :1].expand(B, S2 - Sn), neg], dim=1)
+        ids2 = torch.cat([cond, negp], dim=0).contiguous()
+        pads2 = [shift + (pads[b] if pads else 0) for b in range(B)] + \
+                [S2 - Sn + (npad[b] if npad else 0) for b in range(B)]
+        cs = self._video_spans(cond, n_vid, pads2[:B]) if feats is not None else [vn.NO_VIDEO] * B
+        ns = self._video_spans(negp, n_vid, pads2[B:]) if neg_feats is not None else [vn.NO_VIDEO] * B
+        f2 = None
+        if feats is not None or neg_feats is not None:
+            like = feats if feats is not None else neg_feats
+            zero = torch.zeros(B, *like.shape[1:], dtype=torch.bfloat16, device="cuda")
+            f2 = torch.cat([zero if f is None else f.cuda().to(torch.bfloat16) for f in (feats, neg_feats)], dim=0)
+        spans = torch.tensor(cs + ns, dtype=torch.int32, device=ids.device)
+        return ids2, (pads2 if any(pads2) else None), spans, f2, shift
+
+    @staticmethod
+    def _host_guidance(cond, uncond, g):
+        """HF's UnbatchedClassifierFreeGuidanceLogitsProcessor on fp32 logits [B, V] of the prompts and of their
+        negative prompts: g * (log_softmax(cond) - log_softmax(uncond)) + log_softmax(uncond)"""
+        lc = torch.log_softmax(cond.float(), dim=-1)
+        lu = torch.log_softmax(uncond.float(), dim=-1)
+        return g * (lc - lu) + lu
+
+    @contextlib.contextmanager
+    def _guiding(self, eng, B, g):
+        """Clips 0 .. B-1 are guided by clips B .. 2B-1 with scale g (None: nothing changes) for the duration of the
+        block, and the guidance table is off again afterwards, also when the block raises"""
+        if g is None:
+            yield
+            return
+        clips = list(range(2 * B))
+        eng.set_guidance(clips, [B + b for b in range(B)] + [-1] * B, [g] * B + [1.0] * B)
+        try:
+            yield
+        finally:
+            eng.set_guidance(clips, [-1] * (2 * B), [1.0] * (2 * B))
+
     @torch.no_grad()
     def generate(self, input_ids, video_spatio_temporal_features=None, do_sample=False, temperature=1.0,
                  max_new_tokens=32, stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50,
                  attention_mask=None, seed=None, logprobs=None, top_p=1.0, repetition_penalty=1.0, num_beams=1,
                  num_return_sequences=1, length_penalty=1.0, early_stopping=False, no_repeat_ngram_size=None,
-                 bad_words_ids=None, min_new_tokens=None, **kw):
+                 bad_words_ids=None, min_new_tokens=None, guidance_scale=None, negative_prompt_ids=None,
+                 negative_prompt_attention_mask=None, negative_video_spatio_temporal_features=None, **kw):
         """Returns [B, S+n] int64 INCLUDING the prompt, like HF generate (inference.py:105-120), and
         like HF it stops at EOS (config.eos_token_id unless eos_token_id is given; None disables it):
         finished rows are padded, the call returns when every row has finished.
@@ -927,8 +1014,19 @@ class VideoChatGPTLlamaForCausalLM:
         beams (NotImplementedError), and
         a beam call must fit max_seq whole (S + max_new_tokens <= max_seq: a shorter call would move HF's max-length
         step and so change the search). num_beams must be an int 1 .. 8 on every call (a ValueError otherwise, rather
-        than a silently greedy call); num_return_sequences without beams is ignored, as it always was."""
+        than a silently greedy call); num_return_sequences without beams is ignored, as it always was.
+        guidance_scale (None or 1.0: off): HF's classifier-free guidance (UnbatchedClassifierFreeGuidanceLogitsProcessor;
+        DESIGN.md section 3). Every prompt is decoded next to an unconditional sequence, its negative prompt
+        (negative_prompt_ids [B, S_neg], left-padded by negative_prompt_attention_mask; HF's default without one is the
+        prompt's last token alone), which takes a cache clip of its own (2B <= max_batch), and the scores become
+        g * (log_softmax(cond) - log_softmax(uncond)) + log_softmax(uncond) before every other processor. Each negative
+        row runs as if alone (its positions start at its first real token). negative_video_spatio_temporal_features
+        [B, ., .]: the pooled features of a video span in the negative prompts (e.g. a noised copy); without them a
+        span is embedded as text, as generate does without features. Greedy and seeded calls guide on the device,
+        unseeded sampling on the host step by step. Not with beams (NotImplementedError)."""
         self._not_paged("generate")
+        guide = self._guidance_args(guidance_scale, negative_prompt_ids, negative_prompt_attention_mask,
+                                    negative_video_spatio_temporal_features, input_ids, num_beams)
         beams = self._beam_args(num_beams, num_return_sequences, length_penalty, early_stopping, do_sample, seed,
                                 logprobs, top_p, repetition_penalty, stopping_criteria,
                                 (no_repeat_ngram_size, bad_words_ids, min_new_tokens))
@@ -961,6 +1059,12 @@ class VideoChatGPTLlamaForCausalLM:
         if n <= 0:
             raise ValueError(f"prompt length {S} leaves no room in max_seq {self._max_seq}")
         self._pads = pads
+        self._shift = 0
+        if guide is not None:
+            return self._guided_generate(eng, ids, pads, feats, negative_prompt_ids, negative_prompt_attention_mask,
+                                         negative_video_spatio_temporal_features, guide, max_new_tokens, do_sample,
+                                         seeded, temperature, top_k, seed, top_p, penalty, bans, lp_n,
+                                         stopping_criteria, eos, pad)
         if seeded or lp_n is not None or ((penalty != 1.0 or bans) and not do_sample):
             clips = list(range(B))
             if seeded:
@@ -1012,6 +1116,55 @@ class VideoChatGPTLlamaForCausalLM:
         self._pos = S + new.shape[1] - 1
         self._last_out = torch.cat([ids, new], dim=1)
         return self._last_out
+
+    def _guided_generate(self, eng, ids, pads, feats, neg_ids, neg_mask, neg_feats, g, max_new_tokens, do_sample, seeded,
+                         temperature, top_k, seed, top_p, penalty, bans, lp_n, stopping_criteria, eos, pad):
+        """generate with guidance_scale g: one left-padded prefill of the prompts and the negative prompts (clips B ..
+        2B-1), then the device loops with the guidance table set (greedy and seeded calls; stopping criteria keep
+        _host_stops' chunking), or _stepwise with the combination on the host (unseeded sampling). The prompts' entries
+        of the sampling, ban and log-prob tables are set as an unguided call sets them; the negative clips' entries
+        stay greedy and off. Returns the prompts' rows; the cache is left as after an unguided call on the prompts
+        (padded by `shift` more columns when a negative prompt is longer), which generate_continue continues."""
+        B, S = ids.shape
+        ids2, pads2, spans, f2, shift = self._guided_batch(ids, pads, feats, neg_ids, neg_mask, neg_feats, eng.NV)
+        S2 = ids2.shape[1]
+        ctx = ids2[:B]                           # the prompts as the cache holds them
+        n = min(max_new_tokens, self._max_seq - S2)
+        if n <= 0:
+            raise ValueError(f"prompt length {S2} leaves no room in max_seq {self._max_seq}")
+        self._pads = pads2[:B] if pads2 else None
+        self._shift = shift
+        if do_sample and not seeded:
+            _, logits, _ = eng.prefill(ids2, f2, spans, want_logits=True, want_token=False, n_pad=pads2)
+            self._pos = S2
+            self._last_out = self._stepwise(eng, ctx, logits, n, do_sample, temperature, stopping_criteria, eos, pad,
+                                            top_k, top_p, penalty, bans, guidance=g)
+            return self._last_out[:, shift:]
+        clips = list(range(B))
+        if seeded:
+            samp = self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips], top_p, penalty)
+        elif penalty != 1.0:
+            samp = self._sampling(eng, clips, [0.0] * B, [0] * B, [0] * B, 1.0, penalty)
+        else:
+            samp = contextlib.nullcontext()
+        if penalty != 1.0:
+            self._token_sets(eng, [(b, ids[b]) for b in clips])
+        if bans:   # the extra padding columns hold no token (-1 matches no n-gram or word)
+            self._histories(eng, [(b, torch.cat([torch.full((shift,), -1, dtype=torch.int64, device=ids.device), ids[b]]))
+                                  for b in clips])
+        with samp, self._banning(eng, clips, bans, eos, S2 + (bans.min_new if bans else 0)), \
+                self._logprobs(eng, clips, lp_n), self._guiding(eng, B, g):
+            if eos is None and not stopping_criteria:
+                new = eng.generate(ids2, f2, spans, n, n_pad=pads2)[:B]
+                self._pos = S2 + n - 1
+                self._last_out = torch.cat([ctx, new.to(torch.int64)], dim=1)
+            else:
+                first = eng.generate(ids2, f2, spans, min(n, self._GREEDY_CHUNK), n_pad=pads2)[:B]
+                self._last_out = self._host_stops(eng, ctx, first, n, stopping_criteria, eos, pad, guided=True)
+        if lp_n is not None:   # the token after the prompt takes position S2 - n_pad[b]
+            self.last_logprobs = self._read_logprobs(eng, self._last_out[:, S2:].cpu(),
+                                                     [S2 - (pads2[b] if pads2 else 0) for b in range(B)], lp_n, eos)
+        return self._last_out[:, shift:]
 
     # beam-search steps per vcl_llm_beam_decode call between two host-side replays (see _beam_generate). Measured with
     # tools/bench_beams.py (7B shapes, one clip at S = 448, 4 beams, 256 tokens, H100 at 700 W): 6.38 / 6.11 / 6.06 /
@@ -1088,14 +1241,15 @@ class VideoChatGPTLlamaForCausalLM:
         self.last_beam_scores = scores
         return torch.cat([ids.repeat_interleave(m, dim=0), seqs.to(dev)], dim=1)
 
-    def _host_stops(self, eng, out, new, n, stopping_criteria, eos, pad):
+    def _host_stops(self, eng, out, new, n, stopping_criteria, eos, pad, guided=False):
         """The device-sampled loop of generate / generate_continue: `new` [B, c] int32 holds the first c tokens
         after the context `out` [B, L] (the first at column L). _stepwise's EOS / padding / stopping-criteria
         logic runs token by token over each chunk on the host; the device decodes the next _GREEDY_CHUNK tokens
         from the last kept (padded) token until a rule stops or n tokens are out. Returns [B, L + k]; self._pos
         ends at L + k - 1, where _stepwise leaves it (columns decoded past the stop are overwritten by a
         continuation). The sequence lives in one [B, L + n] buffer on out's device, filled by one copy per chunk;
-        a stopping criterion is called with a view of its first L + j columns, so a call costs no copy."""
+        a stopping criterion is called with a view of its first L + j columns, so a call costs no copy.
+        guided: clips B .. 2B-1 decode the negative prompts next to the B rows and are fed the same tokens."""
         dev, (B, L) = out.device, out.shape
         full = torch.empty(B, L + n, dtype=torch.int64, device=dev)
         full[:, :L] = out
@@ -1126,7 +1280,9 @@ class VideoChatGPTLlamaForCausalLM:
                 break
             m = min(self._GREEDY_CHUNK, n - k)
             last = full[:, L + k - 1].to(torch.int32).contiguous()
-            new = eng.decode_loop(last, L + k - 1, m + 1)[:, 1:]
+            if guided:
+                last = torch.cat([last, last])
+            new = eng.decode_loop(last, L + k - 1, m + 1)[:B, 1:]
         self._pos = L + k - 1
         return full[:, :L + k].clone()
 
@@ -1372,12 +1528,17 @@ class VideoChatGPTLlamaForCausalLM:
                 pads = self._pads
                 self.last_logprobs = self._read_logprobs(eng, self._last_out[:, L:].cpu(),
                                                          [L - (pads[b] if pads else 0) for b in range(B)], lp_n, eos)
-            return self._last_out
+            return self._continued()
         _, logits, _ = eng.prefill_append(tail, start, want_logits=True, want_token=False)
         self._pos = ctx.shape[1]
         self._last_out = self._stepwise(eng, ctx, logits, n, do_sample, temperature, stopping_criteria, eos, pad, top_k,
                                         top_p, penalty, bans)
-        return self._last_out
+        return self._continued()
+
+    def _continued(self):
+        """generate_continue's result: the conversation without the padding columns a guided generate added"""
+        shift = getattr(self, "_shift", 0)
+        return self._last_out[:, shift:] if shift else self._last_out
 
     @staticmethod
     def _host_processors(out, logits, sampled, temperature, top_k, top_p, penalty, bans=None, S=0):
@@ -1406,14 +1567,18 @@ class VideoChatGPTLlamaForCausalLM:
         return lg
 
     def _stepwise(self, eng, out, logits, n, do_sample, temperature, stopping_criteria, eos, pad, top_k=50, top_p=1.0,
-                  penalty=1.0, bans=None):
+                  penalty=1.0, bans=None, guidance=None):
         """One token per C-ABI call. After the loop the cache holds every returned token but the last
         (self._pos = out.shape[1] - 1), the state generate_continue starts from. The logits go through HF's
         processors in HF's order: repetition penalty (over `out` so far), the banned tokens, then temperature, top-k
-        and top-p."""
+        and top-p. guidance: the scale of a guided call, whose logits hold the B rows and then their B negative
+        prompts (clips B .. 2B-1); HF's guidance runs first, and the negative clips are fed the same tokens."""
         S = out.shape[1]
+        B = out.shape[0]
         unfinished = torch.ones(out.shape[0], dtype=torch.bool, device=out.device)
         for step in range(n):
+            if guidance is not None:
+                logits = self._host_guidance(logits[:B], logits[B:], guidance)
             lg = self._host_processors(out, logits, do_sample and temperature > 0, temperature, top_k, top_p, penalty,
                                        bans, S)
             if do_sample and temperature > 0:
@@ -1431,6 +1596,9 @@ class VideoChatGPTLlamaForCausalLM:
                 break
             if step + 1 == n or self._pos >= self._max_seq:
                 break
-            logits, _ = eng.decode_step(nxt.to(torch.int32).contiguous(), self._pos, want_logits=True)
+            feed = nxt.to(torch.int32)
+            if guidance is not None:
+                feed = torch.cat([feed, feed])
+            logits, _ = eng.decode_step(feed.contiguous(), self._pos, want_logits=True)
             self._pos += 1
         return out
