@@ -542,6 +542,35 @@ int vcl_llm_beam_start(vcl_handle* h, const int64_t* ids, const void* video_feat
  * then rejected). */
 int vcl_llm_beam_decode(vcl_handle* h, int n_steps, void* records_out, int32_t* picks_out, void* stream);
 
+/* Contrastive search: transformers 4.x's _contrastive_search (penalty_alpha = a, top_k = k; video_chatgpt/
+ * inference.py:105-112 calls HF generate; DESIGN.md section 3, "Contrastive search"). Per prompt and step:
+ *   p        exp of the greedy log-prob rule of vcl_op_sample_logprobs on the logits of the prompt's last column
+ *   c_1..k   the k most probable tokens, best first, ties to the lower id; each decoded as a cache clip of its own
+ *   s_j      the largest cosine between candidate j's final-norm row and the prompt's context rows (the final-norm
+ *            rows of its real columns so far), fp32 in the order DESIGN.md states
+ *   score_j  (1 - a) * p_j - a * s_j in fp32; the largest wins, ties to the lower j
+ * The prefill keeps every prompt column's final-norm row (and its norm) as the context; each step appends the chosen
+ * row, copies the chosen clip's newest cache column into the prompt's other clips and takes its logits row as the next
+ * step's. Prompt b's k clips are b and B + b * (k - 1) .. B + b * (k - 1) + k - 2, with the prompt's left padding;
+ * after every step they hold the same columns, so clip b holds the chosen sequence.
+ * One RECORD per prompt and step, VCL_CS_RECORD(k) f32: the chosen token, j*, then k candidate tokens, k
+ * probabilities, k max cosines and k scores (token ids and j* as exact floats).
+ * vcl_llm_contrastive_start prefills the B prompts (n_pad as vcl_llm_prefill_padded) and runs step 0: tokens_out [B]
+ * int32, records_out [B][VCL_CS_RECORD(k)]. Rejected before any device work: a null argument, a paged handle, top_k
+ * outside 2 .. VCL_CS_MAX_K, B * top_k > max_batch, penalty_alpha outside (0, 1], a vocabulary beyond
+ * VCL_SAMPLE_WIDE_MAX_V, S + n_new > max_seq (every step decodes its candidates, the last at column S + n_new - 1),
+ * an n_pad outside 0 .. S - 1. */
+#define VCL_CS_MAX_K 64
+#define VCL_CS_RECORD(k) (2 + 4 * (k))
+int vcl_llm_contrastive_start(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
+                              const int32_t* n_pad_host, int B, int S, int top_k, float penalty_alpha, int n_new,
+                              int32_t* tokens_out, float* records_out, void* stream);
+/* The next n_steps steps of the contrastive search vcl_llm_contrastive_start began: one CUDA graph per (B * k, n_steps,
+ * k) of decode steps over the B * k clips, each followed by the rank, the fork and the next candidates. tokens_out
+ * [n_steps][B], records_out [n_steps][B][VCL_CS_RECORD(k)]. Rejected before any device work: a null argument, a paged
+ * handle, no running call, steps past the call's n_new. A new prefill ends the search. */
+int vcl_llm_contrastive_decode(vcl_handle* h, int n_steps, int32_t* tokens_out, float* records_out, void* stream);
+
 /* Paged KV cache (vcl_config.kv_blocks > 0). The cache is a pool of kv_blocks BLOCKS. A block holds 128 cache columns
  * of one sequence across all layers, [layer][K = 0 | V = 1][head][128 columns][128 dims] bf16 (2 * llm_layers *
  * llm_heads * 32 KiB: 64 MiB at 7B, 100 MiB at 13B), one contiguous range. The BLOCK TABLE, int32
@@ -668,6 +697,15 @@ int vcl_op_sample_bans(const float* logits, int64_t ld, int B, int V, const floa
  * 2 num_beams <= V <= VCL_SAMPLE_WIDE_MAX_V. */
 int vcl_op_beam_select(const float* logits, int64_t ld, int B, int num_beams, int V, const float* scores, int eos_token,
                        int last_step, void* records_out, int32_t* picks_out, void* stream);
+/* The contrastive rank on its own (vcl_llm_contrastive_start's rule): prompt b's context is rows n_pad_host[b] ..
+ * n_ctx - 1 of ctx [B][ctx_rows][D] (device bf16; their norms are computed here), its candidates rows b * top_k ..
+ * b * top_k + top_k - 1 of hid [B * top_k][D] (device bf16) with probabilities p and tokens cand_tok (device, [B *
+ * top_k]). records_out [B][VCL_CS_RECORD(top_k)] (device f32); the chosen row is written to ctx row n_ctx. Rejected:
+ * top_k outside 2 .. VCL_CS_MAX_K, penalty_alpha outside (0, 1], D not a multiple of 8 up to 8192, n_ctx outside
+ * 1 .. ctx_rows - 1, an n_pad outside 0 .. n_ctx - 1. */
+int vcl_op_contrastive_rank(void* ctx, int64_t ctx_rows, const int32_t* n_pad_host, int n_ctx, int B, int top_k, int D,
+                            const void* hid, const float* p, const int32_t* cand_tok, float penalty_alpha,
+                            float* records_out, void* stream);
 int vcl_op_layernorm(const void* x, void* y, const void* w, const void* b, int rows, int D, float eps,
                      void* stream);
 int vcl_op_rmsnorm(const void* x, void* y, const void* w, int rows, int D, float eps, void* stream);

@@ -256,6 +256,41 @@ int launch_beam_select(const BeamArgs& a, cudaStream_t stream);
 int launch_kv_fork(bf16* kcache, bf16* vcache, long long layer_elems, int L, int H, int s_max, const int2* fork, int n,
                    const int* ctl, int step, int first, cudaStream_t stream);
 
+// ---- contrastive.cu -----------------------------------------------------------------------------
+// Contrastive search (HF _contrastive_search; DESIGN.md section 3) over B prompts of k candidates (2 <= k <=
+// VCL_CS_MAX_K). Candidate j of prompt b is row b * k + j of hid, or with by_clip cache clip j == 0 ? b : B + b *
+// (k - 1) + j - 1 (its logits row and its token in tok_next too). The step's column is S + t, t = ctl[0] + step,
+// S = ctl[3]; prompt b's context is rows n_pad[b] .. S + t - 1 of ctx [B][ctx_rows][D] with fp32 norms ctx_norm
+// [B][ctx_rows].
+#ifndef VCL_CS_MAX_K
+#define VCL_CS_MAX_K 64   // include/vcl.h
+#endif
+struct CsArgs {
+  int B = 0, k = 0, D = 0, V = 0, by_clip = 0, first = 0, step = 0;
+  const float* alpha = nullptr;                      // the penalty a, on the device
+  const int* ctl = nullptr;
+  const float* logits = nullptr; long long ld = 0;   // candidates: row b (first) or the chosen clip's row
+  int* tok_next = nullptr;                           // [clips] the candidate token each clip feeds next
+  int* cand_tok = nullptr; float* cand_p = nullptr;  // [B][k] best first
+  const bf16* hid = nullptr; long long ldh = 0;      // the candidates' final-norm rows
+  bf16* ctx = nullptr; float* ctx_norm = nullptr; long long ctx_rows = 0;
+  const int* n_pad = nullptr;                        // [B] (by prompt; with by_clip also clip b's)
+  unsigned int* sim_key = nullptr;                   // [B][k] scratch, zero between steps
+  float* gnorm = nullptr;                            // [B][k] scratch
+  int* chosen = nullptr;                             // [B] j* of the last step
+  int* tok_out = nullptr;                            // [step][B] the chosen tokens (optional)
+  float* rec = nullptr;                              // [step][B][2 + 4k]: token, j*, c[k], p[k], s[k], score[k]
+};
+// p, the top k of p (best first, ties to the lower id) and the next tokens of the prompt's clips; one CTA per prompt
+int launch_cs_candidates(const CsArgs& a, cudaStream_t stream);
+// the max cosines (cs_sim), then the scores, the pick, the record and the appended context row (cs_pick)
+int launch_cs_rank(const CsArgs& a, cudaStream_t stream);
+// column S + t of each prompt's chosen clip into its other k - 1 clips, every layer, K and V ([L][clip][H][s_max][128])
+int launch_cs_fork(const CsArgs& a, bf16* kcache, bf16* vcache, long long layer_elems, int L, int H, int s_max,
+                   cudaStream_t stream);
+// ctx_norm[b][r] = the fp32 norm of ctx row r of prompt b, r < rows
+int launch_cs_norms(const bf16* ctx, float* norm, int B, int rows, long long ctx_rows, int D, cudaStream_t stream);
+
 // ---- attention.cu -------------------------------------------------------------------------------
 // softmax(Q K^T * scale [+ causal]) V for S_q == S_kv, bf16, fp32 softmax; element (b,h,s,d) of
 // each operand lives at base + b*sb + h*sh + s*ss + d.

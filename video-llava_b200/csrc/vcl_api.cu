@@ -68,6 +68,8 @@ struct GraphEntry {
                        // are read on the device too (vcl_llm_beam_decode)
   int guided;          // the guidance table has a guided clip: its graphs combine paired rows and hand the tokens on;
                        // the partners and scales are read on the device, so one graph serves every guidance setting
+  int cs;              // contrastive search with this many candidates per prompt (0: none); its step counter and
+                       // penalty are read on the device (vcl_llm_contrastive_decode)
   cudaGraphExec_t exec;
   long long kernels;   // kernel nodes in the graph (for vcl_launch_count)
   unsigned long long last_use;
@@ -88,6 +90,8 @@ struct StepIo {
   bool beam = false;              // beam search: the logits go to beam_select and kv_fork (beam_step), which write the
   int beam_step = 0;              // tokens of the next step; beam_step is this step's index in the chunk
   bool guided = false;            // classifier-free guidance of the clips of the guidance table (SampleAt::guided)
+  bool cs = false;                // contrastive search: the final-norm rows are kept, the lm_head reads them, and the
+  int cs_step = 0;                // rank / fork / candidate kernels (cs_tail) write the next tokens; cs_step as beam_step
 };
 
 // which sampling-table entries the rows of an lm_head call use, and the cache column their tokens take
@@ -219,6 +223,28 @@ struct vcl_handle {
   // whole by one host-to-device copy per call. A handle that never guides holds none and launches what it did before.
   int* guid = nullptr;
   std::vector<int> guid_host;
+  // Contrastive search (vcl_llm_contrastive_start / _decode), allocated by the first call. Prompt b's k candidates
+  // are the cache clips j == 0 ? b : B + b * (k - 1) + j - 1 (kernels.h: CsArgs::by_clip). cs_ctl {t0, 0, 0, S} and
+  // cs_alpha are written by the host before each chunk, so one captured graph per (B * k, n_steps, k) serves every
+  // call. cs_ctx [cs_cap][max_seq][D] holds each prompt's context rows (final-norm output, bf16) and cs_norm their
+  // fp32 norms; it grows with the largest B asked for (and drops the contrastive graphs, which hold its address).
+  int* cs_ctl = nullptr;
+  float* cs_alpha = nullptr;
+  int* cs_tok = nullptr;                        // [max_batch] the candidate token each clip feeds next
+  int* cs_ctok = nullptr;                       // [max_batch] candidates, prompt-major, best first
+  float* cs_p = nullptr;                        // [max_batch] their probabilities
+  unsigned int* cs_skey = nullptr;              // [max_batch] max-cosine keys (zero between steps)
+  float* cs_gnorm = nullptr;                    // [max_batch]
+  int* cs_chosen = nullptr;                     // [max_batch]
+  int2* cs_fork = nullptr;                      // [max_batch] the prompt-prefix forks after the prefill
+  bf16* cs_hid = nullptr;                       // [max_batch][D] the step's final-norm rows, by clip
+  int* cs_out = nullptr;                        // [max_seq][max_batch] chosen tokens of one chunk
+  float* cs_rec = nullptr;                      // [max_seq][5 max_batch] step records of one chunk
+  bf16* cs_ctx = nullptr;
+  float* cs_norm = nullptr;
+  int cs_cap = 0;
+  int cs_ctl_host[4] = {0, 0, 0, 0};
+  int cs_B = 0, cs_k = 0, cs_t = 0, cs_n = 0;   // the running call (cs_k 0: none); cs_t the next step
   const int* guid_partner() const { return guid; }
   const float* guid_scale() const { return reinterpret_cast<const float*>(guid + cfg.max_batch); }
   // some clip of 0 .. B-1 is guided by a partner inside 0 .. B-1
@@ -902,6 +928,7 @@ int llm_prefill(vcl_handle* h, const int64_t* ids, const void* video_feats, cons
               "logits / next token need the full stack (n_layers == %d)", c.llm_layers);
   if (start_pos == 0) {
     h->beam_k = 0;   // a new sequence ends any running beam search (vcl_llm_beam_decode refuses to continue it)
+    h->cs_k = 0;     // ... and any running contrastive search
     int npad_max = 0;
     if (n_pad_host != nullptr) {
       for (int b = 0; b < B; ++b) {
@@ -1053,6 +1080,60 @@ int beam_step(vcl_handle* h, int step, bool first, cudaStream_t st) {
                         h->cfg.max_seq, h->beam_fork, B * k, h->beam_ctl, step, first, st);
 }
 
+// The lm_head on B rows that are normalised already (x, pitch ldx) into h->logits: the 1..4-clip ring kernel reads
+// them in place, wider calls re-lay them out window-major (xwin_norm without weights) for the 5..64-clip kernel, in
+// near-equal chunks of at most 16 rows beyond 64, as lm_head_argmax does.
+int lm_head_rows(vcl_handle* h, const bf16* x, long long ldx, int B, cudaStream_t st) {
+  const vcl_config& c = h->cfg;
+  GemvArgs g;
+  h->lm_head_d.into(g); g.N = c.vocab; g.K = c.llm_hidden;
+  GemvEpilogue e;
+  e.mode = GEMV_LOGITS; e.ldl = c.vocab;
+  if (B <= 4) {
+    g.x = x; g.ldx = ldx; g.B = B;
+    e.logits = h->logits;
+    return launch_gemv(g, e, st);
+  }
+  const int n_chunks = B <= 64 ? 1 : (B + 15) / 16;
+  for (int i = 0; i < n_chunks; ++i) {
+    const int b0 = B * i / n_chunks, nb = B * (i + 1) / n_chunks - b0;
+    g.x = h->d_x; g.ldx = c.llm_hidden; g.B = nb;
+    VCL_TRY(launch_xwin_norm(x + (long long)b0 * ldx, ldx, h->d_x, nullptr, nb, c.llm_hidden, c.rms_eps, st));
+    e.logits = h->logits + (size_t)b0 * c.vocab;
+    VCL_TRY(launch_gemv(g, e, st));
+  }
+  return 0;
+}
+
+// The arguments of the running contrastive search's kernels at chunk step `step`
+CsArgs cs_args(vcl_handle* h, int step) {
+  const vcl_config& c = h->cfg;
+  CsArgs a;
+  a.B = h->cs_B; a.k = h->cs_k; a.D = c.llm_hidden; a.V = c.vocab; a.by_clip = 1; a.step = step;
+  a.alpha = h->cs_alpha; a.ctl = h->cs_ctl;
+  a.logits = h->logits; a.ld = c.vocab; a.tok_next = h->cs_tok; a.cand_tok = h->cs_ctok; a.cand_p = h->cs_p;
+  a.hid = h->cs_hid; a.ldh = c.llm_hidden;
+  a.ctx = h->cs_ctx; a.ctx_norm = h->cs_norm; a.ctx_rows = c.max_seq; a.n_pad = h->d_npad;
+  a.sim_key = h->cs_skey; a.gnorm = h->cs_gnorm; a.chosen = h->cs_chosen;
+  a.tok_out = h->cs_out; a.rec = h->cs_rec;
+  return a;
+}
+
+// The end of a contrastive step over the B * k clips, after the last layer (h->d_h): the final-norm rows into
+// cs_hid and the lm_head on them, the rank (max cosines, scores, pick, record, appended context row), the fork of
+// the new column, and the candidates of the next step from the chosen clips' logits.
+int cs_tail(vcl_handle* h, int Bk, int step, cudaStream_t st) {
+  const vcl_config& c = h->cfg;
+  const int D = c.llm_hidden;
+  VCL_TRY(launch_rmsnorm(h->d_h, D, h->cs_hid, D, h->norm_w, Bk, D, c.rms_eps, st));
+  VCL_TRY(lm_head_rows(h, h->cs_hid, D, Bk, st));
+  const CsArgs a = cs_args(h, step);
+  VCL_TRY(launch_cs_rank(a, st));
+  VCL_TRY(launch_cs_fork(a, h->kcache, h->vcache, (long long)h->cache_layer_elems(), c.llm_layers, c.llm_heads,
+                         c.max_seq, st));
+  return launch_cs_candidates(a, st);
+}
+
 // One decode step: the token of io is fed to clip b at position pos (+ io.pos_dev[b]), key floor h->d_npad[b].
 int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_t st) {
   const vcl_config& c = h->cfg;
@@ -1133,6 +1214,7 @@ int llm_decode_step(vcl_handle* h, const StepIo& io, int B, int pos, cudaStream_
       VCL_TRY(gemm(h->d_act, F, w.wd, F, h->d_h, D, nullptr, h->d_h, D, B, D, F, ACT_NONE, st));
     }
   }
+  if (io.cs) return cs_tail(h, B, io.cs_step, st);
   SampleAt smp;   // the token fed at column c_b is followed by one at column c_b + 1
   smp.on = io.sampled; smp.col = pos + 1; smp.col_dev = pd; smp.guided = io.guided;
   VCL_TRY(lm_head_argmax(h, h->d_h, D, B, io.logits_out, io.tok_out, io.out_stride, st, io.partials_out, smp));
@@ -1179,19 +1261,34 @@ int beam_steps(vcl_handle* h, int Bk, int n_new, cudaStream_t st) {
   return 0;
 }
 
+// n_new contrastive steps over the B * k clips of the running call: step i feeds h->cs_tok[b] to clip b at position
+// h->d_pos[b] + i, then cs_tail ranks, forks and writes the next candidates.
+int cs_steps(vcl_handle* h, int Bk, int n_new, cudaStream_t st) {
+  for (int i = 0; i < n_new; ++i) {
+    StepIo io;
+    io.pos_dev = h->d_pos;
+    io.tok_in = h->cs_tok;
+    io.cs = true; io.cs_step = i;
+    VCL_TRY(llm_decode_step(h, io, Bk, i, st));
+  }
+  return 0;
+}
+
 // decode_steps from one captured graph per (B, n_new, sampled, guided), sampled as h->step_sampler gives it (beam > 0: beam_steps
-// with that many beams per item, one graph per (B, n_new, beam)). The positions (h->d_pos, written by the caller),
+// with that many beams per item, one graph per (B, n_new, beam); cs > 0: cs_steps with that many candidates). The positions (h->d_pos, written by the caller),
 // the pad counts (h->d_npad) and the sampling table are read on the device, so new positions, padding or sampling
 // settings replay the same graph. Bounded LRU cache (an entry holds thousands of nodes). A stream that cannot be
 // captured runs the steps eagerly.
 int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t st, int sampled, int beam = 0,
-                     bool guided = false) {
+                     bool guided = false, int cs = 0) {
   auto steps = [&]() {
-    return beam ? beam_steps(h, B, n_new, st) : decode_steps(h, tk, B, n_new, st, sampled, guided);
+    return cs ? cs_steps(h, B, n_new, st)
+              : beam ? beam_steps(h, B, n_new, st) : decode_steps(h, tk, B, n_new, st, sampled, guided);
   };
   GraphEntry* ge = nullptr;
   for (auto& g : h->graphs)
-    if (g.B == B && g.n_new == n_new && g.sampled == sampled && g.beam == beam && g.guided == (int)guided) ge = &g;
+    if (g.B == B && g.n_new == n_new && g.sampled == sampled && g.beam == beam && g.guided == (int)guided && g.cs == cs)
+      ge = &g;
   const bool can_capture = (st != nullptr) && (st != cudaStreamLegacy);
   if (ge == nullptr && can_capture) {
     if (h->graphs.size() >= MAX_DECODE_GRAPHS) {
@@ -1223,7 +1320,7 @@ int run_decode_steps(vcl_handle* h, int32_t* tk, int B, int n_new, cudaStream_t 
       set_last_error("decode graph instantiate failed: %s", cudaGetErrorString(e));
       return -2;
     }
-    h->graphs.push_back({B, n_new, sampled, beam, (int)guided, exec, nodes, 0});
+    h->graphs.push_back({B, n_new, sampled, beam, (int)guided, cs, exec, nodes, 0});
     ge = &h->graphs.back();
   }
   if (ge == nullptr) return steps();
@@ -2026,6 +2123,129 @@ int vcl_llm_beam_decode(vcl_handle* h, int n_steps, void* records_out, int32_t* 
   return 0;
 }
 
+// Contrastive search (video_chatgpt/inference.py:105-112 calls HF generate; generate(penalty_alpha=a, top_k=k) is HF
+// 4.x's _contrastive_search): one prefill of the B prompts that keeps every column's final-norm row as the prompts'
+// context, the fork of the prompt columns into each prompt's k clips, and step 0.
+int vcl_llm_contrastive_start(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
+                              const int32_t* n_pad_host, int B, int S, int top_k, float penalty_alpha, int n_new,
+                              int32_t* tokens_out, float* records_out, void* stream) {
+  VCL_REQUIRE(h && ids && vid_start && tokens_out && records_out, "vcl_llm_contrastive_start: null argument");
+  VCL_NOT_PAGED(h, "vcl_llm_contrastive_start");
+  const vcl_config& c = h->cfg;
+  const int k = top_k;
+  VCL_REQUIRE(k >= 2 && k <= VCL_CS_MAX_K, "vcl_llm_contrastive_start: top_k=%d outside 2..%d", k, VCL_CS_MAX_K);
+  VCL_REQUIRE(B >= 1 && (long long)B * k <= c.max_batch, "vcl_llm_contrastive_start: B * top_k = %lld outside 1..%d "
+              "(max_batch: every candidate takes a cache clip)", (long long)B * k, c.max_batch);
+  VCL_REQUIRE(penalty_alpha > 0.f && penalty_alpha <= 1.f, "vcl_llm_contrastive_start: penalty_alpha %g outside (0, 1]",
+              (double)penalty_alpha);
+  VCL_REQUIRE(c.vocab <= VCL_SAMPLE_WIDE_MAX_V && c.vocab >= k, "vcl_llm_contrastive_start: contrastive search takes a "
+              "vocabulary of %d..%d tokens (the candidate selection's shared memory), this model has %d", k,
+              VCL_SAMPLE_WIDE_MAX_V, c.vocab);
+  // (every step decodes its candidates, the last one at column S + n_new - 1)
+  VCL_REQUIRE(S >= 1 && n_new >= 1 && S + n_new <= c.max_seq, "vcl_llm_contrastive_start: S + n_new = %d exceeds "
+              "max_seq %d", S + n_new, c.max_seq);
+  VCL_REQUIRE(c.llm_hidden % 8 == 0 && c.llm_hidden <= 8192, "vcl_llm_contrastive_start: llm_hidden %d above 8192",
+              c.llm_hidden);
+  if (n_pad_host != nullptr)
+    for (int b = 0; b < B; ++b)
+      VCL_REQUIRE(n_pad_host[b] >= 0 && n_pad_host[b] < S, "vcl_llm_contrastive_start: n_pad[%d] = %d outside 0..%d",
+                  b, n_pad_host[b], S - 1);
+  VCL_REQUIRE(h->llm_loaded, "LLM weights are not loaded");
+  cudaStream_t st = as_stream(stream);
+  const size_t mb = c.max_batch, D = c.llm_hidden;
+  if (h->cs_ctl == nullptr) {
+    VCL_TRY(dalloc(h, &h->cs_ctl, 4));
+    VCL_TRY(dalloc(h, &h->cs_alpha, 1));
+    VCL_TRY(dalloc(h, &h->cs_tok, mb));
+    VCL_TRY(dalloc(h, &h->cs_ctok, mb));
+    VCL_TRY(dalloc(h, &h->cs_p, mb));
+    VCL_TRY(dalloc(h, &h->cs_skey, mb));
+    VCL_TRY(dalloc(h, &h->cs_gnorm, mb));
+    VCL_TRY(dalloc(h, &h->cs_chosen, mb));
+    VCL_TRY(dalloc(h, &h->cs_fork, mb));
+    VCL_TRY(dalloc(h, &h->cs_hid, mb * D));
+    VCL_TRY(dalloc(h, &h->cs_out, (size_t)c.max_seq * mb));
+    VCL_TRY(dalloc(h, &h->cs_rec, (size_t)c.max_seq * 5 * mb));
+    VCL_CUDA_OK(cudaMemsetAsync(h->cs_skey, 0, mb * sizeof(unsigned int), st));
+  }
+  if (B > h->cs_cap) {   // a larger context buffer: the graphs that hold the old one's address go with it
+    for (void* p : {(void*)h->cs_ctx, (void*)h->cs_norm}) {
+      if (p == nullptr) continue;
+      VCL_CUDA_OK(cudaStreamSynchronize(st));
+      VCL_CUDA_OK(cudaFree(p));
+      h->allocs.erase(std::find(h->allocs.begin(), h->allocs.end(), p));
+    }
+    h->cs_ctx = nullptr; h->cs_norm = nullptr; h->cs_cap = 0;
+    for (size_t i = h->graphs.size(); i-- > 0;)
+      if (h->graphs[i].cs) {
+        cudaGraphExecDestroy(h->graphs[i].exec);
+        h->graphs.erase(h->graphs.begin() + i);
+      }
+    VCL_TRY(dalloc(h, &h->cs_ctx, (size_t)B * c.max_seq * D));
+    VCL_TRY(dalloc(h, &h->cs_norm, (size_t)B * c.max_seq));
+    h->cs_cap = B;
+  }
+  h->cs_k = 0;   // (no running call until this one has started)
+  VCL_TRY(llm_prefill(h, ids, video_feats, vid_start, B, S, c.llm_layers, nullptr, nullptr, nullptr, 1, st, 0,
+                      nullptr, n_pad_host));
+  // the context: every prompt column's final-norm row (the padding's too; the rank skips those rows), its norm, and
+  // the logits of each prompt's last column from that row
+  for (int b = 0; b < B; ++b)
+    VCL_TRY(launch_rmsnorm(h->l_h + (size_t)b * S * D, D, h->cs_ctx + (size_t)b * c.max_seq * D, D, h->norm_w, S,
+                           (int)D, c.rms_eps, st));
+  VCL_TRY(launch_cs_norms(h->cs_ctx, h->cs_norm, B, S, c.max_seq, (int)D, st));
+  VCL_TRY(lm_head_rows(h, h->cs_ctx + (size_t)(S - 1) * D, (long long)c.max_seq * D, B, st));
+  // prompt b's clips, each with the prompt's padding, and the forks of its columns 0 .. S - 1 (kv_fork_kernel at
+  // t = 0, first)
+  const int Bk = B * k;
+  std::vector<int> npad(Bk);
+  std::vector<int2> fork;
+  for (int b = 0; b < B; ++b)
+    for (int j = 0; j < k; ++j) {
+      const int clip = j == 0 ? b : B + b * (k - 1) + j - 1;
+      npad[clip] = n_pad_host != nullptr ? n_pad_host[b] : 0;
+      if (j > 0) fork.push_back(make_int2(b, clip));
+    }
+  if (h->padded)
+    VCL_CUDA_OK(cudaMemcpyAsync(h->d_npad, npad.data(), Bk * sizeof(int), cudaMemcpyHostToDevice, st));
+  VCL_CUDA_OK(cudaMemcpyAsync(h->cs_fork, fork.data(), fork.size() * sizeof(int2), cudaMemcpyHostToDevice, st));
+  h->cs_ctl_host[0] = 0; h->cs_ctl_host[3] = S;
+  VCL_CUDA_OK(cudaMemcpyAsync(h->cs_ctl, h->cs_ctl_host, sizeof(h->cs_ctl_host), cudaMemcpyHostToDevice, st));
+  VCL_CUDA_OK(cudaMemcpyAsync(h->cs_alpha, &penalty_alpha, sizeof(float), cudaMemcpyHostToDevice, st));
+  h->cs_B = B; h->cs_k = k; h->cs_t = 1; h->cs_n = n_new;
+  CsArgs a = cs_args(h, 0);
+  a.first = 1;
+  VCL_TRY(launch_cs_candidates(a, st));
+  VCL_TRY(launch_kv_fork(h->kcache, h->vcache, (long long)h->cache_layer_elems(), c.llm_layers, c.llm_heads,
+                         c.max_seq, h->cs_fork, (int)fork.size(), h->cs_ctl, 0, 1, st));
+  VCL_TRY(launch_fill_int(h->d_pos, S, Bk, st));
+  VCL_TRY(cs_steps(h, Bk, 1, st));
+  VCL_CUDA_OK(cudaMemcpyAsync(tokens_out, h->cs_out, (size_t)B * sizeof(int32_t), cudaMemcpyDefault, st));
+  VCL_CUDA_OK(cudaMemcpyAsync(records_out, h->cs_rec, (size_t)B * (2 + 4 * k) * sizeof(float), cudaMemcpyDefault, st));
+  return 0;
+}
+
+// The next n_steps steps of the running contrastive search, from one captured graph per (B * k, n_steps, k).
+int vcl_llm_contrastive_decode(vcl_handle* h, int n_steps, int32_t* tokens_out, float* records_out, void* stream) {
+  VCL_REQUIRE(h && tokens_out && records_out, "vcl_llm_contrastive_decode: null argument");
+  VCL_NOT_PAGED(h, "vcl_llm_contrastive_decode");
+  VCL_REQUIRE(h->cs_k > 0, "vcl_llm_contrastive_decode: no contrastive search is running (vcl_llm_contrastive_start)");
+  VCL_REQUIRE(n_steps >= 1 && h->cs_t + n_steps <= h->cs_n, "vcl_llm_contrastive_decode: steps %d..%d outside the "
+              "call's %d steps", h->cs_t, h->cs_t + n_steps - 1, h->cs_n);
+  cudaStream_t st = as_stream(stream);
+  const int B = h->cs_B, k = h->cs_k, t0 = h->cs_t;
+  h->cs_ctl_host[0] = t0;
+  VCL_CUDA_OK(cudaMemcpyAsync(h->cs_ctl, h->cs_ctl_host, sizeof(int), cudaMemcpyHostToDevice, st));
+  // step t decodes the candidates of token t at column S + t
+  VCL_TRY(launch_fill_int(h->d_pos, h->cs_ctl_host[3] + t0, B * k, st));
+  VCL_TRY(run_decode_steps(h, nullptr, B * k, n_steps, st, 0, 0, false, k));
+  h->cs_t += n_steps;
+  VCL_CUDA_OK(cudaMemcpyAsync(tokens_out, h->cs_out, (size_t)n_steps * B * sizeof(int32_t), cudaMemcpyDefault, st));
+  VCL_CUDA_OK(cudaMemcpyAsync(records_out, h->cs_rec, (size_t)n_steps * B * (2 + 4 * k) * sizeof(float),
+                              cudaMemcpyDefault, st));
+  return 0;
+}
+
 int vcl_llm_score(vcl_handle* h, const int64_t* ids, const void* video_feats, const int32_t* vid_start,
                   const int32_t* n_pad_host, int B, int S, const int64_t* labels, void* logits_out, float* nll_out,
                   float* loss_out, void* stream) {
@@ -2254,6 +2474,54 @@ int vcl_op_beam_select(const float* logits, int64_t ld, int B, int num_beams, in
     rc = -2;
   }
   if (rc == 0) rc = launch_beam_select(a, st);
+  cudaFreeAsync(scratch, st);
+  return rc;
+}
+
+// The contrastive rank alone (HF _ranking_fast and the pick of _contrastive_search, inference.py:105-112): prompt b's
+// context is rows n_pad[b] .. n_ctx - 1 of ctx [B][ctx_rows][D] (device), its candidates rows b * k .. b * k + k - 1
+// of hid [B * k][D] with probabilities p and tokens cand_tok (device); the chosen row lands in ctx row n_ctx.
+int vcl_op_contrastive_rank(void* ctx, int64_t ctx_rows, const int32_t* n_pad_host, int n_ctx, int B, int top_k, int D,
+                            const void* hid, const float* p, const int32_t* cand_tok, float penalty_alpha,
+                            float* records_out, void* stream) {
+  VCL_REQUIRE(ctx && n_pad_host && hid && p && cand_tok && records_out, "vcl_op_contrastive_rank: null argument");
+  if (check_device() != 0) return -2;
+  const int k = top_k;
+  VCL_REQUIRE(k >= 2 && k <= VCL_CS_MAX_K, "vcl_op_contrastive_rank: top_k=%d outside 2..%d", k, VCL_CS_MAX_K);
+  VCL_REQUIRE(B >= 1, "vcl_op_contrastive_rank: B=%d", B);
+  VCL_REQUIRE(penalty_alpha > 0.f && penalty_alpha <= 1.f, "vcl_op_contrastive_rank: penalty_alpha %g outside (0, 1]",
+              (double)penalty_alpha);
+  VCL_REQUIRE(D >= 8 && D % 8 == 0 && D <= 8192, "vcl_op_contrastive_rank: D=%d must be a multiple of 8 up to 8192", D);
+  VCL_REQUIRE(n_ctx >= 1 && n_ctx < ctx_rows, "vcl_op_contrastive_rank: n_ctx %d outside 1..%lld (a row is appended)",
+              n_ctx, (long long)ctx_rows - 1);
+  for (int b = 0; b < B; ++b)
+    VCL_REQUIRE(n_pad_host[b] >= 0 && n_pad_host[b] < n_ctx, "vcl_op_contrastive_rank: n_pad[%d] = %d outside 0..%d",
+                b, n_pad_host[b], n_ctx - 1);
+  cudaStream_t st = as_stream(stream);
+  // scratch: ctl [4], alpha, n_pad [B], sim_key / gnorm / chosen [B * k], norms [B][ctx_rows]
+  const size_t Bk = (size_t)B * k, words = 5 + B + 3 * Bk;
+  std::vector<int> host(words, 0);
+  host[3] = n_ctx;
+  memcpy(&host[4], &penalty_alpha, 4);
+  memcpy(&host[5], n_pad_host, (size_t)B * 4);
+  unsigned char* scratch = nullptr;
+  VCL_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&scratch), words * 4 + (size_t)B * ctx_rows * 4, st));
+  int* w = reinterpret_cast<int*>(scratch);
+  CsArgs a;
+  a.B = B; a.k = k; a.D = D; a.by_clip = 0; a.step = 0;
+  a.ctl = w; a.alpha = reinterpret_cast<const float*>(w + 4); a.n_pad = w + 5;
+  a.sim_key = reinterpret_cast<unsigned int*>(w + 5 + B); a.gnorm = reinterpret_cast<float*>(w + 5 + B + Bk);
+  a.chosen = w + 5 + B + 2 * Bk;
+  a.ctx = reinterpret_cast<bf16*>(ctx); a.ctx_rows = ctx_rows; a.ctx_norm = reinterpret_cast<float*>(w + words);
+  a.hid = reinterpret_cast<const bf16*>(hid); a.ldh = D;
+  a.cand_p = const_cast<float*>(p); a.cand_tok = const_cast<int*>(cand_tok); a.rec = records_out;
+  int rc = 0;
+  if (cudaMemcpyAsync(scratch, host.data(), words * 4, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+    set_last_error("vcl_op_contrastive_rank: control copy failed");
+    rc = -2;
+  }
+  if (rc == 0) rc = launch_cs_norms(a.ctx, a.ctx_norm, B, n_ctx, ctx_rows, D, st);
+  if (rc == 0) rc = launch_cs_rank(a, st);
   cudaFreeAsync(scratch, st);
   return rc;
 }

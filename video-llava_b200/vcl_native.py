@@ -155,6 +155,9 @@ _SIGNATURES = {
     "vcl_llm_beam_start": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_int, c_int, c_int, c_int,
                                    c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_llm_beam_decode": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "vcl_llm_contrastive_start": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), c_int, c_int,
+                                          c_int, c_float, c_int, c_void_p, c_void_p, c_void_p]),
+    "vcl_llm_contrastive_decode": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_launch_count": (ctypes.c_longlong, []),
     "vcl_kv_cache_copy": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "vcl_llm_set_block_table": (c_int, [c_void_p, POINTER(c_int32), c_void_p]),
@@ -193,6 +196,8 @@ _SIGNATURES = {
                                 c_void_p]),
     "vcl_op_beam_select": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                    c_void_p]),
+    "vcl_op_contrastive_rank": (c_int, [c_void_p, c_int64, POINTER(c_int32), c_int, c_int, c_int, c_int, c_void_p,
+                                        c_void_p, c_void_p, c_float, c_void_p, c_void_p]),
     "vcl_op_layernorm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "vcl_op_rmsnorm": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "vcl_op_im2col": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
@@ -558,6 +563,38 @@ def op_beam_select(logits, scores, num_beams, eos=-1, last_step=False):
     check(lib().vcl_op_beam_select(c_void_p(logits.data_ptr()), logits.stride(0), B, k, ld, ptr(sc), int(eos),
                                    int(bool(last_step)), ptr(rec), ptr(picks), cur_stream()))
     return rec, picks
+
+
+CS_MAX_K = 64                 # include/vcl.h: VCL_CS_MAX_K, the most contrastive-search candidates per prompt
+
+
+def cs_record_len(k):
+    """f32 words per contrastive-search step record (include/vcl.h: VCL_CS_RECORD)"""
+    return 2 + 4 * int(k)
+
+
+def cs_records(rec, k):
+    """records f32 [..., 2 + 4k] -> dict of token / pick int64 [...] and cand int64, p, cos, score f32 [..., k]"""
+    k = int(k)
+    return {"token": rec[..., 0].to(torch.int64), "pick": rec[..., 1].to(torch.int64),
+            "cand": rec[..., 2:2 + k].to(torch.int64), "p": rec[..., 2 + k:2 + 2 * k],
+            "cos": rec[..., 2 + 2 * k:2 + 3 * k], "score": rec[..., 2 + 3 * k:2 + 4 * k]}
+
+
+def op_contrastive_rank(ctx, n_pad, n_ctx, hid, p, cand_tok, penalty_alpha):
+    """The contrastive rank alone (vcl_op_contrastive_rank): ctx [B, rows, D] bf16 on the device (row n_ctx receives
+    each prompt's chosen row), n_pad [B] host ints, hid [B * k, D] bf16, p [B * k] f32, cand_tok [B * k] int32.
+    Returns records f32 [B, 2 + 4k] on the device (cs_records unpacks them)."""
+    B, rows, D = ctx.shape
+    Bk = hid.shape[0]
+    assert ctx.dtype == hid.dtype == torch.bfloat16 and ctx.is_contiguous() and hid.is_contiguous() and Bk % B == 0
+    k = Bk // B
+    pd = p.to(device=ctx.device, dtype=torch.float32).contiguous()
+    td = cand_tok.to(device=ctx.device, dtype=torch.int32).contiguous()
+    rec = torch.empty(B, cs_record_len(k), dtype=torch.float32, device=ctx.device)
+    check(lib().vcl_op_contrastive_rank(c_void_p(ctx.data_ptr()), rows, _host_pads(n_pad, B), int(n_ctx), B, k, D,
+                                        ptr(hid), ptr(pd), ptr(td), float(penalty_alpha), ptr(rec), cur_stream()))
+    return rec
 
 
 def op_gemv(x, w, res=None, norm_w=None, eps=0.0):
@@ -1079,6 +1116,35 @@ class Engine:
         picks = torch.empty(int(n_steps), B, k, dtype=torch.int32, device="cuda")
         check(lib().vcl_llm_beam_decode(self._h, int(n_steps), ptr(rec), ptr(picks), cur_stream()))
         return rec, picks
+
+    # ---- contrastive search ----
+    def contrastive_start(self, ids, video_feats, vid_start, top_k, penalty_alpha, n_new, n_pad=None):
+        """Prefill the B prompts once and run contrastive step 0 (vcl_llm_contrastive_start): top_k candidates per
+        prompt, n_new steps in all, n_pad as in prefill. Returns (tokens int32 [1, B], records f32 [1, B, 2 + 4k]) on
+        the device (cs_records unpacks them)."""
+        B, S = ids.shape
+        k = int(top_k)
+        tok = torch.empty(1, B, dtype=torch.int32, device=ids.device)
+        rec = torch.empty(1, B, cs_record_len(k), dtype=torch.float32, device=ids.device)
+        vf = None
+        if video_feats is not None:
+            vf = video_feats.to(torch.bfloat16).contiguous()
+            assert vf.shape == (B, self.NV, self.cfg.clip_hidden), vf.shape
+        pads = None if n_pad is None else _host_pads(n_pad, B)
+        check(lib().vcl_llm_contrastive_start(self._h, ptr(ids.contiguous()), ptr(vf), ptr(vid_start.contiguous()), pads,
+                                              B, S, k, float(penalty_alpha), int(n_new), ptr(tok), ptr(rec),
+                                              cur_stream()))
+        self._cs_shape = (B, k)
+        return tok, rec
+
+    def contrastive_decode(self, n_steps):
+        """The next n_steps steps of the running contrastive search (vcl_llm_contrastive_decode): (tokens int32
+        [n, B], records f32 [n, B, 2 + 4k]) on the device."""
+        B, k = self._cs_shape
+        tok = torch.empty(int(n_steps), B, dtype=torch.int32, device="cuda")
+        rec = torch.empty(int(n_steps), B, cs_record_len(k), dtype=torch.float32, device="cuda")
+        check(lib().vcl_llm_contrastive_decode(self._h, int(n_steps), ptr(tok), ptr(rec), cur_stream()))
+        return tok, rec
 
     # ---- KV cache read-back (tests) ----
     def _cache_shape(self):

@@ -87,7 +87,7 @@ def video_chatgpt_infer(video_frames, question, conv_mode, model, vision_tower, 
                         video_token_len, transcript=None, do_sample=True, temperature=0.2, max_new_tokens=1024,
                         video_key=None, feature_cache: "VideoFeatureCache | None" = None, seed=None, top_p=1.0,
                         repetition_penalty=1.0, no_repeat_ngram_size=None, bad_words_ids=None, min_new_tokens=None,
-                        guidance_scale=None):
+                        guidance_scale=None, penalty_alpha=None, top_k=None):
     """Same flow as the reference: prompt -> tokenizer -> image processor -> tower -> pool -> generate
     -> decode. `do_sample/temperature/max_new_tokens` default to the reference's hard-coded values.
     Extension (off by default): with `video_key` and a `VideoFeatureCache`, the pooled features of a
@@ -102,7 +102,10 @@ def video_chatgpt_infer(video_frames, question, conv_mode, model, vision_tower, 
     the image processor (video_chatgpt.preprocess).
     guidance_scale (off by default, None): classifier-free guidance against the same conversation built without the
     video span (the transcript is kept), passed to generate as negative_prompt_ids, so every answer token is pushed
-    toward what the video, not the text alone, makes likely (visual contrastive decoding)."""
+    toward what the video, not the text alone, makes likely (visual contrastive decoding).
+    penalty_alpha (off by default, None) with top_k (HF's 50 when None): contrastive search, passed to generate; it
+    decodes without sampling (do_sample is then False, as HF's contrastive search is), for long answers that greedy
+    and sampled decoding tend to repeat."""
     use_se = model.get_model().vision_config.use_vid_start_end
     prompt, conv = build_prompt(question, conv_mode, video_token_len, use_se, transcript)
     inputs = tokenizer([prompt])
@@ -132,6 +135,10 @@ def video_chatgpt_infer(video_frames, question, conv_mode, model, vision_tower, 
     # HF generate stops at the tokenizer's EOS implicitly (generation config); the stop string alone
     # cannot: "</s>" tokenizes to [bos, eos] and is dropped by skip_special_tokens
     eos = getattr(tokenizer, "eos_token_id", None)
+    contrastive = {}
+    if penalty_alpha is not None:
+        contrastive = {"penalty_alpha": penalty_alpha, "top_k": 50 if top_k is None else top_k}
+        do_sample = False
     with torch.inference_mode():
         output_ids = model.generate(input_ids, video_spatio_temporal_features=feats.unsqueeze(0),
                                     do_sample=do_sample, temperature=temperature, max_new_tokens=max_new_tokens,
@@ -139,7 +146,7 @@ def video_chatgpt_infer(video_frames, question, conv_mode, model, vision_tower, 
                                     pad_token_id=getattr(tokenizer, "pad_token_id", None), seed=seed, top_p=top_p,
                                     repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size,
                                     bad_words_ids=bad_words_ids, min_new_tokens=min_new_tokens,
-                                    guidance_scale=guidance_scale, negative_prompt_ids=neg_ids)
+                                    guidance_scale=guidance_scale, negative_prompt_ids=neg_ids, **contrastive)
     n_diff = (input_ids != output_ids[:, :input_ids.shape[1]]).sum().item()
     if n_diff > 0:
         print(f"[Warning] {n_diff} output_ids are not the same as the input_ids")

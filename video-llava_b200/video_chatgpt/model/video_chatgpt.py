@@ -411,6 +411,7 @@ class VideoChatGPTLlamaForCausalLM:
         self.last_logprobs = None      # generate / generate_continue / generate_requests(logprobs=...): per row or request
         self.last_beam_scores = None   # generate(num_beams > 1): HF's sequences_scores, f32 [B * num_return_sequences]
         self._after_beams = False      # the last generate ran beam search: there is no single turn to continue
+        self._after_contrastive = False   # ... or contrastive search (generate_continue refuses both)
         self._pads = None              # the left padding of the last generate (log-prob positions of generate_continue)
         self._sessions: dict = {}      # kept conversations of generate_requests (paged): key -> inflight.PagedSlots' state
         self._session_clock = 0        # last-use stamps of the kept conversations (the least recent is swapped first)
@@ -974,7 +975,8 @@ class VideoChatGPTLlamaForCausalLM:
                  attention_mask=None, seed=None, logprobs=None, top_p=1.0, repetition_penalty=1.0, num_beams=1,
                  num_return_sequences=1, length_penalty=1.0, early_stopping=False, no_repeat_ngram_size=None,
                  bad_words_ids=None, min_new_tokens=None, guidance_scale=None, negative_prompt_ids=None,
-                 negative_prompt_attention_mask=None, negative_video_spatio_temporal_features=None, **kw):
+                 negative_prompt_attention_mask=None, negative_video_spatio_temporal_features=None, penalty_alpha=None,
+                 **kw):
         """Returns [B, S+n] int64 INCLUDING the prompt, like HF generate (inference.py:105-120), and
         like HF it stops at EOS (config.eos_token_id unless eos_token_id is given; None disables it):
         finished rows are padded, the call returns when every row has finished.
@@ -1023,8 +1025,21 @@ class VideoChatGPTLlamaForCausalLM:
         row runs as if alone (its positions start at its first real token). negative_video_spatio_temporal_features
         [B, ., .]: the pooled features of a video span in the negative prompts (e.g. a noised copy); without them a
         span is embedded as text, as generate does without features. Greedy and seeded calls guide on the device,
-        unseeded sampling on the host step by step. Not with beams (NotImplementedError)."""
+        unseeded sampling on the host step by step. Not with beams (NotImplementedError).
+        penalty_alpha (None or 0: off) with top_k > 1: HF's contrastive search (DESIGN.md section 3, "Contrastive
+        search"); see _contrastive_generate. Each step decodes the top_k most probable tokens of every prompt as cache
+        clips of their own (B * top_k <= max_batch, a ValueError otherwise) and keeps the one that best trades its
+        probability against its largest cosine similarity to the prompt's hidden states so far. It runs with
+        attention_mask, EOS / pad_token_id, stopping criteria and video features; sampling, seed, beams, guidance,
+        logprobs, top_p, repetition_penalty and the banned-token settings raise NotImplementedError. top_k <= 1
+        decodes greedily, as in HF. generate_continue cannot continue it (ValueError)."""
         self._not_paged("generate")
+        cs = self._contrastive_args(penalty_alpha, top_k, do_sample, seed, num_beams, guidance_scale, logprobs, top_p,
+                                    repetition_penalty, (no_repeat_ngram_size, bad_words_ids, min_new_tokens))
+        if cs is not None:
+            return self._contrastive_generate(input_ids, video_spatio_temporal_features, attention_mask, max_new_tokens,
+                                              stopping_criteria, eos_token_id, pad_token_id, *cs)
+        self._after_contrastive = False
         guide = self._guidance_args(guidance_scale, negative_prompt_ids, negative_prompt_attention_mask,
                                     negative_video_spatio_temporal_features, input_ids, num_beams)
         beams = self._beam_args(num_beams, num_return_sequences, length_penalty, early_stopping, do_sample, seed,
@@ -1241,7 +1256,74 @@ class VideoChatGPTLlamaForCausalLM:
         self.last_beam_scores = scores
         return torch.cat([ids.repeat_interleave(m, dim=0), seqs.to(dev)], dim=1)
 
-    def _host_stops(self, eng, out, new, n, stopping_criteria, eos, pad, guided=False):
+    def _contrastive_args(self, penalty_alpha, top_k, do_sample, seed, num_beams, guidance_scale, logprobs, top_p,
+                          repetition_penalty, bans):
+        """Checks the contrastive-search arguments of generate on the host -> None (off), or (penalty_alpha,
+        top_k). Off as in HF: penalty_alpha None or 0, or top_k <= 1."""
+        if penalty_alpha is None:
+            return None
+        if isinstance(penalty_alpha, bool) or not isinstance(penalty_alpha, (int, float)) or \
+                not 0.0 <= float(penalty_alpha) <= 1.0:
+            raise ValueError(f"generate: penalty_alpha {penalty_alpha!r} must be a number in [0, 1]")
+        if isinstance(top_k, bool) or not isinstance(top_k, int):
+            raise ValueError(f"generate: top_k {top_k!r} must be an int")
+        if float(penalty_alpha) == 0.0 or top_k <= 1:
+            return None
+        for name, bad in (("do_sample=True", do_sample), ("seed", seed is not None),
+                          ("num_beams > 1", not (isinstance(num_beams, int) and num_beams == 1)),
+                          ("guidance_scale", guidance_scale is not None and float(guidance_scale) != 1.0),
+                          ("logprobs", logprobs is not None), ("top_p", float(top_p) < 1.0),
+                          ("repetition_penalty", float(repetition_penalty) != 1.0),
+                          ("no_repeat_ngram_size", bool(bans[0])), ("bad_words_ids", bans[1] is not None),
+                          ("min_new_tokens", bool(bans[2]))):
+            if bad:
+                raise NotImplementedError(f"generate: {name} is not supported with penalty_alpha (contrastive search "
+                                          "ranks greedy candidates, do_sample=False, without other logits processors)")
+        if top_k > vn.CS_MAX_K:
+            raise ValueError(f"generate: top_k {top_k} exceeds {vn.CS_MAX_K}, the most contrastive-search candidates "
+                             "the device ranks per prompt")
+        if self.config.vocab_size > vn.SAMPLE_WIDE_MAX_V:
+            raise ValueError(f"generate: contrastive search takes a vocabulary of at most {vn.SAMPLE_WIDE_MAX_V} tokens "
+                             f"on the device, this model has {self.config.vocab_size}")
+        return float(penalty_alpha), top_k
+
+    def _contrastive_generate(self, input_ids, feats, attention_mask, max_new_tokens, stopping_criteria, eos_token_id,
+                              pad_token_id, alpha, k):
+        """generate(penalty_alpha=alpha, top_k=k): HF 4.x's _contrastive_search. The device prefills each prompt once,
+        keeping its final-norm rows as the context, then every step decodes the k candidates of each prompt in k
+        cache clips, ranks them, appends the winner's row to the context and copies its cache column into the other
+        clips (vcl_llm_contrastive_start / _decode; one CUDA graph per chunk). EOS, padding and stopping criteria
+        are applied on the host between chunks of _GREEDY_CHUNK tokens, token by token, as for seeded sampling.
+        Returns [B, S + m] like greedy generate."""
+        pads = left_padding(attention_mask, input_ids.shape)
+        B, S = input_ids.shape
+        if B * k > self._max_batch:
+            raise ValueError(f"generate: {B} prompts x top_k {k} = {B * k} candidates exceed max_batch "
+                             f"{self._max_batch} (contrastive search decodes every candidate in a cache clip of its "
+                             "own: pass a smaller top_k or build the model with a larger max_batch)")
+        n = min(int(max_new_tokens), self._max_seq - S)   # (every step decodes its candidates at column S + t)
+        if n <= 0:
+            raise ValueError(f"prompt length {S} leaves no room in max_seq {self._max_seq}")
+        self.last_logprobs = self.last_beam_scores = None
+        self._after_beams = False
+        eng = self._ensure_engine(need_llm=True)
+        dev = self.device
+        ids = input_ids.to(dev).to(torch.int64)
+        vs = self._spans_dev(ids, feats, eng.NV, pads, device=dev)
+        if feats is not None:
+            feats = feats.to(dev)
+        eos, pad = self._eos_pad(eos_token_id, pad_token_id)
+        self._last_out, self._after_contrastive = None, True
+        tok, _ = eng.contrastive_start(ids, feats, vs, k, alpha, n, n_pad=pads)
+        c = n if eos is None and not stopping_criteria else min(n, self._GREEDY_CHUNK)
+        if c > 1:
+            tok = torch.cat([tok, eng.contrastive_decode(c - 1)[0]])
+        if eos is None and not stopping_criteria:
+            return torch.cat([ids, tok.T.to(torch.int64)], dim=1)
+        return self._host_stops(eng, ids, tok.T, n, stopping_criteria, eos, pad,
+                                more=lambda m: eng.contrastive_decode(m)[0].T)
+
+    def _host_stops(self, eng, out, new, n, stopping_criteria, eos, pad, guided=False, more=None):
         """The device-sampled loop of generate / generate_continue: `new` [B, c] int32 holds the first c tokens
         after the context `out` [B, L] (the first at column L). _stepwise's EOS / padding / stopping-criteria
         logic runs token by token over each chunk on the host; the device decodes the next _GREEDY_CHUNK tokens
@@ -1249,7 +1331,9 @@ class VideoChatGPTLlamaForCausalLM:
         ends at L + k - 1, where _stepwise leaves it (columns decoded past the stop are overwritten by a
         continuation). The sequence lives in one [B, L + n] buffer on out's device, filled by one copy per chunk;
         a stopping criterion is called with a view of its first L + j columns, so a call costs no copy.
-        guided: clips B .. 2B-1 decode the negative prompts next to the B rows and are fed the same tokens."""
+        guided: clips B .. 2B-1 decode the negative prompts next to the B rows and are fed the same tokens.
+        more(m): the next m tokens [B, m] of a device loop that keeps its own state (contrastive search), instead of
+        decode_loop from the last kept token."""
         dev, (B, L) = out.device, out.shape
         full = torch.empty(B, L + n, dtype=torch.int64, device=dev)
         full[:, :L] = out
@@ -1279,6 +1363,9 @@ class VideoChatGPTLlamaForCausalLM:
             if done:
                 break
             m = min(self._GREEDY_CHUNK, n - k)
+            if more is not None:
+                new = more(m)
+                continue
             last = full[:, L + k - 1].to(torch.int32).contiguous()
             if guided:
                 last = torch.cat([last, last])
@@ -1449,7 +1536,7 @@ class VideoChatGPTLlamaForCausalLM:
         q = candidate_scoring.check(self, input_ids, candidates, video_spatio_temporal_features, attention_mask,
                                     eng.NV)
         self._last_out, self._pos, self.last_logprobs = None, 0, None
-        self._after_beams, self.last_beam_scores = False, None
+        self._after_beams, self._after_contrastive, self.last_beam_scores = False, False, None
         return candidate_scoring.score(self, eng, q)
 
     def end_session(self, key=None):
@@ -1482,6 +1569,9 @@ class VideoChatGPTLlamaForCausalLM:
         if getattr(self, "_after_beams", False):
             raise ValueError("generate_continue: the last generate() ran beam search (num_beams > 1), which returns "
                              "several hypotheses per prompt and leaves no single turn to continue")
+        if getattr(self, "_after_contrastive", False):
+            raise ValueError("generate_continue: the last generate() ran contrastive search (penalty_alpha), which "
+                             "generate_continue does not continue; start the next turn with generate()")
         if getattr(self, "_last_out", None) is None:
             raise ValueError("generate_continue: no previous generate() to continue")
         lp_n = self._logprobs_arg(logprobs, "generate_continue")
