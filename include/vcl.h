@@ -408,6 +408,18 @@ int vcl_llm_set_sampling_ex(vcl_handle* h, int n, const int32_t* clips_host, con
  * VCL_SAMPLE_WIDE_MAX_V. */
 int vcl_llm_set_token_set(vcl_handle* h, int entry, const int64_t* ids, int n, void* stream);
 
+/* HF's MinPLogitsWarper, TypicalLogitsWarper, EpsilonLogitsWarper and EtaLogitsWarper, in that order after top-p, on
+ * sampled entries (a greedy entry ignores them, as HF does). Per entry i of clips_host: min_p_host[i] (0 .. 1; 0 off),
+ * typical_p_host[i] (> 0 and <= 1; 1 off), epsilon_host[i] and eta_host[i] (>= 0 and < 1; 0 off). Each warper removes
+ * tokens from the set the stages before it kept; the draw and the log-probs use the final set (the exact rules are in
+ * DESIGN.md section 3, "Min-p, typical, epsilon and eta"). vcl_llm_set_sampling and vcl_llm_set_sampling_ex turn all
+ * four off for the entries they write, so call this after them. A sampled entry with a warper on takes the 32-bit
+ * sampler (vcl_llm_set_sampling_ex); the settings live in the sampling table, so its decode graphs serve every
+ * setting. Rejected before any device work: what vcl_llm_set_sampling rejects of the clips, a value outside its range
+ * or NaN (HF's messages), and a warper on a vocabulary over VCL_SAMPLE_WIDE_MAX_V. */
+int vcl_llm_set_warpers(vcl_handle* h, int n, const int32_t* clips_host, const float* min_p_host,
+                        const float* typical_p_host, const float* epsilon_host, const float* eta_host, void* stream);
+
 /* Copy entry `entry`'s token set, ceil(vocab / 32) uint32 words (bit i & 31 of word i >> 5: token i), to bits_out
  * (host or device memory), ordered on `stream`. Rejected: a null argument, an entry outside 0 .. max_batch-1, a
  * handle that never allocated its token sets. */
@@ -680,6 +692,15 @@ int vcl_op_sample_ex(const float* logits, int64_t ld, int B, int V, const float*
                      const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
                      const float* top_p_host, const float* repetition_penalty_host, uint32_t* token_sets,
                      const int32_t* top_n_host, int32_t* tok_out, int32_t* ids_out, float* lp_out, void* stream);
+/* The 32-bit sampler with the warpers on its own (vcl_llm_set_warpers): vcl_op_sample_ex where row b also has
+ * min_p_host[b], typical_p_host[b], epsilon_host[b] and eta_host[b] (HOST memory, [B], vcl_llm_set_warpers' ranges).
+ * A row with all four off gives vcl_op_sample_ex's token and log-probs bit for bit. */
+int vcl_op_sample_warpers(const float* logits, int64_t ld, int B, int V, const float* temperature_host,
+                          const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
+                          const float* top_p_host, const float* repetition_penalty_host, uint32_t* token_sets,
+                          const float* min_p_host, const float* typical_p_host, const float* epsilon_host,
+                          const float* eta_host, const int32_t* top_n_host, int32_t* tok_out, int32_t* ids_out,
+                          float* lp_out, void* stream);
 /* The 32-bit sampler with the ban stage on its own (vcl_llm_set_bans): vcl_op_sample_ex where row b also has a token
  * history histories[b * hist_ld ..] (device int32), and the ban settings ngram_host[b], eos_host[b],
  * eos_from_col_host[b] and words_host[b * VCL_BAN_WORDS_MAX ..] (HOST memory, vcl_llm_set_bans' format). Row b draws

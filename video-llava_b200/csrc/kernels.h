@@ -203,6 +203,11 @@ struct SampleArgs {
   // token it picks at hist[t * hist_ld + c].
   int* hist = nullptr; long long hist_ld = 0;
   const int* bans = nullptr;
+  // HF's min-p, typical, epsilon and eta warpers (32-bit path, min_p set; all four set together): entry t's
+  // min_p[t] (0: off), typical_p[t] (1: off), epsilon[t] and eta[t] (0: off), applied after top-p on sampled rows
+  // by the rules at warp_row in sampling.cu
+  const float* min_p = nullptr; const float* typical_p = nullptr; const float* epsilon = nullptr;
+  const float* eta = nullptr;
 };
 #ifndef VCL_BAN_WORDS_MAX
 #define VCL_BAN_WORDS_MAX 1024   // include/vcl.h

@@ -11,7 +11,7 @@
 //   kept   z_i >= z of the k-th largest logit (ties at the threshold are kept, HF's `scores < kth` rule);
 //          top_k = 0 or top_k >= V keeps every token; a NaN logit is never kept
 //   top-p  (p < 1, sampled rows) of the kept tokens, those whose key is the largest, or whose mass strictly above
-//          it M is below p * W, in the fixed-point rule at top_p_threshold
+//          it M is below p * W, in the fixed-point rule at mass_threshold
 //   w_i    exp(z_i - z_max) over the kept tokens, in fp32
 //   token  the smallest j whose inclusive prefix sum of w exceeds u * W (W = sum of w); if rounding leaves u * W
 //          past the last prefix sum, the last token with a nonzero weight (a -inf logit or an exp that underflows
@@ -44,6 +44,9 @@
 //            EOS            while c < the entry's eos_from_col
 //          A banned token's x' is -inf (after the penalty; the arg-max fallback, the maximum, top-k, top-p, the draw
 //          and the log-probs follow), and the token picked is written at h[c] (DESIGN.md section 3, "Banned tokens").
+//          With the warper settings (SampleArgs::min_p) a sampled row then applies HF's MinP, Typical, Epsilon and
+//          Eta warpers after top-p, each removing tokens from the kept set (warp_row; DESIGN.md section 3, "Min-p,
+//          typical, epsilon and eta"); the draw and the log-probs use the final set and its own maximum.
 #include <math.h>
 
 #include <type_traits>
@@ -82,15 +85,16 @@ constexpr uint32_t KEY_NEG_INF = 0x007fu;   // order_key(-inf)
 // a row of up to 2^17 tokens sum exactly, below 2^53, in any order)
 __device__ __forceinline__ unsigned long long fixed_mass(float w) { return __float2ull_rn(w * 68719476736.f); }
 
-// The top-p threshold of a sampled row on the 32-bit keys: with q the fixed-point masses of the kept tokens
-// (z >= zthr), Q their sum and F(k) the sum of q over the kept keys strictly above k, the smallest key tau such
-// that every kept key k >= tau has F(k) < p * Q (fp64 product of fp64(p) and Q; tau = the largest key when that is
-// 0). Keys >= tau are then exactly the kept keys with F(k) < p * Q, ties whole. Four 8-bit passes from the high
-// byte, each histogramming the masses inside the bytes chosen so far; in a pass the chosen bin is the lowest one
-// whose mass above (those of the higher bins, plus the mass above the prefix) is below p * Q. Integer sums: the
-// same bits on every run. s_mass: 256 + SM_WARPS 64-bit words.
-__device__ __forceinline__ uint32_t top_p_threshold(const uint32_t* skey, int V, float zthr, float zmax, float p,
-                                                    uint32_t kmax, unsigned long long* s_mass, uint32_t* s_sel) {
+// The mass threshold of a sampled row on 32-bit keys, shared by top-p and the typical warper: with key(i) a token's
+// key and q = mass(i) its fixed-point mass (0: not counted), Q the sum of q and F(k) the sum of q over the keys
+// strictly above k, the smallest key tau such that every counted key k >= tau has F(k) < p * Q (fp64 product of
+// fp64(p) and Q; `fallback` when that is 0). Keys >= tau are then exactly the keys with F(k) < p * Q, ties whole.
+// Four 8-bit passes from the high byte, each histogramming the masses inside the bytes chosen so far; in a pass the
+// chosen bin is the lowest one whose mass above (those of the higher bins, plus the mass above the prefix) is below
+// p * Q. Integer sums: the same bits on every run. s_mass: 256 + SM_WARPS 64-bit words.
+template <class KeyF, class MassF>
+__device__ __forceinline__ uint32_t mass_threshold(int V, float p, uint32_t fallback, KeyF key_of, MassF mass_of,
+                                                   unsigned long long* s_mass, uint32_t* s_sel) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   unsigned long long* s_wm = s_mass + 256;
   __shared__ unsigned long long s_base;
@@ -108,10 +112,9 @@ __device__ __forceinline__ uint32_t top_p_threshold(const uint32_t* skey, int V,
       uint32_t bin = 256;             // none
       unsigned long long q = 0;
       if (i < V) {
-        const uint32_t key = skey[i];
-        const float z = key_value32(key);
-        if ((pass == 0 || (key >> (shift + 8)) == prefix) && z >= zthr) {
-          q = fixed_mass(expf(z - zmax));
+        const uint32_t key = key_of(i);
+        if (pass == 0 || (key >> (shift + 8)) == prefix) {
+          q = mass_of(i);
           if (q != 0) bin = (key >> shift) & 0xffu;
         }
       }
@@ -134,11 +137,11 @@ __device__ __forceinline__ uint32_t top_p_threshold(const uint32_t* skey, int V,
       if (lane == 31) s_wm[warp] = incl;
     }
     __syncthreads();
-    if (pass == 0) {   // Q = the whole kept mass
+    if (pass == 0) {   // Q = the whole counted mass
       unsigned long long Q = 0;
       for (int w = 0; w < 8; ++w) Q += s_wm[w];
       P = (double)p * (double)Q;
-      if (!(P > 0.0)) return kmax;   // (uniform: every thread sees the same Q)
+      if (!(P > 0.0)) return fallback;   // (uniform: every thread sees the same Q)
     }
     if (tid < 256) {
       for (int w = 0; w < warp; ++w) incl += s_wm[w];
@@ -157,6 +160,108 @@ __device__ __forceinline__ uint32_t top_p_threshold(const uint32_t* skey, int V,
   return prefix;
 }
 
+// sums of two 64-bit integers over the block, to every thread (exact, so in any order); s_u64: 2 * SM_WARPS words
+__device__ __forceinline__ void block_sum2(unsigned long long* a, unsigned long long* b, unsigned long long* s_u64) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    *a += __shfl_xor_sync(0xffffffffu, *a, o);
+    *b += __shfl_xor_sync(0xffffffffu, *b, o);
+  }
+  __syncthreads();   // (s_u64 is shared memory an earlier stage used)
+  if (lane == 0) { s_u64[warp] = *a; s_u64[SM_WARPS + warp] = *b; }
+  __syncthreads();
+  unsigned long long sa = 0, sb = 0;
+  for (int w = 0; w < SM_WARPS; ++w) { sa += s_u64[w]; sb += s_u64[SM_WARPS + w]; }
+  *a = sa; *b = sb;
+  __syncthreads();
+}
+
+// The warpers of a sampled row on the 32-bit keys (DESIGN.md section 3, "Min-p, typical, epsilon and eta"), in HF's
+// order, each over the set the stages before it kept: the kept tokens are those with z = key_value32(key) >= zthr,
+// and a warper removes a token by rewriting its key to 0 (a NaN, below every key), so the later stages, the draw and
+// the log-probs see the smaller set. With w = expf(z - zmax), q = fixed_mass(w), Q = sum q and D = sum of
+// rint(q * (zmax - z)) in fp64 over the current set (integers: the same in any order):
+//   min-p    (mp > 0)      keep iff w >= mp
+//   typical  (ty < 1)      c = D / Q (the mean of zmax - z, so d = |(zmax - z) - c| = |-log p - H|), d rounded to fp32;
+//                          keep j iff the mass of the tokens of smaller d is < ty * Q (mass_threshold on the keys
+//                          ~order_key32(d)); then zmax becomes the largest kept z, since this set need not hold it
+//   epsilon  (ep > 0)      keep iff q >= fp64(ep) * Q or z = zmax
+//   eta      (et > 0)      H = D / Q + log(Q) - 36 log 2, eta = min(et, sqrt(et) exp(-H)) in fp64; keep iff
+//                          q >= eta * Q or z = zmax
+// Returns the z_max of the final set. s_u64: 256 + SM_WARPS words; s_wmax: SM_WARPS words.
+__device__ __noinline__ float warp_row(uint32_t* skey, int V, float zthr, float zmax, float mp, float ty, float ep,
+                                       float et, unsigned long long* s_u64, uint32_t* s_sel, uint32_t* s_wmax) {
+  const int tid = threadIdx.x;
+  auto mass = [&](int i) -> unsigned long long {
+    const float z = key_value32(skey[i]);
+    return z >= zthr ? fixed_mass(expf(z - zmax)) : 0ull;
+  };
+  auto stats = [&](unsigned long long* Q, unsigned long long* D) {
+    *Q = 0; *D = 0;
+    for (int i = tid; i < V; i += SM_THREADS) {
+      const float z = key_value32(skey[i]);
+      if (z >= zthr) {
+        const unsigned long long q = fixed_mass(expf(z - zmax));
+        if (q != 0) { *Q += q; *D += __double2ull_rn((double)q * ((double)zmax - (double)z)); }
+      }
+    }
+    block_sum2(Q, D, s_u64);
+  };
+  // remove the kept tokens whose mass is below thr, but never one at zmax
+  auto cut = [&](double thr) {
+    for (int i = tid; i < V; i += SM_THREADS) {
+      const float z = key_value32(skey[i]);
+      if (z >= zthr && z != zmax && (double)fixed_mass(expf(z - zmax)) < thr) skey[i] = 0u;
+    }
+    __syncthreads();
+  };
+  if (mp > 0.f) {
+    for (int i = tid; i < V; i += SM_THREADS) {
+      const float z = key_value32(skey[i]);
+      if (z >= zthr && expf(z - zmax) < mp) skey[i] = 0u;
+    }
+    __syncthreads();
+  }
+  if (ty < 1.f) {
+    unsigned long long Q, D;
+    stats(&Q, &D);
+    const double c = (double)D / (double)Q;
+    auto dkey = [&](int i) -> uint32_t {   // a larger key for a smaller deviation; 0 outside the set
+      const float z = key_value32(skey[i]);
+      if (!(z >= zthr)) return 0u;
+      return ~order_key32(__double2float_rn(fabs(((double)zmax - (double)z) - c)));
+    };
+    const uint32_t tau = mass_threshold(V, ty, 0u, dkey, mass, s_u64, s_sel);
+    // the largest kept key afterwards (keys below zthr are below every kept one, removed keys are 0)
+    uint32_t kmax = 0;
+    for (int i = tid; i < V; i += SM_THREADS) {
+      const uint32_t k = skey[i];
+      if (k != 0u && dkey(i) < tau) skey[i] = 0u;
+      else kmax = k > kmax ? k : kmax;
+    }
+    kmax = __reduce_max_sync(0xffffffffu, kmax);
+    if ((tid & 31) == 0) s_wmax[tid >> 5] = kmax;
+    __syncthreads();
+    for (int w = 0; w < SM_WARPS; ++w) kmax = s_wmax[w] > kmax ? s_wmax[w] : kmax;
+    __syncthreads();
+    zmax = key_value32(kmax);
+  }
+  if (ep > 0.f) {
+    unsigned long long Q, D;
+    stats(&Q, &D);
+    cut((double)ep * (double)Q);
+  }
+  if (et > 0.f) {
+    unsigned long long Q, D;
+    stats(&Q, &D);
+    const double H = (double)D / (double)Q + log((double)Q) - 36.0 * 0.69314718055994530942;
+    const double eta = fmin((double)et, sqrt((double)et) * exp(-H));
+    cut(eta * (double)Q);
+  }
+  return zmax;
+}
+
 // place q of a log-prob row
 __device__ __forceinline__ void put_lp(const SampleArgs& a, long long row, int q, int id, float lp) {
   const long long o = row + q;
@@ -173,7 +278,7 @@ sample_kernel(SampleArgs a) {
   Key* skey = reinterpret_cast<Key*>(s_stage);
   __shared__ unsigned long long s_red[SM_WARPS];
   __shared__ float s_sum[SM_WARPS];
-  // the count histogram; on the 32-bit path also the 64-bit masses of top_p_threshold (256 + SM_WARPS words)
+  // the count histogram; on the 32-bit path also the 64-bit masses of mass_threshold (256 + SM_WARPS words)
   __shared__ __align__(8) uint32_t s_hist[WIDE ? 2 * (256 + SM_WARPS) : 256];
   __shared__ uint32_t s_wcnt[8];
   __shared__ uint32_t s_sel[2];
@@ -324,7 +429,7 @@ sample_kernel(SampleArgs a) {
     else return __fdiv_rn(key_value(key), T);
   };
   auto position = [&]() { return col - (a.n_pad != nullptr ? a.n_pad[t] : 0); };
-  const float zmax = zval(kmax);
+  float zmax = zval(kmax);   // (the warpers may lower it)
   if ((greedy && n_lp < 0) || !isfinite(zmax)) {   // greedy entry, or no finite scaled maximum: the arg-max
     if (tid == 0) emit(amax);
     if (n_lp >= 0) {
@@ -349,11 +454,24 @@ sample_kernel(SampleArgs a) {
   if constexpr (WIDE) {   // top-p narrows the kept set to the keys >= tau
     const float top_p = a.top_p[t];
     if (!greedy && top_p < 1.f) {
-      const uint32_t tau = top_p_threshold(reinterpret_cast<const uint32_t*>(skey), V, zthr, zmax, top_p, kmax,
-                                           reinterpret_cast<unsigned long long*>(s_hist), s_sel);
+      const uint32_t* wkey = reinterpret_cast<const uint32_t*>(skey);
+      const uint32_t tau = mass_threshold(
+          V, top_p, kmax, [&](int i) { return wkey[i]; },
+          [&](int i) -> unsigned long long {
+            const float z = key_value32(wkey[i]);
+            return z >= zthr ? fixed_mass(expf(z - zmax)) : 0ull;
+          },
+          reinterpret_cast<unsigned long long*>(s_hist), s_sel);
       const float ztau = key_value32(tau);
       if (ztau > zthr) zthr = ztau;
       __syncthreads();   // s_hist / s_sel are reused below
+    }
+    // min-p, typical, epsilon and eta narrow it further (their table off: the launch has none)
+    if (!greedy && a.min_p != nullptr) {
+      const float mp = a.min_p[t], ty = a.typical_p[t], ep = a.epsilon[t], et = a.eta[t];
+      if (mp > 0.f || ty < 1.f || ep > 0.f || et > 0.f)
+        zmax = warp_row(reinterpret_cast<uint32_t*>(skey), V, zthr, zmax, mp, ty, ep, et,
+                        reinterpret_cast<unsigned long long*>(s_hist), s_sel, s_cnt);
     }
   }
 
@@ -465,6 +583,8 @@ int launch_sample(const SampleArgs& a, cudaStream_t stream) {
               "sample: the 32-bit path needs the repetition penalties and a token set of %d words", (a.V + 31) / 32);
   VCL_REQUIRE(a.bans == nullptr || (wide && a.hist != nullptr && a.hist_ld > 0),
               "sample: a ban table needs the 32-bit path and the token histories");
+  VCL_REQUIRE(a.min_p == nullptr || (wide && a.typical_p && a.epsilon && a.eta),
+              "sample: the warpers need the 32-bit path and all four settings");
   if (a.B == 0) return 0;
   if (wide) {
     static bool attr = false;

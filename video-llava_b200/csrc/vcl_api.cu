@@ -157,10 +157,11 @@ struct vcl_handle {
                                                // written by each vcl_llm_slots_prefill with one host-to-device copy
   // The sampling table (vcl_llm_set_sampling(_ex), vcl_llm_set_logprobs): entry b belongs to clip b / cache slot b.
   // One device block at a fixed address, [max_batch] seeds (u64), temperatures (f32), top_k (i32), top_n (i32),
-  // top_p (f32), repetition penalties (f32), so one sampled decode graph serves every setting; samp_host is its host
-  // copy, written whole by one host-to-device copy per call. Greedy without log-probs (top_n -1), top_p 1 and
-  // penalty 1 at vcl_create.
-  static constexpr int SAMP_BYTES = 28;   // per entry
+  // top_p (f32), repetition penalties (f32), then the warpers (vcl_llm_set_warpers): min_p, typical_p, epsilon and
+  // eta (f32), so one sampled decode graph serves every setting; samp_host is its host copy, written whole by one
+  // host-to-device copy per call. Greedy without log-probs (top_n -1), top_p 1, penalty 1 and the warpers off (min_p
+  // 0, typical_p 1, epsilon 0, eta 0) at vcl_create.
+  static constexpr int SAMP_BYTES = 44;   // per entry
   unsigned char* samp = nullptr;
   std::vector<unsigned char> samp_host;
   unsigned long long* samp_seed(unsigned char* base) const { return reinterpret_cast<unsigned long long*>(base); }
@@ -169,13 +170,27 @@ struct vcl_handle {
   int* samp_topn(unsigned char* base) const { return reinterpret_cast<int*>(base + 16 * cfg.max_batch); }
   float* samp_topp(unsigned char* base) const { return reinterpret_cast<float*>(base + 20 * cfg.max_batch); }
   float* samp_rep(unsigned char* base) const { return reinterpret_cast<float*>(base + 24 * cfg.max_batch); }
+  float* samp_minp(unsigned char* base) const { return reinterpret_cast<float*>(base + 28 * cfg.max_batch); }
+  float* samp_typ(unsigned char* base) const { return reinterpret_cast<float*>(base + 32 * cfg.max_batch); }
+  float* samp_eps(unsigned char* base) const { return reinterpret_cast<float*>(base + 36 * cfg.max_batch); }
+  float* samp_eta(unsigned char* base) const { return reinterpret_cast<float*>(base + 40 * cfg.max_batch); }
+  bool warp_on(int b) {
+    unsigned char* hb = samp_host.data();
+    return samp_minp(hb)[b] > 0.f || samp_typ(hb)[b] < 1.f || samp_eps(hb)[b] > 0.f || samp_eta(hb)[b] > 0.f;
+  }
+  // entry b's warpers off
+  void warp_off(int b) {
+    unsigned char* hb = samp_host.data();
+    samp_minp(hb)[b] = 0.f; samp_typ(hb)[b] = 1.f; samp_eps(hb)[b] = 0.f; samp_eta(hb)[b] = 0.f;
+  }
   // what entry b needs: 0 the arg-max, 1 the sampler (it samples, with a temperature above 0, or wants log-probs),
-  // 2 the 32-bit sampler (a repetition penalty, or top-p on a sampled entry), 3 the 32-bit sampler with bans
+  // 2 the 32-bit sampler (a repetition penalty, or top-p or a warper on a sampled entry), 3 the 32-bit sampler with
+  // bans
   int sampler_of(int b) {
     unsigned char* hb = samp_host.data();
     const float T = samp_temp(hb)[b];
     if (!bans_host.empty() && ban_on(b)) return 3;
-    if (samp_rep(hb)[b] != 1.f || (T > 0.f && samp_topp(hb)[b] < 1.f)) return 2;
+    if (samp_rep(hb)[b] != 1.f || (T > 0.f && (samp_topp(hb)[b] < 1.f || warp_on(b)))) return 2;
     return T > 0.f || samp_topn(hb)[b] >= 0 ? 1 : 0;
   }
   // ... and what entries first .. first + n - 1 need together
@@ -534,6 +549,7 @@ int vcl_create(vcl_handle** out, const vcl_config* c) {
     h->samp_topn(h->samp_host.data())[b] = -1;
     h->samp_topp(h->samp_host.data())[b] = 1.f;
     h->samp_rep(h->samp_host.data())[b] = 1.f;
+    h->warp_off((int)b);
   }
   if (rc == 0) rc = launch_rope_table(h->rope_cos, h->rope_sin, c->max_seq, 128, c->rope_theta, 0);
   if (rc == 0) {
@@ -836,8 +852,10 @@ int lm_head_argmax(vcl_handle* h, const bf16* x, long long ldx, int B, float* lo
       sa.lp_entry = (long long)h->lp_rows() * (1 + VCL_LOGPROBS_MAX); sa.lp_pos = 1 + VCL_LOGPROBS_MAX;
       sa.lp_rows = h->lp_rows();
     }
-    if (smp.on >= 2) {   // the 32-bit sampler: top_p, the penalties and the token sets
+    if (smp.on >= 2) {   // the 32-bit sampler: top_p, the penalties, the token sets and the warpers
       sa.top_p = h->samp_topp(h->samp); sa.rep = h->samp_rep(h->samp);
+      sa.min_p = h->samp_minp(h->samp); sa.typical_p = h->samp_typ(h->samp);
+      sa.epsilon = h->samp_eps(h->samp); sa.eta = h->samp_eta(h->samp);
       sa.tset = h->tset; sa.tset_words = h->tset_words();
     }
     if (smp.on == 3) {   // ... and the bans, over the token histories
@@ -1722,6 +1740,7 @@ int vcl_llm_set_sampling(vcl_handle* h, int n, const int32_t* clips_host, const 
     h->samp_topk(hb)[b] = top_k_host[i];
     h->samp_topp(hb)[b] = 1.f;
     h->samp_rep(hb)[b] = 1.f;
+    h->warp_off(b);
   }
   VCL_CUDA_OK(cudaMemcpyAsync(h->samp, hb, h->samp_host.size(), cudaMemcpyHostToDevice, as_stream(stream)));
   return 0;
@@ -1777,8 +1796,53 @@ int vcl_llm_set_sampling_ex(vcl_handle* h, int n, const int32_t* clips_host, con
     h->samp_topk(hb)[b] = top_k_host[i];
     h->samp_topp(hb)[b] = top_p_host[i];
     h->samp_rep(hb)[b] = repetition_penalty_host[i];
+    h->warp_off(b);
   }
   VCL_CUDA_OK(cudaMemcpyAsync(h->samp, hb, h->samp_host.size(), cudaMemcpyHostToDevice, st));
+  return 0;
+}
+
+// one entry's warper settings, checked with HF's messages (off: min_p 0, typical_p 1, epsilon 0, eta 0)
+static int check_warpers(const char* name, int b, float mp, float ty, float ep, float et) {
+  VCL_REQUIRE(mp >= 0.f && mp <= 1.f, "%s: entry %d: `min_p` has to be a float in the [0, 1] interval, but is %g", name,
+              b, (double)mp);
+  VCL_REQUIRE(ty > 0.f && ty <= 1.f, "%s: entry %d: `typical_p` has to be a float > 0 and < 1 (1: off), but is %g",
+              name, b, (double)ty);
+  VCL_REQUIRE(ep >= 0.f && ep < 1.f, "%s: entry %d: `epsilon_cutoff` has to be a float > 0 and < 1 (0: off), but is %g",
+              name, b, (double)ep);
+  VCL_REQUIRE(et >= 0.f && et < 1.f, "%s: entry %d: `eta_cutoff` has to be a float > 0 and < 1 (0: off), but is %g",
+              name, b, (double)et);
+  return 0;
+}
+
+int vcl_llm_set_warpers(vcl_handle* h, int n, const int32_t* clips_host, const float* min_p_host,
+                        const float* typical_p_host, const float* epsilon_host, const float* eta_host, void* stream) {
+  VCL_REQUIRE(h != nullptr, "vcl_llm_set_warpers: null handle");
+  const int mb = h->cfg.max_batch;
+  VCL_REQUIRE(n >= 1 && n <= mb, "vcl_llm_set_warpers: n=%d outside 1..%d", n, mb);
+  VCL_REQUIRE(clips_host && min_p_host && typical_p_host && epsilon_host && eta_host,
+              "vcl_llm_set_warpers: null argument");
+  for (int i = 0; i < n; ++i) {
+    const int b = clips_host[i];
+    VCL_REQUIRE(b >= 0 && b < mb, "vcl_llm_set_warpers: clip %d outside 0..%d", b, mb - 1);
+    for (int j = 0; j < i; ++j)
+      VCL_REQUIRE(clips_host[j] != b, "vcl_llm_set_warpers: clip %d is given twice", b);
+    VCL_TRY(check_warpers("vcl_llm_set_warpers", b, min_p_host[i], typical_p_host[i], epsilon_host[i], eta_host[i]));
+    const bool on = min_p_host[i] > 0.f || typical_p_host[i] < 1.f || epsilon_host[i] > 0.f || eta_host[i] > 0.f;
+    VCL_REQUIRE(!on || h->cfg.vocab <= VCL_SAMPLE_WIDE_MAX_V,
+                "vcl_llm_set_warpers: clip %d: min_p, typical_p, epsilon_cutoff and eta_cutoff take a vocabulary of at "
+                "most %d tokens (the sampler's shared memory), this model has %d", b, VCL_SAMPLE_WIDE_MAX_V,
+                h->cfg.vocab);
+  }
+  unsigned char* hb = h->samp_host.data();
+  for (int i = 0; i < n; ++i) {
+    const int b = clips_host[i];
+    h->samp_minp(hb)[b] = min_p_host[i];
+    h->samp_typ(hb)[b] = typical_p_host[i];
+    h->samp_eps(hb)[b] = epsilon_host[i];
+    h->samp_eta(hb)[b] = eta_host[i];
+  }
+  VCL_CUDA_OK(cudaMemcpyAsync(h->samp, hb, h->samp_host.size(), cudaMemcpyHostToDevice, as_stream(stream)));
   return 0;
 }
 
@@ -2368,7 +2432,7 @@ int op_sample(const char* name, const float* logits, int64_t ld, int B, int V, c
               const float* top_p_host = nullptr, const float* rep_host = nullptr, uint32_t* tset = nullptr,
               int32_t* hist = nullptr, int64_t hist_ld = 0, const int32_t* ngram_host = nullptr,
               const int32_t* eos_host = nullptr, const int32_t* eos_from_host = nullptr,
-              const int32_t* words_host = nullptr) {
+              const int32_t* words_host = nullptr, const float* const* warp_host = nullptr) {
   if (check_device() != 0) return -2;
   VCL_REQUIRE(logits && temperature_host && top_k_host && seed_host && counter_host && tok_out, "%s: null argument",
               name);
@@ -2383,6 +2447,12 @@ int op_sample(const char* name, const float* logits, int64_t ld, int B, int V, c
                   "%s: row %d: top_p %g outside [0, 1] or repetition_penalty %g not a finite value > 0", name, b,
                   (double)top_p_host[b], (double)rep_host[b]);
   }
+  const bool warp = warp_host != nullptr;   // min_p, typical_p, epsilon, eta [B] each
+  if (warp) {
+    VCL_REQUIRE(wide && warp_host[0] && warp_host[1] && warp_host[2] && warp_host[3], "%s: null argument", name);
+    for (int b = 0; b < B; ++b)
+      VCL_TRY(check_warpers(name, b, warp_host[0][b], warp_host[1][b], warp_host[2][b], warp_host[3][b]));
+  }
   for (int b = 0; b < B; ++b)
     VCL_REQUIRE(isfinite(temperature_host[b]) && temperature_host[b] >= 0.f && top_k_host[b] >= 0 &&
                 counter_host[b] >= 0, "%s: row %d: temperature %g, top_k %d, counter %d", name, b,
@@ -2392,9 +2462,10 @@ int op_sample(const char* name, const float* logits, int64_t ld, int B, int V, c
       VCL_REQUIRE(top_n_host[b] >= -1 && top_n_host[b] <= VCL_LOGPROBS_MAX, "%s: row %d: top_n %d outside -1..%d",
                   name, b, top_n_host[b], VCL_LOGPROBS_MAX);
   // the per-row settings in one stream-ordered block: [B] seeds, temperatures, top_k, counters, top_n, top_p,
-  // penalties, then the ban table [B][VCL_BAN_ROW]
+  // penalties, then the ban table [B][VCL_BAN_ROW], then [4][B] warper settings
   const bool bans = hist != nullptr;
-  std::vector<unsigned char> hb((size_t)B * (wide ? 32 : 24) + (bans ? (size_t)B * VCL_BAN_ROW * 4 : 0));
+  const size_t warp_at = (size_t)B * (wide ? 32 : 24) + (bans ? (size_t)B * VCL_BAN_ROW * 4 : 0);
+  std::vector<unsigned char> hb(warp_at + (warp ? (size_t)B * 16 : 0));
   if (bans) {
     for (int b = 0; b < B; ++b) {
       VCL_REQUIRE(counter_host[b] < hist_ld, "%s: row %d: column %d outside the history of %lld columns", name, b,
@@ -2413,6 +2484,8 @@ int op_sample(const char* name, const float* logits, int64_t ld, int B, int V, c
     memcpy(hb.data() + (size_t)B * 24, top_p_host, (size_t)B * 4);
     memcpy(hb.data() + (size_t)B * 28, rep_host, (size_t)B * 4);
   }
+  if (warp)
+    for (int j = 0; j < 4; ++j) memcpy(hb.data() + warp_at + (size_t)j * B * 4, warp_host[j], (size_t)B * 4);
   cudaStream_t st = as_stream(stream);
   unsigned char* d = nullptr;
   VCL_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&d), hb.size(), st));
@@ -2436,6 +2509,10 @@ int op_sample(const char* name, const float* logits, int64_t ld, int B, int V, c
   if (bans) {   // row b: entry b, its history hist[b * hist_ld ..] and the draw at column counter[b]
     sa.bans = reinterpret_cast<const int*>(d + (size_t)B * 32);
     sa.hist = hist; sa.hist_ld = hist_ld;
+  }
+  if (warp) {
+    const float* w = reinterpret_cast<const float*>(d + warp_at);
+    sa.min_p = w; sa.typical_p = w + B; sa.epsilon = w + 2 * B; sa.eta = w + 3 * B;
   }
   const int rc = launch_sample(sa, st);
   VCL_CUDA_OK(cudaFreeAsync(d, st));
@@ -2579,6 +2656,22 @@ int vcl_op_sample_ex(const float* logits, int64_t ld, int B, int V, const float*
   VCL_REQUIRE(top_n_host == nullptr || (ids_out && lp_out), "vcl_op_sample_ex: log-probs need ids_out and lp_out");
   return op_sample("vcl_op_sample_ex", logits, ld, B, V, temperature_host, top_k_host, seed_host, counter_host,
                    top_n_host, tok_out, ids_out, lp_out, stream, top_p_host, repetition_penalty_host, token_sets);
+}
+
+int vcl_op_sample_warpers(const float* logits, int64_t ld, int B, int V, const float* temperature_host,
+                          const int32_t* top_k_host, const uint64_t* seed_host, const int32_t* counter_host,
+                          const float* top_p_host, const float* repetition_penalty_host, uint32_t* token_sets,
+                          const float* min_p_host, const float* typical_p_host, const float* epsilon_host,
+                          const float* eta_host, const int32_t* top_n_host, int32_t* tok_out, int32_t* ids_out,
+                          float* lp_out, void* stream) {
+  VCL_REQUIRE(top_p_host && repetition_penalty_host && min_p_host && typical_p_host && epsilon_host && eta_host,
+              "vcl_op_sample_warpers: null argument");
+  VCL_REQUIRE(top_n_host == nullptr || (ids_out && lp_out), "vcl_op_sample_warpers: log-probs need ids_out and "
+              "lp_out");
+  const float* warp[4] = {min_p_host, typical_p_host, epsilon_host, eta_host};
+  return op_sample("vcl_op_sample_warpers", logits, ld, B, V, temperature_host, top_k_host, seed_host, counter_host,
+                   top_n_host, tok_out, ids_out, lp_out, stream, top_p_host, repetition_penalty_host, token_sets,
+                   nullptr, 0, nullptr, nullptr, nullptr, nullptr, warp);
 }
 
 int vcl_op_sample_bans(const float* logits, int64_t ld, int B, int V, const float* temperature_host,

@@ -143,6 +143,8 @@ _SIGNATURES = {
                                      POINTER(c_uint64), c_void_p]),
     "vcl_llm_set_sampling_ex": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_float), POINTER(c_int32),
                                         POINTER(c_uint64), POINTER(c_float), POINTER(c_float), c_void_p]),
+    "vcl_llm_set_warpers": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_float), POINTER(c_float),
+                                    POINTER(c_float), POINTER(c_float), c_void_p]),
     "vcl_llm_set_token_set": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "vcl_llm_read_token_set": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "vcl_llm_set_bans": (c_int, [c_void_p, c_int, POINTER(c_int32), POINTER(c_int32), POINTER(c_int32),
@@ -192,6 +194,10 @@ _SIGNATURES = {
     "vcl_op_sample_ex": (c_int, [c_void_p, c_int64, c_int, c_int, POINTER(c_float), POINTER(c_int32), POINTER(c_uint64),
                                  POINTER(c_int32), POINTER(c_float), POINTER(c_float), c_void_p, POINTER(c_int32),
                                  c_void_p, c_void_p, c_void_p, c_void_p]),
+    "vcl_op_sample_warpers": (c_int, [c_void_p, c_int64, c_int, c_int, POINTER(c_float), POINTER(c_int32),
+                                      POINTER(c_uint64), POINTER(c_int32), POINTER(c_float), POINTER(c_float), c_void_p,
+                                      POINTER(c_float), POINTER(c_float), POINTER(c_float), POINTER(c_float),
+                                      POINTER(c_int32), c_void_p, c_void_p, c_void_p, c_void_p]),
     "vcl_op_guidance": (c_int, [c_void_p, c_int64, c_int, c_int, POINTER(c_int32), POINTER(c_float), c_void_p,
                                 c_void_p]),
     "vcl_op_beam_select": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p,
@@ -470,6 +476,36 @@ def op_sample_ex(logits, temperature, top_k, seed, counter, top_p, repetition_pe
                                  _seeds(seed, B), ints(vals[2]), flts(vals[3]), flts(vals[4]), ptr(token_sets),
                                  ints(vals[5]) if top_n is not None else None, ptr(out), ptr(ids), ptr(lp),
                                  cur_stream()))
+    return out if top_n is None else (out, ids, lp)
+
+
+def op_sample_warpers(logits, temperature, top_k, seed, counter, top_p, repetition_penalty, min_p, typical_p,
+                      epsilon, eta, token_sets=None, top_n=None):
+    """The 32-bit sampler with HF's min-p / typical / epsilon / eta warpers alone (vcl_op_sample_warpers):
+    op_sample_ex's arguments plus B host values each of min_p (0: off), typical_p (1: off), epsilon and eta (0: off).
+    Returns what op_sample_ex returns."""
+    B, ld = logits.shape
+    assert logits.dtype == torch.float32 and logits.stride(1) == 1
+    vals = [list(v) for v in (temperature, top_k, counter, top_p, repetition_penalty, min_p, typical_p, epsilon, eta)]
+    if top_n is not None:
+        vals.append(list(top_n))
+    if not all(len(v) == B for v in vals):
+        raise VclError(f"every per-row setting needs {B} entries")
+    if token_sets is not None:
+        assert token_sets.is_cuda and token_sets.dtype == torch.int32 and token_sets.is_contiguous()
+        assert tuple(token_sets.shape) == (B, token_set_words(ld))
+    out = torch.empty(B, dtype=torch.int32, device=logits.device)
+    ids = lp = None
+    if top_n is not None:
+        ids = torch.full((B, LOGPROB_PLACES), -1, dtype=torch.int32, device=logits.device)
+        lp = torch.full((B, LOGPROB_PLACES), float("nan"), dtype=torch.float32, device=logits.device)
+    ints = lambda v: (c_int32 * B)(*[int(x) for x in v])   # noqa: E731
+    flts = lambda v: (c_float * B)(*[float(x) for x in v])   # noqa: E731
+    check(lib().vcl_op_sample_warpers(c_void_p(logits.data_ptr()), logits.stride(0), B, ld, flts(vals[0]),
+                                      ints(vals[1]), _seeds(seed, B), ints(vals[2]), flts(vals[3]), flts(vals[4]),
+                                      ptr(token_sets), flts(vals[5]), flts(vals[6]), flts(vals[7]), flts(vals[8]),
+                                      ints(vals[9]) if top_n is not None else None, ptr(out), ptr(ids), ptr(lp),
+                                      cur_stream()))
     return out if top_n is None else (out, ids, lp)
 
 
@@ -1007,6 +1043,18 @@ class Engine:
         check(lib().vcl_llm_set_sampling_ex(self._h, n, (c_int32 * n)(*[int(b) for b in clips]), flts(temperature),
                                             (c_int32 * n)(*[int(k) for k in top_k]), _seeds(seed, n), flts(top_p),
                                             flts(repetition_penalty), cur_stream()))
+
+    def set_warpers(self, clips, min_p, typical_p, epsilon, eta):
+        """HF's min-p / typical / epsilon / eta warpers of entries `clips` (vcl_llm_set_warpers): min_p[i] (0: off),
+        typical_p[i] (1: off), epsilon[i] and eta[i] (0: off). set_sampling / set_sampling_ex turn them off for the
+        entries they write, so call this after them. Host lists of equal length."""
+        n = len(clips)
+        if not (len(min_p) == len(typical_p) == len(epsilon) == len(eta) == n):
+            raise VclError(f"{n} clips, {len(min_p)} min_p, {len(typical_p)} typical_p, {len(epsilon)} epsilon, "
+                           f"{len(eta)} eta")
+        flts = lambda v: (c_float * n)(*[float(x) for x in v])   # noqa: E731
+        check(lib().vcl_llm_set_warpers(self._h, n, (c_int32 * n)(*[int(b) for b in clips]), flts(min_p),
+                                        flts(typical_p), flts(epsilon), flts(eta), cur_stream()))
 
     def set_token_set(self, entry, ids):
         """Entry `entry`'s token set of the repetition penalty becomes the ids of `ids` (any int tensor or list;

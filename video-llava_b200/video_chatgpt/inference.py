@@ -87,7 +87,8 @@ def video_chatgpt_infer(video_frames, question, conv_mode, model, vision_tower, 
                         video_token_len, transcript=None, do_sample=True, temperature=0.2, max_new_tokens=1024,
                         video_key=None, feature_cache: "VideoFeatureCache | None" = None, seed=None, top_p=1.0,
                         repetition_penalty=1.0, no_repeat_ngram_size=None, bad_words_ids=None, min_new_tokens=None,
-                        guidance_scale=None, penalty_alpha=None, top_k=None):
+                        guidance_scale=None, penalty_alpha=None, top_k=None, min_p=None, typical_p=None,
+                        epsilon_cutoff=None, eta_cutoff=None):
     """Same flow as the reference: prompt -> tokenizer -> image processor -> tower -> pool -> generate
     -> decode. `do_sample/temperature/max_new_tokens` default to the reference's hard-coded values.
     Extension (off by default): with `video_key` and a `VideoFeatureCache`, the pooled features of a
@@ -105,7 +106,9 @@ def video_chatgpt_infer(video_frames, question, conv_mode, model, vision_tower, 
     toward what the video, not the text alone, makes likely (visual contrastive decoding).
     penalty_alpha (off by default, None) with top_k (HF's 50 when None): contrastive search, passed to generate; it
     decodes without sampling (do_sample is then False, as HF's contrastive search is), for long answers that greedy
-    and sampled decoding tend to repeat."""
+    and sampled decoding tend to repeat.
+    min_p / typical_p / epsilon_cutoff / eta_cutoff (off by default, None): HF's min-p, typical, epsilon and eta
+    sampling warpers, passed to generate (min_p suits the reference's low-temperature sampling)."""
     use_se = model.get_model().vision_config.use_vid_start_end
     prompt, conv = build_prompt(question, conv_mode, video_token_len, use_se, transcript)
     inputs = tokenizer([prompt])
@@ -146,7 +149,9 @@ def video_chatgpt_infer(video_frames, question, conv_mode, model, vision_tower, 
                                     pad_token_id=getattr(tokenizer, "pad_token_id", None), seed=seed, top_p=top_p,
                                     repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size,
                                     bad_words_ids=bad_words_ids, min_new_tokens=min_new_tokens,
-                                    guidance_scale=guidance_scale, negative_prompt_ids=neg_ids, **contrastive)
+                                    guidance_scale=guidance_scale, negative_prompt_ids=neg_ids, min_p=min_p,
+                                    typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff,
+                                    **contrastive)
     n_diff = (input_ids != output_ids[:, :input_ids.shape[1]]).sum().item()
     if n_diff > 0:
         print(f"[Warning] {n_diff} output_ids are not the same as the input_ids")

@@ -10,8 +10,8 @@ import vcl_native as vn
 
 def request(model, i, r, max_new_tokens, stopping_criteria, n_vid, samp):
     """One request of generate_requests, checked on the host -> (ids [S] int64 on the host, S, n, feats,
-    vid_start, criteria, its sampling-table entry: temperature (0: greedy), top_k, seed, top_p, penalty, and its bans
-    (model._ban_args; None: none))"""
+    vid_start, criteria, its sampling-table entry: temperature (0: greedy), top_k, seed, top_p, penalty, warp
+    (model._warper_args; None: none), and its bans (model._ban_args; None: none))"""
     if isinstance(r, torch.Tensor):
         r = {"input_ids": r}
     ids = torch.as_tensor(r["input_ids"]).detach().cpu().to(torch.int64)
@@ -44,13 +44,16 @@ def request(model, i, r, max_new_tokens, stopping_criteria, n_vid, samp):
         seed = seed if own else (seed + i) % 2 ** 64
         if T == 0:
             k, seed = 0, 0
+    warp = model._warper_args(r.get("min_p", samp.get("min_p")), r.get("typical_p", samp.get("typical_p")),
+                              r.get("epsilon_cutoff", samp.get("epsilon_cutoff")),
+                              r.get("eta_cutoff", samp.get("eta_cutoff")), f"request {i}", T > 0)
     if T == 0:
         top_p = 1.0                           # HF adds no warpers when greedy
     bans = model._ban_args(r.get("no_repeat_ngram_size", samp.get("no_repeat_ngram_size")),
                            r.get("bad_words_ids", samp.get("bad_words_ids")),
                            r.get("min_new_tokens", samp.get("min_new_tokens")), samp.get("eos"), f"request {i}")
     return SimpleNamespace(ids=ids, S=S, n=n, feats=feats, vid_start=vs, criteria=list(crit or []),
-                           temperature=T, top_k=k, seed=seed, top_p=top_p, penalty=penalty, bans=bans,
+                           temperature=T, top_k=k, seed=seed, top_p=top_p, penalty=penalty, bans=bans, warp=warp,
                            session=r.get("session"),
                            continues=r.get("continues"), start=0, lp=r.get("logprobs", samp.get("logprobs")))
 
@@ -134,7 +137,8 @@ def admit_sampling(model, eng, group, resumed, banning=False, eos=None):
     from column S + min_new_tokens), and the token history of each banning one, from the same ids."""
     rows = list(group) + [(s, r) for s, r, _ in resumed]
     model._set_entries(eng, [s for s, _ in rows], [r.temperature for _, r in rows], [r.top_k for _, r in rows],
-                       [r.seed for _, r in rows], [r.top_p for _, r in rows], [r.penalty for _, r in rows])
+                       [r.seed for _, r in rows], [r.top_p for _, r in rows], [r.penalty for _, r in rows],
+                       [r.warp for _, r in rows])
     ids = [(s, r, r.ids) for s, r in group]
     ids += [(s, r, torch.cat([r.ids, torch.tensor(toks, dtype=torch.int64)])) for s, r, toks in resumed]
     model._token_sets(eng, [(s, t) for s, r, t in ids if r.penalty != 1.0])

@@ -705,21 +705,51 @@ class VideoChatGPTLlamaForCausalLM:
                              f"tokens on the device sampler, this model has {V}")
         return p, r
 
+    def _warper_args(self, min_p, typical_p, epsilon_cutoff, eta_cutoff, what="generate", sampled=True, device=True):
+        """Checks HF's min-p / typical / epsilon / eta settings on the host, with HF's messages -> None when the call
+        runs none of them (greedy calls ignore them, as HF adds no warpers there), else (min_p, typical_p, epsilon,
+        eta) as floats with off as 0, 1, 0, 0. On as in HF's _get_logits_processor: min_p not None, typical_p < 1,
+        0 < epsilon_cutoff < 1, 0 < eta_cutoff < 1. The device sampler's vocabulary limit applies when the call runs
+        there (`device`)."""
+        mp = 0.0 if min_p is None else float(min_p)
+        if not 0.0 <= mp <= 1.0:
+            raise ValueError(f"{what}: `min_p` has to be a float in the [0, 1] interval, but is {min_p}")
+        ty = 1.0 if typical_p is None else float(typical_p)
+        if ty < 1.0 and not ty > 0.0:
+            raise ValueError(f"{what}: `typical_p` has to be a float > 0 and < 1, but is {typical_p}")
+        ty = ty if ty < 1.0 else 1.0
+        ep = 0.0 if epsilon_cutoff is None else float(epsilon_cutoff)
+        ep = ep if 0.0 < ep < 1.0 else 0.0
+        et = 0.0 if eta_cutoff is None else float(eta_cutoff)
+        et = et if 0.0 < et < 1.0 else 0.0
+        if not sampled or (mp == 0.0 and ty == 1.0 and ep == 0.0 and et == 0.0):   # (min_p 0 removes nothing)
+            return None
+        V = self.config.vocab_size
+        if device and V > vn.SAMPLE_WIDE_MAX_V:
+            raise ValueError(f"{what}: min_p, typical_p, epsilon_cutoff and eta_cutoff take a vocabulary of at most "
+                             f"{vn.SAMPLE_WIDE_MAX_V} tokens on the device sampler, this model has {V}")
+        return mp, ty, ep, et
+
     @staticmethod
-    def _set_entries(eng, clips, temperature, top_k, seeds, top_p, penalty):
+    def _set_entries(eng, clips, temperature, top_k, seeds, top_p, penalty, warpers=None):
         """One sampling-table write: set_sampling when every entry has top_p 1 and penalty 1 (what a call without
-        them always made), set_sampling_ex otherwise"""
+        them always made), set_sampling_ex otherwise; then, when some entry of `warpers` (each None or
+        _warper_args' tuple) is on, set_warpers for every entry"""
         if all(p == 1.0 for p in top_p) and all(r == 1.0 for r in penalty):
             eng.set_sampling(clips, temperature, top_k, seeds)
         else:
             eng.set_sampling_ex(clips, temperature, top_k, seeds, top_p, penalty)
+        if warpers is not None and any(w is not None for w in warpers):
+            cols = list(zip(*[w if w is not None else (0.0, 1.0, 0.0, 0.0) for w in warpers]))
+            eng.set_warpers(clips, *cols)
 
     @contextlib.contextmanager
-    def _sampling(self, eng, clips, temperature, top_k, seeds, top_p=1.0, penalty=1.0):
+    def _sampling(self, eng, clips, temperature, top_k, seeds, top_p=1.0, penalty=1.0, warpers=None):
         """Entries `clips` of the engine's sampling table sample (temperature 0: greedy, with the penalty) for the
-        duration of the block and are greedy, without top-p or penalty, again afterwards, also when the block raises."""
+        duration of the block and are greedy, without top-p, penalty or warpers, again afterwards, also when the block
+        raises."""
         n = len(clips)
-        self._set_entries(eng, clips, temperature, top_k, seeds, [top_p] * n, [penalty] * n)
+        self._set_entries(eng, clips, temperature, top_k, seeds, [top_p] * n, [penalty] * n, [warpers] * n)
         try:
             yield
         finally:
@@ -976,7 +1006,7 @@ class VideoChatGPTLlamaForCausalLM:
                  num_return_sequences=1, length_penalty=1.0, early_stopping=False, no_repeat_ngram_size=None,
                  bad_words_ids=None, min_new_tokens=None, guidance_scale=None, negative_prompt_ids=None,
                  negative_prompt_attention_mask=None, negative_video_spatio_temporal_features=None, penalty_alpha=None,
-                 **kw):
+                 min_p=None, typical_p=None, epsilon_cutoff=None, eta_cutoff=None, **kw):
         """Returns [B, S+n] int64 INCLUDING the prompt, like HF generate (inference.py:105-120), and
         like HF it stops at EOS (config.eos_token_id unless eos_token_id is given; None disables it):
         finished rows are padded, the call returns when every row has finished.
@@ -1032,8 +1062,24 @@ class VideoChatGPTLlamaForCausalLM:
         probability against its largest cosine similarity to the prompt's hidden states so far. It runs with
         attention_mask, EOS / pad_token_id, stopping criteria and video features; sampling, seed, beams, guidance,
         logprobs, top_p, repetition_penalty and the banned-token settings raise NotImplementedError. top_k <= 1
-        decodes greedily, as in HF. generate_continue cannot continue it (ValueError)."""
+        decodes greedily, as in HF. generate_continue cannot continue it (ValueError).
+        min_p (None: off), typical_p (None or >= 1: off), epsilon_cutoff and eta_cutoff (on when in (0, 1)): HF's
+        MinPLogitsWarper, TypicalLogitsWarper, EpsilonLogitsWarper and EtaLogitsWarper, after top-p and in that order,
+        when sampling (a greedy call ignores them, as HF does), checked with HF's messages. Seeded sampling applies them
+        on the device (DESIGN.md section 3, "Min-p, typical, epsilon and eta"), guided calls after the guidance;
+        unseeded sampling on the host, step by step. Not with beams or penalty_alpha (NotImplementedError)."""
         self._not_paged("generate")
+        beams = not (isinstance(num_beams, int) and num_beams == 1)
+        contrastive = penalty_alpha is not None and penalty_alpha != 0 and isinstance(top_k, int) and top_k > 1
+        # on as _warper_args has it, so HF's off values (GenerationConfig's typical_p 1.0, epsilon / eta 0.0) pass
+        warp_on = (beams or contrastive) and \
+            self._warper_args(min_p, typical_p, epsilon_cutoff, eta_cutoff, "generate", device=False)
+        if warp_on:
+            name = next(n for n, v, off in zip(("min_p", "typical_p", "epsilon_cutoff", "eta_cutoff"), warp_on,
+                                               (0.0, 1.0, 0.0, 0.0)) if v != off)
+            raise NotImplementedError(f"generate: {name} is not supported with "
+                                      f"{'num_beams > 1' if beams else 'penalty_alpha'} (both decode without "
+                                      "sampling warpers)")
         cs = self._contrastive_args(penalty_alpha, top_k, do_sample, seed, num_beams, guidance_scale, logprobs, top_p,
                                     repetition_penalty, (no_repeat_ngram_size, bad_words_ids, min_new_tokens))
         if cs is not None:
@@ -1055,6 +1101,8 @@ class VideoChatGPTLlamaForCausalLM:
                                       "seed= (unseeded do_sample=True draws from torch's RNG on the host)")
         top_p, penalty = self._nucleus_args(top_p, repetition_penalty, "generate", do_sample,
                                             device=not do_sample or seed is not None)
+        warp = self._warper_args(min_p, typical_p, epsilon_cutoff, eta_cutoff, "generate", do_sample and
+                                 float(temperature) > 0, device=seed is not None)
         eos, pad = self._eos_pad(eos_token_id, pad_token_id)
         bans = self._ban_args(no_repeat_ngram_size, bad_words_ids, min_new_tokens, eos, "generate",
                               device=not do_sample or seed is not None)
@@ -1079,12 +1127,12 @@ class VideoChatGPTLlamaForCausalLM:
             return self._guided_generate(eng, ids, pads, feats, negative_prompt_ids, negative_prompt_attention_mask,
                                          negative_video_spatio_temporal_features, guide, max_new_tokens, do_sample,
                                          seeded, temperature, top_k, seed, top_p, penalty, bans, lp_n,
-                                         stopping_criteria, eos, pad)
+                                         stopping_criteria, eos, pad, warp)
         if seeded or lp_n is not None or ((penalty != 1.0 or bans) and not do_sample):
             clips = list(range(B))
             if seeded:
                 samp = self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips], top_p,
-                                      penalty)
+                                      penalty, warp)
             elif penalty != 1.0:   # greedy entries with the penalty
                 samp = self._sampling(eng, clips, [0.0] * B, [0] * B, [0] * B, 1.0, penalty)
             else:
@@ -1110,7 +1158,7 @@ class VideoChatGPTLlamaForCausalLM:
             _, logits, _ = eng.prefill(ids, feats, vs, want_logits=True, want_token=False, n_pad=pads)
             self._pos = S
             self._last_out = self._stepwise(eng, ids, logits, n, do_sample, temperature, stopping_criteria, eos, pad,
-                                            top_k, top_p, penalty, bans)
+                                            top_k, top_p, penalty, bans, warpers=warp)
             return self._last_out
         if eos is None:
             new = eng.generate(ids, feats, vs, n, n_pad=pads).to(torch.int64)
@@ -1133,7 +1181,7 @@ class VideoChatGPTLlamaForCausalLM:
         return self._last_out
 
     def _guided_generate(self, eng, ids, pads, feats, neg_ids, neg_mask, neg_feats, g, max_new_tokens, do_sample, seeded,
-                         temperature, top_k, seed, top_p, penalty, bans, lp_n, stopping_criteria, eos, pad):
+                         temperature, top_k, seed, top_p, penalty, bans, lp_n, stopping_criteria, eos, pad, warp=None):
         """generate with guidance_scale g: one left-padded prefill of the prompts and the negative prompts (clips B ..
         2B-1), then the device loops with the guidance table set (greedy and seeded calls; stopping criteria keep
         _host_stops' chunking), or _stepwise with the combination on the host (unseeded sampling). The prompts' entries
@@ -1153,11 +1201,12 @@ class VideoChatGPTLlamaForCausalLM:
             _, logits, _ = eng.prefill(ids2, f2, spans, want_logits=True, want_token=False, n_pad=pads2)
             self._pos = S2
             self._last_out = self._stepwise(eng, ctx, logits, n, do_sample, temperature, stopping_criteria, eos, pad,
-                                            top_k, top_p, penalty, bans, guidance=g)
+                                            top_k, top_p, penalty, bans, guidance=g, warpers=warp)
             return self._last_out[:, shift:]
         clips = list(range(B))
         if seeded:
-            samp = self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips], top_p, penalty)
+            samp = self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips], top_p, penalty,
+                                  warp)
         elif penalty != 1.0:
             samp = self._sampling(eng, clips, [0.0] * B, [0] * B, [0] * B, 1.0, penalty)
         else:
@@ -1396,7 +1445,8 @@ class VideoChatGPTLlamaForCausalLM:
     def generate_requests(self, requests, max_new_tokens=32, eos_token_id="config", stopping_criteria=None,
                           slots=None, do_sample=False, packed_admission=False, temperature=1.0, top_k=50, seed=None,
                           chunked_prefill=False, logprobs=None, top_p=1.0, repetition_penalty=1.0, no_repeat_ngram_size=None,
-                          bad_words_ids=None, min_new_tokens=None):
+                          bad_words_ids=None, min_new_tokens=None, min_p=None, typical_p=None, epsilon_cutoff=None,
+                          eta_cutoff=None):
         """Greedy generation for many independent requests by in-flight (continuous) batching: every request
         owns a slot of the KV cache while it runs, and a finished request's slot takes the next queued one at
         once while the other slots keep decoding (a static batch decodes until its longest row finishes).
@@ -1459,7 +1509,10 @@ class VideoChatGPTLlamaForCausalLM:
         no_repeat_ngram_size / bad_words_ids / min_new_tokens, or a request's own keys of those names: as in generate,
         on the device, over the request's own input_ids (a continuation: the whole conversation, whose length is where
         min_new_tokens starts counting). The slot's token history is written where its token set is; a call in which
-        no request bans writes no ban table and launches what it launched before."""
+        no request bans writes no ban table and launches what it launched before.
+        min_p / typical_p / epsilon_cutoff / eta_cutoff, or a request's own keys of those names: as in generate, on the
+        device, for sampled requests; they are written with the request's sampling entry at every admission, resume
+        and continuation."""
         self._logprobs_arg(logprobs, "generate_requests")
         for i, r in enumerate(requests):
             r = r if isinstance(r, dict) else {}
@@ -1472,6 +1525,9 @@ class VideoChatGPTLlamaForCausalLM:
                                           "sampling in flight needs seed= (the call's or the request's own)")
             self._nucleus_args(r.get("top_p", top_p), r.get("repetition_penalty", repetition_penalty), f"request {i}",
                                r.get("do_sample", do_sample))
+            self._warper_args(r.get("min_p", min_p), r.get("typical_p", typical_p),
+                              r.get("epsilon_cutoff", epsilon_cutoff), r.get("eta_cutoff", eta_cutoff), f"request {i}",
+                              r.get("do_sample", do_sample))
         eos, _ = self._eos_pad(eos_token_id, None)
         for i, r in enumerate(requests):
             r = r if isinstance(r, dict) else {}
@@ -1486,7 +1542,8 @@ class VideoChatGPTLlamaForCausalLM:
         eng = self._ensure_engine(need_llm=True)
         samp = dict(do_sample=do_sample, temperature=temperature, top_k=top_k, seed=seed, logprobs=logprobs, top_p=top_p,
                     repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size,
-                    bad_words_ids=bad_words_ids, min_new_tokens=min_new_tokens, eos=eos)
+                    bad_words_ids=bad_words_ids, min_new_tokens=min_new_tokens, eos=eos, min_p=min_p,
+                    typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff)
         reqs = [inflight.request(self, i, r, max_new_tokens, stopping_criteria, eng.NV, samp)
                 for i, r in enumerate(requests)]
         if self._kv_blocks:
@@ -1552,7 +1609,7 @@ class VideoChatGPTLlamaForCausalLM:
     def generate_continue(self, new_input_ids, do_sample=False, temperature=1.0, max_new_tokens=32,
                           stopping_criteria=None, eos_token_id="config", pad_token_id=None, top_k=50, seed=None,
                           logprobs=None, top_p=1.0, repetition_penalty=1.0, no_repeat_ngram_size=None, bad_words_ids=None,
-                          min_new_tokens=None):
+                          min_new_tokens=None, min_p=None, typical_p=None, epsilon_cutoff=None, eta_cutoff=None):
         """Next turn about the SAME video(s): `new_input_ids` [B, S_new] follow everything generated
         so far. Only the tokens the KV cache does not hold yet (the last generated token and the new
         text) are prefilled (vcl_llm_prefill_append); the reference re-runs the tower and the whole
@@ -1563,7 +1620,8 @@ class VideoChatGPTLlamaForCausalLM:
         tokens of this turn. top_p / repetition_penalty: as in generate; the penalty's tokens are the whole
         conversation (every earlier turn, its answers as returned, and the new text). no_repeat_ngram_size /
         bad_words_ids / min_new_tokens: as in generate, over the whole conversation; min_new_tokens counts this turn's
-        tokens (HF's prompt length is the conversation's)."""
+        tokens (HF's prompt length is the conversation's). min_p / typical_p / epsilon_cutoff / eta_cutoff: as in
+        generate."""
         self._not_paged("generate_continue")
         self.last_beam_scores = None
         if getattr(self, "_after_beams", False):
@@ -1581,6 +1639,8 @@ class VideoChatGPTLlamaForCausalLM:
         self.last_logprobs = None
         top_p, penalty = self._nucleus_args(top_p, repetition_penalty, "generate_continue", do_sample,
                                             device=not do_sample or seed is not None)
+        warp = self._warper_args(min_p, typical_p, epsilon_cutoff, eta_cutoff, "generate_continue",
+                                 do_sample and float(temperature) > 0, device=seed is not None)
         eos, pad = self._eos_pad(eos_token_id, pad_token_id)
         bans = self._ban_args(no_repeat_ngram_size, bad_words_ids, min_new_tokens, eos, "generate_continue",
                               device=not do_sample or seed is not None)
@@ -1600,7 +1660,7 @@ class VideoChatGPTLlamaForCausalLM:
             clips = list(range(B))
             if seeded:
                 samp = self._sampling(eng, clips, [temperature] * B, [top_k] * B, [seed + b for b in clips], top_p,
-                                      penalty)
+                                      penalty, warp)
             elif penalty != 1.0:   # greedy entries with the penalty
                 samp = self._sampling(eng, clips, [0.0] * B, [0] * B, [0] * B, 1.0, penalty)
             else:
@@ -1622,7 +1682,7 @@ class VideoChatGPTLlamaForCausalLM:
         _, logits, _ = eng.prefill_append(tail, start, want_logits=True, want_token=False)
         self._pos = ctx.shape[1]
         self._last_out = self._stepwise(eng, ctx, logits, n, do_sample, temperature, stopping_criteria, eos, pad, top_k,
-                                        top_p, penalty, bans)
+                                        top_p, penalty, bans, warpers=warp)
         return self._continued()
 
     def _continued(self):
@@ -1631,11 +1691,12 @@ class VideoChatGPTLlamaForCausalLM:
         return self._last_out[:, shift:] if shift else self._last_out
 
     @staticmethod
-    def _host_processors(out, logits, sampled, temperature, top_k, top_p, penalty, bans=None, S=0):
+    def _host_processors(out, logits, sampled, temperature, top_k, top_p, penalty, bans=None, S=0, warpers=None):
         """HF's logits processors of the stepwise path, in HF's order, on logits [B, V] fp32 after the ids `out`
         [B, L]: RepetitionPenaltyLogitsProcessor, the banned tokens (_host_bans, with `bans` from _ban_args; the call's
-        first new token at column S), then (sampled only) TemperatureLogitsWarper, TopKLogitsWarper and
-        TopPLogitsWarper (min_tokens_to_keep 1); a dropped token is -inf"""
+        first new token at column S), then (sampled only) TemperatureLogitsWarper, TopKLogitsWarper,
+        TopPLogitsWarper and the warpers of `warpers` (_host_warpers) (min_tokens_to_keep 1); a dropped token is
+        -inf"""
         if penalty != 1.0:
             ids = out.to(logits.device)
             sc = torch.gather(logits, 1, ids)
@@ -1654,10 +1715,44 @@ class VideoChatGPTLlamaForCausalLM:
             drop = srt.softmax(dim=-1).cumsum(dim=-1) <= (1 - top_p)
             drop[..., -1:] = False
             lg = lg.masked_fill(drop.scatter(1, idx, drop), float("-inf"))
+        if warpers is not None:
+            lg = VideoChatGPTLlamaForCausalLM._host_warpers(lg, warpers)
+        return lg
+
+    @staticmethod
+    def _host_warpers(lg, warpers):
+        """HF's MinPLogitsWarper, TypicalLogitsWarper, EpsilonLogitsWarper and EtaLogitsWarper (min_tokens_to_keep 1)
+        on scores lg [B, V] fp32, in HF's order and with HF's torch operations; warpers: _warper_args' tuple (off: min_p
+        0, typical_p 1, epsilon 0, eta 0)"""
+        mp, ty, ep, et = warpers
+        ninf = float("-inf")
+        if mp > 0.0:
+            probs = torch.softmax(lg, dim=-1)
+            drop = probs < mp * probs.amax(dim=-1, keepdim=True)
+            drop.scatter_(-1, torch.topk(probs, 1, dim=-1).indices, False)
+            lg = lg.masked_fill(drop, ninf)
+        if ty < 1.0:
+            normalized = torch.nn.functional.log_softmax(lg, dim=-1)
+            ent = -(normalized * torch.exp(normalized)).nansum(-1, keepdim=True)
+            srt, idx = torch.sort(torch.abs((-normalized) - ent), descending=False)
+            last = (lg.gather(-1, idx).softmax(dim=-1).cumsum(dim=-1) < ty).sum(dim=1)
+            last.clamp_(max=srt.shape[-1] - 1)
+            drop = srt > srt.gather(1, last.view(-1, 1))
+            drop[..., :1] = False
+            lg = lg.masked_fill(drop.scatter(1, idx, drop), ninf)
+        if ep > 0.0:
+            drop = (lg.softmax(dim=-1) < ep) & (lg < torch.topk(lg, 1)[0][..., -1, None])
+            lg = lg.masked_fill(drop, ninf)
+        if et > 0.0:
+            e = torch.tensor(et, device=lg.device)
+            entropy = torch.distributions.Categorical(logits=lg).entropy()
+            eta = torch.min(e, torch.sqrt(e) * torch.exp(-entropy))[..., None]
+            drop = (lg.softmax(dim=-1) < eta) & (lg < torch.topk(lg, 1)[0][..., -1, None])
+            lg = lg.masked_fill(drop, ninf)
         return lg
 
     def _stepwise(self, eng, out, logits, n, do_sample, temperature, stopping_criteria, eos, pad, top_k=50, top_p=1.0,
-                  penalty=1.0, bans=None, guidance=None):
+                  penalty=1.0, bans=None, guidance=None, warpers=None):
         """One token per C-ABI call. After the loop the cache holds every returned token but the last
         (self._pos = out.shape[1] - 1), the state generate_continue starts from. The logits go through HF's
         processors in HF's order: repetition penalty (over `out` so far), the banned tokens, then temperature, top-k
@@ -1670,7 +1765,7 @@ class VideoChatGPTLlamaForCausalLM:
             if guidance is not None:
                 logits = self._host_guidance(logits[:B], logits[B:], guidance)
             lg = self._host_processors(out, logits, do_sample and temperature > 0, temperature, top_k, top_p, penalty,
-                                       bans, S)
+                                       bans, S, warpers)
             if do_sample and temperature > 0:
                 nxt = torch.multinomial(torch.softmax(lg, dim=-1), 1)[:, 0]
             else:
