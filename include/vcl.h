@@ -637,7 +637,9 @@ long long vcl_launch_count(void);
 
 /* ---- single-operator entry points (unit tests / profiling of the individual kernels) ---- */
 /* C[M,N] = act(A[M,K] . W[N,K]^T + bias) (+ residual); act: 0 none, 1 quick_gelu, 2 gelu(erf),
- * 3 swiglu over interleaved rows (C is [M,N/2]). block_n: 0 = auto, or 32/64/128/256. */
+ * 3 swiglu over interleaved rows (C is [M,N/2]). block_n: 0 = auto, or 32/64/128/256.
+ * K must be a multiple of 64 and N of 32; pitches (elements) multiples of 8 and at least the row (lda, ldw >= K,
+ * ldc, ldr >= C's width); A, W, C, bias and residual 16-byte aligned. Anything else is refused before a launch. */
 int vcl_op_gemm(const void* A, int64_t lda, const void* W, int64_t ldw, void* C, int64_t ldc,
                 const void* bias, const void* residual, int64_t ldr, int M, int N, int K, int act,
                 int block_n, void* stream);

@@ -516,6 +516,10 @@ int launch_gemm_bf16_tn(const GemmArgs& g, cudaStream_t stream) {
   VCL_REQUIRE(g.K % 64 == 0, "gemm: K=%d must be a multiple of 64", g.K);
   VCL_REQUIRE(g.N % 32 == 0, "gemm: N=%d must be a multiple of 32", g.N);
   VCL_REQUIRE(g.lda % 8 == 0 && g.ldw % 8 == 0 && g.ldc % 8 == 0, "gemm: pitches must be x8");
+  const int n_out = g.act == ACT_SWIGLU ? g.N / 2 : g.N;
+  VCL_REQUIRE(g.lda >= g.K && g.ldw >= g.K && g.ldc >= n_out && (g.residual == nullptr || g.ldr >= n_out),
+              "gemm: pitches must cover a row (lda=%lld ldw=%lld >= K=%d, ldc=%lld ldr=%lld >= output width %d)",
+              g.lda, g.ldw, g.K, g.ldc, g.ldr, n_out);
   VCL_REQUIRE(((uintptr_t)g.A % 16) == 0 && ((uintptr_t)g.W % 16) == 0 &&
                   ((uintptr_t)g.C % 16) == 0, "gemm: pointers must be 16-byte aligned");
   VCL_REQUIRE(g.residual == nullptr || (g.ldr % 8 == 0 && ((uintptr_t)g.residual % 16) == 0),
